@@ -2,8 +2,9 @@
 """Benchmark of the SuDoRM-RF forward path (BASELINE.json metric: mixtures/sec,
 4 s @ 8 kHz, 2 sources).
 
-    python bench.py --gpus N --steps K --warmup W            # B200 arm (this repo's kernels)
+    python bench.py --gpus N --steps K --warmup W            # GPU arm (this repo's kernels)
     python bench.py --impl reference --gpus N --steps K ...  # reference arm (CPU oracle port)
+    python bench.py --gpus 1 --steps K --dump-outputs DIR    # + the last timed step's estimates as DIR/*.npy
 
 One "step" = one forward pass of the separator over one synthetic batch.  At
 N > 1 the batch is sharded by giving every rank its own batch of the same size
@@ -25,7 +26,7 @@ if REPO not in sys.path:
 import torch  # noqa: E402
 
 # BASELINE.json configs (SURVEY.md §8 shapes).  The headline / default workload is
-# configs[1]: Improved SuDoRM-RF U16/512, batch 32 x 4 s @ 8 kHz on one B200.
+# configs[1]: Improved SuDoRM-RF U16/512, batch 32 x 4 s @ 8 kHz on one GPU.
 WORKLOADS = {
     "improved_u16_512": dict(variant="improved", B=32, T=32000, kw=dict(
         out_channels=256, in_channels=512, num_blocks=16, upsampling_depth=5,
@@ -68,17 +69,17 @@ def load_peaks():
     if os.path.exists(path):
         p = json.load(open(path))
         return float(p["hbm_gbs"]), "measured (MEASURED_PEAKS.json)"
-    return 6650.0, "fallback (B200_PROFILING.md)"
+    return 3350.0, "H100 SXM data sheet (HBM3)"
 
 
 def load_tensor_peak():
-    """Dense bf16 TFLOP/s (cuBLAS, burst) measured on this pool's B200s; fallback: the profiling guide's figure."""
+    """Dense bf16 TFLOP/s: MEASURED_PEAKS.json when present, else the H100 SXM data sheet's figure."""
     path = os.path.join(REPO, "MEASURED_PEAKS.json")
     if os.path.exists(path):
         p = json.load(open(path))
         if "bf16_tflops" in p:
             return float(p["bf16_tflops"]), "measured (MEASURED_PEAKS.json, burst)"
-    return 1670.0, "fallback (B200_PROFILING.md)"
+    return 989.0, "H100 SXM data sheet (dense bf16)"
 
 
 # --------------------------------------------------------------------------
@@ -135,7 +136,7 @@ def algorithmic_model(w):
 
 
 # --------------------------------------------------------------------------
-# clocks sampling during the timed region (B200_PROFILING.md)
+# clocks sampling during the timed region
 # --------------------------------------------------------------------------
 class ClockSampler:
     Q = ("clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,"
@@ -259,8 +260,26 @@ def run_reference(args, w, wl_name):
     print(json.dumps(line), flush=True)
 
 
+DUMP_LIMIT_BYTES = 64 * 1024 * 1024
+
+
+def dump_outputs(out_dir, arrays):
+    """Write each output as <out_dir>/<name>.npy in float32.  An output larger than its share of the 64 MB budget
+    is reduced to a fixed, seeded sample of its flattened elements (the same indices for the same shape), so two
+    builds run with the same arguments can be compared element for element."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    share = DUMP_LIMIT_BYTES // max(1, len(arrays))
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if a.nbytes > share:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, size=share // 4, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(out_dir, f"{name}.npy"), np.ascontiguousarray(a, dtype=np.float32))
+
+
 # --------------------------------------------------------------------------
-# B200 arm
+# GPU arm
 # --------------------------------------------------------------------------
 def run_b200(args, w, wl_name):
     import ctypes as C
@@ -273,7 +292,7 @@ def run_b200(args, w, wl_name):
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
     if not torch.cuda.is_available():
-        raise SystemExit("bench.py (B200 arm) needs a CUDA device; there is no CPU fallback")
+        raise SystemExit("bench.py (GPU arm) needs a CUDA device; there is no CPU fallback")
     torch.cuda.set_device(local)
     dev = torch.device("cuda", local)
     if world > 1:
@@ -296,7 +315,7 @@ def run_b200(args, w, wl_name):
     g = torch.Generator().manual_seed(1234 + rank)
     host_x = torch.rand(B, 1, T, generator=g).pin_memory()      # the reference's bench input (notebook :128)
     x = host_x.to(dev)
-    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 126 MB L2
+    flush = torch.empty(256 * 1024 * 1024, dtype=torch.uint8, device=dev)   # > 50 MB L2 (H100)
 
     stream = torch.cuda.Stream(device=dev)
     with torch.no_grad(), torch.cuda.stream(stream):
@@ -332,6 +351,8 @@ def run_b200(args, w, wl_name):
         wall = time.perf_counter() - wall0
         clocks = sampler.stop() if sampler else None
         dev_ms = sum(s.elapsed_time(e) for s, e in evs)
+        if args.dump_outputs and rank == 0:
+            dump_outputs(args.dump_outputs, {"estimates": y})
 
         # ---- end to end: pinned host mixtures in, pinned host estimates out, every step ----
         host_y = torch.empty(B, w["kw"]["num_sources"], T).pin_memory()
@@ -410,7 +431,7 @@ def run_b200(args, w, wl_name):
             "config": {"workload": wl_name, "batch_per_gpu": B, "global_batch": B * world,
                        "samples": T, "sources": w["kw"]["num_sources"], "parallelism": f"dp{world}",
                        "l2": "256 MiB flush write between timed steps; one step streams "
-                             f"{fwd_bytes / 1e9:.1f} GB (algorithmic) through a >1 GB workspace >> 126 MB L2",
+                             f"{fwd_bytes / 1e9:.1f} GB (algorithmic) through a >1 GB workspace >> 50 MB L2",
                        "timing": "CUDA events around each CUDA-graph replay, summed over K steps, max over ranks",
                        "wall_s_timed_loop": wall},
             "e2e": {"value": total_mix / (e2e_ms / 1e3), "unit": UNIT,
@@ -486,7 +507,7 @@ def block_launchers(w, B, dev, stream):
             keep.append(wpk)
             fn = lambda: N.check(lib.sdr_pointwise_mma(P(xin), C.byref(nin), P(wpk), P(bias), P(res), P(None), 0,
                                                        P(yout), P(stats), S, M, K, L, 0, sp))
-            return name + " [pw_mma_kernel tcgen05 bf16x3]", fn
+            return name + " [pw_mma_kernel wgmma bf16x3]", fn
         fn = lambda: N.check(lib.sdr_pointwise(P(xin), C.byref(nin), P(Wt), P(bias), P(res), P(None), 0,
                                                P(yout), P(stats), S, M, K, L, 0, sp))
         return name + " [pw_gemm_kernel FFMA]", fn
@@ -601,7 +622,7 @@ def time_block(w, B, stream, flush, dev, reps=7):
         k = {"kernel": name, "avg_launch_ms": t, "algorithmic_bytes_per_launch": nbytes,
              "achieved": nbytes / t / 1e6, "frac": nbytes / t / 1e6 / peak,
              "tflops_fp32_equivalent": flops / t / 1e9}
-        if "tcgen05" in name:       # fp32-grade result from 3 bf16 products per MAC: the tensor pipe sees 3x the flops
+        if "wgmma" in name:       # fp32-grade result from 3 bf16 products per MAC: the tensor pipe sees 3x the flops
             k["bf16_tflops_issued"] = 3.0 * flops / t / 1e9
             k["frac_tensor"] = 3.0 * flops / t / 1e9 / tpeak
             k["tensor_peak_tflops"] = tpeak
@@ -735,6 +756,8 @@ def main():
     ap.add_argument("--workload", default="improved_u16_512", choices=sorted(WORKLOADS))
     ap.add_argument("--batch", type=int, default=0, help="per-GPU batch (default: the workload's)")
     ap.add_argument("--no-other-configs", action="store_true", help="skip the short runs of BASELINE configs 3 / 4 / 5")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write the last timed step's outputs as DIR/<name>.npy (float32, <= 64 MB in all)")
     args = ap.parse_args()
     w = WORKLOADS[args.workload]
     if args.impl == "reference":

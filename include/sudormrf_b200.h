@@ -1,5 +1,5 @@
 /*
- * sudormrf_b200.h — C ABI of the B200-native SuDoRM-RF forward path.
+ * sudormrf_b200.h — C ABI of the H100-native SuDoRM-RF forward path.
  *
  * The reference (etzinis/sudo_rm_rf) has no native/FFI layer: its boundary is
  * the Python nn.Module contract.  This header is the C-ABI that sits UNDER the
@@ -151,7 +151,7 @@ typedef struct {
 int sdr_encoder(const float* wav, const float* weight, float* enc, double* stats,
                 int B, int A, int64_t T, int N, int K, int L, sdr_stream stream);
 
-/* The same encoder on the tensor cores: the tcgen05 GEMM kernel with a "window" operand producer
+/* The same encoder on the tensor cores: the wgmma GEMM kernel with a "window" operand producer
  * (A[position, tap] = wav[hop*position + tap - pad], built in registers: no im2col in HBM); the
  * weight is converted once to pre-swizzled bf16 hi/lo images (taps zero-padded to 64).  N >= 32. */
 size_t sdr_encoder_mma_packed_bytes(int N, int A, int K);
@@ -168,7 +168,7 @@ int sdr_pointwise(const float* x, const sdr_norm_in* fin, const float* W, const 
                   float* y, double* stats_out,
                   int samples, int M, int Kc, int L, int epilogue, sdr_stream stream);
 
-/* Tensor-core (tcgen05, bf16x3 split, fp32 accumulate) variant of sdr_pointwise for
+/* Tensor-core (wgmma, bf16x3 split, fp32 accumulate) variant of sdr_pointwise for
  * channel counts that fill a tile: M % 128 == 0 and Kc % 64 == 0.  The weight is
  * first converted to pre-swizzled bf16 hi/lo shared-memory images (bulk-TMA source);
  * sdr_pointwise_mma_packed_bytes returns 0 when the shape is not eligible.           */

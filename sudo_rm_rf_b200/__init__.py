@@ -1,4 +1,4 @@
-"""sudo_rm_rf_b200: B200-native (sm_100a) forward inference path of SuDoRM-RF.
+"""sudo_rm_rf_b200: H100-native (sm_90a) forward inference path of SuDoRM-RF.
 
 Mirrors ``sudo_rm_rf.dnn.models.improved_sudormrf`` /
 ``sudo_rm_rf.dnn.models.groupcomm_sudormrf_v2`` /

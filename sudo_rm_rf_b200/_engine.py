@@ -295,8 +295,8 @@ def _check_input(model, cfg, wav: torch.Tensor) -> torch.Tensor:
         raise RuntimeError(f"expected {cfg.in_audio_channels} audio channel(s), got {wav.shape[1]}")
     if not wav.is_cuda:
         raise RuntimeError(
-            "sudo_rm_rf_b200 runs on CUDA (sm_100a) only and has no CPU path: move the model "
-            "and the mixture to a B200 (`model.cuda()`, `mixture.cuda()`).")
+            "sudo_rm_rf_b200 runs on CUDA (sm_90a) only and has no CPU path: move the model "
+            "and the mixture to an H100 (`model.cuda()`, `mixture.cuda()`).")
     if torch.is_grad_enabled() and model.training and \
             any(_fetch(model, n).requires_grad for n in _probe_names(model)):
         raise RuntimeError(

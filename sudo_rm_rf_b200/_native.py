@@ -115,7 +115,7 @@ EXPORTED_SYMBOLS = tuple(_SIGNATURES)
 
 
 def build(verbose: bool = False) -> str:
-    """Compile the CUDA sources for sm_100a into the in-tree shared library."""
+    """Compile the CUDA sources for sm_90a into the in-tree shared library."""
     proc = subprocess.run(["make", "-C", CSRC, "-j8"], capture_output=True, text=True)
     if proc.returncode != 0:
         raise NativeError("building libsudormrf_b200.so failed:\n" + proc.stdout + proc.stderr)

@@ -1,10 +1,10 @@
-"""B200-native mirror of ``sudo_rm_rf/dnn/models/causal_improved_sudormrf_v3.py``.
+"""H100-native mirror of ``sudo_rm_rf/dnn/models/causal_improved_sudormrf_v3.py``.
 
 Same public surface as the reference module (class names, constructor arguments and defaults, public
 attributes, sub-module / parameter names and therefore ``state_dict()`` keys, ``forward(input_wav)``), so
 ``run_fuss_separation.py:134-170``-style model selection, ``load_state_dict`` of checkpoints and whole-module
-pickles keep working.  The arithmetic of ``CausalSuDORMRF.forward`` (reference :191-211) is done by the sm_100a
-kernels behind ``include/sudormrf_b200.h`` (variant 2): the tcgen05 GEMM for every 1x1 convolution, the encoder
+pickles keep working.  The arithmetic of ``CausalSuDORMRF.forward`` (reference :191-211) is done by the sm_90a
+kernels behind ``include/sudormrf_b200.h`` (variant 2): the wgmma GEMM for every 1x1 convolution, the encoder
 and the decoder, and one pass per block for the whole causal depthwise pyramid (``csrc/causal.cu``).  The
 sub-modules below only own the parameters.  Inference only; no CPU path.
 """
@@ -64,7 +64,7 @@ class UConvBlock(nn.Module):
 
 
 class CausalSuDORMRF(_engine.NativeModuleMixin, nn.Module):
-    """Causal SuDoRM-RF separator (reference :120-231) on the B200 native path."""
+    """Causal SuDoRM-RF separator (reference :120-231) on the H100 native path."""
 
     _b200_variant = 2
 

@@ -86,7 +86,7 @@ def separate_corpus(model, wavs: Iterable[torch.Tensor], max_batch: int = 32,
         raise RuntimeError("separate_corpus follows the README recipe, which is written for mono mixtures")
     device = _engine._fetch(model, _engine._probe_names(model)[0]).device
     if device.type != "cuda":
-        raise RuntimeError("sudo_rm_rf_b200 runs on CUDA (sm_100a) only: move the model to a B200")
+        raise RuntimeError("sudo_rm_rf_b200 runs on CUDA (sm_90a) only: move the model to an H100")
     if torch.is_grad_enabled() and model.training:
         raise RuntimeError("sudo_rm_rf_b200 implements the inference forward only: call model.eval()")
     plan = plan_buckets([int(w.shape[0]) for w in wavs], model_padding_rule(cfg), max_batch)
@@ -176,7 +176,7 @@ class CorpusSeparator:
             raise RuntimeError("CorpusSeparator follows the README recipe, which is written for mono mixtures")
         self.device = _engine._fetch(model, _engine._probe_names(model)[0]).device
         if self.device.type != "cuda":
-            raise RuntimeError("sudo_rm_rf_b200 runs on CUDA (sm_100a) only: move the model to a B200")
+            raise RuntimeError("sudo_rm_rf_b200 runs on CUDA (sm_90a) only: move the model to an H100")
         self.quantum = model_padding_rule(self.cfg)      # T -> padded length (the model's own rule)
         self.graphs = {}           # (B, Tp, slot) -> "warm" | CUDAGraph
         self.launches = {"eager": 0, "captured": 0, "replayed": 0}

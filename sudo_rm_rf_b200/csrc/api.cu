@@ -1,4 +1,4 @@
-// C-ABI of the B200-native SuDoRM-RF forward (see include/sudormrf_b200.h):
+// C-ABI of the H100-native SuDoRM-RF forward (see include/sudormrf_b200.h):
 // parameter layout (reference state_dict order), weight packing, workspace
 // planning and the forward orchestration that enqueues every kernel on the
 // caller's stream.
@@ -61,7 +61,7 @@ size_t encoder_mma_packed_bytes(int N, int A, int Kk);
 int pack_encoder_mma(const float* W, int N, int A, int Kk, void* packed, cudaStream_t);
 int launch_encoder_mma(const float*, const void*, const float*, int, float*, double*, int, int, long long, int, int, int, int, cudaStream_t);
 
-// One 1x1 convolution: tensor cores when the channel counts fill a tcgen05 tile, FFMA otherwise.
+// One 1x1 convolution: tensor cores when the channel counts fill a wgmma tile, FFMA otherwise.
 static int pointwise(const float* x, const NormIn& nin, const float* W, const float* wpk, const float* bias,
                      const float* residual, const float* gate, int gate_channels, float* y, double* stats,
                      int samples, int M, int K, int L, int epilogue, cudaStream_t st) {
@@ -641,7 +641,7 @@ const char* sdr_error_string(int code) {
         case SDR_ERR_BAD_ARGUMENT: return "bad argument";
         case SDR_ERR_WORKSPACE: return "workspace or packed-weight buffer too small";
         case SDR_ERR_CUDA: return "CUDA call or kernel launch failed";
-        case SDR_ERR_UNSUPPORTED: return "configuration not supported by the sm_100a kernels";
+        case SDR_ERR_UNSUPPORTED: return "configuration not supported by the sm_90a kernels";
         default: return "unknown error";
     }
 }

@@ -1,4 +1,4 @@
-// Shared device helpers for the SuDoRM-RF sm_100a kernels.
+// Shared device helpers for the SuDoRM-RF sm_90a kernels.
 #pragma once
 #include <cuda_runtime.h>
 #include <stdint.h>

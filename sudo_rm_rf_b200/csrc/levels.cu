@@ -252,8 +252,8 @@ __device__ __forceinline__ float norm_act(float x, const FoldedNorm& f, float sl
     return y;
 }
 
-// tuning knobs, swept on the B200 (profiles/r01_level_kernel_sweep.md): 128 threads x 4 runs (2 for the
-// merge) beat 256x2 / 512x1 / 64x8; ld.global.nc.L1::no_allocate + st.global.cs made stride-2 levels ~25 % slower
+// tuning knobs: 128 threads x 4 runs (2 for the merge); ld.global.nc.L1::no_allocate + st.global.cs are not used
+// (stride-2 levels measured slower with them)
 #ifndef SDR_DW_THREADS
 #define SDR_DW_THREADS 128
 #endif

@@ -1,5 +1,5 @@
 // 1x1 Conv1d as a batched GEMM, fp32 FFMA path (exact-parity path; also the
-// path for the small / odd channel counts that cannot fill a tcgen05 tile).
+// path for the small / odd channel counts that cannot fill a wgmma tile).
 //
 //   y[s, m, l] = sum_k W[m, k] * f(x[s, k, l]) + bias[m]  (+ residual[s, m, l])
 //   f = deferred GlobLN (+PReLU) of the producer, applied while the activation

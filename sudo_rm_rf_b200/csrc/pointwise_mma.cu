@@ -1,18 +1,20 @@
-// 1x1 Conv1d on the 5th-gen tensor cores (tcgen05 / TMEM), sm_100a only.
+// 1x1 Conv1d on the Hopper tensor cores (wgmma, TMA, mbarrier), sm_90a.
 //
 //   y[s, m, l] = sum_k W[m, k] * f(x[s, k, l]) + bias[m]   (+ residual | relu()*gate)
 //
-// GEMM view per tile: D[128 positions, N channels] = A[128, K] * B[N, K]^T with
+// GEMM view per tile: D[128 positions, 128 channels] = A[128, K] * B[128, K]^T with
 //   A = f(x) tile, produced on the fly: the activation tile cannot be TMA'd
 //       straight into the MMA because the producer's deferred GlobLN(+PReLU)
-//       has to be applied first.  8 transform warps read x with coalesced
-//       128 B row segments, apply the per-channel affine (+PReLU), split the
-//       fp32 value into bf16 hi + bf16 lo, and store both into the K-major
-//       SWIZZLE_128B shared-memory layout the UMMA descriptors expect.
+//       has to be applied first.  A TMA warp lands the raw fp32 tile in shared
+//       memory; 8 transform warps apply the per-channel affine (+PReLU), split
+//       the fp32 value into bf16 hi + bf16 lo, and store both into the MN-major
+//       SWIZZLE_128B shared-memory layout the wgmma descriptors expect.
 //   B = weights, pre-split into bf16 hi/lo and pre-swizzled at pack time, so a
-//       k-block is ONE cp.async.bulk (TMA bulk copy) of a contiguous image.
-//   D = fp32 accumulator in TMEM, 2 stages x 256 columns, so the epilogue of
-//       tile i overlaps the main loop of tile i+1 (persistent CTAs, 1 per SM).
+//       k-block is ONE TMA box of a contiguous image.
+//   D = fp32 accumulator in registers: two consumer warpgroups, each owning 64
+//       positions x 128 channels (64 registers per thread), issue the wgmmas
+//       and run the epilogue.  Persistent CTAs, one per SM; the transform and
+//       TMA warps run ahead into the free stages while the consumers drain.
 // Precision: x*w ~= xh*wh + xl*wh + xh*wl (3 bf16 MMAs, fp32 accumulate): the
 // dropped terms are O(2^-16) relative, i.e. fp32-grade for the 1e-3 parity
 // budget, where a single bf16 (5e-3) or tf32 (7e-4) pass is not (SURVEY §7).
@@ -30,69 +32,27 @@
 
 namespace sdr {
 
-// CTA pairs (tcgen05 cta_group::2).  The kernel is launched as clusters of two CTAs (one TPC).  A pair works on one
-// (256 positions x tile_n channels) tile at a time: each CTA transforms ITS 128 positions into its own A stage and
-// loads only ITS half of the weight rows (tile_n / 2) into its own B stage; the leader CTA (cluster rank 0) issues
-// ONE UMMA (M = 256) per k-step for the pair, and each CTA's TMEM receives the accumulator rows of its own positions.
-// Why: with one CTA per tile the weight image (bf16 hi + lo = 4 B per weight) was re-streamed from L2 for every
-// 128-position tile -- 256 KB of weights against 128 KB of activations per proj tile -- and the main loop ran at the
-// L2 fabric limit (proj / mask with the epilogue disabled: 614 MB / 69.6 us and 1.23 GB / 140 us = 8.8 TB/s both,
-// profiles/r01d_tma_epilogue.md).  Pairing halves the weight traffic per position and frees 64 KB of shared memory
-// for a third pipeline stage.
-constexpr int kTileM = 128;            // positions per CTA tile (UMMA M per CTA, TMEM lanes)
+constexpr int kTileM = 128;            // positions per CTA tile (2 consumer warpgroups x wgmma M = 64)
+constexpr int kTileN = 128;            // output channels per tile (wgmma N); 64 fp32 accumulator registers per thread
 constexpr int kBlockK = 64;            // channels per k-block = one 128 B swizzle row of bf16
-#ifndef SDR_MMA_RAW_TMA
-#define SDR_MMA_RAW_TMA 1              // 1: raw activation tiles arrive by TMA into a shared-memory ring, the transform warps
-#endif                                 //    work shared -> shared (no global loads, cursors or prefetch registers in their loop)
-#if SDR_MMA_RAW_TMA
 constexpr int kStages = 2;             // A (transformed activations) and B (weights) stages share one full/empty barrier ring
 constexpr int kRawStages = 2;          // fp32 [64 channels][128 positions] tiles landed by TMA, read once by the transform warps
-#else
-constexpr int kStages = 3;
-constexpr int kRawStages = 0;
-#endif
-constexpr int kRawStageBytes = kTileM * 64 * 4;              // 32 KB
-constexpr int kMaxTileN = 256;         // output channels per tile (UMMA N, TMEM columns per accumulator stage)
+constexpr int kRawStageBytes = kTileM * kBlockK * 4;         // 32 KB
 constexpr int kAHalf = kTileM * 128;   // 16 KB: bf16 [128 rows][64 k]
-constexpr int kBHalfMax = (kMaxTileN / 2) * 128;             // 16 KB: this CTA's tile_n / 2 weight rows, one bf16 image
+constexpr int kBHalf = kTileN * 128;   // 16 KB: bf16 [128 weight rows][64 k]
 constexpr int kAStageBytes = 2 * kAHalf;                     // 32 KB: hi + lo
-constexpr int kBStageBytes = 2 * kBHalfMax;                  // 32 KB: hi + lo
-// Warp roles: [0, 8) epilogue slots (the register exits, MODE 0 / 2, use all 8: two warps per TMEM lane quarter, each
-// owning half of the tile's columns; the staged in-place exit, MODE 3, and MODE 1 use the first 4), 8 MMA issuer,
-// 9 weight TMA, [10, 18) operand transform, 18 raw activation TMA.  The role timeline (tools/trace_gemm.py) showed
-// proj bound by its 4 epilogue warps: 4.1 us to drain a tile + 0.8 us between tiles against 4.0 us of MMA time.
-constexpr int kEpiSlots = 8, kEpiWarps = 4, kMmaWarp = 8, kTmaWarp = 9, kProdWarp0 = 10, kProdWarps = 8;
-// (MODE 2, ReLU x gate: 8 warps with the gate rows prefetched into registers a chunk ahead measured 184 us against
-// 257 us for 4 warps fed by a TMA gate-tile ring at the cfg-2 mask shape.)
-constexpr int epi_warps(int mode) { return (mode == 0 || mode == 2) ? 8 : 4; }
-constexpr int kRawWarp = kProdWarp0 + kProdWarps;             // 18: raw activation tile TMA producer (SDR_MMA_RAW_TMA)
-constexpr int kMmaThreads = 32 * (kProdWarp0 + kProdWarps + (SDR_MMA_RAW_TMA ? 1 : 0));   // 608 (576 without the raw loader)
-#define SDR_MMA_THREADS(MODE) kMmaThreads
-constexpr int kProdThreads = 32 * kProdWarps;                 // 256
-#ifndef SDR_MMA_LEAN_PRODUCER
-#define SDR_MMA_LEAN_PRODUCER 1         // transform loop with pointer-bumped cursors and the (scale, shift) table read before the
-#endif                                  // stage wait (round-2 A/B on the B200: res_conv 90 -> 82 us, bottleneck 84 -> 78 us)
-#ifndef SDR_MMA_TRACE
-#define SDR_MMA_TRACE 0                 // diagnostic build (tools/trace_gemm.py): per-role clock64 timeline of CTA 0
-#endif
-#if SDR_MMA_TRACE
-#define SDR_TR(role, idx, slot) do { if (blockIdx.x == 0 && a.trace && (idx) < 256) a.trace[((role) * 256 + (idx)) * 4 + (slot)] = clock64(); } while (0)
-#else
-#define SDR_TR(role, idx, slot) do { } while (0)
-#endif
-#ifndef SDR_MMA_BULK
-#define SDR_MMA_BULK 1                  // 1: the in-place skip connection (mode 3) leaves through staging tiles + TMA reduce-add
-#endif
-constexpr int kStgBufs = 3;             // ring of [16 channels][128 positions] fp32 staging tiles (one TMA box each)
-constexpr int kStgFloats = 16 * 128;
-constexpr int kEpiChunk = 16;           // TMEM columns per epilogue step (x16 / x32 / x64 measured the same; 16 keeps registers low)
+constexpr int kBStageBytes = 2 * kBHalf;                     // 32 KB: hi + lo
+// Warp roles: [0, 8) the two consumer warpgroups (wgmma + epilogue), [8, 16) operand transform, 16 weight TMA,
+// 17 raw activation TMA.
+constexpr int kConsWarps = 8, kProdWarp0 = 8, kProdWarps = 8, kTmaWarp = 16, kRawWarp = 17;
+constexpr int kMmaThreads = 32 * (kRawWarp + 1);             // 576
+constexpr int kProdThreads = 32 * kProdWarps;                // 256
 constexpr int kProdElems = kTileM * kBlockK / kProdThreads;  // 32 = 8 channels x 4 positions per thread and k-block
 static_assert(kProdWarps == 8 && kProdElems == 32, "one transform warp per 8-channel k-group, 4 positions per lane");
 
 struct MmaArgs {
     const float* x;
     NormIn nin;
-    const uint8_t* wpk;        // packed weight images
     const float* bias;
     const float* residual;
     const float* gate;
@@ -100,15 +60,11 @@ struct MmaArgs {
     float* y;
     double* stats_out;
     int M, K, L;
-    int l_tiles, n_tiles, tile_n;
-    int pos_tiles;        // samples * l_tiles: 128-position tiles, CTA `rank` of a pair takes tile 2 * pp + rank
-    int num_tiles;        // pair tiles = n_tiles * ceil(pos_tiles / 2)
+    int l_tiles, n_tiles;
+    int num_tiles;        // n_tiles * samples * l_tiles; tile t covers channel tile t % n_tiles of position tile t / n_tiles
     int epilogue;
     // window mode (encoder Conv1d as a GEMM without im2col): operand element (position p, k = a*win_k + j)
     // is wav[sample, a, win_hop * p + j - win_pad] (zero outside [0, win_T)); x = wav, K = padded taps
-#if SDR_MMA_TRACE
-    long long* trace;     // diagnostic build: [role 0..5][256][4] clock64 stamps of pair 0's leader CTA
-#endif
     int win_k;            // 0 = normal pointwise mode
     int win_hop, win_pad, win_a;
     long long win_T;
@@ -146,169 +102,78 @@ __device__ __forceinline__ void fence_barrier_init() {
 __device__ __forceinline__ void fence_proxy_async_smem() {
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
 }
-__device__ __forceinline__ void bulk_g2s(void* smem_dst, const void* gsrc, uint32_t bytes, uint64_t* bar) {
-    asm volatile(
-        "cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-        ::"r"(smem_u32(smem_dst)), "l"(gsrc), "r"(bytes), "r"(smem_u32(bar)) : "memory");
+// global -> shared tensor (TMA) loads; out-of-range elements arrive as zeros
+__device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* tm, uint64_t* bar, int c0, int c1) {
+    asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
+                 ::"r"(smem_u32(smem_dst)), "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1) : "memory");
 }
-// shared -> global tensor (TMA) reduce-add of one [16 channels][128 positions] box into the [samples][M][L]
-// output (fp32 add performed in L2); rows / positions outside the tensor are clipped by the hardware.  The issuing thread tracks completion
-// with bulk groups.  (1-D bulk copies of 128 B rows measured ~17 ns per copy: request-rate bound.)
-__device__ __forceinline__ void tma_reduce_add_3d(const CUtensorMap* tm, const void* smem_src, int c0, int c1, int c2) {
-    asm volatile("cp.reduce.async.bulk.tensor.3d.global.shared::cta.add.tile.bulk_group [%0, {%2, %3, %4}], [%1];"
-                 ::"l"(tm), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2) : "memory");
-}
-// global -> shared tensor (TMA) load of one [16 channels][128 positions] box; out-of-range elements arrive as zeros
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* tm, uint64_t* bar, int c0, int c1, int c2) {
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                  ::"r"(smem_u32(smem_dst)), "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
 }
-__device__ __forceinline__ void epi_bar_sync() { asm volatile("bar.sync 1, 128;" ::: "memory"); }
-__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
-template <int N>
-__device__ __forceinline__ void bulk_wait_read() { asm volatile("cp.async.bulk.wait_group.read %0;" ::"n"(N) : "memory"); }
-__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
-__device__ __forceinline__ void prefetch_l2(const void* p) {
-    asm volatile("prefetch.global.L2 [%0];" ::"l"(p));
-}
-__device__ __forceinline__ void tc_fence_before() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-__device__ __forceinline__ void tc_fence_after() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
-// TMEM of a CTA pair: one warp of EACH CTA issues the cta_group::2 allocation / deallocation (same logical warp).
-__device__ __forceinline__ void tmem_alloc(uint32_t* smem_dst, uint32_t cols) {
-    asm volatile("tcgen05.alloc.cta_group::2.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_dst)), "r"(cols) : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::2.sync.aligned;" ::: "memory");
-}
-__device__ __forceinline__ void tmem_dealloc(uint32_t taddr, uint32_t cols) {
-    asm volatile("tcgen05.dealloc.cta_group::2.sync.aligned.b32 %0, %1;" ::"r"(taddr), "r"(cols) : "memory");
-}
-// D[256 x N] (+)= A[256 x 16] * B[N x 16]^T for the CTA pair, issued by ONE thread of the leader CTA: rows 0..127 of
-// A / D are the leader's (its shared memory / TMEM), rows 128..255 the peer's; each CTA holds N / 2 rows of B.
-__device__ __forceinline__ void umma_bf16(uint32_t d_tmem, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accumulate) {
-    asm volatile(
-        "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %4, 0;\n\t"
-        "tcgen05.mma.cta_group::2.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-        ::"r"(d_tmem), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accumulate) : "memory");
-}
-// one arrival on the barrier at the same shared-memory offset in BOTH CTAs of the pair once all prior MMAs retire
-__device__ __forceinline__ void umma_commit(uint64_t* bar) {
-    asm volatile("tcgen05.commit.cta_group::2.mbarrier::arrive::one.shared::cluster.multicast::cluster.b64 [%0], %1;"
-                 ::"r"(smem_u32(bar)), "h"((uint16_t)3) : "memory");
-}
-// ---- cluster (CTA pair) plumbing ----
-__device__ __forceinline__ uint32_t cluster_ctarank() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%cluster_ctarank;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ uint32_t cluster_id_x() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%clusterid.x;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ uint32_t num_clusters_x() {
-    uint32_t r;
-    asm volatile("mov.u32 %0, %%nclusterid.x;" : "=r"(r));
-    return r;
-}
-__device__ __forceinline__ void cluster_sync_all() {
-    asm volatile("barrier.cluster.arrive.release;\n\tbarrier.cluster.wait.acquire;" ::: "memory");
-}
-// shared::cluster address of `local` (a shared::cta address of this CTA) in the CTA of rank `rank`
-__device__ __forceinline__ uint32_t map_to_rank(uint32_t local, uint32_t rank) {
-    uint32_t r;
-    asm volatile("mapa.shared::cluster.u32 %0, %1, %2;" : "=r"(r) : "r"(local), "r"(rank));
-    return r;
-}
-// arrive on a barrier anywhere in the cluster.  Default semantics (.release.cta), as CUTLASS' ClusterBarrier::arrive:
-// what the observer (the leader's MMA thread) consumes are shared-memory operand stages that were published to the
-// async proxy with fence.proxy.async, and TMEM reads closed by tcgen05.fence::before_thread_sync.  An explicit
-// .release.cluster compiles to MEMBAR.ALL.GPU, which also waits for every prefetched global load in flight
-// (measured: proj 87 -> 114 us, res_conv 90 -> 126 us).
-__device__ __forceinline__ void mbar_arrive_cluster(uint32_t cluster_addr) {
-    asm volatile("mbarrier.arrive.shared::cluster.b64 _, [%0];" ::"r"(cluster_addr) : "memory");
-}
-__device__ __forceinline__ void mbar_wait_cluster(uint64_t* bar, uint32_t parity) {   // (an .acquire.cluster wait emits CCTL.IVALL per poll)
-    const uint32_t addr = smem_u32(bar);
-    uint32_t done;
-    do {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done) : "r"(addr), "r"(parity) : "memory");
-    } while (!done);
-}
-// TMA tile load of this CTA's weight rows into ITS shared memory; the bytes are counted on the LEADER's barrier
-// (cta_group::2 form: the mbarrier may live in the peer CTA)
-__device__ __forceinline__ void tma_load_b_2d(void* smem_dst, const CUtensorMap* tm, uint32_t bar_cluster_addr, int c0, int c1) {
-    asm volatile("cp.async.bulk.tensor.2d.cta_group::2.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
-                 ::"r"(smem_u32(smem_dst)), "l"(tm), "r"(bar_cluster_addr), "r"(c0), "r"(c1) : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t (&r)[16]) {
-    asm volatile(
-        "tcgen05.ld.sync.aligned.32x32b.x16.b32 "
-        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, [%16];"
-        : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3]), "=r"(r[4]), "=r"(r[5]), "=r"(r[6]), "=r"(r[7]),
-          "=r"(r[8]), "=r"(r[9]), "=r"(r[10]), "=r"(r[11]), "=r"(r[12]), "=r"(r[13]), "=r"(r[14]), "=r"(r[15])
-        : "r"(taddr) : "memory");
-}
-__device__ __forceinline__ void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute/arch/mma_sm100_desc.hpp
-// documents the bit layout): start address >> 4 in [0,14), LBO (unused for swizzled
-// K-major, canonical value 1) in [16,30), SBO = 1024 B (8 rows x 128 B) in [32,46),
-// version 1 in [46,48), layout type 2 (SWIZZLE_128B) in [61,64).
-__device__ __forceinline__ uint64_t umma_desc_sw128(uint32_t saddr) {
-    uint64_t d = 0;
-    d |= (uint64_t)((saddr >> 4) & 0x3FFF);
-    d |= (uint64_t)1 << 16;
-    d |= (uint64_t)(1024 >> 4) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
-    return d;
-}
-// MN-major, SWIZZLE_128B descriptor (the A operand: positions contiguous).  Canonical layout in
-// 16 B units ((8,n),(8,k)):((1,LBO),(8,SBO)): a 128 B row holds 64 consecutive MN elements of one
-// k; 8 k-rows form a 1024 B atom (16 B chunk index XOR k%8); LBO = byte stride between 64-wide MN
-// blocks, SBO = byte stride between groups of 8 k.
-__device__ __forceinline__ uint64_t umma_desc_mn_sw128(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
+// wgmma shared-memory matrix descriptor (cute/arch/mma_sm90_desc.hpp documents the bit layout): start address >> 4
+// in [0,14), leading byte offset >> 4 in [16,30), stride byte offset >> 4 in [32,46), layout type 1 (SWIZZLE_128B)
+// in [62,64).  Stage bases are 1024 B aligned, so the base offset field stays 0.
+__device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr, uint32_t lbo, uint32_t sbo) {
     uint64_t d = 0;
     d |= (uint64_t)((saddr >> 4) & 0x3FFF);
     d |= (uint64_t)((lbo >> 4) & 0x3FFF) << 16;
     d |= (uint64_t)((sbo >> 4) & 0x3FFF) << 32;
-    d |= (uint64_t)1 << 46;
-    d |= (uint64_t)2 << 61;
+    d |= (uint64_t)1 << 62;
     return d;
 }
-constexpr uint32_t kALbo = 1024;       // A tile: [8 k-groups][2 MN blocks][8 k rows][128 B]
+// A operand, MN-major (positions contiguous).  Canonical layout in 16 B units ((8,n),(8,k)):((1,LBO),(8,SBO)): a 128 B
+// row holds 64 consecutive positions of one k; 8 k-rows form a 1024 B atom (16 B chunk index XOR k%8); LBO = byte
+// stride between 64-wide position blocks (one per consumer warpgroup), SBO = byte stride between groups of 8 k.
+constexpr uint32_t kALbo = 1024;       // A tile: [8 k-groups][2 position blocks][8 k rows][128 B]
 constexpr uint32_t kASbo = 2048;
-// kind::f16 instruction descriptor: D=f32 (bit 4), A=B=bf16 (bits 7,10), A MN-major (bit 15),
-// B K-major, N>>3 in [17,23), M>>4 in [24,29); M = 256: the pair's two 128-row halves (cta_group::2).
-__device__ __forceinline__ uint32_t umma_idesc_bf16(int n) {
-    return (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | ((uint32_t)(n >> 3) << 17) | ((uint32_t)((2 * kTileM) >> 4) << 24);
+// B operand, K-major: 128 B per weight row, 8-row groups 1024 B apart (LBO unused for swizzled K-major, canonical 16 B).
+constexpr uint32_t kBLbo = 16, kBSbo = 1024;
+
+__device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T for the executing warpgroup; A MN-major (imm-trans-a = 1), B K-major.
+// Thread t of the warpgroup holds d[i] at row 16 * (t / 32) + (t % 32) / 4 + 8 * ((i / 2) % 2),
+// column 8 * (i / 4) + 2 * (t % 4) + i % 2.
+__device__ __forceinline__ void wgmma_bf16_m64n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+    asm volatile(
+        "{\n\t.reg .pred p;\n\t"
+        "setp.ne.b32 p, %66, 0;\n\t"
+        "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
+        "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
+        "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, "
+        "%45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
+        "%64, %65, p, 1, 1, 1, 0;\n\t}"
+        : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
+          "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
+          "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
+          "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]),
+          "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]),
+          "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
+          "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
+          "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "memory");
 }
 
 // ---------------------------------------------------------------------------
-// weight packing: W[M][K] fp32 -> per (n_tile, k_block, pair rank) a contiguous image of tile_n rows x 128 B
-// [hi: this rank's tile_n / 2 weight rows | lo: the same rows], rows swizzled exactly as they must sit in
-// shared memory (16 B chunk index XOR row % 8), so a k-block of one CTA is ONE TMA box of [tile_n][128 B].
-// Rank 0 of a pair holds output channels [0, tile_n / 2) of the tile, rank 1 the rest (UMMA cta_group::2 B split).
+// weight packing: W[M][K] fp32 -> per (n_tile, k_block) a contiguous image of 2 x kTileN rows x 128 B
+// [hi: the tile's weight rows | lo: the same rows], rows swizzled exactly as they must sit in shared memory
+// (16 B chunk index XOR row % 8), so a k-block is ONE TMA box of [2 * kTileN][128 B].
 // ---------------------------------------------------------------------------
 __global__ void pack_weight_mma_kernel(const float* __restrict__ W, uint8_t* __restrict__ out,
-                                       int M, int Mpad, int Kreal, int K, int tile_n) {
+                                       int M, int Mpad, int Kreal, int K) {
     const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;   // one 16 B chunk (8 k) per thread
     const long long chunks = (long long)Mpad * K / 8;
     if (i >= chunks) return;
     const int kc = (int)(i % (K / 8));        // chunk index along K
     const int m = (int)(i / (K / 8));
     const int kb = kc / 8, c = kc % 8;
-    const int nt = m / tile_n, rt = m % tile_n;
-    const int hn = tile_n / 2;
-    const int rank = rt / hn, r = rt % hn;
+    const int nt = m / kTileN, r = m % kTileN;
     const int KB = K / kBlockK;
-    const size_t half = (size_t)hn * 128;
-    uint8_t* img = out + (((size_t)nt * KB + kb) * 2 + rank) * 2 * half;
+    uint8_t* img = out + ((size_t)nt * KB + kb) * kBStageBytes;
     const size_t off = (size_t)(r >> 3) * 1024 + (size_t)(r & 7) * 128 + (size_t)((c ^ (r & 7)) << 4);
     __nv_bfloat16 hi[8], lo[8];
 #pragma unroll
@@ -319,101 +184,72 @@ __global__ void pack_weight_mma_kernel(const float* __restrict__ W, uint8_t* __r
         lo[e] = __float2bfloat16_rn(v - __bfloat162float(hi[e]));
     }
     *reinterpret_cast<uint4*>(img + off) = *reinterpret_cast<const uint4*>(hi);
-    *reinterpret_cast<uint4*>(img + half + off) = *reinterpret_cast<const uint4*>(lo);
+    *reinterpret_cast<uint4*>(img + kBHalf + off) = *reinterpret_cast<const uint4*>(lo);
 }
 
 // ---------------------------------------------------------------------------
 // the GEMM kernel
 // ---------------------------------------------------------------------------
 struct TileCoord { int sample, l0, n0; };
-// pair tile -> this CTA's (sample, first position, first output channel).  The last pair of an odd number of
-// position tiles has no tile for rank 1: it gets l0 >= L, which every load / store path already treats as
-// "outside the sample" (zero operand rows, no stores, clipped TMA boxes), so it runs the same barrier protocol.
-__device__ __forceinline__ TileCoord decode_tile(const MmaArgs& a, int tile, int rank) {
+// Consecutive tiles share a position tile (the CTAs working on its channel tiles read the same activations from L2).
+__device__ __forceinline__ TileCoord decode_tile(const MmaArgs& a, int tile) {
     TileCoord t;
-    const int nt = tile % a.n_tiles;
-    const int pos = 2 * (tile / a.n_tiles) + rank;
-    t.n0 = nt * a.tile_n;
-    if (pos < a.pos_tiles) {
-        t.sample = pos / a.l_tiles;
-        t.l0 = (pos - t.sample * a.l_tiles) * kTileM;
-    } else {
-        t.sample = 0;
-        t.l0 = a.l_tiles * kTileM;
-    }
+    const int pos = tile / a.n_tiles;
+    t.n0 = (tile - pos * a.n_tiles) * kTileN;
+    t.sample = pos / a.l_tiles;
+    t.l0 = (pos - t.sample * a.l_tiles) * kTileM;
     return t;
 }
 
-// Compile-time specialisation keeps the hot loops small: the kernel image was 64 KB (ping-pong-unrolled
-// producer + 8 specialised copies of the store loop) against a 32 KB L1.5 instruction cache, and the
-// per-chunk timeline showed the epilogue warps at IPC ~0.1 (instruction fetch stalls).
+// Compile-time specialisation keeps the hot loops small.
 //   WINDOW: encoder mode (strided waveform windows as the A operand)
 //   ACT:    PReLU in the operand transform: 0 none, 1 one shared slope (nn.PReLU()), 2 one slope per input
 //           channel (nn.PReLU(C) of the original model, sudormrf.py:33,71; shared -> shared transform loop only)
-//   MODE:   epilogue 0 = bias only, 1 = + residual (may alias y), 2 = ReLU * gate,
-//           3 = in-place skip connection (y == residual): y += acc + bias as a bulk reduce-add in L2
+//   MODE:   epilogue 0 = bias only, 1 = + residual (may alias y: every element is read by the thread that writes it),
+//           2 = ReLU * gate
 //   STATS:  accumulate (sum, sumsq) of the output
 template <bool WINDOW, int ACT, int MODE, bool STATS>
-__global__ void __launch_bounds__(SDR_MMA_THREADS(MODE), 1)
-pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap tmap,      // tmap: MODE 3 in-place output
-              const __grid_constant__ CUtensorMap wmap,                       // wmap: packed weights as [rows][128 B]
+__global__ void __launch_bounds__(kMmaThreads, 1)
+pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      // wmap: packed weights as [rows][128 B]
               const __grid_constant__ CUtensorMap xmap) {                     // xmap: activations [samples][K][L], box [64][128]
-    // 3 x (32 KB A stage + 32 KB B stage) + 8 KB of tables + 24 KB of epilogue staging + barriers
-    // (224 KB of the 227 KB an sm_100 CTA can own).  SWIZZLE_128B needs the stage bases 1024 B aligned.
-    extern __shared__ __align__(1024) uint8_t smem[];
+    // 2 x (32 KB A stage + 32 KB B stage) + 2 x 32 KB raw tiles + 4 KB of tables + barriers (of the 227 KB an sm_90
+    // CTA can own).  SWIZZLE_128B needs the stage bases 1024 B aligned; the launch reserves 1 KB to align by hand.
+    extern __shared__ uint8_t smem_raw[];
+    uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* a_base = smem;                                                  // kStages x 32 KB
     uint8_t* b_base = smem + kStages * kAStageBytes;                         // kStages x 32 KB
-    // warp-private tables (no CTA-level barrier in the steady state): per transform warp the
-    // (scale, shift) of its 32 channels, double-buffered; per epilogue warp a copy of the tile's bias
     uint8_t* r_base = b_base + kStages * kBStageBytes;                       // kRawStages x 32 KB
-    float2* s_ab = reinterpret_cast<float2*>(r_base + kRawStages * kRawStageBytes);   // [kProdWarps][2][32]
-    float* s_bias = reinterpret_cast<float*>(s_ab + kProdWarps * 64);    // [4][256] or [8][128]: per-warp bias copies
-    float* s_stage = s_bias + kEpiWarps * kMaxTileN;                     // [kStgBufs][16][128], 1024 B aligned
-    uint64_t* bars = reinterpret_cast<uint64_t*>(s_stage + kStgBufs * kStgFloats);
-    // Barriers exist at the same offsets in both CTAs of the pair.
-    //   full_bar   (the LEADER's copy is used): 8 + 8 transform warps of both CTAs + the leader's TMA thread, and the
-    //              tx bytes of both CTAs' weight loads; waited on by the leader's MMA thread.
-    //   empty_bar  (each CTA's own copy): one multicast tcgen05.commit per use, waited on by the CTA's producers.
-    //   tfull_bar  (each CTA's own copy): multicast commit at the end of a tile, waited on by the CTA's epilogue.
-    //   tempty_bar (the LEADER's copy): the epilogue warps of both CTAs (2 x 8 or 2 x 4); waited on by the leader's MMA thread.
+    // warp-private tables (no CTA-level barrier in the steady state): per transform warp the (scale, shift) of its
+    // channels, double-buffered
+    float2* s_ab = reinterpret_cast<float2*>(r_base + kRawStages * kRawStageBytes);   // [kProdWarps][64]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(s_ab + kProdWarps * 64);
+    //   full_bar:   the 8 transform warps + the weight TMA thread (with the weights' tx bytes); waited on by the consumers
+    //   empty_bar:  the 8 consumer warps once their wgmmas reading the stage have retired
+    //   rfull_bar:  raw tile landed (TMA tx bytes); rempty_bar: all 8 transform warps hold it in registers
     uint64_t* full_bar = bars;                       // [kStages]
     uint64_t* empty_bar = full_bar + kStages;        // [kStages]
-    uint64_t* tfull_bar = empty_bar + kStages;       // [2]
-    uint64_t* tempty_bar = tfull_bar + 2;            // [2]
-    uint64_t* rfull_bar = tempty_bar + 2;            // [kRawStages] raw tile landed (TMA tx bytes); CTA-local
-    uint64_t* rempty_bar = rfull_bar + 2;            // [kRawStages] all 8 transform warps hold it in registers; CTA-local
-    uint32_t* s_tmem = reinterpret_cast<uint32_t*>(rempty_bar + 2);
-    if ((smem_u32(smem) & 1023u) != 0) __trap();
+    uint64_t* rfull_bar = empty_bar + kStages;       // [kRawStages]
+    uint64_t* rempty_bar = rfull_bar + kRawStages;   // [kRawStages]
 
     const int tid = threadIdx.x;
     const int warp = tid >> 5, lane = tid & 31;
     const int KB = a.K / kBlockK;
-    const int rank = (int)cluster_ctarank();         // 0 = leader (issues the pair's MMAs)
-    const int tile0 = (int)cluster_id_x();           // pair tiles of this pair: tile0, tile0 + tstep, ...
-    const int tstep = (int)num_clusters_x();
-    const uint32_t bhalf = (uint32_t)(a.tile_n / 2) * 128;     // bytes of this CTA's rows in one bf16 weight image
+    const int tile0 = (int)blockIdx.x;               // tiles of this CTA: tile0, tile0 + tstep, ...
+    const int tstep = (int)gridDim.x;
 
     if (warp == kTmaWarp && lane == 0) {
-        for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 2 * kProdWarps + 1); mbar_init(&empty_bar[s], 1); }
-        for (int s = 0; s < 2; ++s) { mbar_init(&tfull_bar[s], 1); mbar_init(&tempty_bar[s], 2 * epi_warps(MODE)); }
-        for (int s = 0; s < 2; ++s) { mbar_init(&rfull_bar[s], 1); mbar_init(&rempty_bar[s], kProdWarps); }
+        for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], kProdWarps + 1); mbar_init(&empty_bar[s], kConsWarps); }
+        for (int s = 0; s < kRawStages; ++s) { mbar_init(&rfull_bar[s], 1); mbar_init(&rempty_bar[s], kProdWarps); }
         fence_barrier_init();
     }
-    if (warp == kMmaWarp) tmem_alloc(s_tmem, 512);
-    tc_fence_before();
     __syncthreads();
-    cluster_sync_all();                              // the peer's barriers are initialised before anyone signals them
-    tc_fence_after();
-    const uint32_t tmem_base = *s_tmem;
 
     if (warp >= kProdWarp0 && warp < kProdWarp0 + kProdWarps) {
         // ===================== A-operand transform producers =====================
         // Warp w owns the 8 channels of k-group w of every k-block; lane i owns positions 4i..4i+3.
-        // Per channel a thread does ONE float4 load (a warp reads a 512 B row segment), the folded
-        // normalisation (+PReLU), the bf16 hi/lo split, and two conflict-free 8-byte stores into the
-        // MN-major SWIZZLE_128B tile (row = channel, 64 positions per 128 B row).
-        // Rolling prefetch: as soon as channel e of the current step is consumed its register is refilled
-        // with channel e of the NEXT step, so loads stay one k-block ahead with a single copy of the code.
+        // Per channel a thread reads one float4, applies the folded normalisation (+PReLU), splits bf16 hi/lo,
+        // and does two conflict-free 8-byte stores into the MN-major SWIZZLE_128B tile (row = channel, 64
+        // positions per 128 B row).
         const int pw = warp - kProdWarp0;          // k-group (8 channels) of this warp
         const int p4 = lane * 4;                   // first of this lane's 4 positions in the tile
         const bool has_norm = a.nin.stats != nullptr;
@@ -423,7 +259,6 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap tmap,      //
                                                    // channels' PReLU slopes in entries [16, 32) of the same 64-entry slice
         static_assert(!(WINDOW && ACT != 0), "the encoder's window operand has no activation");
         const double inv_count = 1.0 / a.nin.count;
-        const size_t Ls = (size_t)a.L;
         // byte offset of (channel row e = 0, this lane's positions) inside an A half tile
         const uint32_t lane_off = (uint32_t)pw * kASbo + (uint32_t)(lane >> 4) * kALbo + (uint32_t)(lane & 1) * 8;
         const uint32_t lane_chunk = (uint32_t)((lane & 15) >> 1);
@@ -433,26 +268,7 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap tmap,      //
             if (++c.kb == KB) {
                 c.kb = 0;
                 c.tile += tstep;
-                if (c.tile < a.num_tiles) c.tc = decode_tile(a, c.tile, rank);
-            }
-        };
-        // one channel row (4 positions) of step c
-        auto load_row = [&](const Cur& c, int e) -> float4 {
-            const int l = c.tc.l0 + p4;
-            if (c.tile >= a.num_tiles || l >= a.L) return make_float4(0.f, 0.f, 0.f, 0.f);
-            if constexpr (WINDOW) {                // encoder: strided analysis windows of the waveform
-                const int k = c.kb * kBlockK + pw * 8 + e;
-                const int ch = k / a.win_k, j = k - ch * a.win_k;
-                float vv[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) {
-                    const long long t = (long long)a.win_hop * (l + u) + j - a.win_pad;
-                    vv[u] = (l + u < a.L && ch < a.win_a && t >= 0 && t < a.win_T)
-                                ? __ldg(a.x + ((size_t)c.tc.sample * a.win_a + ch) * a.win_T + t) : 0.f;
-                }
-                return make_float4(vv[0], vv[1], vv[2], vv[3]);
-            } else {                               // L % 4 == 0: the quad is entirely inside the row
-                return ldg4(a.x + ((size_t)c.tc.sample * a.K + (size_t)c.kb * kBlockK + pw * 8 + e) * Ls + l);
+                if (c.tile < a.num_tiles) c.tc = decode_tile(a, c.tile);
             }
         };
         struct Aux { float g, b; double s0, s1; float sl; };
@@ -472,259 +288,60 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap tmap,      //
             }
             return x;
         };
-        // L2 prefetch two steps ahead: this warp's 8 channel rows x 512 B = 32 lines, one per lane
-        auto prefetch_step = [&](const Cur& c) {
-            if (!WINDOW && c.tile < a.num_tiles) {
-                const int l = c.tc.l0 + (lane >> 3) * 32;
-                if (l < a.L)
-                    prefetch_l2(a.x + ((size_t)c.tc.sample * a.K + (size_t)c.kb * kBlockK + pw * 8 + (lane & 7)) * Ls + l);
+        // one stage's 8 channel rows (4 positions each) -> folded affine (+PReLU) -> bf16 hi/lo into A stage `stage`
+        auto store_rows = [&](const float4 (&v)[8], const float2 (&abv)[8], const float (&slv)[ACT == 2 ? 8 : 1],
+                              int stage) {
+            uint8_t* a_hi = a_base + (size_t)stage * kAStageBytes;
+            uint8_t* a_lo = a_hi + kAHalf;
+#pragma unroll
+            for (int e = 0; e < 8; ++e) {
+                const float2 ab = abv[e];
+                float y[4] = {fmaf(v[e].x, ab.x, ab.y), fmaf(v[e].y, ab.x, ab.y),
+                              fmaf(v[e].z, ab.x, ab.y), fmaf(v[e].w, ab.x, ab.y)};
+                if constexpr (ACT == 1) {      // PReLU in 2 ops: max(y, s*y) for s <= 1, min otherwise
+#pragma unroll
+                    for (int u = 0; u < 4; ++u) {
+                        const float t = y[u] * slope;
+                        y[u] = slope_le1 ? fmaxf(y[u], t) : fminf(y[u], t);
+                    }
+                } else if constexpr (ACT == 2) {   // this channel's own slope (either side of 1, either sign)
+                    const float sl = slv[ACT == 2 ? e : 0];
+#pragma unroll
+                    for (int u = 0; u < 4; ++u) y[u] = y[u] >= 0.f ? y[u] : y[u] * sl;
+                }
+                // hi = top 16 bits (truncation), lo = bf16(y - hi): y - hi is exact in fp32, so
+                // |y - hi - lo| <= 2^-9 |y - hi| <= 2^-16 |y|
+                uint32_t hb[4];
+#pragma unroll
+                for (int u = 0; u < 4; ++u) hb[u] = __float_as_uint(y[u]) & 0xffff0000u;
+                const uint32_t h01 = __byte_perm(hb[0], hb[1], 0x7632), h23 = __byte_perm(hb[2], hb[3], 0x7632);
+                const __nv_bfloat162 l01 = __floats2bfloat162_rn(y[0] - __uint_as_float(hb[0]), y[1] - __uint_as_float(hb[1]));
+                const __nv_bfloat162 l23 = __floats2bfloat162_rn(y[2] - __uint_as_float(hb[2]), y[3] - __uint_as_float(hb[3]));
+                const uint32_t off = lane_off + (uint32_t)e * 128 + ((lane_chunk ^ (uint32_t)e) << 4);
+                *reinterpret_cast<uint2*>(a_hi + off) = make_uint2(h01, h23);
+                *reinterpret_cast<uint2*>(a_lo + off) = make_uint2(*reinterpret_cast<const uint32_t*>(&l01),
+                                                                    *reinterpret_cast<const uint32_t*>(&l23));
             }
+            fence_proxy_async_smem();          // generic-proxy stores -> visible to the tensor core (async proxy)
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&full_bar[stage]);
         };
 
-        // this CTA's transform warps signal the LEADER's full barrier (the leader's MMA thread consumes both CTAs' stages)
-        const uint32_t full_leader0 = map_to_rank(smem_u32(&full_bar[0]), 0);      // consecutive 8-byte barriers
-#if SDR_MMA_RAW_TMA
-        // Shared -> shared transform.  The raw fp32 tile [64 channels][128 positions] of this k-block was landed by the
-        // raw loader warp's TMA (zero-filled outside the sample), so this loop has no global loads, no L2 prefetch and no
-        // address cursors: 8 conflict-free LDS.128 (a warp reads one 512 B channel row), release of the raw slot, the
-        // folded normalisation (+PReLU), the bf16 hi/lo split and the swizzled stores.  The ncu source view of the
-        // register-prefetch loop had 40 % of its samples on the scoreboard of the prefetched loads and 20 % in cursor code.
-        if constexpr (!WINDOW) {
-            int tile = tile0, kb = 0;
-            if (tile < a.num_tiles) {
-                TileCoord tc = decode_tile(a, tile, rank);
-                Cur c0; c0.tile = tile; c0.kb = 0; c0.tc = tc;
-                Aux aux = load_aux(c0);
-                uint32_t it = 0;
-                int stage = 0, rs = 0;
-                uint32_t phase = 0, rphase = 0;
-                float mean = 0.f, rstd = 1.f;          // of the current tile's sample
-                const uint32_t raw_lane = (uint32_t)(pw * 8) * 512u + (uint32_t)lane * 16u;
-#pragma unroll 1
-                while (tile < a.num_tiles) {
-                    Cur n; n.tile = tile; n.kb = kb + 1; n.tc = tc;
-                    if (n.kb == KB) {
-                        n.kb = 0;
-                        n.tile = tile + tstep;
-                        if (n.tile < a.num_tiles) n.tc = decode_tile(a, n.tile, rank);
-                    }
-                    {                                  // y = x * aa + bb  ==  gamma * (x - mean) * rstd + beta
-                        float aa = 1.f, bb = 0.f;
-                        if (has_norm) {
-                            if (kb == 0) {
-                                const double mu = aux.s0 * inv_count;
-                                double var = aux.s1 * inv_count - mu * mu;
-                                var = var < 0.0 ? 0.0 : var;
-                                mean = (float)mu;
-                                rstd = rsqrtf((float)var + kGlnEps);
-                            }
-                            aa = aux.g * rstd;
-                            bb = aux.b - mean * aa;
-                        }
-                        if (lane < 8) {
-                            my_tab[(it & 1) * 8 + lane] = make_float2(aa, bb);
-                            if constexpr (ACT == 2) my_tab[16 + (it & 1) * 8 + lane] = make_float2(aux.sl, 0.f);
-                        }
-                        aux = load_aux(n);
-                    }
-                    __syncwarp();                      // table visible to the warp (reuse is ordered by the next __syncwarp)
-                    const float2* tab = my_tab + (it & 1) * 8;
-                    float2 abv[8];
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) abv[e] = tab[e];
-                    float slv[ACT == 2 ? 8 : 1];
-                    if constexpr (ACT == 2) {
-#pragma unroll
-                        for (int e = 0; e < 8; ++e) slv[e] = tab[16 + e].x;
-                    }
-                    if (pw == 0 && lane == 0) SDR_TR(0, it, 0);
-                    mbar_wait(&rfull_bar[rs], rphase);                          // raw tile landed
-                    if (pw == 0 && lane == 0) SDR_TR(0, it, 1);
-                    const uint8_t* rp = r_base + (size_t)rs * kRawStageBytes + raw_lane;
-                    float4 v[8];
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) v[e] = *reinterpret_cast<const float4*>(rp + e * 512);
-                    __syncwarp();                      // every lane holds its quads: the slot may be refilled
-                    if (lane == 0) mbar_arrive(&rempty_bar[rs]);
-                    if (++rs == kRawStages) { rs = 0; rphase ^= 1; }
-                    mbar_wait(&empty_bar[stage], phase ^ 1);
-                    if (pw == 0 && lane == 0) SDR_TR(0, it, 2);
-                    uint8_t* a_hi = a_base + (size_t)stage * kAStageBytes;
-                    uint8_t* a_lo = a_hi + kAHalf;
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) {
-                        const float2 ab = abv[e];
-                        float y[4] = {fmaf(v[e].x, ab.x, ab.y), fmaf(v[e].y, ab.x, ab.y),
-                                      fmaf(v[e].z, ab.x, ab.y), fmaf(v[e].w, ab.x, ab.y)};
-                        if constexpr (ACT == 1) {      // PReLU in 2 ops: max(y, s*y) for s <= 1, min otherwise
-#pragma unroll
-                            for (int u = 0; u < 4; ++u) {
-                                const float t = y[u] * slope;
-                                y[u] = slope_le1 ? fmaxf(y[u], t) : fminf(y[u], t);
-                            }
-                        } else if constexpr (ACT == 2) {   // this channel's own slope (either side of 1, either sign)
-                            const float sl = slv[ACT == 2 ? e : 0];
-#pragma unroll
-                            for (int u = 0; u < 4; ++u) y[u] = y[u] >= 0.f ? y[u] : y[u] * sl;
-                        }
-                        uint32_t hb[4];
-#pragma unroll
-                        for (int u = 0; u < 4; ++u) hb[u] = __float_as_uint(y[u]) & 0xffff0000u;
-                        const uint32_t h01 = __byte_perm(hb[0], hb[1], 0x7632), h23 = __byte_perm(hb[2], hb[3], 0x7632);
-                        const __nv_bfloat162 l01 = __floats2bfloat162_rn(y[0] - __uint_as_float(hb[0]), y[1] - __uint_as_float(hb[1]));
-                        const __nv_bfloat162 l23 = __floats2bfloat162_rn(y[2] - __uint_as_float(hb[2]), y[3] - __uint_as_float(hb[3]));
-                        const uint32_t off = lane_off + (uint32_t)e * 128 + ((lane_chunk ^ (uint32_t)e) << 4);
-                        *reinterpret_cast<uint2*>(a_hi + off) = make_uint2(h01, h23);
-                        *reinterpret_cast<uint2*>(a_lo + off) = make_uint2(*reinterpret_cast<const uint32_t*>(&l01),
-                                                                            *reinterpret_cast<const uint32_t*>(&l23));
-                    }
-                    fence_proxy_async_smem();          // generic-proxy stores -> visible to the tensor core (async proxy)
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive_cluster(full_leader0 + 8u * (uint32_t)stage);
-                    if (pw == 0 && lane == 0) SDR_TR(0, it, 3);
-                    ++it;
-                    if (++stage == kStages) { stage = 0; phase ^= 1; }
-                    tile = n.tile; kb = n.kb; tc = n.tc;
-                }
-            }
-        } else
-#elif SDR_MMA_LEAN_PRODUCER
-        // The ncu source view of the loop below (profiles/r01d_tma_epilogue.md): 400 instructions per k-block and warp, of
-        // which only ~200 are the transform; the rest re-derives three (tile, k-block) cursors, 64-bit row addresses and
-        // bounds tests per row, and a quarter of the stall samples sit on the table LDS feeding each channel's first FFMA.
-        // Here: one pointer per cursor (bumped by 64 channel rows inside a tile, recomputed at a tile change), one
-        // predicate per step, and the table read before the stage wait.  Same data, same barrier protocol.
-        if constexpr (!WINDOW) {
-            const size_t kstep = (size_t)kBlockK * Ls;                       // floats between consecutive k-blocks of a row
-            // row 0 (channel pw*8 of k-block kb) at this lane's 4 positions; null: outside the sample (zero operand)
-            auto row0 = [&](const TileCoord& t, int kb) -> const float* {
-                const int l = t.l0 + p4;
-                return l < a.L ? a.x + (((size_t)t.sample * a.K + (size_t)kb * kBlockK + pw * 8) * Ls + l) : nullptr;
-            };
-            // L2 prefetch address of a step: lane -> (channel row lane & 7, 32-position segment lane >> 3)
-            auto pf0 = [&](const TileCoord& t, int kb) -> const float* {
-                const int l = t.l0 + (lane >> 3) * 32;
-                return l < a.L ? a.x + (((size_t)t.sample * a.K + (size_t)kb * kBlockK + pw * 8 + (lane & 7)) * Ls + l) : nullptr;
-            };
-            int tile = tile0, kb = 0;
-            if (tile < a.num_tiles) {
-                TileCoord tc = decode_tile(a, tile, rank);
-                const float* cp0 = row0(tc, 0);
-                float4 v[8];
-#pragma unroll
-                for (int e = 0; e < 8; ++e) v[e] = cp0 ? ldg4(cp0 + (size_t)e * Ls) : make_float4(0.f, 0.f, 0.f, 0.f);
-                Cur c0; c0.tile = tile; c0.kb = 0; c0.tc = tc;
-                Aux aux = load_aux(c0);
-                // prefetch cursor: two steps ahead of the step being transformed
-                int ptile = tile, pkb = 0;
-                const float* pp = pf0(tc, 0);
-                auto pf_advance = [&]() {
-                    if (++pkb == KB) {
-                        pkb = 0;
-                        ptile += tstep;
-                        pp = ptile < a.num_tiles ? pf0(decode_tile(a, ptile, rank), 0) : nullptr;
-                    } else if (pp) {
-                        pp += kstep;
-                    }
-                };
-                pf_advance();
-                if (ptile < a.num_tiles && pp) prefetch_l2(pp);
-                uint32_t it = 0;
-                int stage = 0;
-                uint32_t phase = 0;
-                float mean = 0.f, rstd = 1.f;          // of the current tile's sample
-#pragma unroll 1
-                while (tile < a.num_tiles) {
-                    // next step: same tile -> bump, else decode the CTA's next tile
-                    Cur n; n.tile = tile; n.kb = kb + 1; n.tc = tc;
-                    const float* np = cp0 ? cp0 + kstep : nullptr;
-                    if (n.kb == KB) {
-                        n.kb = 0;
-                        n.tile = tile + tstep;
-                        np = nullptr;
-                        if (n.tile < a.num_tiles) { n.tc = decode_tile(a, n.tile, rank); np = row0(n.tc, 0); }
-                    }
-                    pf_advance();
-                    if (ptile < a.num_tiles && pp) prefetch_l2(pp);
-                    {                                  // y = x * aa + bb  ==  gamma * (x - mean) * rstd + beta
-                        float aa = 1.f, bb = 0.f;
-                        if (has_norm) {
-                            if (kb == 0) {
-                                const double mu = aux.s0 * inv_count;
-                                double var = aux.s1 * inv_count - mu * mu;
-                                var = var < 0.0 ? 0.0 : var;
-                                mean = (float)mu;
-                                rstd = rsqrtf((float)var + kGlnEps);
-                            }
-                            aa = aux.g * rstd;
-                            bb = aux.b - mean * aa;
-                        }
-                        if (lane < 8) my_tab[(it & 1) * 8 + lane] = make_float2(aa, bb);
-                        aux = load_aux(n);
-                    }
-                    __syncwarp();                      // table visible to the warp (reuse is ordered by the next __syncwarp)
-                    const float2* tab = my_tab + (it & 1) * 8;
-                    float2 abv[8];
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) abv[e] = tab[e];               // before the stage wait: latency hidden
-                    mbar_wait(&empty_bar[stage], phase ^ 1);
-                    uint8_t* a_hi = a_base + (size_t)stage * kAStageBytes;
-                    uint8_t* a_lo = a_hi + kAHalf;
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) {
-                        const float2 ab = abv[e];
-                        float y[4] = {fmaf(v[e].x, ab.x, ab.y), fmaf(v[e].y, ab.x, ab.y),
-                                      fmaf(v[e].z, ab.x, ab.y), fmaf(v[e].w, ab.x, ab.y)};
-                        v[e] = np ? ldg4(np + (size_t)e * Ls) : make_float4(0.f, 0.f, 0.f, 0.f);   // refill: next step
-                        if (ACT) {
-#pragma unroll
-                            for (int u = 0; u < 4; ++u) {
-                                const float t = y[u] * slope;
-                                y[u] = slope_le1 ? fmaxf(y[u], t) : fminf(y[u], t);
-                            }
-                        }
-                        uint32_t hb[4];
-#pragma unroll
-                        for (int u = 0; u < 4; ++u) hb[u] = __float_as_uint(y[u]) & 0xffff0000u;
-                        const uint32_t h01 = __byte_perm(hb[0], hb[1], 0x7632), h23 = __byte_perm(hb[2], hb[3], 0x7632);
-                        const __nv_bfloat162 l01 = __floats2bfloat162_rn(y[0] - __uint_as_float(hb[0]), y[1] - __uint_as_float(hb[1]));
-                        const __nv_bfloat162 l23 = __floats2bfloat162_rn(y[2] - __uint_as_float(hb[2]), y[3] - __uint_as_float(hb[3]));
-                        const uint32_t off = lane_off + (uint32_t)e * 128 + ((lane_chunk ^ (uint32_t)e) << 4);
-                        *reinterpret_cast<uint2*>(a_hi + off) = make_uint2(h01, h23);
-                        *reinterpret_cast<uint2*>(a_lo + off) = make_uint2(*reinterpret_cast<const uint32_t*>(&l01),
-                                                                            *reinterpret_cast<const uint32_t*>(&l23));
-                    }
-                    fence_proxy_async_smem();          // generic-proxy stores -> visible to the tensor core (async proxy)
-                    __syncwarp();
-                    if (lane == 0) mbar_arrive_cluster(full_leader0 + 8u * (uint32_t)stage);
-                    ++it;
-                    if (++stage == kStages) { stage = 0; phase ^= 1; }
-                    tile = n.tile; kb = n.kb; tc = n.tc; cp0 = np;
-                }
-            }
-        } else
-#endif
-        {
         Cur c;
         c.tile = tile0; c.kb = 0;
         if (c.tile < a.num_tiles) {
-            c.tc = decode_tile(a, c.tile, rank);
-            float4 v[8];
-#pragma unroll
-            for (int e = 0; e < 8; ++e) v[e] = load_row(c, e);
+            c.tc = decode_tile(a, c.tile);
             Aux aux = load_aux(c);
-            Cur cp = c;
-            advance(cp); prefetch_step(cp);
             uint32_t it = 0;
-            int stage = 0;
-            uint32_t phase = 0;                    // parity of the ring pass (it / kStages)
-            float mean = 0.f, rstd = 1.f;          // of the current tile's sample
+            int stage = 0, rs = 0;
+            uint32_t phase = 0, rphase = 0;    // parities of the ring passes
+            float mean = 0.f, rstd = 1.f;      // of the current tile's sample
+            const uint32_t raw_lane = (uint32_t)(pw * 8) * 512u + (uint32_t)lane * 16u;
 #pragma unroll 1
             while (c.tile < a.num_tiles) {
                 Cur n = c;
-                advance(n);                        // next step (n.tile >= num_tiles: none)
-                advance(cp); prefetch_step(cp);    // two steps ahead
-                {                                  // y = x * aa + bb  ==  gamma * (x - mean) * rstd + beta
+                advance(n);                    // next step (n.tile >= num_tiles: none)
+                {                              // y = x * aa + bb  ==  gamma * (x - mean) * rstd + beta
                     float aa = 1.f, bb = 0.f;
                     if (has_norm) {
                         if (c.kb == 0) {
@@ -737,62 +354,63 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap tmap,      //
                         aa = aux.g * rstd;
                         bb = aux.b - mean * aa;
                     }
-                    if (lane < 8) my_tab[(it & 1) * 8 + lane] = make_float2(aa, bb);
+                    if (lane < 8) {
+                        my_tab[(it & 1) * 8 + lane] = make_float2(aa, bb);
+                        if constexpr (ACT == 2) my_tab[16 + (it & 1) * 8 + lane] = make_float2(aux.sl, 0.f);
+                    }
                     aux = load_aux(n);
                 }
-                __syncwarp();                      // table visible to the warp (reuse is ordered by the next __syncwarp)
-                mbar_wait(&empty_bar[stage], phase ^ 1);
-                uint8_t* a_hi = a_base + (size_t)stage * kAStageBytes;
-                uint8_t* a_lo = a_hi + kAHalf;
+                __syncwarp();                  // table visible to the warp (reuse is ordered by the next __syncwarp)
                 const float2* tab = my_tab + (it & 1) * 8;
+                float2 abv[8];
 #pragma unroll
-                for (int e = 0; e < 8; ++e) {
-                    const float2 ab = tab[e];
-                    float y[4] = {fmaf(v[e].x, ab.x, ab.y), fmaf(v[e].y, ab.x, ab.y),
-                                  fmaf(v[e].z, ab.x, ab.y), fmaf(v[e].w, ab.x, ab.y)};
-                    v[e] = load_row(n, e);         // refill: channel e of the next step
-                    if (ACT) {                     // PReLU in 2 ops: max(y, s*y) for s <= 1, min otherwise
+                for (int e = 0; e < 8; ++e) abv[e] = tab[e];
+                float slv[ACT == 2 ? 8 : 1] = {1.f};
+                if constexpr (ACT == 2) {
+#pragma unroll
+                    for (int e = 0; e < 8; ++e) slv[e] = tab[16 + e].x;
+                }
+                float4 v[8];
+                if constexpr (WINDOW) {        // encoder: strided analysis windows of the waveform, gathered directly
+                    const int l = c.tc.l0 + p4;
+#pragma unroll
+                    for (int e = 0; e < 8; ++e) {
+                        const int k = c.kb * kBlockK + pw * 8 + e;
+                        const int ch = k / a.win_k, j = k - ch * a.win_k;
+                        float vv[4];
 #pragma unroll
                         for (int u = 0; u < 4; ++u) {
-                            const float t = y[u] * slope;
-                            y[u] = slope_le1 ? fmaxf(y[u], t) : fminf(y[u], t);
+                            const long long t = (long long)a.win_hop * (l + u) + j - a.win_pad;
+                            vv[u] = (l + u < a.L && ch < a.win_a && t >= 0 && t < a.win_T)
+                                        ? __ldg(a.x + ((size_t)c.tc.sample * a.win_a + ch) * a.win_T + t) : 0.f;
                         }
+                        v[e] = make_float4(vv[0], vv[1], vv[2], vv[3]);
                     }
-                    // hi = top 16 bits (truncation), lo = bf16(y - hi): y - hi is exact in fp32, so
-                    // |y - hi - lo| <= 2^-9 |y - hi| <= 2^-16 |y|
-                    uint32_t hb[4];
+                } else {                       // the raw tile of this k-block, landed by the raw loader's TMA
+                    mbar_wait(&rfull_bar[rs], rphase);
+                    const uint8_t* rp = r_base + (size_t)rs * kRawStageBytes + raw_lane;
 #pragma unroll
-                    for (int u = 0; u < 4; ++u) hb[u] = __float_as_uint(y[u]) & 0xffff0000u;
-                    const uint32_t h01 = __byte_perm(hb[0], hb[1], 0x7632), h23 = __byte_perm(hb[2], hb[3], 0x7632);
-                    const __nv_bfloat162 l01 = __floats2bfloat162_rn(y[0] - __uint_as_float(hb[0]), y[1] - __uint_as_float(hb[1]));
-                    const __nv_bfloat162 l23 = __floats2bfloat162_rn(y[2] - __uint_as_float(hb[2]), y[3] - __uint_as_float(hb[3]));
-                    const uint32_t off = lane_off + (uint32_t)e * 128 + ((lane_chunk ^ (uint32_t)e) << 4);
-                    *reinterpret_cast<uint2*>(a_hi + off) = make_uint2(h01, h23);
-                    *reinterpret_cast<uint2*>(a_lo + off) = make_uint2(*reinterpret_cast<const uint32_t*>(&l01),
-                                                                        *reinterpret_cast<const uint32_t*>(&l23));
+                    for (int e = 0; e < 8; ++e) v[e] = *reinterpret_cast<const float4*>(rp + e * 512);
+                    __syncwarp();              // every lane holds its quads: the slot may be refilled
+                    if (lane == 0) mbar_arrive(&rempty_bar[rs]);
+                    if (++rs == kRawStages) { rs = 0; rphase ^= 1; }
                 }
-                fence_proxy_async_smem();          // generic-proxy stores -> visible to the tensor core (async proxy)
-                __syncwarp();
-                if (lane == 0) mbar_arrive_cluster(full_leader0 + 8u * (uint32_t)stage);
+                mbar_wait(&empty_bar[stage], phase ^ 1);
+                store_rows(v, abv, slv, stage);
                 ++it;
                 if (++stage == kStages) { stage = 0; phase ^= 1; }
                 c = n;
             }
         }
-        }
-    } else if (SDR_MMA_RAW_TMA && warp == kRawWarp) {
-        // ===================== raw activation tiles: TMA producer (CTA-local ring) =====================
+    } else if (warp == kRawWarp) {
+        // ===================== raw activation tiles: TMA producer =====================
         if (lane == 0 && !WINDOW) {
             int rs = 0;
             uint32_t rphase = 0;
-            [[maybe_unused]] int trit = 0;
             for (int tile = tile0; tile < a.num_tiles; tile += tstep) {
-                const TileCoord tc = decode_tile(a, tile, rank);
+                const TileCoord tc = decode_tile(a, tile);
                 for (int kb = 0; kb < KB; ++kb) {
-                    SDR_TR(1, trit, 0);
                     mbar_wait(&rempty_bar[rs], rphase ^ 1);
-                    SDR_TR(1, trit, 1);
-                    ++trit;
                     mbar_arrive_expect_tx(&rfull_bar[rs], kRawStageBytes);
                     tma_load_3d(r_base + (size_t)rs * kRawStageBytes, &xmap, &rfull_bar[rs], tc.l0, kb * kBlockK, tc.sample);
                     if (++rs == kRawStages) { rs = 0; rphase ^= 1; }
@@ -802,251 +420,78 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap tmap,      //
         __syncwarp();
     } else if (warp == kTmaWarp) {
         // ===================== B-operand (weights) TMA producer =====================
-        // Each CTA loads its own tile_n / 2 weight rows (hi | lo = one [tile_n][128 B] box of the packed image) into
-        // its own stage; the bytes of BOTH CTAs are expected by, and counted on, the leader's full barrier.
         if (lane == 0) {
-            const uint32_t full_leader0 = map_to_rank(smem_u32(&full_bar[0]), 0);
-            [[maybe_unused]] int trit = 0;
             int stage = 0;
             uint32_t phase = 0;
             for (int tile = tile0; tile < a.num_tiles; tile += tstep) {
                 const int nt = tile % a.n_tiles;
                 for (int kb = 0; kb < KB; ++kb) {
-                    SDR_TR(2, trit, 0);
                     mbar_wait(&empty_bar[stage], phase ^ 1);
-                    SDR_TR(2, trit, 1);
-                    ++trit;
-                    if (rank == 0) mbar_arrive_expect_tx(&full_bar[stage], 4 * bhalf);   // 2 CTAs x (hi + lo)
-                    const int row = ((nt * KB + kb) * 2 + rank) * a.tile_n;              // first row of this CTA's box
-                    tma_load_b_2d(b_base + (size_t)stage * kBStageBytes, &wmap,
-                                  full_leader0 + 8u * (uint32_t)stage, 0, row);
+                    mbar_arrive_expect_tx(&full_bar[stage], kBStageBytes);
+                    tma_load_2d(b_base + (size_t)stage * kBStageBytes, &wmap, &full_bar[stage], 0, (nt * KB + kb) * 2 * kTileN);
                     if (++stage == kStages) { stage = 0; phase ^= 1; }
                 }
             }
         }
         __syncwarp();
-    } else if (warp == kMmaWarp) {
-        // ===================== MMA issuer (one thread of the leader CTA) =====================
-        if (lane == 0 && rank == 0) {
-            const uint32_t idesc = umma_idesc_bf16(a.tile_n);
-            uint32_t ti = 0;
-            [[maybe_unused]] int trit = 0;
-            int stage = 0;
-            uint32_t phase = 0;
-            for (int tile = tile0; tile < a.num_tiles; tile += tstep, ++ti) {
-                const int acc = ti & 1;
-                const uint32_t aphase = (ti >> 1) & 1;
-                SDR_TR(4, ti, 0);
-                mbar_wait_cluster(&tempty_bar[acc], aphase ^ 1);          // both CTAs' epilogues drained this accumulator
-                SDR_TR(4, ti, 1);
-                tc_fence_after();
-                const uint32_t d_tmem = tmem_base + (uint32_t)acc * kMaxTileN;
-                for (int kb = 0; kb < KB; ++kb) {
-                    SDR_TR(3, trit, 0);
-                    mbar_wait_cluster(&full_bar[stage], phase);           // A of both CTAs transformed, B of both landed
-                    SDR_TR(3, trit, 1);
-                    tc_fence_after();
-                    const uint32_t sa_hi = smem_u32(a_base + (size_t)stage * kAStageBytes);
-                    const uint32_t sa_lo = sa_hi + kAHalf;
-                    const uint32_t sb_hi = smem_u32(b_base + (size_t)stage * kBStageBytes);
-                    const uint32_t sb_lo = sb_hi + bhalf;
-#pragma unroll
-                    for (int ks = 0; ks < kBlockK / 16; ++ks) {
-                        // A is MN-major: a K=16 step spans two 8-channel groups (2 * SBO bytes apart)
-                        const uint64_t dah = umma_desc_mn_sw128(sa_hi + ks * 2 * kASbo, kALbo, kASbo);
-                        const uint64_t dal = umma_desc_mn_sw128(sa_lo + ks * 2 * kASbo, kALbo, kASbo);
-                        const uint64_t dbh = umma_desc_sw128(sb_hi + ks * 32);
-                        const uint64_t dbl = umma_desc_sw128(sb_lo + ks * 32);
-                        umma_bf16(d_tmem, dah, dbh, idesc, (kb | ks) != 0 ? 1u : 0u);
-                        umma_bf16(d_tmem, dal, dbh, idesc, 1u);
-                        umma_bf16(d_tmem, dah, dbl, idesc, 1u);
-                    }
-                    umma_commit(&empty_bar[stage]);           // frees this stage in BOTH CTAs once these MMAs retire
-                    SDR_TR(3, trit, 2);
-                    ++trit;
-                    if (++stage == kStages) { stage = 0; phase ^= 1; }
-                }
-                umma_commit(&tfull_bar[acc]);                 // accumulator ready for both CTAs' epilogues
-            }
-        }
-        __syncwarp();
-    } else if (warp < epi_warps(MODE)) {
-        // ===================== epilogue: TMEM -> registers -> global =====================
-        constexpr int EG = epi_warps(MODE) / 4;   // warps per TMEM lane quarter; warp w owns columns [col0, col0 + tile_n / EG)
-        const int q = warp & 3;             // TMEM lane quarter of this warp
-        const int col0 = (warp >> 2) * (a.tile_n / EG);
+    } else if (warp < kConsWarps) {
+        // ===================== consumers: wgmma main loop + epilogue from registers =====================
+        const int wg = warp >> 2;                  // position block [64 wg, 64 wg + 64) of the tile
+        const int wr = warp & 3;                   // 16-row slice of the warpgroup's block
         const size_t Ls = (size_t)a.L;
         const bool relu_out = WINDOW && a.epilogue == 2;       // window mode only: ReLU on the way out
-        const int nchunks = a.tile_n / kEpiChunk / EG;
-        // (the same staged exit for plain stores, mode 0, measured slower than direct stores: proj 104 vs 86 us)
-        constexpr bool kBulk = SDR_MMA_BULK && MODE == 3;
-        int stg_i = 0;                       // staging ring cursor (MODE 3)
-        const uint32_t tempty_leader0 = map_to_rank(smem_u32(&tempty_bar[0]), 0);
-        const uint32_t tempty_leader1 = map_to_rank(smem_u32(&tempty_bar[1]), 0);
-        uint32_t ti = 0;
+        int stage = 0;
+        uint32_t phase = 0;
+        float acc[64];
 #pragma unroll 1
-        for (int tile = tile0; tile < a.num_tiles; tile += tstep, ++ti) {
-            const int acc = ti & 1;
-            const uint32_t aphase = (ti >> 1) & 1;
-            const TileCoord tc = decode_tile(a, tile, rank);
-            float* const sb = s_bias + warp * (kMaxTileN / EG);        // this warp's private copy of its columns' bias
-            const int ncols = min(a.tile_n, a.M - tc.n0) - col0;   // real output channels among this warp's columns (<= 0: padding)
-            if (ti == 0) {                                     // first tile: load the bias directly
-                for (int j = lane; j < a.tile_n / EG; j += 32)
-                    sb[j] = (a.bias && j < ncols) ? __ldg(a.bias + tc.n0 + col0 + j) : 0.f;
+        for (int tile = tile0; tile < a.num_tiles; tile += tstep) {
+            const TileCoord tc = decode_tile(a, tile);
+#pragma unroll
+            for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+#pragma unroll 1
+            for (int kb = 0; kb < KB; ++kb) {
+                mbar_wait(&full_bar[stage], phase);   // A transformed, B landed
+                const uint32_t sa_hi = smem_u32(a_base + (size_t)stage * kAStageBytes) + (uint32_t)wg * kALbo;
+                const uint32_t sa_lo = sa_hi + kAHalf;
+                const uint32_t sb_hi = smem_u32(b_base + (size_t)stage * kBStageBytes);
+                const uint32_t sb_lo = sb_hi + kBHalf;
+                wgmma_fence();
+#pragma unroll
+                for (int ks = 0; ks < kBlockK / 16; ++ks) {
+                    // A is MN-major: a K=16 step spans two 8-channel groups (2 * SBO bytes apart)
+                    const uint64_t dah = gmma_desc_sw128(sa_hi + ks * 2 * kASbo, kALbo, kASbo);
+                    const uint64_t dal = gmma_desc_sw128(sa_lo + ks * 2 * kASbo, kALbo, kASbo);
+                    const uint64_t dbh = gmma_desc_sw128(sb_hi + ks * 32, kBLbo, kBSbo);
+                    const uint64_t dbl = gmma_desc_sw128(sb_lo + ks * 32, kBLbo, kBSbo);
+                    wgmma_bf16_m64n128(acc, dah, dbh, (kb | ks) != 0 ? 1u : 0u);
+                    wgmma_bf16_m64n128(acc, dal, dbh, 1u);
+                    wgmma_bf16_m64n128(acc, dah, dbl, 1u);
+                }
+                wgmma_commit();
+                wgmma_wait_all();
                 __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[stage]);   // this warp's reads of the stage have retired
+                if (++stage == kStages) { stage = 0; phase ^= 1; }
             }
-            // the NEXT tile's bias travels in registers while this tile drains (it used to cost ~0.5 us of exposed
-            // L2 latency between two tiles)
-            constexpr int NB = kMaxTileN / EG / 32;
-            float nb[NB];
-            {
-                const int nxt = tile + tstep;
-                const int n0n = (nxt % a.n_tiles) * a.tile_n;
-                const int ncn = min(a.tile_n, a.M - n0n) - col0;
-#pragma unroll
-                for (int r = 0; r < NB; ++r) {
-                    const int j = lane + 32 * r;
-                    nb[r] = (nxt < a.num_tiles && a.bias && j < ncn && j < a.tile_n / EG) ? __ldg(a.bias + n0n + col0 + j) : 0.f;
-                }
-            }
-            const int l = tc.l0 + q * 32 + lane;
-            const bool valid = l < a.L;
-            const size_t out_row0 = ((size_t)tc.sample * a.M + tc.n0 + col0) * Ls + l;   // (m = n0 + col0, l)
-            // MODE 1: residual (may alias y: in-place skip connection); MODE 2: gate operand of this tile
-            const float* ep = nullptr;
-            if (MODE == 1) ep = a.residual + out_row0;
-            if (MODE == 2) ep = a.gate + ((size_t)tc.sample * a.gate_channels + (tc.n0 % a.gate_channels) + col0) * Ls + l;
-            const uint32_t t_acc = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)(acc * kMaxTileN + col0);
+            // epilogue: lane owns positions p and p + 8, and channel pairs 8 j + 2 (lane % 4) + {0, 1}
+            const int l = tc.l0 + wg * 64 + wr * 16 + (lane >> 2);
+            const int ch0 = tc.n0 + 2 * (lane & 3);
             float st_s = 0.f, st_q = 0.f;
-            if (MODE == 1 || MODE == 2) {  // pull this tile's residual / gate rows into L2 while the main loop runs
-                const int lq = tc.l0 + q * 32;
-                if (lq < a.L) {
-                    const float* e0 = ep - lane;               // position lq of row 0
-                    for (int j = lane; j < ncols; j += 32) prefetch_l2(e0 + (size_t)j * Ls);
+            const size_t gate_row0 = MODE == 2 ? (size_t)tc.sample * a.gate_channels + (tc.n0 % a.gate_channels) - tc.n0 : 0;
+#pragma unroll
+            for (int i = 0; i < 64; ++i) {
+                const int m = ch0 + 8 * (i >> 2) + (i & 1);
+                const int p = l + 8 * ((i >> 1) & 1);
+                if (m < a.M && p < a.L) {
+                    float o = acc[i] + (a.bias ? __ldg(a.bias + m) : 0.f);
+                    const size_t idx = ((size_t)tc.sample * a.M + m) * Ls + p;
+                    if (MODE == 1) o += a.residual[idx];           // plain load: may alias y
+                    if (MODE == 2) o = fmaxf(o, 0.f) * __ldg(a.gate + (gate_row0 + m) * Ls + p);
+                    if constexpr (WINDOW) { if (relu_out) o = fmaxf(o, 0.f); }   // the original model's encoder (sudormrf.py:212-218)
+                    a.y[idx] = o;
+                    if (STATS) { st_s += o; st_q = fmaf(o, o, st_q); }
                 }
             }
-            // Extra operand (MODE 1 residual / MODE 2 gate): it does not depend on the accumulator, so the 16
-            // loads of a chunk are issued as one burst a full chunk ahead (EA/EB ping-pong; the first burst before
-            // the accumulator is complete).  They may alias y (in-place skip), so a chunk's loads are always
-            // issued before the stores of the chunk before it, never interleaved after them.  (Rolling
-            // per-column refills, one or two chunks deep, measured 10 % slower.)
-            float EA[MODE != 0 ? kEpiChunk : 1], EB[MODE != 0 ? kEpiChunk : 1];
-            uint32_t R[kEpiChunk];
-            const float* epn = ep;
-            auto issue_ex = [&](float (&E)[MODE != 0 ? kEpiChunk : 1], int c) {
-                if constexpr (MODE != 0) {
-                    if (valid && c < nchunks && (c + 1) * kEpiChunk <= ncols) {
-#pragma unroll
-                        for (int j = 0; j < kEpiChunk; ++j) { E[j] = *epn; epn += Ls; }
-                    } else {
-                        epn += (size_t)kEpiChunk * Ls;         // partial / padded chunk: its slow path loads directly
-                    }
-                }
-            };
-            float* yp = a.y + out_row0;
-            auto do_chunk = [&](const float (&E)[MODE != 0 ? kEpiChunk : 1], int c) {
-                if (c >= nchunks) return;
-                tmem_ld16(t_acc + (uint32_t)(c * kEpiChunk), R);
-                tmem_ld_wait();
-                const int jmax = ncols - c * kEpiChunk;        // >= kEpiChunk for a full chunk
-                if (!valid || jmax <= 0) return;
-                const float4* b4 = reinterpret_cast<const float4*>(sb + c * kEpiChunk);
-                if (jmax >= kEpiChunk) {                       // full chunk: no per-column predicate
-#pragma unroll
-                    for (int j4 = 0; j4 < kEpiChunk / 4; ++j4) {
-                        const float4 bv = b4[j4];
-                        const float bb[4] = {bv.x, bv.y, bv.z, bv.w};
-#pragma unroll
-                        for (int u = 0; u < 4; ++u) {
-                            const int j = j4 * 4 + u;
-                            float o = __uint_as_float(R[j]) + bb[u];
-                            if (MODE == 1) o += E[MODE != 0 ? j : 0];
-                            if (MODE == 2) o = fmaxf(o, 0.f) * E[MODE != 0 ? j : 0];
-                            if constexpr (WINDOW) { if (relu_out) o = fmaxf(o, 0.f); }   // the original model's encoder (sudormrf.py:212-218)
-                            *yp = o;
-                            yp += Ls;
-                            if (STATS) { st_s += o; st_q = fmaf(o, o, st_q); }
-                        }
-                    }
-                } else {                                       // last, partially padded chunk of a padded tile
-#pragma unroll 1
-                    for (int j = 0; j < jmax; ++j) {
-                        float o = __uint_as_float(R[0]);
-#pragma unroll
-                        for (int u = 1; u < kEpiChunk; ++u) if (u == j) o = __uint_as_float(R[u]);
-                        o += sb[c * kEpiChunk + j];
-                        float ev = 0.f;
-                        if (MODE != 0) ev = ep[(size_t)(c * kEpiChunk + j) * Ls];
-                        if (MODE == 1) o += ev;
-                        if (MODE == 2) o = fmaxf(o, 0.f) * ev;
-                        if constexpr (WINDOW) { if (relu_out) o = fmaxf(o, 0.f); }
-                        yp[(size_t)j * Ls] = o;
-                        if (STATS) { st_s += o; st_q = fmaf(o, o, st_q); }
-                    }
-                }
-            };
-            if constexpr (kBulk) {
-                // Staged exit: a chunk's [16 channels][128 positions] goes to a shared-memory tile (lane =
-                // position: conflict-free rows) and leaves as ONE TMA tensor store (or fp32 reduce-add, for the
-                // in-place skip connection).  Nothing waits on global memory; the tensor map clips ragged
-                // position tiles and padded channels.  One 128-thread barrier per chunk; thread 0 issues.
-                if (warp == 0 && lane == 0) SDR_TR(5, ti, 0);
-                mbar_wait(&tfull_bar[acc], aphase);
-                if (warp == 0 && lane == 0) SDR_TR(5, ti, 1);
-                tc_fence_after();
-#pragma unroll 1
-                for (int c = 0; c < nchunks; ++c) {
-                    if (ncols - c * kEpiChunk <= 0) break;         // padded output channels: nothing to store
-                    tmem_ld16(t_acc + (uint32_t)(c * kEpiChunk), R);
-                    float* const buf = s_stage + stg_i * kStgFloats;
-                    stg_i = stg_i == kStgBufs - 1 ? 0 : stg_i + 1;
-                    const float4* b4 = reinterpret_cast<const float4*>(sb + c * kEpiChunk);
-                    float* const bp = buf + q * 32 + lane;
-                    tmem_ld_wait();
-#pragma unroll
-                    for (int j4 = 0; j4 < kEpiChunk / 4; ++j4) {
-                        const float4 bv = b4[j4];
-                        const float bb[4] = {bv.x, bv.y, bv.z, bv.w};
-#pragma unroll
-                        for (int u = 0; u < 4; ++u) {
-                            const int j = j4 * 4 + u;
-                            const float o = __uint_as_float(R[j]) + bb[u];
-                            bp[j * 128] = o;
-                            if (STATS) { if (valid) { st_s += o; st_q = fmaf(o, o, st_q); } }
-                        }
-                    }
-                    fence_proxy_async_smem();
-                    // before anyone refills the NEXT buffer, the store that read it two chunks ago must be done
-                    if (tid == 0) bulk_wait_read<kStgBufs - 2>();
-                    epi_bar_sync();
-                    if (tid == 0) {
-                        tma_reduce_add_3d(&tmap, buf, tc.l0, tc.n0 + c * kEpiChunk, tc.sample);
-                        bulk_commit();
-                    }
-                }
-            } else {
-                issue_ex(EA, 0);
-                if (warp == 0 && lane == 0) SDR_TR(5, ti, 0);
-                mbar_wait(&tfull_bar[acc], aphase);
-                if (warp == 0 && lane == 0) SDR_TR(5, ti, 1);
-                tc_fence_after();
-    #pragma unroll 1
-                for (int c = 0; c < nchunks; c += 2) {
-                    issue_ex(EB, c + 1);
-                    do_chunk(EA, c);
-                    issue_ex(EA, c + 2);
-                    do_chunk(EB, c + 1);
-                }
-            }
-            tc_fence_before();
-            __syncwarp();                                  // every lane's tcgen05.ld of this accumulator has completed
-            if (lane == 0) mbar_arrive_cluster(acc ? tempty_leader1 : tempty_leader0);
-            if (warp == 0 && lane == 0) SDR_TR(5, ti, 2);
-#pragma unroll
-            for (int r = 0; r < NB; ++r)                       // (the __syncwarp above ordered the last reads of sb)
-                if (lane + 32 * r < a.tile_n / EG) sb[lane + 32 * r] = nb[r];
-            __syncwarp();
             if (STATS) {
                 st_s = warp_sum(st_s);
                 st_q = warp_sum(st_q);
@@ -1057,22 +502,12 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap tmap,      //
             }
         }
     }
-
-    if (tid == 0) bulk_wait_all();              // staged output tiles have left shared memory and are written
-    tc_fence_before();
-    __syncthreads();
-    cluster_sync_all();                         // the peer no longer signals this CTA's barriers or reads its operand stages
-    if (warp == kMmaWarp) {
-        tc_fence_after();
-        tmem_dealloc(tmem_base, 512);
-    }
 }
 
 // ---------------------------------------------------------------------------
 // host side
 // ---------------------------------------------------------------------------
-static inline int mma_pad_m(int M) { return (M + 127) / 128 * 128; }
-static inline int mma_tile_n(int M) { return (mma_pad_m(M) % 256 == 0) ? 256 : 128; }
+static inline int mma_pad_m(int M) { return (M + kTileN - 1) / kTileN * kTileN; }
 
 // Output-channel counts that are not a multiple of 128 are zero-padded (decoder: 2*21 = 42 rows);
 // the reduction dimension must fill whole 64-channel k-blocks.
@@ -1090,18 +525,15 @@ int pack_pointwise_mma(const float* W, int M, int K, void* packed, cudaStream_t 
     const int Mpad = mma_pad_m(M);
     const long long chunks = (long long)Mpad * K / 8;
     pack_weight_mma_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, st>>>(
-        W, static_cast<uint8_t*>(packed), M, Mpad, K, K, mma_tile_n(M));
+        W, static_cast<uint8_t*>(packed), M, Mpad, K, K);
     return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
 }
 
-constexpr size_t kMmaSmemBytes = (size_t)kStages * (kAStageBytes + kBStageBytes) + (size_t)kRawStages * kRawStageBytes +
-                                 kProdWarps * 64 * sizeof(float2) + kEpiWarps * kMaxTileN * sizeof(float) +
-                                 (size_t)kStgBufs * kStgFloats * sizeof(float) +
-                                 (2 * kStages + 4 + 4 + 2) * sizeof(uint64_t);
-static_assert(kEpiChunk == 16, "tmem_ld16 is hard-wired in the epilogue");
-static_assert(kMmaSmemBytes <= 232448, "exceeds the 227 KB a CTA may own on sm_100");
+constexpr size_t kMmaSmemBytes = 1024 + (size_t)kStages * (kAStageBytes + kBStageBytes) +
+                                 (size_t)kRawStages * kRawStageBytes + kProdWarps * 64 * sizeof(float2) +
+                                 (2 * kStages + 2 * kRawStages) * sizeof(uint64_t);
+static_assert(kMmaSmemBytes <= 232448, "exceeds the 227 KB a CTA may own on sm_90");
 
-// Tensor map of the fp32 output [samples][M][L] with a [1][16][128] box (the epilogue's staging tile).
 // cuTensorMapEncodeTiled is a pure host-side encoder; it is fetched through the runtime so that the library
 // carries no link-time dependency on libcuda.
 typedef CUresult (*EncodeTiledFn)(CUtensorMap*, CUtensorMapDataType, cuuint32_t, void*, const cuuint64_t*,
@@ -1118,30 +550,16 @@ static EncodeTiledFn encode_tiled_fn() {
     }();
     return fn;
 }
-static int make_tile_map(CUtensorMap* tm, const float* y, int samples, int M, int L, bool needed) {
-    memset(tm, 0, sizeof(*tm));
-    if (!needed) return SDR_OK;
-    EncodeTiledFn enc = encode_tiled_fn();
-    if (!enc) return SDR_ERR_CUDA;
-    const cuuint64_t dims[3] = {(cuuint64_t)L, (cuuint64_t)M, (cuuint64_t)samples};
-    const cuuint64_t strides[2] = {(cuuint64_t)L * 4, (cuuint64_t)L * M * 4};        // bytes, dims 1..2
-    const cuuint32_t box[3] = {(cuuint32_t)kTileM, (cuuint32_t)kEpiChunk, 1};
-    const cuuint32_t estr[3] = {1, 1, 1};
-    const CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(y), dims, strides, box, estr,
-                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
-                           CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
-    return r == CUDA_SUCCESS ? SDR_OK : SDR_ERR_UNSUPPORTED;
-}
 
-// Tensor map of a packed weight buffer seen as [rows][128 B]: one box = the tile_n rows (hi | lo) of one
-// (n_tile, k_block, pair rank) image, already in shared-memory order (no TMA swizzle).
-static int make_weight_map(CUtensorMap* tm, const void* wpk, size_t bytes, int tile_n) {
+// Tensor map of a packed weight buffer seen as [rows][128 B]: one box = the 2 x kTileN rows (hi | lo) of one
+// (n_tile, k_block) image, already in shared-memory order (no TMA swizzle).
+static int make_weight_map(CUtensorMap* tm, const void* wpk, size_t bytes) {
     memset(tm, 0, sizeof(*tm));
     EncodeTiledFn enc = encode_tiled_fn();
     if (!enc) return SDR_ERR_CUDA;
     const cuuint64_t dims[2] = {32, (cuuint64_t)(bytes / 128)};
     const cuuint64_t strides[1] = {128};
-    const cuuint32_t box[2] = {32, (cuuint32_t)tile_n};
+    const cuuint32_t box[2] = {32, (cuuint32_t)(2 * kTileN)};
     const cuuint32_t estr[2] = {1, 1};
     const CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<void*>(wpk), dims, strides, box, estr,
                            CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
@@ -1149,11 +567,10 @@ static int make_weight_map(CUtensorMap* tm, const void* wpk, size_t bytes, int t
     return r == CUDA_SUCCESS ? SDR_OK : SDR_ERR_UNSUPPORTED;
 }
 
-// Tensor map of the activations [samples][K][L] with a [1][64][128] box: one raw k-block tile of one CTA
-// (positions beyond L arrive as zeros: ragged last tiles and the idle CTA of an odd pair need no special case).
+// Tensor map of the activations [samples][K][L] with a [1][64][128] box: one raw k-block tile
+// (positions beyond L arrive as zeros: ragged last tiles need no special case).
 static int make_act_map(CUtensorMap* tm, const float* x, int samples, int K, int L) {
     memset(tm, 0, sizeof(*tm));
-    if (!SDR_MMA_RAW_TMA) return SDR_OK;
     EncodeTiledFn enc = encode_tiled_fn();
     if (!enc) return SDR_ERR_CUDA;
     const cuuint64_t dims[3] = {(cuuint64_t)L, (cuuint64_t)K, (cuuint64_t)samples};
@@ -1166,109 +583,71 @@ static int make_act_map(CUtensorMap* tm, const float* x, int samples, int K, int
     return r == CUDA_SUCCESS ? SDR_OK : SDR_ERR_UNSUPPORTED;
 }
 
-// Persistent launch as clusters of two CTAs (a CTA pair shares one TPC): as many pairs as can be resident at once
-// (queried once per kernel instantiation and device), never more than there are pair tiles.
+// Persistent launch: one CTA per SM (the shared-memory footprint allows no second), never more than there are tiles.
 // (All instantiations share one function-pointer type, so the per-kernel state is keyed by the pointer, not by Kern.)
-struct PairLaunchInfo { const void* fn; int dev; int max_pairs; };
-static std::mutex g_pair_mutex;
-static std::vector<PairLaunchInfo> g_pair_info;
+struct MmaLaunchInfo { const void* fn; int dev; int sms; };
+static std::mutex g_launch_mutex;
+static std::vector<MmaLaunchInfo> g_launch_info;
 
 template <typename Kern>
-static int launch_pairs(Kern kern, const MmaArgs& a, const CUtensorMap& tmap, const CUtensorMap& wmap, const CUtensorMap& xmap,
-                        cudaStream_t st) {
+static int launch_persistent(Kern kern, const MmaArgs& a, const CUtensorMap& wmap, const CUtensorMap& xmap,
+                             cudaStream_t st) {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) return SDR_ERR_CUDA;
-    cudaLaunchConfig_t cfg;
-    memset(&cfg, 0, sizeof(cfg));
-    cudaLaunchAttribute attr[1];
-    attr[0].id = cudaLaunchAttributeClusterDimension;
-    attr[0].val.clusterDim.x = 2; attr[0].val.clusterDim.y = 1; attr[0].val.clusterDim.z = 1;
-    cfg.blockDim = dim3(kMmaThreads, 1, 1);
-    cfg.dynamicSmemBytes = kMmaSmemBytes;
-    cfg.stream = st;
-    cfg.attrs = attr;
-    cfg.numAttrs = 1;
-    int max_pairs = 0;
+    int sms = 0;
     {
-        std::lock_guard<std::mutex> lock(g_pair_mutex);
-        for (const PairLaunchInfo& e : g_pair_info)
-            if (e.fn == reinterpret_cast<const void*>(kern) && e.dev == dev) { max_pairs = e.max_pairs; break; }
-        if (max_pairs == 0) {                     // first launch of this kernel on this device
+        std::lock_guard<std::mutex> lock(g_launch_mutex);
+        for (const MmaLaunchInfo& e : g_launch_info)
+            if (e.fn == reinterpret_cast<const void*>(kern) && e.dev == dev) { sms = e.sms; break; }
+        if (sms == 0) {                           // first launch of this kernel on this device
             if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMmaSmemBytes) != cudaSuccess) {
                 cudaGetLastError();
                 return SDR_ERR_CUDA;
             }
-            int sms = 0, n = 0;
-            if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return SDR_ERR_CUDA;
-            cfg.gridDim = dim3((unsigned)(sms & ~1), 1, 1);
-            if (cudaOccupancyMaxActiveClusters(&n, kern, &cfg) != cudaSuccess || n <= 0) { cudaGetLastError(); n = sms / 2; }
-            max_pairs = n < sms / 2 ? n : sms / 2;
-            if (max_pairs < 1) max_pairs = 1;
-            g_pair_info.push_back(PairLaunchInfo{reinterpret_cast<const void*>(kern), dev, max_pairs});
-            if (getenv("SDR_B200_DEBUG")) fprintf(stderr, "[sdr] pair kernel %p: %d SMs, %d resident pairs (occupancy query %d)\n",
-                                                  reinterpret_cast<const void*>(kern), sms, max_pairs, n);
+            if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) return SDR_ERR_CUDA;
+            g_launch_info.push_back(MmaLaunchInfo{reinterpret_cast<const void*>(kern), dev, sms});
         }
     }
-    const int pairs = a.num_tiles < max_pairs ? a.num_tiles : max_pairs;
-    cfg.gridDim = dim3((unsigned)(2 * pairs), 1, 1);
-    if (cudaLaunchKernelEx(&cfg, kern, a, tmap, wmap, xmap) != cudaSuccess) { cudaGetLastError(); return SDR_ERR_CUDA; }
+    const int grid = a.num_tiles < sms ? a.num_tiles : sms;
+    kern<<<grid, kMmaThreads, kMmaSmemBytes, st>>>(a, wmap, xmap);
+    if (cudaGetLastError() != cudaSuccess) return SDR_ERR_CUDA;
     return SDR_OK;
 }
-
-#if SDR_MMA_TRACE
-static long long* g_trace_buf = nullptr;
-extern "C" __attribute__((visibility("default"))) void sdr_debug_set_trace(void* device_buf) {
-    g_trace_buf = static_cast<long long*>(device_buf);
-}
-#endif
 
 int launch_pointwise_mma(const float* x, const NormIn& nin, const void* wpk, const float* bias,
                          const float* residual, const float* gate, int gate_channels,
                          float* y, double* stats_out, int samples, int M, int K, int L,
                          int epilogue, cudaStream_t st) {
     if (!pointwise_mma_eligible(M, K) || (L % 4) != 0 || (reinterpret_cast<uintptr_t>(x) % 16) != 0)
-        return SDR_ERR_UNSUPPORTED;                      // float4 activation loads
+        return SDR_ERR_UNSUPPORTED;                      // TMA rows of the activations: 16 B aligned
     if (samples <= 0 || L <= 0 || !x || !wpk || !y) return SDR_ERR_BAD_ARGUMENT;
     if (epilogue == 1 && (!gate || gate_channels <= 0)) return SDR_ERR_BAD_ARGUMENT;
-    if (epilogue == 1 && (gate_channels % mma_tile_n(M)) != 0) return SDR_ERR_UNSUPPORTED;
+    if (epilogue == 1 && (gate_channels % kTileN) != 0) return SDR_ERR_UNSUPPORTED;
     if (reinterpret_cast<uintptr_t>(wpk) % 16) return SDR_ERR_BAD_ARGUMENT;
     MmaArgs a;
-    a.x = x; a.nin = nin; a.wpk = static_cast<const uint8_t*>(wpk); a.bias = bias; a.residual = residual;
+    a.x = x; a.nin = nin; a.bias = bias; a.residual = residual;
     a.gate = gate; a.gate_channels = gate_channels; a.y = y; a.stats_out = stats_out;
     a.M = M; a.K = K; a.L = L; a.epilogue = epilogue;
-#if SDR_MMA_TRACE
-    a.trace = g_trace_buf;
-#endif
     a.win_k = 0; a.win_hop = 0; a.win_pad = 0; a.win_a = 0; a.win_T = 0;
-    a.tile_n = mma_tile_n(M);
-    a.n_tiles = mma_pad_m(M) / a.tile_n;
+    a.n_tiles = mma_pad_m(M) / kTileN;
     a.l_tiles = (L + kTileM - 1) / kTileM;
-    const long long pos_tiles = (long long)samples * a.l_tiles;
-    const long long tiles = (pos_tiles + 1) / 2 * a.n_tiles;
-    if (pos_tiles > 0x3fffffffLL || tiles > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-    a.pos_tiles = (int)pos_tiles;
+    const long long tiles = (long long)samples * a.l_tiles * a.n_tiles;
+    if (tiles > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
     a.num_tiles = (int)tiles;
     const int act = nin.prelu ? (nin.prelu_pc ? 2 : 1) : 0;
-    if (act == 2 && !SDR_MMA_RAW_TMA) return SDR_ERR_UNSUPPORTED;     // per-channel slopes exist in the shared -> shared transform loop only
-    // in-place skip connection (every U-ConvBlock's res_conv): the residual add happens in L2 (bulk reduce-add)
-    const bool inplace = SDR_MMA_BULK && residual == y && (reinterpret_cast<uintptr_t>(y) % 16) == 0;
-    const int mode = epilogue == 1 ? 2 : (residual ? (inplace ? 3 : 1) : 0);
+    const int mode = epilogue == 1 ? 2 : (residual ? 1 : 0);
     const bool stats = stats_out != nullptr;
-    CUtensorMap ymap;      // MODE 3: the in-place output
-    if (int rc = make_tile_map(&ymap, y, samples, M, L, mode == 3)) return rc;
     CUtensorMap wmap, xmap;
-    if (int rc = make_weight_map(&wmap, wpk, pointwise_mma_packed_bytes(M, K), a.tile_n)) return rc;
+    if (int rc = make_weight_map(&wmap, wpk, pointwise_mma_packed_bytes(M, K))) return rc;
     if (int rc = make_act_map(&xmap, x, samples, K, L)) return rc;
 #define SDR_MMA_CASE(A, MD, ST)                                                                                   \
-    if (act == A && mode == MD && stats == ST) return launch_pairs(pw_mma_kernel<false, A, MD, ST>, a, ymap, wmap, xmap, st);
+    if (act == A && mode == MD && stats == ST) return launch_persistent(pw_mma_kernel<false, A, MD, ST>, a, wmap, xmap, st);
     SDR_MMA_CASE(0, 0, false) SDR_MMA_CASE(0, 0, true)
     SDR_MMA_CASE(1, 0, false) SDR_MMA_CASE(1, 0, true)
     SDR_MMA_CASE(0, 1, false) SDR_MMA_CASE(0, 1, true)
     SDR_MMA_CASE(1, 1, false) SDR_MMA_CASE(1, 1, true)
     SDR_MMA_CASE(0, 2, false) SDR_MMA_CASE(0, 2, true)
     SDR_MMA_CASE(1, 2, false) SDR_MMA_CASE(1, 2, true)
-    SDR_MMA_CASE(0, 3, false) SDR_MMA_CASE(0, 3, true)
-    SDR_MMA_CASE(1, 3, false) SDR_MMA_CASE(1, 3, true)
     SDR_MMA_CASE(2, 0, false) SDR_MMA_CASE(2, 0, true)      // the original model: proj_1x1 / conv_1x1_exp / mask front
 #undef SDR_MMA_CASE
     return SDR_ERR_UNSUPPORTED;
@@ -1287,7 +666,7 @@ int pack_encoder_mma(const float* W, int N, int A, int Kk, void* packed, cudaStr
     const int Mpad = mma_pad_m(N), K = enc_kpad(A, Kk);
     const long long chunks = (long long)Mpad * K / 8;
     pack_weight_mma_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, st>>>(
-        W, static_cast<uint8_t*>(packed), N, Mpad, A * Kk, K, mma_tile_n(N));
+        W, static_cast<uint8_t*>(packed), N, Mpad, A * Kk, K);
     return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
 }
 
@@ -1297,28 +676,20 @@ int launch_encoder_mma(const float* wav, const void* wpk, const float* bias, int
     if (B <= 0 || T <= 0 || L <= 0 || !wav || !wpk || !enc) return SDR_ERR_BAD_ARGUMENT;
     MmaArgs a;
     a.x = wav; a.nin = NormIn{nullptr, nullptr, nullptr, nullptr, 1.0};
-    a.wpk = static_cast<const uint8_t*>(wpk); a.bias = bias; a.residual = nullptr; a.gate = nullptr;
+    a.bias = bias; a.residual = nullptr; a.gate = nullptr;
     a.gate_channels = 0; a.y = enc; a.stats_out = stats;
     a.M = N; a.K = enc_kpad(A, Kk); a.L = L; a.epilogue = relu ? 2 : 0;      // (window kernels read it as "ReLU on the way out")
-#if SDR_MMA_TRACE
-    a.trace = nullptr;
-#endif
     a.win_k = Kk; a.win_hop = Kk / 2; a.win_pad = pad; a.win_a = A; a.win_T = T;   // pad = hop; 2 * hop for the causal model
-    a.tile_n = mma_tile_n(N);
-    a.n_tiles = mma_pad_m(N) / a.tile_n;
+    a.n_tiles = mma_pad_m(N) / kTileN;
     a.l_tiles = (L + kTileM - 1) / kTileM;
-    const long long pos_tiles = (long long)B * a.l_tiles;
-    const long long tiles = (pos_tiles + 1) / 2 * a.n_tiles;
-    if (pos_tiles > 0x3fffffffLL || tiles > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-    a.pos_tiles = (int)pos_tiles;
+    const long long tiles = (long long)B * a.l_tiles * a.n_tiles;
+    if (tiles > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
     a.num_tiles = (int)tiles;
-    CUtensorMap ymap, wmap;
-    if (int rc = make_tile_map(&ymap, enc, B, N, L, false)) return rc;
-    if (int rc = make_weight_map(&wmap, wpk, encoder_mma_packed_bytes(N, A, Kk), a.tile_n)) return rc;
-    CUtensorMap xmap;
+    CUtensorMap wmap, xmap;
+    if (int rc = make_weight_map(&wmap, wpk, encoder_mma_packed_bytes(N, A, Kk))) return rc;
     memset(&xmap, 0, sizeof(xmap));               // window mode gathers the waveform itself
-    if (stats) return launch_pairs(pw_mma_kernel<true, 0, 0, true>, a, ymap, wmap, xmap, st);
-    return launch_pairs(pw_mma_kernel<true, 0, 0, false>, a, ymap, wmap, xmap, st);
+    if (stats) return launch_persistent(pw_mma_kernel<true, 0, 0, true>, a, wmap, xmap, st);
+    return launch_persistent(pw_mma_kernel<true, 0, 0, false>, a, wmap, xmap, st);
 }
 
 }  // namespace sdr

@@ -131,7 +131,7 @@ __device__ __forceinline__ void pyr_bulk_g2s(void* dst, const void* src, uint32_
 // waits on a global load (one CTA per row with plain loads measured 1.7 us per row and SM: launch-to-first-use
 // latency of y, of the 28 parameters and of the fp64 statistics in every CTA).  One barrier per row.
 #ifndef SDR_PYR_MINB
-#define SDR_PYR_MINB 6                  // resident CTAs per SM the <= 256-thread instantiation is compiled for (A/B on the B200: 4 -> 177 us, 5 -> 175, 6 -> 165 at cfg 2)
+#define SDR_PYR_MINB 6                  // resident CTAs per SM the <= 256-thread instantiation is compiled for
 #endif
 // PC: one PReLU slope per channel (the original model's nn.PReLU(C), sudormrf.py:33): a row is one channel, so the
 // slope simply travels with the row's other parameters; the shared-slope instantiations are unchanged.

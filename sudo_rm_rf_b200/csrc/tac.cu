@@ -147,7 +147,7 @@ tac_kernel(const float* __restrict__ x, TacParams p, float* __restrict__ o,
 // The FFMA kernel above ran at 0.19 of the HBM roofline (173 us for 210 MB at the benchmark shape): 27.6 k MACs per
 // time column on the FP32 pipe.  The three linear maps are small GEMMs over positions, so here a WARP owns 16
 // consecutive positions of one batch element and walks the groups with warp-level MMAs (mma.sync m16n8k16, bf16
-// operands split hi/lo in three products like the tcgen05 GEMM, fp32 accumulate):
+// operands split hi/lo in three products like the wgmma GEMM, fp32 accumulate):
 //   pass 1, per group g:  h_g[16 x 48] = PReLU(X_g[16 x 16] W1^T + b1), accumulated into the group mean (registers)
 //   once:                 q = PReLU(mean W2^T + b2),   u = q W3[:, 48:]^T + b3
 //   pass 2, per group g:  h_g again (X_g is re-read from L1/L2; keeping 16 groups of h would take 384 registers),

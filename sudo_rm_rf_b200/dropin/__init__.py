@@ -1,4 +1,4 @@
-"""Two ways to make the reference's import paths resolve to the B200-native modules.
+"""Two ways to make the reference's import paths resolve to the H100-native modules.
 
 1. Path overlay: put THIS directory ahead of the reference checkout on ``sys.path``.  The overlay
    packages under ``sudo_rm_rf/`` hold only the accelerated modules and extend their ``__path__``

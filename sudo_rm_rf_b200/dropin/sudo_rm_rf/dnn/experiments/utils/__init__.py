@@ -1,4 +1,4 @@
-"""Drop-in overlay package: only the B200-native modules live here.
+"""Drop-in overlay package: only the H100-native modules live here.
 
 Every other sub-module of this package (losses, arg parsers, dataset loaders, the other model
 families ...) must keep resolving to the reference checkout that sits LATER on ``sys.path``, so the

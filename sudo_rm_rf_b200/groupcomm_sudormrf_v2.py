@@ -1,9 +1,9 @@
-"""B200-native mirror of ``sudo_rm_rf/dnn/models/groupcomm_sudormrf_v2.py``.
+"""H100-native mirror of ``sudo_rm_rf/dnn/models/groupcomm_sudormrf_v2.py``.
 
 Same constructor, attributes, sub-module / parameter names (``state_dict()``
 keys such as ``sm.3.TAC.TAC_input.0.weight`` / ``sm.3.UBlock.proj_1x1.conv.weight``)
 and ``forward(input_wav)`` as the reference's ``GroupCommSudoRmRf``
-(groupcomm_sudormrf_v2.py:231-339); the arithmetic runs in the sm_100a
+(groupcomm_sudormrf_v2.py:231-339); the arithmetic runs in the sm_90a
 kernels behind ``include/sudormrf_b200.h``.
 """
 import torch
@@ -44,7 +44,7 @@ class GC_UConvBlock(nn.Module):
 
 
 class GroupCommSudoRmRf(_engine.NativeModuleMixin, nn.Module):
-    """Group-communication SuDoRM-RF (reference :231-339) on the B200 native path."""
+    """Group-communication SuDoRM-RF (reference :231-339) on the H100 native path."""
 
     def __init__(self, in_audio_channels=1, out_channels=256, in_channels=512, num_blocks=16,
                  upsampling_depth=5, enc_kernel_size=21, enc_num_basis=512, num_sources=2,

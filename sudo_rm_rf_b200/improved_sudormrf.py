@@ -1,4 +1,4 @@
-"""B200-native mirror of ``sudo_rm_rf/dnn/models/improved_sudormrf.py``.
+"""H100-native mirror of ``sudo_rm_rf/dnn/models/improved_sudormrf.py``.
 
 Same public surface as the reference module (class names, constructor
 arguments and defaults, public attributes, sub-module / parameter names and
@@ -6,7 +6,7 @@ therefore ``state_dict()`` keys, ``forward(input_wav)`` signature), so the
 reference's notebooks, ``dnn/experiments`` runners, ``load_state_dict`` of
 published checkpoints and ``torch.load`` of whole-module pickles keep working.
 The arithmetic of ``SuDORMRF.forward`` (improved_sudormrf.py:283-301) is done
-by hand-written sm_100a kernels behind ``include/sudormrf_b200.h``; the
+by hand-written sm_90a kernels behind ``include/sudormrf_b200.h``; the
 sub-modules below only own the parameters.  Inference only: there is no
 autograd through the native path and no CPU path.
 """
@@ -20,7 +20,7 @@ from . import _engine
 
 def _not_standalone(self, *_, **__):
     raise NotImplementedError(
-        f"{type(self).__name__} is a parameter container of the B200 forward path; "
+        f"{type(self).__name__} is a parameter container of the H100 forward path; "
         "call the parent SuDORMRF / GroupCommSudoRmRf module instead.")
 
 
@@ -107,7 +107,7 @@ def _xavier_uniform_(w):
 
 
 class SuDORMRF(_engine.NativeModuleMixin, nn.Module):
-    """Improved SuDoRM-RF separator (reference :223-318) on the B200 native path."""
+    """Improved SuDoRM-RF separator (reference :223-318) on the H100 native path."""
 
     def __init__(self, out_channels=128, in_channels=512, num_blocks=16, upsampling_depth=4,
                  enc_kernel_size=21, enc_num_basis=512, num_sources=2):

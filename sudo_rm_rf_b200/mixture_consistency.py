@@ -1,4 +1,4 @@
-"""B200-native mirror of ``sudo_rm_rf/dnn/experiments/utils/mixture_consistency.py``."""
+"""H100-native mirror of ``sudo_rm_rf/dnn/experiments/utils/mixture_consistency.py``."""
 import ctypes as C
 
 import torch

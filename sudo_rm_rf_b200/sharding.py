@@ -3,7 +3,7 @@
 Every mixture is independent end to end (all reductions of the forward are
 within a sample), so the path shards by splitting the batch; there is NO
 collective inside the step.  The only communication is ONE broadcast of the
-weights at load time -- the B200-native replacement for ``nn.DataParallel``'s
+weights at load time -- the H100-native replacement for ``nn.DataParallel``'s
 per-forward module replication (run_improved_sudormrf.py:118 of the reference).
 """
 from __future__ import annotations

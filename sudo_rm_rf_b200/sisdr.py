@@ -1,4 +1,4 @@
-"""B200-native mirror of the evaluation metrics in ``sudo_rm_rf/dnn/losses/sisdr.py``.
+"""H100-native mirror of the evaluation metrics in ``sudo_rm_rf/dnn/losses/sisdr.py``.
 
 ``PermInvariantSISDR`` keeps the reference's constructor arguments, ``forward``
 signature and return conventions (sisdr.py:66-194), but it is the *metric* the

@@ -1,12 +1,12 @@
-"""B200-native mirror of ``sudo_rm_rf/dnn/models/sudormrf.py`` (the ORIGINAL SuDoRM-RF).
+"""H100-native mirror of ``sudo_rm_rf/dnn/models/sudormrf.py`` (the ORIGINAL SuDoRM-RF).
 
 Same public surface as the reference module (class names, constructor arguments and defaults, public
 attributes, sub-module / parameter names and therefore ``state_dict()`` keys, ``forward(input_wav)``), so
 ``run_fuss_separation.py:134-170``-style model selection, ``load_state_dict`` of checkpoints and whole-module
-pickles keep working.  The arithmetic of ``SuDORMRF.forward`` (reference :266-292) is done by the sm_100a kernels
+pickles keep working.  The arithmetic of ``SuDORMRF.forward`` (reference :266-292) is done by the sm_90a kernels
 behind ``include/sudormrf_b200.h`` (variant 3): ``GroupNorm(1, C, eps=1e-8)`` is the same normalisation as the
 improved model's GlobLN and is deferred to the consumers' operand loads in the same way, the per-channel PReLUs
-ride on those loads, the ``(N + 1) x 1`` mask ``Conv2d`` runs as one more GEMM on the tcgen05 kernel (a Toeplitz
+ride on those loads, the ``(N + 1) x 1`` mask ``Conv2d`` runs as one more GEMM on the wgmma kernel (a Toeplitz
 matrix expanded at pack time), the grouped decoder as block-diagonal weights of the frames GEMM
 (``csrc/original.cu``).  The sub-modules below only own the parameters.  Inference only; no CPU path.
 """
@@ -96,7 +96,7 @@ class UBlock(nn.Module):
 
 
 class SuDORMRF(_engine.NativeModuleMixin, nn.Module):
-    """The original SuDoRM-RF separator (reference :185-297) on the B200 native path."""
+    """The original SuDoRM-RF separator (reference :185-297) on the H100 native path."""
 
     _b200_variant = 3
 

@@ -16,7 +16,7 @@ GOLDEN_DIR = os.path.join(REPO, "tests", "golden")
 
 
 def pytest_configure(config):
-    config.addinivalue_line("markers", "gpu: needs a CUDA device (run on the B200 box)")
+    config.addinivalue_line("markers", "gpu: needs a CUDA device")
 
 
 def pytest_collection_modifyitems(config, items):

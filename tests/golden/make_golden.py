@@ -1,8 +1,8 @@
 """Generate the golden fixtures in this directory from the UNMODIFIED reference.
 
-Run in the build container only (needs /root/reference):
+Needs a checkout of the original sudo_rm_rf repository, named by SUDO_RM_RF_REFERENCE:
 
-    python tests/golden/make_golden.py
+    SUDO_RM_RF_REFERENCE=/path/to/sudo_rm_rf python tests/golden/make_golden.py
 
 The reference (etzinis/sudo_rm_rf) ships no golden vectors for its forward path
 (SURVEY.md §4), so these fixtures are outputs of the reference's own
@@ -22,7 +22,7 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(os.path.dirname(HERE))
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.environ["SUDO_RM_RF_REFERENCE"])
 sys.path.insert(0, REPO)
 warnings.filterwarnings("ignore")
 

@@ -1,7 +1,8 @@
 """Golden fixtures for the steps either side of the forward (SURVEY.md 8f rows 1-2),
-generated from the UNMODIFIED reference.  Build container only (needs /root/reference):
+generated from the UNMODIFIED reference.  Needs a checkout of the original sudo_rm_rf repository,
+named by SUDO_RM_RF_REFERENCE:
 
-    python tests/golden/make_golden_prepost.py
+    SUDO_RM_RF_REFERENCE=/path/to/sudo_rm_rf python tests/golden/make_golden_prepost.py
 
 * ``prepost_separate_*.npz``: the README inference recipe (README.md:100-114) executed with
   the reference's own modules on raw (un-normalised) mixtures: state_dict, wav, estimates
@@ -19,7 +20,7 @@ import torch
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 REPO = os.path.dirname(os.path.dirname(HERE))
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.environ["SUDO_RM_RF_REFERENCE"])
 sys.path.insert(0, REPO)
 warnings.filterwarnings("ignore")
 

@@ -1,10 +1,11 @@
-"""The reference's import paths resolve to the B200-native modules through the overlay WITHOUT hiding
+"""The reference's import paths resolve to the H100-native modules through the overlay WITHOUT hiding
 the rest of the reference package (losses, argument parsers, the other model families), and a
 whole-module pickle written against those paths loads (README.md:75 `torch.load(model.pt)`).
 
 The import block under test is the reference's own: dnn/experiments/run_improved_sudormrf.py:23-29
 and utils/simple_whamr_evaluation.py:40-44 (minus the modules that need comet_ml / glob2 /
-speechbrain, which are not installed in this image)."""
+speechbrain).  The original checkout is stood in for by a stub tree with the same package layout
+(``original_tree``): what is under test is which tree each import resolves to, not the original's code."""
 import os
 import subprocess
 import sys
@@ -12,7 +13,35 @@ import sys
 import pytest
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REFERENCE = "/root/reference"
+
+# module -> source of the stub original tree; the accelerated modules hold markers that must never be imported
+STUB_MODULES = {
+    "sudo_rm_rf/__init__.py": "",
+    "sudo_rm_rf/dnn/__init__.py": "",
+    "sudo_rm_rf/dnn/experiments/__init__.py": "",
+    "sudo_rm_rf/dnn/experiments/utils/__init__.py": "",
+    "sudo_rm_rf/dnn/experiments/utils/improved_cmd_args_parser_v2.py": "def get_args():\n    return {}\n",
+    "sudo_rm_rf/dnn/experiments/utils/mixture_consistency.py": "apply = 'original tree'\n",
+    "sudo_rm_rf/dnn/losses/__init__.py": "",
+    "sudo_rm_rf/dnn/losses/sisdr.py": ("class PermInvariantSISDR:\n"
+                                       "    def __init__(self, **kwargs):\n        self.kwargs = kwargs\n"),
+    "sudo_rm_rf/dnn/losses/snr.py": "",
+    "sudo_rm_rf/dnn/models/__init__.py": "",
+    "sudo_rm_rf/dnn/models/improved_sudormrf.py": "SuDORMRF = 'original tree'\n",
+    "sudo_rm_rf/dnn/models/sudormrf.py": "SuDORMRF = 'original tree'\n",
+    "sudo_rm_rf/dnn/models/groupcomm_sudormrf_v2.py": "GroupCommSudoRmRf = 'original tree'\n",
+    "sudo_rm_rf/dnn/models/causal_improved_sudormrf_v3.py": "CausalSuDORMRF = 'original tree'\n",
+}
+
+
+@pytest.fixture(scope="module")
+def original_tree(tmp_path_factory):
+    root = tmp_path_factory.mktemp("original")
+    for rel, src in STUB_MODULES.items():
+        path = root / rel
+        path.parent.mkdir(parents=True, exist_ok=True)
+        path.write_text(src)
+    return str(root)
 
 PICKLE = r"""
 import io, sys, torch
@@ -79,26 +108,23 @@ def test_overlay_import_paths_and_pickle():
     assert "overlay ok" in _run(PICKLE.format(repo=REPO))
 
 
-@pytest.mark.skipif(not os.path.isdir(REFERENCE), reason="reference checkout not present (GPU box)")
-def test_overlay_keeps_rest_of_reference_importable():
+def test_overlay_keeps_rest_of_reference_importable(original_tree):
     setup = (f"sys.path.insert(0, {REPO!r}); sys.path.insert(0, {REPO!r} + '/sudo_rm_rf_b200/dropin')\n"
-             f"sys.path.append({REFERENCE!r})")
-    assert "runner imports ok" in _run(RUNNER_IMPORTS.format(setup=setup, reference=REFERENCE))
+             f"sys.path.append({original_tree!r})")
+    assert "runner imports ok" in _run(RUNNER_IMPORTS.format(setup=setup, reference=original_tree))
 
 
-@pytest.mark.skipif(not os.path.isdir(REFERENCE), reason="reference checkout not present (GPU box)")
-def test_meta_path_redirect_with_reference_first():
+def test_meta_path_redirect_with_reference_first(original_tree):
     """`sudo_rm_rf_b200.dropin.install()`: reference FIRST on sys.path, only the accelerated names are redirected."""
-    setup = (f"sys.path.insert(0, {REPO!r}); sys.path.insert(0, {REFERENCE!r})\n"
+    setup = (f"sys.path.insert(0, {REPO!r}); sys.path.insert(0, {original_tree!r})\n"
              "import sudo_rm_rf_b200.dropin as D; D.install()")
-    assert "runner imports ok" in _run(RUNNER_IMPORTS.format(setup=setup, reference=REFERENCE))
+    assert "runner imports ok" in _run(RUNNER_IMPORTS.format(setup=setup, reference=original_tree))
 
 
-@pytest.mark.skipif(not os.path.isdir(REFERENCE), reason="reference checkout not present (GPU box)")
-def test_overlay_without_reference_modules_fails_normally():
+def test_overlay_without_reference_modules_fails_normally(original_tree):
     """A module neither the overlay nor the reference has is a plain ModuleNotFoundError."""
     script = (f"import sys; sys.path.insert(0, {REPO!r}); sys.path.insert(0, {REPO!r} + '/sudo_rm_rf_b200/dropin')\n"
-              f"sys.path.append({REFERENCE!r})\n"
+              f"sys.path.append({original_tree!r})\n"
               "try:\n    import sudo_rm_rf.dnn.models.no_such_model\n"
               "except ModuleNotFoundError:\n    print('fine')\n")
     assert "fine" in _run(script)

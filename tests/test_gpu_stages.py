@@ -301,12 +301,13 @@ def test_encoder(B, A, T, N_, K, D):
     enc = torch.full((B, N_, L), float("nan"), device=DEV)
     st = torch.zeros(B, 2, dtype=torch.float64, device=DEV)
     N.check(N.lib().sdr_encoder(p(wav), p(w), p(enc), p(st), B, A, T, N_, K, L, stream()))
-    xp = torch.zeros(B, A, Tp, device=DEV)
+    # fp64 reference: an fp32 cuDNN convolution may run in TF32 (~1e-3 relative), far above the kernel's error
+    xp = torch.zeros(B, A, Tp, device=DEV, dtype=torch.float64)
     xp[..., :T] = wav
-    want = F.conv1d(xp, w, None, stride=hop, padding=hop)
+    want = F.conv1d(xp, w.double(), None, stride=hop, padding=hop)
     assert want.shape[-1] == L
     close(enc, want)
-    check_stats(st, want)
+    check_stats(st, want.float())
 
 
 @pytest.mark.parametrize("B,A,T,N_,K,D", [
@@ -314,7 +315,7 @@ def test_encoder(B, A, T, N_, K, D):
     (2, 2, 333, 160, 11, 3), (1, 1, 7, 70, 21, 1), (1, 1, 3000, 64, 91, 4), (40, 1, 6400, 256, 21, 5),
 ])
 def test_encoder_tensor_core(B, A, T, N_, K, D):
-    """Encoder on the tcgen05 kernel (window operand, bf16x3)."""
+    """Encoder on the wgmma kernel (window operand, bf16x3)."""
     lib = N.lib()
     g = torch.Generator().manual_seed(3)
     cfg = O.Config(enc_kernel_size=K, upsampling_depth=D)
@@ -400,19 +401,19 @@ def test_mixture_consistency(kind):
 
 @pytest.mark.parametrize("samples,M,K,L,mode", [
     (2, 256, 512, 3200, "norm"),          # bottleneck (cfg 2)
-    (3, 512, 256, 640, "plain_stats"),    # proj_1x1: two 256-wide n-tiles
+    (3, 512, 256, 640, "plain_stats"),    # proj_1x1: four 128-wide n-tiles
     (2, 256, 512, 1280, "res"),           # res_conv + in-place skip
     (2, 1024, 256, 384, "mask"),          # mask_net
     (2, 128, 64, 200, "res"),             # single k-block, 128-wide tile, ragged last position tile
     (1, 384, 192, 100, "plain_stats"),    # tile_n = 128 x 3, 3 k-blocks, L < 128
     (5, 256, 128, 132, "norm"),           # positions spill into a 2nd, ragged tile
-    (40, 512, 512, 384, "plain_stats"),   # > 148 tiles: persistent CTAs loop, both TMEM stages reused
+    (40, 512, 512, 384, "plain_stats"),   # > 132 tiles: persistent CTAs loop over several tiles
     (3, 42, 1024, 200, "plain"),          # decoder GEMM: 42 rows zero-padded to one 128-wide tile
     (2, 300, 128, 332, "res"),            # 300 rows -> padded to 384 = 3 tiles of 128, last one partial
-    (2, 160, 64, 64, "plain_stats"),      # padded to 256: one 256-wide tile with 96 padding columns
-    (2, 256, 512, 640, "res_out"),        # skip connection written out of place (register epilogue)
+    (2, 160, 64, 64, "plain_stats"),      # padded to 256: two 128-wide tiles, 96 padding columns
+    (2, 256, 512, 640, "res_out"),        # skip connection written out of place
     (2, 300, 128, 332, "res_out"),
-    (3, 256, 256, 36, "res"),             # L < 128 and not a multiple of 32: clipped bulk rows
+    (3, 256, 256, 36, "res"),             # L < 128 and not a multiple of 32
     (3, 512, 128, 200, "mask"),           # ragged last position tile: zero-filled gate boxes
     (20, 512, 64, 1280, "mask"),          # many tiles per CTA: the gate ring wraps across tile boundaries
     # per-channel PReLU slopes in the operand transform (the original model, sudormrf.py:33,71)
@@ -423,7 +424,7 @@ def test_mixture_consistency(kind):
     (1, 256, 64, 100, "pc_stats"),        # a single k-block
 ])
 def test_pointwise_tensor_core(samples, M, K, L, mode):
-    """tcgen05 path (bf16x3 split, fp32 accumulate) against an fp64 reference."""
+    """wgmma path (bf16x3 split, fp32 accumulate) against an fp64 reference."""
     lib = N.lib()
     g = torch.Generator().manual_seed(7)
     x = (torch.randn(samples, K, L, generator=g) + 0.5).to(DEV)
@@ -449,7 +450,7 @@ def test_pointwise_tensor_core(samples, M, K, L, mode):
         fx = ref_norm(x.double(), gamma.double(), beta.double(), slope.double())
         residual = torch.randn(samples, M, L, generator=g).to(DEV)
         if mode == "res":
-            y = residual.clone()              # in place: y is its own residual (L2 reduce-add exit)
+            y = residual.clone()              # in place: y is its own residual
     elif mode == "mask":
         nin = norm_in(None, None, None, slope, 1.0)
         fx = O.prelu1(x.double(), slope.double())
