@@ -159,6 +159,18 @@ int sdr_encoder_mma_pack(const float* weight, int N, int A, int K, void* packed,
 int sdr_encoder_mma(const float* wav, const void* packed_w, float* enc, double* stats,
                     int B, int A, int64_t T, int N, int K, int L, sdr_stream stream);
 
+/* Both encoders with every mode the model forwards use:
+ *   enc[b,n,p] = act(sum_{a,j} w[n,a,j] * wav[b,a, hop*p + j - pad] + bias[n]), zero outside [0, T),
+ * hop = K/2; pad = hop (improved / groupcomm / original models), 2*hop (the causal model's encoder,
+ * causal_improved_sudormrf_v3.py:194); bias NULL = none; relu != 0: act = ReLU (the original model,
+ * sudormrf.py:212-218,269), else identity; stats NULL = no statistics, else (sum, sumsq) of the final output.
+ * sdr_encoder_mma_ex takes the image of sdr_encoder_mma_pack in place of the weight.                     */
+int sdr_encoder_ex(const float* wav, const float* weight, const float* bias_or_null, int relu, int pad,
+                   float* enc, double* stats_or_null, int B, int A, int64_t T, int N, int K, int L, sdr_stream stream);
+int sdr_encoder_mma_ex(const float* wav, const void* packed_w, const float* bias_or_null, int relu, int pad,
+                       float* enc, double* stats_or_null, int B, int A, int64_t T, int N, int K, int L,
+                       sdr_stream stream);
+
 /* 1x1 Conv1d as a GEMM: y[b,m,l] = sum_k W[m,k] f(x[b,k,l]) + bias[m]
  * (+ residual[b,m,l]); f = deferred norm/PReLU.  epilogue 0: plain,
  * 1: relu(y) * gate[b, m % gate_channels, l] (mask path, improved_sudormrf.py:296-298).
@@ -221,6 +233,20 @@ int sdr_merge(const float* const* z, const sdr_norm_in* fins, int depth,
  * tensors before TAC_norm, state_dict order.                                 */
 int sdr_tac(const float* x, const float* const* params, float* o, double* stats_out,
             int B, int G, int n, int L, sdr_stream stream);
+
+/* TAC's residual + norm (groupcomm_sudormrf_v2.py:381-383): out = x + GlobLN(o) per sample, with
+ * x, o, out [samples,n,L] (samples = B*G) and norm = the statistics of sdr_tac + TAC_norm's gamma / beta.   */
+int sdr_tac_apply(const float* x, const float* o, const sdr_norm_in* norm, float* out, int samples, int n, int L,
+                  sdr_stream stream);
+
+/* GroupComm proj_1x1 with TAC's residual + norm fused into its operand load:
+ *   xt_out = x + GlobLN(pre_add),  y = W xt_out + bias (+ (sum, sumsq) of y into stats_out unless NULL)
+ * x, pre_add, xt_out [samples,Kc,L]; y [samples,M,L]; pre_norm as for sdr_tac_apply.  SDR_ERR_UNSUPPORTED
+ * when the small-channel kernels cannot take the shape (L % 4, unaligned pointers, Kc > 64 or M > 64): the
+ * forward then runs sdr_tac_apply and sdr_pointwise.                                                        */
+int sdr_pointwise_preadd(const float* x, const float* pre_add, const sdr_norm_in* pre_norm, float* xt_out,
+                         const float* W, const float* bias, float* y, double* stats_out,
+                         int samples, int M, int Kc, int L, sdr_stream stream);
 
 /* ConvTranspose1d overlap-add + crop (+ uniform mixture consistency):
  * frames [B, SA*K, L] -> out [B, SA, T] (improved_sudormrf.py:272-279,300-301). */

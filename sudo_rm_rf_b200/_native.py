@@ -67,6 +67,10 @@ _SIGNATURES = {
     "sdr_encoder_mma_pack": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "sdr_encoder_mma": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                   C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "sdr_encoder_ex": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                 C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "sdr_encoder_mma_ex": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p, C.c_void_p,
+                                     C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "sdr_pointwise": (C.c_int, [C.c_void_p, C.POINTER(SdrNormIn), C.c_void_p, C.c_void_p,
                                 C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                 C.c_int, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
@@ -90,6 +94,11 @@ _SIGNATURES = {
                             C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "sdr_tac": (C.c_int, [C.c_void_p, C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_int,
                           C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "sdr_tac_apply": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(SdrNormIn), C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                C.c_void_p]),
+    "sdr_pointwise_preadd": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(SdrNormIn), C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
+                                       C.c_void_p]),
     "sdr_residual_norm": (C.c_int, [C.c_void_p, C.POINTER(SdrNormIn), C.c_void_p, C.POINTER(SdrNormIn), C.c_void_p,
                                     C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "sdr_softmax_gate": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),

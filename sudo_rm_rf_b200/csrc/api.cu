@@ -846,6 +846,22 @@ int sdr_encoder_mma(const float* wav, const void* packed_w, float* enc, double* 
     return launch_encoder_mma(wav, packed_w, nullptr, 0, enc, stats, B, A, T, N, K, L, K / 2, static_cast<cudaStream_t>(stream));
 }
 
+int sdr_encoder_ex(const float* wav, const float* weight, const float* bias_or_null, int relu, int pad, float* enc,
+                   double* stats_or_null, int B, int A, int64_t T, int N, int K, int L, sdr_stream stream) {
+    if (!wav || !weight || !enc || pad < 0) return SDR_ERR_BAD_ARGUMENT;
+    if (K % 2 == 0) return SDR_ERR_BAD_CONFIG;
+    return launch_encoder(wav, weight, bias_or_null, relu, enc, stats_or_null, B, A, T, N, K, L, pad,
+                          static_cast<cudaStream_t>(stream));
+}
+
+int sdr_encoder_mma_ex(const float* wav, const void* packed_w, const float* bias_or_null, int relu, int pad, float* enc,
+                       double* stats_or_null, int B, int A, int64_t T, int N, int K, int L, sdr_stream stream) {
+    if (pad < 0) return SDR_ERR_BAD_ARGUMENT;
+    if (K % 2 == 0) return SDR_ERR_BAD_CONFIG;
+    return launch_encoder_mma(wav, packed_w, bias_or_null, relu, enc, stats_or_null, B, A, T, N, K, L, pad,
+                              static_cast<cudaStream_t>(stream));
+}
+
 int sdr_pointwise(const float* x, const sdr_norm_in* fin, const float* W, const float* bias,
                   const float* residual, const float* gate, int gate_channels, float* y,
                   double* stats_out, int samples, int M, int Kc, int L, int epilogue, sdr_stream stream) {
@@ -922,6 +938,21 @@ int sdr_tac(const float* x, const float* const* params, float* o, double* stats_
             int B, int G, int n, int L, sdr_stream stream) {
     if (!x || !params || !o || !stats_out) return SDR_ERR_BAD_ARGUMENT;
     return launch_tac(x, params, o, stats_out, B, G, n, L, static_cast<cudaStream_t>(stream));
+}
+
+int sdr_tac_apply(const float* x, const float* o, const sdr_norm_in* norm, float* out, int samples, int n, int L,
+                  sdr_stream stream) {
+    if (!x || !o || !norm || !norm->stats || !norm->gamma || !norm->beta || !out) return SDR_ERR_BAD_ARGUMENT;
+    if (samples <= 0 || n <= 0 || L <= 0) return SDR_ERR_BAD_ARGUMENT;
+    return launch_tac_apply(x, o, make_norm(norm), out, samples, n, L, static_cast<cudaStream_t>(stream));
+}
+
+int sdr_pointwise_preadd(const float* x, const float* pre_add, const sdr_norm_in* pre_norm, float* xt_out,
+                         const float* W, const float* bias, float* y, double* stats_out,
+                         int samples, int M, int Kc, int L, sdr_stream stream) {
+    if (!pre_norm) return SDR_ERR_BAD_ARGUMENT;
+    return launch_pointwise_small_preadd(x, pre_add, make_norm(pre_norm), xt_out, W, bias, y, stats_out,
+                                         samples, M, Kc, L, static_cast<cudaStream_t>(stream));
 }
 
 int sdr_overlap_add(const float* frames, const float* mix_or_null, float* out, int B, int SA, int K,

@@ -414,8 +414,8 @@ def test_mixture_consistency(kind):
     (2, 256, 512, 640, "res_out"),        # skip connection written out of place
     (2, 300, 128, 332, "res_out"),
     (3, 256, 256, 36, "res"),             # L < 128 and not a multiple of 32
-    (3, 512, 128, 200, "mask"),           # ragged last position tile: zero-filled gate boxes
-    (20, 512, 64, 1280, "mask"),          # many tiles per CTA: the gate ring wraps across tile boundaries
+    (3, 512, 128, 200, "mask"),           # ragged last position tile: the epilogue's gate reads stop at L
+    (20, 512, 64, 1280, "mask"),          # many tiles per CTA, each reading its gate rows straight from global memory
     # per-channel PReLU slopes in the operand transform (the original model, sudormrf.py:33,71)
     (2, 512, 128, 3200, "pc_stats"),      # its proj_1x1 (Co = 128 -> Ci = 512)
     (2, 128, 512, 3200, "pc_stats"),      # its conv_1x1_exp
@@ -483,7 +483,8 @@ def test_pointwise_tensor_core(samples, M, K, L, mode):
 
 
 def test_pointwise_tensor_core_refuses_unaligned_length():
-    """float4 activation loads need L % 4 == 0; the forward uses the FFMA kernel for such lengths."""
+    """The activations' TMA tensor map needs a 16 B row stride, i.e. L % 4 == 0; the forward uses the FFMA kernel for
+    other lengths."""
     lib = N.lib()
     x = torch.zeros(1, 64, 130, device=DEV)
     W = torch.zeros(128, 64, device=DEV)
