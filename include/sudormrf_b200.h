@@ -105,10 +105,13 @@ int sdr_forward(const sdr_config* cfg, const void* packed,
                 int apply_mixture_consistency,
                 void* workspace, size_t workspace_bytes, sdr_stream stream);
 
-/* Number of kernels one sdr_forward enqueues (the benchmark's gpu_launches claim): for T = 32000 samples, and for
- * any length (the depthwise levels run as one pass or level by level depending on the padded length).          */
+/* Number of kernels one sdr_forward of B mixtures of T samples enqueues (the benchmark's gpu_launches claim).  The
+ * depthwise levels of a block run as one pass or level by level depending on the padded length and, through the
+ * pyramid's per-sample table, on the number of GlobLN samples (B, or B * group_size for GroupComm).
+ * sdr_forward_launch_count is the count for B = 1, T = 32000; sdr_forward_launch_count_at for B = 1 at any T.  */
 int sdr_forward_launch_count(const sdr_config* cfg);
 int sdr_forward_launch_count_at(const sdr_config* cfg, int64_t T);
+int sdr_forward_launch_count_for(const sdr_config* cfg, int B, int64_t T);
 
 /* Same call with HOST buffers (pinned for real asynchrony): H2D copy of the
  * mixture, forward, D2H copy of the estimates, all on `stream`.  `dev_io` is a
@@ -203,7 +206,8 @@ int sdr_depthwise(const float* x, const sdr_norm_in* fin, const float* w5, const
  * chains RAW stride-2 convolutions without waiting for any statistics: z[0] receives level 0's output, z[d]
  * (d >= 1) the raw chain R_d [samples,C,L>>d]; a second small kernel reproduces every level's GlobLN from row
  * statistics and leaves the coefficients of the merge in `scratch` (sdr_pyramid_scratch_bytes; 0 = shape not
- * eligible: D < 4, L % 16, L >> (D-1) < 6, or rows too long for shared memory -> use sdr_depthwise / sdr_merge).
+ * eligible: D < 4, L % 16, L >> (D-1) < 6, rows too long for shared memory, or more than 4096 samples -> use
+ * sdr_depthwise / sdr_merge; both pyramid entries then return SDR_ERR_UNSUPPORTED).
  * w5[d] [C][5], bias[d] [C]: level d's depthwise conv; gamma[d] / beta[d] [C]: spp_dw[d].norm.
  * stats0: zeroed (sum, sumsq) slot per sample for level 0's output.
  * sdr_merge_pyramid then writes m[c,t] = sum_d GLN_d(z_d)[c, t>>d] (+ its statistics), reading z and scratch. */

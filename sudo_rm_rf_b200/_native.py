@@ -55,6 +55,7 @@ _SIGNATURES = {
                               C.c_int64, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
     "sdr_forward_launch_count": (C.c_int, [C.POINTER(SdrConfig)]),
     "sdr_forward_launch_count_at": (C.c_int, [C.POINTER(SdrConfig), C.c_int64]),
+    "sdr_forward_launch_count_for": (C.c_int, [C.POINTER(SdrConfig), C.c_int, C.c_int64]),
     "sdr_host_staging_bytes": (C.c_size_t, [C.POINTER(SdrConfig), C.c_int, C.c_int64]),
     "sdr_forward_host": (C.c_int, [C.POINTER(SdrConfig), C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_int, C.c_int64, C.c_int, C.c_void_p, C.c_size_t,

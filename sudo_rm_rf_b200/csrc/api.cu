@@ -14,7 +14,7 @@ namespace sdr {
 int launch_depthwise(const float*, const NormIn&, const float*, const float*, float*, double*, int, int, int, int, cudaStream_t);
 int launch_merge(const float* const*, const NormIn*, int, float*, double*, int, int, int, cudaStream_t);
 // depthwise pyramid in one pass (pyramid.cu)
-bool pyramid_eligible(int D, int C, int L);
+bool pyramid_eligible(int D, int samples, int C, int L);
 size_t pyramid_rowstats_bytes(int samples, int C, int D);
 size_t pyramid_table_bytes(int samples, int C, int D);
 int launch_pyramid(const float*, const NormIn&, const float* const*, const float* const*, const float* const*,
@@ -346,7 +346,7 @@ static Plan make_plan(const Layout& l, int B, long long T) {
     p.o_o = l.gc ? seg(BL * l.Co) : ((l.orig && l.rs_w) ? seg(BL * l.N) : 0);   // orig: reshape_before_masks output
     p.o_y = seg(BL * l.Ci);
     for (int d = 0; d < kMaxDepthApi; ++d) p.o_z[d] = (d < l.D && !(l.causal && d > 0)) ? seg((BL * l.Ci) >> d) : 0;
-    p.pyramid = !l.causal && pyramid_eligible(l.D, l.cib, p.L);
+    p.pyramid = !l.causal && pyramid_eligible(l.D, p.samples, l.cib, p.L);
     p.o_rowstats = p.pyramid ? seg(pyramid_rowstats_bytes(p.samples, l.cib, l.D)) : 0;
     p.o_table = p.pyramid ? seg(pyramid_table_bytes(p.samples, l.cib, l.D)) : 0;
     p.o_masked = seg(BL * l.S * l.A * l.N);
@@ -765,31 +765,31 @@ int sdr_forward(const sdr_config* cfg, const void* packed, const float* mixture,
                         static_cast<cudaStream_t>(stream));
 }
 
-static int launch_count(const Layout& l, long long T) {
+static int launch_count(const Layout& l, int B, long long T) {
     // encoder + bottleneck + U * (proj + levels + merge + res [+ tac (+ tac_apply unless it is folded into proj)])
-    // + mask + decoder GEMM + overlap-add; levels = pyramid + solve when the one-pass path takes the shape, else D launches
+    // + mask + decoder GEMM + overlap-add; levels = pyramid + solve when the plan takes the one-pass path, else D launches
     if (l.causal) return 2 + 3 * l.U + 3;      // encoder, bottleneck, U x (proj, depthwise pyramid, res), mask, decoder, overlap-add
-    if (l.orig) {                              // encoder, l1, U x (proj, levels, merge, exp, residual-norm), [reshape], mask GEMM, softmax-gate, decoder, overlap-add
-        const int Lo = (int)(padded_len(l, T) / l.hop);
-        const int lev = pyramid_eligible(l.D, l.Ci, Lo) ? 2 : l.D;
-        return 2 + l.U * (lev + 4) + (l.rs_w ? 1 : 0) + 4;
-    }
+    const int levels = make_plan(l, B, T).pyramid ? 2 : l.D;
+    if (l.orig)                                // encoder, l1, U x (proj, levels, merge, exp, residual-norm), [reshape], mask GEMM, softmax-gate, decoder, overlap-add
+        return 2 + l.U * (levels + 4) + (l.rs_w ? 1 : 0) + 4;
     const bool folded = l.gc && l.U > 0 && !l.ub[0].proj_pk && l.cob <= 64 && l.cib <= 64 && l.D >= 2;   // L % 4 == 0 then
-    const int L = (int)(padded_len(l, T) / l.hop);
-    const int levels = pyramid_eligible(l.D, l.cib, L) ? 2 : l.D;
     return 2 + l.U * (levels + 3 + (l.gc ? (folded ? 1 : 2) : 0)) + 3;
 }
 
 int sdr_forward_launch_count(const sdr_config* cfg) {          // at the reference's 4 s @ 8 kHz length
     const Layout l = make_layout(cfg);
     if (!l.ok) return SDR_ERR_BAD_CONFIG;
-    return launch_count(l, 32000);
+    return launch_count(l, 1, 32000);
 }
 
 int sdr_forward_launch_count_at(const sdr_config* cfg, int64_t T) {
+    return sdr_forward_launch_count_for(cfg, 1, T);
+}
+
+int sdr_forward_launch_count_for(const sdr_config* cfg, int B, int64_t T) {
     const Layout l = make_layout(cfg);
-    if (!l.ok || T <= 0) return SDR_ERR_BAD_CONFIG;
-    return launch_count(l, T);
+    if (!l.ok || B <= 0 || T <= 0) return SDR_ERR_BAD_CONFIG;
+    return launch_count(l, B, T);
 }
 
 size_t sdr_host_staging_bytes(const sdr_config* cfg, int B, int64_t T) {
@@ -897,7 +897,7 @@ static size_t pyr_table_offset(int samples, int C, int D) {
 }
 
 size_t sdr_pyramid_scratch_bytes(int samples, int C, int D, int L) {
-    if (samples <= 0 || !pyramid_eligible(D, C, L)) return 0;
+    if (samples <= 0 || !pyramid_eligible(D, samples, C, L)) return 0;
     return pyr_table_offset(samples, C, D) + pyramid_table_bytes(samples, C, D);
 }
 
@@ -905,7 +905,7 @@ int sdr_depthwise_pyramid(const float* y, const sdr_norm_in* fin, const float* c
                           const float* const* gamma, const float* const* beta, float* const* z, double* stats0,
                           void* scratch, int D, int samples, int C, int L, sdr_stream stream) {
     if (!y || !w5 || !bias || !gamma || !beta || !z || !stats0 || !scratch) return SDR_ERR_BAD_ARGUMENT;
-    if (!pyramid_eligible(D, C, L)) return SDR_ERR_UNSUPPORTED;
+    if (!pyramid_eligible(D, samples, C, L)) return SDR_ERR_UNSUPPORTED;
     char* sc = static_cast<char*>(scratch);
     return launch_pyramid(y, make_norm(fin), w5, bias, gamma, beta, z, stats0, reinterpret_cast<double*>(sc),
                           reinterpret_cast<float*>(sc + pyr_table_offset(samples, C, D)), D, samples, C, L,
@@ -915,7 +915,7 @@ int sdr_depthwise_pyramid(const float* y, const sdr_norm_in* fin, const float* c
 int sdr_merge_pyramid(const float* const* z, const void* scratch, int D, float* m, double* stats_out,
                       int samples, int C, int L, sdr_stream stream) {
     if (!z || !scratch || !m || !stats_out) return SDR_ERR_BAD_ARGUMENT;
-    if (!pyramid_eligible(D, C, L)) return SDR_ERR_UNSUPPORTED;
+    if (!pyramid_eligible(D, samples, C, L)) return SDR_ERR_UNSUPPORTED;
     const char* sc = static_cast<const char*>(scratch);
     return launch_merge_pyramid(z, reinterpret_cast<const float*>(sc + pyr_table_offset(samples, C, D)), D, m, stats_out,
                                 samples, C, L, static_cast<cudaStream_t>(stream));

@@ -629,8 +629,11 @@ static int pyramid_windows(int D, int L) {                     // warps per row
     const int step = D == 4 ? PyrGeom<4>::kStep : (D == 5 ? PyrGeom<5>::kStep : PyrGeom<6>::kStep);
     return (L + step - 1) / step;
 }
-bool pyramid_eligible(int D, int C, int L) {
+// The one predicate for "the one-pass pyramid takes this block": the forward's plan (scratch and launch count), the
+// scratch size of the stage entry and both launchers all ask it, so they cannot disagree about a shape.
+bool pyramid_eligible(int D, int samples, int C, int L) {
     if (D < 4 || D > 6 || C <= 0 || C > kSolveKC * kSolveThreads) return false;   // levels 0..3 by lane chunks, 4 per lane, 5 per lane pair
+    if (samples > kPyrMaxSamples) return false;                // per-sample (mean, rstd) of y in shared memory
     if (L % 16 != 0 || (L % (1 << (D - 1))) != 0) return false;
     if ((L >> (D - 1)) < 6) return false;                      // the edge bookkeeping assumes 2 + 1 distinct edge positions
     return pyramid_windows(D, L) <= 32;                        // one CTA (<= 1024 threads) per row
@@ -642,7 +645,7 @@ size_t pyramid_table_bytes(int samples, int C, int D) { return (size_t)samples *
 int launch_pyramid(const float* y, const NormIn& nin, const float* const* w5, const float* const* bias,
                    const float* const* gamma, const float* const* beta, float* const* z, double* stats0,
                    double* rowstats, float* table, int D, int samples, int C, int L, cudaStream_t st) {
-    if (!pyramid_eligible(D, C, L)) return SDR_ERR_UNSUPPORTED;
+    if (!pyramid_eligible(D, samples, C, L)) return SDR_ERR_UNSUPPORTED;
     if (!y || !stats0 || !rowstats || !table || samples <= 0) return SDR_ERR_BAD_ARGUMENT;
     uintptr_t al = reinterpret_cast<uintptr_t>(y);
     for (int d = 0; d < D; ++d) {
@@ -664,7 +667,6 @@ int launch_pyramid(const float* y, const NormIn& nin, const float* const* w5, co
         s.gamma[d] = gamma[d]; s.beta[d] = beta[d]; s.w[d] = w5[d]; s.bias[d] = bias[d];
     }
     const int threads = 32 * pyramid_windows(D, L);
-    if (samples > kPyrMaxSamples) return SDR_ERR_UNSUPPORTED;
     const size_t smem = (2 * (size_t)(L + 8)) * sizeof(float) + (size_t)samples * sizeof(float2);
     int dev = 0, sms = 0;
     if (cudaGetDevice(&dev) != cudaSuccess ||
@@ -702,7 +704,7 @@ int launch_pyramid(const float* y, const NormIn& nin, const float* const* w5, co
 
 int launch_merge_pyramid(const float* const* z, const float* table, int D, float* m, double* stats_out,
                          int samples, int C, int L, cudaStream_t st) {
-    if (!pyramid_eligible(D, C, L)) return SDR_ERR_UNSUPPORTED;
+    if (!pyramid_eligible(D, samples, C, L)) return SDR_ERR_UNSUPPORTED;
     MergePyrArgs a;
     memset(&a, 0, sizeof(a));
     a.table = table; a.D = D; a.C = C; a.L = L;
