@@ -77,24 +77,39 @@ __device__ __forceinline__ float warp_sum(float v) {
     return v;
 }
 
-// Block-wide (sum, sumsq) -> one fp64 atomic pair per CTA on stats[2*sample].
-// All threads of the block must call it.  `red` is >= 2*32 floats of shared memory.
-__device__ __forceinline__ void block_stats_atomic(float s, float q, double* stats, int sample,
-                                                   float* red) {
-    s = warp_sum(s);
-    q = warp_sum(q);
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+    return v;
+}
+
+// Per-thread (sum, sumsq) of a producer's output.  The squares of a sample offset by r standard deviations are about
+// r^2 times its variance, and the variance is what survives sumsq/n - mean^2, so a long fp32 chain loses it: values are
+// summed in fp32 over a short run (at most 16 outputs, add_run) and the runs in fp64.
+struct StatAcc {
+    double s = 0.0, q = 0.0;
+    __device__ __forceinline__ void add(float v) { s += (double)v; q = fma((double)v, (double)v, q); }
+    __device__ __forceinline__ void add_run(float rs, float rq) { s += (double)rs; q += (double)rq; }
+    template <int N> __device__ __forceinline__ void add_run(const float (&o)[N]) {
+        float rs = 0.f, rq = 0.f;
+#pragma unroll
+        for (int i = 0; i < N; ++i) { rs += o[i]; rq = fmaf(o[i], o[i], rq); }
+        add_run(rs, rq);
+    }
+};
+
+// Block-wide (sum, sumsq) -> one fp64 atomic pair per CTA on stats[2*sample], reduced in fp64 from the thread up.
+// All threads of the block must call it.  `red` is >= 2*32 doubles of shared memory.
+__device__ __forceinline__ void block_stats_atomic(const StatAcc& acc, double* stats, int sample, double* red) {
+    const double s = warp_sum_f64(acc.s);
+    const double q = warp_sum_f64(acc.q);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int nwarps = (blockDim.x + 31) >> 5;
     if (lane == 0) { red[warp] = s; red[32 + warp] = q; }
     __syncthreads();
     if (warp == 0) {
-        double ds = (lane < nwarps) ? (double)red[lane] : 0.0;
-        double dq = (lane < nwarps) ? (double)red[32 + lane] : 0.0;
-#pragma unroll
-        for (int o = 16; o > 0; o >>= 1) {
-            ds += __shfl_xor_sync(0xffffffffu, ds, o);
-            dq += __shfl_xor_sync(0xffffffffu, dq, o);
-        }
+        const double ds = warp_sum_f64((lane < nwarps) ? red[lane] : 0.0);
+        const double dq = warp_sum_f64((lane < nwarps) ? red[32 + lane] : 0.0);
         if (lane == 0) {
             atomicAdd(stats + 2 * (size_t)sample, ds);
             atomicAdd(stats + 2 * (size_t)sample + 1, dq);

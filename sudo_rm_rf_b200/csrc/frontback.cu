@@ -29,7 +29,7 @@ encoder_kernel(const float* __restrict__ wav, const float* __restrict__ weight, 
                float* __restrict__ enc, double* __restrict__ stats,
                int A, long long T, int N, int K, int L, int t_tiles, int pad, int relu) {
     extern __shared__ __align__(16) float smem[];
-    __shared__ float s_red[64];
+    __shared__ double s_red[64];
     const int hop = K / 2;
     const int span = hop * (kEncThreads - 1) + K;        // samples needed by 128 positions
     float* s_x = smem;                                     // [A][span]
@@ -53,7 +53,7 @@ encoder_kernel(const float* __restrict__ wav, const float* __restrict__ weight, 
     __syncthreads();
 
     const int t = t0 + tid;
-    float st_s = 0.f, st_q = 0.f;
+    StatAcc acc;
     const int AK = A * K;
     for (int nn = 0; nn < kEncNB; nn += 4) {
         float a0 = 0.f, a1 = 0.f, a2 = 0.f, a3 = 0.f;
@@ -70,6 +70,7 @@ encoder_kernel(const float* __restrict__ wav, const float* __restrict__ weight, 
         (void)AK;
         if (t < L) {
             float o[4] = {a0, a1, a2, a3};
+            float rs = 0.f, rq = 0.f;
 #pragma unroll
             for (int e = 0; e < 4; ++e) {
                 const int n = n0 + nn + e;
@@ -77,12 +78,13 @@ encoder_kernel(const float* __restrict__ wav, const float* __restrict__ weight, 
                     if (bias) o[e] += __ldg(bias + n);
                     if (relu) o[e] = fmaxf(o[e], 0.f);
                     enc[((size_t)b * N + n) * L + t] = o[e];
-                    st_s += o[e]; st_q = fmaf(o[e], o[e], st_q);
+                    rs += o[e]; rq = fmaf(o[e], o[e], rq);
                 }
             }
+            acc.add_run(rs, rq);
         }
     }
-    if (stats) block_stats_atomic(st_s, st_q, stats, b, s_red);
+    if (stats) block_stats_atomic(acc, stats, b, s_red);
 }
 
 int launch_encoder(const float* wav, const float* weight, const float* bias, int relu, float* enc, double* stats,

@@ -24,7 +24,7 @@ dw5_vec_kernel(const float* __restrict__ x, NormIn nin,
                float* __restrict__ y, double* __restrict__ stats_out,
                int C, int Lin, int Lout, int chunks_per_sample) {
     __shared__ SampleNorm s_norm;
-    __shared__ float s_red[64];
+    __shared__ double s_red[64];
     const int sample = blockIdx.x / chunks_per_sample;
     const int chunk = blockIdx.x - sample * chunks_per_sample;
     if (threadIdx.x == 0) s_norm = sample_norm(nin, sample);
@@ -36,7 +36,7 @@ dw5_vec_kernel(const float* __restrict__ x, NormIn nin,
     const float* xs = x + (size_t)sample * C * Lin;
     float* ys = y + (size_t)sample * C * Lout;
 
-    float acc_s = 0.f, acc_q = 0.f;
+    StatAcc acc;
 #pragma unroll
     for (int it = 0; it < kDwItems; ++it) {
         const int item = (chunk * kDwItems + it) * kDwThreads + threadIdx.x;
@@ -94,11 +94,10 @@ dw5_vec_kernel(const float* __restrict__ x, NormIn nin,
                 }
             }
             *reinterpret_cast<float4*>(ys + (size_t)c * Lout + 4 * q) = make_float4(o[0], o[1], o[2], o[3]);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) { acc_s += o[i]; acc_q = fmaf(o[i], o[i], acc_q); }
+            acc.add_run(o);
         }
     }
-    block_stats_atomic(acc_s, acc_q, stats_out, sample, s_red);
+    block_stats_atomic(acc, stats_out, sample, s_red);
 }
 
 // scalar fallback (any Lin/Lout): one output element per thread-iteration
@@ -108,7 +107,7 @@ dw5_scalar_kernel(const float* __restrict__ x, NormIn nin,
                   float* __restrict__ y, double* __restrict__ stats_out,
                   int C, int Lin, int Lout, int stride, int chunks_per_sample) {
     __shared__ SampleNorm s_norm;
-    __shared__ float s_red[64];
+    __shared__ double s_red[64];
     const int sample = blockIdx.x / chunks_per_sample;
     const int chunk = blockIdx.x - sample * chunks_per_sample;
     if (threadIdx.x == 0) s_norm = sample_norm(nin, sample);
@@ -117,7 +116,7 @@ dw5_scalar_kernel(const float* __restrict__ x, NormIn nin,
     const int items = C * Lout;
     const float* xs = x + (size_t)sample * C * Lin;
     float* ys = y + (size_t)sample * C * Lout;
-    float acc_s = 0.f, acc_q = 0.f;
+    StatAcc acc;
     for (int it = 0; it < 4; ++it) {
         const int item = (chunk * 4 + it) * kDwThreads + threadIdx.x;
         if (item < items) {
@@ -132,10 +131,10 @@ dw5_scalar_kernel(const float* __restrict__ x, NormIn nin,
                     a = fmaf(__ldg(w5 + c * 5 + j), apply_norm(cn, __ldg(xs + (size_t)c * Lin + p)), a);
             }
             ys[(size_t)c * Lout + t] = a;
-            acc_s += a; acc_q = fmaf(a, a, acc_q);
+            acc.add(a);
         }
     }
-    block_stats_atomic(acc_s, acc_q, stats_out, sample, s_red);
+    block_stats_atomic(acc, stats_out, sample, s_red);
 }
 
 // ---------------------------------------------------------------------------
@@ -157,7 +156,7 @@ __global__ void __launch_bounds__(kMgThreads)
 merge_vec_kernel(MergeArgs a, float* __restrict__ m, double* __restrict__ stats_out,
                  int C, int L, int chunks_per_sample) {
     __shared__ SampleNorm s_norm[kMaxDepth];
-    __shared__ float s_red[64];
+    __shared__ double s_red[64];
     const int sample = blockIdx.x / chunks_per_sample;
     const int chunk = blockIdx.x - sample * chunks_per_sample;
     if (threadIdx.x < a.depth) s_norm[threadIdx.x] = sample_norm(a.n[threadIdx.x], sample);
@@ -165,7 +164,7 @@ merge_vec_kernel(MergeArgs a, float* __restrict__ m, double* __restrict__ stats_
 
     const int QR = L >> 2;
     const int items = C * QR;
-    float acc_s = 0.f, acc_q = 0.f;
+    StatAcc acc;
 #pragma unroll
     for (int it = 0; it < kMgItems; ++it) {
         const int item = (chunk * kMgItems + it) * kMgThreads + threadIdx.x;
@@ -192,24 +191,23 @@ merge_vec_kernel(MergeArgs a, float* __restrict__ m, double* __restrict__ stats_
                 o[0] += v; o[1] += v; o[2] += v; o[3] += v;
             }
             *reinterpret_cast<float4*>(m + row * L + 4 * q) = make_float4(o[0], o[1], o[2], o[3]);
-#pragma unroll
-            for (int i = 0; i < 4; ++i) { acc_s += o[i]; acc_q = fmaf(o[i], o[i], acc_q); }
+            acc.add_run(o);
         }
     }
-    block_stats_atomic(acc_s, acc_q, stats_out, sample, s_red);
+    block_stats_atomic(acc, stats_out, sample, s_red);
 }
 
 __global__ void __launch_bounds__(kMgThreads)
 merge_scalar_kernel(MergeArgs a, float* __restrict__ m, double* __restrict__ stats_out,
                     int C, int L, int chunks_per_sample) {
     __shared__ SampleNorm s_norm[kMaxDepth];
-    __shared__ float s_red[64];
+    __shared__ double s_red[64];
     const int sample = blockIdx.x / chunks_per_sample;
     const int chunk = blockIdx.x - sample * chunks_per_sample;
     if (threadIdx.x < a.depth) s_norm[threadIdx.x] = sample_norm(a.n[threadIdx.x], sample);
     __syncthreads();
     const int items = C * L;
-    float acc_s = 0.f, acc_q = 0.f;
+    StatAcc acc;
     for (int it = 0; it < 4; ++it) {
         const int item = (chunk * 4 + it) * kMgThreads + threadIdx.x;
         if (item < items) {
@@ -222,10 +220,10 @@ merge_scalar_kernel(MergeArgs a, float* __restrict__ m, double* __restrict__ sta
                 o += apply_norm(cn, __ldg(a.z[d] + row * (L >> d) + (t >> d)));
             }
             m[row * L + t] = o;
-            acc_s += o; acc_q = fmaf(o, o, acc_q);
+            acc.add(o);
         }
     }
-    block_stats_atomic(acc_s, acc_q, stats_out, sample, s_red);
+    block_stats_atomic(acc, stats_out, sample, s_red);
 }
 
 
@@ -298,7 +296,7 @@ dw5_wide_kernel(const float* __restrict__ x, NormIn nin,
                 float* __restrict__ y, double* __restrict__ stats_out,
                 int C, int Lin, int Lout, int chunks_per_sample) {
     __shared__ SampleNorm s_norm;
-    __shared__ float s_red[64];
+    __shared__ double s_red[64];
     const int sample = blockIdx.x / chunks_per_sample;
     const int chunk = blockIdx.x - sample * chunks_per_sample;
     if (threadIdx.x == 0) s_norm = sample_norm(nin, sample);
@@ -311,7 +309,7 @@ dw5_wide_kernel(const float* __restrict__ x, NormIn nin,
     const int items = C * QR;                 // per sample
     const float* xs = x + (size_t)sample * C * Lin;
     float* ys = y + (size_t)sample * C * Lout;
-    float acc_s = 0.f, acc_q = 0.f;
+    StatAcc acc;
 #pragma unroll
     for (int it = 0; it < kDw8Items; ++it) {
         const int item = (chunk * kDw8Items + it) * kDw8Threads + threadIdx.x;
@@ -374,11 +372,10 @@ dw5_wide_kernel(const float* __restrict__ x, NormIn nin,
             float* yr = ys + (size_t)c * Lout + 8 * q;
             st_stream4(yr, make_float4(o[0], o[1], o[2], o[3]));
             st_stream4(yr + 4, make_float4(o[4], o[5], o[6], o[7]));
-#pragma unroll
-            for (int i = 0; i < 8; ++i) { acc_s += o[i]; acc_q = fmaf(o[i], o[i], acc_q); }
+            acc.add_run(o);
         }
     }
-    block_stats_atomic(acc_s, acc_q, stats_out, sample, s_red);
+    block_stats_atomic(acc, stats_out, sample, s_red);
 }
 
 
@@ -390,14 +387,14 @@ __global__ void __launch_bounds__(kMg16Threads)
 merge_wide_kernel(MergeArgs a, float* __restrict__ m, double* __restrict__ stats_out,
                   int C, int L, int chunks_per_sample) {
     __shared__ SampleNorm s_norm[kMaxDepth];
-    __shared__ float s_red[64];
+    __shared__ double s_red[64];
     const int sample = blockIdx.x / chunks_per_sample;
     const int chunk = blockIdx.x - sample * chunks_per_sample;
     if (threadIdx.x < a.depth) s_norm[threadIdx.x] = sample_norm(a.n[threadIdx.x], sample);
     __syncthreads();
     const int QR = L >> 4;
     const int items = C * QR;
-    float acc_s = 0.f, acc_q = 0.f;
+    StatAcc acc;
 #pragma unroll
     for (int iti = 0; iti < kMg16Items; ++iti) {
       const int item = (chunk * kMg16Items + iti) * kMg16Threads + threadIdx.x;
@@ -438,11 +435,10 @@ merge_wide_kernel(MergeArgs a, float* __restrict__ m, double* __restrict__ stats
 #pragma unroll
         for (int i = 0; i < 4; ++i)
             st_stream4(mr + 4 * i, make_float4(o[4 * i], o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]));
-#pragma unroll
-        for (int i = 0; i < 16; ++i) { acc_s += o[i]; acc_q = fmaf(o[i], o[i], acc_q); }
+        acc.add_run(o);
       }
     }
-    block_stats_atomic(acc_s, acc_q, stats_out, sample, s_red);
+    block_stats_atomic(acc, stats_out, sample, s_red);
 }
 
 

@@ -27,7 +27,7 @@ __global__ void __launch_bounds__(kRnThreads)
 residual_norm_kernel(const float* __restrict__ e, NormIn fe, float* x, NormIn fx, double* __restrict__ stats_out,
                      int C, int L, int chunks_per_sample) {
     __shared__ SampleNorm s_n[2];
-    __shared__ float s_red[64];
+    __shared__ double s_red[64];
     const int sample = blockIdx.x / chunks_per_sample;
     const int chunk = blockIdx.x - sample * chunks_per_sample;
     if (threadIdx.x == 0) { s_n[0] = sample_norm(fe, sample); s_n[1] = sample_norm(fx, sample); }
@@ -35,7 +35,7 @@ residual_norm_kernel(const float* __restrict__ e, NormIn fe, float* x, NormIn fx
     const SampleNorm ne = s_n[0], nx = s_n[1];
     const size_t base = (size_t)sample * C * L;
     const int items = VEC ? (C * L) >> 2 : C * L;
-    float st_s = 0.f, st_q = 0.f;
+    StatAcc acc;
 #pragma unroll
     for (int it = 0; it < kRnItems; ++it) {
         const int item = (chunk * kRnItems + it) * kRnThreads + threadIdx.x;
@@ -52,19 +52,17 @@ residual_norm_kernel(const float* __restrict__ e, NormIn fe, float* x, NormIn fx
                 o.z = apply_norm(ce, v.z) + apply_norm(cx, r.z);
                 o.w = apply_norm(ce, v.w) + apply_norm(cx, r.w);
                 *reinterpret_cast<float4*>(x + base + idx) = o;
-                st_s += (o.x + o.y) + (o.z + o.w);
-                st_q = fmaf(o.x, o.x, st_q); st_q = fmaf(o.y, o.y, st_q);
-                st_q = fmaf(o.z, o.z, st_q); st_q = fmaf(o.w, o.w, st_q);
+                acc.add_run((o.x + o.y) + (o.z + o.w), fmaf(o.x, o.x, fmaf(o.y, o.y, fmaf(o.z, o.z, o.w * o.w))));
             } else {
                 const int c = item / L;
                 const ChanNorm ce = chan_norm(fe, ne, c), cx = chan_norm(fx, nx, c);
                 const float o = apply_norm(ce, __ldg(e + base + item)) + apply_norm(cx, x[base + item]);
                 x[base + item] = o;
-                st_s += o; st_q = fmaf(o, o, st_q);
+                acc.add(o);
             }
         }
     }
-    block_stats_atomic(st_s, st_q, stats_out, sample, s_red);
+    block_stats_atomic(acc, stats_out, sample, s_red);
 }
 
 int launch_residual_norm(const float* e, const NormIn& fe, float* x, const NormIn& fx, double* stats_out,

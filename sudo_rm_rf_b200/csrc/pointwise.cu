@@ -48,7 +48,7 @@ pw_gemm_kernel(const PwArgs a) {
     __shared__ __align__(16) float As[2][kBK][AS];
     __shared__ __align__(16) float Bs[2][kBK][kBN];
     __shared__ SampleNorm s_norm;
-    __shared__ float s_red[64];
+    __shared__ double s_red[64];
 
     const int tid = threadIdx.x;
     const int sample = blockIdx.x / a.l_tiles;
@@ -148,7 +148,7 @@ pw_gemm_kernel(const PwArgs a) {
     }
 
     // ---- epilogue: bias, residual, gate, store, statistics ----
-    float st_s = 0.f, st_q = 0.f;
+    StatAcc st;
 #pragma unroll
     for (int i = 0; i < TM; ++i) {
         int mr;
@@ -178,8 +178,7 @@ pw_gemm_kernel(const PwArgs a) {
                         o[2] = fmaxf(o[2], 0.f) * g.z; o[3] = fmaxf(o[3], 0.f) * g.w;
                     }
                     *reinterpret_cast<float4*>(a.y + row + l) = make_float4(o[0], o[1], o[2], o[3]);
-#pragma unroll
-                    for (int e = 0; e < 4; ++e) { st_s += o[e]; st_q = fmaf(o[e], o[e], st_q); }
+                    st.add_run(o);
                 }
             } else {
 #pragma unroll
@@ -189,13 +188,13 @@ pw_gemm_kernel(const PwArgs a) {
                         if (a.residual) v += a.residual[row + l + e];
                         if (a.epilogue == 1) v = fmaxf(v, 0.f) * __ldg(grow + l + e);
                         a.y[row + l + e] = v;
-                        st_s += v; st_q = fmaf(v, v, st_q);
+                        st.add(v);
                     }
                 }
             }
         }
     }
-    if (a.stats_out) block_stats_atomic(st_s, st_q, a.stats_out, sample, s_red);
+    if (a.stats_out) block_stats_atomic(st, a.stats_out, sample, s_red);
 }
 
 
@@ -226,7 +225,7 @@ pw_small_kernel(const PwArgs a, int chunks_per_sample) {
     __shared__ float2 sAB[kSmMaxK];                         // folded norm: y = x*a + b
     __shared__ float2 sPre[kSmMaxK];                        // folded norm of the pre-add operand
     __shared__ float sBias[kSmMT];
-    __shared__ float s_red[64];
+    __shared__ double s_red[64];
     const int tid = threadIdx.x, nthr = blockDim.x;
     const int sample = blockIdx.x / chunks_per_sample;
     const int chunk = blockIdx.x - sample * chunks_per_sample;
@@ -258,7 +257,7 @@ pw_small_kernel(const PwArgs a, int chunks_per_sample) {
 
     const int QR = a.L >> 2;
     const int q = chunk * nthr + tid;
-    float st_s = 0.f, st_q = 0.f;
+    StatAcc st;
     if (q < QR) {
         const float* xp = a.x + (size_t)sample * a.K * a.L + 4 * q;
         float acc[kSmMT][4];
@@ -328,12 +327,11 @@ pw_small_kernel(const PwArgs a, int chunks_per_sample) {
                     o[2] = fmaxf(o[2], 0.f) * g.z; o[3] = fmaxf(o[3], 0.f) * g.w;
                 }
                 *reinterpret_cast<float4*>(a.y + idx) = make_float4(o[0], o[1], o[2], o[3]);
-#pragma unroll
-                for (int e = 0; e < 4; ++e) { st_s += o[e]; st_q = fmaf(o[e], o[e], st_q); }
+                st.add_run(o);
             }
         }
     }
-    if (a.stats_out) block_stats_atomic(st_s, st_q, a.stats_out, sample, s_red);
+    if (a.stats_out) block_stats_atomic(st, a.stats_out, sample, s_red);
 }
 
 // ---------------------------------------------------------------------------
@@ -368,7 +366,7 @@ pw_tile_kernel(const PwArgs a, int tiles_per_sample, int P) {
     __shared__ float2 sAB[kStMaxK];                         // folded norm of the operand: y = x*a + b
     __shared__ float2 sPre[kStMaxK];                        // folded norm of the pre-add operand
     __shared__ float sBias[MT];
-    __shared__ float s_red[64];
+    __shared__ double s_red[64];
     __shared__ __align__(8) uint64_t s_bar;
     const int tid = threadIdx.x, nthr = blockDim.x;
     const int sample = blockIdx.x / tiles_per_sample;
@@ -420,7 +418,7 @@ pw_tile_kernel(const PwArgs a, int tiles_per_sample, int P) {
         } while (!done);
     }
     const int t2 = 2 * tid;                                 // this thread's 2 positions inside the tile
-    float st_s = 0.f, st_q = 0.f;
+    StatAcc st;
     if (t2 < np) {
         float acc[MT][2];
 #pragma unroll
@@ -476,6 +474,7 @@ pw_tile_kernel(const PwArgs a, int tiles_per_sample, int P) {
             }
         }
         const bool want_stats = a.stats_out != nullptr;
+        float rs = 0.f, rq = 0.f;                           // fp32 run of at most 8 rows (StatAcc)
         if (a.M == MT && (MT == 16 || !a.residual)) {       // every row real, nothing left to add: pointer-bumped stores
             float* yp = a.y + obase;
 #pragma unroll
@@ -483,8 +482,9 @@ pw_tile_kernel(const PwArgs a, int tiles_per_sample, int P) {
                 *reinterpret_cast<float2*>(yp) = make_float2(acc[m][0], acc[m][1]);
                 yp += a.L;
                 if (want_stats) {
-                    st_s += acc[m][0] + acc[m][1];
-                    st_q = fmaf(acc[m][0], acc[m][0], st_q); st_q = fmaf(acc[m][1], acc[m][1], st_q);
+                    rs += acc[m][0] + acc[m][1];
+                    rq = fmaf(acc[m][0], acc[m][0], rq); rq = fmaf(acc[m][1], acc[m][1], rq);
+                    if ((m & 7) == 7) { st.add_run(rs, rq); rs = rq = 0.f; }
                 }
             }
         } else {
@@ -504,14 +504,16 @@ pw_tile_kernel(const PwArgs a, int tiles_per_sample, int P) {
                 const int m = m8 + j;
                 if (m < a.M) {
                     *reinterpret_cast<float2*>(a.y + obase + (size_t)m * a.L) = make_float2(acc[m][0], acc[m][1]);
-                    st_s += acc[m][0] + acc[m][1];
-                    st_q = fmaf(acc[m][0], acc[m][0], st_q); st_q = fmaf(acc[m][1], acc[m][1], st_q);
+                    rs += acc[m][0] + acc[m][1];
+                    rq = fmaf(acc[m][0], acc[m][0], rq); rq = fmaf(acc[m][1], acc[m][1], rq);
                 }
             }
+            st.add_run(rs, rq);
+            rs = rq = 0.f;
         }
         }
     }
-    if (a.stats_out) block_stats_atomic(st_s, st_q, a.stats_out, sample, s_red);
+    if (a.stats_out) block_stats_atomic(st, a.stats_out, sample, s_red);
 }
 
 // Tile geometry of pw_tile_kernel: threads = the multiple of 32 in [128, 256] that wastes the fewest threads on rows of

@@ -476,7 +476,8 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
             // epilogue: lane owns positions p and p + 8, and channel pairs 8 j + 2 (lane % 4) + {0, 1}
             const int l = tc.l0 + wg * 64 + wr * 16 + (lane >> 2);
             const int ch0 = tc.n0 + 2 * (lane & 3);
-            float st_s = 0.f, st_q = 0.f;
+            StatAcc st;
+            float rs = 0.f, rq = 0.f;
             const size_t gate_row0 = MODE == 2 ? (size_t)tc.sample * a.gate_channels + (tc.n0 % a.gate_channels) - tc.n0 : 0;
 #pragma unroll
             for (int i = 0; i < 64; ++i) {
@@ -489,15 +490,15 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
                     if (MODE == 2) o = fmaxf(o, 0.f) * __ldg(a.gate + (gate_row0 + m) * Ls + p);
                     if constexpr (WINDOW) { if (relu_out) o = fmaxf(o, 0.f); }   // the original model's encoder (sudormrf.py:212-218)
                     a.y[idx] = o;
-                    if (STATS) { st_s += o; st_q = fmaf(o, o, st_q); }
+                    if (STATS) { rs += o; rq = fmaf(o, o, rq); }
                 }
+                if (STATS && (i & 15) == 15) { st.add_run(rs, rq); rs = rq = 0.f; }   // fp32 runs of 16 (StatAcc)
             }
             if (STATS) {
-                st_s = warp_sum(st_s);
-                st_q = warp_sum(st_q);
+                const double ds = warp_sum_f64(st.s), dq = warp_sum_f64(st.q);
                 if (lane == 0) {
-                    atomicAdd(a.stats_out + 2 * (size_t)tc.sample, (double)st_s);
-                    atomicAdd(a.stats_out + 2 * (size_t)tc.sample + 1, (double)st_q);
+                    atomicAdd(a.stats_out + 2 * (size_t)tc.sample, ds);
+                    atomicAdd(a.stats_out + 2 * (size_t)tc.sample + 1, dq);
                 }
             }
         }

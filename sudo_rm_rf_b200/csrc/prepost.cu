@@ -10,12 +10,6 @@
 
 namespace sdr {
 
-__device__ __forceinline__ double warp_sum_f64(double v) {
-#pragma unroll
-    for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-    return v;
-}
-
 // ---------------------------------------------------------------------------
 // utterance moments: sums[row] = (sum_t x, sum_t x^2), fp64
 // grid = rows * chunks, 256 threads; the caller zeroes `sums`.

@@ -554,7 +554,7 @@ constexpr int kMpItems = SDR_MP_ITEMS;
 
 __global__ void __launch_bounds__(kMpThreads)
 merge_pyramid_kernel(const MergePyrArgs a, float* __restrict__ m, double* __restrict__ stats_out, int chunks_per_sample) {
-    __shared__ float s_red[64];
+    __shared__ double s_red[64];
     const int sample = blockIdx.x / chunks_per_sample;
     const int chunk = blockIdx.x - sample * chunks_per_sample;
     const int L = a.L, D = a.D, C = a.C;
@@ -563,7 +563,7 @@ merge_pyramid_kernel(const MergePyrArgs a, float* __restrict__ m, double* __rest
     const int TW = pyr_table_width(D);
     const int left_runs = (2 << (D - 1)) >> 4;            // runs whose positions satisfy t >> d < 2 for some d: t < 2^D
     const int right_runs = ((1 << (D - 1)) + 15) >> 4;    // t >> d == L_d - 1 for some d: t >= L - 2^(D-1)
-    float acc_s = 0.f, acc_q = 0.f;
+    StatAcc acc;
 #pragma unroll
     for (int iti = 0; iti < kMpItems; ++iti) {
         const int item = (chunk * kMpItems + iti) * kMpThreads + threadIdx.x;
@@ -614,11 +614,10 @@ merge_pyramid_kernel(const MergePyrArgs a, float* __restrict__ m, double* __rest
 #pragma unroll
             for (int i = 0; i < 4; ++i)
                 *reinterpret_cast<float4*>(mr + 4 * i) = make_float4(o[4 * i], o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]);
-#pragma unroll
-            for (int i = 0; i < 16; ++i) { acc_s += o[i]; acc_q = fmaf(o[i], o[i], acc_q); }
+            acc.add_run(o);
         }
     }
-    block_stats_atomic(acc_s, acc_q, stats_out, sample, s_red);
+    block_stats_atomic(acc, stats_out, sample, s_red);
 }
 
 // ---------------------------------------------------------------------------

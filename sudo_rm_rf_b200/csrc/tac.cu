@@ -133,11 +133,11 @@ tac_kernel(const float* __restrict__ x, TacParams p, float* __restrict__ o,
             st_s += v; st_q = fmaf(v, v, st_q);
         }
     }
-    st_s = warp_sum(st_s);
-    st_q = warp_sum(st_q);
+    const double ds = warp_sum_f64((double)st_s);
+    const double dq = warp_sum_f64((double)st_q);
     if (lane == 0) {
-        atomicAdd(stats + 2 * ((size_t)b * G + g), (double)st_s);
-        atomicAdd(stats + 2 * ((size_t)b * G + g) + 1, (double)st_q);
+        atomicAdd(stats + 2 * ((size_t)b * G + g), ds);
+        atomicAdd(stats + 2 * ((size_t)b * G + g) + 1, dq);
     }
 }
 
@@ -339,11 +339,11 @@ tac_mma16_kernel(const float* __restrict__ x, TacParams p, float* __restrict__ o
                 if (v0) { orow[0] = od[0]; orow[Ls] = od[1]; st_s += od[0] + od[1]; st_q = fmaf(od[0], od[0], fmaf(od[1], od[1], st_q)); }
                 if (v1) { orow[8] = od[2]; orow[Ls + 8] = od[3]; st_s += od[2] + od[3]; st_q = fmaf(od[2], od[2], fmaf(od[3], od[3], st_q)); }
             }
-            st_s = warp_sum(st_s);
-            st_q = warp_sum(st_q);
+            const double ds = warp_sum_f64((double)st_s);
+            const double dq = warp_sum_f64((double)st_q);
             if (lane == 0) {
-                atomicAdd(stats + 2 * ((size_t)b * G + g), (double)st_s);
-                atomicAdd(stats + 2 * ((size_t)b * G + g) + 1, (double)st_q);
+                atomicAdd(stats + 2 * ((size_t)b * G + g), ds);
+                atomicAdd(stats + 2 * ((size_t)b * G + g) + 1, dq);
             }
         }
     }
