@@ -605,15 +605,19 @@ int launch_pointwise_ffma(const float* x, const NormIn& nin, const float* W, con
     return launch_bm<32>(a, samples, vec, st);
 }
 
+// The one predicate for "the streaming pre-add kernel takes this shape": the forward's plan (whether the GroupComm
+// block folds tac_apply into proj_1x1, and so its launch count) and the launcher both ask it.
+bool preadd_eligible(int M, int K, int L) { return (L % 4) == 0 && K <= kSmMaxK && M <= 64; }
+
 // 1x1 conv of x + GlobLN(pre_add) for the small-channel (GroupComm) blocks; xt_out receives x + GlobLN(pre_add).
-// SDR_ERR_UNSUPPORTED when the streaming kernel cannot take the shape (the caller then materialises xt first).
+// SDR_ERR_UNSUPPORTED when the streaming kernel cannot take the shape or the buffers are not 16-byte aligned.
 int launch_pointwise_small_preadd(const float* x, const float* pre_add, const NormIn& pre_norm, float* xt_out,
                                   const float* W, const float* bias, float* y, double* stats_out,
                                   int samples, int M, int K, int L, cudaStream_t st) {
     if (samples <= 0 || M <= 0 || K <= 0 || L <= 0 || !x || !pre_add || !xt_out || !W || !y) return SDR_ERR_BAD_ARGUMENT;
     const uintptr_t al = reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y) |
                          reinterpret_cast<uintptr_t>(pre_add) | reinterpret_cast<uintptr_t>(xt_out);
-    if ((L % 4) != 0 || (al % 16) != 0 || K > kSmMaxK || M > 64) return SDR_ERR_UNSUPPORTED;
+    if (!preadd_eligible(M, K, L) || (al % 16) != 0) return SDR_ERR_UNSUPPORTED;
     PwArgs a;
     a.x = x; a.nin = NormIn{nullptr, nullptr, nullptr, nullptr, 1.0}; a.W = W; a.bias = bias; a.residual = nullptr;
     a.gate = nullptr; a.gate_channels = 0; a.y = y; a.stats_out = stats_out;

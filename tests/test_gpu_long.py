@@ -12,8 +12,9 @@ keep the long clips cheap).
 - the per-level kernels and their merge at L = 16000 / 32000, the shapes the forward hands them past the pyramid;
 - the causal pyramid over 4 to 8 windows, with a causality check at every inner window boundary;
 - improved / GroupComm / original models on both sides of the 32-window switch, 10 s clips at 16 kHz, GroupComm at
-  257 mixtures (4112 samples) and a corpus whose utterances straddle the switch; for each, the kernels one forward
-  enqueues are counted with torch.profiler and compared with sdr_forward_launch_count_for.
+  257 mixtures (4112 samples) and a corpus whose utterances straddle the switch, GroupComm at upsampling_depth 1 on
+  both sides of the TAC pre-add fold (L % 4); for each, the kernels one forward enqueues are counted with
+  torch.profiler and compared with sdr_forward_launch_count_for.
 """
 import collections
 import ctypes as C
@@ -282,6 +283,8 @@ ORIGINAL = dict(out_channels=128, in_channels=512, num_blocks=2, upsampling_dept
                 enc_num_basis=128, num_sources=2)
 CAUSAL = dict(in_audio_channels=1, out_channels=128, in_channels=512, num_blocks=2, upsampling_depth=4,
               enc_kernel_size=21, enc_num_basis=128, num_sources=2)
+GROUPCOMM_D1 = dict(out_channels=64, in_channels=128, num_blocks=3, upsampling_depth=1, enc_kernel_size=21,
+                    enc_num_basis=128, num_sources=2, group_size=4)
 MODEL_CASES = [   # id, variant, kwargs, T, one-pass pyramid expected (None: the causal block)
     ("improved_L14848_pyramid", "improved", IMPROVED, 148480, True),        # 32 windows
     ("improved_L14880_levels", "improved", IMPROVED, 148481, False),        # 33 windows
@@ -291,6 +294,8 @@ MODEL_CASES = [   # id, variant, kwargs, T, one-pass pyramid expected (None: the
     ("original_L15376_levels", "original", ORIGINAL, 153760, False),        # 33 windows (L % 16 == 0 still)
     ("improved_4src_10s_16k", "improved", dict(IMPROVED, num_sources=4), 160000, False),   # a FUSS clip
     ("causal_10s_16k", "causal", CAUSAL, 160000, None),                     # 4 causal windows per row
+    ("groupcomm_D1_L320_folded", "groupcomm", GROUPCOMM_D1, 3200, False),   # TAC pre-add inside proj_1x1
+    ("groupcomm_D1_L322_apart", "groupcomm", GROUPCOMM_D1, 3210, False),    # L % 4 == 2: tac_apply, then proj_1x1
 ]
 
 
@@ -436,6 +441,14 @@ def test_pyramid_limits_agree():
     # one length past 32 windows at B = 1: the same switch
     assert count(1, 148481) == count(1, 148480) + U * (D - 2)
     assert lib.sdr_forward_launch_count_for(C.byref(cfg), 0, T) < 0
+
+
+def test_tac_fold_follows_the_length():
+    """At upsampling_depth 1 a GroupComm model pads to an even frame count only: its blocks fold tac_apply into
+    proj_1x1 (one launch fewer each) exactly when L % 4 == 0."""
+    cfg = P._engine.make_config(P.GroupCommSudoRmRf(**GROUPCOMM_D1))
+    count = lambda T: N.lib().sdr_forward_launch_count_for(C.byref(cfg), 1, T)
+    assert count(3200) == count(3210) - GROUPCOMM_D1["num_blocks"]      # L = 320 / 322
 
 
 def test_benchmark_launch_claim_holds_at_its_batch():
