@@ -217,6 +217,14 @@ int sdr_depthwise_pyramid(const float* y, const sdr_norm_in* fin, const float* c
                           void* scratch, int D, int samples, int C, int L, sdr_stream stream);
 int sdr_merge_pyramid(const float* const* z, const void* scratch, int D, float* m, double* stats_out,
                       int samples, int C, int L, sdr_stream stream);
+/* The same stage without the levels in HBM (what the forward runs): one pass over y keeps only the row statistics,
+ * the solve fills `scratch`, and a second pass over y rebuilds the raw chain and writes the merge m [samples,C,L]
+ * (+ its statistics in stats_m, a zeroed slot) from registers.  m is bitwise what sdr_depthwise_pyramid +
+ * sdr_merge_pyramid compute.  m may be y itself (the forward merges in place); otherwise it must not overlap y.
+ * Same eligibility and scratch as sdr_depthwise_pyramid. */
+int sdr_depthwise_pyramid_fused(const float* y, const sdr_norm_in* fin, const float* const* w5, const float* const* bias,
+                                const float* const* gamma, const float* const* beta, float* m, double* stats0,
+                                double* stats_m, void* scratch, int D, int samples, int C, int L, sdr_stream stream);
 
 /* The depthwise stage of the causal U-ConvBlock (causal_improved_sudormrf_v3.py:106-116) in one pass: PReLU of
  * proj_1x1 on load (slope_in), D levels of [causally masked 21-tap depthwise conv (stride 1, then 2) + bias + PReLU]

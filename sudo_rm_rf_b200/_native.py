@@ -89,6 +89,10 @@ _SIGNATURES = {
                                         C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "sdr_merge_pyramid": (C.c_int, [C.POINTER(C.c_void_p), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p,
                                     C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "sdr_depthwise_pyramid_fused": (C.c_int, [C.c_void_p, C.POINTER(SdrNormIn), C.POINTER(C.c_void_p),
+                                              C.POINTER(C.c_void_p), C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                              C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                              C.c_int, C.c_void_p]),
     "sdr_causal_pyramid": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
                                      C.POINTER(C.c_void_p), C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "sdr_merge": (C.c_int, [C.POINTER(C.c_void_p), C.POINTER(SdrNormIn), C.c_int, C.c_void_p,

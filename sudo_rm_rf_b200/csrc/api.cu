@@ -20,6 +20,8 @@ size_t pyramid_table_bytes(int samples, int C, int D);
 int launch_pyramid(const float*, const NormIn&, const float* const*, const float* const*, const float* const*,
                    const float* const*, float* const*, double*, double*, float*, int, int, int, int, cudaStream_t);
 int launch_merge_pyramid(const float* const*, const float*, int, float*, double*, int, int, int, cudaStream_t);
+int launch_pyramid_fused(const float*, const NormIn&, const float* const*, const float* const*, const float* const*,
+                         const float* const*, float*, double*, double*, double*, float*, int, int, int, int, cudaStream_t);
 int launch_pointwise_ffma(const float*, const NormIn&, const float*, const float*, const float*, const float*, int,
                           float*, double*, int, int, int, int, int, cudaStream_t);
 int launch_encoder(const float*, const float*, const float*, int, float*, double*, int, int, long long, int, int, int, int, cudaStream_t);
@@ -377,9 +379,9 @@ static int decoder_tail(const Layout& l, const Plan& p, const float* pk, const N
 
 // spp_dw and the merge of block i (improved_sudormrf.py / sudormrf.py UBlock): y holds the raw proj_1x1 output with its
 // statistics in slot 0, read through GlobLN + PReLU (one slope per channel for the original model); the merge m
-// replaces it in y with its statistics in slot D + 1.  Every level from one pass over y when the plan takes the
-// pyramid (raw convolution chain + row statistics, every GlobLN solved afterwards, the merge as an affine
-// combination of the raw tensors), else level by level.
+// replaces it in y with its statistics in slot D + 1.  When the plan takes the pyramid, two passes over y (row
+// statistics of the raw convolution chain, every GlobLN solved from them, then the chain rebuilt and merged as an
+// affine combination of the raw levels), with no level in HBM; else level by level.
 static int depthwise_stage(const Layout& l, const Plan& p, const NormBlockOff& u, int i, int prelu_pc, const float* pk,
                            char* ws, cudaStream_t st) {
     const int L = p.L, D = l.D, ns = p.samples, C = l.cib;
@@ -391,10 +393,8 @@ static int depthwise_stage(const Layout& l, const Plan& p, const NormBlockOff& u
     if (p.pyramid) {
         const float *pw[kMaxDepthApi], *pb[kMaxDepthApi], *pg[kMaxDepthApi], *pbe[kMaxDepthApi];
         for (int d = 0; d < D; ++d) { pw[d] = pk + u.dw_w[d]; pb[d] = pk + u.dw_b[d]; pg[d] = pk + u.dw_g[d]; pbe[d] = pk + u.dw_be[d]; }
-        float* table = p.buf(ws, p.o_table);
-        SDR_TRY(launch_pyramid(y, n0, pw, pb, pg, pbe, z, p.slot(ws, i, 1), reinterpret_cast<double*>(ws + p.o_rowstats),
-                               table, D, ns, C, L, st));
-        return launch_merge_pyramid(zc, table, D, y, p.slot(ws, i, D + 1), ns, C, L, st);
+        return launch_pyramid_fused(y, n0, pw, pb, pg, pbe, y, p.slot(ws, i, 1), p.slot(ws, i, D + 1),
+                                    reinterpret_cast<double*>(ws + p.o_rowstats), p.buf(ws, p.o_table), D, ns, C, L, st);
     }
     SDR_TRY(launch_depthwise(y, n0, pk + u.dw_w[0], pk + u.dw_b[0], z[0], p.slot(ws, i, 1), ns, C, L, 1, st));
     for (int d = 1; d < D; ++d) {
@@ -828,6 +828,17 @@ int sdr_merge_pyramid(const float* const* z, const void* scratch, int D, float* 
     const char* sc = static_cast<const char*>(scratch);
     return launch_merge_pyramid(z, reinterpret_cast<const float*>(sc + pyr_table_offset(samples, C, D)), D, m, stats_out,
                                 samples, C, L, static_cast<cudaStream_t>(stream));
+}
+
+int sdr_depthwise_pyramid_fused(const float* y, const sdr_norm_in* fin, const float* const* w5, const float* const* bias,
+                                const float* const* gamma, const float* const* beta, float* m, double* stats0,
+                                double* stats_m, void* scratch, int D, int samples, int C, int L, sdr_stream stream) {
+    if (!y || !w5 || !bias || !gamma || !beta || !m || !stats0 || !stats_m || !scratch) return SDR_ERR_BAD_ARGUMENT;
+    if (!pyramid_eligible(D, samples, C, L)) return SDR_ERR_UNSUPPORTED;
+    char* sc = static_cast<char*>(scratch);
+    return launch_pyramid_fused(y, make_norm(fin), w5, bias, gamma, beta, m, stats0, stats_m, reinterpret_cast<double*>(sc),
+                                reinterpret_cast<float*>(sc + pyr_table_offset(samples, C, D)), D, samples, C, L,
+                                static_cast<cudaStream_t>(stream));
 }
 
 int sdr_causal_pyramid(const float* y, const float* slope_in, const float* const* w21, const float* const* bias,

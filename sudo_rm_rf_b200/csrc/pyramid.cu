@@ -20,8 +20,12 @@
 // and emits, per (sample, channel), the coefficients of the merge, which is again affine in the raw tensors:
 //     m[t] = sum_d P_d R_d[t >> d] + Q(t),   Q(t) = Q_int + edge corrections at t >> d in {0, 1, L_d - 1}.
 // `merge_pyramid_kernel` evaluates that (and accumulates the statistics of m for final_norm).
-// Traffic per block: y + z_0 + R_d read/written once = 0.62 GB instead of 1.04 GB at the benchmark shape, and
-// 3 launches instead of D + 1.  Shapes outside the fast path (D < 4, rows longer than the shared-memory budget,
+// Written out, z_0 and R_d are 1.94 tensors of y's size (D = 5) that the merge reads straight back.  The forward
+// therefore runs the fused stage instead (`launch_pyramid_fused`): dw_pyramid_kernel<.., kPyrStats> reads y and keeps
+// only the statistics, the solve runs, and dw_pyramid_kernel<.., kPyrMerge> reads y again, rebuilds the same chain
+// with the same instructions and evaluates the merge from the registers that hold a lane's 16 positions of every
+// level.  Traffic per block at the benchmark shape: y twice + m = 0.63 GB instead of y + 2 x levels + m = 1.23 GB,
+// still 3 launches instead of D + 1.  Shapes outside the fast path (D < 4, rows longer than the shared-memory budget,
 // L_d < 6) keep the per-level kernels in levels.cu.
 #include <cstring>
 #include <type_traits>
@@ -46,8 +50,17 @@ struct PyrArgs {
     float* z[kPyrMaxDepth];         // z[0] = z_0 (raw, with bias), z[d] = R_d (raw convolution chain)
     double* stats0;                 // per-sample (sum, sumsq) of z_0
     double* rowstats;               // [samples][D - 1][C][kRowStat]: a (sample, level) block is contiguous for the solve
+    const float* table;             // kPyrMerge: the solve's merge coefficients [rows][pyr_table_width(D)]
+    float* m;                       // kPyrMerge: the merged output [rows][L]; may be y itself
+    double* stats_m;                // kPyrMerge: per-sample (sum, sumsq) of m
     int D, C, L, rows;
 };
+
+// What one pass of dw_pyramid_kernel leaves in HBM.  kPyrLevels: z_0, R_1 .. R_{D-1}, their row statistics and the
+// statistics of z_0 (read by sdr_merge_pyramid).  The fused stage runs two passes over y instead and never writes the
+// levels: kPyrStats keeps only the statistics, the solve turns them into the merge table, and kPyrMerge rebuilds the
+// same pyramid bit for bit and evaluates the merge from the registers that hold it (m and its statistics).
+enum PyrMode : int { kPyrLevels = 0, kPyrStats = 1, kPyrMerge = 2 };
 
 // One CTA per row, one WARP per 512-position window of the row, the whole pyramid of the window in REGISTERS:
 // lane l owns 16 consecutive positions of level 0 (its u, z_0), 8 of R_1, 4 of R_2, 2 of R_3, 1 of R_4 (and, for
@@ -133,16 +146,26 @@ __device__ __forceinline__ void pyr_bulk_g2s(void* dst, const void* src, uint32_
 #ifndef SDR_PYR_MINB
 #define SDR_PYR_MINB 6                  // resident CTAs per SM the <= 256-thread instantiation is compiled for
 #endif
+#ifndef SDR_PYR_STATS_MINB
+#define SDR_PYR_STATS_MINB 5            // the same for kPyrStats (at 6, 40 registers, the per-channel-slope D = 6 one spills)
+#endif
+#ifndef SDR_PYR_MERGE_MINB
+#define SDR_PYR_MERGE_MINB 4            // the same for kPyrMerge, which holds every level of its 16 positions live at once
+#endif                                  // (64 registers; at 5 it spills)
 // PC: one PReLU slope per channel (the original model's nn.PReLU(C), sudormrf.py:33): a row is one channel, so the
 // slope simply travels with the row's other parameters; the shared-slope instantiations are unchanged.
-template <int D, int MAXT, int MINB, bool PC>
+template <int D, int MAXT, int MINB, bool PC, int MODE = kPyrLevels>
 __global__ void __launch_bounds__(MAXT, MINB)
 dw_pyramid_kernel(const PyrArgs a) {
     static_assert(D >= 4 && D <= 6, "register pyramid: levels 0..3 by lane chunks, 4 per lane, 5 per lane pair");
     constexpr int S = PyrGeom<D>::kStep, ML = PyrGeom<D>::kLeft;
+    constexpr bool kMerge = MODE == kPyrMerge;
+    constexpr int NP = 5 * D + 3 + (PC ? 1 : 0);            // per-row parameters ...
+    constexpr int TW = pyr_table_width(D);                  // ... followed, for the merge, by the row's table
     extern __shared__ __align__(16) float pyr_smem[];       // [2][L + 8]: raw rows of y with 4 floats of slack on either side
-    __shared__ float s_par[2][5 * D + 3 + (PC ? 1 : 0)];    // taps of every level, bias_0, gamma_y, beta_y (one row ahead) [, slope]
-    __shared__ float s_part[2][32][2 * D];
+    __shared__ float s_par[2][NP + (kMerge ? TW : 0)];      // taps of every level, bias_0, gamma_y, beta_y (one row ahead) [, slope] [, table]
+    __shared__ float s_part[2][32][kMerge ? 1 : 2 * D];
+    __shared__ double s_mst[2][32][kMerge ? 2 : 1];         // kPyrMerge: per-warp (sum, sumsq) of m
     __shared__ __align__(8) uint64_t s_bar[2];
     const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
     const int L = a.L;
@@ -155,10 +178,11 @@ dw_pyramid_kernel(const PyrArgs a) {
     bool sle1 = slope <= 1.f;
 
     auto stage_params = [&](int row, int slot) {
-        for (int i = tid; i < 5 * D + 3 + (PC ? 1 : 0); i += blockDim.x) {
+        for (int i = tid; i < NP + (kMerge ? TW : 0); i += blockDim.x) {
             const int c = row % a.C;
             const float* src;
-            if (i < 5 * D) src = a.w[i / 5] + c * 5 + (i % 5);
+            if (kMerge && i >= NP) src = a.table + (size_t)row * TW + (i - NP);
+            else if (i < 5 * D) src = a.w[i / 5] + c * 5 + (i % 5);
             else if (i == 5 * D) src = a.bias0 + c;
             else if (i == 5 * D + 1) src = a.nin.stats ? a.nin.gamma + c : a.bias0 + c;
             else if (PC && i == 5 * D + 3) src = act ? a.nin.prelu + c : a.bias0 + c;
@@ -272,11 +296,13 @@ dw_pyramid_kernel(const PyrArgs a) {
 #pragma unroll
             for (int i = 0; i < 16; ++i) z0[i] = 0.f;
         }
-        if (valid) {
-            float* zr = a.z[0] + (size_t)row * L + g0;
+        if (valid && !kMerge) {
+            if constexpr (MODE == kPyrLevels) {
+                float* zr = a.z[0] + (size_t)row * L + g0;
 #pragma unroll
-            for (int k = 0; k < 4; ++k)
-                *reinterpret_cast<float4*>(zr + 4 * k) = make_float4(z0[4 * k], z0[4 * k + 1], z0[4 * k + 2], z0[4 * k + 3]);
+                for (int k = 0; k < 4; ++k)
+                    *reinterpret_cast<float4*>(zr + 4 * k) = make_float4(z0[4 * k], z0[4 * k + 1], z0[4 * k + 2], z0[4 * k + 3]);
+            }
 #pragma unroll
             for (int i = 0; i < 16; ++i) { part[0] += z0[i]; part[1] = fmaf(z0[i], z0[i], part[1]); }
         }
@@ -305,17 +331,19 @@ dw_pyramid_kernel(const PyrArgs a) {
 #pragma unroll
             for (int i = 0; i < N; ++i) cur[i] = 0.f;
         }
-        if (valid) {
-            const int Ld = L >> d;
-            float* rr = a.z[d] + (size_t)row * Ld + (g0 >> d);
-            if constexpr (N >= 4) {
+        if (valid && !kMerge) {
+            if constexpr (MODE == kPyrLevels) {
+                const int Ld = L >> d;
+                float* rr = a.z[d] + (size_t)row * Ld + (g0 >> d);
+                if constexpr (N >= 4) {
 #pragma unroll
-                for (int k = 0; k < N / 4; ++k)
-                    *reinterpret_cast<float4*>(rr + 4 * k) = make_float4(cur[4 * k], cur[4 * k + 1], cur[4 * k + 2], cur[4 * k + 3]);
-            } else if constexpr (N == 2) {
-                *reinterpret_cast<float2*>(rr) = make_float2(cur[0], cur[1]);
-            } else {
-                rr[0] = cur[0];
+                    for (int k = 0; k < N / 4; ++k)
+                        *reinterpret_cast<float4*>(rr + 4 * k) = make_float4(cur[4 * k], cur[4 * k + 1], cur[4 * k + 2], cur[4 * k + 3]);
+                } else if constexpr (N == 2) {
+                    *reinterpret_cast<float2*>(rr) = make_float2(cur[0], cur[1]);
+                } else {
+                    rr[0] = cur[0];
+                }
             }
 #pragma unroll
             for (int i = 0; i < N; ++i) { part[2 * d] += cur[i]; part[2 * d + 1] = fmaf(cur[i], cur[i], part[2 * d + 1]); }
@@ -328,7 +356,7 @@ dw_pyramid_kernel(const PyrArgs a) {
             if (g0 + 16 == L) rs[(d - 1) * rsl + 4] = (double)cur[N - 1];
         }
     };
-    float r1[8], r2[4], r3[2], r4[1];
+    float r1[8], r2[4], r3[2], r4[1], r5 = 0.f;
     level(std::integral_constant<int, 8>{}, z0, r1, 1);
     level(std::integral_constant<int, 4>{}, r1, r2, 2);
     level(std::integral_constant<int, 2>{}, r2, r3, 3);
@@ -343,8 +371,10 @@ dw_pyramid_kernel(const PyrArgs a) {
         acc = fmaf(w[2], r4[0], acc);
         acc = fmaf(w[3], p1, acc);
         acc = fmaf(w[4], p2, acc);
-        if (valid && (lane & 1) == 0) {                     // S and the window origin are multiples of 32: the pair is valid together
-            a.z[5][(size_t)row * (L >> 5) + (g0 >> 5)] = acc;
+        if constexpr (kMerge) {
+            r5 = __shfl_sync(0xffffffffu, acc, lane & ~1);  // the odd lane's 16 outputs read the same entry
+        } else if (valid && (lane & 1) == 0) {              // S and the window origin are multiples of 32: the pair is valid together
+            if constexpr (MODE == kPyrLevels) a.z[5][(size_t)row * (L >> 5) + (g0 >> 5)] = acc;
             part[10] += acc;
             part[11] = fmaf(acc, acc, part[11]);
             if (g0 == 0) rs[4 * rsl + 2] = (double)acc;
@@ -353,15 +383,67 @@ dw_pyramid_kernel(const PyrArgs a) {
         }
     }
 
-    // ---- row sums of every level (s_part alternates between rows: one barrier per row) ----
-    warp_multi_sum<2 * D>(part, lane);
-    {
+    // ---- kPyrMerge: m[t] = sum_d P_d R_d[t >> d] + Q(t) over the lane's 16 positions, in merge_pyramid_kernel's order
+    // (coarse to fine, then the edge corrections), so m is bitwise what the level-writing pair computes ----
+    StatAcc macc;
+    if constexpr (kMerge) {
+        if (valid) {
+            const float* tb = par + NP;
+            const int q = g0 >> 4, QR = L >> 4;
+            const int left_runs = (2 << (D - 1)) >> 4, right_runs = ((1 << (D - 1)) + 15) >> 4;
+            float base = tb[pyr_q_index()];
+            if constexpr (D > 4) base = fmaf(r4[0], tb[pyr_p_index(D, 4)], base);
+            if constexpr (D > 5) base = fmaf(r5, tb[pyr_p_index(D, 5)], base);
+            const float p0 = tb[pyr_p_index(D, 0)], p1 = tb[pyr_p_index(D, 1)];
+            const float p2 = tb[pyr_p_index(D, 2)], p3 = tb[pyr_p_index(D, 3)];
+            float s3[2], s2[4], s1[8], o[16];
+            s3[0] = fmaf(r3[0], p3, base); s3[1] = fmaf(r3[1], p3, base);
+#pragma unroll
+            for (int i = 0; i < 4; ++i) s2[i] = fmaf(r2[i], p2, s3[i >> 1]);
+#pragma unroll
+            for (int i = 0; i < 8; ++i) s1[i] = fmaf(r1[i], p1, s2[i >> 1]);
+#pragma unroll
+            for (int i = 0; i < 16; ++i) o[i] = fmaf(z0[i], p0, s1[i >> 1]);
+            if (q < left_runs || q >= QR - right_runs) {
+#pragma unroll 1
+                for (int d = 1; d < D; ++d) {
+                    const float dq0 = tb[pyr_dq_index(D, d)], dq1 = tb[pyr_dq_index(D, d) + 1], dqr = tb[pyr_dq_index(D, d) + 2];
+                    const int last = (L >> d) - 1;
+#pragma unroll
+                    for (int i = 0; i < 16; ++i) {
+                        const int idx = (16 * q + i) >> d;
+                        o[i] += idx == 0 ? dq0 : (idx == 1 ? dq1 : 0.f);
+                        o[i] += idx == last ? dqr : 0.f;
+                    }
+                }
+            }
+            float* mr = a.m + (size_t)row * L + g0;         // (in place over y: this row is already in shared memory)
+#pragma unroll
+            for (int k = 0; k < 4; ++k)
+                *reinterpret_cast<float4*>(mr + 4 * k) = make_float4(o[4 * k], o[4 * k + 1], o[4 * k + 2], o[4 * k + 3]);
+            macc.add_run(o);
+        }
+    }
+
+    // ---- row sums of every level, or of m (s_part / s_mst alternate between rows: one barrier per row) ----
+    if constexpr (kMerge) {
+        const double ms = warp_sum_f64(macc.s), mq = warp_sum_f64(macc.q);
+        if (lane == 0) { s_mst[cur][warp][0] = ms; s_mst[cur][warp][1] = mq; }
+    } else {
+        warp_multi_sum<2 * D>(part, lane);
         const int own = warp_multi_owner<2 * D>(lane);
         if (own >= 0) s_part[cur][warp][own] = part[0];
     }
     asm volatile("cp.async.wait_all;" ::: "memory");        // the next row's parameters (issued at the top of this row)
     __syncthreads();
-    if (tid < 2 * D) {
+    if constexpr (kMerge) {
+        if (tid < 2) {
+            const int nw = blockDim.x >> 5;
+            double tot = 0.0;
+            for (int wv = 0; wv < nw; ++wv) tot += s_mst[cur][wv][tid];
+            atomicAdd(a.stats_m + 2 * (size_t)sample + tid, tot);
+        }
+    } else if (tid < 2 * D) {
         const int nw = blockDim.x >> 5;
         double tot = 0.0;
         for (int wv = 0; wv < nw; ++wv) tot += (double)s_part[cur][wv][tid];
@@ -640,49 +722,64 @@ bool pyramid_eligible(int D, int samples, int C, int L) {
 size_t pyramid_rowstats_bytes(int samples, int C, int D) { return (size_t)samples * C * (D - 1) * kRowStat * sizeof(double); }
 size_t pyramid_table_bytes(int samples, int C, int D) { return (size_t)samples * C * pyr_table_width(D) * sizeof(float); }
 
-// y [samples][C][L] -> z[0] = z_0, z[d] = R_d, table (merge coefficients).  stats0: zeroed slot for the statistics of z_0.
-int launch_pyramid(const float* y, const NormIn& nin, const float* const* w5, const float* const* bias,
-                   const float* const* gamma, const float* const* beta, float* const* z, double* stats0,
-                   double* rowstats, float* table, int D, int samples, int C, int L, cudaStream_t st) {
+// The arguments of the pyramid pass and of the solve, shared by both launchers.  z: the level outputs (kPyrLevels),
+// or null.
+static int pyramid_args(const float* y, const NormIn& nin, const float* const* w5, const float* const* bias,
+                        const float* const* gamma, const float* const* beta, float* const* z, double* stats0,
+                        double* rowstats, float* table, int D, int samples, int C, int L, PyrArgs& a, SolveArgs& s) {
     if (!pyramid_eligible(D, samples, C, L)) return SDR_ERR_UNSUPPORTED;
     if (!y || !stats0 || !rowstats || !table || samples <= 0) return SDR_ERR_BAD_ARGUMENT;
     uintptr_t al = reinterpret_cast<uintptr_t>(y);
     for (int d = 0; d < D; ++d) {
-        if (!w5[d] || !bias[d] || !gamma[d] || !beta[d] || !z[d]) return SDR_ERR_BAD_ARGUMENT;
-        al |= reinterpret_cast<uintptr_t>(z[d]);
+        if (!w5[d] || !bias[d] || !gamma[d] || !beta[d] || (z && !z[d])) return SDR_ERR_BAD_ARGUMENT;
+        if (z) al |= reinterpret_cast<uintptr_t>(z[d]);
     }
     if (al % 16 != 0) return SDR_ERR_UNSUPPORTED;
     const long long rows = (long long)samples * C;
     if (rows > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-    PyrArgs a;
     memset(&a, 0, sizeof(a));
     a.y = y; a.nin = nin; a.bias0 = bias[0]; a.stats0 = stats0; a.rowstats = rowstats;
     a.D = D; a.C = C; a.L = L; a.rows = (int)rows;
-    SolveArgs s;
     memset(&s, 0, sizeof(s));
     s.stats0 = stats0; s.rowstats = rowstats; s.table = table; s.D = D; s.C = C; s.L = L;
     for (int d = 0; d < D; ++d) {
-        a.w[d] = w5[d]; a.z[d] = z[d];
+        a.w[d] = w5[d]; a.z[d] = z ? z[d] : nullptr;
         s.gamma[d] = gamma[d]; s.beta[d] = beta[d]; s.w[d] = w5[d]; s.bias[d] = bias[d];
     }
-    const int threads = 32 * pyramid_windows(D, L);
-    const size_t smem = (2 * (size_t)(L + 8)) * sizeof(float) + (size_t)samples * sizeof(float2);
+    return SDR_OK;
+}
+
+// One pass of dw_pyramid_kernel on persistent CTAs: exactly as many as are resident at once.
+template <typename K>
+static int launch_pyramid_pass(K kern, const PyrArgs& a, int samples, cudaStream_t st) {
+    const int threads = 32 * pyramid_windows(a.D, a.L);
+    const size_t smem = (2 * (size_t)(a.L + 8)) * sizeof(float) + (size_t)samples * sizeof(float2);
     int dev = 0, sms = 0;
     if (cudaGetDevice(&dev) != cudaSuccess ||
         cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return SDR_ERR_CUDA;
-    auto launch = [&](auto kern) -> int {
-        if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return SDR_ERR_CUDA;
-        int per_sm = 0;                                        // persistent CTAs: exactly what is resident at once
-        if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem) != cudaSuccess || per_sm < 1) {
-            cudaGetLastError();
-            per_sm = 1;
-        }
-        long long grid = (long long)sms * per_sm;
-        if (grid > rows) grid = rows;
-        kern<<<(unsigned)grid, threads, smem, st>>>(a);
-        return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
-    };
-    int rc;
+    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return SDR_ERR_CUDA;
+    int per_sm = 0;
+    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem) != cudaSuccess || per_sm < 1) {
+        cudaGetLastError();
+        per_sm = 1;
+    }
+    long long grid = (long long)sms * per_sm;
+    if (grid > a.rows) grid = a.rows;
+    kern<<<(unsigned)grid, threads, smem, st>>>(a);
+    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+}
+
+// y [samples][C][L] -> z[0] = z_0, z[d] = R_d, table (merge coefficients).  stats0: zeroed slot for the statistics of z_0.
+int launch_pyramid(const float* y, const NormIn& nin, const float* const* w5, const float* const* bias,
+                   const float* const* gamma, const float* const* beta, float* const* z, double* stats0,
+                   double* rowstats, float* table, int D, int samples, int C, int L, cudaStream_t st) {
+    if (!z) return SDR_ERR_BAD_ARGUMENT;
+    PyrArgs a;
+    SolveArgs s;
+    int rc = pyramid_args(y, nin, w5, bias, gamma, beta, z, stats0, rowstats, table, D, samples, C, L, a, s);
+    if (rc != SDR_OK) return rc;
+    const int threads = 32 * pyramid_windows(D, L);
+    auto launch = [&](auto kern) -> int { return launch_pyramid_pass(kern, a, samples, st); };
     if (nin.prelu && nin.prelu_pc) {
         if (threads <= 256)
             rc = D == 4 ? launch(dw_pyramid_kernel<4, 256, SDR_PYR_MINB, true>)
@@ -699,6 +796,47 @@ int launch_pyramid(const float* y, const NormIn& nin, const float* const* w5, co
     if (rc != SDR_OK) return rc;
     pyramid_solve_kernel<<<(unsigned)samples, kSolveThreads, 0, st>>>(s);
     return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+}
+
+// One pass of the fused stage (M = kPyrStats or kPyrMerge), with the instantiation the row length and slope call for.
+template <int M>
+static int launch_fused_pass(const PyrArgs& a, bool pc, int samples, cudaStream_t st) {
+    constexpr int MB = M == kPyrMerge ? SDR_PYR_MERGE_MINB : SDR_PYR_STATS_MINB;
+    const int D = a.D, threads = 32 * pyramid_windows(a.D, a.L);
+    auto launch = [&](auto kern) -> int { return launch_pyramid_pass(kern, a, samples, st); };
+    if (pc) {
+        if (threads <= 256)
+            return D == 4 ? launch(dw_pyramid_kernel<4, 256, MB, true, M>)
+                          : (D == 5 ? launch(dw_pyramid_kernel<5, 256, MB, true, M>) : launch(dw_pyramid_kernel<6, 256, MB, true, M>));
+        return D == 4 ? launch(dw_pyramid_kernel<4, 1024, 1, true, M>)
+                      : (D == 5 ? launch(dw_pyramid_kernel<5, 1024, 1, true, M>) : launch(dw_pyramid_kernel<6, 1024, 1, true, M>));
+    }
+    if (threads <= 256)
+        return D == 4 ? launch(dw_pyramid_kernel<4, 256, MB, false, M>)
+                      : (D == 5 ? launch(dw_pyramid_kernel<5, 256, MB, false, M>) : launch(dw_pyramid_kernel<6, 256, MB, false, M>));
+    return D == 4 ? launch(dw_pyramid_kernel<4, 1024, 1, false, M>)
+                  : (D == 5 ? launch(dw_pyramid_kernel<5, 1024, 1, false, M>) : launch(dw_pyramid_kernel<6, 1024, 1, false, M>));
+}
+
+// The whole depthwise stage without the levels in HBM: statistics pass over y, solve, merge pass over y.
+// y [samples][C][L] -> m [samples][C][L] (m == y or disjoint), stats_m.  stats0 / stats_m: zeroed slots.
+int launch_pyramid_fused(const float* y, const NormIn& nin, const float* const* w5, const float* const* bias,
+                         const float* const* gamma, const float* const* beta, float* m, double* stats0, double* stats_m,
+                         double* rowstats, float* table, int D, int samples, int C, int L, cudaStream_t st) {
+    PyrArgs a;
+    SolveArgs s;
+    int rc = pyramid_args(y, nin, w5, bias, gamma, beta, nullptr, stats0, rowstats, table, D, samples, C, L, a, s);
+    if (rc != SDR_OK) return rc;
+    if (!m || !stats_m) return SDR_ERR_BAD_ARGUMENT;
+    const size_t n = (size_t)samples * C * L;
+    if (m != y && m < y + n && y < m + n) return SDR_ERR_BAD_ARGUMENT;   // a row's m would overwrite rows not yet read
+    if (reinterpret_cast<uintptr_t>(m) % 16 != 0) return SDR_ERR_UNSUPPORTED;
+    const bool pc = nin.prelu && nin.prelu_pc;
+    if ((rc = launch_fused_pass<kPyrStats>(a, pc, samples, st)) != SDR_OK) return rc;
+    pyramid_solve_kernel<<<(unsigned)samples, kSolveThreads, 0, st>>>(s);
+    if (cudaGetLastError() != cudaSuccess) return SDR_ERR_CUDA;
+    a.table = table; a.m = m; a.stats_m = stats_m;
+    return launch_fused_pass<kPyrMerge>(a, pc, samples, st);
 }
 
 int launch_merge_pyramid(const float* const* z, const float* table, int D, float* m, double* stats_out,
