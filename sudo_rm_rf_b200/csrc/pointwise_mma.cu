@@ -15,6 +15,10 @@
 //       positions x 128 channels (64 registers per thread), issue the wgmmas
 //       and run the epilogue.  Persistent CTAs, one per SM; the transform and
 //       TMA warps run ahead into the free stages while the consumers drain.
+//   Epilogue: through a 16 KB shared-memory slot holding one quarter of the tile
+//       (one warpgroup's 64 positions x 64 channels).  The residual / gate quarter
+//       arrives there by TMA, the warpgroup combines it with its accumulators in
+//       place, and one thread stores the quarter to y by TMA.
 // Precision: x*w ~= xh*wh + xl*wh + xh*wl (3 bf16 MMAs, fp32 accumulate): the
 // dropped terms are O(2^-16) relative, i.e. fp32-grade for the 1e-3 parity
 // budget, where a single bf16 (5e-3) or tf32 (7e-4) pass is not (SURVEY §7).
@@ -42,6 +46,11 @@ constexpr int kAHalf = kTileM * 128;   // 16 KB: bf16 [128 rows][64 k]
 constexpr int kBHalf = kTileN * 128;   // 16 KB: bf16 [128 weight rows][64 k]
 constexpr int kAStageBytes = 2 * kAHalf;                     // 32 KB: hi + lo
 constexpr int kBStageBytes = 2 * kBHalf;                     // 32 KB: hi + lo
+// Epilogue slot: fp32 [64 channels][64 positions] as two TMA boxes of [64 channels][32 positions] (128 B rows,
+// SWIZZLE_128B: 16 B chunk index XOR channel % 8, which keeps the accumulator-fragment accesses conflict-free).
+constexpr int kEpiBoxL = 32;
+constexpr int kSlotHalf = 64 * kEpiBoxL * 4;                 // 8 KB
+constexpr int kSlotBytes = 2 * kSlotHalf;                    // 16 KB
 // Warp roles: [0, 8) the two consumer warpgroups (wgmma + epilogue), [8, 16) operand transform, 16 weight TMA,
 // 17 raw activation TMA.
 constexpr int kConsWarps = 8, kProdWarp0 = 8, kProdWarps = 8, kTmaWarp = 16, kRawWarp = 17;
@@ -53,9 +62,7 @@ static_assert(kProdWarps == 8 && kProdElems == 32, "one transform warp per 8-cha
 struct MmaArgs {
     const float* x;
     NormIn nin;
-    const float* bias;
-    const float* residual;
-    const float* gate;
+    const float* bias;    // residual, gate and (outside window mode) y are read and written through tensor maps
     int gate_channels;
     float* y;
     double* stats_out;
@@ -110,6 +117,18 @@ __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* t
 __device__ __forceinline__ void tma_load_3d(void* smem_dst, const CUtensorMap* tm, uint64_t* bar, int c0, int c1, int c2) {
     asm volatile("cp.async.bulk.tensor.3d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5}], [%2];"
                  ::"r"(smem_u32(smem_dst)), "l"(tm), "r"(smem_u32(bar)), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+// shared -> global tensor (TMA) store; out-of-range elements are not written
+__device__ __forceinline__ void tma_store_3d(const CUtensorMap* tm, const void* smem_src, int c0, int c1, int c2) {
+    asm volatile("cp.async.bulk.tensor.3d.global.shared::cta.bulk_group [%0, {%2, %3, %4}], [%1];"
+                 ::"l"(tm), "r"(smem_u32(smem_src)), "r"(c0), "r"(c1), "r"(c2) : "memory");
+}
+__device__ __forceinline__ void bulk_commit() { asm volatile("cp.async.bulk.commit_group;" ::: "memory"); }
+// the committed stores have finished reading shared memory / have completed
+__device__ __forceinline__ void bulk_wait_read_all() { asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory"); }
+__device__ __forceinline__ void bulk_wait_all() { asm volatile("cp.async.bulk.wait_group 0;" ::: "memory"); }
+__device__ __forceinline__ void named_bar_sync(uint32_t id, uint32_t threads) {
+    asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
 }
 
 // wgmma shared-memory matrix descriptor (cute/arch/mma_sm90_desc.hpp documents the bit layout): start address >> 4
@@ -205,31 +224,39 @@ __device__ __forceinline__ TileCoord decode_tile(const MmaArgs& a, int tile) {
 //   WINDOW: encoder mode (strided waveform windows as the A operand)
 //   ACT:    PReLU in the operand transform: 0 none, 1 one shared slope (nn.PReLU()), 2 one slope per input
 //           channel (nn.PReLU(C) of the original model, sudormrf.py:33,71; shared -> shared transform loop only)
-//   MODE:   epilogue 0 = bias only, 1 = + residual (may alias y: every element is read by the thread that writes it),
-//           2 = ReLU * gate
+//   MODE:   epilogue 0 = bias only, 1 = + residual (may alias y: a tile's residual is loaded before its output is
+//           stored), 2 = ReLU * gate
 //   STATS:  accumulate (sum, sumsq) of the output
 template <bool WINDOW, int ACT, int MODE, bool STATS>
 __global__ void __launch_bounds__(kMmaThreads, 1)
 pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      // wmap: packed weights as [rows][128 B]
-              const __grid_constant__ CUtensorMap xmap) {                     // xmap: activations [samples][K][L], box [64][128]
-    // 2 x (32 KB A stage + 32 KB B stage) + 2 x 32 KB raw tiles + 4 KB of tables + barriers (of the 227 KB an sm_90
-    // CTA can own).  SWIZZLE_128B needs the stage bases 1024 B aligned; the launch reserves 1 KB to align by hand.
+              const __grid_constant__ CUtensorMap xmap,                       // xmap: activations [samples][K][L], box [64][128]
+              const __grid_constant__ CUtensorMap emap,                       // emap: residual (MODE 1) or gate (MODE 2)
+              const __grid_constant__ CUtensorMap ymap) {                     // ymap: output (not in window mode)
+    // 2 x (32 KB A stage + 32 KB B stage) + 2 x 32 KB raw tiles + 16 KB epilogue slot + 4 KB of tables + barriers (of
+    // the 227 KB an sm_90 CTA can own).  SWIZZLE_128B needs the stage and slot bases 1024 B aligned; the launch
+    // reserves 1 KB to align by hand.
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
     uint8_t* a_base = smem;                                                  // kStages x 32 KB
     uint8_t* b_base = smem + kStages * kAStageBytes;                         // kStages x 32 KB
     uint8_t* r_base = b_base + kStages * kBStageBytes;                       // kRawStages x 32 KB
+    uint8_t* slot = r_base + kRawStages * kRawStageBytes;                    // 16 KB
     // warp-private tables (no CTA-level barrier in the steady state): per transform warp the (scale, shift) of its
     // channels, double-buffered
-    float2* s_ab = reinterpret_cast<float2*>(r_base + kRawStages * kRawStageBytes);   // [kProdWarps][64]
+    float2* s_ab = reinterpret_cast<float2*>(slot + kSlotBytes);             // [kProdWarps][64]
     uint64_t* bars = reinterpret_cast<uint64_t*>(s_ab + kProdWarps * 64);
     //   full_bar:   the 8 transform warps + the weight TMA thread (with the weights' tx bytes); waited on by the consumers
     //   empty_bar:  the 8 consumer warps once their wgmmas reading the stage have retired
     //   rfull_bar:  raw tile landed (TMA tx bytes); rempty_bar: all 8 transform warps hold it in registers
+    //   slot_bar:   per consumer warpgroup: the slot is its own (the previous quarter's store has read it) and, in
+    //               MODE 1 / 2, holds the quarter's residual / gate (TMA tx bytes).  One barrier per warpgroup: a
+    //               shared one could complete twice while a warpgroup waits, and a parity wait cannot tell.
     uint64_t* full_bar = bars;                       // [kStages]
     uint64_t* empty_bar = full_bar + kStages;        // [kStages]
     uint64_t* rfull_bar = empty_bar + kStages;       // [kRawStages]
     uint64_t* rempty_bar = rfull_bar + kRawStages;   // [kRawStages]
+    uint64_t* slot_bar = rempty_bar + kRawStages;    // [2]
 
     const int tid = threadIdx.x;
     const int warp = tid >> 5, lane = tid & 31;
@@ -240,6 +267,8 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
     if (warp == kTmaWarp && lane == 0) {
         for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], kProdWarps + 1); mbar_init(&empty_bar[s], kConsWarps); }
         for (int s = 0; s < kRawStages; ++s) { mbar_init(&rfull_bar[s], 1); mbar_init(&rempty_bar[s], kProdWarps); }
+        mbar_init(&slot_bar[0], 1);
+        mbar_init(&slot_bar[1], 1);
         fence_barrier_init();
     }
     __syncthreads();
@@ -435,11 +464,30 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
         }
         __syncwarp();
     } else if (warp < kConsWarps) {
-        // ===================== consumers: wgmma main loop + epilogue from registers =====================
+        // ===================== consumers: wgmma main loop + epilogue through the slot =====================
         const int wg = warp >> 2;                  // position block [64 wg, 64 wg + 64) of the tile
         const int wr = warp & 3;                   // 16-row slice of the warpgroup's block
-        const size_t Ls = (size_t)a.L;
+        const bool issuer = (tid & 127) == 0;      // the warpgroup's thread that issues its slot's TMA traffic
         const bool relu_out = WINDOW && a.epilogue == 2;       // window mode only: ReLU on the way out
+        // The slot passes through the tile's quarters in the order (wg 0, half 0), (wg 1, half 0), (wg 0, half 1),
+        // (wg 1, half 1), then to the next tile.  Whoever has drained a quarter hands the slot to the next one:
+        // loads its residual / gate (MODE 1 / 2) or just arrives (MODE 0).  The first quarter of a tile thus loads
+        // while the tile's main loop runs.
+        auto fill_slot = [&](int tile, int qwg, int qh) {
+            uint64_t* bar = &slot_bar[qwg];
+            if constexpr (MODE == 0) {
+                mbar_arrive(bar);
+            } else {
+                const TileCoord q = decode_tile(a, tile);
+                const int c0 = q.l0 + 64 * qwg;
+                const int c1 = (MODE == 1 ? q.n0 : q.n0 % a.gate_channels) + 64 * qh;
+                mbar_arrive_expect_tx(bar, kSlotBytes);
+                tma_load_3d(slot, &emap, bar, c0, c1, q.sample);
+                tma_load_3d(slot + kSlotHalf, &emap, bar, c0 + kEpiBoxL, c1, q.sample);
+            }
+        };
+        if (tid == 0) fill_slot(tile0, 0, 0);
+        uint32_t slot_phase = 0;
         int stage = 0;
         uint32_t phase = 0;
         float acc[64];
@@ -473,26 +521,77 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
                 if (lane == 0) mbar_arrive(&empty_bar[stage]);   // this warp's reads of the stage have retired
                 if (++stage == kStages) { stage = 0; phase ^= 1; }
             }
-            // epilogue: lane owns positions p and p + 8, and channel pairs 8 j + 2 (lane % 4) + {0, 1}
-            const int l = tc.l0 + wg * 64 + wr * 16 + (lane >> 2);
-            const int ch0 = tc.n0 + 2 * (lane & 3);
+            // epilogue, one channel half h (accumulators [32 h, 32 h + 32)) at a time: lane owns positions pp and
+            // pp + 8 of its warp's 32-position box, and channel pairs 8 j + 2 (lane % 4) + {0, 1} of the half
+            // Accumulator u of the half sits at channel row c = 8 (u / 4) + 2 (lane % 4) + u % 2 of the box and
+            // position pp = 16 (wr % 2) + lane / 4 + 8 ((u / 2) % 2); its swizzled byte offset is
+            // 128 c + 16 ((pp / 4) ^ (c % 8)) + 4 (pp % 4) = eoff[u % 4] + 1024 (u / 4).
+            uint8_t* const box = slot + (wr >> 1) * kSlotHalf;
+            uint32_t eoff[4];
+#pragma unroll
+            for (int v = 0; v < 4; ++v) {
+                const uint32_t c = 2 * (lane & 3) + (v & 1), pp = 16 * (wr & 1) + (lane >> 2) + 8 * (v >> 1);
+                eoff[v] = c * 128 + (((pp >> 2) ^ c) << 4) + (pp & 3) * 4;
+            }
+            const int prem = a.L - (tc.l0 + wg * 64 + 32 * (wr >> 1) + 16 * (wr & 1) + (lane >> 2));   // positions left
             StatAcc st;
             float rs = 0.f, rq = 0.f;
-            const size_t gate_row0 = MODE == 2 ? (size_t)tc.sample * a.gate_channels + (tc.n0 % a.gate_channels) - tc.n0 : 0;
 #pragma unroll
-            for (int i = 0; i < 64; ++i) {
-                const int m = ch0 + 8 * (i >> 2) + (i & 1);
-                const int p = l + 8 * ((i >> 1) & 1);
-                if (m < a.M && p < a.L) {
-                    float o = acc[i] + (a.bias ? __ldg(a.bias + m) : 0.f);
-                    const size_t idx = ((size_t)tc.sample * a.M + m) * Ls + p;
-                    if (MODE == 1) o += a.residual[idx];           // plain load: may alias y
-                    if (MODE == 2) o = fmaxf(o, 0.f) * __ldg(a.gate + (gate_row0 + m) * Ls + p);
-                    if constexpr (WINDOW) { if (relu_out) o = fmaxf(o, 0.f); }   // the original model's encoder (sudormrf.py:212-218)
-                    a.y[idx] = o;
-                    if (STATS) { rs += o; rq = fmaf(o, o, rq); }
+            for (int h = 0; h < 2; ++h) {
+                const int m0 = tc.n0 + 64 * h + 2 * (lane & 3);
+                const int mrem = a.M - m0;             // channels left from this lane's first one
+                mbar_wait(&slot_bar[wg], slot_phase);
+                slot_phase ^= 1;
+#pragma unroll
+                for (int j = 0; j < 8; ++j) {          // channels m0 + 8 j + {0, 1}
+                    float bv[2];
+#pragma unroll
+                    for (int b = 0; b < 2; ++b) bv[b] = (a.bias && 8 * j + b < mrem) ? __ldg(a.bias + m0 + 8 * j + b) : 0.f;
+#pragma unroll
+                    for (int v = 0; v < 4; ++v) {
+                        const int u = 4 * j + v, i = 32 * h + u;
+                        float* e = reinterpret_cast<float*>(box + eoff[v] + 1024 * j);
+                        float o = acc[i] + bv[v & 1];
+                        if (MODE == 1) o += *e;
+                        if (MODE == 2) o = fmaxf(o, 0.f) * *e;
+                        if constexpr (WINDOW) { if (relu_out) o = fmaxf(o, 0.f); }   // the original model's encoder (sudormrf.py:212-218)
+                        *e = o;
+                        if (STATS && 8 * j + (v & 1) < mrem && 8 * (v >> 1) < prem) { rs += o; rq = fmaf(o, o, rq); }
+                        if (STATS && (i & 15) == 15) { st.add_run(rs, rq); rs = rq = 0.f; }   // fp32 runs of 16 (StatAcc)
+                    }
                 }
-                if (STATS && (i & 15) == 15) { st.add_run(rs, rq); rs = rq = 0.f; }   // fp32 runs of 16 (StatAcc)
+                if constexpr (WINDOW) {
+                    // the encoder's frame count is arbitrary, so its rows need not be 16 B aligned for TMA: the
+                    // warpgroup copies the quarter out, one 128 B row segment per warp instruction
+                    named_bar_sync(1 + wg, 128);
+#pragma unroll 4
+                    for (int r = wr; r < 64; r += 4) {
+                        const int m = tc.n0 + 64 * h + r;
+#pragma unroll
+                        for (int half = 0; half < 2; ++half) {
+                            const int p = tc.l0 + wg * 64 + half * kEpiBoxL + lane;
+                            const float v = *reinterpret_cast<const float*>(
+                                slot + half * kSlotHalf + r * 128 + (((lane >> 2) ^ (r & 7)) << 4) + (lane & 3) * 4);
+                            if (m < a.M && p < a.L) a.y[((size_t)tc.sample * a.M + m) * a.L + p] = v;
+                        }
+                    }
+                    named_bar_sync(1 + wg, 128);
+                } else {
+                    fence_proxy_async_smem();          // generic-proxy stores -> visible to the TMA store
+                    named_bar_sync(1 + wg, 128);
+                    if (issuer) {
+                        const int c0 = tc.l0 + wg * 64, c1 = tc.n0 + 64 * h;
+                        tma_store_3d(&ymap, slot, c0, c1, tc.sample);
+                        tma_store_3d(&ymap, slot + kSlotHalf, c0 + kEpiBoxL, c1, tc.sample);
+                        bulk_commit();
+                        bulk_wait_read_all();
+                    }
+                }
+                if (issuer) {                          // hand the slot on
+                    if (wg == 0) fill_slot(tile, 1, h);
+                    else if (h == 0) fill_slot(tile, 0, 1);
+                    else if (tile + tstep < a.num_tiles) fill_slot(tile + tstep, 0, 0);
+                }
             }
             if (STATS) {
                 const double ds = warp_sum_f64(st.s), dq = warp_sum_f64(st.q);
@@ -502,6 +601,7 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
                 }
             }
         }
+        if (!WINDOW && issuer) bulk_wait_all();        // the last stores have completed
     }
 }
 
@@ -531,8 +631,8 @@ int pack_pointwise_mma(const float* W, int M, int K, void* packed, cudaStream_t 
 }
 
 constexpr size_t kMmaSmemBytes = 1024 + (size_t)kStages * (kAStageBytes + kBStageBytes) +
-                                 (size_t)kRawStages * kRawStageBytes + kProdWarps * 64 * sizeof(float2) +
-                                 (2 * kStages + 2 * kRawStages) * sizeof(uint64_t);
+                                 (size_t)kRawStages * kRawStageBytes + kSlotBytes + kProdWarps * 64 * sizeof(float2) +
+                                 (2 * kStages + 2 * kRawStages + 2) * sizeof(uint64_t);
 static_assert(kMmaSmemBytes <= 232448, "exceeds the 227 KB a CTA may own on sm_90");
 
 // cuTensorMapEncodeTiled is a pure host-side encoder; it is fetched through the runtime so that the library
@@ -568,21 +668,24 @@ static int make_weight_map(CUtensorMap* tm, const void* wpk, size_t bytes) {
     return r == CUDA_SUCCESS ? SDR_OK : SDR_ERR_UNSUPPORTED;
 }
 
-// Tensor map of the activations [samples][K][L] with a [1][64][128] box: one raw k-block tile
-// (positions beyond L arrive as zeros: ragged last tiles need no special case).
-static int make_act_map(CUtensorMap* tm, const float* x, int samples, int K, int L) {
+// Tensor map of an fp32 activation tensor [samples][C][L] with a [1][64][box_l] box.  Loads fill positions beyond L
+// and channels beyond C with zeros and stores skip them: ragged last tiles need no special case.
+//   activations: box [64][128], one raw k-block tile, unswizzled;
+//   epilogue (residual, gate, y): box [64][32], one half of a slot, SWIZZLE_128B.
+static int make_act_map(CUtensorMap* tm, const float* x, int samples, int C, int L, int box_l, CUtensorMapSwizzle swz) {
     memset(tm, 0, sizeof(*tm));
     EncodeTiledFn enc = encode_tiled_fn();
     if (!enc) return SDR_ERR_CUDA;
-    const cuuint64_t dims[3] = {(cuuint64_t)L, (cuuint64_t)K, (cuuint64_t)samples};
-    const cuuint64_t strides[2] = {(cuuint64_t)L * 4, (cuuint64_t)L * K * 4};
-    const cuuint32_t box[3] = {(cuuint32_t)kTileM, (cuuint32_t)kBlockK, 1};
+    const cuuint64_t dims[3] = {(cuuint64_t)L, (cuuint64_t)C, (cuuint64_t)samples};
+    const cuuint64_t strides[2] = {(cuuint64_t)L * 4, (cuuint64_t)L * C * 4};
+    const cuuint32_t box[3] = {(cuuint32_t)box_l, 64, 1};
     const cuuint32_t estr[3] = {1, 1, 1};
     const CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), dims, strides, box, estr,
-                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_NONE,
+                           CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS ? SDR_OK : SDR_ERR_UNSUPPORTED;
 }
+static_assert(kBlockK == 64 && kTileN == 2 * 64, "activation boxes are 64 channels: one k-block, half a channel tile");
 
 // Persistent launch: one CTA per SM (the shared-memory footprint allows no second), never more than there are tiles.
 // (All instantiations share one function-pointer type, so the per-kernel state is keyed by the pointer, not by Kern.)
@@ -592,7 +695,7 @@ static std::vector<MmaLaunchInfo> g_launch_info;
 
 template <typename Kern>
 static int launch_persistent(Kern kern, const MmaArgs& a, const CUtensorMap& wmap, const CUtensorMap& xmap,
-                             cudaStream_t st) {
+                             const CUtensorMap& emap, const CUtensorMap& ymap, cudaStream_t st) {
     int dev = 0;
     if (cudaGetDevice(&dev) != cudaSuccess) return SDR_ERR_CUDA;
     int sms = 0;
@@ -610,7 +713,7 @@ static int launch_persistent(Kern kern, const MmaArgs& a, const CUtensorMap& wma
         }
     }
     const int grid = a.num_tiles < sms ? a.num_tiles : sms;
-    kern<<<grid, kMmaThreads, kMmaSmemBytes, st>>>(a, wmap, xmap);
+    kern<<<grid, kMmaThreads, kMmaSmemBytes, st>>>(a, wmap, xmap, emap, ymap);
     if (cudaGetLastError() != cudaSuccess) return SDR_ERR_CUDA;
     return SDR_OK;
 }
@@ -619,15 +722,17 @@ int launch_pointwise_mma(const float* x, const NormIn& nin, const void* wpk, con
                          const float* residual, const float* gate, int gate_channels,
                          float* y, double* stats_out, int samples, int M, int K, int L,
                          int epilogue, cudaStream_t st) {
-    if (!pointwise_mma_eligible(M, K) || (L % 4) != 0 || (reinterpret_cast<uintptr_t>(x) % 16) != 0)
-        return SDR_ERR_UNSUPPORTED;                      // TMA rows of the activations: 16 B aligned
+    auto misaligned = [](const float* p) { return (reinterpret_cast<uintptr_t>(p) % 16) != 0; };
+    if (!pointwise_mma_eligible(M, K) || (L % 4) != 0 || misaligned(x) || misaligned(y) ||
+        (epilogue != 1 && misaligned(residual)) || (epilogue == 1 && misaligned(gate)))
+        return SDR_ERR_UNSUPPORTED;                      // TMA rows of the activations and outputs: 16 B aligned
     if (samples <= 0 || L <= 0 || !x || !wpk || !y) return SDR_ERR_BAD_ARGUMENT;
     if (epilogue == 1 && (!gate || gate_channels <= 0)) return SDR_ERR_BAD_ARGUMENT;
     if (epilogue == 1 && (gate_channels % kTileN) != 0) return SDR_ERR_UNSUPPORTED;
     if (reinterpret_cast<uintptr_t>(wpk) % 16) return SDR_ERR_BAD_ARGUMENT;
     MmaArgs a;
-    a.x = x; a.nin = nin; a.bias = bias; a.residual = residual;
-    a.gate = gate; a.gate_channels = gate_channels; a.y = y; a.stats_out = stats_out;
+    a.x = x; a.nin = nin; a.bias = bias;
+    a.gate_channels = gate_channels; a.y = y; a.stats_out = stats_out;
     a.M = M; a.K = K; a.L = L; a.epilogue = epilogue;
     a.win_k = 0; a.win_hop = 0; a.win_pad = 0; a.win_a = 0; a.win_T = 0;
     a.n_tiles = mma_pad_m(M) / kTileN;
@@ -638,11 +743,18 @@ int launch_pointwise_mma(const float* x, const NormIn& nin, const void* wpk, con
     const int act = nin.prelu ? (nin.prelu_pc ? 2 : 1) : 0;
     const int mode = epilogue == 1 ? 2 : (residual ? 1 : 0);
     const bool stats = stats_out != nullptr;
-    CUtensorMap wmap, xmap;
+    CUtensorMap wmap, xmap, emap, ymap;
     if (int rc = make_weight_map(&wmap, wpk, pointwise_mma_packed_bytes(M, K))) return rc;
-    if (int rc = make_act_map(&xmap, x, samples, K, L)) return rc;
+    if (int rc = make_act_map(&xmap, x, samples, K, L, kTileM, CU_TENSOR_MAP_SWIZZLE_NONE)) return rc;
+    if (int rc = make_act_map(&ymap, y, samples, M, L, kEpiBoxL, CU_TENSOR_MAP_SWIZZLE_128B)) return rc;
+    memset(&emap, 0, sizeof(emap));
+    if (mode == 1)
+        if (int rc = make_act_map(&emap, residual, samples, M, L, kEpiBoxL, CU_TENSOR_MAP_SWIZZLE_128B)) return rc;
+    if (mode == 2)
+        if (int rc = make_act_map(&emap, gate, samples, gate_channels, L, kEpiBoxL, CU_TENSOR_MAP_SWIZZLE_128B)) return rc;
 #define SDR_MMA_CASE(A, MD, ST)                                                                                   \
-    if (act == A && mode == MD && stats == ST) return launch_persistent(pw_mma_kernel<false, A, MD, ST>, a, wmap, xmap, st);
+    if (act == A && mode == MD && stats == ST)                                                                    \
+        return launch_persistent(pw_mma_kernel<false, A, MD, ST>, a, wmap, xmap, emap, ymap, st);
     SDR_MMA_CASE(0, 0, false) SDR_MMA_CASE(0, 0, true)
     SDR_MMA_CASE(1, 0, false) SDR_MMA_CASE(1, 0, true)
     SDR_MMA_CASE(0, 1, false) SDR_MMA_CASE(0, 1, true)
@@ -677,7 +789,7 @@ int launch_encoder_mma(const float* wav, const void* wpk, const float* bias, int
     if (B <= 0 || T <= 0 || L <= 0 || !wav || !wpk || !enc) return SDR_ERR_BAD_ARGUMENT;
     MmaArgs a;
     a.x = wav; a.nin = NormIn{nullptr, nullptr, nullptr, nullptr, 1.0};
-    a.bias = bias; a.residual = nullptr; a.gate = nullptr;
+    a.bias = bias;
     a.gate_channels = 0; a.y = enc; a.stats_out = stats;
     a.M = N; a.K = enc_kpad(A, Kk); a.L = L; a.epilogue = relu ? 2 : 0;      // (window kernels read it as "ReLU on the way out")
     a.win_k = Kk; a.win_hop = Kk / 2; a.win_pad = pad; a.win_a = A; a.win_T = T;   // pad = hop; 2 * hop for the causal model
@@ -686,11 +798,11 @@ int launch_encoder_mma(const float* wav, const void* wpk, const float* bias, int
     const long long tiles = (long long)B * a.l_tiles * a.n_tiles;
     if (tiles > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
     a.num_tiles = (int)tiles;
-    CUtensorMap wmap, xmap;
+    CUtensorMap wmap, none;
     if (int rc = make_weight_map(&wmap, wpk, encoder_mma_packed_bytes(N, A, Kk))) return rc;
-    memset(&xmap, 0, sizeof(xmap));               // window mode gathers the waveform itself
-    if (stats) return launch_persistent(pw_mma_kernel<true, 0, 0, true>, a, wmap, xmap, st);
-    return launch_persistent(pw_mma_kernel<true, 0, 0, false>, a, wmap, xmap, st);
+    memset(&none, 0, sizeof(none));               // window mode gathers the waveform and writes enc itself
+    if (stats) return launch_persistent(pw_mma_kernel<true, 0, 0, true>, a, wmap, none, none, none, st);
+    return launch_persistent(pw_mma_kernel<true, 0, 0, false>, a, wmap, none, none, none, st);
 }
 
 }  // namespace sdr

@@ -86,8 +86,10 @@ def pointwise(name, M, K, mode, samples=S):
     stt = stats_of(x)
     nin = N.SdrNormIn(stt.data_ptr(), ones(K).data_ptr(), zeros(K).data_ptr(),
                       slope.data_ptr() if mode == "res" else 0, float(K * L))
-    if mode == "plain":
+    if mode in ("plain", "dec"):
         nin = N.SdrNormIn(0, 0, 0, 0, 1.0)
+    if mode == "dec":                  # the decoder GEMM: no bias, no statistics
+        bias = None
     y = torch.randn(samples, M, L, device=dev)
     sto = torch.zeros(samples, 2, dtype=torch.float64, device=dev)
     gate = torch.randn(samples, NB, L, device=dev) if mode == "mask" else None
@@ -114,6 +116,7 @@ pointwise("proj_1x1", Ci, Co, "plain")
 pointwise("res_conv+skip", Co, Ci, "res")
 pointwise("bottleneck", kw["out_channels"], NB, "norm", samples=B)
 pointwise("mask_net", kw["num_sources"] * NB, kw["out_channels"], "mask", samples=B)
+pointwise("decoder", kw["num_sources"] * kw["enc_kernel_size"], kw["num_sources"] * NB, "dec", samples=B)
 
 # depthwise levels
 for d in range(D):
