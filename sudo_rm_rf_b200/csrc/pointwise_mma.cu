@@ -5,20 +5,21 @@
 // GEMM view per tile: D[128 positions, 128 channels] = A[128, K] * B[128, K]^T with
 //   A = f(x) tile, produced on the fly: the activation tile cannot be TMA'd
 //       straight into the MMA because the producer's deferred GlobLN(+PReLU)
-//       has to be applied first.  A TMA warp lands the raw fp32 tile in shared
-//       memory; 8 transform warps apply the per-channel affine (+PReLU), split
-//       the fp32 value into bf16 hi + bf16 lo, and store both into the MN-major
-//       SWIZZLE_128B shared-memory layout the wgmma descriptors expect.
+//       has to be applied first.  A TMA warp lands the raw fp32 k-block in shared
+//       memory together with a table of its channels' folded (scale, shift); the
+//       consumer warpgroups read their A fragments from it, apply the affine
+//       (+PReLU), split each fp32 value into bf16 hi + bf16 lo and hand both to the
+//       tensor cores from registers.
 //   B = weights, pre-split into bf16 hi/lo and pre-swizzled at pack time, so a
 //       k-block is ONE TMA box of a contiguous image.
 //   D = fp32 accumulator in registers: two consumer warpgroups, each owning 64
-//       positions x 128 channels (64 registers per thread), issue the wgmmas
-//       and run the epilogue.  Persistent CTAs, one per SM; the transform and
+//       positions x 128 channels (64 registers per thread), transform their A,
+//       issue the wgmmas and run the epilogue.  Persistent CTAs, one per SM; the
 //       TMA warps run ahead into the free stages while the consumers drain.
-//   Epilogue: through a 16 KB shared-memory slot holding one quarter of the tile
+//   Epilogue: through four 16 KB shared-memory slots, one per quarter of the tile
 //       (one warpgroup's 64 positions x 64 channels).  The residual / gate quarter
-//       arrives there by TMA, the warpgroup combines it with its accumulators in
-//       place, and one thread stores the quarter to y by TMA.
+//       arrives there by TMA while the tile's main loop runs, the warpgroup combines
+//       it with its accumulators in place, and one thread stores the quarter to y by TMA.
 // Precision: x*w ~= xh*wh + xl*wh + xh*wl (3 bf16 MMAs, fp32 accumulate): the
 // dropped terms are O(2^-16) relative, i.e. fp32-grade for the 1e-3 parity
 // budget, where a single bf16 (5e-3) or tf32 (7e-4) pass is not (SURVEY §7).
@@ -39,25 +40,21 @@ namespace sdr {
 constexpr int kTileM = 128;            // positions per CTA tile (2 consumer warpgroups x wgmma M = 64)
 constexpr int kTileN = 128;            // output channels per tile (wgmma N); 64 fp32 accumulator registers per thread
 constexpr int kBlockK = 64;            // channels per k-block = one 128 B swizzle row of bf16
-constexpr int kStages = 2;             // A (transformed activations) and B (weights) stages share one full/empty barrier ring
-constexpr int kRawStages = 2;          // fp32 [64 channels][128 positions] tiles landed by TMA, read once by the transform warps
-constexpr int kRawStageBytes = kTileM * kBlockK * 4;         // 32 KB
-constexpr int kAHalf = kTileM * 128;   // 16 KB: bf16 [128 rows][64 k]
+constexpr int kStages = 3;             // weight stages: one is released a k-block after its wgmmas were issued
+constexpr int kRawStages = 2;          // fp32 activation k-blocks, released once the consumers hold them in registers
+// Raw k-blocks and epilogue slots share one box format: fp32 [64 channels][32 positions], 128 B rows, SWIZZLE_128B
+// (16 B chunk index XOR channel % 8), which keeps the A-fragment and accumulator-fragment accesses conflict-free.
+constexpr int kBoxL = 32;
+constexpr int kBoxBytes = 64 * kBoxL * 4;                    // 8 KB
+constexpr int kRawStageBytes = kTileM / kBoxL * kBoxBytes;   // 32 KB: the k-block's 128 positions as 4 boxes
 constexpr int kBHalf = kTileN * 128;   // 16 KB: bf16 [128 weight rows][64 k]
-constexpr int kAStageBytes = 2 * kAHalf;                     // 32 KB: hi + lo
 constexpr int kBStageBytes = 2 * kBHalf;                     // 32 KB: hi + lo
-// Epilogue slot: fp32 [64 channels][64 positions] as two TMA boxes of [64 channels][32 positions] (128 B rows,
-// SWIZZLE_128B: 16 B chunk index XOR channel % 8, which keeps the accumulator-fragment accesses conflict-free).
-constexpr int kEpiBoxL = 32;
-constexpr int kSlotHalf = 64 * kEpiBoxL * 4;                 // 8 KB
-constexpr int kSlotBytes = 2 * kSlotHalf;                    // 16 KB
-// Warp roles: [0, 8) the two consumer warpgroups (wgmma + epilogue), [8, 16) operand transform, 16 weight TMA,
-// 17 raw activation TMA.
-constexpr int kConsWarps = 8, kProdWarp0 = 8, kProdWarps = 8, kTmaWarp = 16, kRawWarp = 17;
-constexpr int kMmaThreads = 32 * (kRawWarp + 1);             // 576
-constexpr int kProdThreads = 32 * kProdWarps;                // 256
-constexpr int kProdElems = kTileM * kBlockK / kProdThreads;  // 32 = 8 channels x 4 positions per thread and k-block
-static_assert(kProdWarps == 8 && kProdElems == 32, "one transform warp per 8-channel k-group, 4 positions per lane");
+constexpr int kSlotBytes = 2 * kBoxBytes;                    // 16 KB: a quarter of the tile, 64 channels x 64 positions
+constexpr int kSlots = 4;                                    // slot 2 wg + h: warpgroup wg's channel half h
+// Warp roles: [0, 8) the two consumer warpgroups (operand transform, wgmma, epilogue), 8 weight TMA, 9 raw activation
+// TMA; in window mode warps 9 and 10 instead gather the waveform windows into the raw ring.
+constexpr int kConsWarps = 8, kTmaWarp = 8, kRawWarp = 9, kGatherWarps = 2;
+template <bool WINDOW> constexpr int kMmaThreads = 32 * (kRawWarp + (WINDOW ? kGatherWarps : 1));   // 320 / 352
 
 struct MmaArgs {
     const float* x;
@@ -142,29 +139,27 @@ __device__ __forceinline__ uint64_t gmma_desc_sw128(uint32_t saddr, uint32_t lbo
     d |= (uint64_t)1 << 62;
     return d;
 }
-// A operand, MN-major (positions contiguous).  Canonical layout in 16 B units ((8,n),(8,k)):((1,LBO),(8,SBO)): a 128 B
-// row holds 64 consecutive positions of one k; 8 k-rows form a 1024 B atom (16 B chunk index XOR k%8); LBO = byte
-// stride between 64-wide position blocks (one per consumer warpgroup), SBO = byte stride between groups of 8 k.
-constexpr uint32_t kALbo = 1024;       // A tile: [8 k-groups][2 position blocks][8 k rows][128 B]
-constexpr uint32_t kASbo = 2048;
 // B operand, K-major: 128 B per weight row, 8-row groups 1024 B apart (LBO unused for swizzled K-major, canonical 16 B).
 constexpr uint32_t kBLbo = 16, kBSbo = 1024;
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
-// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T for the executing warpgroup; A MN-major (imm-trans-a = 1), B K-major.
-// Thread t of the warpgroup holds d[i] at row 16 * (t / 32) + (t % 32) / 4 + 8 * ((i / 2) % 2),
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// D[64 x 128] (+)= A[64 x 16] * B[128 x 16]^T for the executing warpgroup; A from registers, B K-major in shared memory.
+// Thread t of the warpgroup holds a[j] (two bf16, the lower k in the low half) at row 16 * (t / 32) + (t % 32) / 4 +
+// 8 * (j % 2), k 2 * (t % 4) + 8 * (j / 2) + {0, 1}, and d[i] at row 16 * (t / 32) + (t % 32) / 4 + 8 * ((i / 2) % 2),
 // column 8 * (i / 4) + 2 * (t % 4) + i % 2.
-__device__ __forceinline__ void wgmma_bf16_m64n128(float (&d)[64], uint64_t adesc, uint64_t bdesc, uint32_t accumulate) {
+__device__ __forceinline__ void wgmma_bf16_m64n128_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t bdesc,
+                                                      uint32_t accumulate) {
     asm volatile(
         "{\n\t.reg .pred p;\n\t"
-        "setp.ne.b32 p, %66, 0;\n\t"
+        "setp.ne.b32 p, %69, 0;\n\t"
         "wgmma.mma_async.sync.aligned.m64n128k16.f32.bf16.bf16 "
         "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, "
         "%23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, "
         "%45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, "
-        "%64, %65, p, 1, 1, 1, 0;\n\t}"
+        "{%64, %65, %66, %67}, %68, p, 1, 1, 0;\n\t}"
         : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]),
           "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]),
           "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]),
@@ -173,7 +168,7 @@ __device__ __forceinline__ void wgmma_bf16_m64n128(float (&d)[64], uint64_t ades
           "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]),
           "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]),
           "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
-        : "l"(adesc), "l"(bdesc), "r"(accumulate)
+        : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(bdesc), "r"(accumulate)
         : "memory");
 }
 
@@ -220,43 +215,52 @@ __device__ __forceinline__ TileCoord decode_tile(const MmaArgs& a, int tile) {
     return t;
 }
 
+// The consumers issue a k-block as kGroups wgmma groups of kGroupSteps k-steps each and double-buffer the A fragments
+// per group: 64 accumulators + 2 x 16 fragment registers.  (Whole k-blocks would take 2 x 32 and spill: 10 warps put
+// 3 on one SM sub-partition, which caps a thread at 168 registers.)
+constexpr int kGroupSteps = 2;
+constexpr int kGroups = kBlockK / 16 / kGroupSteps;
+static_assert(kGroups == 2, "group g of every k-block uses fragment buffer g");
+// A operand of one group for one thread: per k-step the m64k16 register fragments of bf16 hi and bf16 lo.
+struct AFrag { uint32_t hi[kGroupSteps][4], lo[kGroupSteps][4]; };
+
 // Compile-time specialisation keeps the hot loops small.
 //   WINDOW: encoder mode (strided waveform windows as the A operand)
 //   ACT:    PReLU in the operand transform: 0 none, 1 one shared slope (nn.PReLU()), 2 one slope per input
-//           channel (nn.PReLU(C) of the original model, sudormrf.py:33,71; shared -> shared transform loop only)
+//           channel (nn.PReLU(C) of the original model, sudormrf.py:33,71)
 //   MODE:   epilogue 0 = bias only, 1 = + residual (may alias y: a tile's residual is loaded before its output is
 //           stored), 2 = ReLU * gate
 //   STATS:  accumulate (sum, sumsq) of the output
 template <bool WINDOW, int ACT, int MODE, bool STATS>
-__global__ void __launch_bounds__(kMmaThreads, 1)
+__global__ void __launch_bounds__(kMmaThreads<WINDOW>, 1)
 pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      // wmap: packed weights as [rows][128 B]
-              const __grid_constant__ CUtensorMap xmap,                       // xmap: activations [samples][K][L], box [64][128]
+              const __grid_constant__ CUtensorMap xmap,                       // xmap: activations [samples][K][L], box [64][32]
               const __grid_constant__ CUtensorMap emap,                       // emap: residual (MODE 1) or gate (MODE 2)
               const __grid_constant__ CUtensorMap ymap) {                     // ymap: output (not in window mode)
-    // 2 x (32 KB A stage + 32 KB B stage) + 2 x 32 KB raw tiles + 16 KB epilogue slot + 4 KB of tables + barriers (of
+    static_assert(!(WINDOW && ACT != 0), "the encoder's window operand has no activation");
+    // 2 x 32 KB raw k-blocks + 3 x 32 KB weight stages + 4 x 16 KB epilogue slots + 1.5 KB of tables + barriers (of
     // the 227 KB an sm_90 CTA can own).  SWIZZLE_128B needs the stage and slot bases 1024 B aligned; the launch
     // reserves 1 KB to align by hand.
     extern __shared__ uint8_t smem_raw[];
     uint8_t* smem = smem_raw + ((1024u - (smem_u32(smem_raw) & 1023u)) & 1023u);
-    uint8_t* a_base = smem;                                                  // kStages x 32 KB
-    uint8_t* b_base = smem + kStages * kAStageBytes;                         // kStages x 32 KB
-    uint8_t* r_base = b_base + kStages * kBStageBytes;                       // kRawStages x 32 KB
-    uint8_t* slot = r_base + kRawStages * kRawStageBytes;                    // 16 KB
-    // warp-private tables (no CTA-level barrier in the steady state): per transform warp the (scale, shift) of its
-    // channels, double-buffered
-    float2* s_ab = reinterpret_cast<float2*>(slot + kSlotBytes);             // [kProdWarps][64]
-    uint64_t* bars = reinterpret_cast<uint64_t*>(s_ab + kProdWarps * 64);
-    //   full_bar:   the 8 transform warps + the weight TMA thread (with the weights' tx bytes); waited on by the consumers
-    //   empty_bar:  the 8 consumer warps once their wgmmas reading the stage have retired
-    //   rfull_bar:  raw tile landed (TMA tx bytes); rempty_bar: all 8 transform warps hold it in registers
-    //   slot_bar:   per consumer warpgroup: the slot is its own (the previous quarter's store has read it) and, in
-    //               MODE 1 / 2, holds the quarter's residual / gate (TMA tx bytes).  One barrier per warpgroup: a
-    //               shared one could complete twice while a warpgroup waits, and a parity wait cannot tell.
+    uint8_t* r_base = smem;                                                  // kRawStages x 32 KB
+    uint8_t* b_base = r_base + kRawStages * kRawStageBytes;                  // kStages x 32 KB
+    uint8_t* slots = b_base + kStages * kBStageBytes;                        // kSlots x 16 KB
+    // per raw stage, its 64 channels' folded (scale, shift) and (ACT 2) PReLU slopes, written by the raw TMA warp
+    float2* s_ab = reinterpret_cast<float2*>(slots + kSlots * kSlotBytes);   // [kRawStages][64]
+    float* s_sl = reinterpret_cast<float*>(s_ab + kRawStages * kBlockK);     // [kRawStages][64]
+    uint64_t* bars = reinterpret_cast<uint64_t*>(s_sl + kRawStages * kBlockK);
+    //   full_bar:   weight stage landed (TMA tx bytes); empty_bar: the 8 consumer warps' wgmmas reading it have retired
+    //   rfull_bar:  raw k-block ready: the TMA thread's arrival with the tx bytes and the raw warp's once the stage's
+    //               table is written (window mode: one arrival per gather warp)
+    //   rempty_bar: the 8 consumer warps hold the raw k-block's values in registers
+    //   slot_bar:   per slot: the previous quarter's store has read it and, in MODE 1 / 2, it holds the quarter's
+    //               residual / gate (TMA tx bytes)
     uint64_t* full_bar = bars;                       // [kStages]
     uint64_t* empty_bar = full_bar + kStages;        // [kStages]
     uint64_t* rfull_bar = empty_bar + kStages;       // [kRawStages]
     uint64_t* rempty_bar = rfull_bar + kRawStages;   // [kRawStages]
-    uint64_t* slot_bar = rempty_bar + kRawStages;    // [2]
+    uint64_t* slot_bar = rempty_bar + kRawStages;    // [kSlots]
 
     const int tid = threadIdx.x;
     const int warp = tid >> 5, lane = tid & 31;
@@ -265,188 +269,105 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
     const int tstep = (int)gridDim.x;
 
     if (warp == kTmaWarp && lane == 0) {
-        for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], kProdWarps + 1); mbar_init(&empty_bar[s], kConsWarps); }
-        for (int s = 0; s < kRawStages; ++s) { mbar_init(&rfull_bar[s], 1); mbar_init(&rempty_bar[s], kProdWarps); }
-        mbar_init(&slot_bar[0], 1);
-        mbar_init(&slot_bar[1], 1);
+        for (int s = 0; s < kStages; ++s) { mbar_init(&full_bar[s], 1); mbar_init(&empty_bar[s], kConsWarps); }
+        for (int s = 0; s < kRawStages; ++s) {
+            mbar_init(&rfull_bar[s], WINDOW ? kGatherWarps : 2);
+            mbar_init(&rempty_bar[s], kConsWarps);
+        }
+        for (int s = 0; s < kSlots; ++s) mbar_init(&slot_bar[s], 1);
         fence_barrier_init();
     }
     __syncthreads();
 
-    if (warp >= kProdWarp0 && warp < kProdWarp0 + kProdWarps) {
-        // ===================== A-operand transform producers =====================
-        // Warp w owns the 8 channels of k-group w of every k-block; lane i owns positions 4i..4i+3.
-        // Per channel a thread reads one float4, applies the folded normalisation (+PReLU), splits bf16 hi/lo,
-        // and does two conflict-free 8-byte stores into the MN-major SWIZZLE_128B tile (row = channel, 64
-        // positions per 128 B row).
-        const int pw = warp - kProdWarp0;          // k-group (8 channels) of this warp
-        const int p4 = lane * 4;                   // first of this lane's 4 positions in the tile
-        const bool has_norm = a.nin.stats != nullptr;
-        const float slope = ACT == 1 ? __ldg(a.nin.prelu) : 1.f;
-        const bool slope_le1 = slope <= 1.f;
-        float2* const my_tab = s_ab + pw * 64;     // this warp's [2][8] (scale, shift) table (lane e < 8); ACT == 2: the
-                                                   // channels' PReLU slopes in entries [16, 32) of the same 64-entry slice
-        static_assert(!(WINDOW && ACT != 0), "the encoder's window operand has no activation");
-        const double inv_count = 1.0 / a.nin.count;
-        // byte offset of (channel row e = 0, this lane's positions) inside an A half tile
-        const uint32_t lane_off = (uint32_t)pw * kASbo + (uint32_t)(lane >> 4) * kALbo + (uint32_t)(lane & 1) * 8;
-        const uint32_t lane_chunk = (uint32_t)((lane & 15) >> 1);
-
-        struct Cur { int tile, kb; TileCoord tc; };
-        auto advance = [&](Cur& c) {              // next (tile, k-block) of this CTA; tile >= num_tiles == end
-            if (++c.kb == KB) {
-                c.kb = 0;
-                c.tile += tstep;
-                if (c.tile < a.num_tiles) c.tc = decode_tile(a, c.tile);
-            }
-        };
-        struct Aux { float g, b; double s0, s1; float sl; };
-        auto load_aux = [&](const Cur& c) -> Aux {   // lane e: gamma/beta of channel e of this warp's k-group
-            Aux x{1.f, 0.f, 0.0, 1.0, 1.f};
-            if constexpr (ACT == 2) {
-                if (c.tile < a.num_tiles) x.sl = __ldg(a.nin.prelu + c.kb * kBlockK + pw * 8 + (lane & 7));
-            }
-            if (has_norm && c.tile < a.num_tiles) {
-                const int k = c.kb * kBlockK + pw * 8 + (lane & 7);
-                x.g = __ldg(a.nin.gamma + k);
-                x.b = __ldg(a.nin.beta + k);
-                if (c.kb == 0) {                   // new tile: its sample's (sum, sumsq)
-                    x.s0 = a.nin.stats[2 * (size_t)c.tc.sample];
-                    x.s1 = a.nin.stats[2 * (size_t)c.tc.sample + 1];
-                }
-            }
-            return x;
-        };
-        // one stage's 8 channel rows (4 positions each) -> folded affine (+PReLU) -> bf16 hi/lo into A stage `stage`
-        auto store_rows = [&](const float4 (&v)[8], const float2 (&abv)[8], const float (&slv)[ACT == 2 ? 8 : 1],
-                              int stage) {
-            uint8_t* a_hi = a_base + (size_t)stage * kAStageBytes;
-            uint8_t* a_lo = a_hi + kAHalf;
-#pragma unroll
-            for (int e = 0; e < 8; ++e) {
-                const float2 ab = abv[e];
-                float y[4] = {fmaf(v[e].x, ab.x, ab.y), fmaf(v[e].y, ab.x, ab.y),
-                              fmaf(v[e].z, ab.x, ab.y), fmaf(v[e].w, ab.x, ab.y)};
-                if constexpr (ACT == 1) {      // PReLU in 2 ops: max(y, s*y) for s <= 1, min otherwise
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) {
-                        const float t = y[u] * slope;
-                        y[u] = slope_le1 ? fmaxf(y[u], t) : fminf(y[u], t);
-                    }
-                } else if constexpr (ACT == 2) {   // this channel's own slope (either side of 1, either sign)
-                    const float sl = slv[ACT == 2 ? e : 0];
-#pragma unroll
-                    for (int u = 0; u < 4; ++u) y[u] = y[u] >= 0.f ? y[u] : y[u] * sl;
-                }
-                // hi = top 16 bits (truncation), lo = bf16(y - hi): y - hi is exact in fp32, so
-                // |y - hi - lo| <= 2^-9 |y - hi| <= 2^-16 |y|
-                uint32_t hb[4];
-#pragma unroll
-                for (int u = 0; u < 4; ++u) hb[u] = __float_as_uint(y[u]) & 0xffff0000u;
-                const uint32_t h01 = __byte_perm(hb[0], hb[1], 0x7632), h23 = __byte_perm(hb[2], hb[3], 0x7632);
-                const __nv_bfloat162 l01 = __floats2bfloat162_rn(y[0] - __uint_as_float(hb[0]), y[1] - __uint_as_float(hb[1]));
-                const __nv_bfloat162 l23 = __floats2bfloat162_rn(y[2] - __uint_as_float(hb[2]), y[3] - __uint_as_float(hb[3]));
-                const uint32_t off = lane_off + (uint32_t)e * 128 + ((lane_chunk ^ (uint32_t)e) << 4);
-                *reinterpret_cast<uint2*>(a_hi + off) = make_uint2(h01, h23);
-                *reinterpret_cast<uint2*>(a_lo + off) = make_uint2(*reinterpret_cast<const uint32_t*>(&l01),
-                                                                    *reinterpret_cast<const uint32_t*>(&l23));
-            }
-            fence_proxy_async_smem();          // generic-proxy stores -> visible to the tensor core (async proxy)
-            __syncwarp();
-            if (lane == 0) mbar_arrive(&full_bar[stage]);
-        };
-
-        Cur c;
-        c.tile = tile0; c.kb = 0;
-        if (c.tile < a.num_tiles) {
-            c.tc = decode_tile(a, c.tile);
-            Aux aux = load_aux(c);
-            uint32_t it = 0;
-            int stage = 0, rs = 0;
-            uint32_t phase = 0, rphase = 0;    // parities of the ring passes
-            float mean = 0.f, rstd = 1.f;      // of the current tile's sample
-            const uint32_t raw_lane = (uint32_t)(pw * 8) * 512u + (uint32_t)lane * 16u;
+    if (warp >= kRawWarp) {
+        int rs = 0;
+        uint32_t rphase = 0;
+        if constexpr (WINDOW) {
+            // ===================== window gather: strided waveform windows -> raw ring =====================
+            // Warp g writes channels [32 g, 32 g + 32) of every k-block, 16 at a time, in the raw TMA's box layout;
+            // lane = position within a box, so each row write is one conflict-free 128 B store.
+            constexpr int kGatherCh = kBlockK / kGatherWarps;
+            const int c0 = (warp - kRawWarp) * kGatherCh;
 #pragma unroll 1
-            while (c.tile < a.num_tiles) {
-                Cur n = c;
-                advance(n);                    // next step (n.tile >= num_tiles: none)
-                {                              // y = x * aa + bb  ==  gamma * (x - mean) * rstd + beta
-                    float aa = 1.f, bb = 0.f;
-                    if (has_norm) {
-                        if (c.kb == 0) {
-                            const double mu = aux.s0 * inv_count;
-                            double var = aux.s1 * inv_count - mu * mu;
-                            var = var < 0.0 ? 0.0 : var;
-                            mean = (float)mu;
-                            rstd = rsqrtf((float)var + kGlnEps);
-                        }
-                        aa = aux.g * rstd;
-                        bb = aux.b - mean * aa;
-                    }
-                    if (lane < 8) {
-                        my_tab[(it & 1) * 8 + lane] = make_float2(aa, bb);
-                        if constexpr (ACT == 2) my_tab[16 + (it & 1) * 8 + lane] = make_float2(aux.sl, 0.f);
-                    }
-                    aux = load_aux(n);
-                }
-                __syncwarp();                  // table visible to the warp (reuse is ordered by the next __syncwarp)
-                const float2* tab = my_tab + (it & 1) * 8;
-                float2 abv[8];
-#pragma unroll
-                for (int e = 0; e < 8; ++e) abv[e] = tab[e];
-                float slv[ACT == 2 ? 8 : 1] = {1.f};
-                if constexpr (ACT == 2) {
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) slv[e] = tab[16 + e].x;
-                }
-                float4 v[8];
-                if constexpr (WINDOW) {        // encoder: strided analysis windows of the waveform, gathered directly
-                    const int l = c.tc.l0 + p4;
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) {
-                        const int k = c.kb * kBlockK + pw * 8 + e;
-                        const int ch = k / a.win_k, j = k - ch * a.win_k;
-                        float vv[4];
-#pragma unroll
-                        for (int u = 0; u < 4; ++u) {
-                            const long long t = (long long)a.win_hop * (l + u) + j - a.win_pad;
-                            vv[u] = (l + u < a.L && ch < a.win_a && t >= 0 && t < a.win_T)
-                                        ? __ldg(a.x + ((size_t)c.tc.sample * a.win_a + ch) * a.win_T + t) : 0.f;
-                        }
-                        v[e] = make_float4(vv[0], vv[1], vv[2], vv[3]);
-                    }
-                } else {                       // the raw tile of this k-block, landed by the raw loader's TMA
-                    mbar_wait(&rfull_bar[rs], rphase);
-                    const uint8_t* rp = r_base + (size_t)rs * kRawStageBytes + raw_lane;
-#pragma unroll
-                    for (int e = 0; e < 8; ++e) v[e] = *reinterpret_cast<const float4*>(rp + e * 512);
-                    __syncwarp();              // every lane holds its quads: the slot may be refilled
-                    if (lane == 0) mbar_arrive(&rempty_bar[rs]);
-                    if (++rs == kRawStages) { rs = 0; rphase ^= 1; }
-                }
-                mbar_wait(&empty_bar[stage], phase ^ 1);
-                store_rows(v, abv, slv, stage);
-                ++it;
-                if (++stage == kStages) { stage = 0; phase ^= 1; }
-                c = n;
-            }
-        }
-    } else if (warp == kRawWarp) {
-        // ===================== raw activation tiles: TMA producer =====================
-        if (lane == 0 && !WINDOW) {
-            int rs = 0;
-            uint32_t rphase = 0;
             for (int tile = tile0; tile < a.num_tiles; tile += tstep) {
                 const TileCoord tc = decode_tile(a, tile);
+#pragma unroll 1
                 for (int kb = 0; kb < KB; ++kb) {
+                    uint8_t* rp = r_base + (size_t)rs * kRawStageBytes + (lane & 3) * 4;
+#pragma unroll
+                    for (int i0 = 0; i0 < kGatherCh; i0 += 16) {
+                        float v[16][kTileM / kBoxL];
+#pragma unroll
+                        for (int i = 0; i < 16; ++i) {
+                            const int k = kb * kBlockK + c0 + i0 + i;
+                            const int ch = k / a.win_k, j = k - ch * a.win_k;
+                            const float* src = a.x + ((size_t)tc.sample * a.win_a + ch) * a.win_T;
+#pragma unroll
+                            for (int b = 0; b < kTileM / kBoxL; ++b) {
+                                const int l = tc.l0 + b * kBoxL + lane;
+                                const long long t = (long long)a.win_hop * l + j - a.win_pad;
+                                v[i][b] = (l < a.L && ch < a.win_a && t >= 0 && t < a.win_T) ? __ldg(src + t) : 0.f;
+                            }
+                        }
+                        if (i0 == 0) mbar_wait(&rempty_bar[rs], rphase ^ 1);
+#pragma unroll
+                        for (int i = 0; i < 16; ++i) {
+                            const int c = c0 + i0 + i;
+#pragma unroll
+                            for (int b = 0; b < kTileM / kBoxL; ++b)
+                                *reinterpret_cast<float*>(rp + b * kBoxBytes + c * 128 + (((lane >> 2) ^ (c & 7)) << 4)) = v[i][b];
+                        }
+                    }
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&rfull_bar[rs]);
+                    if (++rs == kRawStages) { rs = 0; rphase ^= 1; }
+                }
+            }
+        } else {
+            // ===================== raw activation k-blocks: TMA + the channels' folded affine =====================
+            // y = x * aa + bb  ==  gamma * (x - mean) * rstd + beta; lane e computes channels 2 e and 2 e + 1.
+            const bool has_norm = a.nin.stats != nullptr;
+            const double inv_count = 1.0 / a.nin.count;
+#pragma unroll 1
+            for (int tile = tile0; tile < a.num_tiles; tile += tstep) {
+                const TileCoord tc = decode_tile(a, tile);
+                float mean = 0.f, rstd = 1.f;          // of the tile's sample
+                if (has_norm) {
+                    const double mu = a.nin.stats[2 * (size_t)tc.sample] * inv_count;
+                    double var = a.nin.stats[2 * (size_t)tc.sample + 1] * inv_count - mu * mu;
+                    var = var < 0.0 ? 0.0 : var;
+                    mean = (float)mu;
+                    rstd = rsqrtf((float)var + kGlnEps);
+                }
+#pragma unroll 1
+                for (int kb = 0; kb < KB; ++kb) {
+                    const int k = kb * kBlockK + 2 * lane;
+                    float g[2] = {1.f, 1.f}, be[2] = {0.f, 0.f}, sl[2] = {1.f, 1.f};
+                    if (has_norm) {
+                        g[0] = __ldg(a.nin.gamma + k); g[1] = __ldg(a.nin.gamma + k + 1);
+                        be[0] = __ldg(a.nin.beta + k); be[1] = __ldg(a.nin.beta + k + 1);
+                    }
+                    if constexpr (ACT == 2) { sl[0] = __ldg(a.nin.prelu + k); sl[1] = __ldg(a.nin.prelu + k + 1); }
                     mbar_wait(&rempty_bar[rs], rphase ^ 1);
-                    mbar_arrive_expect_tx(&rfull_bar[rs], kRawStageBytes);
-                    tma_load_3d(r_base + (size_t)rs * kRawStageBytes, &xmap, &rfull_bar[rs], tc.l0, kb * kBlockK, tc.sample);
+                    if (lane == 0) {
+                        mbar_arrive_expect_tx(&rfull_bar[rs], kRawStageBytes);
+                        for (int b = 0; b < kTileM / kBoxL; ++b)
+                            tma_load_3d(r_base + (size_t)rs * kRawStageBytes + b * kBoxBytes, &xmap, &rfull_bar[rs],
+                                        tc.l0 + b * kBoxL, kb * kBlockK, tc.sample);
+                    }
+                    float aa[2] = {1.f, 1.f}, bb[2] = {0.f, 0.f};
+                    if (has_norm) {
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) { aa[e] = g[e] * rstd; bb[e] = be[e] - mean * aa[e]; }
+                    }
+                    *reinterpret_cast<float4*>(s_ab + rs * kBlockK + 2 * lane) = make_float4(aa[0], bb[0], aa[1], bb[1]);
+                    if constexpr (ACT == 2) *reinterpret_cast<float2*>(s_sl + rs * kBlockK + 2 * lane) = make_float2(sl[0], sl[1]);
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&rfull_bar[rs]);
                     if (++rs == kRawStages) { rs = 0; rphase ^= 1; }
                 }
             }
         }
-        __syncwarp();
     } else if (warp == kTmaWarp) {
         // ===================== B-operand (weights) TMA producer =====================
         if (lane == 0) {
@@ -463,85 +384,151 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
             }
         }
         __syncwarp();
-    } else if (warp < kConsWarps) {
-        // ===================== consumers: wgmma main loop + epilogue through the slot =====================
+    } else {
+        // ===================== consumers: operand transform + wgmma main loop + epilogue =====================
         const int wg = warp >> 2;                  // position block [64 wg, 64 wg + 64) of the tile
         const int wr = warp & 3;                   // 16-row slice of the warpgroup's block
-        const bool issuer = (tid & 127) == 0;      // the warpgroup's thread that issues its slot's TMA traffic
+        const int q = lane & 3;
+        const bool issuer = (tid & 127) == 0;      // the warpgroup's thread that issues its slots' TMA traffic
         const bool relu_out = WINDOW && a.epilogue == 2;       // window mode only: ReLU on the way out
-        // The slot passes through the tile's quarters in the order (wg 0, half 0), (wg 1, half 0), (wg 0, half 1),
-        // (wg 1, half 1), then to the next tile.  Whoever has drained a quarter hands the slot to the next one:
-        // loads its residual / gate (MODE 1 / 2) or just arrives (MODE 0).  The first quarter of a tile thus loads
-        // while the tile's main loop runs.
-        auto fill_slot = [&](int tile, int qwg, int qh) {
-            uint64_t* bar = &slot_bar[qwg];
+        const float slope = ACT == 1 ? __ldg(a.nin.prelu) : 1.f;
+        const bool slope_le1 = slope <= 1.f;
+        // The lane's A-fragment and accumulator elements sit in box 2 wg + wr / 2 of a raw stage or box wr / 2 of a
+        // slot, at channel row c = 2 (lane % 4) + v % 2 (+ 8 j) and position pp = 16 (wr % 2) + lane / 4 + 8 (v / 2);
+        // the swizzled byte offset of (c, pp) is 128 c + 16 ((pp / 4) ^ (c % 8)) + 4 (pp % 4) = boff[v] + 1024 j.
+        uint32_t boff[4];
+#pragma unroll
+        for (int v = 0; v < 4; ++v) {
+            const uint32_t c = 2 * q + (v & 1), pp = 16 * (wr & 1) + (lane >> 2) + 8 * (v >> 1);
+            boff[v] = c * 128 + (((pp >> 2) ^ c) << 4) + (pp & 3) * 4;
+        }
+        const uint32_t raw_box = (uint32_t)(2 * wg + (wr >> 1)) * kBoxBytes;
+        uint8_t* const my_slots = slots + (size_t)(2 * wg) * kSlotBytes;
+        // Each warpgroup owns slots 2 wg (channels 0-63 of the tile) and 2 wg + 1 (64-127).  Once a quarter's store has
+        // read its slot, the issuer loads the same quarter of the CTA's next tile (MODE 1 / 2) or only arrives (MODE 0),
+        // so all four residual / gate quarters land while that tile's main loop runs.
+        auto fill_slot = [&](int tile, int h) {
+            uint64_t* bar = &slot_bar[2 * wg + h];
             if constexpr (MODE == 0) {
                 mbar_arrive(bar);
             } else {
-                const TileCoord q = decode_tile(a, tile);
-                const int c0 = q.l0 + 64 * qwg;
-                const int c1 = (MODE == 1 ? q.n0 : q.n0 % a.gate_channels) + 64 * qh;
+                const TileCoord t = decode_tile(a, tile);
+                const int c0 = t.l0 + 64 * wg;
+                const int c1 = (MODE == 1 ? t.n0 : t.n0 % a.gate_channels) + 64 * h;
+                uint8_t* const dst = my_slots + (size_t)h * kSlotBytes;
                 mbar_arrive_expect_tx(bar, kSlotBytes);
-                tma_load_3d(slot, &emap, bar, c0, c1, q.sample);
-                tma_load_3d(slot + kSlotHalf, &emap, bar, c0 + kEpiBoxL, c1, q.sample);
+                tma_load_3d(dst, &emap, bar, c0, c1, t.sample);
+                tma_load_3d(dst + kBoxBytes, &emap, bar, c0 + kBoxL, c1, t.sample);
             }
         };
-        if (tid == 0) fill_slot(tile0, 0, 0);
-        uint32_t slot_phase = 0;
-        int stage = 0;
-        uint32_t phase = 0;
+        if (issuer) { fill_slot(tile0, 0); fill_slot(tile0, 1); }
+
+        int rs = 0, stage = 0, prev_stage = 0;
+        uint32_t rphase = 0, phase = 0, slot_phase = 0;
+        // Group g of the current raw k-block -> folded affine (+PReLU) -> A fragments of bf16 hi (truncation) and lo
+        // (bf16(y - hi)): y - hi is exact in fp32, so |y - hi - lo| <= 2^-9 |y - hi| <= 2^-16 |y|.  The last group
+        // releases the raw stage.
+        auto transform = [&](AFrag& f, int g) {
+            if (g == 0) mbar_wait(&rfull_bar[rs], rphase);
+            const uint8_t* rp = r_base + (size_t)rs * kRawStageBytes + raw_box;
+            const float2* tab = s_ab + rs * kBlockK + 2 * q;
+            const float* tsl = s_sl + rs * kBlockK + 2 * q;
+#pragma unroll
+            for (int s = 0; s < kGroupSteps; ++s) {
+#pragma unroll
+                for (int h = 0; h < 2; ++h) {      // channels 16 ks + 8 h + 2 q + {0, 1}: fragment registers 2 h, 2 h + 1
+                    const int c = 16 * (g * kGroupSteps + s) + 8 * h;
+                    float4 ab = make_float4(1.f, 0.f, 1.f, 0.f);
+                    float2 sl = make_float2(1.f, 1.f);
+                    if constexpr (!WINDOW) ab = *reinterpret_cast<const float4*>(tab + c);
+                    if constexpr (ACT == 2) sl = *reinterpret_cast<const float2*>(tsl + c);
+#pragma unroll
+                    for (int ph = 0; ph < 2; ++ph) {   // positions + 8 ph
+                        float y[2];
+#pragma unroll
+                        for (int e = 0; e < 2; ++e) {
+                            const float x = *reinterpret_cast<const float*>(rp + boff[e + 2 * ph] + c * 128);
+                            y[e] = WINDOW ? x : fmaf(x, e ? ab.z : ab.x, e ? ab.w : ab.y);
+                            if constexpr (ACT == 1) {      // PReLU in 2 ops: max(y, s*y) for s <= 1, min otherwise
+                                const float t = y[e] * slope;
+                                y[e] = slope_le1 ? fmaxf(y[e], t) : fminf(y[e], t);
+                            } else if constexpr (ACT == 2) {   // this channel's own slope (either side of 1, either sign)
+                                y[e] = y[e] >= 0.f ? y[e] : y[e] * (e ? sl.y : sl.x);
+                            }
+                        }
+                        const uint32_t h0 = __float_as_uint(y[0]) & 0xffff0000u, h1 = __float_as_uint(y[1]) & 0xffff0000u;
+                        const __nv_bfloat162 lo = __floats2bfloat162_rn(y[0] - __uint_as_float(h0), y[1] - __uint_as_float(h1));
+                        f.hi[s][2 * h + ph] = __byte_perm(h0, h1, 0x7632);
+                        f.lo[s][2 * h + ph] = *reinterpret_cast<const uint32_t*>(&lo);
+                    }
+                }
+            }
+            if (g == kGroups - 1) {
+                __syncwarp();                      // every lane holds its values: the raw stage may be refilled
+                if (lane == 0) mbar_arrive(&rempty_bar[rs]);
+                if (++rs == kRawStages) { rs = 0; rphase ^= 1; }
+            }
+        };
         float acc[64];
+        // Group g of k-block kb: 3 products per k-step (xh*wh, xl*wh, xh*wl) with A from `cur`.  Once the previous
+        // group's wgmmas have retired (fragment buffer `nxt` is free, and at g == 0 the previous k-block's weight
+        // stage), the next group is transformed into `nxt` while these run.
+        auto mma_group = [&](int kb, int g, const AFrag& cur, AFrag& nxt) {
+            if (g == 0) mbar_wait(&full_bar[stage], phase);
+            const uint32_t sb_hi = smem_u32(b_base + (size_t)stage * kBStageBytes);
+            const uint32_t sb_lo = sb_hi + kBHalf;
+            wgmma_fence();                         // cur's registers were written by the transform
+#pragma unroll
+            for (int s = 0; s < kGroupSteps; ++s) {
+                const int ks = g * kGroupSteps + s;
+                const uint64_t dbh = gmma_desc_sw128(sb_hi + ks * 32, kBLbo, kBSbo);
+                const uint64_t dbl = gmma_desc_sw128(sb_lo + ks * 32, kBLbo, kBSbo);
+                wgmma_bf16_m64n128_rs(acc, cur.hi[s], dbh, (kb | ks) != 0 ? 1u : 0u);
+                wgmma_bf16_m64n128_rs(acc, cur.lo[s], dbh, 1u);
+                wgmma_bf16_m64n128_rs(acc, cur.hi[s], dbl, 1u);
+            }
+            wgmma_commit();
+            wgmma_wait<1>();
+            if (g == 0 && kb > 0) {
+                __syncwarp();
+                if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);
+            }
+            if (g == kGroups - 1) {
+                prev_stage = stage;
+                if (++stage == kStages) { stage = 0; phase ^= 1; }
+                if (kb + 1 < KB) transform(nxt, 0);
+            } else {
+                transform(nxt, g + 1);
+            }
+        };
+        AFrag fa, fb;
 #pragma unroll 1
         for (int tile = tile0; tile < a.num_tiles; tile += tstep) {
             const TileCoord tc = decode_tile(a, tile);
 #pragma unroll
             for (int i = 0; i < 64; ++i) acc[i] = 0.f;
+            transform(fa, 0);
 #pragma unroll 1
             for (int kb = 0; kb < KB; ++kb) {
-                mbar_wait(&full_bar[stage], phase);   // A transformed, B landed
-                const uint32_t sa_hi = smem_u32(a_base + (size_t)stage * kAStageBytes) + (uint32_t)wg * kALbo;
-                const uint32_t sa_lo = sa_hi + kAHalf;
-                const uint32_t sb_hi = smem_u32(b_base + (size_t)stage * kBStageBytes);
-                const uint32_t sb_lo = sb_hi + kBHalf;
-                wgmma_fence();
-#pragma unroll
-                for (int ks = 0; ks < kBlockK / 16; ++ks) {
-                    // A is MN-major: a K=16 step spans two 8-channel groups (2 * SBO bytes apart)
-                    const uint64_t dah = gmma_desc_sw128(sa_hi + ks * 2 * kASbo, kALbo, kASbo);
-                    const uint64_t dal = gmma_desc_sw128(sa_lo + ks * 2 * kASbo, kALbo, kASbo);
-                    const uint64_t dbh = gmma_desc_sw128(sb_hi + ks * 32, kBLbo, kBSbo);
-                    const uint64_t dbl = gmma_desc_sw128(sb_lo + ks * 32, kBLbo, kBSbo);
-                    wgmma_bf16_m64n128(acc, dah, dbh, (kb | ks) != 0 ? 1u : 0u);
-                    wgmma_bf16_m64n128(acc, dal, dbh, 1u);
-                    wgmma_bf16_m64n128(acc, dah, dbl, 1u);
-                }
-                wgmma_commit();
-                wgmma_wait_all();
-                __syncwarp();
-                if (lane == 0) mbar_arrive(&empty_bar[stage]);   // this warp's reads of the stage have retired
-                if (++stage == kStages) { stage = 0; phase ^= 1; }
+                mma_group(kb, 0, fa, fb);
+                mma_group(kb, 1, fb, fa);
             }
-            // epilogue, one channel half h (accumulators [32 h, 32 h + 32)) at a time: lane owns positions pp and
-            // pp + 8 of its warp's 32-position box, and channel pairs 8 j + 2 (lane % 4) + {0, 1} of the half
-            // Accumulator u of the half sits at channel row c = 8 (u / 4) + 2 (lane % 4) + u % 2 of the box and
-            // position pp = 16 (wr % 2) + lane / 4 + 8 ((u / 2) % 2); its swizzled byte offset is
-            // 128 c + 16 ((pp / 4) ^ (c % 8)) + 4 (pp % 4) = eoff[u % 4] + 1024 (u / 4).
-            uint8_t* const box = slot + (wr >> 1) * kSlotHalf;
-            uint32_t eoff[4];
-#pragma unroll
-            for (int v = 0; v < 4; ++v) {
-                const uint32_t c = 2 * (lane & 3) + (v & 1), pp = 16 * (wr & 1) + (lane >> 2) + 8 * (v >> 1);
-                eoff[v] = c * 128 + (((pp >> 2) ^ c) << 4) + (pp & 3) * 4;
-            }
+            wgmma_wait<0>();
+            __syncwarp();
+            if (lane == 0) mbar_arrive(&empty_bar[prev_stage]);   // the last k-block's wgmmas have retired
+            // epilogue, one channel half h (accumulators [32 h, 32 h + 32), slot 2 wg + h) at a time: lane owns
+            // positions pp and pp + 8 of its warp's 32-position box, and channel pairs 8 j + 2 (lane % 4) + {0, 1} of
+            // the half; accumulator u of the half sits at boff[u % 4] + 1024 (u / 4) of the box.
             const int prem = a.L - (tc.l0 + wg * 64 + 32 * (wr >> 1) + 16 * (wr & 1) + (lane >> 2));   // positions left
             StatAcc st;
-            float rs = 0.f, rq = 0.f;
+            float rs_ = 0.f, rq = 0.f;
 #pragma unroll
             for (int h = 0; h < 2; ++h) {
-                const int m0 = tc.n0 + 64 * h + 2 * (lane & 3);
+                uint8_t* const slot = my_slots + (size_t)h * kSlotBytes;
+                uint8_t* const box = slot + (wr >> 1) * kBoxBytes;
+                const int m0 = tc.n0 + 64 * h + 2 * q;
                 const int mrem = a.M - m0;             // channels left from this lane's first one
-                mbar_wait(&slot_bar[wg], slot_phase);
-                slot_phase ^= 1;
+                mbar_wait(&slot_bar[2 * wg + h], slot_phase);
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {          // channels m0 + 8 j + {0, 1}
                     float bv[2];
@@ -550,14 +537,14 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
 #pragma unroll
                     for (int v = 0; v < 4; ++v) {
                         const int u = 4 * j + v, i = 32 * h + u;
-                        float* e = reinterpret_cast<float*>(box + eoff[v] + 1024 * j);
+                        float* e = reinterpret_cast<float*>(box + boff[v] + 1024 * j);
                         float o = acc[i] + bv[v & 1];
                         if (MODE == 1) o += *e;
                         if (MODE == 2) o = fmaxf(o, 0.f) * *e;
                         if constexpr (WINDOW) { if (relu_out) o = fmaxf(o, 0.f); }   // the original model's encoder (sudormrf.py:212-218)
                         *e = o;
-                        if (STATS && 8 * j + (v & 1) < mrem && 8 * (v >> 1) < prem) { rs += o; rq = fmaf(o, o, rq); }
-                        if (STATS && (i & 15) == 15) { st.add_run(rs, rq); rs = rq = 0.f; }   // fp32 runs of 16 (StatAcc)
+                        if (STATS && 8 * j + (v & 1) < mrem && 8 * (v >> 1) < prem) { rs_ += o; rq = fmaf(o, o, rq); }
+                        if (STATS && (i & 15) == 15) { st.add_run(rs_, rq); rs_ = rq = 0.f; }   // fp32 runs of 16 (StatAcc)
                     }
                 }
                 if constexpr (WINDOW) {
@@ -569,9 +556,9 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
                         const int m = tc.n0 + 64 * h + r;
 #pragma unroll
                         for (int half = 0; half < 2; ++half) {
-                            const int p = tc.l0 + wg * 64 + half * kEpiBoxL + lane;
+                            const int p = tc.l0 + wg * 64 + half * kBoxL + lane;
                             const float v = *reinterpret_cast<const float*>(
-                                slot + half * kSlotHalf + r * 128 + (((lane >> 2) ^ (r & 7)) << 4) + (lane & 3) * 4);
+                                slot + half * kBoxBytes + r * 128 + (((lane >> 2) ^ (r & 7)) << 4) + (lane & 3) * 4);
                             if (m < a.M && p < a.L) a.y[((size_t)tc.sample * a.M + m) * a.L + p] = v;
                         }
                     }
@@ -582,17 +569,14 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
                     if (issuer) {
                         const int c0 = tc.l0 + wg * 64, c1 = tc.n0 + 64 * h;
                         tma_store_3d(&ymap, slot, c0, c1, tc.sample);
-                        tma_store_3d(&ymap, slot + kSlotHalf, c0 + kEpiBoxL, c1, tc.sample);
+                        tma_store_3d(&ymap, slot + kBoxBytes, c0 + kBoxL, c1, tc.sample);
                         bulk_commit();
                         bulk_wait_read_all();
                     }
                 }
-                if (issuer) {                          // hand the slot on
-                    if (wg == 0) fill_slot(tile, 1, h);
-                    else if (h == 0) fill_slot(tile, 0, 1);
-                    else if (tile + tstep < a.num_tiles) fill_slot(tile + tstep, 0, 0);
-                }
+                if (issuer && tile + tstep < a.num_tiles) fill_slot(tile + tstep, h);
             }
+            slot_phase ^= 1;
             if (STATS) {
                 const double ds = warp_sum_f64(st.s), dq = warp_sum_f64(st.q);
                 if (lane == 0) {
@@ -630,9 +614,9 @@ int pack_pointwise_mma(const float* W, int M, int K, void* packed, cudaStream_t 
     return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
 }
 
-constexpr size_t kMmaSmemBytes = 1024 + (size_t)kStages * (kAStageBytes + kBStageBytes) +
-                                 (size_t)kRawStages * kRawStageBytes + kSlotBytes + kProdWarps * 64 * sizeof(float2) +
-                                 (2 * kStages + 2 * kRawStages + 2) * sizeof(uint64_t);
+constexpr size_t kMmaSmemBytes = 1024 + (size_t)kRawStages * kRawStageBytes + (size_t)kStages * kBStageBytes +
+                                 (size_t)kSlots * kSlotBytes + kRawStages * kBlockK * (sizeof(float2) + sizeof(float)) +
+                                 (2 * kStages + 2 * kRawStages + kSlots) * sizeof(uint64_t);
 static_assert(kMmaSmemBytes <= 232448, "exceeds the 227 KB a CTA may own on sm_90");
 
 // cuTensorMapEncodeTiled is a pure host-side encoder; it is fetched through the runtime so that the library
@@ -668,20 +652,19 @@ static int make_weight_map(CUtensorMap* tm, const void* wpk, size_t bytes) {
     return r == CUDA_SUCCESS ? SDR_OK : SDR_ERR_UNSUPPORTED;
 }
 
-// Tensor map of an fp32 activation tensor [samples][C][L] with a [1][64][box_l] box.  Loads fill positions beyond L
-// and channels beyond C with zeros and stores skip them: ragged last tiles need no special case.
-//   activations: box [64][128], one raw k-block tile, unswizzled;
-//   epilogue (residual, gate, y): box [64][32], one half of a slot, SWIZZLE_128B.
-static int make_act_map(CUtensorMap* tm, const float* x, int samples, int C, int L, int box_l, CUtensorMapSwizzle swz) {
+// Tensor map of an fp32 activation tensor [samples][C][L] with a [1][64][32] box, SWIZZLE_128B: a quarter of a raw
+// k-block (activations) or half of an epilogue slot (residual, gate, y).  Loads fill positions beyond L and channels
+// beyond C with zeros and stores skip them: ragged last tiles need no special case.
+static int make_act_map(CUtensorMap* tm, const float* x, int samples, int C, int L) {
     memset(tm, 0, sizeof(*tm));
     EncodeTiledFn enc = encode_tiled_fn();
     if (!enc) return SDR_ERR_CUDA;
     const cuuint64_t dims[3] = {(cuuint64_t)L, (cuuint64_t)C, (cuuint64_t)samples};
     const cuuint64_t strides[2] = {(cuuint64_t)L * 4, (cuuint64_t)L * C * 4};
-    const cuuint32_t box[3] = {(cuuint32_t)box_l, 64, 1};
+    const cuuint32_t box[3] = {(cuuint32_t)kBoxL, 64, 1};
     const cuuint32_t estr[3] = {1, 1, 1};
     const CUresult r = enc(tm, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 3, const_cast<float*>(x), dims, strides, box, estr,
-                           CU_TENSOR_MAP_INTERLEAVE_NONE, swz,
+                           CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B,
                            CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     return r == CUDA_SUCCESS ? SDR_OK : SDR_ERR_UNSUPPORTED;
 }
@@ -693,7 +676,7 @@ struct MmaLaunchInfo { const void* fn; int dev; int sms; };
 static std::mutex g_launch_mutex;
 static std::vector<MmaLaunchInfo> g_launch_info;
 
-template <typename Kern>
+template <bool WINDOW, typename Kern>
 static int launch_persistent(Kern kern, const MmaArgs& a, const CUtensorMap& wmap, const CUtensorMap& xmap,
                              const CUtensorMap& emap, const CUtensorMap& ymap, cudaStream_t st) {
     int dev = 0;
@@ -713,7 +696,7 @@ static int launch_persistent(Kern kern, const MmaArgs& a, const CUtensorMap& wma
         }
     }
     const int grid = a.num_tiles < sms ? a.num_tiles : sms;
-    kern<<<grid, kMmaThreads, kMmaSmemBytes, st>>>(a, wmap, xmap, emap, ymap);
+    kern<<<grid, kMmaThreads<WINDOW>, kMmaSmemBytes, st>>>(a, wmap, xmap, emap, ymap);
     if (cudaGetLastError() != cudaSuccess) return SDR_ERR_CUDA;
     return SDR_OK;
 }
@@ -745,16 +728,16 @@ int launch_pointwise_mma(const float* x, const NormIn& nin, const void* wpk, con
     const bool stats = stats_out != nullptr;
     CUtensorMap wmap, xmap, emap, ymap;
     if (int rc = make_weight_map(&wmap, wpk, pointwise_mma_packed_bytes(M, K))) return rc;
-    if (int rc = make_act_map(&xmap, x, samples, K, L, kTileM, CU_TENSOR_MAP_SWIZZLE_NONE)) return rc;
-    if (int rc = make_act_map(&ymap, y, samples, M, L, kEpiBoxL, CU_TENSOR_MAP_SWIZZLE_128B)) return rc;
+    if (int rc = make_act_map(&xmap, x, samples, K, L)) return rc;
+    if (int rc = make_act_map(&ymap, y, samples, M, L)) return rc;
     memset(&emap, 0, sizeof(emap));
     if (mode == 1)
-        if (int rc = make_act_map(&emap, residual, samples, M, L, kEpiBoxL, CU_TENSOR_MAP_SWIZZLE_128B)) return rc;
+        if (int rc = make_act_map(&emap, residual, samples, M, L)) return rc;
     if (mode == 2)
-        if (int rc = make_act_map(&emap, gate, samples, gate_channels, L, kEpiBoxL, CU_TENSOR_MAP_SWIZZLE_128B)) return rc;
+        if (int rc = make_act_map(&emap, gate, samples, gate_channels, L)) return rc;
 #define SDR_MMA_CASE(A, MD, ST)                                                                                   \
     if (act == A && mode == MD && stats == ST)                                                                    \
-        return launch_persistent(pw_mma_kernel<false, A, MD, ST>, a, wmap, xmap, emap, ymap, st);
+        return launch_persistent<false>(pw_mma_kernel<false, A, MD, ST>, a, wmap, xmap, emap, ymap, st);
     SDR_MMA_CASE(0, 0, false) SDR_MMA_CASE(0, 0, true)
     SDR_MMA_CASE(1, 0, false) SDR_MMA_CASE(1, 0, true)
     SDR_MMA_CASE(0, 1, false) SDR_MMA_CASE(0, 1, true)
@@ -801,8 +784,8 @@ int launch_encoder_mma(const float* wav, const void* wpk, const float* bias, int
     CUtensorMap wmap, none;
     if (int rc = make_weight_map(&wmap, wpk, encoder_mma_packed_bytes(N, A, Kk))) return rc;
     memset(&none, 0, sizeof(none));               // window mode gathers the waveform and writes enc itself
-    if (stats) return launch_persistent(pw_mma_kernel<true, 0, 0, true>, a, wmap, none, none, none, st);
-    return launch_persistent(pw_mma_kernel<true, 0, 0, false>, a, wmap, none, none, none, st);
+    if (stats) return launch_persistent<true>(pw_mma_kernel<true, 0, 0, true>, a, wmap, none, none, none, st);
+    return launch_persistent<true>(pw_mma_kernel<true, 0, 0, false>, a, wmap, none, none, none, st);
 }
 
 }  // namespace sdr

@@ -103,7 +103,7 @@ def pointwise(name, M, K, mode, samples=S):
         wpk = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         N.check(lib.sdr_pointwise_mma_pack(P(Wt), M, K, P(wpk), sp))
         keep.append(wpk)
-        timeit(name + " [tcgen05]", lambda: N.check(lib.sdr_pointwise_mma(
+        timeit(name + " [wgmma]", lambda: N.check(lib.sdr_pointwise_mma(
             P(x), C.byref(nin), P(wpk), P(bias), P(res), P(gate), NB, P(y),
             P(sto) if mode == "plain" else P(None), samples, M, K, L, epi, sp)), nb, fl)
     timeit(name + " [ffma]", lambda: N.check(lib.sdr_pointwise(
