@@ -124,6 +124,44 @@ int sdr_forward_host(const sdr_config* cfg, const void* packed,
                      void* dev_io, size_t dev_io_bytes,
                      void* workspace, size_t workspace_bytes, sdr_stream stream);
 
+/* ---- streaming of the causal model (variant 2) ---------------------------
+ * CausalSuDORMRF has no normalisation layers, so it can run chunk by chunk with
+ * a small carried state per slot and produce what model(x) produces on the
+ * concatenation, delayed by hop = enc_kernel_size / 2 samples:
+ *   cat(step(x_0) .. step(x_{n-1}))[..., hop:] == model(x)[..., :n*C - hop]
+ *   flush() == model(x)[..., n*C - hop : n*C]      when n*C % (hop * 2^depth) == 0
+ * (otherwise the reference's zero padding adds one more frame, and only the
+ * first identity holds).  The first hop samples of the first step are zeros.
+ *
+ * Granule G = hop * max(4, 2^(depth-1)) samples; a chunk C is a multiple of G
+ * of at most 4096 * hop samples.  The state ([B] slots; layout private, slots
+ * contiguous) and the step workspace are caller-allocated device buffers; the
+ * state must be zeroed by sdr_stream_reset before the first step.  Nothing
+ * synchronises, and a step can be captured in a CUDA graph.  Variants other
+ * than 2 and chunks that are not a multiple of G return SDR_ERR_UNSUPPORTED.  */
+int64_t sdr_stream_granule(const sdr_config* cfg);
+size_t  sdr_stream_state_bytes(const sdr_config* cfg, int B);
+size_t  sdr_stream_workspace_bytes(const sdr_config* cfg, int B, int64_t C);
+/* 3 * num_blocks + 6 kernels per step */
+int     sdr_stream_launch_count(const sdr_config* cfg, int B, int64_t C);
+/* zero every slot (host_slots_or_null = NULL) or the n slots listed (host array) */
+int     sdr_stream_reset(const sdr_config* cfg, void* state, int B, const int32_t* host_slots_or_null, int n,
+                         sdr_stream stream);
+/* chunk [B, A, C] -> out [B, S*A, C]: the model's output samples c*C - hop .. (c+1)*C - hop - 1 of the c-th step;
+ * apply_mixture_consistency: the uniform projection against the mixture delayed by hop (mono models only)      */
+int     sdr_stream_step(const sdr_config* cfg, const void* packed, void* state, const float* chunk, float* out,
+                        int B, int64_t C, int apply_mixture_consistency, void* ws, size_t ws_bytes, sdr_stream stream);
+/* tail [B, S*A, hop]: the pending overlap-add sums; the state is left as it is */
+int     sdr_stream_flush(const sdr_config* cfg, void* state, float* tail, int B, int apply_mixture_consistency,
+                         sdr_stream stream);
+/* The stream stage of one causal U-ConvBlock: the depthwise pyramid of sdr_causal_pyramid over one chunk of F
+ * frames per slot, with the last 10 inputs of every level carried in history [B][D][10][C] (zero to start).
+ * y, m [C][B*F] (columns slot-major); m is bitwise what sdr_causal_pyramid computes over the concatenated chunks.
+ * F % 4 == 0, F % 2^(D-1) == 0 and F <= 4096, else SDR_ERR_UNSUPPORTED.                                      */
+int     sdr_causal_stream_stage(const float* y, const float* slope_in, const float* const* w21,
+                                const float* const* bias, const float* const* slope, float* history, float* m,
+                                int D, int B, int C, int F, sdr_stream stream);
+
 /* mixture_consistency.apply (mixture_consistency.py:14-36).
  * weights_type: 0 = 'uniform', 1 = 'magsq'.  est/out [B,S,T], mix [B,1,T].
  * `scratch` (device, >= B*S doubles) is only used by 'magsq'.               */

@@ -60,6 +60,17 @@ _SIGNATURES = {
     "sdr_forward_host": (C.c_int, [C.POINTER(SdrConfig), C.c_void_p, C.c_void_p, C.c_void_p,
                                    C.c_int, C.c_int64, C.c_int, C.c_void_p, C.c_size_t,
                                    C.c_void_p, C.c_size_t, C.c_void_p]),
+    "sdr_stream_granule": (C.c_int64, [C.POINTER(SdrConfig)]),
+    "sdr_stream_state_bytes": (C.c_size_t, [C.POINTER(SdrConfig), C.c_int]),
+    "sdr_stream_workspace_bytes": (C.c_size_t, [C.POINTER(SdrConfig), C.c_int, C.c_int64]),
+    "sdr_stream_launch_count": (C.c_int, [C.POINTER(SdrConfig), C.c_int, C.c_int64]),
+    "sdr_stream_reset": (C.c_int, [C.POINTER(SdrConfig), C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]),
+    "sdr_stream_step": (C.c_int, [C.POINTER(SdrConfig), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                  C.c_int64, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "sdr_stream_flush": (C.c_int, [C.POINTER(SdrConfig), C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
+    "sdr_causal_stream_stage": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(C.c_void_p), C.POINTER(C.c_void_p),
+                                          C.POINTER(C.c_void_p), C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                          C.c_int, C.c_void_p]),
     "sdr_mixture_consistency": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                           C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
     "sdr_encoder": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,

@@ -126,6 +126,12 @@ class CausalSuDORMRF(_engine.NativeModuleMixin, nn.Module):
         """End-to-end call on pinned HOST tensors (H2D, forward, D2H on the current stream)."""
         return _engine.forward_host(self, host_wav, host_out, mixture_consistency)
 
+    def stream(self, batch_size, chunk_samples, mixture_consistency=False):
+        """A ``streaming.CausalStream`` of ``batch_size`` slots taking ``chunk_samples`` samples per step (a multiple
+        of ``hop * max(4, 2**(upsampling_depth - 1))``); its output is ``forward``'s, delayed by ``hop`` samples."""
+        from .streaming import CausalStream
+        return CausalStream(self, batch_size, chunk_samples, mixture_consistency=mixture_consistency)
+
     def pad_to_appropriate_length(self, x):
         """Reference :213-224 (device-side; the native encoder pads implicitly)."""
         T = x.shape[-1]

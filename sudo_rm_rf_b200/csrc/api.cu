@@ -38,6 +38,14 @@ int launch_causal_pyramid(const float*, const float*, const float* const*, const
                           int, int, int, int, cudaStream_t);
 int launch_take_taps(const float*, float*, long long, int, int, cudaStream_t);
 int launch_scale_by_scalar(const float*, const float*, float*, long long, cudaStream_t);
+// streaming of the causal model (stream.cu)
+bool causal_stream_eligible(int D, int F);
+int launch_stream_frame(const float*, const float*, long long, float*, int, int, int, int, int, long long, cudaStream_t);
+int launch_causal_stream(const float*, const float*, const float* const*, const float* const*, const float* const*,
+                         float*, long long, float*, int, int, int, int, cudaStream_t);
+int launch_stream_ola(const float*, const float*, float*, long long, long long, float*, int, int, int, int, int,
+                      long long, int, cudaStream_t);
+int launch_stream_flush(const float*, long long, long long, float*, int, int, int, int, cudaStream_t);
 // original model (original.cu)
 int launch_residual_norm(const float*, const NormIn&, float*, const NormIn&, double*, int, int, int, cudaStream_t);
 int launch_softmax_gate(const float*, const float*, float*, int, int, int, int, cudaStream_t);
@@ -437,6 +445,109 @@ static int forward_causal(const Layout& l, const Plan& p, const float* pk, const
     return decoder_tail(l, p, pk, pn, nullptr, mixture, apply_mc, rescale, out, B, T, ws, st);
 }
 
+// ---------------------------------------------------------------------------
+// streaming of the causal model (stream.cu): state layout, step plan and orchestration
+// ---------------------------------------------------------------------------
+// Chunk granule: a multiple of 4 frames (float4 rows) that starts every level's chunk on an integer position.
+static long long stream_granule(const Layout& l) {
+    return (long long)l.hop * (1 << (l.D - 1) > 4 ? 1 << (l.D - 1) : 4);
+}
+
+// Per-slot state, in floats: waveform context [A][2 hop], decoder carry [S*A][hop + 1], a flag set by the slot's
+// first step, level histories [U][D][10][Ci]; slots are 256 B apart so that a slot's state is one contiguous range.
+struct StreamState { size_t ctx, carry, hist, slot; };
+static StreamState stream_state(const Layout& l) {
+    StreamState s;
+    s.ctx = 0;
+    s.carry = (size_t)l.A * 2 * l.hop;
+    s.hist = (s.carry + (size_t)l.S * l.A * (l.hop + 1) + 1 + 3) & ~(size_t)3;
+    s.slot = (s.hist + (size_t)l.U * l.D * 10 * l.Ci + 63) & ~(size_t)63;
+    return s;
+}
+
+// Workspace of one step: every activation is [channels][B*F] with columns (slot, frame).
+struct StreamPlan {
+    int F, BF, Kr;                             // Kr: rows of the encoder operand (taps padded to a k-block for the image)
+    size_t o_framed, o_e, o_x, o_y, o_m, o_masked, o_frames, total;   // bytes
+    float* buf(char* ws, size_t o) const { return reinterpret_cast<float*>(ws + o); }
+};
+static StreamPlan make_stream_plan(const Layout& l, int B, long long C) {
+    StreamPlan p;
+    p.F = (int)(C / l.hop);
+    p.BF = B * p.F;
+    p.Kr = l.enc_pk ? (l.A * l.K + 63) / 64 * 64 : l.A * l.K;
+    size_t cur = 0;
+    auto seg = [&](size_t rows) { size_t o = cur; cur += (rows * p.BF * sizeof(float) + 255) & ~(size_t)255; return o; };
+    p.o_framed = seg(p.Kr);
+    p.o_e = seg(l.N);
+    p.o_x = seg(l.Co);
+    p.o_y = seg(l.Ci);
+    p.o_m = seg(l.Ci);
+    p.o_masked = seg((size_t)l.S * l.A * l.N);
+    p.o_frames = seg((size_t)l.S * l.A * l.K);
+    p.total = cur;
+    return p;
+}
+
+static int check_stream_config(const Layout& l) {
+    if (!l.ok) return SDR_ERR_BAD_CONFIG;
+    if (!l.causal) return SDR_ERR_UNSUPPORTED;         // GlobLN / GroupNorm statistics span the whole clip
+    if (2 * l.hop + 2 > 256) return SDR_ERR_UNSUPPORTED;
+    return SDR_OK;
+}
+
+static int check_stream_args(const Layout& l, int B, long long C) {
+    SDR_TRY(check_stream_config(l));
+    if (B <= 0 || B > 65535 || C <= 0) return SDR_ERR_BAD_ARGUMENT;
+    if (C % stream_granule(l)) return SDR_ERR_UNSUPPORTED;
+    const long long F = C / l.hop;
+    if (!causal_stream_eligible(l.D, (int)(F < 0x7fffffffLL ? F : 0)) || (long long)B * F > 0x7fffffffLL)
+        return SDR_ERR_UNSUPPORTED;
+    return SDR_OK;
+}
+
+// One step: framing, encoder, bottleneck, U x (proj, stream stage, res_conv), mask, decoder, overlap-add.
+static int stream_step(const Layout& l, const StreamPlan& p, const float* pk, float* state, const float* chunk,
+                       float* out, int B, long long C, int apply_mc, char* ws, cudaStream_t st) {
+    const StreamState ss = stream_state(l);
+    const int BF = p.BF, D = l.D, SA = l.S * l.A;
+    float* framed = p.buf(ws, p.o_framed);
+    float* e = p.buf(ws, p.o_e);
+    float* x = p.buf(ws, p.o_x);
+    float* y = p.buf(ws, p.o_y);
+    float* m = p.buf(ws, p.o_m);
+    float* masked = p.buf(ws, p.o_masked);
+    float* frames = p.buf(ws, p.o_frames);
+    const NormIn none{nullptr, nullptr, nullptr, nullptr, 1.0, 0};
+    SDR_TRY(launch_stream_frame(chunk, state, (long long)ss.slot, framed, B, l.A, l.K, p.Kr, p.F, C, st));
+    if (l.enc_pk)                                      // the window encoder's image is a plain [N][Kr] GEMM image
+        SDR_TRY(launch_pointwise_mma(framed, none, pk + l.enc_pk, nullptr, nullptr, nullptr, 0, e, nullptr,
+                                     1, l.N, p.Kr, BF, 0, st));
+    else
+        SDR_TRY(launch_pointwise_ffma(framed, none, pk + l.enc_src, nullptr, nullptr, nullptr, 0, e, nullptr,
+                                      1, l.N, l.A * l.K, BF, 0, st));
+    SDR_TRY(pointwise(e, none, pk, l.bn_w, l.bn_pk, pk + l.bn_b, nullptr, nullptr, 0, x, nullptr, 1, l.Co, l.N, BF, 0, st));
+    for (int i = 0; i < l.U; ++i) {
+        const CausalBlockOff& u = l.cb[i];
+        SDR_TRY(pointwise(x, none, pk, u.proj_w, u.proj_pk, pk + u.proj_b, nullptr, nullptr, 0,
+                          y, nullptr, 1, l.Ci, l.Co, BF, 0, st));
+        const float *w[kMaxDepthApi], *b[kMaxDepthApi], *a[kMaxDepthApi];
+        for (int d = 0; d < D; ++d) { w[d] = pk + u.dw_w[d]; b[d] = pk + u.dw_b[d]; a[d] = pk + u.dw_a[d]; }
+        SDR_TRY(launch_causal_stream(y, pk + u.proj_a, w, b, a, state + ss.hist + (size_t)i * D * 10 * l.Ci,
+                                     (long long)ss.slot, m, D, B, l.Ci, p.F, st));
+        SDR_TRY(pointwise(m, none, pk, u.res_wg, u.res_pk, pk + u.res_bg, x, nullptr, 0,
+                          x, nullptr, 1, l.Co, l.Ci, BF, 0, st));
+    }
+    const NormIn pm{nullptr, nullptr, nullptr, pk + l.mask_a, 1.0, 0};
+    SDR_TRY(pointwise(x, pm, pk, l.mask_w, l.mask_pk, pk + l.mask_b, nullptr, nullptr, 0,
+                      masked, nullptr, 1, SA * l.N, l.Co, BF, 0, st));
+    const NormIn pn{nullptr, nullptr, nullptr, pk + l.mask_nl, 1.0, 0};
+    SDR_TRY(pointwise(masked, pn, pk, l.dec_wt, l.dec_pk, nullptr, nullptr, nullptr, 0,
+                      frames, nullptr, 1, SA * l.K, SA * l.N, BF, 0, st));
+    return launch_stream_ola(frames, chunk, state, (long long)ss.slot, (long long)ss.carry, out, B, SA, l.A, l.K, p.F, C,
+                             apply_mc, st);
+}
+
 // The original SuDORMRF.forward (sudormrf.py:266-292; UBlock.forward :164-186).
 static int forward_original(const Layout& l, const Plan& p, const float* pk, const float* mixture, float* out,
                             int B, long long T, int apply_mc, char* ws, cudaStream_t st, const float2* rescale) {
@@ -686,6 +797,83 @@ int sdr_forward_launch_count_for(const sdr_config* cfg, int B, int64_t T) {
     const Layout l = make_layout(cfg);
     if (!l.ok || B <= 0 || T <= 0) return SDR_ERR_BAD_CONFIG;
     return launch_count(l, make_plan(l, B, T));
+}
+
+// ---- streaming of the causal model ----
+
+int64_t sdr_stream_granule(const sdr_config* cfg) {
+    const Layout l = make_layout(cfg);
+    SDR_TRY(check_stream_config(l));
+    return stream_granule(l);
+}
+
+size_t sdr_stream_state_bytes(const sdr_config* cfg, int B) {
+    const Layout l = make_layout(cfg);
+    if (check_stream_config(l) != SDR_OK || B <= 0) return 0;
+    return (size_t)B * stream_state(l).slot * sizeof(float);
+}
+
+size_t sdr_stream_workspace_bytes(const sdr_config* cfg, int B, int64_t C) {
+    const Layout l = make_layout(cfg);
+    if (check_stream_args(l, B, C) != SDR_OK) return 0;
+    return make_stream_plan(l, B, C).total;
+}
+
+int sdr_stream_launch_count(const sdr_config* cfg, int B, int64_t C) {
+    const Layout l = make_layout(cfg);
+    SDR_TRY(check_stream_args(l, B, C));
+    return 3 * l.U + 6;                // framing, encoder, bottleneck, U x (proj, stream stage, res), mask, decoder, overlap-add
+}
+
+int sdr_stream_reset(const sdr_config* cfg, void* state, int B, const int32_t* host_slots_or_null, int n,
+                     sdr_stream stream) {
+    const Layout l = make_layout(cfg);
+    SDR_TRY(check_stream_config(l));
+    if (!state || B <= 0 || (host_slots_or_null && n < 0)) return SDR_ERR_BAD_ARGUMENT;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const size_t slot = stream_state(l).slot * sizeof(float);
+    if (!host_slots_or_null)
+        return cudaMemsetAsync(state, 0, (size_t)B * slot, st) == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    for (int i = 0; i < n; ++i)
+        if (host_slots_or_null[i] < 0 || host_slots_or_null[i] >= B) return SDR_ERR_BAD_ARGUMENT;
+    for (int i = 0; i < n; ++i)
+        if (cudaMemsetAsync(static_cast<char*>(state) + (size_t)host_slots_or_null[i] * slot, 0, slot, st) != cudaSuccess)
+            return SDR_ERR_CUDA;
+    return SDR_OK;
+}
+
+int sdr_stream_step(const sdr_config* cfg, const void* packed, void* state, const float* chunk, float* out, int B,
+                    int64_t C, int apply_mixture_consistency, void* ws, size_t ws_bytes, sdr_stream stream) {
+    const Layout l = make_layout(cfg);
+    SDR_TRY(check_stream_args(l, B, C));
+    if (apply_mixture_consistency && l.A != 1) return SDR_ERR_UNSUPPORTED;
+    if (!packed || !state || !chunk || !out || !ws) return SDR_ERR_BAD_ARGUMENT;
+    const StreamPlan p = make_stream_plan(l, B, C);
+    if (ws_bytes < p.total) return SDR_ERR_WORKSPACE;
+    if (reinterpret_cast<uintptr_t>(ws) % 256 || reinterpret_cast<uintptr_t>(packed) % 16 ||
+        reinterpret_cast<uintptr_t>(state) % 16)
+        return SDR_ERR_BAD_ARGUMENT;
+    return stream_step(l, p, static_cast<const float*>(packed), static_cast<float*>(state), chunk, out, B, C,
+                       apply_mixture_consistency, static_cast<char*>(ws), static_cast<cudaStream_t>(stream));
+}
+
+int sdr_stream_flush(const sdr_config* cfg, void* state, float* tail, int B, int apply_mixture_consistency,
+                     sdr_stream stream) {
+    const Layout l = make_layout(cfg);
+    SDR_TRY(check_stream_config(l));
+    if (apply_mixture_consistency && l.A != 1) return SDR_ERR_UNSUPPORTED;
+    if (!state || !tail || B <= 0) return SDR_ERR_BAD_ARGUMENT;
+    const StreamState ss = stream_state(l);
+    return launch_stream_flush(static_cast<const float*>(state), (long long)ss.slot, (long long)ss.carry, tail, B,
+                               l.S * l.A, l.hop, apply_mixture_consistency, static_cast<cudaStream_t>(stream));
+}
+
+int sdr_causal_stream_stage(const float* y, const float* slope_in, const float* const* w21, const float* const* bias,
+                            const float* const* slope, float* history, float* m, int D, int B, int C, int F,
+                            sdr_stream stream) {
+    if (D < 1 || D > kMaxDepthApi) return SDR_ERR_UNSUPPORTED;
+    return launch_causal_stream(y, slope_in, w21, bias, slope, history, (long long)D * 10 * C, m, D, B, C, F,
+                                static_cast<cudaStream_t>(stream));
 }
 
 // Byte offsets of the buffers either side of the forward.  sdr_forward_host stages the mixture at 0 and the estimates

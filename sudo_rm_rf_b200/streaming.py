@@ -1,0 +1,123 @@
+"""Chunk-by-chunk inference of ``CausalSuDORMRF`` (variant 2 of ``include/sudormrf_b200.h``).
+
+Every convolution of the causal model is causally masked and it has no normalisation layers, so a stream that
+carries a small state per slot (the last input samples, the last inputs of every depthwise level, the pending
+overlap-add sums) produces exactly what ``model(x)`` produces on the concatenated audio, delayed by
+``hop = enc_kernel_size // 2`` samples::
+
+    cat(step(x_0), ..., step(x_{n-1}))[..., hop:] == model(x)[..., :n*C - hop]
+    flush() == model(x)[..., n*C - hop:n*C]          when n*C is a multiple of hop * 2**upsampling_depth
+
+A step costs the same whatever has been streamed before.  The other variants normalise over the whole clip and
+cannot be streamed.
+"""
+from __future__ import annotations
+
+import ctypes as C
+from typing import Iterable, Optional
+
+import torch
+
+from . import _engine
+from . import _native as N
+
+
+class CausalStream:
+    """``batch_size`` independent streams (slots) of ``chunk_samples`` samples per step.
+
+    Owns its state and step workspace, apart from the model's forward workspace, so ``model(x)`` and open streams
+    can interleave.  Every step reads the model's weights through the same packed-weight cache as ``forward``, so
+    changed weights are picked up on the next step.  Steps run on the current CUDA stream, never synchronise and can
+    be captured in a CUDA graph (``step(chunk, out=...)`` with fixed buffers)."""
+
+    def __init__(self, model, batch_size: int, chunk_samples: int, mixture_consistency: bool = False):
+        lib = N.lib()
+        cfg = _engine.make_config(model)
+        if cfg.variant != 2:
+            raise RuntimeError("only CausalSuDORMRF can be streamed: the other models normalise over the whole clip")
+        device = _engine._fetch(model, "encoder.weight").device
+        if device.type != "cuda":
+            raise RuntimeError("sudo_rm_rf_b200 streams on CUDA (sm_90a) only and has no CPU path: move the model "
+                               "to an H100 (`model.cuda()`)")
+        if device.index is None:
+            device = torch.device("cuda", torch.cuda.current_device())
+        granule = lib.sdr_stream_granule(C.byref(cfg))
+        if granule < 0:
+            N.check(int(granule), "sdr_stream_granule")
+        B, Cs = int(batch_size), int(chunk_samples)
+        if B <= 0 or Cs <= 0 or Cs % granule:
+            raise ValueError(f"chunk_samples must be a positive multiple of the granule ({granule} samples) and "
+                             f"batch_size positive; got batch_size={batch_size}, chunk_samples={chunk_samples}")
+        if mixture_consistency and cfg.in_audio_channels != 1:
+            raise RuntimeError("mixture consistency (mixture_consistency.py:14-36) is defined for mono mixtures only; "
+                               f"this model has in_audio_channels={cfg.in_audio_channels}")
+        ws_bytes = lib.sdr_stream_workspace_bytes(C.byref(cfg), B, Cs)
+        if ws_bytes == 0:
+            raise ValueError(f"chunk_samples={Cs} is longer than a step takes (at most {4096 * (cfg.enc_kernel_size // 2)})")
+        self.model = model
+        self.device = device
+        self.batch_size = B
+        self.chunk_samples = Cs
+        self.granule = int(granule)
+        self.latency = cfg.enc_kernel_size // 2
+        self.mixture_consistency = bool(mixture_consistency)
+        self._cfg = cfg
+        self._state = torch.empty(lib.sdr_stream_state_bytes(C.byref(cfg), B), dtype=torch.uint8, device=device)
+        self._ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+        self.reset()
+
+    def _stream_ptr(self):
+        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
+
+    def reset(self, slots: Optional[Iterable[int]] = None) -> None:
+        """Start slots over (all of them when ``slots`` is None): their next step is the start of a new stream."""
+        lib = N.lib()
+        with torch.cuda.device(self.device):
+            if slots is None:
+                rc = lib.sdr_stream_reset(C.byref(self._cfg), C.c_void_p(self._state.data_ptr()), self.batch_size,
+                                          None, 0, self._stream_ptr())
+            else:
+                idx = [int(s) for s in slots]
+                if any(s < 0 or s >= self.batch_size for s in idx):
+                    raise IndexError(f"slots {idx} out of range for batch_size={self.batch_size}")
+                arr = (C.c_int32 * max(1, len(idx)))(*idx)
+                rc = lib.sdr_stream_reset(C.byref(self._cfg), C.c_void_p(self._state.data_ptr()), self.batch_size,
+                                          arr, len(idx), self._stream_ptr())
+            N.check(rc, "sdr_stream_reset")
+
+    def step(self, chunk: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
+        """[B, A, C] chunk -> [B, S*A, C] estimates of the model's output samples ``c*C - hop .. (c+1)*C - hop - 1``."""
+        lib = N.lib()
+        cfg = self._cfg
+        x = _engine._check_input(self.model, cfg, chunk)
+        B, Cs = self.batch_size, self.chunk_samples
+        if x.shape[0] != B or x.shape[2] != Cs:
+            raise RuntimeError(f"expected a chunk of shape [{B}, {cfg.in_audio_channels}, {Cs}], got {list(chunk.shape)}")
+        if x.device != self.device:
+            raise RuntimeError(f"chunk is on {x.device}, the stream on {self.device}")
+        SA = cfg.num_sources * cfg.in_audio_channels
+        if out is None:
+            out = torch.empty((B, SA, Cs), dtype=torch.float32, device=self.device)
+        elif tuple(out.shape) != (B, SA, Cs) or out.dtype != torch.float32 or out.device != self.device \
+                or not out.is_contiguous():
+            raise RuntimeError(f"out must be a contiguous fp32 tensor [{B}, {SA}, {Cs}] on {self.device}")
+        with torch.cuda.device(self.device):
+            packed = _engine.packed_weights(self.model, cfg, self.device)
+            N.check(lib.sdr_stream_step(C.byref(cfg), C.c_void_p(packed.data_ptr()), C.c_void_p(self._state.data_ptr()),
+                                        C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()), B, Cs,
+                                        1 if self.mixture_consistency else 0, C.c_void_p(self._ws.data_ptr()),
+                                        self._ws.numel(), self._stream_ptr()), "sdr_stream_step")
+        return out
+
+    def flush(self) -> torch.Tensor:
+        """[B, S*A, hop]: the last ``hop`` output samples, which only the end of the stream completes.  The state is
+        left as it is; ``reset()`` starts the slots over."""
+        lib = N.lib()
+        cfg = self._cfg
+        tail = torch.empty((self.batch_size, cfg.num_sources * cfg.in_audio_channels, self.latency),
+                           dtype=torch.float32, device=self.device)
+        with torch.cuda.device(self.device):
+            N.check(lib.sdr_stream_flush(C.byref(cfg), C.c_void_p(self._state.data_ptr()), C.c_void_p(tail.data_ptr()),
+                                         self.batch_size, 1 if self.mixture_consistency else 0, self._stream_ptr()),
+                    "sdr_stream_flush")
+        return tail
