@@ -21,6 +21,9 @@ import torch
 from . import _engine
 from . import _native as N
 
+MAX_SLOTS = 65535            # slots per step (one grid row per slot, include/sudormrf_b200.h)
+MAX_CHUNK_FRAMES = 4096      # encoder frames per slot and step, i.e. chunk_samples <= 4096 * hop
+
 
 class CausalStream:
     """``batch_size`` independent streams (slots) of ``chunk_samples`` samples per step.
@@ -35,25 +38,32 @@ class CausalStream:
         cfg = _engine.make_config(model)
         if cfg.variant != 2:
             raise RuntimeError("only CausalSuDORMRF can be streamed: the other models normalise over the whole clip")
+        granule = lib.sdr_stream_granule(C.byref(cfg))
+        if granule < 0:
+            N.check(int(granule), "sdr_stream_granule")
+        # the arguments are checked before the device, so that each refusal names the limit it hit
+        B, Cs = int(batch_size), int(chunk_samples)
+        if B <= 0 or B > MAX_SLOTS:
+            raise ValueError(f"batch_size={batch_size} is outside the slots a step takes (1 .. {MAX_SLOTS})")
+        if Cs <= 0 or Cs % granule:
+            raise ValueError(f"chunk_samples must be a positive multiple of the granule ({granule} samples); "
+                             f"got chunk_samples={chunk_samples}")
+        max_chunk = MAX_CHUNK_FRAMES * (cfg.enc_kernel_size // 2)
+        if Cs > max_chunk:
+            raise ValueError(f"chunk_samples={Cs} is longer than a step takes (at most {max_chunk} samples: "
+                             f"{MAX_CHUNK_FRAMES} frames of hop {cfg.enc_kernel_size // 2})")
+        if mixture_consistency and cfg.in_audio_channels != 1:
+            raise RuntimeError("mixture consistency (mixture_consistency.py:14-36) is defined for mono mixtures only; "
+                               f"this model has in_audio_channels={cfg.in_audio_channels}")
+        ws_bytes = lib.sdr_stream_workspace_bytes(C.byref(cfg), B, Cs)
+        if ws_bytes == 0:
+            raise ValueError(f"sdr_stream_workspace_bytes refused batch_size={B}, chunk_samples={Cs}")
         device = _engine._fetch(model, "encoder.weight").device
         if device.type != "cuda":
             raise RuntimeError("sudo_rm_rf_b200 streams on CUDA (sm_90a) only and has no CPU path: move the model "
                                "to an H100 (`model.cuda()`)")
         if device.index is None:
             device = torch.device("cuda", torch.cuda.current_device())
-        granule = lib.sdr_stream_granule(C.byref(cfg))
-        if granule < 0:
-            N.check(int(granule), "sdr_stream_granule")
-        B, Cs = int(batch_size), int(chunk_samples)
-        if B <= 0 or Cs <= 0 or Cs % granule:
-            raise ValueError(f"chunk_samples must be a positive multiple of the granule ({granule} samples) and "
-                             f"batch_size positive; got batch_size={batch_size}, chunk_samples={chunk_samples}")
-        if mixture_consistency and cfg.in_audio_channels != 1:
-            raise RuntimeError("mixture consistency (mixture_consistency.py:14-36) is defined for mono mixtures only; "
-                               f"this model has in_audio_channels={cfg.in_audio_channels}")
-        ws_bytes = lib.sdr_stream_workspace_bytes(C.byref(cfg), B, Cs)
-        if ws_bytes == 0:
-            raise ValueError(f"chunk_samples={Cs} is longer than a step takes (at most {4096 * (cfg.enc_kernel_size // 2)})")
         self.model = model
         self.device = device
         self.batch_size = B

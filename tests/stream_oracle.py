@@ -30,6 +30,10 @@ class CausalStreamOracle:
         self.carry = torch.zeros(batch, SA, hop + 1, dtype=dtype)
         self.started = False
 
+    def set_weights(self, sd):
+        """New weights from the next step on (the state is kept), as a stream picks up a model's changed weights."""
+        self.sd = {k: v.to(self.dtype) for k, v in sd.items()}
+
     def _block(self, x, i):
         sd, p, D = self.sd, f"sm.{i}.", self.cfg.upsampling_depth
         Ci = sd[p + "proj_1x1.conv.weight"].shape[0]

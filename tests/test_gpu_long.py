@@ -222,8 +222,10 @@ def causal_window_starts(D, L):
     return list(range(0, L, W))
 
 
-# L = 16000 / 32000: 4 / 8 windows (10 / 20 s at 16 kHz); 28736: 8 windows, the last one 2752 frames at D = 6
-CAUSAL_PARAMS = [(D, L) for L in (16000, 28736, 32000) for D in range(1, 7)]
+# L = 16000 / 32000: 4 / 8 windows (10 / 20 s at 16 kHz); 28736: 8 windows, the last one 2752 frames at D = 6.
+# D = 7, 8 (left halo 756 / 1524 frames): 16384 and 32000, 4 and 8 windows (28736 does not halve 7 times)
+CAUSAL_PARAMS = [(D, L) for L in (16000, 28736, 32000) for D in range(1, 7)] + \
+                [(D, L) for L in (16384, 32000) for D in (7, 8)]
 
 
 @pytest.mark.gpu

@@ -1,5 +1,6 @@
 """Streaming of CausalSuDORMRF on the GPU: the concatenated steps against the fp64 oracle and the native offline
-forward, the stream stage kernel against the one-pass causal pyramid, slot independence, reset, CUDA-graph replay,
+forward, the stream stage kernel against the one-pass causal pyramid and an fp64 chain at every depth and at each
+channels-per-CTA width it picks, slot independence, reset, CUDA-graph replay,
 mixture consistency, the launch count and argument errors.
 
 Contract (model output delayed by hop samples):
@@ -103,10 +104,43 @@ def test_small_model_on_ffma_kernels():
         check_against_forward(cfg, sd, m, x, g * granule(cfg))
 
 
-# ---- the stream stage alone against the one-pass causal pyramid ----
-def _stage_case(D, F, B, Cc=40):
+# ---- the stream stage alone against the one-pass causal pyramid and an fp64 chain ----
+def stage_rows(D, F):
+    """(R, dynamic shared memory) that launch_causal_stream (stream.cu) picks: every level's buffer holds 10 history
+    values and its new inputs, pos = sum_d (10 + nin_d) + (F >> (D-1)) floats per channel, and R = 32 channels per CTA
+    halve while R * pos floats exceed 48 KB (down to R = 1, which asks for more than 48 KB at D = 7 and 8, F = 4096)."""
+    pos = sum(10 + (F if d == 0 else F >> (d - 1)) for d in range(D)) + (F >> (D - 1))
+    R = 32
+    while R > 1 and R * pos * 4 > 48 * 1024:
+        R //= 2
+    return R, R * pos * 4
+
+
+def first_chunk_with_rows(D, R):
+    """The shortest chunk (frames) at which the stage runs R channels per CTA, None if no chunk does."""
+    gran = max(4, 2 ** (D - 1))
+    return next((F for F in range(gran, 4097, gran) if stage_rows(D, F)[0] == R), None)
+
+
+def stage_reference(y, slope_in, w, bias, sl):
+    """fp64 PReLU -> D x (causally masked 21-tap depthwise conv + PReLU) -> nearest up-sampling and skip adds."""
+    Cc = y.shape[1]
+    cur = O.prelu1(y.double(), slope_in.double())
+    levels = []
+    for d in range(len(w)):
+        cur = O.prelu1(torch.nn.functional.conv1d(cur, O.causal_weight(w[d].double()), bias[d].double(),
+                                                  stride=1 if d == 0 else 2, padding=10, groups=Cc), sl[d].double())
+        levels.append(cur)
+    for _ in range(len(w) - 1):
+        top = levels.pop()
+        levels[-1] = levels[-1] + torch.nn.functional.interpolate(top, scale_factor=2, mode="nearest")
+    return levels[0]
+
+
+def _stage_case(D, F, B, Cc=40, n=6):
+    """n chunks of F frames: six turn the deepest level's history over completely at the granule (2 new inputs per
+    chunk, 4 at D = 1), and an even count keeps the concatenation a multiple of 2^D for sdr_causal_pyramid."""
     g = torch.Generator().manual_seed(D * 1000 + F + B)
-    n = 2                                       # two chunks: L = 2F halves exactly D times
     L = n * F
     y = torch.randn(B, Cc, L, generator=g).to(DEV)
     w = [(torch.randn(Cc, 1, 21, generator=g) / 3).to(DEV) for _ in range(D)]
@@ -120,36 +154,75 @@ def _stage_case(D, F, B, Cc=40):
     ref = torch.empty_like(y)
     N.check(lib.sdr_causal_pyramid(C.c_void_p(y.data_ptr()), C.c_void_p(slope_in.data_ptr()), ptrs(w), ptrs(bias),
                                    ptrs(sl), C.c_void_p(ref.data_ptr()), D, B, Cc, L, None), "sdr_causal_pyramid")
+    ref64 = stage_reference(y, slope_in, w, bias, sl)
     gd = Guards()
     hist = gd.output("history", torch.zeros(B, D, 10, Cc, device=DEV))
     wg = [gd.input(f"w{d}", w[d]) for d in range(D)]
+    bg = [gd.input(f"b{d}", bias[d]) for d in range(D)]
+    sg = [gd.input(f"slope{d}", sl[d]) for d in range(D)]
+    sin = gd.input("slope_in", slope_in)
+    err = 0.0
     for c in range(n):
         yc = gd.input(f"y{c}", y[..., c * F:(c + 1) * F].permute(1, 0, 2).reshape(Cc, B * F))
-        mc = gd.output(f"m{c}", torch.zeros(Cc, B * F, device=DEV))
-        N.check(lib.sdr_causal_stream_stage(C.c_void_p(yc.data_ptr()), C.c_void_p(slope_in.data_ptr()), ptrs(wg),
-                                            ptrs(bias), ptrs(sl), C.c_void_p(hist.data_ptr()), C.c_void_p(mc.data_ptr()),
+        mc = gd.output(f"m{c}", torch.full((Cc, B * F), float("nan"), device=DEV))
+        N.check(lib.sdr_causal_stream_stage(C.c_void_p(yc.data_ptr()), C.c_void_p(sin.data_ptr()), ptrs(wg),
+                                            ptrs(bg), ptrs(sg), C.c_void_p(hist.data_ptr()), C.c_void_p(mc.data_ptr()),
                                             D, B, Cc, F, None), "sdr_causal_stream_stage")
         gd.check()
         got = mc.reshape(Cc, B, F).permute(1, 0, 2)
         want = ref[..., c * F:(c + 1) * F]
         assert torch.equal(got, want), (D, F, B, c, float((got - want).abs().max()))
+        e = O.parity_errors(got, ref64[..., c * F:(c + 1) * F])
+        err = max(err, *e)
+        assert max(e) < 2e-5, (D, F, B, c, e)
+    R, smem = stage_rows(D, F)
+    print(f"stage D={D} F={F} B={B} C={Cc}: R={R} smem={smem} B, {n} chunks bitwise == sdr_causal_pyramid, "
+          f"vs fp64 chain {err:.2e}")
     return lib
 
 
-@pytest.mark.parametrize("D", [1, 4, 5, 6])
-@pytest.mark.parametrize("F", ["granule", "twice", "max"])
-@pytest.mark.parametrize("B", [1, 3, 130])
-def test_stream_stage_bitwise_vs_pyramid(D, F, B):
+STAGE_CHANNELS = {1: 40, 3: 37, 130: 5}     # 37: a partial CTA at every R >= 2; 5: fewer channels than one CTA's R
+
+
+def stage_cases():
+    """(D, chunk kind, F, B): the granule, twice, thrice it and 4096 frames at 1, 3 and 130 slots; at 3 slots, the
+    shortest chunk at which the host picks each R that is not the granule's."""
+    cases = []
+    for B in (1, 3, 130):
+        for kind in ("granule", "twice", "max", "thrice", "R32", "R16", "R8", "R4", "R2", "R1"):
+            for D in (1, 4, 5, 6, 2, 3, 7, 8):
+                gran = max(4, 2 ** (D - 1))
+                if kind.startswith("R"):
+                    F = first_chunk_with_rows(D, int(kind[1:]))
+                    if B != 3 or F is None or F == gran:
+                        continue
+                else:
+                    F = {"granule": gran, "twice": 2 * gran, "thrice": 3 * gran, "max": 4096}[kind]
+                cases.append(pytest.param(D, kind, F, B, id=f"{B}-{kind}-{D}"))
+    return cases
+
+
+@pytest.mark.parametrize("D,F_kind,F,B", stage_cases())
+def test_stream_stage_bitwise_vs_pyramid(D, F_kind, F, B):
     gran = max(4, 2 ** (D - 1))
-    Fv = {"granule": gran, "twice": 2 * gran, "max": 4096}[F]
-    if F == "max" and B == 130 and D != 4:
-        pytest.skip("the longest chunk at 130 slots once (D = 4) is enough")
-    lib = _stage_case(D, Fv, B)
-    if F == "max":
+    if F_kind.startswith("R"):
+        assert stage_rows(D, F)[0] == int(F_kind[1:]) and stage_rows(D, F - gran)[0] != int(F_kind[1:])
+    lib = _stage_case(D, F, B, Cc=STAGE_CHANNELS[B])
+    if F_kind == "max":
+        assert stage_rows(D, 4096)[1] > 48 * 1024 if D >= 7 else stage_rows(D, 4096)[1] <= 48 * 1024
         z = torch.zeros(16, device=DEV)
         ptrs = (C.c_void_p * D)(*([C.c_void_p(z.data_ptr())] * D))
         p = C.c_void_p(z.data_ptr())
         assert lib.sdr_causal_stream_stage(p, p, ptrs, ptrs, ptrs, p, p, D, B, 40, 4096 + gran, None) == -5
+
+
+def test_stream_stage_65535_slots():
+    """grid.y = 65535 CTAs, one per slot, at the granule; 65536 slots are refused."""
+    _stage_case(3, 4, 65535, Cc=3)
+    z = torch.zeros(16, device=DEV)
+    ptrs = (C.c_void_p * 3)(*([C.c_void_p(z.data_ptr())] * 3))
+    p = C.c_void_p(z.data_ptr())
+    assert N.lib().sdr_causal_stream_stage(p, p, ptrs, ptrs, ptrs, p, p, 3, 65536, 3, 4, None) == -5
 
 
 # ---- slots, reset, graphs ----
