@@ -25,6 +25,7 @@ int launch_pyramid_fused(const float*, const NormIn&, const float* const*, const
 int launch_pointwise_ffma(const float*, const NormIn&, const float*, const float*, const float*, const float*, int,
                           float*, double*, int, int, int, int, int, cudaStream_t);
 int launch_encoder(const float*, const float*, const float*, int, float*, double*, int, int, long long, int, int, int, int, cudaStream_t);
+bool encoder_ffma_fits(int A, int K);
 int launch_overlap_add(const float*, const float*, const float*, const float2*, float*, int, int, int, int, long long, cudaStream_t);
 int launch_mixture_consistency(const float*, const float*, float*, int, int, long long, int, void*, cudaStream_t);
 int launch_tac(const float*, const float* const*, float*, double*, int, int, int, int, cudaStream_t);
@@ -761,6 +762,8 @@ static int check_forward_args(const Layout& l, int B, int64_t T) {
         if (!(n == 4 || n == 8 || n == 16 || n == 32) || l.G > 16) return SDR_ERR_UNSUPPORTED;
     }
     if (padded_len(l, T) / l.hop > 0x3fffffffLL) return SDR_ERR_UNSUPPORTED;
+    // the FFMA encoder (no tensor-core image: N < 32) holds A audio channels x K taps in one CTA's shared memory
+    if (!l.enc_pk && !encoder_ffma_fits(l.A, l.K)) return SDR_ERR_UNSUPPORTED;
     if (l.causal && !causal_pyramid_eligible(l.D, (int)(padded_len(l, T) / l.hop))) return SDR_ERR_UNSUPPORTED;
     // original model: lcm(hop, 2^D) padding makes L a multiple of 2^D / gcd(hop, 2^D); the D - 1 stride-2 levels need
     // exact halvings (the reference's up-sample + add fails otherwise, sudormrf.py:180-182)

@@ -87,13 +87,20 @@ encoder_kernel(const float* __restrict__ wav, const float* __restrict__ weight, 
     if (stats) block_stats_atomic(acc, stats, b, s_red);
 }
 
+// Dynamic shared memory of one CTA: the waveform chunk of every audio channel and the [A*K][kEncNB] weight slab.
+static size_t encoder_smem_bytes(int A, int K) {
+    const int span = (K / 2) * (kEncThreads - 1) + K;
+    return (size_t)(((A * span + 3) & ~3) + A * K * kEncNB) * sizeof(float);
+}
+
+// Whether the FFMA encoder can take A audio channels and K taps (its CTA would need more than 200 KB otherwise).
+bool encoder_ffma_fits(int A, int K) { return encoder_smem_bytes(A, K) <= 200 * 1024; }
+
 int launch_encoder(const float* wav, const float* weight, const float* bias, int relu, float* enc, double* stats,
                    int B, int A, long long T, int N, int K, int L, int pad, cudaStream_t st) {
     if (B <= 0 || A <= 0 || T <= 0 || N <= 0 || K < 3 || L <= 0) return SDR_ERR_BAD_ARGUMENT;
-    const int hop = K / 2;
-    const int span = hop * (kEncThreads - 1) + K;
-    const size_t smem = (size_t)(((A * span + 3) & ~3) + A * K * kEncNB) * sizeof(float);
-    if (smem > 200 * 1024) return SDR_ERR_UNSUPPORTED;
+    if (!encoder_ffma_fits(A, K)) return SDR_ERR_UNSUPPORTED;
+    const size_t smem = encoder_smem_bytes(A, K);
     if (smem > 48 * 1024) {
         cudaError_t e = cudaFuncSetAttribute(encoder_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
         if (e != cudaSuccess) return SDR_ERR_CUDA;

@@ -110,14 +110,16 @@ class StabilizedPermInvSISDRMetric(nn.Module):
             assert self.n_actual_sources == 1
 
     def forward(self, pr_batch, t_batch, eps=1e-9, return_best_permutation=False):
-        """pr_batch ``[B, n_estimated (any number when single_source), T]``, t_batch ``[B, n_actual, T]``."""
+        """pr_batch ``[B, rows, T]``, t_batch ``[B, n_actual, T]``.  Without ``single_source`` the first
+        ``n_estimated_sources`` rows are scored and any further rows are ignored, as in the reference; with it, every
+        row is summed into the one estimate."""
         if pr_batch.dim() != 3 or t_batch.dim() != 3 or pr_batch.shape[0] != t_batch.shape[0] \
                 or pr_batch.shape[-1] != t_batch.shape[-1]:
             raise RuntimeError("expected pr_batch [B, n_estimated, T] and t_batch [B, n_actual, T]")
         if t_batch.shape[1] != self.n_actual_sources:
             raise RuntimeError(f"expected {self.n_actual_sources} actual sources, got {t_batch.shape[1]}")   # sisdr.py:521
-        if not self.single_source and pr_batch.shape[1] != self.n_estimated_sources:
-            raise RuntimeError(f"expected {self.n_estimated_sources} estimated sources, got {pr_batch.shape[1]}")
+        if not self.single_source and pr_batch.shape[1] < self.n_estimated_sources:
+            raise RuntimeError(f"expected at least {self.n_estimated_sources} estimated sources, got {pr_batch.shape[1]}")
         if self.single_source and self.n_estimated_sources != 1:
             raise RuntimeError("single_source sums the estimates into one: construct the metric with "
                                "n_estimated_sources=1 (the reference's permutation table indexes the summed tensor)")
@@ -127,6 +129,10 @@ class StabilizedPermInvSISDRMetric(nn.Module):
             raise RuntimeError("sudo_rm_rf_b200.sisdr is the evaluation metric only (no autograd): "
                                "wrap the call in torch.no_grad()")
         dev = pr_batch.device
+        if not self.single_source:
+            # the assignments index rows 0 .. n_estimated - 1 only (sisdr.py:490-492,526-527): run_fuss_separation.py
+            # scores its one-source set with n_estimated_sources=1 on every output row of the model
+            pr_batch = pr_batch[:, :self.n_estimated_sources]
         est = pr_batch.detach().to(torch.float32).contiguous()
         tgt = t_batch.detach().to(device=dev, dtype=torch.float32).contiguous()
         B, rows, T = est.shape

@@ -43,6 +43,35 @@ CASES = [
                       enc_kernel_size=21, enc_num_basis=128, num_sources=2), 3333),
     ("original", dict(out_channels=32, in_channels=64, num_blocks=2, upsampling_depth=5,
                       enc_kernel_size=21, enc_num_basis=32, num_sources=4), 1600),   # no reshape layer, T a multiple of the lcm
+    # the geometry around the blocks: filter lengths 3 / 5 / 41 / 91 (hop 1, 2, 20, 45), 1 / 4 / 5 / 16 sources,
+    # 4 and 16 audio channels, a group count that is not a power of two
+    ("improved", dict(out_channels=32, in_channels=64, num_blocks=2, upsampling_depth=4,
+                      enc_kernel_size=41, enc_num_basis=64, num_sources=4), 341),
+    ("improved", dict(out_channels=16, in_channels=32, num_blocks=1, upsampling_depth=3,
+                      enc_kernel_size=3, enc_num_basis=32, num_sources=16), 151),
+    ("improved", dict(out_channels=16, in_channels=32, num_blocks=1, upsampling_depth=3,
+                      enc_kernel_size=5, enc_num_basis=32, num_sources=1), 333),
+    ("groupcomm", dict(out_channels=64, in_channels=128, num_blocks=1, upsampling_depth=3,
+                       enc_kernel_size=91, enc_num_basis=64, num_sources=4, group_size=16), 401),
+    ("groupcomm", dict(in_audio_channels=4, out_channels=24, in_channels=48, num_blocks=1, upsampling_depth=3,
+                       enc_kernel_size=5, enc_num_basis=16, num_sources=4, group_size=3), 101),
+    ("groupcomm", dict(in_audio_channels=16, out_channels=48, in_channels=96, num_blocks=1, upsampling_depth=3,
+                       enc_kernel_size=3, enc_num_basis=16, num_sources=1, group_size=12), 101),
+    ("original", dict(out_channels=32, in_channels=64, num_blocks=2, upsampling_depth=4,
+                      enc_kernel_size=11, enc_num_basis=48, num_sources=5), 401),    # hop 5: lcm 80
+    ("original", dict(out_channels=32, in_channels=64, num_blocks=1, upsampling_depth=3,
+                      enc_kernel_size=5, enc_num_basis=32, num_sources=1), 400),     # one source: sigmoid
+    ("original", dict(out_channels=16, in_channels=32, num_blocks=1, upsampling_depth=3,
+                      enc_kernel_size=3, enc_num_basis=16, num_sources=16), 48),     # hop 1
+    ("original", dict(out_channels=32, in_channels=64, num_blocks=1, upsampling_depth=4,
+                      enc_kernel_size=41, enc_num_basis=32, num_sources=4), 401),    # hop 20: pads to 480, L = 24
+]
+# Lengths the original model itself cannot run: padding to a multiple of lcm(hop, 2^D) leaves L = Tp / hop with
+# L % 2^(D-1) != 0, and the up-sample + add of its U-ConvBlock (sudormrf.py:180-182) then meets mismatched lengths.
+# The C-ABI refuses these lengths for the same reason.
+REFUSED = [
+    ("original", dict(out_channels=32, in_channels=64, num_blocks=1, upsampling_depth=4,
+                      enc_kernel_size=41, enc_num_basis=32, num_sources=4), 240),    # L = 12
 ]
 CLASSES = {"improved": ri.SuDORMRF, "groupcomm": rg.GroupCommSudoRmRf, "causal": rc.CausalSuDORMRF,
            "original": ro.SuDORMRF}
@@ -64,10 +93,21 @@ def main():
         m = CLASSES[variant](**kw).eval()
         assert list(m.state_dict().keys()) == list(sd.keys())
         m.load_state_dict(sd)
-        x = torch.randn(2, 1, T, generator=torch.Generator().manual_seed(INPUT_SEED))
+        x = torch.randn(2, kw.get("in_audio_channels", 1), T, generator=torch.Generator().manual_seed(INPUT_SEED))
         with torch.no_grad():
             arrays[f"c{i}/out"] = m(x).numpy().astype(np.float32)
         meta["cases"].append({"variant": variant, "kw": kw, "T": T})
+    meta["reference_refuses"] = []
+    for variant, kw, T in REFUSED:
+        m = CLASSES[variant](**kw).eval()
+        m.load_state_dict(O.make_state_dict(O.Config(variant=variant, **kw), seed=MODEL_SEED))
+        try:
+            with torch.no_grad():
+                m(torch.randn(2, 1, T, generator=torch.Generator().manual_seed(INPUT_SEED)))
+        except RuntimeError as e:
+            meta["reference_refuses"].append({"variant": variant, "kw": kw, "T": T, "error": str(e).splitlines()[0]})
+        else:
+            raise AssertionError(f"the reference ran {variant} {kw} at T = {T}")
     est, tgt, mix = pit_inputs()
     fn = ref_sisdr.PermInvariantSISDR(batch_size=6, zero_mean=True, n_sources=3, backward_loss=False,
                                       improvement=True, return_individual_results=True)

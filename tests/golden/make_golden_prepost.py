@@ -139,18 +139,21 @@ def make_pairwise():
 def make_stabilized():
     """``prepost_stabilized.npz``: ``StabilizedPermInvSISDRMetric`` (dnn/losses/sisdr.py:460-591), the validation
     metric of run_fuss_separation.py:111-131: more estimated than actual sources, one source, single_source (the
-    estimates are summed first), with / without zero-mean and improvement."""
+    estimates are summed first), with / without zero-mean and improvement, and the script's one-source set: a metric
+    constructed for one estimated source and handed all four output rows, of which it scores the first."""
     arrays, cases = {}, []
     g = torch.Generator().manual_seed(777)
-    for ci, (n_est, n_act, B, T, zero_mean, improvement, single) in enumerate([
-            (4, 2, 4, 3000, True, True, False), (4, 3, 3, 2000, True, True, False), (4, 4, 2, 1500, True, True, False),
-            (3, 1, 3, 1234, False, False, False), (2, 2, 3, 800, False, True, False), (1, 1, 2, 600, True, False, False),
-            (3, 1, 2, 900, True, False, True), (4, 1, 2, 500, False, False, False)]):
+    for ci, (n_est, n_act, B, T, zero_mean, improvement, single, ctor_est) in enumerate([
+            (4, 2, 4, 3000, True, True, False, 4), (4, 3, 3, 2000, True, True, False, 4),
+            (4, 4, 2, 1500, True, True, False, 4), (3, 1, 3, 1234, False, False, False, 3),
+            (2, 2, 3, 800, False, True, False, 2), (1, 1, 2, 600, True, False, False, 1),
+            # single_source sums the estimates first (sisdr.py:576-577), so the constructor is given ONE estimated
+            # source (its permutation table indexes the summed tensor, :490-492,527); the model still returned n_est
+            (3, 1, 2, 900, True, False, True, 1), (4, 1, 2, 500, False, False, False, 4),
+            # run_fuss_separation.py:111-116,296-307: n_estimated_sources=1 without single_source on four rows
+            (4, 1, 3, 700, True, False, False, 1)]):
         tgt = torch.randn(B, n_act, T, generator=g) * (0.2 + torch.rand(B, n_act, 1, generator=g)) + 0.05
         est = torch.randn(B, n_est, T, generator=g) * 0.05                       # inactive outputs: low-level noise
-        # single_source sums the estimates first (sisdr.py:576-577), so the constructor is given ONE estimated source
-        # (its permutation table indexes the summed tensor, :490-492,527); the model still returned n_est outputs
-        ctor_est = 1 if single else n_est
         for b in range(B):
             slots = torch.randperm(n_est, generator=g)[:n_act]
             for j in range(n_act):
@@ -169,7 +172,7 @@ def make_stabilized():
         arrays.update({k + "est": est.numpy(), k + "tgt": tgt.numpy(), k + "best": best.numpy(),
                        k + "perms": perms.numpy(), k + "loss": scalar.reshape(1).numpy()})
         cases.append(dict(n_est=n_est, n_act=n_act, B=B, T=T, zero_mean=zero_mean, improvement=improvement,
-                          single_source=single))
+                          single_source=single, ctor_est=ctor_est))
         print(f"stabilized/c{ci}: {n_est}->{n_act} best={best.numpy().round(3)} perms={perms.numpy().tolist()}")
     arrays["meta"] = np.frombuffer(json.dumps(dict(cases=cases, torch=torch.__version__)).encode(), dtype=np.uint8)
     path = os.path.join(HERE, "prepost_stabilized.npz")

@@ -196,6 +196,11 @@ def test_stabilized_metric_host_conventions():
         fn(torch.zeros(1, 4, 10), torch.zeros(1, 2, 10))
     with pytest.raises(RuntimeError, match="actual"):
         fn(torch.zeros(1, 4, 10), torch.zeros(1, 3, 10))
+    with pytest.raises(RuntimeError, match="estimated"):       # fewer rows than estimated sources: the reference fails too
+        fn(torch.zeros(1, 3, 10), torch.zeros(1, 2, 10))
+    one = sisdr.StabilizedPermInvSISDRMetric(zero_mean=True, n_estimated_sources=1, n_actual_sources=1)
+    with pytest.raises(RuntimeError, match="CUDA"):             # four rows pass the row check: the first one is scored
+        one(torch.zeros(1, 4, 10), torch.zeros(1, 1, 10))
     with pytest.raises(AssertionError):
         sisdr.StabilizedPermInvSISDRMetric(n_estimated_sources=1, n_actual_sources=2)
     with pytest.raises(AssertionError):
@@ -203,3 +208,21 @@ def test_stabilized_metric_host_conventions():
     lib = _native.lib()
     assert lib.sdr_stabilized_sisdr_scratch_bytes(3, 4, 2) == 8 * 3 * (4 + 2 + 8 + 4 + 4)
     assert lib.sdr_stabilized_sisdr_scratch_bytes(3, 2, 3) == 0 and lib.sdr_stabilized_sisdr_scratch_bytes(3, 5, 2) == 0
+
+
+def test_ffma_encoder_limit_refused_before_launch():
+    """Below 32 basis functions the encoder is the FFMA kernel, whose CTA holds A channels x K taps of weights and
+    waveform in at most 200 KB of shared memory: A = 4 takes K = 99 and not 101, A = 16 takes K = 25 and not 27.
+    sdr_forward refuses the larger filters with its other argument checks, before it reads a buffer or enqueues a
+    kernel (null buffers then return SDR_ERR_BAD_ARGUMENT instead); the tensor-core encoder (N = 32) has no such limit."""
+    lib = _native.lib()
+
+    def fwd(A, K, N_, S):
+        m = P.GroupCommSudoRmRf(in_audio_channels=A, out_channels=16, in_channels=32, num_blocks=1, upsampling_depth=3,
+                                enc_kernel_size=K, enc_num_basis=N_, num_sources=S, group_size=4)
+        c = _engine.make_config(m)
+        assert lib.sdr_workspace_bytes(C.byref(c), 2, 1001) > 0
+        return lib.sdr_forward(C.byref(c), None, None, None, 2, 1001, 0, None, 0, None)
+    assert (fwd(4, 99, 16, 4), fwd(4, 101, 16, 4)) == (-2, -5)
+    assert (fwd(16, 25, 16, 1), fwd(16, 27, 16, 1)) == (-2, -5)
+    assert lib.sdr_encoder_mma_packed_bytes(32, 4, 101) > 0 and fwd(4, 101, 32, 4) == -2

@@ -138,12 +138,13 @@ def _stabilized_cases():
             for ci, c in enumerate(meta["cases"])]
 
 
-@pytest.mark.parametrize("ci", range(8))
+@pytest.mark.parametrize("ci", range(9))
 def test_stabilized_sisdr_golden(ci):
     """sisdr.StabilizedPermInvSISDRMetric (same constructor / forward as dnn/losses/sisdr.py:460-591) against outputs of
-    the reference class: 4 -> 2 / 3 / 4 and 3 / 4 -> 1 sources, single_source, zero-mean and improvement on and off."""
+    the reference class: 4 -> 2 / 3 / 4 and 3 / 4 -> 1 sources, single_source, zero-mean and improvement on and off,
+    and a metric constructed for one estimated source given four rows (it scores the first)."""
     c, t = _stabilized_cases()[ci]
-    n_est = 1 if c["single_source"] else c["n_est"]
+    n_est = c["ctor_est"]
     fn = S.StabilizedPermInvSISDRMetric(zero_mean=c["zero_mean"], single_source=c["single_source"],
                                         n_estimated_sources=n_est, n_actual_sources=c["n_act"], backward_loss=False,
                                         improvement=c["improvement"], return_individual_results=True)

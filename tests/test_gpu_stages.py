@@ -339,13 +339,23 @@ def test_encoder_tensor_core(B, A, T, N_, K, D):
     check_stats(st, want.float(), rtol=3e-5)
 
 
-@pytest.mark.parametrize("B,SA,K,L,T,mc", [
+OVERLAP_ADD = [
     (2, 2, 21, 3200, 32000, False), (2, 2, 21, 3232, 32079, True), (3, 3, 21, 64, 640, False),
     (2, 4, 11, 72, 333, False), (1, 2, 21, 32, 7, True), (1, 2, 91, 80, 3000, False),
-])
+    # filter lengths 3 .. 201 (hop 1 .. 100), 1 / 3 / 5 / 16 outputs, T < K, T not a multiple of the hop, mixture
+    # consistency where 1/SA != 0.5
+    (2, 1, 3, 40, 37, True), (3, 5, 3, 333, 333, False), (2, 3, 5, 50, 99, True), (1, 5, 7, 30, 89, True),
+    (2, 16, 7, 20, 58, False), (2, 16, 41, 8, 30, True), (1, 3, 41, 40, 799, False), (2, 16, 91, 12, 517, True),
+    (2, 1, 91, 3, 50, False), (1, 3, 201, 6, 150, True), (2, 1, 201, 20, 1999, False), (1, 16, 201, 4, 399, True),
+]
+
+
+@pytest.mark.parametrize("B,SA,K,L,T,mc", OVERLAP_ADD)
 def test_overlap_add(B, SA, K, L, T, mc):
+    """Against conv_transpose1d + crop (and mixture consistency) in fp64."""
     g = torch.Generator().manual_seed(4)
     hop = K // 2
+    assert T <= hop * L
     C_ = 6
     masked = torch.randn(B, C_, L, generator=g).to(DEV)
     wd = torch.randn(C_, SA, K, generator=g).to(DEV)
@@ -354,10 +364,10 @@ def test_overlap_add(B, SA, K, L, T, mc):
     mix = torch.randn(B, 1, T, generator=g).to(DEV) if mc else None
     out = torch.full((B, SA, T), float("nan"), device=DEV)
     N.check(N.lib().sdr_overlap_add(p(frames), p(mix), p(out), B, SA, K, L, T, stream()))
-    want = F.conv_transpose1d(masked, wd, None, stride=hop, padding=hop,
+    want = F.conv_transpose1d(masked.double(), wd.double(), None, stride=hop, padding=hop,
                               output_padding=hop - 1)[..., :T]
     if mc:
-        want = O.mixture_consistency(want.cpu(), mix.cpu()).to(DEV)
+        want = O.mixture_consistency(want, mix.double())
     close(out, want)
 
 
@@ -387,16 +397,39 @@ def test_tac(B, G, n, L):
     check_stats(st, want.reshape(B * G, n, L), rtol=1e-4 if n == 16 else 1e-5)
 
 
-@pytest.mark.parametrize("kind", ["uniform", "magsq"])
-def test_mixture_consistency(kind):
+MIXTURE_CONSISTENCY = [   # kind, S, T, silent estimates; the first two keep their ids
+    ("uniform", 2, 32079, "none"), ("magsq", 2, 32079, "none"),
+    ("uniform", 1, 2049, "none"), ("magsq", 1, 2048, "none"), ("uniform", 3, 2047, "none"), ("magsq", 3, 2049, "none"),
+    ("uniform", 16, 4097, "none"), ("magsq", 16, 2048, "none"), ("magsq", 3, 2049, "one"), ("magsq", 16, 4096, "one"),
+    ("magsq", 3, 2047, "all"), ("magsq", 1, 2049, "all"), ("uniform", 16, 2049, "all"),
+]
+
+
+def _mc_id(c):
+    return c[0] if c[1:] == (2, 32079, "none") else "-".join(str(v) for v in c)
+
+
+@pytest.mark.parametrize("kind,S,T,silent", MIXTURE_CONSISTENCY, ids=[_mc_id(c) for c in MIXTURE_CONSISTENCY])
+def test_mixture_consistency(kind, S, T, silent):
+    """Against mixture_consistency.py in fp64: 1, 2, 3 and 16 sources, both weight types, one or every estimate
+    silent ('magsq' then gives it no share of the residual), T on both sides of the power kernel's 2048-sample step."""
     import sudo_rm_rf_b200.mixture_consistency as mc
     g = torch.Generator().manual_seed(6)
-    est = torch.randn(3, 2, 32079, generator=g)
-    mix = torch.randn(3, 1, 32079, generator=g)
+    est = torch.randn(3, S, T, generator=g)
+    mix = torch.randn(3, 1, T, generator=g)
+    if silent == "one":
+        est[:, S // 2] = 0
+    elif silent == "all":
+        est.zero_()
     got = mc.apply(est.to(DEV), mix.to(DEV), kind)
-    close(got, O.mixture_consistency(est, mix, kind), tol=1e-5)
+    want = O.mixture_consistency(est.double(), mix.double(), kind)
+    close(got, want, tol=1e-5)
     if kind == "uniform":
-        assert torch.allclose(got.sum(1, keepdim=True).cpu(), mix, atol=1e-5)
+        assert torch.allclose(got.sum(1, keepdim=True).cpu(), mix, atol=1e-5 * S)
+    if silent == "one":
+        assert torch.equal(got[:, S // 2].cpu(), torch.zeros(3, T))
+    if kind == "magsq" and silent == "all":
+        assert torch.equal(got.cpu(), est)
 
 
 @pytest.mark.parametrize("samples,M,K,L,mode", [
@@ -530,17 +563,54 @@ def test_residual_norm(samples, C_, L, first):
     check_stats(st, want)
 
 
-@pytest.mark.parametrize("B,S,N_,L,inplace", [
-    (2, 2, 512, 3200, True), (3, 3, 24, 52, False), (2, 1, 16, 80, True), (1, 4, 7, 3, False), (2, 16, 8, 10, True),
-])
-def test_softmax_gate(B, S, N_, L, inplace):
-    """Masks of the original model (sudormrf.py:285-289): softmax over the sources (sigmoid for one) x encoder output."""
+SOFTMAX_GATE = [   # B, S, N, L, inplace, logits; the first five keep their ids
+    (2, 2, 512, 3200, True, "randn"), (3, 3, 24, 52, False, "randn"), (2, 1, 16, 80, True, "randn"),
+    (1, 4, 7, 3, False, "randn"), (2, 16, 8, 10, True, "randn"),
+]
+# every source count on the vector path (N*L % 4 == 0) and on the scalar path (N*L % 4 != 0)
+SOFTMAX_GATE += [(2, S, 8, 12, S % 2 == 0, "randn") for S in range(1, 17)]
+SOFTMAX_GATE += [(2, S, 5, 7, S % 2 == 1, "randn") for S in range(1, 17)]
+# float4-sized rows behind a pointer that is not 16-byte aligned: the scalar path
+SOFTMAX_GATE += [(2, S, 8, 12, False, "offset") for S in (1, 2, 4, 5, 16)]
+# logits of +-1e4 (exp underflows to 0 for every source below the largest; the sigmoid saturates), exact ties
+SOFTMAX_GATE += [(2, S, 8, 12, True, "1e4") for S in (1, 2, 3, 4, 7, 16)]
+SOFTMAX_GATE += [(1, S, 5, 7, False, "1e4") for S in (1, 3, 16)]
+SOFTMAX_GATE += [(2, S, 8, 12, False, "ties") for S in (2, 3, 4, 9, 16)]
+SOFTMAX_GATE += [(1, S, 5, 7, True, "ties") for S in (3, 16)]
+
+
+def _sg_id(c):
+    return "-".join(str(v) for v in (c[:5] if SOFTMAX_GATE.index(c) < 5 else c))
+
+
+@pytest.mark.parametrize("B,S,N_,L,inplace,logits", SOFTMAX_GATE, ids=[_sg_id(c) for c in SOFTMAX_GATE])
+def test_softmax_gate(B, S, N_, L, inplace, logits):
+    """Masks of the original model (sudormrf.py:285-289): softmax over the sources (sigmoid for one) x encoder output,
+    against fp64 torch.softmax / torch.sigmoid."""
     g = torch.Generator().manual_seed(22)
-    logits = (torch.randn(B, S, N_, L, generator=g) * 3).to(DEV)
-    enc = torch.relu(torch.randn(B, N_, L, generator=g)).to(DEV)
-    want = (torch.sigmoid(logits) if S == 1 else torch.softmax(logits, dim=1)) * enc.unsqueeze(1)
-    out = logits.clone() if inplace else torch.full_like(logits, float("nan"))
-    N.check(N.lib().sdr_softmax_gate(p(out if inplace else logits), p(enc), p(out), B, S, N_, L, stream()))
+    lg = torch.randn(B, S, N_, L, generator=g) * 3
+    if logits == "1e4":          # one source at +1e4 and the rest at -1e4, each source in turn; every third position
+        pos = torch.arange(N_ * L).view(1, 1, N_, L)              # +-1e4 at random (ties among the largest)
+        lg = torch.full((B, S, N_, L), -1e4).scatter_(1, (pos % S).expand(B, 1, N_, L), 1e4)
+        rnd = torch.where(torch.rand(B, S, N_, L, generator=g) < 0.5, -1e4, 1e4)
+        lg = torch.where(pos % 3 == 2, rnd, lg)
+    elif logits == "ties":       # every source ties at each position; on odd positions the first two share the max
+        lg = (torch.randn(B, 1, N_, L, generator=g) * 3).expand(B, S, N_, L).clone()
+        lg[:, 2:, :, 1::2] -= 1.5
+    enc = torch.relu(torch.randn(B, N_, L, generator=g))
+    want = (torch.sigmoid(lg.double()) if S == 1 else torch.softmax(lg.double(), dim=1)) * enc.double().unsqueeze(1)
+    shift = 1 if logits == "offset" else 0   # one float into a fresh allocation: 4-byte but not 16-byte aligned
+    lbuf = torch.empty(lg.numel() + shift, device=DEV)
+    ebuf = torch.empty(enc.numel() + shift, device=DEV)
+    lbuf[shift:] = lg.reshape(-1).to(DEV)
+    ebuf[shift:] = enc.reshape(-1).to(DEV)
+    lgd, encd = lbuf[shift:].view(B, S, N_, L), ebuf[shift:].view(B, N_, L)
+    if inplace:
+        out = lgd
+    else:
+        obuf = torch.full((lg.numel() + shift,), float("nan"), device=DEV)
+        out = obuf[shift:].view(B, S, N_, L)
+    N.check(N.lib().sdr_softmax_gate(p(lgd), p(encd), p(out), B, S, N_, L, stream()))
     close(out, want, tol=1e-5)
 
 

@@ -111,14 +111,15 @@ def load_stabilized():
             for ci, c in enumerate(meta["cases"])]
 
 
-@pytest.mark.parametrize("ci", range(8))
+@pytest.mark.parametrize("ci", range(9))
 def test_stabilized_sisdr_matches_reference_golden(ci):
-    """StabilizedPermInvSISDRMetric (sisdr.py:460-591): more estimated than actual sources, single_source, SI-SDRi."""
+    """StabilizedPermInvSISDRMetric (sisdr.py:460-591): more estimated than actual sources, single_source, SI-SDRi, and
+    a metric built for one estimated source handed four rows (run_fuss_separation.py's one-source set)."""
     c, t = load_stabilized()[ci]
+    n_est = c["ctor_est"]
     best, idx = O.stabilized_pit_sisdr(t["est"], t["tgt"], zero_mean=c["zero_mean"], single_source=c["single_source"],
-                                       improvement=c["improvement"])
+                                       improvement=c["improvement"], n_estimated=n_est)
     assert torch.allclose(best, t["best"], atol=1e-4, rtol=0)
-    n_est = 1 if c["single_source"] else c["n_est"]
     perms = list(itertools.permutations(range(n_est), r=c["n_act"]))
     assert [perms[int(i)] for i in idx] == [tuple(int(v) for v in row) for row in t["perms"]]
     assert torch.allclose(-best.mean(), t["loss"][0], atol=1e-4, rtol=0)
