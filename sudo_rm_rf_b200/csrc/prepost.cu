@@ -170,6 +170,15 @@ pit_gram_kernel(const float* __restrict__ est, const float* __restrict__ tgt, co
     }
 }
 
+// A mean-removed energy sum(x^2) - n * mean^2 can round to a few ulp below zero (a constant row under zero_mean);
+// the energy it stands for is never negative.  NaN passes through.
+__device__ __forceinline__ double clamp_energy(double v) { return v < 0.0 ? 0.0 : v; }
+
+// torch.max's selection over candidates in order: the first NaN wins and is kept, otherwise the first maximum.
+__device__ __forceinline__ bool takes_max(double m, double best, int idx) {
+    return idx == 0 || (!isnan(best) && (isnan(m) || m > best));
+}
+
 __device__ __forceinline__ double sisnr_from_dots(double et, double tt, double ee, double eps) {
     const double alpha = et / (tt + eps);
     const double st = alpha * alpha * tt;
@@ -196,16 +205,16 @@ pit_finalize_kernel(const double* __restrict__ acc, float* __restrict__ best, in
         if (zero_mean) mm = a[2 * S] / n;
         double tt[S], ee[S], sn[S][S];
 #pragma unroll
-        for (int j = 0; j < S; ++j) tt[j] = a[P::TT + j] - n * mt[j] * mt[j];
+        for (int j = 0; j < S; ++j) tt[j] = clamp_energy(a[P::TT + j] - n * mt[j] * mt[j]);
 #pragma unroll
-        for (int i = 0; i < S; ++i) ee[i] = a[P::EE + i] - n * me[i] * me[i];
+        for (int i = 0; i < S; ++i) ee[i] = clamp_energy(a[P::EE + i] - n * me[i] * me[i]);
 #pragma unroll
         for (int i = 0; i < S; ++i)
 #pragma unroll
             for (int j = 0; j < S; ++j)
                 sn[i][j] = sisnr_from_dots(a[P::ET + i * S + j] - n * me[i] * mt[j], tt[j], ee[i], eps);
         // permutations in lexicographic order (itertools.permutations(range(S))): perm p maps target j -> estimate p[j]
-        double bestv = -1e300;
+        double bestv = 0.0;
         int besti = 0, idx = 0;
         int p[S];
 #pragma unroll
@@ -214,7 +223,7 @@ pit_finalize_kernel(const double* __restrict__ acc, float* __restrict__ best, in
             double m = 0.0;
             for (int j = 0; j < S; ++j) m += sn[p[j]][j];
             m /= (double)S;
-            if (m > bestv) { bestv = m; besti = idx; }     // torch.max keeps the first maximum
+            if (takes_max(m, bestv, idx)) { bestv = m; besti = idx; }
             ++idx;
             // next lexicographic permutation
             int k = S - 2;
@@ -228,7 +237,7 @@ pit_finalize_kernel(const double* __restrict__ acc, float* __restrict__ best, in
         best[b] = (float)bestv;
         perm[b] = besti;
         if (improvement) {
-            const double em = a[P::MM] - n * mm * mm;
+            const double em = clamp_energy(a[P::MM] - n * mm * mm);
             for (int j = 0; j < S; ++j)
                 base_sum += sisnr_from_dots(a[P::MT + j] - n * mm * mt[j], tt[j], em, eps);
         }
@@ -284,14 +293,15 @@ pairwise_finalize_kernel(const double* __restrict__ acc, float* __restrict__ out
         for (int i = 0; i < S; ++i) { me[i] = zero_mean ? a[i] / n : 0.0; mt[i] = zero_mean ? a[S + i] / n : 0.0; }
 #pragma unroll
         for (int i = 0; i < S; ++i) {
-            const double ee = a[P::EE + i] - n * me[i] * me[i];
+            const double ee = clamp_energy(a[P::EE + i] - n * me[i] * me[i]);
 #pragma unroll
             for (int j = 0; j < S; ++j) {
-                const double tt = a[P::TT + j] - n * mt[j] * mt[j];
+                const double tt = clamp_energy(a[P::TT + j] - n * mt[j] * mt[j]);
                 const double d = a[P::ET + i * S + j] - n * me[i] * mt[j];
                 const double c = d / (tt + 1e-8);
                 const double proj = sdr_type == 0 ? tt : c * c * tt;                       // 0 snr, 1 sisdr, 2 sdsdr
                 double noise = sdr_type == 1 ? ee - 2.0 * c * d + c * c * tt : ee - 2.0 * d + tt;
+                if (sdr_type != 1 && isinf(ee) && isfinite(tt)) noise = ee;    // |e - t|^2 with an inf in e: inf - inf above
                 if (noise < 0.0) noise = 0.0;
                 double v = proj / (noise + 1e-8);
                 if (take_log) v = 10.0 * log10(v + 1e-8);
@@ -400,7 +410,8 @@ stab_gram_kernel(const float* __restrict__ est, const float* __restrict__ tgt, d
 }
 
 __device__ __forceinline__ double stab_sisnr(double et, double ee, double tt, double eps) {
-    const double rho = et * et / (ee * tt + eps);
+    double rho = et * et / (ee * tt + eps);
+    if (rho > 1.0) rho = 1.0;          // a squared correlation; rounding of the Gram form can push it past 1 (then NaN)
     return 10.0 * log10((rho + eps) / (1.0 - rho + eps));
 }
 
@@ -427,14 +438,16 @@ stab_finalize_kernel(const double* __restrict__ acc, float* __restrict__ best, i
 #pragma unroll
             for (int k = 0; k < SA; ++k) tt[j][k] = a[P::TT + j * SA + k] - n * mt[j] * mt[k];
 #pragma unroll
+        for (int j = 0; j < SA; ++j) tt[j][j] = clamp_energy(tt[j][j]);
+#pragma unroll
         for (int i = 0; i < SE; ++i) {
-            const double ee = a[P::EE + i] - n * me[i] * me[i];
+            const double ee = clamp_energy(a[P::EE + i] - n * me[i] * me[i]);
 #pragma unroll
             for (int j = 0; j < SA; ++j)
                 sn[i][j] = stab_sisnr(a[P::ET + i * SA + j] - n * me[i] * mt[j], ee, tt[j][j], eps);
         }
         // assignments p[0..SA) of distinct estimates, lexicographic (= itertools.permutations(range(SE), r=SA))
-        double bestv = -1e300;
+        double bestv = 0.0;
         int besti = 0, idx = 0;
         int total = 1;
 #pragma unroll
@@ -458,7 +471,7 @@ stab_finalize_kernel(const double* __restrict__ acc, float* __restrict__ best, i
                 m += v;
             }
             m /= (double)SA;
-            if (m > bestv) { bestv = m; besti = idx; }     // torch.max keeps the first maximum
+            if (takes_max(m, bestv, idx)) { bestv = m; besti = idx; }
             ++idx;
         }
         best[b] = (float)bestv;
@@ -469,6 +482,7 @@ stab_finalize_kernel(const double* __restrict__ acc, float* __restrict__ best, i
             for (int j = 0; j < SA; ++j)
 #pragma unroll
                 for (int k = 0; k < SA; ++k) mm += tt[j][k];
+            mm = clamp_energy(mm);
 #pragma unroll
             for (int j = 0; j < SA; ++j) {
                 double mtj = 0.0;

@@ -9,6 +9,8 @@ named by SUDO_RM_RF_REFERENCE:
   without and with the mixture-consistency step.
 * ``prepost_sisdr.npz``: ``PermInvariantSISDR`` (dnn/losses/sisdr.py:66-194) outputs for
   2, 3 and 4 sources, with/without zero-mean and improvement.
+* ``prepost_degenerate.npz``: the three metrics on degenerate rows (a NaN sample, a constant target under
+  zero-mean, a silent target, two identical estimates, a perfect estimate).
 """
 import json
 import os
@@ -180,7 +182,80 @@ def make_stabilized():
     print(f"stabilized -> {os.path.getsize(path)/1024:.0f} KiB")
 
 
+DEGENERATE_CASES = ["nan_row", "constant_target", "silent_target", "tie", "perfect"]
+
+
+def degenerate_signals(case, n_est, n_act, B, T, g):
+    """Item 0 of the batch carries the case; the other items are ordinary."""
+    tgt = torch.randn(B, n_act, T, generator=g) * (0.2 + torch.rand(B, n_act, 1, generator=g)) + 0.05
+    est = torch.randn(B, n_est, T, generator=g) * 0.05
+    est[:, :n_act] += 0.8 * tgt.flip(1) + 0.1 * torch.randn(B, n_act, T, generator=g)
+    if case == "nan_row":
+        est[0, n_est - 1, T // 3] = float("nan")
+    elif case == "constant_target":
+        tgt[0] = torch.tensor([0.37, -1.7, 3.3, 1000.0][:n_act]).view(n_act, 1).expand(n_act, T)
+    elif case == "silent_target":
+        tgt[0, 0] = 0.0
+    elif case == "tie":
+        est[0, 1] = est[0, 0]
+    elif case == "perfect":
+        est[0, :n_act] = tgt[0]
+    return est, tgt
+
+
+def make_degenerate():
+    """``prepost_degenerate.npz``: ``PermInvariantSISDR`` (2 sources, SI-SDRi), ``StabilizedPermInvSISDRMetric``
+    (4 estimated, 1 actual source for the NaN row as FUSS scores it, else 2) and ``PairwiseNegSDR`` (sisdr, 3 sources)
+    on each degenerate case, zero-mean on (which the constant target needs)."""
+    arrays, cases = {}, []
+    g = torch.Generator().manual_seed(2024)
+    B, T = 3, 500
+    ci = 0
+    for case in DEGENERATE_CASES:
+        for metric in ("pit", "stabilized", "pairwise"):
+            k = f"c{ci}/"
+            meta = dict(name=f"{metric}/{case}", case=case, metric=metric, zero_mean=True, B=B, T=T)
+            if metric == "pit":
+                est, tgt = degenerate_signals(case, 2, 2, B, T, g)
+                mix = tgt.sum(1, keepdim=True)
+                improvement = case != "constant_target"      # SI-SDRi against a constant target is -inf - (-inf)
+                fn = ref_sisdr.PermInvariantSISDR(batch_size=B, zero_mean=True, n_sources=2, backward_loss=False,
+                                                  improvement=improvement, return_individual_results=True)
+                with torch.no_grad():
+                    best, perms = fn(est, tgt, initial_mixtures=mix, return_best_permutation=True)
+                allp = fn.permutations_tensor.tolist()
+                arrays[k + "mix"] = mix.numpy()
+                meta["improvement"] = improvement
+            elif metric == "stabilized":
+                n_act = 1 if case == "nan_row" else 2
+                est, tgt = degenerate_signals(case, 4, n_act, B, T, g)
+                fn = ref_sisdr.StabilizedPermInvSISDRMetric(zero_mean=True, n_estimated_sources=4,
+                                                            n_actual_sources=n_act, backward_loss=False,
+                                                            improvement=False, return_individual_results=True)
+                with torch.no_grad():
+                    best, perms = fn(est, tgt, return_best_permutation=True)
+                allp = fn.permutations_tensor.tolist()
+                meta["improvement"] = False
+            else:
+                est, tgt = degenerate_signals(case, 3, 3, B, T, g)
+                with torch.no_grad():
+                    best = -ref_sisdr.PairwiseNegSDR("sisdr", zero_mean=True, take_log=True)(est, tgt)   # SDR in dB
+                meta["sdr_type"] = "sisdr"
+            if metric != "pairwise":
+                idx = torch.tensor([allp.index(r) for r in perms.tolist()], dtype=torch.int64)
+                arrays[k + "idx"] = idx.numpy()
+            arrays.update({k + "est": est.numpy(), k + "tgt": tgt.numpy(), k + "score": best.numpy()})
+            cases.append(meta)
+            print(f"degenerate/c{ci} {meta['name']}: {best.flatten()[:6].numpy()}")
+            ci += 1
+    arrays["meta"] = np.frombuffer(json.dumps(dict(cases=cases, torch=torch.__version__)).encode(), dtype=np.uint8)
+    path = os.path.join(HERE, "prepost_degenerate.npz")
+    np.savez_compressed(path, **arrays)
+    print(f"degenerate: {ci} cases -> {os.path.getsize(path)/1024:.0f} KiB")
+
+
 if __name__ == "__main__":
-    todo = sys.argv[1:] or ["separate", "sisdr", "pairwise", "stabilized"]       # name a subset to leave the other fixtures alone
+    todo = sys.argv[1:] or ["separate", "sisdr", "pairwise", "stabilized", "degenerate"]   # name a subset to leave the other fixtures alone
     for name in todo:
-        {"separate": make_separate, "sisdr": make_sisdr, "pairwise": make_pairwise, "stabilized": make_stabilized}[name]()
+        {"separate": make_separate, "sisdr": make_sisdr, "pairwise": make_pairwise, "stabilized": make_stabilized,
+         "degenerate": make_degenerate}[name]()

@@ -27,11 +27,18 @@ def build(variant, kw, sd):
     return m.to(DEV).eval()
 
 
-@pytest.mark.parametrize("rows,T", [(1, 1000), (5, 517), (32, 32000), (3, 7), (2, 100003)])
-def test_utterance_stats(rows, T):
+@pytest.mark.parametrize("rows,T,r", [pytest.param(rows, T, None, id=f"{rows}-{T}")
+                                      for rows, T in [(1, 1000), (5, 517), (32, 32000), (3, 7), (2, 100003)]]
+                         # 8192-sample chunks, 64 at most per row; r = |mean| / std up to 1e4
+                         + [(3, 8191, 1e4), (3, 8192, 10.0), (3, 8193, 1e3), (2, 524288, 1e4), (2, 524289, 1e4)])
+def test_utterance_stats(rows, T, r):
     g = torch.Generator().manual_seed(rows * 1000 + T)
-    wav = (torch.randn(rows, T, generator=g) * torch.logspace(-2, 1, rows).view(rows, 1)
-           + torch.linspace(-3, 50, rows).view(rows, 1)).to(DEV)          # DC up to 50x the AC level
+    if r is None:
+        wav = (torch.randn(rows, T, generator=g) * torch.logspace(-2, 1, rows).view(rows, 1)
+               + torch.linspace(-3, 50, rows).view(rows, 1)).to(DEV)      # DC up to 50x the AC level
+    else:
+        ac = torch.logspace(-2, 1, rows).view(rows, 1)
+        wav = ((torch.randn(rows, T, generator=g) + r * torch.linspace(-1, 1, rows).view(rows, 1)) * ac).to(DEV)
     ms = torch.full((rows, 2), float("nan"), device=DEV)
     scratch = torch.empty(rows * 2, dtype=torch.float64, device=DEV)
     N.check(N.lib().sdr_utterance_stats(C.c_void_p(wav.data_ptr()), C.c_void_p(ms.data_ptr()), rows, T,

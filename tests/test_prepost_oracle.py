@@ -123,3 +123,44 @@ def test_stabilized_sisdr_matches_reference_golden(ci):
     perms = list(itertools.permutations(range(n_est), r=c["n_act"]))
     assert [perms[int(i)] for i in idx] == [tuple(int(v) for v in row) for row in t["perms"]]
     assert torch.allclose(-best.mean(), t["loss"][0], atol=1e-4, rtol=0)
+
+
+def load_degenerate():
+    z = np.load(os.path.join(GOLDEN_DIR, "prepost_degenerate.npz"))
+    meta = json.loads(bytes(z["meta"]).decode())
+    return [(c, {k[len(f"c{ci}/"):]: torch.from_numpy(z[k]) for k in z.files if k.startswith(f"c{ci}/")})
+            for ci, c in enumerate(meta["cases"])]
+
+
+def _degenerate_oracle(c, t, dtype):
+    est, tgt = t["est"].to(dtype), t["tgt"].to(dtype)
+    if c["metric"] == "pit":
+        return O.pit_sisdr(est, tgt, t["mix"].to(dtype), zero_mean=c["zero_mean"], improvement=c["improvement"])
+    if c["metric"] == "stabilized":
+        return O.stabilized_pit_sisdr(est, tgt, zero_mean=c["zero_mean"], improvement=c["improvement"])
+    return -O.pairwise_neg_sdr(est, tgt, c["sdr_type"], c["zero_mean"], True), None
+
+
+@pytest.mark.parametrize("ci", range(15))
+def test_degenerate_matches_reference_golden(ci):
+    """The metrics on degenerate rows (a NaN sample, a constant target under zero-mean, a silent target, two identical
+    estimates, a perfect estimate) against the unmodified reference: the fp32 oracle to 1e-4 dB with NaN and inf in
+    the same places and the same assignment; the fp64 oracle in the same class (NaN, +inf, -inf or finite), except for
+    the constant target, where rounding decides the fp32 value and both are -inf or at most -60 dB."""
+    c, t = load_degenerate()[ci]
+    ref = t["score"].double()
+    best, idx = _degenerate_oracle(c, t, torch.float32)
+    assert torch.allclose(best.double(), ref, atol=1e-4, rtol=0, equal_nan=True), (c["name"], best, ref)
+    if idx is not None:
+        assert torch.equal(idx, t["idx"]), c["name"]
+    best64, idx64 = _degenerate_oracle(c, t, torch.float64)
+    if idx64 is not None:
+        assert torch.equal(idx64, t["idx"]), c["name"]
+    if c["case"] == "constant_target":
+        for v in (best64[0], ref[0]):
+            assert not torch.isnan(v).any() and bool(((v == -float("inf")) | (v <= -60)).all()), (c["name"], v)
+        best64, ref = best64[1:], ref[1:]
+    cls = lambda v: (torch.isnan(v), v == float("inf"), v == -float("inf"))      # noqa: E731
+    assert all(torch.equal(a, b) for a, b in zip(cls(best64), cls(ref))), (c["name"], best64, ref)
+    if c["case"] == "nan_row" and c["metric"] == "stabilized":      # FUSS's 4 -> 1 scoring: the first NaN assignment
+        assert torch.isnan(ref[0]) and int(t["idx"][0]) == 3
