@@ -382,6 +382,54 @@ int sdr_stabilized_sisdr(const float* est, const float* target, float* best, int
                          int B, int est_rows, int n_est, int n_act, int64_t T,
                          int zero_mean, int improvement, double eps, void* scratch, sdr_stream stream);
 
+/* ---- training of the improved model (variant 0) ---------------------------
+ * sdr_forward_train runs sdr_forward's kernels (same plan, pyramid choice and GEMMs, no mixture consistency) and
+ * also copies into `saved` what the backward recomputes from: the statistics slots, the raw encoder output and every
+ * U-ConvBlock input x_0..x_U, each segment 256-byte aligned (4 B L ((U+1) Co + N) bytes plus the statistics).
+ * sdr_backward takes dL/d(estimates) [B, S, T] and WRITES (never accumulates) the gradient of every parameter into
+ * grad_params: flat fp32, state_dict order, sdr_param_numel(i) floats each, no padding.  Every gradient reduction
+ * runs in a fixed order (no atomics), so a backward is bitwise reproducible.  The gradient with respect to the
+ * mixture is not computed.  Neither call synchronises or allocates; `saved` and the workspaces are 256-byte aligned.
+ * Any other variant: 0 bytes / SDR_ERR_UNSUPPORTED.                                                                  */
+size_t sdr_train_saved_bytes(const sdr_config* cfg, int B, int64_t T);
+size_t sdr_backward_workspace_bytes(const sdr_config* cfg, int B, int64_t T);
+int    sdr_forward_train(const sdr_config* cfg, const void* packed, const float* mixture, float* out, int B, int64_t T,
+                         void* saved, size_t saved_bytes, void* ws, size_t ws_bytes, sdr_stream stream);
+int    sdr_backward(const sdr_config* cfg, const void* packed, const float* mixture, const void* saved,
+                    const float* grad_out, float* grad_params, int B, int64_t T, void* ws, size_t ws_bytes,
+                    sdr_stream stream);
+/* kernels one sdr_backward enqueues (memsets not counted): 22 + U (14 + 5 D + [D > 1]) */
+int    sdr_backward_launch_count(const sdr_config* cfg, int B, int64_t T);
+
+/* stage entries of the backward kernels (activations [samples][channels][L]) */
+/* dW[m][k] = sum_{b,t} dy[b][m][t] f(x[b][k][t]) (f: the deferred GlobLN / PReLU of `fin`, NULL = identity),
+ * db[m] = sum dy; per-CTA fp32 partials over <= 512 positions in `scratch`, summed in fp64 in order */
+size_t sdr_pointwise_wgrad_scratch_bytes(int samples, int M, int Kc, int L);
+int    sdr_pointwise_wgrad(const float* dy, const float* x, const sdr_norm_in* fin, float* dw, float* db_or_null,
+                           void* scratch, int samples, int M, int Kc, int L, sdr_stream stream);
+/* backward of p = PReLU(GlobLN(x)) (fin->stats set) or p = PReLU(x) (fin->stats NULL): dx (or dx += when
+ * accumulate), dgamma / dbeta [C], dslope [1] (each may be NULL); one shared slope only */
+size_t sdr_norm_act_backward_scratch_bytes(int samples, int C);
+int    sdr_norm_act_backward(const float* x, const sdr_norm_in* fin, const float* dp, float* dx, int accumulate,
+                             float* dgamma, float* dbeta, float* dslope, void* scratch, int samples, int C, int L,
+                             sdr_stream stream);
+/* backward of z = dw5(f(x)) (padding 2, stride 1 or 2, Lin even for stride 2): dx[tau] = (dw^T dz)[tau] +
+ * sum_{i < pool_factor} pool[pool_factor tau + i] (dz or pool may be NULL), dw5 [C][5] and dbias [C] */
+size_t sdr_depthwise_backward_scratch_bytes(int samples, int C);
+int    sdr_depthwise_backward(const float* dz, const float* x, const sdr_norm_in* fin, const float* w5,
+                              const float* pool_or_null, int pool_factor, float* dx, float* dw5, float* dbias,
+                              void* scratch, int samples, int C, int Lin, int stride, sdr_stream stream);
+/* masked = relu(mlog) * enc: dmasked [B][S*N][L] becomes dmlog in place, denc [B][N][L] = sum_s dmasked relu(mlog) */
+int    sdr_mask_backward(const float* mlog, const float* enc, float* dmasked, float* denc, int B, int S, int N, int L,
+                         sdr_stream stream);
+/* crop + overlap-add read backwards: grad_frames[b][s K + j][t] = grad_out[b][s][hop t + j - hop] (0 outside [0,T)) */
+int    sdr_overlap_add_backward(const float* grad_out, float* grad_frames, int B, int SA, int K, int L, int64_t T,
+                                sdr_stream stream);
+/* dW[n][j] = sum_{b,t} denc[b][n][t] wav[b][hop t + j - hop] (mono, 0 outside [0, T)) */
+size_t sdr_encoder_wgrad_scratch_bytes(int B, int N, int K, int L);
+int    sdr_encoder_wgrad(const float* denc, const float* wav, float* dw, void* scratch, int B, int N, int K, int L,
+                         int64_t T, sdr_stream stream);
+
 #ifdef __cplusplus
 }
 #endif

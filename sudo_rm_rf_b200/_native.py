@@ -134,6 +134,31 @@ _SIGNATURES = {
     "sdr_stabilized_sisdr_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     "sdr_stabilized_sisdr": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                        C.c_int64, C.c_int, C.c_int, C.c_double, C.c_void_p, C.c_void_p]),
+    "sdr_train_saved_bytes": (C.c_size_t, [C.POINTER(SdrConfig), C.c_int, C.c_int64]),
+    "sdr_backward_workspace_bytes": (C.c_size_t, [C.POINTER(SdrConfig), C.c_int, C.c_int64]),
+    "sdr_forward_train": (C.c_int, [C.POINTER(SdrConfig), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64,
+                                    C.c_void_p, C.c_size_t, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "sdr_backward": (C.c_int, [C.POINTER(SdrConfig), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                               C.c_int, C.c_int64, C.c_void_p, C.c_size_t, C.c_void_p]),
+    "sdr_backward_launch_count": (C.c_int, [C.POINTER(SdrConfig), C.c_int, C.c_int64]),
+    "sdr_pointwise_wgrad_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    "sdr_pointwise_wgrad": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(SdrNormIn), C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_void_p]),
+    "sdr_norm_act_backward_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "sdr_norm_act_backward": (C.c_int, [C.c_void_p, C.POINTER(SdrNormIn), C.c_void_p, C.c_void_p, C.c_int,
+                                        C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                        C.c_void_p]),
+    "sdr_depthwise_backward_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "sdr_depthwise_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.POINTER(SdrNormIn), C.c_void_p, C.c_void_p,
+                                         C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                         C.c_int, C.c_int, C.c_void_p]),
+    "sdr_mask_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                    C.c_int, C.c_void_p]),
+    "sdr_overlap_add_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int, C.c_int64,
+                                           C.c_void_p]),
+    "sdr_encoder_wgrad_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int]),
+    "sdr_encoder_wgrad": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                    C.c_int, C.c_int64, C.c_void_p]),
 }
 
 EXPORTED_SYMBOLS = tuple(_SIGNATURES)

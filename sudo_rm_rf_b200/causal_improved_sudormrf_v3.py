@@ -111,6 +111,11 @@ class CausalSuDORMRF(_engine.NativeModuleMixin, nn.Module):
             return tensor / float(blk.beta) if float(blk.beta) != 1.0 else tensor
         return tensor
 
+    def enable_training(self, enabled: bool = True):
+        """Native training covers the improved SuDORMRF only."""
+        raise NotImplementedError("CausalSuDORMRF: native training (enable_training) covers the improved SuDORMRF "
+                                  "only; the causal model has no backward kernels")
+
     def forward(self, input_wav):
         """[B, in_audio_channels, T] mixture -> [B, num_sources * in_audio_channels, T] estimates (fp32)."""
         return _engine.forward(self, input_wav, mixture_consistency=False)

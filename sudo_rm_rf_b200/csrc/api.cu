@@ -69,6 +69,20 @@ int pack_pointwise_mma(const float* W, int M, int K, void* packed, cudaStream_t)
 int launch_pointwise_mma(const float*, const NormIn&, const void*, const float*, const float*, const float*, int,
                          float*, double*, int, int, int, int, int, cudaStream_t);
 
+// backward of the improved model (backward.cu)
+size_t wgrad_scratch_bytes(int samples, int M, int K, int L);
+int launch_wgrad(const float*, const float*, const NormIn&, float*, float*, float*, int, int, int, int, cudaStream_t);
+size_t norm_bwd_scratch_bytes(int samples, int C);
+int launch_norm_bwd(const float*, const NormIn&, const float*, float*, int, float*, float*, float*, double*, int, int,
+                    int, cudaStream_t);
+size_t dw_bwd_scratch_bytes(int samples, int C);
+int launch_dw_bwd(const float*, const float*, const NormIn&, const float*, const float*, int, float*, float*, float*,
+                  double*, int, int, int, int, cudaStream_t);
+int launch_mask_apply(const float*, const float*, float*, int, int, int, int, cudaStream_t);
+int launch_mask_bwd(const float*, const float*, float*, float*, int, int, int, int, cudaStream_t);
+int launch_frame_gather(const float*, float*, int, int, int, int, long long, cudaStream_t);
+int launch_transpose(const float*, float*, int, int, cudaStream_t);
+
 size_t encoder_mma_packed_bytes(int N, int A, int Kk);
 int pack_encoder_mma(const float* W, int N, int A, int Kk, void* packed, cudaStream_t);
 int launch_encoder_mma(const float*, const void*, const float*, int, float*, double*, int, int, long long, int, int, int, int, cudaStream_t);
@@ -598,9 +612,33 @@ static int forward_original(const Layout& l, const Plan& p, const float* pk, con
     return decoder_tail(l, p, pk, none, pk + l.dec_b, mixture, apply_mc, rescale, out, B, T, ws, st);   // :291
 }
 
+// What a training forward keeps for the backward (improved model): the forward's statistics slots, the raw encoder
+// output e and every block input x_0..x_U (x_U feeds the mask), each segment 256-byte aligned.
+struct Saved {
+    size_t o_stats, o_e, o_x, x_stride, total;
+    const float* x(const char* s, int i) const { return reinterpret_cast<const float*>(s + o_x + (size_t)i * x_stride); }
+};
+static Saved saved_layout(const Layout& l, const Plan& p, int B) {
+    Saved s;
+    size_t cur = 0;
+    auto seg = [&](size_t bytes) { size_t o = cur; cur += (bytes + 255) & ~(size_t)255; return o; };
+    const size_t BL = (size_t)B * p.L * sizeof(float);
+    s.o_stats = seg(p.stats_doubles * sizeof(double));
+    s.o_e = seg(BL * l.N);
+    s.x_stride = (BL * l.Co + 255) & ~(size_t)255;
+    s.o_x = cur;
+    s.total = cur + s.x_stride * (l.U + 1);
+    return s;
+}
+
+static int copy_d2d(void* dst, const void* src, size_t bytes, cudaStream_t st) {
+    return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st) == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+}
+
+// `save` (improved model only, else null): the training forward's copy of what saved_layout lists.
 static int forward_impl(const Layout& l, const Plan& p, const float* pk, const float* mixture, float* out,
                         int B, long long T, int apply_mc, char* ws, cudaStream_t st,
-                        const float2* rescale = nullptr) {
+                        const float2* rescale = nullptr, char* save = nullptr) {
     // mixture_consistency.apply (mixture_consistency.py:14-36) sums the estimates over dim 1 and broadcasts against a
     // [B, 1, T] mixture: it is only defined for mono models; refuse instead of silently skipping the projection
     if (apply_mc && l.A != 1) return SDR_ERR_UNSUPPORTED;
@@ -622,6 +660,9 @@ static int forward_impl(const Layout& l, const Plan& p, const float* pk, const f
         NormIn ln{p.stats(ws), pk + l.ln_g, pk + l.ln_be, nullptr, (double)l.N * L, 0};
         SDR_TRY(pointwise(e, ln, pk, l.bn_w, l.bn_pk, pk + l.bn_b, nullptr, nullptr, 0, x, nullptr, B, l.Co, l.N, L, 0, st));
     }
+    const Saved sv = save ? saved_layout(l, p, B) : Saved{};
+    const size_t xbytes = (size_t)B * L * l.Co * sizeof(float);
+    if (save) SDR_TRY(copy_d2d(save + sv.o_x, x, xbytes, st));
     // separation module
     const int ns = p.samples, cob = l.cob, cib = l.cib;
     for (int i = 0; i < l.U; ++i) {
@@ -653,6 +694,11 @@ static int forward_impl(const Layout& l, const Plan& p, const float* pk, const f
             NormIn nf{p.slot(ws, i, D + 1), pk + u.fn_g, pk + u.fn_be, pk + u.fn_a, (double)cib * L, 0};
             SDR_TRY(pointwise(y, nf, pk, u.res_w, u.res_pk, pk + u.res_b, bin, nullptr, 0, x, nullptr, ns, cob, cib, L, 0, st));
         }
+        if (save) SDR_TRY(copy_d2d(save + sv.o_x + (size_t)(i + 1) * sv.x_stride, x, xbytes, st));
+    }
+    if (save) {
+        SDR_TRY(copy_d2d(save + sv.o_e, e, (size_t)B * L * l.N * sizeof(float), st));
+        SDR_TRY(copy_d2d(save + sv.o_stats, p.stats(ws), p.stats_doubles * sizeof(double), st));
     }
     // mask: PReLU -> 1x1 -> ReLU -> * encoder output
     {
@@ -662,6 +708,181 @@ static int forward_impl(const Layout& l, const Plan& p, const float* pk, const f
     }
     // decoder: frames = Wd^T masked, then overlap-add / crop / mixture consistency
     return decoder_tail(l, p, pk, none, nullptr, mixture, apply_mc, rescale, out, B, T, ws, st);
+}
+
+// ---------------------------------------------------------------------------
+// backward of the improved model: workspace plan and orchestration
+// ---------------------------------------------------------------------------
+// Transposed 1x1 weights for the input-gradient GEMMs, one block's recomputed tensors and their statistics, the
+// gradient buffers, and the scratch of the fixed-order reductions.  Every activation buffer is [B][channels][L].
+struct BwdPlan {
+    size_t o_wt_mask, o_wt_bn, o_wt_p, o_wt_r, wt_block;    // wt_p / wt_r: per block, wt_block bytes apart
+    size_t o_stats, o_dx, o_y, o_m, o_z[kMaxDepthApi], o_dn[kMaxDepthApi], o_dp;
+    size_t o_mlog, o_dmask, o_frames, o_de, o_dq, o_win;
+    size_t o_npart, o_dwpart, o_wpart, total;
+    float* buf(char* ws, size_t o) const { return reinterpret_cast<float*>(ws + o); }
+};
+
+static BwdPlan make_bwd_plan(const Layout& l, const Plan& p, int B) {
+    BwdPlan b;
+    size_t cur = 0;
+    auto seg = [&](size_t bytes) { size_t o = cur; cur += (bytes + 255) & ~(size_t)255; return o; };
+    const size_t F = sizeof(float), BL = (size_t)B * p.L * F;
+    const int L = p.L, Co = l.Co, Ci = l.Ci, N = l.N, SN = l.S * l.N, SK = l.S * l.K;
+    b.o_wt_mask = seg((size_t)SN * Co * F);
+    b.o_wt_bn = seg((size_t)N * Co * F);
+    b.wt_block = ((size_t)Co * Ci * F + 255) & ~(size_t)255;
+    b.o_wt_p = cur; cur += b.wt_block * l.U;
+    b.o_wt_r = cur; cur += b.wt_block * l.U;
+    b.o_stats = seg((size_t)(l.D + 2) * B * 2 * sizeof(double));
+    b.o_dx = seg(BL * Co);
+    b.o_y = seg(BL * Ci);
+    b.o_m = seg(BL * Ci);
+    for (int d = 0; d < kMaxDepthApi; ++d) b.o_z[d] = d < l.D ? seg((BL * Ci) >> d) : 0;
+    for (int d = 0; d < kMaxDepthApi; ++d) b.o_dn[d] = d < l.D ? seg((BL * Ci) >> d) : 0;
+    b.o_dp = seg(BL * Ci);
+    b.o_mlog = seg(BL * SN);
+    b.o_dmask = seg(BL * SN);
+    b.o_frames = seg(BL * SK);
+    b.o_de = seg(BL * N);
+    b.o_dq = seg(BL * (Co > N ? Co : N));
+    b.o_win = seg(BL * l.K);
+    const int cmax = Ci > Co ? (Ci > N ? Ci : N) : (Co > N ? Co : N);
+    b.o_npart = seg(norm_bwd_scratch_bytes(B, cmax));
+    b.o_dwpart = seg(dw_bwd_scratch_bytes(B, Ci));
+    // every weight-gradient GEMM the backward runs: decoder, mask, res_conv, proj_1x1, bottleneck, encoder
+    const int shapes[6][2] = {{SN, SK}, {SN, Co}, {Co, Ci}, {Ci, Co}, {Co, N}, {N, l.K}};
+    size_t wp = 0;
+    for (const auto& s : shapes) { const size_t w = wgrad_scratch_bytes(B, s[0], s[1], L); wp = w > wp ? w : wp; }
+    b.o_wpart = seg(wp);
+    b.total = cur;
+    return b;
+}
+
+// Kernels one backward enqueues: transposes (2 + 2U), mask and decoder (12), per block (12 + 5D, + 1 pooling launch
+// when D > 1), bottleneck, ln and encoder (8).
+static int bwd_launch_count(const Layout& l) {
+    return 2 + 2 * l.U + 12 + l.U * (12 + 5 * l.D + (l.D > 1 ? 1 : 0)) + 8;
+}
+
+// grads: flat fp32, state_dict order, each tensor sdr_param_numel floats.  Written, never accumulated.
+static int backward_impl(const Layout& l, const Plan& p, const BwdPlan& bp, const float* pk, const float* mixture,
+                         const char* saved, const float* gout, float* grads, int B, long long T, char* ws,
+                         cudaStream_t st) {
+    const int L = p.L, D = l.D, N = l.N, Co = l.Co, Ci = l.Ci, S = l.S, K = l.K, SN = S * N, SK = S * K;
+    const Saved sv = saved_layout(l, p, B);
+    const float* e = reinterpret_cast<const float*>(saved + sv.o_e);
+    const double* fstats = reinterpret_cast<const double*>(saved + sv.o_stats);   // slot 0: the encoder output's
+    std::vector<size_t> goff(l.off.size());
+    for (size_t i = 0, acc = 0; i < l.off.size(); ++i) { goff[i] = acc; acc += l.numel[i]; }
+    auto G = [&](size_t packed_off) -> float* {           // gradient of the parameter stored at packed_off
+        for (size_t i = 0; i < l.off.size(); ++i)
+            if (l.off[i] == packed_off) return grads + goff[i];
+        return nullptr;
+    };
+    const NormIn none{nullptr, nullptr, nullptr, nullptr, 1.0, 0};
+    double* nsc = reinterpret_cast<double*>(ws + bp.o_npart);
+    double* dsc = reinterpret_cast<double*>(ws + bp.o_dwpart);
+    float* wsc = bp.buf(ws, bp.o_wpart);
+    float* wt_mask = bp.buf(ws, bp.o_wt_mask);
+    float* wt_bn = bp.buf(ws, bp.o_wt_bn);
+    auto wt_p = [&](int i) { return bp.buf(ws, bp.o_wt_p + (size_t)i * bp.wt_block); };
+    auto wt_r = [&](int i) { return bp.buf(ws, bp.o_wt_r + (size_t)i * bp.wt_block); };
+    SDR_TRY(launch_transpose(pk + l.mask_w, wt_mask, SN, Co, st));                 // [Co][S*N]
+    SDR_TRY(launch_transpose(pk + l.bn_w, wt_bn, Co, N, st));                      // [N][Co]
+    for (int i = 0; i < l.U; ++i) {
+        SDR_TRY(launch_transpose(pk + l.ub[i].proj_w, wt_p(i), Ci, Co, st));       // [Co][Ci]
+        SDR_TRY(launch_transpose(pk + l.ub[i].res_w, wt_r(i), Co, Ci, st));        // [Ci][Co]
+    }
+    float* dx = bp.buf(ws, bp.o_dx);
+    float* mlog = bp.buf(ws, bp.o_mlog);
+    float* dmask = bp.buf(ws, bp.o_dmask);
+    float* frames = bp.buf(ws, bp.o_frames);
+    float* de = bp.buf(ws, bp.o_de);
+    float* dq = bp.buf(ws, bp.o_dq);
+
+    // mask and decoder: mlog = W_m PReLU_m(x_U) + b_m, masked = relu(mlog) * e, frames = Wd^T masked, crop + overlap-add
+    const float* xU = sv.x(saved, l.U);
+    const NormIn pm{nullptr, nullptr, nullptr, pk + l.mask_a, 1.0, 0};
+    SDR_TRY(launch_pointwise_ffma(xU, pm, pk + l.mask_w, pk + l.mask_b, nullptr, nullptr, 0, mlog, nullptr,
+                                  B, SN, Co, L, 0, st));      // fp32: the ReLU mask bits follow the logits closely
+    SDR_TRY(launch_mask_apply(mlog, e, dmask, B, S, N, L, st));                    // dmask holds masked for now
+    SDR_TRY(launch_frame_gather(gout, frames, B, S, K, L, T, st));                 // dF
+    SDR_TRY(launch_wgrad(dmask, frames, none, G(l.dec_w), nullptr, wsc, B, SN, SK, L, st));   // [S*N][S][K] layout
+    SDR_TRY(launch_pointwise_ffma(frames, none, pk + l.dec_w, nullptr, nullptr, nullptr, 0, dmask, nullptr,
+                                  B, SN, SK, L, 0, st));                           // dmasked = Wd dF
+    SDR_TRY(launch_mask_bwd(mlog, e, dmask, de, B, S, N, L, st));                  // dmlog (in dmask), de
+    SDR_TRY(launch_wgrad(dmask, xU, pm, G(l.mask_w), G(l.mask_b), wsc, B, SN, Co, L, st));
+    SDR_TRY(launch_pointwise_ffma(dmask, none, wt_mask, nullptr, nullptr, nullptr, 0, dq, nullptr,
+                                  B, Co, SN, L, 0, st));                           // W_m^T dmlog
+    SDR_TRY(launch_norm_bwd(xU, pm, dq, dx, 0, nullptr, nullptr, G(l.mask_a), nsc, B, Co, L, st));   // dx_U
+
+    // U-ConvBlocks, last to first: recompute from x_i, then backward; dx carries the residual stream's gradient
+    double* bst = reinterpret_cast<double*>(ws + bp.o_stats);
+    auto slot = [&](int k) { return bst + (size_t)k * B * 2; };
+    float* y = bp.buf(ws, bp.o_y);
+    float* m = bp.buf(ws, bp.o_m);
+    float* dp = bp.buf(ws, bp.o_dp);
+    float* z[kMaxDepthApi];
+    float* dn[kMaxDepthApi];
+    const float* zc[kMaxDepthApi];
+    for (int d = 0; d < D; ++d) { zc[d] = z[d] = bp.buf(ws, bp.o_z[d]); dn[d] = bp.buf(ws, bp.o_dn[d]); }
+    for (int i = l.U - 1; i >= 0; --i) {
+        const UBlockOff& u = l.ub[i];
+        const float* xi = sv.x(saved, i);
+        if (cudaMemsetAsync(bst, 0, (size_t)(D + 2) * B * 2 * sizeof(double), st) != cudaSuccess) return SDR_ERR_CUDA;
+        SDR_TRY(pointwise(xi, none, pk, u.proj_w, u.proj_pk, pk + u.proj_b, nullptr, nullptr, 0, y, slot(0),
+                          B, Ci, Co, L, 0, st));
+        const NormIn n0{slot(0), pk + u.proj_g, pk + u.proj_be, pk + u.proj_a, (double)Ci * L, 0};
+        NormIn nl[kMaxDepthApi];
+        for (int d = 0; d < D; ++d)
+            nl[d] = NormIn{slot(1 + d), pk + u.dw_g[d], pk + u.dw_be[d], nullptr, (double)Ci * (L >> d), 0};
+        SDR_TRY(launch_depthwise(y, n0, pk + u.dw_w[0], pk + u.dw_b[0], z[0], slot(1), B, Ci, L, 1, st));
+        for (int d = 1; d < D; ++d)
+            SDR_TRY(launch_depthwise(z[d - 1], nl[d - 1], pk + u.dw_w[d], pk + u.dw_b[d], z[d], slot(1 + d),
+                                     B, Ci, L >> (d - 1), 2, st));
+        SDR_TRY(launch_merge(zc, nl, D, m, slot(D + 1), B, Ci, L, st));
+        const NormIn nf{slot(D + 1), pk + u.fn_g, pk + u.fn_be, pk + u.fn_a, (double)Ci * L, 0};
+
+        // out = W_r PReLU_f(GLN_f(m)) + b_r + x
+        SDR_TRY(launch_wgrad(dx, m, nf, G(u.res_w), G(u.res_b), wsc, B, Co, Ci, L, st));
+        SDR_TRY(launch_pointwise_ffma(dx, none, wt_r(i), nullptr, nullptr, nullptr, 0, dp, nullptr,
+                                      B, Ci, Co, L, 0, st));
+        SDR_TRY(launch_norm_bwd(m, nf, dp, dp, 0, G(u.fn_g), G(u.fn_be), G(u.fn_a), nsc, B, Ci, L, st));   // dm
+        // m[t] = sum_d n_d[t >> d]: the deepest level's gradient is dm pooled; the others get theirs from the
+        // depthwise backward of the level below them
+        const float* up = dp;
+        if (D > 1) {
+            SDR_TRY(launch_dw_bwd(nullptr, nullptr, none, nullptr, dp, 1 << (D - 1), dn[D - 1], nullptr, nullptr,
+                                  nullptr, B, Ci, L >> (D - 1), 2, st));
+            up = dn[D - 1];
+        }
+        for (int d = D - 1; d >= 0; --d) {
+            const int Ld = L >> d;
+            SDR_TRY(launch_norm_bwd(z[d], nl[d], up, dn[d], 0, G(u.dw_g[d]), G(u.dw_be[d]), nullptr, nsc,
+                                    B, Ci, Ld, st));                               // dz_d
+            if (d > 0)      // dn_{d-1} = pool(dm) + dw_d^T dz_d
+                SDR_TRY(launch_dw_bwd(dn[d], z[d - 1], nl[d - 1], pk + u.dw_w[d], dp, 1 << (d - 1), dn[d - 1],
+                                      G(u.dw_w[d]), G(u.dw_b[d]), dsc, B, Ci, L >> (d - 1), 2, st));
+            else            // gradient of PReLU_p(GLN_p(y)), over dm (no longer needed)
+                SDR_TRY(launch_dw_bwd(dn[0], y, n0, pk + u.dw_w[0], nullptr, 0, dp, G(u.dw_w[0]), G(u.dw_b[0]), dsc,
+                                      B, Ci, L, 1, st));
+            up = d > 0 ? dn[d - 1] : nullptr;
+        }
+        SDR_TRY(launch_norm_bwd(y, n0, dp, dp, 0, G(u.proj_g), G(u.proj_be), G(u.proj_a), nsc, B, Ci, L, st));   // dy
+        SDR_TRY(launch_wgrad(dp, xi, none, G(u.proj_w), G(u.proj_b), wsc, B, Ci, Co, L, st));
+        SDR_TRY(launch_pointwise_ffma(dp, none, wt_p(i), nullptr, dx, nullptr, 0, dx, nullptr,
+                                      B, Co, Ci, L, 0, st));                       // dx += W_p^T dy
+    }
+
+    // x_0 = W_bn GLN_ln(e) + b_bn; e = encoder(mixture)
+    const NormIn ln{fstats, pk + l.ln_g, pk + l.ln_be, nullptr, (double)N * L, 0};
+    SDR_TRY(launch_wgrad(dx, e, ln, G(l.bn_w), G(l.bn_b), wsc, B, Co, N, L, st));
+    SDR_TRY(launch_pointwise_ffma(dx, none, wt_bn, nullptr, nullptr, nullptr, 0, dq, nullptr, B, N, Co, L, 0, st));
+    SDR_TRY(launch_norm_bwd(e, ln, dq, de, 1, G(l.ln_g), G(l.ln_be), nullptr, nsc, B, N, L, st));   // de += GLN bwd
+    float* win = bp.buf(ws, bp.o_win);
+    SDR_TRY(launch_frame_gather(mixture, win, B, 1, K, L, T, st));                 // the encoder's input windows
+    return launch_wgrad(de, win, none, G(l.enc_w), nullptr, wsc, B, N, K, L, st);
 }
 
 }  // namespace sdr
@@ -800,6 +1021,125 @@ int sdr_forward_launch_count_for(const sdr_config* cfg, int B, int64_t T) {
     const Layout l = make_layout(cfg);
     if (!l.ok || B <= 0 || T <= 0) return SDR_ERR_BAD_CONFIG;
     return launch_count(l, make_plan(l, B, T));
+}
+
+// ---- training of the improved model: forward that keeps what the backward needs, and the backward ----
+
+static int check_train_args(const Layout& l, int B, int64_t T) {
+    if (!l.ok) return SDR_ERR_BAD_CONFIG;
+    if (l.gc || l.causal || l.orig) return SDR_ERR_UNSUPPORTED;     // improved model only
+    return check_forward_args(l, B, T);
+}
+
+size_t sdr_train_saved_bytes(const sdr_config* cfg, int B, int64_t T) {
+    const Layout l = make_layout(cfg);
+    if (check_train_args(l, B, T) != SDR_OK) return 0;
+    return saved_layout(l, make_plan(l, B, T), B).total;
+}
+
+size_t sdr_backward_workspace_bytes(const sdr_config* cfg, int B, int64_t T) {
+    const Layout l = make_layout(cfg);
+    if (check_train_args(l, B, T) != SDR_OK) return 0;
+    return make_bwd_plan(l, make_plan(l, B, T), B).total;
+}
+
+int sdr_forward_train(const sdr_config* cfg, const void* packed, const float* mixture, float* out, int B, int64_t T,
+                      void* saved, size_t saved_bytes, void* ws, size_t ws_bytes, sdr_stream stream) {
+    const Layout l = make_layout(cfg);
+    SDR_TRY(check_train_args(l, B, T));
+    if (!packed || !mixture || !out || !saved || !ws) return SDR_ERR_BAD_ARGUMENT;
+    const Plan p = make_plan(l, B, T);
+    if (ws_bytes < p.total || saved_bytes < saved_layout(l, p, B).total) return SDR_ERR_WORKSPACE;
+    if (reinterpret_cast<uintptr_t>(ws) % 256 || reinterpret_cast<uintptr_t>(saved) % 256 ||
+        reinterpret_cast<uintptr_t>(packed) % 16)
+        return SDR_ERR_BAD_ARGUMENT;
+    return forward_impl(l, p, static_cast<const float*>(packed), mixture, out, B, T, 0, static_cast<char*>(ws),
+                        static_cast<cudaStream_t>(stream), nullptr, static_cast<char*>(saved));
+}
+
+int sdr_backward(const sdr_config* cfg, const void* packed, const float* mixture, const void* saved,
+                 const float* grad_out, float* grad_params, int B, int64_t T, void* ws, size_t ws_bytes,
+                 sdr_stream stream) {
+    const Layout l = make_layout(cfg);
+    SDR_TRY(check_train_args(l, B, T));
+    if (!packed || !mixture || !saved || !grad_out || !grad_params || !ws) return SDR_ERR_BAD_ARGUMENT;
+    const Plan p = make_plan(l, B, T);
+    const BwdPlan bp = make_bwd_plan(l, p, B);
+    if (ws_bytes < bp.total) return SDR_ERR_WORKSPACE;
+    if (reinterpret_cast<uintptr_t>(ws) % 256 || reinterpret_cast<uintptr_t>(saved) % 256 ||
+        reinterpret_cast<uintptr_t>(packed) % 16)
+        return SDR_ERR_BAD_ARGUMENT;
+    return backward_impl(l, p, bp, static_cast<const float*>(packed), mixture, static_cast<const char*>(saved),
+                         grad_out, grad_params, B, T, static_cast<char*>(ws), static_cast<cudaStream_t>(stream));
+}
+
+int sdr_backward_launch_count(const sdr_config* cfg, int B, int64_t T) {
+    const Layout l = make_layout(cfg);
+    SDR_TRY(check_train_args(l, B, T));
+    return bwd_launch_count(l);
+}
+
+// stage entries of the backward kernels
+size_t sdr_pointwise_wgrad_scratch_bytes(int samples, int M, int Kc, int L) {
+    if (samples <= 0 || M <= 0 || Kc <= 0 || L <= 0) return 0;
+    return wgrad_scratch_bytes(samples, M, Kc, L);
+}
+
+int sdr_pointwise_wgrad(const float* dy, const float* x, const sdr_norm_in* fin, float* dw, float* db_or_null,
+                        void* scratch, int samples, int M, int Kc, int L, sdr_stream stream) {
+    return launch_wgrad(dy, x, make_norm(fin), dw, db_or_null, static_cast<float*>(scratch), samples, M, Kc, L,
+                        static_cast<cudaStream_t>(stream));
+}
+
+size_t sdr_norm_act_backward_scratch_bytes(int samples, int C) {
+    return samples > 0 && C > 0 ? norm_bwd_scratch_bytes(samples, C) : 0;
+}
+
+int sdr_norm_act_backward(const float* x, const sdr_norm_in* fin, const float* dp, float* dx, int accumulate,
+                          float* dgamma, float* dbeta, float* dslope, void* scratch, int samples, int C, int L,
+                          sdr_stream stream) {
+    if (scratch && reinterpret_cast<uintptr_t>(scratch) % 8) return SDR_ERR_BAD_ARGUMENT;
+    return launch_norm_bwd(x, make_norm(fin), dp, dx, accumulate, dgamma, dbeta, dslope, static_cast<double*>(scratch),
+                           samples, C, L, static_cast<cudaStream_t>(stream));
+}
+
+size_t sdr_depthwise_backward_scratch_bytes(int samples, int C) {
+    return samples > 0 && C > 0 ? dw_bwd_scratch_bytes(samples, C) : 0;
+}
+
+int sdr_depthwise_backward(const float* dz, const float* x, const sdr_norm_in* fin, const float* w5,
+                           const float* pool_or_null, int pool_factor, float* dx, float* dw5, float* dbias,
+                           void* scratch, int samples, int C, int Lin, int stride, sdr_stream stream) {
+    if (scratch && reinterpret_cast<uintptr_t>(scratch) % 8) return SDR_ERR_BAD_ARGUMENT;
+    return launch_dw_bwd(dz, x, make_norm(fin), w5, pool_or_null, pool_factor, dx, dw5, dbias,
+                         static_cast<double*>(scratch), samples, C, Lin, stride, static_cast<cudaStream_t>(stream));
+}
+
+int sdr_mask_backward(const float* mlog, const float* enc, float* dmasked, float* denc, int B, int S, int N, int L,
+                      sdr_stream stream) {
+    return launch_mask_bwd(mlog, enc, dmasked, denc, B, S, N, L, static_cast<cudaStream_t>(stream));
+}
+
+int sdr_overlap_add_backward(const float* grad_out, float* grad_frames, int B, int SA, int K, int L, int64_t T,
+                             sdr_stream stream) {
+    return launch_frame_gather(grad_out, grad_frames, B, SA, K, L, T, static_cast<cudaStream_t>(stream));
+}
+
+size_t sdr_encoder_wgrad_scratch_bytes(int B, int N, int K, int L) {
+    if (B <= 0 || N <= 0 || K <= 0 || L <= 0) return 0;
+    return (((size_t)B * K * L * sizeof(float) + 255) & ~(size_t)255) + wgrad_scratch_bytes(B, N, K, L);
+}
+
+int sdr_encoder_wgrad(const float* denc, const float* wav, float* dw, void* scratch, int B, int N, int K, int L,
+                      int64_t T, sdr_stream stream) {
+    if (!scratch || reinterpret_cast<uintptr_t>(scratch) % 16) return SDR_ERR_BAD_ARGUMENT;
+    cudaStream_t st = static_cast<cudaStream_t>(stream);
+    float* win = static_cast<float*>(scratch);
+    float* part = reinterpret_cast<float*>(static_cast<char*>(scratch) +
+                                           (((size_t)B * K * L * sizeof(float) + 255) & ~(size_t)255));
+    SDR_TRY(launch_frame_gather(wav, win, B, 1, K, L, T, st));
+    const NormIn none{nullptr, nullptr, nullptr, nullptr, 1.0, 0};
+    return launch_wgrad(denc, win, none, dw, nullptr, part, B, N, K, L, st);
 }
 
 // ---- streaming of the causal model ----

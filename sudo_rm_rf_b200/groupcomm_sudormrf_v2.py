@@ -82,6 +82,11 @@ class GroupCommSudoRmRf(_engine.NativeModuleMixin, nn.Module):
         _xavier_uniform_(self.decoder.weight)
         self.mask_nl_class = nn.ReLU()
 
+    def enable_training(self, enabled: bool = True):
+        """Native training covers the improved SuDORMRF only."""
+        raise NotImplementedError("GroupCommSudoRmRf: native training (enable_training) covers the improved SuDORMRF "
+                                  "only; the GroupComm model (TAC backward) has no backward kernels")
+
     def forward(self, input_wav):
         """[B, in_audio_channels, T] -> [B, num_sources*in_audio_channels, T]."""
         return _engine.forward(self, input_wav, mixture_consistency=False)

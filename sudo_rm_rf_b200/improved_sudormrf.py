@@ -7,8 +7,12 @@ reference's notebooks, ``dnn/experiments`` runners, ``load_state_dict`` of
 published checkpoints and ``torch.load`` of whole-module pickles keep working.
 The arithmetic of ``SuDORMRF.forward`` (improved_sudormrf.py:283-301) is done
 by hand-written sm_90a kernels behind ``include/sudormrf_b200.h``; the
-sub-modules below only own the parameters.  Inference only: there is no
-autograd through the native path and no CPU path.
+sub-modules below only own the parameters.  There is no CPU path.
+
+``enable_training()`` makes ``model(wav)`` differentiable with respect to every
+parameter (sudo_rm_rf_b200/training.py: native sm_90a backward kernels behind
+one autograd function) whenever grad mode is on and a parameter requires grad;
+otherwise, and by default, the forward is inference only.
 """
 import math
 
@@ -16,6 +20,7 @@ import torch
 import torch.nn as nn
 
 from . import _engine
+from . import training
 
 
 def _not_standalone(self, *_, **__):
@@ -137,9 +142,23 @@ class SuDORMRF(_engine.NativeModuleMixin, nn.Module):
                                           output_padding=hop - 1, groups=1, bias=False)
         _xavier_uniform_(self.decoder.weight)
         self.mask_nl_class = nn.ReLU()
+        self.native_training = False
+
+    def enable_training(self, enabled: bool = True):
+        """Make ``model(wav)`` differentiable on the native path (off by default).
+
+        With it on, grad mode enabled and a parameter requiring grad, ``model(wav)`` returns estimates with a
+        ``grad_fn`` in train and eval mode alike, and ``backward()`` fills every parameter's ``.grad``.  The flag
+        is a plain attribute: it travels with ``copy.deepcopy``, ``torch.save`` of the module and
+        ``nn.DataParallel`` replicas, and is not part of ``state_dict()``.  ``separate``, ``forward_host`` and the
+        streaming / corpus paths stay inference only."""
+        self.native_training = bool(enabled)
+        return self
 
     def forward(self, input_wav):
         """[B, 1, T] mixture -> [B, num_sources, T] estimates (fp32, same device)."""
+        if training.wants_autograd(self, input_wav):
+            return training.forward(self, input_wav)
         return _engine.forward(self, input_wav, mixture_consistency=False)
 
     def separate(self, input_wav, mixture_consistency=False, normalize=False):

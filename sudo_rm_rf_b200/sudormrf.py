@@ -131,6 +131,11 @@ class SuDORMRF(_engine.NativeModuleMixin, nn.Module):
                                           padding=hop, groups=num_sources)
         self.ln_mask_in = nn.GroupNorm(1, enc_num_basis, eps=1e-08)      # registered by the reference (:253), never used
 
+    def enable_training(self, enabled: bool = True):
+        """Native training covers the improved SuDORMRF only."""
+        raise NotImplementedError("SuDORMRF (original, sudormrf.py): native training (enable_training) covers the improved SuDORMRF "
+                                  "only; the original model has no backward kernels")
+
     def forward(self, input_wav):
         """[B, 1, T] mixture -> [B, num_sources, T] estimates (fp32, same device)."""
         return _engine.forward(self, input_wav, mixture_consistency=False)
