@@ -4,6 +4,7 @@
 // caller's stream.
 #include <vector>
 #include <cstring>
+#include <initializer_list>
 #include "common.cuh"
 
 #define SDR_TRY(expr) do { int _e = (expr); if (_e != SDR_OK) return _e; } while (0)
@@ -87,50 +88,47 @@ size_t encoder_mma_packed_bytes(int N, int A, int Kk);
 int pack_encoder_mma(const float* W, int N, int A, int Kk, void* packed, cudaStream_t);
 int launch_encoder_mma(const float*, const void*, const float*, int, float*, double*, int, int, long long, int, int, int, int, cudaStream_t);
 
-// One 1x1 convolution with the weight at pk + w_off: tensor cores when its image was packed (pk_off != 0, the channel
-// counts fill a wgmma tile), FFMA otherwise.
-static int pointwise(const float* x, const NormIn& nin, const float* pk, size_t w_off, size_t pk_off, const float* bias,
-                     const float* residual, const float* gate, int gate_channels, float* y, double* stats,
-                     int samples, int M, int K, int L, int epilogue, cudaStream_t st) {
-    if (pk_off && (L % 4) == 0)    // the tensor-core kernel loads activations as float4
-        return launch_pointwise_mma(x, nin, pk + pk_off, bias, residual, gate, gate_channels, y, stats,
-                                    samples, M, K, L, epilogue, st);
-    return launch_pointwise_ffma(x, nin, pk + w_off, bias, residual, gate, gate_channels, y, stats,
-                                 samples, M, K, L, epilogue, st);
-}
+static const NormIn kNoNorm{nullptr, nullptr, nullptr, nullptr, 1.0, 0};   // operand read as stored
 
 // ---------------------------------------------------------------------------
 // parameter layout: offsets (in floats) of every tensor inside the packed buffer
 // ---------------------------------------------------------------------------
+// A tensor of the packed buffer: its offset there and, for a state_dict entry, its offset in the flat gradient buffer
+// of sdr_backward.  It converts to the packed offset (0 = absent), so `pk + p` addresses the tensor.
+struct Param {
+    size_t off = 0, grad = 0;
+    operator size_t() const { return off; }
+};
+// One 1x1 convolution: [M][K] weight w, bias b (absent when 0) and the bf16 hi/lo, pre-swizzled tensor-core image of w
+// at pk (0 = the channel counts do not fill a wgmma tile -> FFMA kernel).
+struct Conv1x1 { Param w, b; size_t pk = 0; int M = 0, K = 0; };
+
 // What the improved / GroupComm block and the original block share: proj_1x1 (conv, norm, PReLU), spp_dw[d]
 // (depthwise conv, norm) and final_norm (norm, PReLU), so one depthwise stage takes either.
 struct NormBlockOff {
-    size_t proj_w, proj_b, proj_g, proj_be, proj_a;
-    size_t dw_w[kMaxDepthApi], dw_b[kMaxDepthApi], dw_g[kMaxDepthApi], dw_be[kMaxDepthApi];
-    size_t fn_g, fn_be, fn_a;
-    size_t proj_pk;               // tensor-core image (0 = not eligible -> FFMA kernel)
+    Conv1x1 proj;
+    Param proj_g, proj_be, proj_a;
+    Param dw_w[kMaxDepthApi], dw_b[kMaxDepthApi], dw_g[kMaxDepthApi], dw_be[kMaxDepthApi];
+    Param fn_g, fn_be, fn_a;
 };
-struct UBlockOff : NormBlockOff {
-    size_t res_w, res_b, res_pk;
-};
+struct UBlockOff : NormBlockOff { Conv1x1 res; };
 // sudormrf.py:134-162: proj_1x1 (conv, GroupNorm, PReLU(Ci)), spp_dw[d] (depthwise conv, GroupNorm), conv_1x1_exp (conv,
 // GroupNorm), final_norm (GroupNorm, PReLU(Ci)), module_act (GroupNorm, PReLU(Co)), in state_dict order
 struct OrigBlockOff : NormBlockOff {
-    size_t exp_w, exp_b, exp_g, exp_be;
-    size_t ma_g, ma_be, ma_a;
-    size_t exp_pk;
+    Conv1x1 exp;
+    Param exp_g, exp_be;
+    Param ma_g, ma_be, ma_a;
 };
-struct TacOff { size_t p[9]; size_t g, be; };
+struct TacOff { Param p[9]; Param g, be; };
 // causal_improved_sudormrf_v3.py:71-96: one scalar gain, proj (conv + PReLU), D x (21-tap depthwise + PReLU), res_conv
 struct CausalBlockOff {
-    size_t gain, proj_w, proj_b, proj_a;
-    size_t dw_w[kMaxDepthApi], dw_b[kMaxDepthApi], dw_a[kMaxDepthApi];
-    size_t res_w, res_b;
-    size_t res_wg, res_bg;        // derived: gain * res_conv.{weight,bias}
-    size_t proj_pk, res_pk;
+    Param gain;
+    Conv1x1 proj;
+    Param proj_a;
+    Param dw_w[kMaxDepthApi], dw_b[kMaxDepthApi], dw_a[kMaxDepthApi];
+    Conv1x1 res;
+    Conv1x1 res_g;                // derived: gain * res_conv.{weight,bias}, the one the forward runs
 };
-// the bf16 hi/lo, pre-swizzled tensor-core image at dst of the [M][K] 1x1 weight at src
-struct PackedImage { size_t src; int M, K; size_t dst; };
 
 struct Layout {
     bool ok = false;
@@ -140,21 +138,38 @@ struct Layout {
     bool causal = false;          // variant 2: CausalSuDORMRF
     bool orig = false;            // variant 3: the original SuDORMRF (sudormrf.py)
     std::vector<OrigBlockOff> ob;
-    size_t enc_b = 0, rs_w = 0, rs_b = 0, m_w = 0, m_b = 0, dec_b = 0;   // orig: encoder bias, reshape_before_masks, m, decoder bias
-    size_t toep_w = 0, toep_b = 0, rs_pk = 0;                            // orig, derived: [S*N][N] mask matrix + its row bias
+    Param enc_b, m_w, m_b, dec_b; // orig: encoder bias, m, decoder bias
+    Conv1x1 rs;                   // orig: reshape_before_masks (absent when Co == N)
     std::vector<CausalBlockOff> cb;
-    size_t mask_nl = 0;           // causal: mask_nl_class.weight (PReLU on the masks)
+    Param mask_nl;                // causal: mask_nl_class.weight (PReLU on the masks)
     size_t enc_wc = 0;            // causal: derived [N][A][K], the encoder taps the causal mask keeps
-    size_t enc_w = 0, ln_g = 0, ln_be = 0, bn_w = 0, bn_b = 0, mask_a = 0, mask_w = 0, mask_b = 0, dec_w = 0;
-    size_t dec_wt = 0;            // derived: decoder weight as [S*A*K, S*A*N]
-    size_t bn_pk = 0, mask_pk = 0, dec_pk = 0;   // tensor-core images of the 1x1 weights (0 = not eligible)
+    Param enc_w, ln_g, ln_be, mask_a, dec_w;
+    Conv1x1 bn;                   // bottleneck (orig: l1)
+    Conv1x1 mask;                 // mask 1x1 (orig: derived [S*N][N] Toeplitz matrix of the m convolution + row bias)
+    Conv1x1 dec;                  // derived: decoder weight as [S*A*K][S*A*N], no bias
     size_t enc_pk = 0, enc_src = 0;              // encoder window image (0 = not eligible) and the [N][A][K] weight behind it
     std::vector<UBlockOff> ub;
     std::vector<TacOff> tac;
-    std::vector<PackedImage> images;  // every 1x1 image, in reservation order
+    std::vector<Conv1x1> images;  // every 1x1 convolution with a tensor-core image, in reservation order
     std::vector<size_t> off, numel;   // per state_dict entry
     size_t total = 0;             // floats
 };
+
+// Epilogue of a 1x1 convolution beyond its bias (pointwise.cu): residual add, gate by `gate_channels` rows of `gate`,
+// and the epilogue mode.
+struct Epi { const float* residual = nullptr; const float* gate = nullptr; int gate_channels = 0, mode = 0; };
+
+// y = conv(x read through nin) (+ statistics unless `stats` is null): tensor cores when its image was packed, FFMA
+// otherwise.
+static int gemm(const float* pk, const Conv1x1& c, const float* x, const NormIn& nin, float* y, double* stats,
+                int samples, int L, cudaStream_t st, const Epi& epi = {}) {
+    const float* bias = c.b ? pk + c.b : nullptr;
+    if (c.pk && (L % 4) == 0)    // the tensor-core kernel loads activations as float4
+        return launch_pointwise_mma(x, nin, pk + c.pk, bias, epi.residual, epi.gate, epi.gate_channels, y, stats,
+                                    samples, c.M, c.K, L, epi.mode, st);
+    return launch_pointwise_ffma(x, nin, pk + c.w, bias, epi.residual, epi.gate, epi.gate_channels, y, stats,
+                                 samples, c.M, c.K, L, epi.mode, st);
+}
 
 static Layout make_layout(const sdr_config* c) {
     Layout l;
@@ -176,85 +191,71 @@ static Layout make_layout(const sdr_config* c) {
     l.cob = l.Co / l.G; l.cib = l.Ci / l.G;
     if (l.orig && (l.N % 2)) return l;   // (N+1) x 1 mask conv with padding N - N/2 returns N rows only for an even N (sudormrf.py:239-242,289)
 
-    size_t cur = 0;
-    auto derived = [&](size_t n) { const size_t o = cur; cur += (n + 3) & ~(size_t)3; return o; };   // made by sdr_pack_weights
-    auto add = [&](size_t n) { l.off.push_back(cur); l.numel.push_back(n); return derived(n); };      // state_dict entry
+    size_t cur = 0, grad = 0;
+    auto derived = [&](size_t n) { const size_t o = cur; cur += (n + 3) & ~(size_t)3; return Param{o}; };   // made by sdr_pack_weights
+    auto add = [&](size_t n) {                                                                               // state_dict entry
+        l.off.push_back(cur); l.numel.push_back(n);
+        const Param p{derived(n).off, grad};
+        grad += n;
+        return p;
+    };
+    auto conv = [&](int M, int K) { Conv1x1 c; c.M = M; c.K = K; c.w = add((size_t)M * K); c.b = add(M); return c; };
     auto begin_images = [&] { cur = (cur + 63) & ~(size_t)63; };   // 256 B alignment for the bulk-TMA images
-    auto image = [&](size_t src, int M, int K) -> size_t {
-        const size_t b = pointwise_mma_packed_bytes(M, K);
-        if (!b) return 0;
-        l.images.push_back(PackedImage{src, M, K, cur});
+    auto image = [&](Conv1x1& c) {
+        const size_t b = pointwise_mma_packed_bytes(c.M, c.K);
+        if (!b) return;
+        c.pk = cur;
         cur += b / sizeof(float);
-        return l.images.back().dst;
+        l.images.push_back(c);
     };
     auto proj_and_levels = [&](NormBlockOff& u, size_t slopes) {   // proj_1x1 and spp_dw: cib channels
-        u.proj_w = add((size_t)l.cib * l.cob); u.proj_b = add(l.cib);
+        u.proj = conv(l.cib, l.cob);
         u.proj_g = add(l.cib); u.proj_be = add(l.cib); u.proj_a = add(slopes);
         for (int d = 0; d < l.D; ++d) {
             u.dw_w[d] = add((size_t)l.cib * 5); u.dw_b[d] = add(l.cib);
             u.dw_g[d] = add(l.cib); u.dw_be[d] = add(l.cib);
         }
     };
+    const int SA = l.S * l.A;
     if (l.orig) {
         // state_dict order of the original SuDORMRF (sudormrf.py:211-252; block :134-162) without ln_mask_in (:253, unused)
         l.enc_w = add((size_t)l.N * l.K); l.enc_b = add(l.N);
         l.ln_g = add(l.N); l.ln_be = add(l.N);
-        l.bn_w = add((size_t)l.Co * l.N); l.bn_b = add(l.Co);                      // l1
+        l.bn = conv(l.Co, l.N);                                                    // l1
         for (int i = 0; i < l.U; ++i) {
             OrigBlockOff u;
             proj_and_levels(u, l.Ci);
-            u.exp_w = add((size_t)l.Co * l.Ci); u.exp_b = add(l.Co); u.exp_g = add(l.Co); u.exp_be = add(l.Co);
+            u.exp = conv(l.Co, l.Ci); u.exp_g = add(l.Co); u.exp_be = add(l.Co);
             u.fn_g = add(l.Ci); u.fn_be = add(l.Ci); u.fn_a = add(l.Ci);
             u.ma_g = add(l.Co); u.ma_be = add(l.Co); u.ma_a = add(l.Co);
             l.ob.push_back(u);
         }
-        if (l.Co != l.N) { l.rs_w = add((size_t)l.N * l.Co); l.rs_b = add(l.N); }   // :233-236
+        if (l.Co != l.N) l.rs = conv(l.N, l.Co);                                   // :233-236
         l.m_w = add((size_t)l.S * (l.N + 1)); l.m_b = add(l.S);
         l.dec_w = add((size_t)l.S * l.N * l.K); l.dec_b = add(l.S);
-        l.toep_w = derived((size_t)l.S * l.N * l.N);
-        l.toep_b = derived((size_t)l.S * l.N);
-        l.dec_wt = derived((size_t)l.S * l.K * l.S * l.N);
-        begin_images();
-        l.bn_pk = image(l.bn_w, l.Co, l.N);
-        for (OrigBlockOff& u : l.ob) {
-            u.proj_pk = image(u.proj_w, l.Ci, l.Co);
-            u.exp_pk = image(u.exp_w, l.Co, l.Ci);
-        }
-        if (l.rs_w) l.rs_pk = image(l.rs_w, l.N, l.Co);
-        l.mask_pk = image(l.toep_w, l.S * l.N, l.N);
+        l.mask.M = l.S * l.N; l.mask.K = l.N;
+        l.mask.w = derived((size_t)l.mask.M * l.mask.K);
+        l.mask.b = derived(l.mask.M);
     } else if (l.causal) {
         // state_dict order of CausalSuDORMRF (causal_improved_sudormrf_v3.py:146-189; block :71-96)
         l.enc_w = add((size_t)l.N * l.A * (2 * l.K - 1));
-        l.bn_w = add((size_t)l.Co * l.N); l.bn_b = add(l.Co);
+        l.bn = conv(l.Co, l.N);
         for (int i = 0; i < l.U; ++i) {
             CausalBlockOff u;
             u.gain = add(1);
-            u.proj_w = add((size_t)l.Ci * l.Co); u.proj_b = add(l.Ci); u.proj_a = add(1);
+            u.proj = conv(l.Ci, l.Co); u.proj_a = add(1);
             for (int d = 0; d < l.D; ++d) { u.dw_w[d] = add((size_t)l.Ci * 21); u.dw_b[d] = add(l.Ci); u.dw_a[d] = add(1); }
-            u.res_w = add((size_t)l.Co * l.Ci); u.res_b = add(l.Co);
+            u.res = conv(l.Co, l.Ci);
             l.cb.push_back(u);
         }
         l.mask_a = add(1);
-        l.mask_w = add((size_t)l.S * l.N * l.A * l.Co); l.mask_b = add((size_t)l.S * l.N * l.A);
-        l.dec_w = add((size_t)l.N * l.S * l.A * l.S * l.A * l.K);
+        l.mask = conv(SA * l.N, l.Co);
+        l.dec_w = add((size_t)l.N * SA * SA * l.K);
         l.mask_nl = add(1);
-        l.dec_wt = derived((size_t)l.S * l.A * l.K * l.S * l.A * l.N);
-        l.enc_wc = derived((size_t)l.N * l.A * l.K);
-        for (CausalBlockOff& u : l.cb) {
-            u.res_wg = derived((size_t)l.Co * l.Ci);
-            u.res_bg = derived(l.Co);
-        }
-        begin_images();
-        l.bn_pk = image(l.bn_w, l.Co, l.N);
-        for (CausalBlockOff& u : l.cb) {
-            u.proj_pk = image(u.proj_w, l.Ci, l.Co);
-            u.res_pk = image(u.res_wg, l.Co, l.Ci);
-        }
-        l.mask_pk = image(l.mask_w, l.S * l.A * l.N, l.Co);
     } else {
         l.enc_w = add((size_t)l.N * l.A * l.K);
         l.ln_g = add(l.N); l.ln_be = add(l.N);
-        l.bn_w = add((size_t)l.Co * l.N); l.bn_b = add(l.Co);
+        l.bn = conv(l.Co, l.N);
         for (int i = 0; i < l.U; ++i) {
             if (l.gc) {
                 TacOff t;
@@ -268,23 +269,33 @@ static Layout make_layout(const sdr_config* c) {
             UBlockOff u;
             proj_and_levels(u, 1);
             u.fn_g = add(l.cib); u.fn_be = add(l.cib); u.fn_a = add(1);
-            u.res_w = add((size_t)l.cob * l.cib); u.res_b = add(l.cob);
+            u.res = conv(l.cob, l.cib);
             l.ub.push_back(u);
         }
         l.mask_a = add(1);
-        l.mask_w = add((size_t)l.S * l.N * l.A * l.Co); l.mask_b = add((size_t)l.S * l.N * l.A);
-        l.dec_w = add((size_t)l.N * l.S * l.A * l.S * l.A * l.K);
-        l.dec_wt = derived((size_t)l.S * l.A * l.K * l.S * l.A * l.N);
-        begin_images();
-        l.bn_pk = image(l.bn_w, l.Co, l.N);
-        for (UBlockOff& u : l.ub) {
-            u.proj_pk = image(u.proj_w, l.cib, l.cob);
-            u.res_pk = image(u.res_w, l.cob, l.cib);
-        }
-        // the gated epilogue needs an output tile (128/256 channels) to stay inside one source's N basis rows
-        if (l.N % 256 == 0) l.mask_pk = image(l.mask_w, l.S * l.A * l.N, l.Co);
+        l.mask = conv(SA * l.N, l.Co);
+        l.dec_w = add((size_t)l.N * SA * SA * l.K);
     }
-    l.dec_pk = image(l.dec_wt, l.S * l.A * l.K, l.S * l.A * l.N);
+    l.dec.M = SA * l.K; l.dec.K = SA * l.N;
+    l.dec.w = derived((size_t)l.dec.M * l.dec.K);
+    if (l.causal) {
+        l.enc_wc = derived((size_t)l.N * l.A * l.K);
+        for (CausalBlockOff& u : l.cb) {
+            u.res_g.M = l.Co; u.res_g.K = l.Ci;
+            u.res_g.w = derived((size_t)l.Co * l.Ci);
+            u.res_g.b = derived(l.Co);
+        }
+    }
+    begin_images();
+    image(l.bn);
+    for (OrigBlockOff& u : l.ob) { image(u.proj); image(u.exp); }
+    for (CausalBlockOff& u : l.cb) { image(u.proj); image(u.res_g); }
+    for (UBlockOff& u : l.ub) { image(u.proj); image(u.res); }
+    if (l.rs.w) image(l.rs);
+    // improved / GroupComm: the gated epilogue needs an output tile (128/256 channels) to stay inside one source's N
+    // basis rows
+    if (l.orig || l.causal || l.N % 256 == 0) image(l.mask);
+    image(l.dec);
     // the original model's biased encoder + ReLU runs the same window kernel with bias / ReLU on the way out
     l.enc_src = l.causal ? l.enc_wc : l.enc_w;
     const size_t enc_bytes = encoder_mma_packed_bytes(l.N, l.A, l.K);
@@ -317,14 +328,21 @@ __global__ void transpose_decoder_kernel(const float* __restrict__ w, float* __r
     wt[i] = w[(size_t)c * SAK + r];
 }
 
+// Byte offsets of 256-byte aligned segments, handed out in order; `total` bytes hold them all.
+struct Segments {
+    size_t total = 0;
+    size_t take(size_t bytes) { const size_t o = total; total += (bytes + 255) & ~(size_t)255; return o; }
+    float* buf(char* ws, size_t o) const { return reinterpret_cast<float*>(ws + o); }
+};
+
 // ---------------------------------------------------------------------------
 // workspace plan: every choice that changes which kernels a forward runs is made here, once
 // ---------------------------------------------------------------------------
-struct Plan {
+struct Plan : Segments {
     long long Tp; int L; int samples;          // samples = B (improved) or B*G
     int block_slots;                           // statistics slots per block; slot 0 holds the encoder output's
     int slots; size_t stats_doubles;
-    size_t o_stats, o_e, o_x, o_xt, o_o, o_y, o_z[kMaxDepthApi], o_masked, o_frames, total;  // bytes
+    size_t o_stats, o_e, o_x, o_xt, o_o, o_y, o_z[kMaxDepthApi], o_masked, o_frames;  // bytes
     bool pyramid;                              // the depthwise pyramid runs as one pass (pyramid.cu)
     bool tac_folded;                           // GroupComm: tac_apply rides on proj_1x1's operand load (pointwise.cu)
     size_t o_rowstats, o_table;
@@ -332,7 +350,6 @@ struct Plan {
     double* stats(char* ws) const { return reinterpret_cast<double*>(ws + o_stats); }
     // statistics slot k of block i
     double* slot(char* ws, int i, int k) const { return stats(ws) + (1 + (size_t)i * block_slots + k) * samples * 2; }
-    float* buf(char* ws, size_t o) const { return reinterpret_cast<float*>(ws + o); }
 };
 
 static Plan make_plan(const Layout& l, int B, long long T) {
@@ -344,24 +361,21 @@ static Plan make_plan(const Layout& l, int B, long long T) {
     p.block_slots = l.causal ? 0 : l.D + 2 + (l.gc ? 1 : 0) + (l.orig ? 2 : 0);
     p.slots = 1 + l.U * p.block_slots;
     p.stats_doubles = (size_t)p.slots * p.samples * 2;
-    size_t cur = 0;
-    auto seg = [&](size_t bytes) { size_t o = cur; cur += (bytes + 255) & ~(size_t)255; return o; };
     const size_t BL = (size_t)B * p.L * sizeof(float);
-    p.o_stats = seg(p.stats_doubles * sizeof(double));
-    p.o_e = seg(BL * l.N);
-    p.o_x = seg(BL * l.Co);
-    p.o_xt = (l.gc || l.orig) ? seg(BL * l.Co) : 0;                       // orig: conv_1x1_exp output
-    p.o_o = l.gc ? seg(BL * l.Co) : ((l.orig && l.rs_w) ? seg(BL * l.N) : 0);   // orig: reshape_before_masks output
-    p.o_y = seg(BL * l.Ci);
-    for (int d = 0; d < kMaxDepthApi; ++d) p.o_z[d] = (d < l.D && !(l.causal && d > 0)) ? seg((BL * l.Ci) >> d) : 0;
+    p.o_stats = p.take(p.stats_doubles * sizeof(double));
+    p.o_e = p.take(BL * l.N);
+    p.o_x = p.take(BL * l.Co);
+    p.o_xt = (l.gc || l.orig) ? p.take(BL * l.Co) : 0;                       // orig: conv_1x1_exp output
+    p.o_o = l.gc ? p.take(BL * l.Co) : ((l.orig && l.rs.w) ? p.take(BL * l.N) : 0);   // orig: reshape_before_masks output
+    p.o_y = p.take(BL * l.Ci);
+    for (int d = 0; d < kMaxDepthApi; ++d) p.o_z[d] = (d < l.D && !(l.causal && d > 0)) ? p.take((BL * l.Ci) >> d) : 0;
     p.pyramid = !l.causal && pyramid_eligible(l.D, p.samples, l.cib, p.L);
     // proj_1x1 weights of every block have one shape, so they share one tensor-core eligibility
-    p.tac_folded = l.gc && l.U > 0 && !l.ub[0].proj_pk && preadd_eligible(l.cib, l.cob, p.L);
-    p.o_rowstats = p.pyramid ? seg(pyramid_rowstats_bytes(p.samples, l.cib, l.D)) : 0;
-    p.o_table = p.pyramid ? seg(pyramid_table_bytes(p.samples, l.cib, l.D)) : 0;
-    p.o_masked = seg(BL * l.S * l.A * l.N);
-    p.o_frames = seg(BL * l.S * l.A * l.K);
-    p.total = cur;
+    p.tac_folded = l.gc && l.U > 0 && !l.ub[0].proj.pk && preadd_eligible(l.cib, l.cob, p.L);
+    p.o_rowstats = p.pyramid ? p.take(pyramid_rowstats_bytes(p.samples, l.cib, l.D)) : 0;
+    p.o_table = p.pyramid ? p.take(pyramid_table_bytes(p.samples, l.cib, l.D)) : 0;
+    p.o_masked = p.take(BL * l.S * l.A * l.N);
+    p.o_frames = p.take(BL * l.S * l.A * l.K);
     return p;
 }
 
@@ -372,7 +386,7 @@ static int launch_count(const Layout& l, const Plan& p) {
     if (l.causal) return 2 + 3 * l.U + 3;      // encoder, bottleneck, U x (proj, depthwise pyramid, res), mask, decoder, overlap-add
     const int levels = p.pyramid ? 2 : l.D;
     if (l.orig)                                // encoder, l1, U x (proj, levels, merge, exp, residual-norm), [reshape], mask GEMM, softmax-gate, decoder, overlap-add
-        return 2 + l.U * (levels + 4) + (l.rs_w ? 1 : 0) + 4;
+        return 2 + l.U * (levels + 4) + (l.rs.w ? 1 : 0) + 4;
     return 2 + l.U * (levels + 3 + (l.gc ? (p.tac_folded ? 1 : 2) : 0)) + 3;
 }
 
@@ -393,11 +407,36 @@ static int encoder(const Layout& l, const float* pk, const float* mixture, float
 static int decoder_tail(const Layout& l, const Plan& p, const float* pk, const NormIn& nin, const float* bias,
                         const float* mixture, int apply_mc, const float2* rescale, float* out, int B, long long T,
                         char* ws, cudaStream_t st) {
-    const int SA = l.S * l.A;
     float* frames = p.buf(ws, p.o_frames);
-    SDR_TRY(pointwise(p.buf(ws, p.o_masked), nin, pk, l.dec_wt, l.dec_pk, nullptr, nullptr, nullptr, 0,
-                      frames, nullptr, B, SA * l.K, SA * l.N, p.L, 0, st));
-    return launch_overlap_add(frames, apply_mc ? mixture : nullptr, bias, rescale, out, B, SA, l.K, p.L, T, st);
+    SDR_TRY(gemm(pk, l.dec, p.buf(ws, p.o_masked), nin, frames, nullptr, B, p.L, st));
+    return launch_overlap_add(frames, apply_mc ? mixture : nullptr, bias, rescale, out, B, l.S * l.A, l.K, p.L, T, st);
+}
+
+// The front end of the models with statistics: the statistics cleared, the encoder into e (+ its statistics in slot 0)
+// and the bottleneck (original model: l1) into x with ln folded into its operand load.
+static int front_end(const Layout& l, const Plan& p, const float* pk, const float* mixture, int B, long long T,
+                     char* ws, cudaStream_t st) {
+    if (cudaMemsetAsync(p.stats(ws), 0, p.stats_doubles * sizeof(double), st) != cudaSuccess) return SDR_ERR_CUDA;
+    float* e = p.buf(ws, p.o_e);
+    SDR_TRY(encoder(l, pk, mixture, e, p.stats(ws), B, T, p.L, st));
+    const NormIn ln{p.stats(ws), pk + l.ln_g, pk + l.ln_be, nullptr, (double)l.N * p.L, 0};
+    return gemm(pk, l.bn, e, ln, p.buf(ws, p.o_x), nullptr, B, p.L, st);
+}
+
+// spp_dw level by level and the merge (levels.cu): y, read through n0, into the levels z[0..D-1], merged into m.
+// Statistics slot k is s0 + k * samples * 2: level d's in slot 1 + d, the merge's in slot D + 1.  nl receives how each
+// level is read (its GlobLN).
+static int depthwise_levels(const NormBlockOff& u, const float* pk, int D, const float* y, const NormIn& n0,
+                            float* const* z, float* m, double* s0, NormIn* nl, int samples, int C, int L,
+                            cudaStream_t st) {
+    auto slot = [&](int k) { return s0 + (size_t)k * samples * 2; };
+    for (int d = 0; d < D; ++d)
+        nl[d] = NormIn{slot(1 + d), pk + u.dw_g[d], pk + u.dw_be[d], nullptr, (double)C * (L >> d), 0};
+    SDR_TRY(launch_depthwise(y, n0, pk + u.dw_w[0], pk + u.dw_b[0], z[0], slot(1), samples, C, L, 1, st));
+    for (int d = 1; d < D; ++d)
+        SDR_TRY(launch_depthwise(z[d - 1], nl[d - 1], pk + u.dw_w[d], pk + u.dw_b[d], z[d], slot(1 + d),
+                                 samples, C, L >> (d - 1), 2, st));
+    return launch_merge(z, nl, D, m, slot(D + 1), samples, C, L, st);
 }
 
 // spp_dw and the merge of block i (improved_sudormrf.py / sudormrf.py UBlock): y holds the raw proj_1x1 output with its
@@ -409,9 +448,6 @@ static int depthwise_stage(const Layout& l, const Plan& p, const NormBlockOff& u
                            char* ws, cudaStream_t st) {
     const int L = p.L, D = l.D, ns = p.samples, C = l.cib;
     float* y = p.buf(ws, p.o_y);
-    float* z[kMaxDepthApi];
-    const float* zc[kMaxDepthApi];
-    for (int d = 0; d < D; ++d) zc[d] = z[d] = p.buf(ws, p.o_z[d]);
     const NormIn n0{p.slot(ws, i, 0), pk + u.proj_g, pk + u.proj_be, pk + u.proj_a, (double)C * L, prelu_pc};
     if (p.pyramid) {
         const float *pw[kMaxDepthApi], *pb[kMaxDepthApi], *pg[kMaxDepthApi], *pbe[kMaxDepthApi];
@@ -419,45 +455,48 @@ static int depthwise_stage(const Layout& l, const Plan& p, const NormBlockOff& u
         return launch_pyramid_fused(y, n0, pw, pb, pg, pbe, y, p.slot(ws, i, 1), p.slot(ws, i, D + 1),
                                     reinterpret_cast<double*>(ws + p.o_rowstats), p.buf(ws, p.o_table), D, ns, C, L, st);
     }
-    SDR_TRY(launch_depthwise(y, n0, pk + u.dw_w[0], pk + u.dw_b[0], z[0], p.slot(ws, i, 1), ns, C, L, 1, st));
-    for (int d = 1; d < D; ++d) {
-        const NormIn nd{p.slot(ws, i, d), pk + u.dw_g[d - 1], pk + u.dw_be[d - 1], nullptr, (double)C * (L >> (d - 1)), 0};
-        SDR_TRY(launch_depthwise(z[d - 1], nd, pk + u.dw_w[d], pk + u.dw_b[d], z[d], p.slot(ws, i, 1 + d),
-                                 ns, C, L >> (d - 1), 2, st));
-    }
-    NormIn nm[kMaxDepthApi];
-    for (int d = 0; d < D; ++d)
-        nm[d] = NormIn{p.slot(ws, i, 1 + d), pk + u.dw_g[d], pk + u.dw_be[d], nullptr, (double)C * (L >> d), 0};
-    return launch_merge(zc, nm, D, y, p.slot(ws, i, D + 1), ns, C, L, st);
+    float* z[kMaxDepthApi];
+    for (int d = 0; d < D; ++d) z[d] = p.buf(ws, p.o_z[d]);
+    NormIn nl[kMaxDepthApi];
+    return depthwise_levels(u, pk, D, y, n0, z, y, p.slot(ws, i, 0), nl, ns, C, L, st);
 }
 
-// CausalSuDORMRF.forward (causal_improved_sudormrf_v3.py:191-211): no normalisation anywhere, so nothing is deferred
-// except the PReLUs, which ride on the consumers' operand loads.
-static int forward_causal(const Layout& l, const Plan& p, const float* pk, const float* mixture, float* out,
-                          int B, long long T, int apply_mc, char* ws, cudaStream_t st, const float2* rescale) {
-    const int L = p.L, D = l.D;
-    float* e = p.buf(ws, p.o_e);
-    float* x = p.buf(ws, p.o_x);
-    float* y = p.buf(ws, p.o_y);
-    float* m = p.buf(ws, p.o_z[0]);
-    const NormIn none{nullptr, nullptr, nullptr, nullptr, 1.0, 0};
-    SDR_TRY(encoder(l, pk, mixture, e, nullptr, B, T, L, st));                                    // :194
-    SDR_TRY(pointwise(e, none, pk, l.bn_w, l.bn_pk, pk + l.bn_b, nullptr, nullptr, 0,
-                      x, nullptr, B, l.Co, l.N, L, 0, st));                                       // :199
-    for (const CausalBlockOff& u : l.cb) {
-        SDR_TRY(pointwise(x, none, pk, u.proj_w, u.proj_pk, pk + u.proj_b, nullptr, nullptr, 0,
-                          y, nullptr, B, l.Ci, l.Co, L, 0, st));                                  // :105 (PReLU deferred)
+// What CausalSuDORMRF.forward (causal_improved_sudormrf_v3.py:191-211) and a stream step share, from the encoder output
+// e to the decoder's frames: the bottleneck, U x (proj, the depthwise stage into m, res_conv with the gain folded in and
+// the skip in place), the mask 1x1 and the decoder GEMM.  No normalisation anywhere, so nothing is deferred except the
+// PReLUs, which ride on the consumers' operand loads.  The GEMMs see [samples][channels][L]; the depthwise stage sees B
+// rows of Lb frames, and continues each row from its level histories in the stream state `hist` (rows `row` floats
+// apart) when that is given.
+static int causal_body(const Layout& l, const float* pk, const float* e, float* x, float* y, float* m, float* masked,
+                       float* frames, int samples, int L, int B, int Lb, float* hist, long long row, cudaStream_t st) {
+    const int D = l.D;
+    SDR_TRY(gemm(pk, l.bn, e, kNoNorm, x, nullptr, samples, L, st));                              // :199
+    for (int i = 0; i < l.U; ++i) {
+        const CausalBlockOff& u = l.cb[i];
+        SDR_TRY(gemm(pk, u.proj, x, kNoNorm, y, nullptr, samples, L, st));                        // :105 (PReLU deferred)
         const float *w[kMaxDepthApi], *b[kMaxDepthApi], *a[kMaxDepthApi];
         for (int d = 0; d < D; ++d) { w[d] = pk + u.dw_w[d]; b[d] = pk + u.dw_b[d]; a[d] = pk + u.dw_a[d]; }
-        SDR_TRY(launch_causal_pyramid(y, pk + u.proj_a, w, b, a, m, D, B, l.Ci, L, st));          // :106-116
-        SDR_TRY(pointwise(m, none, pk, u.res_wg, u.res_pk, pk + u.res_bg, x, nullptr, 0,
-                          x, nullptr, B, l.Co, l.Ci, L, 0, st));                                  // :118
+        if (hist)                                                                                 // :106-116
+            SDR_TRY(launch_causal_stream(y, pk + u.proj_a, w, b, a, hist + (size_t)i * D * 10 * l.Ci, row, m,
+                                         D, B, l.Ci, Lb, st));
+        else
+            SDR_TRY(launch_causal_pyramid(y, pk + u.proj_a, w, b, a, m, D, B, l.Ci, Lb, st));
+        SDR_TRY(gemm(pk, u.res_g, m, kNoNorm, x, nullptr, samples, L, st, {x}));                  // :118
     }
     const NormIn pm{nullptr, nullptr, nullptr, pk + l.mask_a, 1.0, 0};                            // :202 PReLU -> 1x1
-    SDR_TRY(pointwise(x, pm, pk, l.mask_w, l.mask_pk, pk + l.mask_b, nullptr, nullptr, 0,
-                      p.buf(ws, p.o_masked), nullptr, B, l.S * l.A * l.N, l.Co, L, 0, st));
+    SDR_TRY(gemm(pk, l.mask, x, pm, masked, nullptr, samples, L, st));
     const NormIn pn{nullptr, nullptr, nullptr, pk + l.mask_nl, 1.0, 0};                           // :206 PReLU, :209 decoder
-    return decoder_tail(l, p, pk, pn, nullptr, mixture, apply_mc, rescale, out, B, T, ws, st);
+    return gemm(pk, l.dec, masked, pn, frames, nullptr, samples, L, st);
+}
+
+static int forward_causal(const Layout& l, const Plan& p, const float* pk, const float* mixture, float* out,
+                          int B, long long T, int apply_mc, char* ws, cudaStream_t st, const float2* rescale) {
+    float* e = p.buf(ws, p.o_e);
+    float* frames = p.buf(ws, p.o_frames);
+    SDR_TRY(encoder(l, pk, mixture, e, nullptr, B, T, p.L, st));                                  // :194
+    SDR_TRY(causal_body(l, pk, e, p.buf(ws, p.o_x), p.buf(ws, p.o_y), p.buf(ws, p.o_z[0]), p.buf(ws, p.o_masked),
+                        frames, B, p.L, B, p.L, nullptr, 0, st));
+    return launch_overlap_add(frames, apply_mc ? mixture : nullptr, nullptr, rescale, out, B, l.S * l.A, l.K, p.L, T, st);
 }
 
 // ---------------------------------------------------------------------------
@@ -481,26 +520,23 @@ static StreamState stream_state(const Layout& l) {
 }
 
 // Workspace of one step: every activation is [channels][B*F] with columns (slot, frame).
-struct StreamPlan {
+struct StreamPlan : Segments {
     int F, BF, Kr;                             // Kr: rows of the encoder operand (taps padded to a k-block for the image)
-    size_t o_framed, o_e, o_x, o_y, o_m, o_masked, o_frames, total;   // bytes
-    float* buf(char* ws, size_t o) const { return reinterpret_cast<float*>(ws + o); }
+    size_t o_framed, o_e, o_x, o_y, o_m, o_masked, o_frames;   // bytes
 };
 static StreamPlan make_stream_plan(const Layout& l, int B, long long C) {
     StreamPlan p;
     p.F = (int)(C / l.hop);
     p.BF = B * p.F;
     p.Kr = l.enc_pk ? (l.A * l.K + 63) / 64 * 64 : l.A * l.K;
-    size_t cur = 0;
-    auto seg = [&](size_t rows) { size_t o = cur; cur += (rows * p.BF * sizeof(float) + 255) & ~(size_t)255; return o; };
-    p.o_framed = seg(p.Kr);
-    p.o_e = seg(l.N);
-    p.o_x = seg(l.Co);
-    p.o_y = seg(l.Ci);
-    p.o_m = seg(l.Ci);
-    p.o_masked = seg((size_t)l.S * l.A * l.N);
-    p.o_frames = seg((size_t)l.S * l.A * l.K);
-    p.total = cur;
+    auto rows = [&](size_t n) { return p.take(n * p.BF * sizeof(float)); };
+    p.o_framed = rows(p.Kr);
+    p.o_e = rows(l.N);
+    p.o_x = rows(l.Co);
+    p.o_y = rows(l.Ci);
+    p.o_m = rows(l.Ci);
+    p.o_masked = rows((size_t)l.S * l.A * l.N);
+    p.o_frames = rows((size_t)l.S * l.A * l.K);
     return p;
 }
 
@@ -525,109 +561,69 @@ static int check_stream_args(const Layout& l, int B, long long C) {
 static int stream_step(const Layout& l, const StreamPlan& p, const float* pk, float* state, const float* chunk,
                        float* out, int B, long long C, int apply_mc, char* ws, cudaStream_t st) {
     const StreamState ss = stream_state(l);
-    const int BF = p.BF, D = l.D, SA = l.S * l.A;
     float* framed = p.buf(ws, p.o_framed);
     float* e = p.buf(ws, p.o_e);
-    float* x = p.buf(ws, p.o_x);
-    float* y = p.buf(ws, p.o_y);
-    float* m = p.buf(ws, p.o_m);
-    float* masked = p.buf(ws, p.o_masked);
     float* frames = p.buf(ws, p.o_frames);
-    const NormIn none{nullptr, nullptr, nullptr, nullptr, 1.0, 0};
     SDR_TRY(launch_stream_frame(chunk, state, (long long)ss.slot, framed, B, l.A, l.K, p.Kr, p.F, C, st));
     if (l.enc_pk)                                      // the window encoder's image is a plain [N][Kr] GEMM image
-        SDR_TRY(launch_pointwise_mma(framed, none, pk + l.enc_pk, nullptr, nullptr, nullptr, 0, e, nullptr,
-                                     1, l.N, p.Kr, BF, 0, st));
+        SDR_TRY(launch_pointwise_mma(framed, kNoNorm, pk + l.enc_pk, nullptr, nullptr, nullptr, 0, e, nullptr,
+                                     1, l.N, p.Kr, p.BF, 0, st));
     else
-        SDR_TRY(launch_pointwise_ffma(framed, none, pk + l.enc_src, nullptr, nullptr, nullptr, 0, e, nullptr,
-                                      1, l.N, l.A * l.K, BF, 0, st));
-    SDR_TRY(pointwise(e, none, pk, l.bn_w, l.bn_pk, pk + l.bn_b, nullptr, nullptr, 0, x, nullptr, 1, l.Co, l.N, BF, 0, st));
-    for (int i = 0; i < l.U; ++i) {
-        const CausalBlockOff& u = l.cb[i];
-        SDR_TRY(pointwise(x, none, pk, u.proj_w, u.proj_pk, pk + u.proj_b, nullptr, nullptr, 0,
-                          y, nullptr, 1, l.Ci, l.Co, BF, 0, st));
-        const float *w[kMaxDepthApi], *b[kMaxDepthApi], *a[kMaxDepthApi];
-        for (int d = 0; d < D; ++d) { w[d] = pk + u.dw_w[d]; b[d] = pk + u.dw_b[d]; a[d] = pk + u.dw_a[d]; }
-        SDR_TRY(launch_causal_stream(y, pk + u.proj_a, w, b, a, state + ss.hist + (size_t)i * D * 10 * l.Ci,
-                                     (long long)ss.slot, m, D, B, l.Ci, p.F, st));
-        SDR_TRY(pointwise(m, none, pk, u.res_wg, u.res_pk, pk + u.res_bg, x, nullptr, 0,
-                          x, nullptr, 1, l.Co, l.Ci, BF, 0, st));
-    }
-    const NormIn pm{nullptr, nullptr, nullptr, pk + l.mask_a, 1.0, 0};
-    SDR_TRY(pointwise(x, pm, pk, l.mask_w, l.mask_pk, pk + l.mask_b, nullptr, nullptr, 0,
-                      masked, nullptr, 1, SA * l.N, l.Co, BF, 0, st));
-    const NormIn pn{nullptr, nullptr, nullptr, pk + l.mask_nl, 1.0, 0};
-    SDR_TRY(pointwise(masked, pn, pk, l.dec_wt, l.dec_pk, nullptr, nullptr, nullptr, 0,
-                      frames, nullptr, 1, SA * l.K, SA * l.N, BF, 0, st));
-    return launch_stream_ola(frames, chunk, state, (long long)ss.slot, (long long)ss.carry, out, B, SA, l.A, l.K, p.F, C,
-                             apply_mc, st);
+        SDR_TRY(launch_pointwise_ffma(framed, kNoNorm, pk + l.enc_src, nullptr, nullptr, nullptr, 0, e, nullptr,
+                                      1, l.N, l.A * l.K, p.BF, 0, st));
+    SDR_TRY(causal_body(l, pk, e, p.buf(ws, p.o_x), p.buf(ws, p.o_y), p.buf(ws, p.o_m), p.buf(ws, p.o_masked), frames,
+                        1, p.BF, B, p.F, state + ss.hist, (long long)ss.slot, st));
+    return launch_stream_ola(frames, chunk, state, (long long)ss.slot, (long long)ss.carry, out, B, l.S * l.A, l.A, l.K,
+                             p.F, C, apply_mc, st);
 }
 
 // The original SuDORMRF.forward (sudormrf.py:266-292; UBlock.forward :164-186).
 static int forward_original(const Layout& l, const Plan& p, const float* pk, const float* mixture, float* out,
                             int B, long long T, int apply_mc, char* ws, cudaStream_t st, const float2* rescale) {
-    const int L = p.L, D = l.D, Co = l.Co, Ci = l.Ci, N = l.N, S = l.S;
+    const int L = p.L, D = l.D, Co = l.Co, Ci = l.Ci;
     float* e = p.buf(ws, p.o_e);
     float* x = p.buf(ws, p.o_x);
     float* ex = p.buf(ws, p.o_xt);
     float* y = p.buf(ws, p.o_y);
     float* masked = p.buf(ws, p.o_masked);
-    const NormIn none{nullptr, nullptr, nullptr, nullptr, 1.0, 0};
-    if (cudaMemsetAsync(p.stats(ws), 0, p.stats_doubles * sizeof(double), st) != cudaSuccess) return SDR_ERR_CUDA;
-
-    // front end (:268-276): biased encoder + ReLU (+stats), ln folded into l1's operand load
-    SDR_TRY(encoder(l, pk, mixture, e, p.stats(ws), B, T, L, st));
-    {
-        NormIn ln{p.stats(ws), pk + l.ln_g, pk + l.ln_be, nullptr, (double)N * L, 0};
-        SDR_TRY(pointwise(e, ln, pk, l.bn_w, l.bn_pk, pk + l.bn_b, nullptr, nullptr, 0, x, nullptr, B, Co, N, L, 0, st));
-    }
+    SDR_TRY(front_end(l, p, pk, mixture, B, T, ws, st));                // :268-276: the encoder has a bias and a ReLU
     // x holds u_i = GN(conv_1x1_exp(..)) + block input (raw); the block output PReLU_c(GN_ma(u_i)) is applied by its readers
-    NormIn xin = none;
+    NormIn xin = kNoNorm;
     for (int i = 0; i < l.U; ++i) {
         const OrigBlockOff& u = l.ob[i];
-        SDR_TRY(pointwise(x, xin, pk, u.proj_w, u.proj_pk, pk + u.proj_b, nullptr, nullptr, 0,
-                          y, p.slot(ws, i, 0), B, Ci, Co, L, 0, st));                                // :171
+        SDR_TRY(gemm(pk, u.proj, x, xin, y, p.slot(ws, i, 0), B, L, st));                           // :171
         SDR_TRY(depthwise_stage(l, p, u, i, 1, pk, ws, st));                                         // :172-182, m in y
-        {                                                                                            // :184 conv_1x1_exp.conv
-            NormIn nf{p.slot(ws, i, D + 1), pk + u.fn_g, pk + u.fn_be, pk + u.fn_a, (double)Ci * L, 1};
-            SDR_TRY(pointwise(y, nf, pk, u.exp_w, u.exp_pk, pk + u.exp_b, nullptr, nullptr, 0,
-                              ex, p.slot(ws, i, D + 2), B, Co, Ci, L, 0, st));
-        }
-        {                                                                                            // :184 .norm, :186 + x
-            NormIn ne{p.slot(ws, i, D + 2), pk + u.exp_g, pk + u.exp_be, nullptr, (double)Co * L, 0};
-            SDR_TRY(launch_residual_norm(ex, ne, x, xin, p.slot(ws, i, D + 3), B, Co, L, st));
-        }
+        const NormIn nf{p.slot(ws, i, D + 1), pk + u.fn_g, pk + u.fn_be, pk + u.fn_a, (double)Ci * L, 1};
+        SDR_TRY(gemm(pk, u.exp, y, nf, ex, p.slot(ws, i, D + 2), B, L, st));                         // :184 conv_1x1_exp.conv
+        const NormIn ne{p.slot(ws, i, D + 2), pk + u.exp_g, pk + u.exp_be, nullptr, (double)Co * L, 0};
+        SDR_TRY(launch_residual_norm(ex, ne, x, xin, p.slot(ws, i, D + 3), B, Co, L, st));            // :184 .norm, :186 + x
         xin = NormIn{p.slot(ws, i, D + 3), pk + u.ma_g, pk + u.ma_be, pk + u.ma_a, (double)Co * L, 1};   // :186 module_act
     }
     const float* mask_in = x;                              // input of the mask convolution and how to read it
     NormIn mnin = xin;
-    if (l.rs_w) {                                                                                     // :279-281
+    if (l.rs.w) {                                                                                     // :279-281
         float* r = p.buf(ws, p.o_o);
-        SDR_TRY(pointwise(x, xin, pk, l.rs_w, l.rs_pk, pk + l.rs_b, nullptr, nullptr, 0, r, nullptr, B, N, Co, L, 0, st));
-        mask_in = r; mnin = none;
+        SDR_TRY(gemm(pk, l.rs, x, xin, r, nullptr, B, L, st));
+        mask_in = r; mnin = kNoNorm;
     }
-    SDR_TRY(pointwise(mask_in, mnin, pk, l.toep_w, l.mask_pk, pk + l.toep_b, nullptr, nullptr, 0,
-                      masked, nullptr, B, S * N, N, L, 0, st));                                       // :284
-    SDR_TRY(launch_softmax_gate(masked, e, masked, B, S, N, L, st));                                  // :285-289
-    return decoder_tail(l, p, pk, none, pk + l.dec_b, mixture, apply_mc, rescale, out, B, T, ws, st);   // :291
+    SDR_TRY(gemm(pk, l.mask, mask_in, mnin, masked, nullptr, B, L, st));                              // :284
+    SDR_TRY(launch_softmax_gate(masked, e, masked, B, l.S, l.N, L, st));                              // :285-289
+    return decoder_tail(l, p, pk, kNoNorm, pk + l.dec_b, mixture, apply_mc, rescale, out, B, T, ws, st);   // :291
 }
 
 // What a training forward keeps for the backward (improved model): the forward's statistics slots, the raw encoder
 // output e and every block input x_0..x_U (x_U feeds the mask), each segment 256-byte aligned.
-struct Saved {
-    size_t o_stats, o_e, o_x, x_stride, total;
+struct Saved : Segments {
+    size_t o_stats, o_e, o_x, x_stride;
     const float* x(const char* s, int i) const { return reinterpret_cast<const float*>(s + o_x + (size_t)i * x_stride); }
 };
 static Saved saved_layout(const Layout& l, const Plan& p, int B) {
     Saved s;
-    size_t cur = 0;
-    auto seg = [&](size_t bytes) { size_t o = cur; cur += (bytes + 255) & ~(size_t)255; return o; };
     const size_t BL = (size_t)B * p.L * sizeof(float);
-    s.o_stats = seg(p.stats_doubles * sizeof(double));
-    s.o_e = seg(BL * l.N);
+    s.o_stats = s.take(p.stats_doubles * sizeof(double));
+    s.o_e = s.take(BL * l.N);
     s.x_stride = (BL * l.Co + 255) & ~(size_t)255;
-    s.o_x = cur;
-    s.total = cur + s.x_stride * (l.U + 1);
+    s.o_x = s.take(s.x_stride * (l.U + 1));
     return s;
 }
 
@@ -650,16 +646,7 @@ static int forward_impl(const Layout& l, const Plan& p, const float* pk, const f
     float* xt = l.gc ? p.buf(ws, p.o_xt) : nullptr;
     float* o = l.gc ? p.buf(ws, p.o_o) : nullptr;
     float* y = p.buf(ws, p.o_y);
-    const NormIn none{nullptr, nullptr, nullptr, nullptr, 1.0, 0};
-
-    if (cudaMemsetAsync(p.stats(ws), 0, p.stats_doubles * sizeof(double), st) != cudaSuccess) return SDR_ERR_CUDA;
-
-    // front end: encoder (+stats), ln folded into the bottleneck's operand load
-    SDR_TRY(encoder(l, pk, mixture, e, p.stats(ws), B, T, L, st));
-    {
-        NormIn ln{p.stats(ws), pk + l.ln_g, pk + l.ln_be, nullptr, (double)l.N * L, 0};
-        SDR_TRY(pointwise(e, ln, pk, l.bn_w, l.bn_pk, pk + l.bn_b, nullptr, nullptr, 0, x, nullptr, B, l.Co, l.N, L, 0, st));
-    }
+    SDR_TRY(front_end(l, p, pk, mixture, B, T, ws, st));
     const Saved sv = save ? saved_layout(l, p, B) : Saved{};
     const size_t xbytes = (size_t)B * L * l.Co * sizeof(float);
     if (save) SDR_TRY(copy_d2d(save + sv.o_x, x, xbytes, st));
@@ -679,21 +666,17 @@ static int forward_impl(const Layout& l, const Plan& p, const float* pk, const f
             // xt = x + GlobLN(o) is formed inside proj_1x1's operand load (and written once for the skip connection)
             // when the plan folds it; otherwise it is materialised first
             if (p.tac_folded)
-                SDR_TRY(launch_pointwise_small_preadd(x, o, tn, xt, pk + u.proj_w, pk + u.proj_b, y, p.slot(ws, i, 0),
-                                                      ns, cib, cob, L, st));
+                SDR_TRY(launch_pointwise_small_preadd(x, o, tn, xt, pk + u.proj.w, pk + u.proj.b, y, p.slot(ws, i, 0),
+                                                      ns, u.proj.M, u.proj.K, L, st));
             else
                 SDR_TRY(launch_tac_apply(x, o, tn, xt, ns, cob, L, st));
         }
         // proj_1x1: raw + stats
-        if (!p.tac_folded)
-            SDR_TRY(pointwise(bin, none, pk, u.proj_w, u.proj_pk, pk + u.proj_b, nullptr, nullptr, 0,
-                              y, p.slot(ws, i, 0), ns, cib, cob, L, 0, st));
+        if (!p.tac_folded) SDR_TRY(gemm(pk, u.proj, bin, kNoNorm, y, p.slot(ws, i, 0), ns, L, st));
         SDR_TRY(depthwise_stage(l, p, u, i, 0, pk, ws, st));              // m reuses y's storage
         // res_conv + skip
-        {
-            NormIn nf{p.slot(ws, i, D + 1), pk + u.fn_g, pk + u.fn_be, pk + u.fn_a, (double)cib * L, 0};
-            SDR_TRY(pointwise(y, nf, pk, u.res_w, u.res_pk, pk + u.res_b, bin, nullptr, 0, x, nullptr, ns, cob, cib, L, 0, st));
-        }
+        const NormIn nf{p.slot(ws, i, D + 1), pk + u.fn_g, pk + u.fn_be, pk + u.fn_a, (double)cib * L, 0};
+        SDR_TRY(gemm(pk, u.res, y, nf, x, nullptr, ns, L, st, {bin}));
         if (save) SDR_TRY(copy_d2d(save + sv.o_x + (size_t)(i + 1) * sv.x_stride, x, xbytes, st));
     }
     if (save) {
@@ -701,13 +684,10 @@ static int forward_impl(const Layout& l, const Plan& p, const float* pk, const f
         SDR_TRY(copy_d2d(save + sv.o_stats, p.stats(ws), p.stats_doubles * sizeof(double), st));
     }
     // mask: PReLU -> 1x1 -> ReLU -> * encoder output
-    {
-        NormIn pm{nullptr, nullptr, nullptr, pk + l.mask_a, 1.0, 0};
-        SDR_TRY(pointwise(x, pm, pk, l.mask_w, l.mask_pk, pk + l.mask_b, nullptr, e, l.N,
-                          p.buf(ws, p.o_masked), nullptr, B, l.S * l.A * l.N, l.Co, L, 1, st));
-    }
+    const NormIn pm{nullptr, nullptr, nullptr, pk + l.mask_a, 1.0, 0};
+    SDR_TRY(gemm(pk, l.mask, x, pm, p.buf(ws, p.o_masked), nullptr, B, L, st, {nullptr, e, l.N, 1}));
     // decoder: frames = Wd^T masked, then overlap-add / crop / mixture consistency
-    return decoder_tail(l, p, pk, none, nullptr, mixture, apply_mc, rescale, out, B, T, ws, st);
+    return decoder_tail(l, p, pk, kNoNorm, nullptr, mixture, apply_mc, rescale, out, B, T, ws, st);
 }
 
 // ---------------------------------------------------------------------------
@@ -715,47 +695,44 @@ static int forward_impl(const Layout& l, const Plan& p, const float* pk, const f
 // ---------------------------------------------------------------------------
 // Transposed 1x1 weights for the input-gradient GEMMs, one block's recomputed tensors and their statistics, the
 // gradient buffers, and the scratch of the fixed-order reductions.  Every activation buffer is [B][channels][L].
-struct BwdPlan {
+struct BwdPlan : Segments {
     size_t o_wt_mask, o_wt_bn, o_wt_p, o_wt_r, wt_block;    // wt_p / wt_r: per block, wt_block bytes apart
     size_t o_stats, o_dx, o_y, o_m, o_z[kMaxDepthApi], o_dn[kMaxDepthApi], o_dp;
     size_t o_mlog, o_dmask, o_frames, o_de, o_dq, o_win;
-    size_t o_npart, o_dwpart, o_wpart, total;
-    float* buf(char* ws, size_t o) const { return reinterpret_cast<float*>(ws + o); }
+    size_t o_npart, o_dwpart, o_wpart;
 };
 
 static BwdPlan make_bwd_plan(const Layout& l, const Plan& p, int B) {
     BwdPlan b;
-    size_t cur = 0;
-    auto seg = [&](size_t bytes) { size_t o = cur; cur += (bytes + 255) & ~(size_t)255; return o; };
     const size_t F = sizeof(float), BL = (size_t)B * p.L * F;
     const int L = p.L, Co = l.Co, Ci = l.Ci, N = l.N, SN = l.S * l.N, SK = l.S * l.K;
-    b.o_wt_mask = seg((size_t)SN * Co * F);
-    b.o_wt_bn = seg((size_t)N * Co * F);
+    b.o_wt_mask = b.take((size_t)l.mask.M * l.mask.K * F);
+    b.o_wt_bn = b.take((size_t)l.bn.M * l.bn.K * F);
     b.wt_block = ((size_t)Co * Ci * F + 255) & ~(size_t)255;
-    b.o_wt_p = cur; cur += b.wt_block * l.U;
-    b.o_wt_r = cur; cur += b.wt_block * l.U;
-    b.o_stats = seg((size_t)(l.D + 2) * B * 2 * sizeof(double));
-    b.o_dx = seg(BL * Co);
-    b.o_y = seg(BL * Ci);
-    b.o_m = seg(BL * Ci);
-    for (int d = 0; d < kMaxDepthApi; ++d) b.o_z[d] = d < l.D ? seg((BL * Ci) >> d) : 0;
-    for (int d = 0; d < kMaxDepthApi; ++d) b.o_dn[d] = d < l.D ? seg((BL * Ci) >> d) : 0;
-    b.o_dp = seg(BL * Ci);
-    b.o_mlog = seg(BL * SN);
-    b.o_dmask = seg(BL * SN);
-    b.o_frames = seg(BL * SK);
-    b.o_de = seg(BL * N);
-    b.o_dq = seg(BL * (Co > N ? Co : N));
-    b.o_win = seg(BL * l.K);
+    b.o_wt_p = b.take(b.wt_block * l.U);
+    b.o_wt_r = b.take(b.wt_block * l.U);
+    b.o_stats = b.take((size_t)(l.D + 2) * B * 2 * sizeof(double));
+    b.o_dx = b.take(BL * Co);
+    b.o_y = b.take(BL * Ci);
+    b.o_m = b.take(BL * Ci);
+    for (int d = 0; d < kMaxDepthApi; ++d) b.o_z[d] = d < l.D ? b.take((BL * Ci) >> d) : 0;
+    for (int d = 0; d < kMaxDepthApi; ++d) b.o_dn[d] = d < l.D ? b.take((BL * Ci) >> d) : 0;
+    b.o_dp = b.take(BL * Ci);
+    b.o_mlog = b.take(BL * SN);
+    b.o_dmask = b.take(BL * SN);
+    b.o_frames = b.take(BL * SK);
+    b.o_de = b.take(BL * N);
+    b.o_dq = b.take(BL * (Co > N ? Co : N));
+    b.o_win = b.take(BL * l.K);
     const int cmax = Ci > Co ? (Ci > N ? Ci : N) : (Co > N ? Co : N);
-    b.o_npart = seg(norm_bwd_scratch_bytes(B, cmax));
-    b.o_dwpart = seg(dw_bwd_scratch_bytes(B, Ci));
-    // every weight-gradient GEMM the backward runs: decoder, mask, res_conv, proj_1x1, bottleneck, encoder
-    const int shapes[6][2] = {{SN, SK}, {SN, Co}, {Co, Ci}, {Ci, Co}, {Co, N}, {N, l.K}};
+    b.o_npart = b.take(norm_bwd_scratch_bytes(B, cmax));
+    b.o_dwpart = b.take(dw_bwd_scratch_bytes(B, Ci));
+    // every weight-gradient GEMM the backward runs: decoder (on its [S*N][S*K] weight), mask, res_conv and proj_1x1
+    // (stated here: with U = 0 there is no block to read them from), bottleneck, encoder
+    const int shapes[6][2] = {{l.dec.K, l.dec.M}, {l.mask.M, l.mask.K}, {Co, Ci}, {Ci, Co}, {l.bn.M, l.bn.K}, {N, l.K}};
     size_t wp = 0;
     for (const auto& s : shapes) { const size_t w = wgrad_scratch_bytes(B, s[0], s[1], L); wp = w > wp ? w : wp; }
-    b.o_wpart = seg(wp);
-    b.total = cur;
+    b.o_wpart = b.take(wp);
     return b;
 }
 
@@ -769,18 +746,11 @@ static int bwd_launch_count(const Layout& l) {
 static int backward_impl(const Layout& l, const Plan& p, const BwdPlan& bp, const float* pk, const float* mixture,
                          const char* saved, const float* gout, float* grads, int B, long long T, char* ws,
                          cudaStream_t st) {
-    const int L = p.L, D = l.D, N = l.N, Co = l.Co, Ci = l.Ci, S = l.S, K = l.K, SN = S * N, SK = S * K;
+    const int L = p.L, D = l.D, N = l.N, Ci = l.Ci, S = l.S, K = l.K;
     const Saved sv = saved_layout(l, p, B);
     const float* e = reinterpret_cast<const float*>(saved + sv.o_e);
     const double* fstats = reinterpret_cast<const double*>(saved + sv.o_stats);   // slot 0: the encoder output's
-    std::vector<size_t> goff(l.off.size());
-    for (size_t i = 0, acc = 0; i < l.off.size(); ++i) { goff[i] = acc; acc += l.numel[i]; }
-    auto G = [&](size_t packed_off) -> float* {           // gradient of the parameter stored at packed_off
-        for (size_t i = 0; i < l.off.size(); ++i)
-            if (l.off[i] == packed_off) return grads + goff[i];
-        return nullptr;
-    };
-    const NormIn none{nullptr, nullptr, nullptr, nullptr, 1.0, 0};
+    auto G = [&](const Param& t) { return grads + t.grad; };
     double* nsc = reinterpret_cast<double*>(ws + bp.o_npart);
     double* dsc = reinterpret_cast<double*>(ws + bp.o_dwpart);
     float* wsc = bp.buf(ws, bp.o_wpart);
@@ -788,11 +758,21 @@ static int backward_impl(const Layout& l, const Plan& p, const BwdPlan& bp, cons
     float* wt_bn = bp.buf(ws, bp.o_wt_bn);
     auto wt_p = [&](int i) { return bp.buf(ws, bp.o_wt_p + (size_t)i * bp.wt_block); };
     auto wt_r = [&](int i) { return bp.buf(ws, bp.o_wt_r + (size_t)i * bp.wt_block); };
-    SDR_TRY(launch_transpose(pk + l.mask_w, wt_mask, SN, Co, st));                 // [Co][S*N]
-    SDR_TRY(launch_transpose(pk + l.bn_w, wt_bn, Co, N, st));                      // [N][Co]
+    // W^T ([K][M]) of a 1x1 convolution into wt, for its input-gradient GEMM
+    auto transpose = [&](const Conv1x1& c, float* wt) { return launch_transpose(pk + c.w, wt, c.M, c.K, st); };
+    // input gradient on FFMA: dx = W^T dy (+ acc unless null), W^T read from wt
+    auto dgrad = [&](const Conv1x1& c, const float* wt, const float* dy, const float* acc, float* dx) {
+        return launch_pointwise_ffma(dy, kNoNorm, wt, nullptr, acc, nullptr, 0, dx, nullptr, B, c.K, c.M, L, 0, st);
+    };
+    // weight and bias gradients of a 1x1 convolution whose input x was read through nin
+    auto wgrad = [&](const Conv1x1& c, const float* dy, const float* x, const NormIn& nin) {
+        return launch_wgrad(dy, x, nin, G(c.w), G(c.b), wsc, B, c.M, c.K, L, st);
+    };
+    SDR_TRY(transpose(l.mask, wt_mask));
+    SDR_TRY(transpose(l.bn, wt_bn));
     for (int i = 0; i < l.U; ++i) {
-        SDR_TRY(launch_transpose(pk + l.ub[i].proj_w, wt_p(i), Ci, Co, st));       // [Co][Ci]
-        SDR_TRY(launch_transpose(pk + l.ub[i].res_w, wt_r(i), Co, Ci, st));        // [Ci][Co]
+        SDR_TRY(transpose(l.ub[i].proj, wt_p(i)));
+        SDR_TRY(transpose(l.ub[i].res, wt_r(i)));
     }
     float* dx = bp.buf(ws, bp.o_dx);
     float* mlog = bp.buf(ws, bp.o_mlog);
@@ -804,18 +784,17 @@ static int backward_impl(const Layout& l, const Plan& p, const BwdPlan& bp, cons
     // mask and decoder: mlog = W_m PReLU_m(x_U) + b_m, masked = relu(mlog) * e, frames = Wd^T masked, crop + overlap-add
     const float* xU = sv.x(saved, l.U);
     const NormIn pm{nullptr, nullptr, nullptr, pk + l.mask_a, 1.0, 0};
-    SDR_TRY(launch_pointwise_ffma(xU, pm, pk + l.mask_w, pk + l.mask_b, nullptr, nullptr, 0, mlog, nullptr,
-                                  B, SN, Co, L, 0, st));      // fp32: the ReLU mask bits follow the logits closely
+    SDR_TRY(launch_pointwise_ffma(xU, pm, pk + l.mask.w, pk + l.mask.b, nullptr, nullptr, 0, mlog, nullptr,
+                                  B, l.mask.M, l.mask.K, L, 0, st));   // fp32: the ReLU mask bits follow the logits closely
     SDR_TRY(launch_mask_apply(mlog, e, dmask, B, S, N, L, st));                    // dmask holds masked for now
     SDR_TRY(launch_frame_gather(gout, frames, B, S, K, L, T, st));                 // dF
-    SDR_TRY(launch_wgrad(dmask, frames, none, G(l.dec_w), nullptr, wsc, B, SN, SK, L, st));   // [S*N][S][K] layout
-    SDR_TRY(launch_pointwise_ffma(frames, none, pk + l.dec_w, nullptr, nullptr, nullptr, 0, dmask, nullptr,
-                                  B, SN, SK, L, 0, st));                           // dmasked = Wd dF
+    // decoder.weight [S*N][S][K] is the transpose of l.dec
+    SDR_TRY(launch_wgrad(dmask, frames, kNoNorm, G(l.dec_w), nullptr, wsc, B, l.dec.K, l.dec.M, L, st));
+    SDR_TRY(dgrad(l.dec, pk + l.dec_w, frames, nullptr, dmask));                   // dmasked = Wd dF
     SDR_TRY(launch_mask_bwd(mlog, e, dmask, de, B, S, N, L, st));                  // dmlog (in dmask), de
-    SDR_TRY(launch_wgrad(dmask, xU, pm, G(l.mask_w), G(l.mask_b), wsc, B, SN, Co, L, st));
-    SDR_TRY(launch_pointwise_ffma(dmask, none, wt_mask, nullptr, nullptr, nullptr, 0, dq, nullptr,
-                                  B, Co, SN, L, 0, st));                           // W_m^T dmlog
-    SDR_TRY(launch_norm_bwd(xU, pm, dq, dx, 0, nullptr, nullptr, G(l.mask_a), nsc, B, Co, L, st));   // dx_U
+    SDR_TRY(wgrad(l.mask, dmask, xU, pm));
+    SDR_TRY(dgrad(l.mask, wt_mask, dmask, nullptr, dq));                           // W_m^T dmlog
+    SDR_TRY(launch_norm_bwd(xU, pm, dq, dx, 0, nullptr, nullptr, G(l.mask_a), nsc, B, l.Co, L, st));   // dx_U
 
     // U-ConvBlocks, last to first: recompute from x_i, then backward; dx carries the residual stream's gradient
     double* bst = reinterpret_cast<double*>(ws + bp.o_stats);
@@ -825,35 +804,26 @@ static int backward_impl(const Layout& l, const Plan& p, const BwdPlan& bp, cons
     float* dp = bp.buf(ws, bp.o_dp);
     float* z[kMaxDepthApi];
     float* dn[kMaxDepthApi];
-    const float* zc[kMaxDepthApi];
-    for (int d = 0; d < D; ++d) { zc[d] = z[d] = bp.buf(ws, bp.o_z[d]); dn[d] = bp.buf(ws, bp.o_dn[d]); }
+    for (int d = 0; d < D; ++d) { z[d] = bp.buf(ws, bp.o_z[d]); dn[d] = bp.buf(ws, bp.o_dn[d]); }
     for (int i = l.U - 1; i >= 0; --i) {
         const UBlockOff& u = l.ub[i];
         const float* xi = sv.x(saved, i);
         if (cudaMemsetAsync(bst, 0, (size_t)(D + 2) * B * 2 * sizeof(double), st) != cudaSuccess) return SDR_ERR_CUDA;
-        SDR_TRY(pointwise(xi, none, pk, u.proj_w, u.proj_pk, pk + u.proj_b, nullptr, nullptr, 0, y, slot(0),
-                          B, Ci, Co, L, 0, st));
+        SDR_TRY(gemm(pk, u.proj, xi, kNoNorm, y, slot(0), B, L, st));
         const NormIn n0{slot(0), pk + u.proj_g, pk + u.proj_be, pk + u.proj_a, (double)Ci * L, 0};
         NormIn nl[kMaxDepthApi];
-        for (int d = 0; d < D; ++d)
-            nl[d] = NormIn{slot(1 + d), pk + u.dw_g[d], pk + u.dw_be[d], nullptr, (double)Ci * (L >> d), 0};
-        SDR_TRY(launch_depthwise(y, n0, pk + u.dw_w[0], pk + u.dw_b[0], z[0], slot(1), B, Ci, L, 1, st));
-        for (int d = 1; d < D; ++d)
-            SDR_TRY(launch_depthwise(z[d - 1], nl[d - 1], pk + u.dw_w[d], pk + u.dw_b[d], z[d], slot(1 + d),
-                                     B, Ci, L >> (d - 1), 2, st));
-        SDR_TRY(launch_merge(zc, nl, D, m, slot(D + 1), B, Ci, L, st));
+        SDR_TRY(depthwise_levels(u, pk, D, y, n0, z, m, slot(0), nl, B, Ci, L, st));
         const NormIn nf{slot(D + 1), pk + u.fn_g, pk + u.fn_be, pk + u.fn_a, (double)Ci * L, 0};
 
         // out = W_r PReLU_f(GLN_f(m)) + b_r + x
-        SDR_TRY(launch_wgrad(dx, m, nf, G(u.res_w), G(u.res_b), wsc, B, Co, Ci, L, st));
-        SDR_TRY(launch_pointwise_ffma(dx, none, wt_r(i), nullptr, nullptr, nullptr, 0, dp, nullptr,
-                                      B, Ci, Co, L, 0, st));
+        SDR_TRY(wgrad(u.res, dx, m, nf));
+        SDR_TRY(dgrad(u.res, wt_r(i), dx, nullptr, dp));
         SDR_TRY(launch_norm_bwd(m, nf, dp, dp, 0, G(u.fn_g), G(u.fn_be), G(u.fn_a), nsc, B, Ci, L, st));   // dm
         // m[t] = sum_d n_d[t >> d]: the deepest level's gradient is dm pooled; the others get theirs from the
         // depthwise backward of the level below them
         const float* up = dp;
         if (D > 1) {
-            SDR_TRY(launch_dw_bwd(nullptr, nullptr, none, nullptr, dp, 1 << (D - 1), dn[D - 1], nullptr, nullptr,
+            SDR_TRY(launch_dw_bwd(nullptr, nullptr, kNoNorm, nullptr, dp, 1 << (D - 1), dn[D - 1], nullptr, nullptr,
                                   nullptr, B, Ci, L >> (D - 1), 2, st));
             up = dn[D - 1];
         }
@@ -870,19 +840,29 @@ static int backward_impl(const Layout& l, const Plan& p, const BwdPlan& bp, cons
             up = d > 0 ? dn[d - 1] : nullptr;
         }
         SDR_TRY(launch_norm_bwd(y, n0, dp, dp, 0, G(u.proj_g), G(u.proj_be), G(u.proj_a), nsc, B, Ci, L, st));   // dy
-        SDR_TRY(launch_wgrad(dp, xi, none, G(u.proj_w), G(u.proj_b), wsc, B, Ci, Co, L, st));
-        SDR_TRY(launch_pointwise_ffma(dp, none, wt_p(i), nullptr, dx, nullptr, 0, dx, nullptr,
-                                      B, Co, Ci, L, 0, st));                       // dx += W_p^T dy
+        SDR_TRY(wgrad(u.proj, dp, xi, kNoNorm));
+        SDR_TRY(dgrad(u.proj, wt_p(i), dp, dx, dx));                               // dx += W_p^T dy
     }
 
     // x_0 = W_bn GLN_ln(e) + b_bn; e = encoder(mixture)
     const NormIn ln{fstats, pk + l.ln_g, pk + l.ln_be, nullptr, (double)N * L, 0};
-    SDR_TRY(launch_wgrad(dx, e, ln, G(l.bn_w), G(l.bn_b), wsc, B, Co, N, L, st));
-    SDR_TRY(launch_pointwise_ffma(dx, none, wt_bn, nullptr, nullptr, nullptr, 0, dq, nullptr, B, N, Co, L, 0, st));
+    SDR_TRY(wgrad(l.bn, dx, e, ln));
+    SDR_TRY(dgrad(l.bn, wt_bn, dx, nullptr, dq));
     SDR_TRY(launch_norm_bwd(e, ln, dq, de, 1, G(l.ln_g), G(l.ln_be), nullptr, nsc, B, N, L, st));   // de += GLN bwd
     float* win = bp.buf(ws, bp.o_win);
     SDR_TRY(launch_frame_gather(mixture, win, B, 1, K, L, T, st));                 // the encoder's input windows
-    return launch_wgrad(de, win, none, G(l.enc_w), nullptr, wsc, B, N, K, L, st);
+    return launch_wgrad(de, win, kNoNorm, G(l.enc_w), nullptr, wsc, B, N, K, L, st);
+}
+
+// A buffer handed to an entry that enqueues a whole model: `align` bytes of alignment, and at least `need` bytes where
+// the caller says it has `bytes`.
+struct Buf { const void* ptr; size_t align = 1, bytes = 0, need = 0; };
+// Refuses a null buffer first, then one that is too small, then one that is misaligned.
+static int check_buffers(std::initializer_list<Buf> bufs) {
+    for (const Buf& b : bufs) if (!b.ptr) return SDR_ERR_BAD_ARGUMENT;
+    for (const Buf& b : bufs) if (b.bytes < b.need) return SDR_ERR_WORKSPACE;
+    for (const Buf& b : bufs) if (reinterpret_cast<uintptr_t>(b.ptr) % b.align) return SDR_ERR_BAD_ARGUMENT;
+    return SDR_OK;
 }
 
 }  // namespace sdr
@@ -949,22 +929,22 @@ int sdr_pack_weights(const sdr_config* cfg, const float* const* params, int n_pa
     }
     // the derived regions, then the images (some are packed from a derived region): all in stream order
     if (l.orig) {
-        SDR_TRY(launch_toeplitz_mask(pk + l.m_w, pk + l.m_b, pk + l.toep_w, pk + l.toep_b, l.S, l.N, st));
-        SDR_TRY(launch_grouped_decoder(pk + l.dec_w, pk + l.dec_wt, l.S, l.N, l.K, st));
+        SDR_TRY(launch_toeplitz_mask(pk + l.m_w, pk + l.m_b, pk + l.mask.w, pk + l.mask.b, l.S, l.N, st));
+        SDR_TRY(launch_grouped_decoder(pk + l.dec_w, pk + l.dec.w, l.S, l.N, l.K, st));
     } else {
-        const int C = l.S * l.A * l.N, SAK = l.S * l.A * l.K;
+        const int C = l.dec.K, SAK = l.dec.M;
         const long long n = (long long)C * SAK;
-        transpose_decoder_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(pk + l.dec_w, pk + l.dec_wt, C, SAK);
+        transpose_decoder_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(pk + l.dec_w, pk + l.dec.w, C, SAK);
         if (cudaGetLastError() != cudaSuccess) return SDR_ERR_CUDA;
     }
     if (l.causal) {
         SDR_TRY(launch_take_taps(pk + l.enc_w, pk + l.enc_wc, (long long)l.N * l.A, 2 * l.K - 1, l.K, st));
         for (const CausalBlockOff& u : l.cb) {
-            SDR_TRY(launch_scale_by_scalar(pk + u.res_w, pk + u.gain, pk + u.res_wg, (long long)l.Co * l.Ci, st));
-            SDR_TRY(launch_scale_by_scalar(pk + u.res_b, pk + u.gain, pk + u.res_bg, l.Co, st));
+            SDR_TRY(launch_scale_by_scalar(pk + u.res.w, pk + u.gain, pk + u.res_g.w, (long long)u.res.M * u.res.K, st));
+            SDR_TRY(launch_scale_by_scalar(pk + u.res.b, pk + u.gain, pk + u.res_g.b, u.res.M, st));
         }
     }
-    for (const PackedImage& im : l.images) SDR_TRY(pack_pointwise_mma(pk + im.src, im.M, im.K, pk + im.dst, st));
+    for (const Conv1x1& c : l.images) SDR_TRY(pack_pointwise_mma(pk + c.w, c.M, c.K, pk + c.pk, st));
     if (l.enc_pk) SDR_TRY(pack_encoder_mma(pk + l.enc_src, l.N, l.A, l.K, pk + l.enc_pk, st));
     return SDR_OK;
 }
@@ -997,11 +977,8 @@ int sdr_forward(const sdr_config* cfg, const void* packed, const float* mixture,
                 void* workspace, size_t workspace_bytes, sdr_stream stream) {
     const Layout l = make_layout(cfg);
     SDR_TRY(check_forward_args(l, B, T));
-    if (!packed || !mixture || !out || !workspace) return SDR_ERR_BAD_ARGUMENT;
     const Plan p = make_plan(l, B, T);
-    if (workspace_bytes < p.total) return SDR_ERR_WORKSPACE;
-    if (reinterpret_cast<uintptr_t>(workspace) % 256 || reinterpret_cast<uintptr_t>(packed) % 16)
-        return SDR_ERR_BAD_ARGUMENT;
+    SDR_TRY(check_buffers({{packed, 16}, {mixture}, {out}, {workspace, 256, workspace_bytes, p.total}}));
     return forward_impl(l, p, static_cast<const float*>(packed), mixture, out, B, T,
                         apply_mixture_consistency, static_cast<char*>(workspace),
                         static_cast<cudaStream_t>(stream));
@@ -1047,12 +1024,9 @@ int sdr_forward_train(const sdr_config* cfg, const void* packed, const float* mi
                       void* saved, size_t saved_bytes, void* ws, size_t ws_bytes, sdr_stream stream) {
     const Layout l = make_layout(cfg);
     SDR_TRY(check_train_args(l, B, T));
-    if (!packed || !mixture || !out || !saved || !ws) return SDR_ERR_BAD_ARGUMENT;
     const Plan p = make_plan(l, B, T);
-    if (ws_bytes < p.total || saved_bytes < saved_layout(l, p, B).total) return SDR_ERR_WORKSPACE;
-    if (reinterpret_cast<uintptr_t>(ws) % 256 || reinterpret_cast<uintptr_t>(saved) % 256 ||
-        reinterpret_cast<uintptr_t>(packed) % 16)
-        return SDR_ERR_BAD_ARGUMENT;
+    SDR_TRY(check_buffers({{packed, 16}, {mixture}, {out}, {saved, 256, saved_bytes, saved_layout(l, p, B).total},
+                           {ws, 256, ws_bytes, p.total}}));
     return forward_impl(l, p, static_cast<const float*>(packed), mixture, out, B, T, 0, static_cast<char*>(ws),
                         static_cast<cudaStream_t>(stream), nullptr, static_cast<char*>(saved));
 }
@@ -1062,13 +1036,10 @@ int sdr_backward(const sdr_config* cfg, const void* packed, const float* mixture
                  sdr_stream stream) {
     const Layout l = make_layout(cfg);
     SDR_TRY(check_train_args(l, B, T));
-    if (!packed || !mixture || !saved || !grad_out || !grad_params || !ws) return SDR_ERR_BAD_ARGUMENT;
     const Plan p = make_plan(l, B, T);
     const BwdPlan bp = make_bwd_plan(l, p, B);
-    if (ws_bytes < bp.total) return SDR_ERR_WORKSPACE;
-    if (reinterpret_cast<uintptr_t>(ws) % 256 || reinterpret_cast<uintptr_t>(saved) % 256 ||
-        reinterpret_cast<uintptr_t>(packed) % 16)
-        return SDR_ERR_BAD_ARGUMENT;
+    SDR_TRY(check_buffers({{packed, 16}, {mixture}, {saved, 256}, {grad_out}, {grad_params},
+                           {ws, 256, ws_bytes, bp.total}}));
     return backward_impl(l, p, bp, static_cast<const float*>(packed), mixture, static_cast<const char*>(saved),
                          grad_out, grad_params, B, T, static_cast<char*>(ws), static_cast<cudaStream_t>(stream));
 }
@@ -1138,8 +1109,7 @@ int sdr_encoder_wgrad(const float* denc, const float* wav, float* dw, void* scra
     float* part = reinterpret_cast<float*>(static_cast<char*>(scratch) +
                                            (((size_t)B * K * L * sizeof(float) + 255) & ~(size_t)255));
     SDR_TRY(launch_frame_gather(wav, win, B, 1, K, L, T, st));
-    const NormIn none{nullptr, nullptr, nullptr, nullptr, 1.0, 0};
-    return launch_wgrad(denc, win, none, dw, nullptr, part, B, N, K, L, st);
+    return launch_wgrad(denc, win, kNoNorm, dw, nullptr, part, B, N, K, L, st);
 }
 
 // ---- streaming of the causal model ----
@@ -1190,12 +1160,8 @@ int sdr_stream_step(const sdr_config* cfg, const void* packed, void* state, cons
     const Layout l = make_layout(cfg);
     SDR_TRY(check_stream_args(l, B, C));
     if (apply_mixture_consistency && l.A != 1) return SDR_ERR_UNSUPPORTED;
-    if (!packed || !state || !chunk || !out || !ws) return SDR_ERR_BAD_ARGUMENT;
     const StreamPlan p = make_stream_plan(l, B, C);
-    if (ws_bytes < p.total) return SDR_ERR_WORKSPACE;
-    if (reinterpret_cast<uintptr_t>(ws) % 256 || reinterpret_cast<uintptr_t>(packed) % 16 ||
-        reinterpret_cast<uintptr_t>(state) % 16)
-        return SDR_ERR_BAD_ARGUMENT;
+    SDR_TRY(check_buffers({{packed, 16}, {state, 16}, {chunk}, {out}, {ws, 256, ws_bytes, p.total}}));
     return stream_step(l, p, static_cast<const float*>(packed), static_cast<float*>(state), chunk, out, B, C,
                        apply_mixture_consistency, static_cast<char*>(ws), static_cast<cudaStream_t>(stream));
 }
@@ -1224,12 +1190,16 @@ int sdr_causal_stream_stage(const float* y, const float* slope_in, const float* 
 // `sums`) and the per-row (mean, std) (at `ms`) to the forward's workspace (`separate` bytes past its end).
 struct IoOffsets { size_t est, staging, sums, ms, separate; };
 static IoOffsets io_offsets(const Layout& l, int B, long long T) {
-    auto seg = [](size_t bytes) { return (bytes + 255) & ~(size_t)255; };
+    const size_t mixture = (size_t)B * l.A * T * sizeof(float);
     IoOffsets o;
-    o.est = o.sums = seg((size_t)B * l.A * T * sizeof(float));
-    o.staging = o.est + seg((size_t)B * l.S * l.A * T * sizeof(float));
-    o.ms = o.sums + seg((size_t)B * 2 * sizeof(double));
-    o.separate = o.ms + seg((size_t)B * sizeof(float2));
+    Segments staging, extra;
+    staging.take(mixture);
+    o.est = staging.take((size_t)B * l.S * l.A * T * sizeof(float));
+    o.staging = staging.total;
+    extra.take(mixture);
+    o.sums = extra.take((size_t)B * 2 * sizeof(double));
+    o.ms = extra.take((size_t)B * sizeof(float2));
+    o.separate = extra.total;
     return o;
 }
 
@@ -1444,12 +1414,9 @@ static int separate_impl(const sdr_config* cfg, const void* packed, const float*
     const Layout l = make_layout(cfg);
     SDR_TRY(check_forward_args(l, B, T));
     if (l.A != 1) return SDR_ERR_UNSUPPORTED;            // the README recipe is written for mono mixtures
-    if (!packed || !wav || !out || !workspace) return SDR_ERR_BAD_ARGUMENT;
     const Plan p = make_plan(l, B, T);
     const IoOffsets io = io_offsets(l, B, T);
-    if (workspace_bytes < p.total + io.separate) return SDR_ERR_WORKSPACE;
-    if (reinterpret_cast<uintptr_t>(workspace) % 256 || reinterpret_cast<uintptr_t>(packed) % 16)
-        return SDR_ERR_BAD_ARGUMENT;
+    SDR_TRY(check_buffers({{packed, 16}, {wav}, {out}, {workspace, 256, workspace_bytes, p.total + io.separate}}));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     char* ws = static_cast<char*>(workspace);
     char* extra = ws + p.total;
