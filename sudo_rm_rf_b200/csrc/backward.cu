@@ -41,14 +41,17 @@ __device__ __forceinline__ void block_sum_f64(double (&v)[NV], double* red /* >=
 // ---------------------------------------------------------------------------
 // One CTA per (64 x 64 output tile, sample, chunk of kWgChunk positions); its fp32 tile goes to part[p] with
 // p = sample * nchunk + chunk, laid out [M*K] followed by the bias partial [M] (written by the column-0 CTAs).
+// The grid is one-dimensional, column tile fastest, then row tile, then p, so that samples * nchunk may exceed the
+// 65535 a grid's y and z dimensions allow.
 __global__ void __launch_bounds__(kBwThreads)
 wgrad_partial_kernel(const float* __restrict__ dY, const float* __restrict__ X, NormIn nin, float* __restrict__ part,
-                     int M, int K, int L, int nchunk, int with_bias) {
+                     int M, int K, int L, int nchunk, int ktiles, int mtiles, int with_bias) {
     __shared__ float As[kWgStep][kWgTile + 4];
     __shared__ float Bs[kWgStep][kWgTile + 4];
     __shared__ ChanNorm cns[kWgTile];
-    const int kt = blockIdx.x * kWgTile, mt = blockIdx.y * kWgTile;
-    const int p = blockIdx.z, b = p / nchunk, chunk = p % nchunk;
+    const int kti = blockIdx.x % ktiles, mti = (blockIdx.x / ktiles) % mtiles;
+    const int kt = kti * kWgTile, mt = mti * kWgTile;
+    const int p = blockIdx.x / (ktiles * mtiles), b = p / nchunk, chunk = p % nchunk;
     const int t0 = chunk * kWgChunk, t1 = min(L, t0 + kWgChunk);
     const int tid = threadIdx.x, tx = tid & 15, ty = tid >> 4;
     if (tid < kWgTile) {
@@ -56,7 +59,7 @@ wgrad_partial_kernel(const float* __restrict__ dY, const float* __restrict__ X, 
         cns[tid] = chan_norm(nin, sn, kt + tid < K ? kt + tid : 0);
     }
     __syncthreads();
-    const bool bias_cta = with_bias && blockIdx.x == 0;
+    const bool bias_cta = with_bias && kti == 0;
     float acc[4][4] = {};
     float bacc = 0.f;
     for (int t = t0; t < t1; t += kWgStep) {
@@ -120,9 +123,11 @@ int launch_wgrad(const float* dY, const float* X, const NormIn& nin, float* dW, 
     if (!dY || !X || !dW || !scratch || samples <= 0 || M <= 0 || K <= 0 || L <= 0) return SDR_ERR_BAD_ARGUMENT;
     const int nchunk = wgrad_chunks(L);
     const long long P = (long long)samples * nchunk;
-    if (P > 65535 || (M + kWgTile - 1) / kWgTile > 65535) return SDR_ERR_UNSUPPORTED;
-    dim3 grid((unsigned)((K + kWgTile - 1) / kWgTile), (unsigned)((M + kWgTile - 1) / kWgTile), (unsigned)P);
-    wgrad_partial_kernel<<<grid, kBwThreads, 0, st>>>(dY, X, nin, scratch, M, K, L, nchunk, db ? 1 : 0);
+    const int ktiles = (K + kWgTile - 1) / kWgTile, mtiles = (M + kWgTile - 1) / kWgTile;
+    const long long ctas = P * ktiles * mtiles;
+    if (ctas > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
+    wgrad_partial_kernel<<<(unsigned)ctas, kBwThreads, 0, st>>>(dY, X, nin, scratch, M, K, L, nchunk, ktiles, mtiles,
+                                                                 db ? 1 : 0);
     if (cudaGetLastError() != cudaSuccess) return SDR_ERR_CUDA;
     const long long MK = (long long)M * K, n = MK + (db ? M : 0);
     // the partial stride is M*K + M whether or not the bias is reduced
