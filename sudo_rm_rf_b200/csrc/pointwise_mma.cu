@@ -19,7 +19,8 @@
 //   Epilogue: through four 16 KB shared-memory slots, one per quarter of the tile
 //       (one warpgroup's 64 positions x 64 channels).  The residual / gate quarter
 //       arrives there by TMA while the tile's main loop runs, the warpgroup combines
-//       it with its accumulators in place, and one thread stores the quarter to y by TMA.
+//       it with its accumulators in place and goes straight on; a store warp stores
+//       the quarter to y by TMA and refills the slot with the next tile's quarter.
 // Precision: x*w ~= xh*wh + xl*wh + xh*wl (3 bf16 MMAs, fp32 accumulate): the
 // dropped terms are O(2^-16) relative, i.e. fp32-grade for the 1e-3 parity
 // budget, where a single bf16 (5e-3) or tf32 (7e-4) pass is not (SURVEY §7).
@@ -52,9 +53,11 @@ constexpr int kBStageBytes = 2 * kBHalf;                     // 32 KB: hi + lo
 constexpr int kSlotBytes = 2 * kBoxBytes;                    // 16 KB: a quarter of the tile, 64 channels x 64 positions
 constexpr int kSlots = 4;                                    // slot 2 wg + h: warpgroup wg's channel half h
 // Warp roles: [0, 8) the two consumer warpgroups (operand transform, wgmma, epilogue), 8 weight TMA, 9 raw activation
-// TMA; in window mode warps 9 and 10 instead gather the waveform windows into the raw ring.
-constexpr int kConsWarps = 8, kTmaWarp = 8, kRawWarp = 9, kGatherWarps = 2;
-template <bool WINDOW> constexpr int kMmaThreads = 32 * (kRawWarp + (WINDOW ? kGatherWarps : 1));   // 320 / 352
+// TMA, 10 epilogue stores and residual / gate refills; in window mode warps 9 and 10 instead gather the waveform
+// windows into the raw ring (and the consumers copy their output out themselves).
+constexpr int kConsWarps = 8, kTmaWarp = 8, kRawWarp = 9, kStoreWarp = 10, kGatherWarps = 2;
+constexpr int kMmaThreads = 32 * (kStoreWarp + 1);   // 352: 11 warps, still at most 3 on one SM sub-partition
+static_assert(kRawWarp + kGatherWarps == kStoreWarp + 1, "window mode's gather warps take the raw and store warps' places");
 
 struct MmaArgs {
     const float* x;
@@ -216,7 +219,7 @@ __device__ __forceinline__ TileCoord decode_tile(const MmaArgs& a, int tile) {
 }
 
 // The consumers issue a k-block as kGroups wgmma groups of kGroupSteps k-steps each and double-buffer the A fragments
-// per group: 64 accumulators + 2 x 16 fragment registers.  (Whole k-blocks would take 2 x 32 and spill: 10 warps put
+// per group: 64 accumulators + 2 x 16 fragment registers.  (Whole k-blocks would take 2 x 32 and spill: 11 warps put
 // 3 on one SM sub-partition, which caps a thread at 168 registers.)
 constexpr int kGroupSteps = 2;
 constexpr int kGroups = kBlockK / 16 / kGroupSteps;
@@ -232,7 +235,7 @@ struct AFrag { uint32_t hi[kGroupSteps][4], lo[kGroupSteps][4]; };
 //           stored), 2 = ReLU * gate
 //   STATS:  accumulate (sum, sumsq) of the output
 template <bool WINDOW, int ACT, int MODE, bool STATS>
-__global__ void __launch_bounds__(kMmaThreads<WINDOW>, 1)
+__global__ void __launch_bounds__(kMmaThreads, 1)
 pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      // wmap: packed weights as [rows][128 B]
               const __grid_constant__ CUtensorMap xmap,                       // xmap: activations [samples][K][L], box [64][32]
               const __grid_constant__ CUtensorMap emap,                       // emap: residual (MODE 1) or gate (MODE 2)
@@ -255,12 +258,14 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
     //               table is written (window mode: one arrival per gather warp)
     //   rempty_bar: the 8 consumer warps hold the raw k-block's values in registers
     //   slot_bar:   per slot: the previous quarter's store has read it and, in MODE 1 / 2, it holds the quarter's
-    //               residual / gate (TMA tx bytes)
+    //               residual / gate (TMA tx bytes); the store warp's arrival
+    //   slot_full:  per slot: the owning warpgroup's 4 warps have written the combined quarter (not in window mode)
     uint64_t* full_bar = bars;                       // [kStages]
     uint64_t* empty_bar = full_bar + kStages;        // [kStages]
     uint64_t* rfull_bar = empty_bar + kStages;       // [kRawStages]
     uint64_t* rempty_bar = rfull_bar + kRawStages;   // [kRawStages]
     uint64_t* slot_bar = rempty_bar + kRawStages;    // [kSlots]
+    uint64_t* slot_full = slot_bar + kSlots;         // [kSlots]
 
     const int tid = threadIdx.x;
     const int warp = tid >> 5, lane = tid & 31;
@@ -274,12 +279,12 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
             mbar_init(&rfull_bar[s], WINDOW ? kGatherWarps : 2);
             mbar_init(&rempty_bar[s], kConsWarps);
         }
-        for (int s = 0; s < kSlots; ++s) mbar_init(&slot_bar[s], 1);
+        for (int s = 0; s < kSlots; ++s) { mbar_init(&slot_bar[s], 1); mbar_init(&slot_full[s], kConsWarps / 2); }
         fence_barrier_init();
     }
     __syncthreads();
 
-    if (warp >= kRawWarp) {
+    if (WINDOW ? warp >= kRawWarp : warp == kRawWarp) {
         int rs = 0;
         uint32_t rphase = 0;
         if constexpr (WINDOW) {
@@ -384,12 +389,56 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
             }
         }
         __syncwarp();
+    } else if (warp == kStoreWarp) {
+        // ===================== epilogue stores + residual / gate refills (not in window mode) =====================
+        // Slot 2 wg + h holds warpgroup wg's channel half h.  The warp walks the consumers' tiles and slots in their
+        // order; once a quarter's store has read its slot it loads the same quarter of the CTA's next tile (MODE 1 /
+        // 2) or only arrives (MODE 0), so all four residual / gate quarters land while that tile's main loop runs.
+        // The in-place skip stays correct: a tile's region is touched by its own CTA only, and this thread refills a
+        // slot only after its store has read it.
+        if constexpr (!WINDOW) {
+            if (lane == 0) {
+                auto fill_slot = [&](int tile, int s) {
+                    if constexpr (MODE == 0) {
+                        mbar_arrive(&slot_bar[s]);
+                    } else {
+                        const TileCoord t = decode_tile(a, tile);
+                        const int c0 = t.l0 + 64 * (s >> 1);
+                        const int c1 = (MODE == 1 ? t.n0 : t.n0 % a.gate_channels) + 64 * (s & 1);
+                        uint8_t* const dst = slots + (size_t)s * kSlotBytes;
+                        mbar_arrive_expect_tx(&slot_bar[s], kSlotBytes);
+                        tma_load_3d(dst, &emap, &slot_bar[s], c0, c1, t.sample);
+                        tma_load_3d(dst + kBoxBytes, &emap, &slot_bar[s], c0 + kBoxL, c1, t.sample);
+                    }
+                };
+                for (int s = 0; s < kSlots; ++s) fill_slot(tile0, s);
+                uint32_t phase = 0;
+#pragma unroll 1
+                for (int tile = tile0; tile < a.num_tiles; tile += tstep) {
+                    const TileCoord tc = decode_tile(a, tile);
+#pragma unroll 1
+                    for (int i = 0; i < kSlots; ++i) {
+                        const int h = i >> 1, wg = i & 1, s = 2 * wg + h;   // both warpgroups' half 0, then half 1
+                        uint8_t* const slot = slots + (size_t)s * kSlotBytes;
+                        const int c0 = tc.l0 + 64 * wg, c1 = tc.n0 + 64 * h;
+                        mbar_wait(&slot_full[s], phase);
+                        tma_store_3d(&ymap, slot, c0, c1, tc.sample);
+                        tma_store_3d(&ymap, slot + kBoxBytes, c0 + kBoxL, c1, tc.sample);
+                        bulk_commit();
+                        bulk_wait_read_all();
+                        if (tile + tstep < a.num_tiles) fill_slot(tile + tstep, s);
+                    }
+                    phase ^= 1;
+                }
+                bulk_wait_all();                   // the last stores have completed
+            }
+            __syncwarp();
+        }
     } else {
         // ===================== consumers: operand transform + wgmma main loop + epilogue =====================
         const int wg = warp >> 2;                  // position block [64 wg, 64 wg + 64) of the tile
         const int wr = warp & 3;                   // 16-row slice of the warpgroup's block
         const int q = lane & 3;
-        const bool issuer = (tid & 127) == 0;      // the warpgroup's thread that issues its slots' TMA traffic
         const bool relu_out = WINDOW && a.epilogue == 2;       // window mode only: ReLU on the way out
         const float slope = ACT == 1 ? __ldg(a.nin.prelu) : 1.f;
         const bool slope_le1 = slope <= 1.f;
@@ -403,25 +452,8 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
             boff[v] = c * 128 + (((pp >> 2) ^ c) << 4) + (pp & 3) * 4;
         }
         const uint32_t raw_box = (uint32_t)(2 * wg + (wr >> 1)) * kBoxBytes;
+        // Each warpgroup owns slots 2 wg (channels 0-63 of the tile) and 2 wg + 1 (64-127).
         uint8_t* const my_slots = slots + (size_t)(2 * wg) * kSlotBytes;
-        // Each warpgroup owns slots 2 wg (channels 0-63 of the tile) and 2 wg + 1 (64-127).  Once a quarter's store has
-        // read its slot, the issuer loads the same quarter of the CTA's next tile (MODE 1 / 2) or only arrives (MODE 0),
-        // so all four residual / gate quarters land while that tile's main loop runs.
-        auto fill_slot = [&](int tile, int h) {
-            uint64_t* bar = &slot_bar[2 * wg + h];
-            if constexpr (MODE == 0) {
-                mbar_arrive(bar);
-            } else {
-                const TileCoord t = decode_tile(a, tile);
-                const int c0 = t.l0 + 64 * wg;
-                const int c1 = (MODE == 1 ? t.n0 : t.n0 % a.gate_channels) + 64 * h;
-                uint8_t* const dst = my_slots + (size_t)h * kSlotBytes;
-                mbar_arrive_expect_tx(bar, kSlotBytes);
-                tma_load_3d(dst, &emap, bar, c0, c1, t.sample);
-                tma_load_3d(dst + kBoxBytes, &emap, bar, c0 + kBoxL, c1, t.sample);
-            }
-        };
-        if (issuer) { fill_slot(tile0, 0); fill_slot(tile0, 1); }
 
         int rs = 0, stage = 0, prev_stage = 0;
         uint32_t rphase = 0, phase = 0, slot_phase = 0;
@@ -528,7 +560,7 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
                 uint8_t* const box = slot + (wr >> 1) * kBoxBytes;
                 const int m0 = tc.n0 + 64 * h + 2 * q;
                 const int mrem = a.M - m0;             // channels left from this lane's first one
-                mbar_wait(&slot_bar[2 * wg + h], slot_phase);
+                if constexpr (!WINDOW) mbar_wait(&slot_bar[2 * wg + h], slot_phase);
 #pragma unroll
                 for (int j = 0; j < 8; ++j) {          // channels m0 + 8 j + {0, 1}
                     float bv[2];
@@ -549,7 +581,8 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
                 }
                 if constexpr (WINDOW) {
                     // the encoder's frame count is arbitrary, so its rows need not be 16 B aligned for TMA: the
-                    // warpgroup copies the quarter out, one 128 B row segment per warp instruction
+                    // warpgroup copies the quarter out, one 128 B row segment per warp instruction; the second
+                    // barrier frees the slot for the next tile
                     named_bar_sync(1 + wg, 128);
 #pragma unroll 4
                     for (int r = wr; r < 64; r += 4) {
@@ -564,17 +597,10 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
                     }
                     named_bar_sync(1 + wg, 128);
                 } else {
-                    fence_proxy_async_smem();          // generic-proxy stores -> visible to the TMA store
-                    named_bar_sync(1 + wg, 128);
-                    if (issuer) {
-                        const int c0 = tc.l0 + wg * 64, c1 = tc.n0 + 64 * h;
-                        tma_store_3d(&ymap, slot, c0, c1, tc.sample);
-                        tma_store_3d(&ymap, slot + kBoxBytes, c0 + kBoxL, c1, tc.sample);
-                        bulk_commit();
-                        bulk_wait_read_all();
-                    }
+                    fence_proxy_async_smem();          // generic-proxy stores -> visible to the store warp's TMA store
+                    __syncwarp();
+                    if (lane == 0) mbar_arrive(&slot_full[2 * wg + h]);
                 }
-                if (issuer && tile + tstep < a.num_tiles) fill_slot(tile + tstep, h);
             }
             slot_phase ^= 1;
             if (STATS) {
@@ -585,7 +611,6 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
                 }
             }
         }
-        if (!WINDOW && issuer) bulk_wait_all();        // the last stores have completed
     }
 }
 
@@ -616,7 +641,7 @@ int pack_pointwise_mma(const float* W, int M, int K, void* packed, cudaStream_t 
 
 constexpr size_t kMmaSmemBytes = 1024 + (size_t)kRawStages * kRawStageBytes + (size_t)kStages * kBStageBytes +
                                  (size_t)kSlots * kSlotBytes + kRawStages * kBlockK * (sizeof(float2) + sizeof(float)) +
-                                 (2 * kStages + 2 * kRawStages + kSlots) * sizeof(uint64_t);
+                                 (2 * kStages + 2 * kRawStages + 2 * kSlots) * sizeof(uint64_t);
 static_assert(kMmaSmemBytes <= 232448, "exceeds the 227 KB a CTA may own on sm_90");
 
 // cuTensorMapEncodeTiled is a pure host-side encoder; it is fetched through the runtime so that the library
@@ -676,7 +701,7 @@ struct MmaLaunchInfo { const void* fn; int dev; int sms; };
 static std::mutex g_launch_mutex;
 static std::vector<MmaLaunchInfo> g_launch_info;
 
-template <bool WINDOW, typename Kern>
+template <typename Kern>
 static int launch_persistent(Kern kern, const MmaArgs& a, const CUtensorMap& wmap, const CUtensorMap& xmap,
                              const CUtensorMap& emap, const CUtensorMap& ymap, cudaStream_t st) {
     int dev = 0;
@@ -696,7 +721,7 @@ static int launch_persistent(Kern kern, const MmaArgs& a, const CUtensorMap& wma
         }
     }
     const int grid = a.num_tiles < sms ? a.num_tiles : sms;
-    kern<<<grid, kMmaThreads<WINDOW>, kMmaSmemBytes, st>>>(a, wmap, xmap, emap, ymap);
+    kern<<<grid, kMmaThreads, kMmaSmemBytes, st>>>(a, wmap, xmap, emap, ymap);
     if (cudaGetLastError() != cudaSuccess) return SDR_ERR_CUDA;
     return SDR_OK;
 }
@@ -737,7 +762,7 @@ int launch_pointwise_mma(const float* x, const NormIn& nin, const void* wpk, con
         if (int rc = make_act_map(&emap, gate, samples, gate_channels, L)) return rc;
 #define SDR_MMA_CASE(A, MD, ST)                                                                                   \
     if (act == A && mode == MD && stats == ST)                                                                    \
-        return launch_persistent<false>(pw_mma_kernel<false, A, MD, ST>, a, wmap, xmap, emap, ymap, st);
+        return launch_persistent(pw_mma_kernel<false, A, MD, ST>, a, wmap, xmap, emap, ymap, st);
     SDR_MMA_CASE(0, 0, false) SDR_MMA_CASE(0, 0, true)
     SDR_MMA_CASE(1, 0, false) SDR_MMA_CASE(1, 0, true)
     SDR_MMA_CASE(0, 1, false) SDR_MMA_CASE(0, 1, true)
@@ -784,8 +809,8 @@ int launch_encoder_mma(const float* wav, const void* wpk, const float* bias, int
     CUtensorMap wmap, none;
     if (int rc = make_weight_map(&wmap, wpk, encoder_mma_packed_bytes(N, A, Kk))) return rc;
     memset(&none, 0, sizeof(none));               // window mode gathers the waveform and writes enc itself
-    if (stats) return launch_persistent<true>(pw_mma_kernel<true, 0, 0, true>, a, wmap, none, none, none, st);
-    return launch_persistent<true>(pw_mma_kernel<true, 0, 0, false>, a, wmap, none, none, none, st);
+    if (stats) return launch_persistent(pw_mma_kernel<true, 0, 0, true>, a, wmap, none, none, none, st);
+    return launch_persistent(pw_mma_kernel<true, 0, 0, false>, a, wmap, none, none, none, st);
 }
 
 }  // namespace sdr
