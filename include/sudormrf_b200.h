@@ -89,7 +89,11 @@ int    sdr_pack_weights(const sdr_config* cfg,
                         void* packed, size_t packed_bytes, sdr_stream stream);
 
 /* Caller-allocated scratch for a forward at batch B, length T (all
- * intermediates + the GlobLN statistics).                                    */
+ * intermediates + the GlobLN statistics).  The forward, the separate() recipe and
+ * sdr_mixture_consistency take any B whose buffers fit; no kernel's grid limits the
+ * batch.  Refused (this query then returns 0, the launch count and the forward
+ * SDR_ERR_UNSUPPORTED): B * group_size > 2^31 - 1, and more than 2^31 - 1
+ * channels x frames in one GlobLN sample; the kernels count both in int.     */
 size_t sdr_workspace_bytes(const sdr_config* cfg, int B, int64_t T);
 
 /* SuDORMRF.forward (improved_sudormrf.py:283-301) /

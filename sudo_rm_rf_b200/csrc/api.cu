@@ -2,6 +2,7 @@
 // parameter layout (reference state_dict order), weight packing, workspace
 // planning and the forward orchestration that enqueues every kernel on the
 // caller's stream.
+#include <algorithm>
 #include <vector>
 #include <cstring>
 #include <initializer_list>
@@ -351,6 +352,13 @@ struct Plan : Segments {
     // statistics slot k of block i
     double* slot(char* ws, int i, int k) const { return stats(ws) + (1 + (size_t)i * block_slots + k) * samples * 2; }
 };
+
+// Counts the kernels hold in int: samples = B * G in the plan and every launcher, and the items of one sample (channels
+// x frames) in the depthwise, merge, TAC-apply and residual-norm kernels.  A forward past either is refused.
+static bool counts_fit(const Layout& l, int B, long long T) {
+    const long long C = std::max(std::max(l.cib, l.cob), l.N);
+    return (long long)B * l.G <= 0x7fffffffLL && C * (padded_len(l, T) / l.hop) <= 0x7fffffffLL;
+}
 
 static Plan make_plan(const Layout& l, int B, long long T) {
     Plan p;
@@ -951,13 +959,14 @@ int sdr_pack_weights(const sdr_config* cfg, const float* const* params, int n_pa
 
 size_t sdr_workspace_bytes(const sdr_config* cfg, int B, int64_t T) {
     const Layout l = make_layout(cfg);
-    if (!l.ok || B <= 0 || T <= 0) return 0;
+    if (!l.ok || B <= 0 || T <= 0 || !counts_fit(l, B, T)) return 0;
     return make_plan(l, B, T).total;
 }
 
 static int check_forward_args(const Layout& l, int B, int64_t T) {
     if (!l.ok) return SDR_ERR_BAD_CONFIG;
     if (B <= 0 || T <= 0) return SDR_ERR_BAD_ARGUMENT;
+    if (!counts_fit(l, B, T)) return SDR_ERR_UNSUPPORTED;
     if (l.gc) {
         const int n = l.cob;
         if (!(n == 4 || n == 8 || n == 16 || n == 32) || l.G > 16) return SDR_ERR_UNSUPPORTED;
@@ -997,6 +1006,7 @@ int sdr_forward_launch_count_at(const sdr_config* cfg, int64_t T) {
 int sdr_forward_launch_count_for(const sdr_config* cfg, int B, int64_t T) {
     const Layout l = make_layout(cfg);
     if (!l.ok || B <= 0 || T <= 0) return SDR_ERR_BAD_CONFIG;
+    if (!counts_fit(l, B, T)) return SDR_ERR_UNSUPPORTED;
     return launch_count(l, make_plan(l, B, T));
 }
 
@@ -1404,7 +1414,7 @@ int sdr_utterance_stats(const float* wav, float* mean_std, int rows, int64_t T, 
 
 size_t sdr_separate_workspace_bytes(const sdr_config* cfg, int B, int64_t T) {
     const Layout l = make_layout(cfg);
-    if (!l.ok || B <= 0 || T <= 0) return 0;
+    if (!l.ok || B <= 0 || T <= 0 || !counts_fit(l, B, T)) return 0;
     return make_plan(l, B, T).total + io_offsets(l, B, T).separate;
 }
 

@@ -122,42 +122,44 @@ constexpr int kMaxSrc = 16;
 
 __global__ void __launch_bounds__(256)
 overlap_add_kernel(const float* __restrict__ frames, const float* __restrict__ mix, const float* __restrict__ bias,
-                   const float2* __restrict__ rescale, float* __restrict__ out, int SA, int K, int L, long long T) {
+                   const float2* __restrict__ rescale, float* __restrict__ out, int B, int SA, int K, int L, long long T) {
     const int hop = K / 2;
     const long long tau = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const int b = blockIdx.y;
     if (tau >= T) return;
     // j = tau + hop - hop*t in [0, K)  ->  t in [ceil((tau+hop-K+1)/hop), floor((tau+hop)/hop)]
     const long long thi = (tau + hop) / hop;
     long long tlo = tau + hop - (K - 1);
     tlo = tlo <= 0 ? 0 : (tlo + hop - 1) / hop;
-    float est[kMaxSrc];
-    float sum = 0.f;
-    // separate(): undo the per-utterance input normalisation, est * std + mean (README.md:109), before the
-    // mixture-consistency projection, which the README applies to the rescaled estimates (README.md:113-114)
-    const float2 rs = rescale ? rescale[b] : make_float2(0.f, 1.f);
-    for (int s = 0; s < SA; ++s) {
-        float acc = 0.f;
-        for (long long t = tlo; t <= thi && t < L; ++t) {
-            const int j = (int)(tau + hop - hop * t);
-            acc += __ldg(frames + ((size_t)b * SA * K + (size_t)s * K + j) * L + t);
+    // grid.y is capped at 65535; each CTA row strides over the batch
+    for (long long b = blockIdx.y; b < B; b += gridDim.y) {   // long long: b + gridDim.y may pass INT_MAX
+        float est[kMaxSrc];
+        float sum = 0.f;
+        // separate(): undo the per-utterance input normalisation, est * std + mean (README.md:109), before the
+        // mixture-consistency projection, which the README applies to the rescaled estimates (README.md:113-114)
+        const float2 rs = rescale ? rescale[b] : make_float2(0.f, 1.f);
+        for (int s = 0; s < SA; ++s) {
+            float acc = 0.f;
+            for (long long t = tlo; t <= thi && t < L; ++t) {
+                const int j = (int)(tau + hop - hop * t);
+                acc += __ldg(frames + ((size_t)b * SA * K + (size_t)s * K + j) * L + t);
+            }
+            if (bias) acc += __ldg(bias + s);            // decoder bias of the original model (one per source)
+            if (rescale) acc = __fadd_rn(__fmul_rn(acc, rs.y), rs.x);
+            est[s] = acc;
+            sum += acc;
         }
-        if (bias) acc += __ldg(bias + s);            // decoder bias of the original model (one per source)
-        if (rescale) acc = __fadd_rn(__fmul_rn(acc, rs.y), rs.x);
-        est[s] = acc;
-        sum += acc;
+        float corr = 0.f;
+        if (mix) corr = (__ldg(mix + (size_t)b * T + tau) - sum) * (1.0f / SA);   // mixture_consistency.py:29-35
+        for (int s = 0; s < SA; ++s) out[((size_t)b * SA + s) * T + tau] = est[s] + corr;
     }
-    float corr = 0.f;
-    if (mix) corr = (__ldg(mix + (size_t)b * T + tau) - sum) * (1.0f / SA);   // mixture_consistency.py:29-35
-    for (int s = 0; s < SA; ++s) out[((size_t)b * SA + s) * T + tau] = est[s] + corr;
 }
 
 int launch_overlap_add(const float* frames, const float* mix, const float* bias, const float2* rescale, float* out,
                        int B, int SA, int K, int L, long long T, cudaStream_t st) {
     if (B <= 0 || SA <= 0 || K < 3 || L <= 0 || T <= 0) return SDR_ERR_BAD_ARGUMENT;
-    if (SA > kMaxSrc || B > 65535) return SDR_ERR_UNSUPPORTED;
-    dim3 grid((unsigned)((T + 255) / 256), (unsigned)B);
-    overlap_add_kernel<<<grid, 256, 0, st>>>(frames, mix, bias, rescale, out, SA, K, L, T);
+    if (SA > kMaxSrc) return SDR_ERR_UNSUPPORTED;
+    dim3 grid((unsigned)((T + 255) / 256), (unsigned)(B < 65535 ? B : 65535));
+    overlap_add_kernel<<<grid, 256, 0, st>>>(frames, mix, bias, rescale, out, B, SA, K, L, T);
     return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
 }
 
@@ -165,70 +167,75 @@ int launch_overlap_add(const float* frames, const float* mix, const float* bias,
 // standalone mixture consistency (mixture_consistency.py:14-36)
 // ---------------------------------------------------------------------------
 __global__ void __launch_bounds__(256)
-mc_power_kernel(const float* __restrict__ est, double* __restrict__ power, long long T) {
-    // power[b*S+s] += sum_t est^2   (grid.y = B*S)
+mc_power_kernel(const float* __restrict__ est, double* __restrict__ power, int rows, long long T) {
+    // power[b*S+s] += sum_t est^2   (grid.y = min(B*S, 65535), striding over the rows)
     __shared__ float red[32];
-    const size_t row = blockIdx.y;
-    float q = 0.f;
-    for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < T;
-         t += (long long)gridDim.x * blockDim.x) {
-        const float v = __ldg(est + row * T + t);
-        q = fmaf(v, v, q);
-    }
-    q = warp_sum(q);
-    if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = q;
-    __syncthreads();
-    if (threadIdx.x < 32) {
-        double d = threadIdx.x < (blockDim.x >> 5) ? (double)red[threadIdx.x] : 0.0;
+    for (long long r = blockIdx.y; r < rows; r += gridDim.y) {    // long long: r + gridDim.y may pass INT_MAX
+        const size_t row = r;
+        float q = 0.f;
+        for (long long t = (long long)blockIdx.x * blockDim.x + threadIdx.x; t < T;
+             t += (long long)gridDim.x * blockDim.x) {
+            const float v = __ldg(est + row * T + t);
+            q = fmaf(v, v, q);
+        }
+        q = warp_sum(q);
+        if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5] = q;
+        __syncthreads();
+        if (threadIdx.x < 32) {
+            double d = threadIdx.x < (blockDim.x >> 5) ? (double)red[threadIdx.x] : 0.0;
 #pragma unroll
-        for (int o = 16; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
-        if (threadIdx.x == 0) atomicAdd(power + row, d);
+            for (int o = 16; o > 0; o >>= 1) d += __shfl_xor_sync(0xffffffffu, d, o);
+            if (threadIdx.x == 0) atomicAdd(power + row, d);
+        }
+        __syncthreads();                                   // red is reused by the next row
     }
 }
 
 __global__ void __launch_bounds__(256)
 mc_apply_kernel(const float* __restrict__ est, const float* __restrict__ mix,
-                const double* __restrict__ power, float* __restrict__ out, int S, long long T) {
+                const double* __restrict__ power, float* __restrict__ out, int B, int S, long long T) {
     const long long tau = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    const int b = blockIdx.y;
     if (tau >= T) return;
-    float sum = 0.f;
-    for (int s = 0; s < S; ++s) sum += __ldg(est + ((size_t)b * S + s) * T + tau);
-    const float resid = __ldg(mix + (size_t)b * T + tau) - sum;
-    float wsum = 0.f;
-    if (power) {
-        for (int s = 0; s < S; ++s) wsum += (float)(power[(size_t)b * S + s] / (double)T);
-    }
-    for (int s = 0; s < S; ++s) {
-        float w;
+    for (long long b = blockIdx.y; b < B; b += gridDim.y) {   // long long: b + gridDim.y may pass INT_MAX
+        float sum = 0.f;
+        for (int s = 0; s < S; ++s) sum += __ldg(est + ((size_t)b * S + s) * T + tau);
+        const float resid = __ldg(mix + (size_t)b * T + tau) - sum;
+        float wsum = 0.f;
         if (power) {
-            const float mw = (float)(power[(size_t)b * S + s] / (double)T);  // mean(est^2, -1)
-            w = mw / (wsum + 1e-9f);                                          // mixture_consistency.py:27-28
-        } else {
-            w = 1.0f / S;
+            for (int s = 0; s < S; ++s) wsum += (float)(power[(size_t)b * S + s] / (double)T);
         }
-        const size_t i = ((size_t)b * S + s) * T + tau;
-        out[i] = __ldg(est + i) + w * resid;
+        for (int s = 0; s < S; ++s) {
+            float w;
+            if (power) {
+                const float mw = (float)(power[(size_t)b * S + s] / (double)T);  // mean(est^2, -1)
+                w = mw / (wsum + 1e-9f);                                          // mixture_consistency.py:27-28
+            } else {
+                w = 1.0f / S;
+            }
+            const size_t i = ((size_t)b * S + s) * T + tau;
+            out[i] = __ldg(est + i) + w * resid;
+        }
     }
 }
 
 int launch_mixture_consistency(const float* est, const float* mix, float* out, int B, int S,
                                long long T, int weights_type, void* scratch, cudaStream_t st) {
     if (B <= 0 || S <= 0 || T <= 0 || !est || !mix || !out) return SDR_ERR_BAD_ARGUMENT;
-    if (B > 65535 || (long long)B * S > 65535) return SDR_ERR_UNSUPPORTED;
+    if ((long long)B * S > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;   // rows are indexed in int
     double* power = nullptr;
     if (weights_type == 1) {
         if (!scratch) return SDR_ERR_BAD_ARGUMENT;
         power = static_cast<double*>(scratch);
-        if (cudaMemsetAsync(power, 0, sizeof(double) * B * S, st) != cudaSuccess) return SDR_ERR_CUDA;
+        const int rows = B * S;
+        if (cudaMemsetAsync(power, 0, sizeof(double) * rows, st) != cudaSuccess) return SDR_ERR_CUDA;
         int gx = (int)((T + 256 * 8 - 1) / (256 * 8));
         if (gx < 1) gx = 1;
-        mc_power_kernel<<<dim3((unsigned)gx, (unsigned)(B * S)), 256, 0, st>>>(est, power, T);
+        mc_power_kernel<<<dim3((unsigned)gx, (unsigned)(rows < 65535 ? rows : 65535)), 256, 0, st>>>(est, power, rows, T);
     } else if (weights_type != 0) {
         return SDR_ERR_BAD_ARGUMENT;
     }
-    dim3 grid((unsigned)((T + 255) / 256), (unsigned)B);
-    mc_apply_kernel<<<grid, 256, 0, st>>>(est, mix, power, out, S, T);
+    dim3 grid((unsigned)((T + 255) / 256), (unsigned)(B < 65535 ? B : 65535));
+    mc_apply_kernel<<<grid, 256, 0, st>>>(est, mix, power, out, B, S, T);
     return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
 }
 

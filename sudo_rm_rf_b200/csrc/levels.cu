@@ -449,6 +449,7 @@ int launch_depthwise(const float* x, const NormIn& nin, const float* w5, const f
                      float* y, double* stats_out, int samples, int C, int Lin, int stride,
                      cudaStream_t st) {
     if (samples <= 0 || C <= 0 || Lin <= 0 || (stride != 1 && stride != 2)) return SDR_ERR_BAD_ARGUMENT;
+    if ((long long)C * Lin > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;   // the kernels count a sample's items in int
     const int Lout = (Lin + 4 - 5) / stride + 1;
     const bool vec = (Lout % 4 == 0) && (stride == 1 || Lin == 2 * Lout) &&
                      ((reinterpret_cast<uintptr_t>(x) | reinterpret_cast<uintptr_t>(y)) % 16 == 0);
@@ -486,6 +487,7 @@ int launch_merge(const float* const* z, const NormIn* nins, int depth, float* m,
                  int samples, int C, int L, cudaStream_t st) {
     if (depth < 1 || depth > kMaxDepth) return SDR_ERR_UNSUPPORTED;
     if (samples <= 0 || C <= 0 || L <= 0 || (L % (1 << (depth - 1))) != 0) return SDR_ERR_BAD_ARGUMENT;
+    if ((long long)C * L > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;     // the kernels count a sample's items in int
     MergeArgs a;
     a.depth = depth;
     bool aligned = reinterpret_cast<uintptr_t>(m) % 16 == 0;

@@ -101,14 +101,11 @@ __device__ __forceinline__ void sg_store(float* p, const float (&v)[4]) {
 // up to kSgMaxSrc (the first version, every S through 16 predicated copies: 92 registers, 557 instructions per warp,
 // 433 us for the 1.05 GB of the default model's masks, profiles/r02b_kernels.md).
 template <bool VEC, int SS>
-__global__ void __launch_bounds__(256)
-softmax_gate_kernel(const float* logits, const float* __restrict__ enc, float* out, int S_rt, long long NL) {
+__device__ __forceinline__ void softmax_gate_item(const float* logits, const float* __restrict__ enc, float* out,
+                                                  int S_rt, long long NL, int b, long long i) {
     constexpr int W = VEC ? 4 : 1;
     constexpr int SMAX = SS ? SS : kSgMaxSrc;
     const int S = SS ? SS : S_rt;
-    const int b = blockIdx.y;
-    const long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * W;
-    if (i >= NL) return;
     const float* lp = logits + (size_t)b * S * NL + i;
     float* op = out + (size_t)b * S * NL + i;
     float g[4];
@@ -152,28 +149,39 @@ softmax_gate_kernel(const float* logits, const float* __restrict__ enc, float* o
     }
 }
 
+// grid.y is capped at 65535; each CTA row strides over the batch
+template <bool VEC, int SS>
+__global__ void __launch_bounds__(256)
+softmax_gate_kernel(const float* logits, const float* __restrict__ enc, float* out, int B, int S_rt, long long NL) {
+    const long long i = ((long long)blockIdx.x * blockDim.x + threadIdx.x) * (VEC ? 4 : 1);
+    if (i >= NL) return;
+    for (long long b = blockIdx.y; b < B; b += gridDim.y)      // long long: b + gridDim.y may pass INT_MAX
+        softmax_gate_item<VEC, SS>(logits, enc, out, S_rt, NL, (int)b, i);
+}
+
 template <bool VEC>
-static void launch_sg(dim3 grid, const float* logits, const float* enc, float* out, int S, long long NL, cudaStream_t st) {
+static void launch_sg(dim3 grid, const float* logits, const float* enc, float* out, int B, int S, long long NL,
+                      cudaStream_t st) {
     switch (S) {
-        case 2: softmax_gate_kernel<VEC, 2><<<grid, 256, 0, st>>>(logits, enc, out, S, NL); break;
-        case 3: softmax_gate_kernel<VEC, 3><<<grid, 256, 0, st>>>(logits, enc, out, S, NL); break;
-        case 4: softmax_gate_kernel<VEC, 4><<<grid, 256, 0, st>>>(logits, enc, out, S, NL); break;
-        default: softmax_gate_kernel<VEC, 0><<<grid, 256, 0, st>>>(logits, enc, out, S, NL); break;
+        case 2: softmax_gate_kernel<VEC, 2><<<grid, 256, 0, st>>>(logits, enc, out, B, S, NL); break;
+        case 3: softmax_gate_kernel<VEC, 3><<<grid, 256, 0, st>>>(logits, enc, out, B, S, NL); break;
+        case 4: softmax_gate_kernel<VEC, 4><<<grid, 256, 0, st>>>(logits, enc, out, B, S, NL); break;
+        default: softmax_gate_kernel<VEC, 0><<<grid, 256, 0, st>>>(logits, enc, out, B, S, NL); break;
     }
 }
 
 int launch_softmax_gate(const float* logits, const float* enc, float* out, int B, int S, int N, int L, cudaStream_t st) {
     if (!logits || !enc || !out || B <= 0 || S <= 0 || N <= 0 || L <= 0) return SDR_ERR_BAD_ARGUMENT;
-    if (S > kSgMaxSrc || B > 65535) return SDR_ERR_UNSUPPORTED;
+    if (S > kSgMaxSrc) return SDR_ERR_UNSUPPORTED;
     const long long NL = (long long)N * L;
     const bool vec = (NL % 4 == 0) &&
                      ((reinterpret_cast<uintptr_t>(logits) | reinterpret_cast<uintptr_t>(enc) | reinterpret_cast<uintptr_t>(out)) % 16 == 0);
     const long long threads = vec ? NL / 4 : NL;
     const long long gx = (threads + 255) / 256;
     if (gx > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-    dim3 grid((unsigned)gx, (unsigned)B);
-    if (vec) launch_sg<true>(grid, logits, enc, out, S, NL, st);
-    else     launch_sg<false>(grid, logits, enc, out, S, NL, st);
+    dim3 grid((unsigned)gx, (unsigned)(B < 65535 ? B : 65535));
+    if (vec) launch_sg<true>(grid, logits, enc, out, B, S, NL, st);
+    else     launch_sg<false>(grid, logits, enc, out, B, S, NL, st);
     return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
 }
 

@@ -66,15 +66,17 @@ __global__ void row_mean_std_kernel(const double* __restrict__ sums, float2* __r
 
 // y = (x - mean) / (std + 1e-9)      (README.md:103)
 __global__ void __launch_bounds__(256)
-normalize_rows_kernel(const float* __restrict__ x, const float2* __restrict__ ms, float* __restrict__ y, long long T,
-                      const long long* __restrict__ lengths) {
-    const int row = blockIdx.y;
-    const float2 m = ms[row];
-    const float den = m.y + 1e-9f;
-    const size_t base = (size_t)row * T;
-    const long long Tr = row_length(lengths, row, T);      // beyond the utterance: the zero padding stays zero
-    for (long long t = (long long)blockIdx.x * 256 + threadIdx.x; t < T; t += (long long)gridDim.x * 256)
-        y[base + t] = t < Tr ? (__ldg(x + base + t) - m.x) / den : 0.f;
+normalize_rows_kernel(const float* __restrict__ x, const float2* __restrict__ ms, float* __restrict__ y, int rows,
+                      long long T, const long long* __restrict__ lengths) {
+    for (long long row = blockIdx.y; row < rows; row += gridDim.y) {   // grid.y is capped at 65535; row + gridDim.y
+                                                                       // may pass INT_MAX
+        const float2 m = ms[row];
+        const float den = m.y + 1e-9f;
+        const size_t base = (size_t)row * T;
+        const long long Tr = row_length(lengths, row, T);      // beyond the utterance: the zero padding stays zero
+        for (long long t = (long long)blockIdx.x * 256 + threadIdx.x; t < T; t += (long long)gridDim.x * 256)
+            y[base + t] = t < Tr ? (__ldg(x + base + t) - m.x) / den : 0.f;
+    }
 }
 
 int launch_utterance_stats(const float* wav, double* sums, float2* mean_std, int rows, long long T,
@@ -94,11 +96,11 @@ int launch_utterance_stats(const float* wav, double* sums, float2* mean_std, int
 int launch_normalize_rows(const float* wav, const float2* mean_std, float* out, int rows, long long T,
                           const long long* lengths, cudaStream_t st) {
     if (!wav || !mean_std || !out || rows <= 0 || T <= 0) return SDR_ERR_BAD_ARGUMENT;
-    if (rows > 65535) return SDR_ERR_UNSUPPORTED;
     long long gx = (T + 256 * 4 - 1) / (256 * 4);
     if (gx < 1) gx = 1;
     if (gx > 4096) gx = 4096;
-    normalize_rows_kernel<<<dim3((unsigned)gx, (unsigned)rows), 256, 0, st>>>(wav, mean_std, out, T, lengths);
+    normalize_rows_kernel<<<dim3((unsigned)gx, (unsigned)(rows < 65535 ? rows : 65535)), 256, 0, st>>>(
+        wav, mean_std, out, rows, T, lengths);
     return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
 }
 

@@ -423,6 +423,7 @@ tac_apply_kernel(const float* __restrict__ x, const float* __restrict__ o, NormI
 int launch_tac_apply(const float* x, const float* o, const NormIn& nin, float* out,
                      int samples, int n, int L, cudaStream_t st) {
     const long long items = (long long)n * L;
+    if (items > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;                // the kernel counts a sample's items in int
     const int chunks = (int)((items + 1023) / 1024);
     const long long grid = (long long)chunks * samples;
     if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
