@@ -7,87 +7,11 @@
 #include <cstring>
 #include <initializer_list>
 #include "common.cuh"
+#include "launchers.cuh"
 
 #define SDR_TRY(expr) do { int _e = (expr); if (_e != SDR_OK) return _e; } while (0)
 
 namespace sdr {
-
-// kernel launchers (levels.cu, pointwise.cu, frontback.cu, tac.cu)
-int launch_depthwise(const float*, const NormIn&, const float*, const float*, float*, double*, int, int, int, int, cudaStream_t);
-int launch_merge(const float* const*, const NormIn*, int, float*, double*, int, int, int, cudaStream_t);
-// depthwise pyramid in one pass (pyramid.cu)
-bool pyramid_eligible(int D, int samples, int C, int L);
-size_t pyramid_rowstats_bytes(int samples, int C, int D);
-size_t pyramid_table_bytes(int samples, int C, int D);
-int launch_pyramid(const float*, const NormIn&, const float* const*, const float* const*, const float* const*,
-                   const float* const*, float* const*, double*, double*, float*, int, int, int, int, cudaStream_t);
-int launch_merge_pyramid(const float* const*, const float*, int, float*, double*, int, int, int, cudaStream_t);
-int launch_pyramid_fused(const float*, const NormIn&, const float* const*, const float* const*, const float* const*,
-                         const float* const*, float*, double*, double*, double*, float*, int, int, int, int, cudaStream_t);
-int launch_pointwise_ffma(const float*, const NormIn&, const float*, const float*, const float*, const float*, int,
-                          float*, double*, int, int, int, int, int, cudaStream_t);
-int launch_encoder(const float*, const float*, const float*, int, float*, double*, int, int, long long, int, int, int, int, cudaStream_t);
-bool encoder_ffma_fits(int A, int K);
-int launch_overlap_add(const float*, const float*, const float*, const float2*, float*, int, int, int, int, long long, cudaStream_t);
-int launch_mixture_consistency(const float*, const float*, float*, int, int, long long, int, void*, cudaStream_t);
-int launch_tac(const float*, const float* const*, float*, double*, int, int, int, int, cudaStream_t);
-int launch_tac_apply(const float*, const float*, const NormIn&, float*, int, int, int, cudaStream_t);
-bool preadd_eligible(int M, int K, int L);
-int launch_pointwise_small_preadd(const float*, const float*, const NormIn&, float*, const float*, const float*, float*,
-                                  double*, int, int, int, int, cudaStream_t);
-// causal model (causal.cu)
-bool causal_pyramid_eligible(int D, int L);
-int launch_causal_pyramid(const float*, const float*, const float* const*, const float* const*, const float* const*, float*,
-                          int, int, int, int, cudaStream_t);
-int launch_take_taps(const float*, float*, long long, int, int, cudaStream_t);
-int launch_scale_by_scalar(const float*, const float*, float*, long long, cudaStream_t);
-// streaming of the causal model (stream.cu)
-bool causal_stream_eligible(int D, int F);
-int launch_stream_frame(const float*, const float*, long long, float*, int, int, int, int, int, long long, cudaStream_t);
-int launch_causal_stream(const float*, const float*, const float* const*, const float* const*, const float* const*,
-                         float*, long long, float*, int, int, int, int, cudaStream_t);
-int launch_stream_ola(const float*, const float*, float*, long long, long long, float*, int, int, int, int, int,
-                      long long, int, cudaStream_t);
-int launch_stream_flush(const float*, long long, long long, float*, int, int, int, int, cudaStream_t);
-// original model (original.cu)
-int launch_residual_norm(const float*, const NormIn&, float*, const NormIn&, double*, int, int, int, cudaStream_t);
-int launch_softmax_gate(const float*, const float*, float*, int, int, int, int, cudaStream_t);
-int launch_toeplitz_mask(const float*, const float*, float*, float*, int, int, cudaStream_t);
-int launch_grouped_decoder(const float*, float*, int, int, int, cudaStream_t);
-// pre/post steps (prepost.cu)
-int launch_utterance_stats(const float*, double*, float2*, int, long long, const long long*, cudaStream_t);
-int launch_normalize_rows(const float*, const float2*, float*, int, long long, const long long*, cudaStream_t);
-size_t pit_sisdr_scratch_bytes(int B, int S);
-size_t stabilized_sisdr_scratch_bytes(int B, int n_est, int n_act);
-int launch_stabilized_sisdr(const float*, const float*, float*, int*, int, int, int, int, long long, int, int, double, void*,
-                            cudaStream_t);
-int launch_pairwise_neg_sdr(const float*, const float*, float*, int, int, long long, int, int, int, void*, cudaStream_t);
-int launch_pit_sisdr(const float*, const float*, const float*, float*, int*, int, int, long long, int, int, double,
-                     void*, cudaStream_t);
-// tensor-core path (pointwise_mma.cu)
-bool pointwise_mma_eligible(int M, int K);
-size_t pointwise_mma_packed_bytes(int M, int K);
-int pack_pointwise_mma(const float* W, int M, int K, void* packed, cudaStream_t);
-int launch_pointwise_mma(const float*, const NormIn&, const void*, const float*, const float*, const float*, int,
-                         float*, double*, int, int, int, int, int, cudaStream_t);
-
-// backward of the improved model (backward.cu)
-size_t wgrad_scratch_bytes(int samples, int M, int K, int L);
-int launch_wgrad(const float*, const float*, const NormIn&, float*, float*, float*, int, int, int, int, cudaStream_t);
-size_t norm_bwd_scratch_bytes(int samples, int C);
-int launch_norm_bwd(const float*, const NormIn&, const float*, float*, int, float*, float*, float*, double*, int, int,
-                    int, cudaStream_t);
-size_t dw_bwd_scratch_bytes(int samples, int C);
-int launch_dw_bwd(const float*, const float*, const NormIn&, const float*, const float*, int, float*, float*, float*,
-                  double*, int, int, int, int, cudaStream_t);
-int launch_mask_apply(const float*, const float*, float*, int, int, int, int, cudaStream_t);
-int launch_mask_bwd(const float*, const float*, float*, float*, int, int, int, int, cudaStream_t);
-int launch_frame_gather(const float*, float*, int, int, int, int, long long, cudaStream_t);
-int launch_transpose(const float*, float*, int, int, cudaStream_t);
-
-size_t encoder_mma_packed_bytes(int N, int A, int Kk);
-int pack_encoder_mma(const float* W, int N, int A, int Kk, void* packed, cudaStream_t);
-int launch_encoder_mma(const float*, const void*, const float*, int, float*, double*, int, int, long long, int, int, int, int, cudaStream_t);
 
 static const NormIn kNoNorm{nullptr, nullptr, nullptr, nullptr, 1.0, 0};   // operand read as stored
 

@@ -5,6 +5,7 @@
 // at most kWgChunk positions, or fp64 block sums) go to the workspace and a second pass adds them up in fp64, one
 // output per thread, in index order.  No atomics touch a gradient, so a backward is bitwise reproducible.
 #include "common.cuh"
+#include "launchers.cuh"
 
 namespace sdr {
 

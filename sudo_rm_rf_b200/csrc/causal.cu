@@ -14,8 +14,8 @@
 // shared memory; each thread produces four consecutive outputs of a level from 4-5 LDS.128 of its input; the
 // merge reads every level once and stores float4.  HBM traffic: y once (+ halo, from L2) and m once,
 // 8 B per (row, position) against the 5 round trips of a level-by-level schedule.
-#include <cstdlib>
 #include "common.cuh"
+#include "launchers.cuh"
 
 namespace sdr {
 
@@ -40,13 +40,6 @@ struct CausalPyrArgs {
     int h[kMaxDepthApi];             // left halo of level d, in level-d positions
     int off[kMaxDepthApi];           // float offset of level d's buffer in shared memory (y's buffer is at 0)
 };
-
-__device__ __forceinline__ float prelu(float v, float s) { return v >= 0.f ? v : v * s; }
-// PReLU in two instructions: max(v, s*v) for s <= 1, min otherwise (the side of 1 is uniform per level)
-__device__ __forceinline__ float prelu2(float v, float s, bool s_le1) {
-    const float t = v * s;
-    return s_le1 ? fmaxf(v, t) : fminf(v, t);
-}
 
 __global__ void __launch_bounds__(kCzThreads)
 causal_pyramid_kernel(const CausalPyrArgs a) {
@@ -205,10 +198,6 @@ int launch_causal_pyramid(const float* y, const float* slope_in, const float* co
     // memory): 128 / 160 / 192 / 224 / 256 threads = 206 / 192 / 187 / 193 / 196 us; short windows take fewer threads
     int threads = 192;
     while (threads > 128 && (a.W >> 2) < threads) threads -= 32;
-    if (const char* e = getenv("SDR_CZ_THREADS")) {       // measurement override (tools/): 128..256, a multiple of 32
-        const int t = atoi(e);
-        if (t >= 128 && t <= kCzThreads && t % 32 == 0) threads = t;
-    }
     causal_pyramid_kernel<<<(unsigned)grid, threads, smem, st>>>(a);
     return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
 }

@@ -71,6 +71,22 @@ __device__ __forceinline__ float apply_norm(const ChanNorm& c, float x) {
     return (y >= 0.f) ? y : y * c.slope;          // slope == 1 when no activation
 }
 
+// The same GlobLN with the mean folded into the shift: y = x * a + b, a = gamma * rstd, b = beta - mean * a (one fmaf
+// per element; no PReLU fields).  ChanNorm subtracts the mean first and FoldedNorm folds it in, so the two round
+// differently and are NOT interchangeable: each kernel keeps the one it was validated with.
+struct FoldedNorm { float a, b; };
+__device__ __forceinline__ FoldedNorm fold_norm(const NormIn& n, const SampleNorm& s, int c) {
+    FoldedNorm f{1.f, 0.f};
+    if (n.stats) { f.a = __ldg(n.gamma + c) * s.rstd; f.b = fmaf(-s.mean, f.a, __ldg(n.beta + c)); }
+    return f;
+}
+
+// PReLU in two instructions: max(v, s*v) for s <= 1, min otherwise (the caller decides the slope's side of 1 once)
+__device__ __forceinline__ float prelu2(float v, float s, bool s_le1) {
+    const float t = v * s;
+    return s_le1 ? fmaxf(v, t) : fminf(v, t);
+}
+
 __device__ __forceinline__ float warp_sum(float v) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);

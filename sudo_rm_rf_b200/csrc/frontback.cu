@@ -12,6 +12,7 @@
 //   remove_trailing_zeros       improved_sudormrf.py:316-318      crop to T
 //   mixture_consistency.apply   mixture_consistency.py:14-36
 #include "common.cuh"
+#include "launchers.cuh"
 
 namespace sdr {
 

@@ -7,6 +7,7 @@
 // Each kernel stores its RAW result once and accumulates the (sum, sumsq) of
 // that result per sample in fp64 so the consumer can normalise while loading.
 #include "common.cuh"
+#include "launchers.cuh"
 
 namespace sdr {
 
@@ -237,56 +238,16 @@ merge_scalar_kernel(MergeArgs a, float* __restrict__ m, double* __restrict__ sta
 // (t = y*slope; y = slope <= 1 ? max(y,t) : min(y,t)), so the kernels sit on the
 // HBM roofline instead of the issue roofline.
 // ---------------------------------------------------------------------------
-struct FoldedNorm { float a, b; };
-__device__ __forceinline__ FoldedNorm fold_norm(const NormIn& n, const SampleNorm& s, int c) {
-    FoldedNorm f{1.f, 0.f};
-    if (n.stats) { f.a = __ldg(n.gamma + c) * s.rstd; f.b = fmaf(-s.mean, f.a, __ldg(n.beta + c)); }
-    return f;
-}
 template <bool ACT>
 __device__ __forceinline__ float norm_act(float x, const FoldedNorm& f, float slope, bool slope_le1) {
-    float y = fmaf(x, f.a, f.b);
-    if (ACT) { const float t = y * slope; y = slope_le1 ? fmaxf(y, t) : fminf(y, t); }
-    return y;
+    const float y = fmaf(x, f.a, f.b);
+    return ACT ? prelu2(y, slope, slope_le1) : y;
 }
 
-// tuning knobs: 128 threads x 4 runs (2 for the merge); ld.global.nc.L1::no_allocate + st.global.cs are not used
-// (stride-2 levels measured slower with them)
-#ifndef SDR_DW_THREADS
-#define SDR_DW_THREADS 128
-#endif
-#ifndef SDR_DW_ITEMS
-#define SDR_DW_ITEMS 4
-#endif
-#ifndef SDR_MG_THREADS
-#define SDR_MG_THREADS 128
-#endif
-#ifndef SDR_MG_ITEMS
-#define SDR_MG_ITEMS 2
-#endif
-#ifndef SDR_STREAM_HINTS
-#define SDR_STREAM_HINTS 0
-#endif
-// streaming accesses: every byte of these kernels is touched once, so (optionally) keep it out of L1
-__device__ __forceinline__ float4 ld_stream4(const float* p) {
-#if SDR_STREAM_HINTS
-    float4 r;
-    asm volatile("ld.global.nc.L1::no_allocate.v4.f32 {%0, %1, %2, %3}, [%4];"
-                 : "=f"(r.x), "=f"(r.y), "=f"(r.z), "=f"(r.w) : "l"(p));
-    return r;
-#else
-    return ldg4(p);
-#endif
-}
-__device__ __forceinline__ void st_stream4(float* p, float4 v) {
-#if SDR_STREAM_HINTS
-    asm volatile("st.global.cs.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(p), "f"(v.x), "f"(v.y), "f"(v.z), "f"(v.w) : "memory");
-#else
-    *reinterpret_cast<float4*>(p) = v;
-#endif
-}
-constexpr int kDw8Threads = SDR_DW_THREADS;
-constexpr int kDw8Items = SDR_DW_ITEMS;       // runs of 8 outputs per thread
+// 128 threads x 4 runs (2 for the merge).  Every byte of these kernels is touched once, but the L1-bypass hints
+// (ld.global.nc.L1::no_allocate + st.global.cs) measured slower on the stride-2 levels, so the accesses are plain.
+constexpr int kDw8Threads = 128;
+constexpr int kDw8Items = 4;         // runs of 8 outputs per thread
 
 // requires Lout % 8 == 0
 template <int STRIDE, bool ACT>
@@ -325,7 +286,7 @@ dw5_wide_kernel(const float* __restrict__ x, NormIn nin,
             if (STRIDE == 1) {
                 const float* xr = xs + (size_t)c * Lin + 8 * q;       // window v[0..11] = positions 8q-2 .. 8q+9
                 float v[12];
-                const float4 m0 = ld_stream4(xr), m1 = ld_stream4(xr + 4);
+                const float4 m0 = ldg4(xr), m1 = ldg4(xr + 4);
                 float2 l = make_float2(0.f, 0.f), r = make_float2(0.f, 0.f);
                 const bool hl = q > 0, hr = q < QR - 1;
                 if (hl) l = __ldg(reinterpret_cast<const float2*>(xr - 2));
@@ -348,7 +309,7 @@ dw5_wide_kernel(const float* __restrict__ x, NormIn nin,
             } else {
                 const float* xr = xs + (size_t)c * Lin + 16 * q;      // window v[0..18] = positions 16q-2 .. 16q+16
                 float v[19];
-                const float4 m0 = ld_stream4(xr), m1 = ld_stream4(xr + 4), m2 = ld_stream4(xr + 8), m3 = ld_stream4(xr + 12);
+                const float4 m0 = ldg4(xr), m1 = ldg4(xr + 4), m2 = ldg4(xr + 8), m3 = ldg4(xr + 12);
                 float2 l = make_float2(0.f, 0.f);
                 float r = 0.f;
                 const bool hl = q > 0, hr = 16 * q + 16 < Lin;
@@ -370,8 +331,8 @@ dw5_wide_kernel(const float* __restrict__ x, NormIn nin,
                 }
             }
             float* yr = ys + (size_t)c * Lout + 8 * q;
-            st_stream4(yr, make_float4(o[0], o[1], o[2], o[3]));
-            st_stream4(yr + 4, make_float4(o[4], o[5], o[6], o[7]));
+            *reinterpret_cast<float4*>(yr) = make_float4(o[0], o[1], o[2], o[3]);
+            *reinterpret_cast<float4*>(yr + 4) = make_float4(o[4], o[5], o[6], o[7]);
             acc.add_run(o);
         }
     }
@@ -381,8 +342,8 @@ dw5_wide_kernel(const float* __restrict__ x, NormIn nin,
 
 // merge, 16 outputs per thread, coarse-to-fine: s_d[i] = z_d[i]*a_d + (b_d + s_{d+1}[i>>1])
 // requires depth >= 4 and L % 16 == 0
-constexpr int kMg16Threads = SDR_MG_THREADS;
-constexpr int kMg16Items = SDR_MG_ITEMS;
+constexpr int kMg16Threads = 128;
+constexpr int kMg16Items = 2;
 __global__ void __launch_bounds__(kMg16Threads)
 merge_wide_kernel(MergeArgs a, float* __restrict__ m, double* __restrict__ stats_out,
                   int C, int L, int chunks_per_sample) {
@@ -404,10 +365,10 @@ merge_wide_kernel(MergeArgs a, float* __restrict__ m, double* __restrict__ stats
         const size_t row = (size_t)sample * C + c;
         // issue every load of this run first
         const float* z0 = a.z[0] + row * L + 16 * q;
-        const float4 v00 = ld_stream4(z0), v01 = ld_stream4(z0 + 4), v02 = ld_stream4(z0 + 8), v03 = ld_stream4(z0 + 12);
+        const float4 v00 = ldg4(z0), v01 = ldg4(z0 + 4), v02 = ldg4(z0 + 8), v03 = ldg4(z0 + 12);
         const float* z1 = a.z[1] + row * (L >> 1) + 8 * q;
-        const float4 v10 = ld_stream4(z1), v11 = ld_stream4(z1 + 4);
-        const float4 v2 = ld_stream4(a.z[2] + row * (L >> 2) + 4 * q);
+        const float4 v10 = ldg4(z1), v11 = ldg4(z1 + 4);
+        const float4 v2 = ldg4(a.z[2] + row * (L >> 2) + 4 * q);
         const float2 v3 = __ldg(reinterpret_cast<const float2*>(a.z[3] + row * (L >> 3) + 2 * q));
         float base = 0.f;                      // levels >= 4 are constant over the run
         for (int d = 4; d < a.depth; ++d) {
@@ -434,7 +395,7 @@ merge_wide_kernel(MergeArgs a, float* __restrict__ m, double* __restrict__ stats
         float* mr = m + row * L + 16 * q;
 #pragma unroll
         for (int i = 0; i < 4; ++i)
-            st_stream4(mr + 4 * i, make_float4(o[4 * i], o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]));
+            *reinterpret_cast<float4*>(mr + 4 * i) = make_float4(o[4 * i], o[4 * i + 1], o[4 * i + 2], o[4 * i + 3]);
         acc.add_run(o);
       }
     }

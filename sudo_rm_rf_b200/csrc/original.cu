@@ -13,6 +13,7 @@
 //     softmax over the sources (sigmoid for one source) times the encoder output is one element-wise pass.
 //   * the grouped ConvTranspose1d decoder, :245-252: block-diagonal weights for the same frames GEMM + overlap-add.
 #include "common.cuh"
+#include "launchers.cuh"
 
 namespace sdr {
 

@@ -12,6 +12,8 @@
 //   mask_net          improved_sudormrf.py:268-269,295-298  f = PReLU, epilogue relu()*encoder
 //   decoder (as GEMM) improved_sudormrf.py:272-279,300   frames = Wd^T . masked
 #include "common.cuh"
+#include "sm90.cuh"
+#include "launchers.cuh"
 
 namespace sdr {
 
@@ -206,9 +208,6 @@ pw_gemm_kernel(const PwArgs a) {
 // warp), 64 FMAs against 16 weights broadcast from shared memory, float4 stores.
 // Requires K <= 64, L % 4 == 0.
 // ---------------------------------------------------------------------------
-#ifndef SDR_PW_TILE
-#define SDR_PW_TILE 1                  // 1: shapes the tile-staged kernel takes (M <= 32, K <= 32) run on it; 0: pw_small_kernel (A/B builds)
-#endif
 constexpr int kSmMaxThreads = 256;
 constexpr int kSmMT = 16;          // output channels per thread (8 per thread, 5 CTAs per SM, measured slower: res_conv shape 72 -> 88 us)
 constexpr int kSmKT = 8;           // input rows whose loads are issued together (8 x 16 B in flight per thread)
@@ -235,6 +234,9 @@ pw_small_kernel(const PwArgs a, int chunks_per_sample) {
         sW[k][m] = (m0 + m < a.M) ? __ldg(a.W + (size_t)(m0 + m) * a.K + k) : 0.f;
     }
     if (tid < kSmMT) sBias[tid] = (a.bias && m0 + tid < a.M) ? __ldg(a.bias + m0 + tid) : 0.f;
+    // FoldedNorm's arithmetic, written out here and in pw_tile_kernel: through fold_norm() the compiler emits
+    // sample_norm's mu * mu ahead of the second fp64 division, ptxas then no longer fuses it into the variance's
+    // subtraction, and the statistics round differently from what these kernels were validated with.
     if (tid < a.K) {
         float aa = 1.f, bb = 0.f;
         if (a.nin.stats) {
@@ -347,19 +349,14 @@ pw_small_kernel(const PwArgs a, int chunks_per_sample) {
 constexpr int kStMaxRows = 64;         // input rows staged per CTA (K, or 2K with the pre-add operand)
 constexpr int kStMaxK = 32;
 
-__device__ __forceinline__ uint32_t st_smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-
 constexpr int kStThreads = 160;        // block size bound (the launcher picks 128 or 160)
-#ifndef SDR_ST_MINB32
-#define SDR_ST_MINB32 3                // resident CTAs per SM the 32-outputs-per-thread instantiations are compiled for (4: 96 registers
-#endif                                 // with 300 B of spills, 77 us against 69 us at the cfg-4 proj shape)
-#ifndef SDR_ST_MINB16
-#define SDR_ST_MINB16 4                // ... and the 16-outputs-per-thread ones (4 / 5 / 6: 62.8 / 64.8 / 66.4 us at the cfg-4 res_conv shape)
-#endif
+constexpr int kStMinB32 = 3;           // resident CTAs per SM the 32-outputs-per-thread instantiations are compiled for (4: 96 registers
+                                       // with 300 B of spills, 77 us against 69 us at the cfg-4 proj shape)
+constexpr int kStMinB16 = 4;           // ... and the 16-outputs-per-thread ones (4 / 5 / 6: 62.8 / 64.8 / 66.4 us at the cfg-4 res_conv shape)
 // (A persistent version with a double buffer - the next tile's copy in flight during the FFMA loop, 2 CTAs per SM by
 //  shared memory - measured 92 / 73 us against 69 / 63 us for one tile per CTA: profiles/r02b_kernels.md.)
 template <bool PRE, int MT>
-__global__ void __launch_bounds__(kStThreads, MT == 32 ? SDR_ST_MINB32 : SDR_ST_MINB16)
+__global__ void __launch_bounds__(kStThreads, MT == 32 ? kStMinB32 : kStMinB16)
 pw_tile_kernel(const PwArgs a, int tiles_per_sample, int P) {
     extern __shared__ __align__(16) float st_buf[];        // [rows][P]
     __shared__ __align__(16) float sW[kStMaxK][MT];        // [k][m]
@@ -374,15 +371,14 @@ pw_tile_kernel(const PwArgs a, int tiles_per_sample, int P) {
     const int np = min(P, a.L - p0);                        // positions of this tile (a multiple of 4)
     const int rows = PRE ? 2 * a.K : a.K;
     if (tid == 0) {
-        asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(st_smem_u32(&s_bar)), "r"(1) : "memory");
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_init(&s_bar, 1);
+        fence_barrier_init();
         const uint32_t bytes = (uint32_t)np * sizeof(float);
-        asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(st_smem_u32(&s_bar)), "r"(bytes * (uint32_t)rows) : "memory");
+        mbar_arrive_expect_tx(&s_bar, bytes * (uint32_t)rows);
         for (int r = 0; r < rows; ++r) {
             const float* src = (PRE && r >= a.K) ? a.pre_add + ((size_t)sample * a.K + (r - a.K)) * a.L + p0
                                                  : a.x + ((size_t)sample * a.K + r) * a.L + p0;
-            asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                         ::"r"(st_smem_u32(st_buf + (size_t)r * P)), "l"(src), "r"(bytes), "r"(st_smem_u32(&s_bar)) : "memory");
+            bulk_g2s(st_buf + (size_t)r * P, src, bytes, &s_bar);
         }
     }
     for (int i = tid; i < a.K * MT; i += nthr) {
@@ -409,14 +405,7 @@ pw_tile_kernel(const PwArgs a, int tiles_per_sample, int P) {
     const bool act = a.nin.prelu != nullptr;
     const float slope = act ? __ldg(a.nin.prelu) : 1.f;
     __syncthreads();                                        // tables + the initialised barrier are visible
-    {
-        const uint32_t addr = st_smem_u32(&s_bar);
-        uint32_t done;
-        do {
-            asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                         : "=r"(done) : "r"(addr), "r"(0) : "memory");
-        } while (!done);
-    }
+    mbar_wait(&s_bar, 0);
     const int t2 = 2 * tid;                                 // this thread's 2 positions inside the tile
     StatAcc st;
     if (t2 < np) {
@@ -591,7 +580,7 @@ int launch_pointwise_ffma(const float* x, const NormIn& nin, const float* W, con
     const bool vec = (L % 4 == 0) && (al % 16 == 0);
     if (vec && K <= kSmMaxK && M <= 64 && !nin.prelu_pc) {   // streaming small-channel kernels (one shared PReLU slope)
         int tt = 0;
-        if (SDR_PW_TILE && tile_shape(M, K, K, L, epilogue, true, &tt)) return launch_tile<false>(a, samples, tt, st);
+        if (tile_shape(M, K, K, L, epilogue, true, &tt)) return launch_tile<false>(a, samples, tt, st);
         const int threads = small_block_threads(L / 4);
         const int chunks = (L / 4 + threads - 1) / threads;
         const long long gx = (long long)chunks * samples;
@@ -625,7 +614,7 @@ int launch_pointwise_small_preadd(const float* x, const float* pre_add, const No
     a.pre_add = pre_add; a.pre_norm = pre_norm; a.pre_out = xt_out;
     {
         int tt = 0;
-        if (SDR_PW_TILE && tile_shape(M, K, 2 * K, L, 0, true, &tt)) return launch_tile<true>(a, samples, tt, st);
+        if (tile_shape(M, K, 2 * K, L, 0, true, &tt)) return launch_tile<true>(a, samples, tt, st);
     }
     const int threads = small_block_threads(L / 4);
     const int chunks = (L / 4 + threads - 1) / threads;

@@ -35,6 +35,8 @@
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include "common.cuh"
+#include "sm90.cuh"
+#include "launchers.cuh"
 
 namespace sdr {
 
@@ -78,37 +80,8 @@ struct MmaArgs {
 };
 
 // ---------------------------------------------------------------------------
-// PTX wrappers
+// PTX wrappers with this file as their only user (the shared ones: sm90.cuh)
 // ---------------------------------------------------------------------------
-__device__ __forceinline__ uint32_t smem_u32(const void* p) {
-    return static_cast<uint32_t>(__cvta_generic_to_shared(p));
-}
-__device__ __forceinline__ void mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive(uint64_t* bar) {
-    asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(bar)) : "memory");
-}
-__device__ __forceinline__ void mbar_arrive_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void mbar_wait(uint64_t* bar, uint32_t parity) {
-    const uint32_t addr = smem_u32(bar);
-    uint32_t done;
-    do {
-        asm volatile(
-            "{\n\t.reg .pred p;\n\t"
-            "mbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\t"
-            "selp.u32 %0, 1, 0, p;\n\t}"
-            : "=r"(done) : "r"(addr), "r"(parity) : "memory");
-    } while (!done);
-}
-__device__ __forceinline__ void fence_barrier_init() {
-    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
-}
-__device__ __forceinline__ void fence_proxy_async_smem() {
-    asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-}
 // global -> shared tensor (TMA) loads; out-of-range elements arrive as zeros
 __device__ __forceinline__ void tma_load_2d(void* smem_dst, const CUtensorMap* tm, uint64_t* bar, int c0, int c1) {
     asm volatile("cp.async.bulk.tensor.2d.shared::cluster.global.tile.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4}], [%2];"
@@ -481,9 +454,8 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
                         for (int e = 0; e < 2; ++e) {
                             const float x = *reinterpret_cast<const float*>(rp + boff[e + 2 * ph] + c * 128);
                             y[e] = WINDOW ? x : fmaf(x, e ? ab.z : ab.x, e ? ab.w : ab.y);
-                            if constexpr (ACT == 1) {      // PReLU in 2 ops: max(y, s*y) for s <= 1, min otherwise
-                                const float t = y[e] * slope;
-                                y[e] = slope_le1 ? fmaxf(y[e], t) : fminf(y[e], t);
+                            if constexpr (ACT == 1) {
+                                y[e] = prelu2(y[e], slope, slope_le1);
                             } else if constexpr (ACT == 2) {   // this channel's own slope (either side of 1, either sign)
                                 y[e] = y[e] >= 0.f ? y[e] : y[e] * (e ? sl.y : sl.x);
                             }

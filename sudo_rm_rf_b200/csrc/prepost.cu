@@ -7,6 +7,7 @@
 // Both are tiny HBM-streaming reductions next to the forward (a few MB per batch);
 // they exist so that `separate()` and the validation metric never leave the device.
 #include "common.cuh"
+#include "launchers.cuh"
 
 namespace sdr {
 

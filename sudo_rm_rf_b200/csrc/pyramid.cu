@@ -30,6 +30,8 @@
 #include <cstring>
 #include <type_traits>
 #include "common.cuh"
+#include "sm90.cuh"
+#include "launchers.cuh"
 
 namespace sdr {
 
@@ -119,39 +121,15 @@ __device__ __forceinline__ void warp_multi_sum(float (&v)[NV], int lane) {
         n = half + (n & 1);
     }
 }
-__device__ __forceinline__ uint32_t pyr_smem_u32(const void* p) { return static_cast<uint32_t>(__cvta_generic_to_shared(p)); }
-__device__ __forceinline__ void pyr_mbar_init(uint64_t* bar, uint32_t count) {
-    asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(pyr_smem_u32(bar)), "r"(count) : "memory");
-}
-__device__ __forceinline__ void pyr_mbar_expect_tx(uint64_t* bar, uint32_t bytes) {
-    asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(pyr_smem_u32(bar)), "r"(bytes) : "memory");
-}
-__device__ __forceinline__ void pyr_mbar_wait(uint64_t* bar, uint32_t parity) {
-    const uint32_t addr = pyr_smem_u32(bar);
-    uint32_t done;
-    do {
-        asm volatile("{\n\t.reg .pred p;\n\tmbarrier.try_wait.parity.shared::cta.b64 p, [%1], %2;\n\tselp.u32 %0, 1, 0, p;\n\t}"
-                     : "=r"(done) : "r"(addr), "r"(parity) : "memory");
-    } while (!done);
-}
-__device__ __forceinline__ void pyr_bulk_g2s(void* dst, const void* src, uint32_t bytes, uint64_t* bar) {
-    asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
-                 ::"r"(pyr_smem_u32(dst)), "l"(src), "r"(bytes), "r"(pyr_smem_u32(bar)) : "memory");
-}
 
 // Persistent CTAs: rows blockIdx.x, + gridDim.x, ...  The NEXT row's y arrives by 1-D bulk TMA into the other half of
 // a double buffer and its per-row parameters by 4-byte cp.async while the current row is computed, so no thread ever
 // waits on a global load (one CTA per row with plain loads measured 1.7 us per row and SM: launch-to-first-use
 // latency of y, of the 28 parameters and of the fp64 statistics in every CTA).  One barrier per row.
-#ifndef SDR_PYR_MINB
-#define SDR_PYR_MINB 6                  // resident CTAs per SM the <= 256-thread instantiation is compiled for
-#endif
-#ifndef SDR_PYR_STATS_MINB
-#define SDR_PYR_STATS_MINB 5            // the same for kPyrStats (at 6, 40 registers, the per-channel-slope D = 6 one spills)
-#endif
-#ifndef SDR_PYR_MERGE_MINB
-#define SDR_PYR_MERGE_MINB 4            // the same for kPyrMerge, which holds every level of its 16 positions live at once
-#endif                                  // (64 registers; at 5 it spills)
+constexpr int kPyrMinB = 6;                 // resident CTAs per SM the <= 256-thread instantiation is compiled for
+constexpr int kPyrStatsMinB = 5;            // the same for kPyrStats (at 6, 40 registers, the per-channel-slope D = 6 one spills)
+constexpr int kPyrMergeMinB = 4;            // the same for kPyrMerge, which holds every level of its 16 positions live at once
+                                            // (64 registers; at 5 it spills)
 // PC: one PReLU slope per channel (the original model's nn.PReLU(C), sudormrf.py:33): a row is one channel, so the
 // slope simply travels with the row's other parameters; the shared-slope instantiations are unchanged.
 template <int D, int MAXT, int MINB, bool PC, int MODE = kPyrLevels>
@@ -187,7 +165,7 @@ dw_pyramid_kernel(const PyrArgs a) {
             else if (i == 5 * D + 1) src = a.nin.stats ? a.nin.gamma + c : a.bias0 + c;
             else if (PC && i == 5 * D + 3) src = act ? a.nin.prelu + c : a.bias0 + c;
             else src = a.nin.stats ? a.nin.beta + c : a.bias0 + c;
-            asm volatile("cp.async.ca.shared.global [%0], [%1], 4;" ::"r"(pyr_smem_u32(&s_par[slot][i])), "l"(src) : "memory");
+            cp_async4(&s_par[slot][i], src);
         }
     };
     for (int sidx = tid; sidx < samples; sidx += blockDim.x) {
@@ -199,16 +177,16 @@ dw_pyramid_kernel(const PyrArgs a) {
         pyr_smem[LB + (tid < 4 ? tid : L + tid)] = 0.f;
     }
     if (tid == 0) {
-        pyr_mbar_init(&s_bar[0], 1);
-        pyr_mbar_init(&s_bar[1], 1);
-        asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+        mbar_init(&s_bar[0], 1);
+        mbar_init(&s_bar[1], 1);
+        fence_barrier_init();
         if ((int)blockIdx.x < a.rows) {
-            pyr_mbar_expect_tx(&s_bar[0], row_bytes);
-            pyr_bulk_g2s(pyr_smem + 4, a.y + (size_t)blockIdx.x * L, row_bytes, &s_bar[0]);
+            mbar_arrive_expect_tx(&s_bar[0], row_bytes);
+            bulk_g2s(pyr_smem + 4, a.y + (size_t)blockIdx.x * L, row_bytes, &s_bar[0]);
         }
     }
     if ((int)blockIdx.x < a.rows) stage_params(blockIdx.x, 0);
-    asm volatile("cp.async.wait_all;" ::: "memory");
+    cp_async_wait_all();
     __syncthreads();
 
     const int w0 = warp * S - ML;
@@ -225,8 +203,8 @@ dw_pyramid_kernel(const PyrArgs a) {
     if (tid == 0) {
         const int nxt = row + gridDim.x;
         if (nxt < a.rows) {
-            pyr_mbar_expect_tx(&s_bar[cur ^ 1], row_bytes);
-            pyr_bulk_g2s(pyr_smem + (size_t)(cur ^ 1) * LB + 4, a.y + (size_t)nxt * L, row_bytes, &s_bar[cur ^ 1]);
+            mbar_arrive_expect_tx(&s_bar[cur ^ 1], row_bytes);
+            bulk_g2s(pyr_smem + (size_t)(cur ^ 1) * LB + 4, a.y + (size_t)nxt * L, row_bytes, &s_bar[cur ^ 1]);
         }
     }
     if (row + (int)gridDim.x < a.rows) stage_params(row + gridDim.x, cur ^ 1);
@@ -234,7 +212,7 @@ dw_pyramid_kernel(const PyrArgs a) {
     float na = 1.f, nb = 0.f;
     if (a.nin.stats) { const float2 mr = s_mr[sample]; na = par[5 * D + 1] * mr.y; nb = fmaf(-mr.x, na, par[5 * D + 2]); }
     if constexpr (PC) { if (act) { slope = par[5 * D + 3]; sle1 = slope <= 1.f; } }      // this row's (channel's) own slope
-    pyr_mbar_wait(&s_bar[cur], (it >> 1) & 1);
+    mbar_wait(&s_bar[cur], (it >> 1) & 1);
 
     // y[g0-2 .. g0+17] from the row buffer (index 4 + position), then u = PReLU(GLN(y)), 0 outside the row
     float u[20];
@@ -434,7 +412,7 @@ dw_pyramid_kernel(const PyrArgs a) {
         const int own = warp_multi_owner<2 * D>(lane);
         if (own >= 0) s_part[cur][warp][own] = part[0];
     }
-    asm volatile("cp.async.wait_all;" ::: "memory");        // the next row's parameters (issued at the top of this row)
+    cp_async_wait_all();                                    // the next row's parameters (issued at the top of this row)
     __syncthreads();
     if constexpr (kMerge) {
         if (tid < 2) {
@@ -625,14 +603,8 @@ struct MergePyrArgs {
     const float* table;
     int D, C, L;
 };
-#ifndef SDR_MP_THREADS
-#define SDR_MP_THREADS 128
-#endif
-#ifndef SDR_MP_ITEMS
-#define SDR_MP_ITEMS 4                 // runs of 16 outputs per thread (1 / 2 / 4 on one box: 116.2 / 108.7 / 104.7 us at cfg 2; 256 threads x 1: 130.9)
-#endif
-constexpr int kMpThreads = SDR_MP_THREADS;
-constexpr int kMpItems = SDR_MP_ITEMS;
+constexpr int kMpThreads = 128;
+constexpr int kMpItems = 4;            // runs of 16 outputs per thread (1 / 2 / 4 on one box: 116.2 / 108.7 / 104.7 us at cfg 2; 256 threads x 1: 130.9)
 
 __global__ void __launch_bounds__(kMpThreads)
 merge_pyramid_kernel(const MergePyrArgs a, float* __restrict__ m, double* __restrict__ stats_out, int chunks_per_sample) {
@@ -782,14 +754,14 @@ int launch_pyramid(const float* y, const NormIn& nin, const float* const* w5, co
     auto launch = [&](auto kern) -> int { return launch_pyramid_pass(kern, a, samples, st); };
     if (nin.prelu && nin.prelu_pc) {
         if (threads <= 256)
-            rc = D == 4 ? launch(dw_pyramid_kernel<4, 256, SDR_PYR_MINB, true>)
-                        : (D == 5 ? launch(dw_pyramid_kernel<5, 256, SDR_PYR_MINB, true>) : launch(dw_pyramid_kernel<6, 256, SDR_PYR_MINB, true>));
+            rc = D == 4 ? launch(dw_pyramid_kernel<4, 256, kPyrMinB, true>)
+                        : (D == 5 ? launch(dw_pyramid_kernel<5, 256, kPyrMinB, true>) : launch(dw_pyramid_kernel<6, 256, kPyrMinB, true>));
         else
             rc = D == 4 ? launch(dw_pyramid_kernel<4, 1024, 1, true>)
                         : (D == 5 ? launch(dw_pyramid_kernel<5, 1024, 1, true>) : launch(dw_pyramid_kernel<6, 1024, 1, true>));
     } else if (threads <= 256)      // rows up to 7-8 windows (L <= 3712 / 3328): compiled for several resident CTAs per SM
-        rc = D == 4 ? launch(dw_pyramid_kernel<4, 256, SDR_PYR_MINB, false>)
-                    : (D == 5 ? launch(dw_pyramid_kernel<5, 256, SDR_PYR_MINB, false>) : launch(dw_pyramid_kernel<6, 256, SDR_PYR_MINB, false>));
+        rc = D == 4 ? launch(dw_pyramid_kernel<4, 256, kPyrMinB, false>)
+                    : (D == 5 ? launch(dw_pyramid_kernel<5, 256, kPyrMinB, false>) : launch(dw_pyramid_kernel<6, 256, kPyrMinB, false>));
     else
         rc = D == 4 ? launch(dw_pyramid_kernel<4, 1024, 1, false>)
                     : (D == 5 ? launch(dw_pyramid_kernel<5, 1024, 1, false>) : launch(dw_pyramid_kernel<6, 1024, 1, false>));
@@ -801,7 +773,7 @@ int launch_pyramid(const float* y, const NormIn& nin, const float* const* w5, co
 // One pass of the fused stage (M = kPyrStats or kPyrMerge), with the instantiation the row length and slope call for.
 template <int M>
 static int launch_fused_pass(const PyrArgs& a, bool pc, int samples, cudaStream_t st) {
-    constexpr int MB = M == kPyrMerge ? SDR_PYR_MERGE_MINB : SDR_PYR_STATS_MINB;
+    constexpr int MB = M == kPyrMerge ? kPyrMergeMinB : kPyrStatsMinB;
     const int D = a.D, threads = 32 * pyramid_windows(a.D, a.L);
     auto launch = [&](auto kern) -> int { return launch_pyramid_pass(kern, a, samples, st); };
     if (pc) {

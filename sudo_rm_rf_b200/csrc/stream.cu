@@ -9,6 +9,7 @@
 // convolutions are one GEMM each over all columns.  Chunks start on multiples of 2^(D-1) frames, so every level's
 // chunk starts on an integer position of that level.  All state starts at zero, the reference's zero padding.
 #include "common.cuh"
+#include "launchers.cuh"
 
 namespace sdr {
 
@@ -77,11 +78,6 @@ struct StreamStageArgs {
     int ooff;
 };
 
-__device__ __forceinline__ float st_prelu2(float v, float s, bool s_le1) {   // prelu2 of causal.cu
-    const float t = v * s;
-    return s_le1 ? fmaxf(v, t) : fminf(v, t);
-}
-
 __host__ __device__ __forceinline__ int st_nin(int d, int F) { return d == 0 ? F : F >> (d - 1); }
 
 __global__ void __launch_bounds__(kStThreads)
@@ -114,8 +110,8 @@ causal_stream_kernel(const StreamStageArgs a) {
             if (row >= nr) continue;
             const float4 v = ldg4(a.y + (size_t)(c0 + row) * BF + (size_t)slot * F + 4 * q);
             float* dst = smem + (a.xoff[0] + kStHist + 4 * q) * R + row;
-            dst[0] = st_prelu2(v.x, sp, sp1); dst[R] = st_prelu2(v.y, sp, sp1);
-            dst[2 * R] = st_prelu2(v.z, sp, sp1); dst[3 * R] = st_prelu2(v.w, sp, sp1);
+            dst[0] = prelu2(v.x, sp, sp1); dst[R] = prelu2(v.y, sp, sp1);
+            dst[2 * R] = prelu2(v.z, sp, sp1); dst[3 * R] = prelu2(v.w, sp, sp1);
         }
     }
     __syncthreads();
@@ -146,7 +142,7 @@ causal_stream_kernel(const StreamStageArgs a) {
                 float acc = bias;
 #pragma unroll
                 for (int j = 0; j < kStTaps; ++j) acc = fmaf(w[j], x[j * R], acc);
-                out[p * R] = st_prelu2(acc, sl, sl1);
+                out[p * R] = prelu2(acc, sl, sl1);
             }
         }
         __syncthreads();

@@ -15,6 +15,7 @@
 // x + GlobLN(o) which is both the U-ConvBlock input and its residual.
 #include <cuda_bf16.h>
 #include "common.cuh"
+#include "launchers.cuh"
 
 namespace sdr {
 
@@ -194,10 +195,8 @@ struct TacFrags {
     float b1[kTacH], b2[kTacH], b3[16];
 };
 
-#ifndef SDR_TAC_MINB
-#define SDR_TAC_MINB 2                 // resident CTAs per SM tac_mma16_kernel is compiled (and its persistent grid sized) for
-#endif
-__global__ void __launch_bounds__(32 * kTacWarps, SDR_TAC_MINB)
+constexpr int kTacMinB = 2;           // resident CTAs per SM tac_mma16_kernel is compiled (and its persistent grid sized) for
+__global__ void __launch_bounds__(32 * kTacWarps, kTacMinB)
 tac_mma16_kernel(const float* __restrict__ x, TacParams p, float* __restrict__ o, double* __restrict__ stats,
                  int G, int L, int tiles_per_b, int total_tiles) {
     extern __shared__ __align__(16) uint8_t tac_smem[];
@@ -360,7 +359,7 @@ static int launch_tac_mma16(const float* x, const TacParams& p, float* o, double
     if (cudaFuncSetAttribute(tac_mma16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
         return SDR_ERR_CUDA;
     long long grid = (total + kTacWarps - 1) / kTacWarps;
-    if (grid > (long long)SDR_TAC_MINB * sms) grid = (long long)SDR_TAC_MINB * sms;                   // warps loop over tiles; the weight fragments are built once per CTA
+    if (grid > (long long)kTacMinB * sms) grid = (long long)kTacMinB * sms;                   // warps loop over tiles; the weight fragments are built once per CTA
     tac_mma16_kernel<<<(unsigned)grid, 32 * kTacWarps, smem, st>>>(x, p, o, stats, G, L, tiles_per_b, (int)total);
     return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
 }
