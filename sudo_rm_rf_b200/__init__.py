@@ -12,6 +12,8 @@ from .improved_sudormrf import SuDORMRF                                       # 
 from .groupcomm_sudormrf_v2 import GroupCommSudoRmRf                          # noqa: F401
 from .causal_improved_sudormrf_v3 import CausalSuDORMRF                       # noqa: F401
 from .sudormrf import SuDORMRF as OriginalSuDORMRF                            # noqa: F401
+from ._engine import refresh_weights                                          # noqa: F401
 
 __all__ = ["SuDORMRF", "GroupCommSudoRmRf", "CausalSuDORMRF", "OriginalSuDORMRF", "improved_sudormrf",
-           "groupcomm_sudormrf_v2", "causal_improved_sudormrf_v3", "sudormrf", "mixture_consistency"]
+           "groupcomm_sudormrf_v2", "causal_improved_sudormrf_v3", "sudormrf", "mixture_consistency",
+           "refresh_weights"]

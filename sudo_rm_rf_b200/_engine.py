@@ -13,11 +13,25 @@ import warnings
 from typing import List
 
 import torch
+from torch.optim.optimizer import register_optimizer_step_post_hook
 
 from . import _native as N
 
 _tls_lock = threading.Lock()
 _warned_detached = False
+
+# Bumped after every optimizer step, of any optimizer.  Fused optimizers (``fused=True``) write the parameters
+# without bumping their version counters, so the weight signature also carries this generation: any step forces a
+# repack on the next call, as the foreach and single-tensor optimizers already do through the counters.
+_generation = 0
+
+
+def _bump_generation(*_):
+    global _generation
+    _generation += 1
+
+
+register_optimizer_step_post_hook(_bump_generation)
 
 
 def make_config(model) -> N.SdrConfig:
@@ -114,11 +128,14 @@ def _fetch(model, dotted: str) -> torch.Tensor:
 
 class _DeviceState:
     """Per (model, device) cache: packed weights + workspace."""
-    __slots__ = ("sig", "packed", "workspace", "staging", "tensors", "pslots", "mslots", "graphs",
-                 "stream", "event")
+    __slots__ = ("sig", "storages", "packed", "workspace", "staging", "captured", "retired", "tensors", "pslots",
+                 "mslots", "graphs", "stream", "event")
 
     def __init__(self):
         self.sig = None
+        self.storages = None     # the storages `sig` describes, kept alive so that no other tensor takes their addresses
+        self.captured = set()    # buffer slots ("packed", "workspace", "staging") a CUDA-graph capture has addressed
+        self.retired = []        # replaced buffers a captured graph may still address: never handed back to the allocator
         self.packed = None
         self.workspace = None
         self.staging = None
@@ -142,8 +159,23 @@ def _state(model, device) -> _DeviceState:
 
 
 def drop_cache(model) -> None:
-    """Forget packed weights, workspaces and captured graphs (they are rebuilt on the next call)."""
+    """Forget packed weights, workspaces and captured graphs (they are rebuilt on the next call).  This frees every
+    buffer a CUDA graph captured from this model addresses: such graphs must not be replayed afterwards."""
     model.__dict__.pop("_b200_cache", None)
+
+
+def refresh_weights(model) -> None:
+    """Make the next native call re-pack ``model``'s weights.
+
+    Writes through autograd-visible tensors (``load_state_dict``, in-place ops under ``no_grad``, ``detach()``,
+    ``state_dict()`` tensors, ``nn.init``), optimizer steps of any kind and replaced Parameters or sub-modules are
+    noticed without it.  Writes that bypass the version counter are not: ``p.data.<op>_()``, ``p.data.copy_()``,
+    DLPack and other foreign writers, ``dist.broadcast(p.data)``.  Call this after them.  Graphs captured earlier keep
+    the weights they were captured with; capture again after the next call."""
+    if isinstance(model, torch.nn.DataParallel):
+        model = model.module
+    for st in model.__dict__.get("_b200_cache", {}).values():
+        st.sig = None
 
 
 class NativeModuleMixin:
@@ -183,13 +215,31 @@ def _leave_stream(st: _DeviceState, cur) -> None:
     st.stream = cur
 
 
+def _hand_out(st: _DeviceState, slot: str) -> None:
+    """Called when the buffer in ``slot`` is given to a kernel: under stream capture the graph keeps its address."""
+    if torch.cuda.is_current_stream_capturing():
+        st.captured.add(slot)
+
+
+def _replace(st: _DeviceState, slot: str, buf) -> None:
+    """Puts ``buf`` in ``slot``.  The old buffer is freed, unless a captured graph addresses it: a user's graph
+    outlives the cache's view of it, and its replay would write into (or read weights from) whatever tensor the
+    allocator handed that memory to next.  Such buffers are retired instead, and live as long as the cache."""
+    old = getattr(st, slot)
+    if old is not None and slot in st.captured:
+        st.retired.append(old)
+    st.captured.discard(slot)
+    setattr(st, slot, buf)
+
+
 def _ensure_workspace(st: _DeviceState, nbytes: int, device) -> None:
     if st.workspace is None or st.workspace.numel() < nbytes:
         if st.event is not None:
             st.event.synchronize()      # kernels of an earlier call (possibly on another stream) still use it
-        st.workspace = None
+        _replace(st, "workspace", None)
         st.graphs.clear()               # captured graphs point into the old workspace
         st.workspace = torch.empty(nbytes, dtype=torch.uint8, device=device)
+    _hand_out(st, "workspace")
 
 
 def _walk(model, names):
@@ -227,11 +277,24 @@ def _cached_tensors(st: _DeviceState):
     return st.tensors
 
 
+def weight_signature(tensors) -> tuple:
+    """What the packed weights were made from: the optimizer-step generation and each tensor's address and version
+    counter.  Host only.  An address names the data only while its storage is alive; the cache keeps the storages
+    of the signature it holds (``weight_storages``), so a tensor swapped in through ``p.data = t`` cannot land on the
+    address of the one it replaced."""
+    return (_generation, tuple([(t.data_ptr(), t._version) for t in tensors]))
+
+
+def weight_storages(tensors) -> list:
+    return [t.untyped_storage() for t in tensors]
+
+
 def packed_weights(model, cfg: N.SdrConfig, device) -> torch.Tensor:
     """Flat packed-weight buffer for ``model`` on ``device``.
 
-    Master modules: re-packed whenever a parameter's storage or version counter changes, or a Parameter /
-    sub-module object was replaced (identity of every object on the path is checked, ~50 us).
+    Master modules: re-packed whenever a parameter's storage or version counter changes, an optimizer steps, or a
+    Parameter / sub-module object was replaced (identity of every object on the path is checked, ~50 us), or after
+    ``refresh_weights``.
     ``nn.DataParallel`` replicas: packed on EVERY forward.  Their parameters are fresh broadcast copies whose
     ``_version`` is always 0 and whose addresses the caching allocator reuses, so no signature can tell a new
     set of weights from the previous one; the replica shares ``_b200_cache`` with its master."""
@@ -253,8 +316,9 @@ def packed_weights(model, cfg: N.SdrConfig, device) -> torch.Tensor:
             except KeyError:           # parameters held as plain attributes: no caching
                 tensors = [_fetch(model, n) for n in names]
                 st.tensors = st.pslots = st.mslots = None
-        sig = tuple([(t.data_ptr(), t._version) for t in tensors])
+        sig = weight_signature(tensors)
         if st.sig == sig and st.packed is not None:
+            _hand_out(st, "packed")
             return st.packed
     if names is None:
         names = state_dict_names(cfg)
@@ -282,7 +346,9 @@ def packed_weights(model, cfg: N.SdrConfig, device) -> torch.Tensor:
     ptrs = (C.c_void_p * n)(*[C.c_void_p(t.data_ptr()) for t in flat])
     N.check(lib.sdr_pack_weights(C.byref(cfg), ptrs, n, C.c_void_p(packed.data_ptr()), nbytes,
                                  _stream_ptr(device)), "sdr_pack_weights")
-    st.sig, st.packed = sig, packed
+    st.sig, st.storages = sig, (weight_storages(tensors) if sig is not None else None)
+    _replace(st, "packed", packed)
+    _hand_out(st, "packed")
     st.graphs.clear()          # captured graphs hold the old packed buffer
     return packed
 
@@ -415,7 +481,8 @@ def forward_host(model, host_wav: torch.Tensor, host_out: torch.Tensor = None,
             if st.event is not None:
                 st.event.synchronize()
             st.graphs.clear()
-            st.staging = torch.empty(io_bytes, dtype=torch.uint8, device=device)
+            _replace(st, "staging", torch.empty(io_bytes, dtype=torch.uint8, device=device))
+        _hand_out(st, "staging")
         cur0 = _enter_stream(st, device)
 
         def enqueue():

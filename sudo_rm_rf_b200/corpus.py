@@ -104,10 +104,7 @@ def separate_corpus(model, wavs: Iterable[torch.Tensor], max_batch: int = 32,
             ws_bytes = lib.sdr_separate_workspace_bytes(C.byref(cfg), B, Tp)
             if ws_bytes == 0:
                 raise N.NativeError("bad model configuration (sdr_separate_workspace_bytes returned 0)")
-            if st.workspace is None or st.workspace.numel() < ws_bytes:
-                st.workspace = None
-                st.graphs.clear()
-                st.workspace = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+            _engine._ensure_workspace(st, ws_bytes, device)
             out = torch.empty((B, S, Tp), dtype=torch.float32, device=device)
             N.check(lib.sdr_separate_ragged(
                 C.byref(cfg), C.c_void_p(packed.data_ptr()), C.c_void_p(batch.data_ptr()),

@@ -394,9 +394,10 @@ def test_sgd_ten_steps_track_oracle():
         print(f"sgd step {step}: worst parameter {worst[2]} native rel_l2 {worst[0]:.2e} (fp32 eager {worst[1]:.2e})")
 
 
-def _runner_loop(model, params, forward, steps=10):
-    """run_improved_sudormrf.py's step: PIT(neg SI-SDR) -> backward -> clip_grad_norm_(5.0) -> Adam(1e-3)."""
-    opt = torch.optim.Adam(params, lr=1e-3)
+def _runner_loop(model, params, forward, steps=10, make_opt=None):
+    """run_improved_sudormrf.py's step: PIT(neg SI-SDR) -> backward -> clip_grad_norm_(5.0) -> Adam(1e-3), or the
+    optimizer `make_opt(params)` builds."""
+    opt = make_opt(params) if make_opt is not None else torch.optim.Adam(params, lr=1e-3)
     gen = torch.Generator().manual_seed(33)
     B, T = 2, 4000
     tgt = torch.randn(B, 2, T, generator=gen)
