@@ -14,6 +14,22 @@
  * stream passed in; nothing synchronises.  Fully re-entrant (nn.DataParallel
  * calls forward from one host thread per device).
  *
+ * Caller-owned buffers (tests/test_gpu_scratch.py runs every entry on exactly-sized, guarded buffers filled with
+ * NaN and with 1e30 patterns):
+ *   - Contents on entry are ignored for every workspace and scratch buffer, `saved` of sdr_forward_train, the device
+ *     staging buffer of sdr_forward_host, the packed buffer of sdr_pack_weights and every output: a result depends on
+ *     the weights and the inputs only, whatever an earlier call of any shape or variant left behind.  Every element
+ *     of an output is written.  Nothing outside the stated sizes is read or written, and inputs are not modified.
+ *   - Required on entry: the stream state reset by sdr_stream_reset before a slot's first step; the statistics
+ *     slots of the per-stage entries zeroed (they are accumulated into: a pre-loaded `stats0` / `stats_m` of the
+ *     pyramid entries comes back as pre-load + sums); the padding of a ragged batch zero (sdr_separate_ragged).
+ *   - Size: the byte count the matching size query returns suffices exactly.
+ *   - Alignment: 256 bytes for workspaces, `saved` and the staging buffer; 16 bytes for the packed weights and the
+ *     stream state; 8 bytes for the scratch of the three metrics.
+ *   - The whole-model entries (sdr_pack_weights, sdr_forward, sdr_forward_host, sdr_separate, sdr_separate_ragged,
+ *     sdr_stream_reset / _step / _flush, sdr_forward_train, sdr_backward) refuse a null, too small
+ *     (SDR_ERR_WORKSPACE) or misaligned (SDR_ERR_BAD_ARGUMENT) buffer before anything is enqueued.
+ *
  * Errors: integer return codes, 0 = OK, negative = failure (see
  * sdr_error_string).  No C++ exceptions cross the ABI.
  */

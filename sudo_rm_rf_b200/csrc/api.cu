@@ -849,8 +849,8 @@ int sdr_pack_weights(const sdr_config* cfg, const float* const* params, int n_pa
                      void* packed, size_t packed_bytes, sdr_stream stream) {
     const Layout l = make_layout(cfg);
     if (!l.ok) return SDR_ERR_BAD_CONFIG;
-    if (!params || !packed || n_params != (int)l.off.size()) return SDR_ERR_BAD_ARGUMENT;
-    if (packed_bytes < l.total * sizeof(float)) return SDR_ERR_WORKSPACE;
+    if (!params || n_params != (int)l.off.size()) return SDR_ERR_BAD_ARGUMENT;
+    SDR_TRY(check_buffers({{packed, 16, packed_bytes, l.total * sizeof(float)}}));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     float* pk = static_cast<float*>(packed);
     if (cudaMemsetAsync(pk, 0, l.total * sizeof(float), st) != cudaSuccess) return SDR_ERR_CUDA;
@@ -1076,7 +1076,8 @@ int sdr_stream_reset(const sdr_config* cfg, void* state, int B, const int32_t* h
                      sdr_stream stream) {
     const Layout l = make_layout(cfg);
     SDR_TRY(check_stream_config(l));
-    if (!state || B <= 0 || (host_slots_or_null && n < 0)) return SDR_ERR_BAD_ARGUMENT;
+    if (B <= 0 || (host_slots_or_null && n < 0)) return SDR_ERR_BAD_ARGUMENT;
+    SDR_TRY(check_buffers({{state, 16}}));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t slot = stream_state(l).slot * sizeof(float);
     if (!host_slots_or_null)
@@ -1105,7 +1106,8 @@ int sdr_stream_flush(const sdr_config* cfg, void* state, float* tail, int B, int
     const Layout l = make_layout(cfg);
     SDR_TRY(check_stream_config(l));
     if (apply_mixture_consistency && l.A != 1) return SDR_ERR_UNSUPPORTED;
-    if (!state || !tail || B <= 0) return SDR_ERR_BAD_ARGUMENT;
+    if (B <= 0) return SDR_ERR_BAD_ARGUMENT;
+    SDR_TRY(check_buffers({{state, 16}, {tail}}));
     const StreamState ss = stream_state(l);
     return launch_stream_flush(static_cast<const float*>(state), (long long)ss.slot, (long long)ss.carry, tail, B,
                                l.S * l.A, l.hop, apply_mixture_consistency, static_cast<cudaStream_t>(stream));
@@ -1149,9 +1151,10 @@ int sdr_forward_host(const sdr_config* cfg, const void* packed, const float* hos
                      sdr_stream stream) {
     const Layout l = make_layout(cfg);
     SDR_TRY(check_forward_args(l, B, T));
-    if (!host_mixture || !host_out || !dev_io) return SDR_ERR_BAD_ARGUMENT;
     const IoOffsets io = io_offsets(l, B, T);
-    if (dev_io_bytes < io.staging) return SDR_ERR_WORKSPACE;
+    // every buffer before the first copy is enqueued, the forward's workspace included
+    SDR_TRY(check_buffers({{packed, 16}, {host_mixture}, {host_out}, {dev_io, 256, dev_io_bytes, io.staging},
+                           {workspace, 256, workspace_bytes, make_plan(l, B, T).total}}));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t in_bytes = (size_t)B * l.A * T * sizeof(float);
     const size_t out_bytes = (size_t)B * l.S * l.A * T * sizeof(float);
@@ -1384,6 +1387,7 @@ int sdr_separate_ragged(const sdr_config* cfg, const void* packed, const float* 
 
 int sdr_pairwise_neg_sdr(const float* est, const float* target, float* out, int B, int S, int64_t T, int sdr_type,
                          int zero_mean, int take_log, void* scratch, sdr_stream stream) {
+    if (scratch && reinterpret_cast<uintptr_t>(scratch) % 8) return SDR_ERR_BAD_ARGUMENT;
     return launch_pairwise_neg_sdr(est, target, out, B, S, T, sdr_type, zero_mean, take_log, scratch,
                                    static_cast<cudaStream_t>(stream));
 }
