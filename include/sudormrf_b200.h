@@ -29,6 +29,8 @@
  *   - The whole-model entries (sdr_pack_weights, sdr_forward, sdr_forward_host, sdr_separate, sdr_separate_ragged,
  *     sdr_stream_reset / _step / _flush, sdr_forward_train, sdr_backward) refuse a null, too small
  *     (SDR_ERR_WORKSPACE) or misaligned (SDR_ERR_BAD_ARGUMENT) buffer before anything is enqueued.
+ *   - Non-finite inputs are neither refused nor sanitised: a NaN or inf in mixture (slot, utterance) j changes no
+ *     other mixture's output, and makes j's output non-finite where the reference's is (DESIGN.md section 2).
  *
  * Errors: integer return codes, 0 = OK, negative = failure (see
  * sdr_error_string).  No C++ exceptions cross the ABI.

@@ -350,7 +350,7 @@ mask_apply_kernel(const float* __restrict__ mlog, const float* __restrict__ e, f
     if (i >= total) return;
     const long long NL = (long long)N * L;
     const long long b = i / (S * NL), r = i % NL;
-    masked[i] = fmaxf(mlog[i], 0.f) * __ldg(e + b * NL + r);
+    masked[i] = relu(mlog[i]) * __ldg(e + b * NL + r);
 }
 
 // dmlog = dmasked * e * [mlog > 0] (in place over dmasked), de = sum_s dmasked * relu(mlog).

@@ -81,6 +81,14 @@ __device__ __forceinline__ FoldedNorm fold_norm(const NormIn& n, const SampleNor
     return f;
 }
 
+// ReLU as torch.relu: NaN stays NaN (fmaxf(NaN, 0) would be 0 and hide a corrupt mixture).  max.NaN is fmaxf's one
+// instruction with NaN propagation, so every other value, signed zeros included, comes out as fmaxf(v, 0) does.
+__device__ __forceinline__ float relu(float v) {
+    float r;
+    asm("max.NaN.f32 %0, %1, 0f00000000;" : "=f"(r) : "f"(v));
+    return r;
+}
+
 // PReLU in two instructions: max(v, s*v) for s <= 1, min otherwise (the caller decides the slope's side of 1 once)
 __device__ __forceinline__ float prelu2(float v, float s, bool s_le1) {
     const float t = v * s;

@@ -28,7 +28,7 @@ constexpr int kEncNB = 64;
 __global__ void __launch_bounds__(kEncThreads)
 encoder_kernel(const float* __restrict__ wav, const float* __restrict__ weight, const float* __restrict__ bias,
                float* __restrict__ enc, double* __restrict__ stats,
-               int A, long long T, int N, int K, int L, int t_tiles, int pad, int relu) {
+               int A, long long T, int N, int K, int L, int t_tiles, int pad, int relu_out) {
     extern __shared__ __align__(16) float smem[];
     __shared__ double s_red[64];
     const int hop = K / 2;
@@ -77,7 +77,7 @@ encoder_kernel(const float* __restrict__ wav, const float* __restrict__ weight, 
                 const int n = n0 + nn + e;
                 if (n < N) {
                     if (bias) o[e] += __ldg(bias + n);
-                    if (relu) o[e] = fmaxf(o[e], 0.f);
+                    if (relu_out) o[e] = relu(o[e]);
                     enc[((size_t)b * N + n) * L + t] = o[e];
                     rs += o[e]; rq = fmaf(o[e], o[e], rq);
                 }

@@ -176,8 +176,8 @@ pw_gemm_kernel(const PwArgs a) {
                     }
                     if (a.epilogue == 1) {
                         const float4 g = ldg4(grow + l);
-                        o[0] = fmaxf(o[0], 0.f) * g.x; o[1] = fmaxf(o[1], 0.f) * g.y;
-                        o[2] = fmaxf(o[2], 0.f) * g.z; o[3] = fmaxf(o[3], 0.f) * g.w;
+                        o[0] = relu(o[0]) * g.x; o[1] = relu(o[1]) * g.y;
+                        o[2] = relu(o[2]) * g.z; o[3] = relu(o[3]) * g.w;
                     }
                     *reinterpret_cast<float4*>(a.y + row + l) = make_float4(o[0], o[1], o[2], o[3]);
                     st.add_run(o);
@@ -188,7 +188,7 @@ pw_gemm_kernel(const PwArgs a) {
                     if (l + e < a.L) {
                         float v = o[e];
                         if (a.residual) v += a.residual[row + l + e];
-                        if (a.epilogue == 1) v = fmaxf(v, 0.f) * __ldg(grow + l + e);
+                        if (a.epilogue == 1) v = relu(v) * __ldg(grow + l + e);
                         a.y[row + l + e] = v;
                         st.add(v);
                     }
@@ -325,8 +325,8 @@ pw_small_kernel(const PwArgs a, int chunks_per_sample) {
                 }
                 if (a.epilogue == 1) {
                     const float4 g = ldg4(a.gate + ((size_t)sample * a.gate_channels + ((m0 + m) % a.gate_channels)) * a.L + 4 * q);
-                    o[0] = fmaxf(o[0], 0.f) * g.x; o[1] = fmaxf(o[1], 0.f) * g.y;
-                    o[2] = fmaxf(o[2], 0.f) * g.z; o[3] = fmaxf(o[3], 0.f) * g.w;
+                    o[0] = relu(o[0]) * g.x; o[1] = relu(o[1]) * g.y;
+                    o[2] = relu(o[2]) * g.z; o[3] = relu(o[3]) * g.w;
                 }
                 *reinterpret_cast<float4*>(a.y + idx) = make_float4(o[0], o[1], o[2], o[3]);
                 st.add_run(o);

@@ -544,8 +544,8 @@ pw_mma_kernel(const MmaArgs a, const __grid_constant__ CUtensorMap wmap,      //
                         float* e = reinterpret_cast<float*>(box + boff[v] + 1024 * j);
                         float o = acc[i] + bv[v & 1];
                         if (MODE == 1) o += *e;
-                        if (MODE == 2) o = fmaxf(o, 0.f) * *e;
-                        if constexpr (WINDOW) { if (relu_out) o = fmaxf(o, 0.f); }   // the original model's encoder (sudormrf.py:212-218)
+                        if (MODE == 2) o = relu(o) * *e;
+                        if constexpr (WINDOW) { if (relu_out) o = relu(o); }   // the original model's encoder (sudormrf.py:212-218)
                         *e = o;
                         if (STATS && 8 * j + (v & 1) < mrem && 8 * (v >> 1) < prem) { rs_ += o; rq = fmaf(o, o, rq); }
                         if (STATS && (i & 15) == 15) { st.add_run(rs_, rq); rs_ = rq = 0.f; }   // fp32 runs of 16 (StatAcc)
