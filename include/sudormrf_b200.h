@@ -191,6 +191,15 @@ int sdr_mixture_consistency(const float* est, const float* mix, float* out,
                             int B, int S, int64_t T, int weights_type,
                             void* scratch, sdr_stream stream);
 
+/* Backward of sdr_mixture_consistency: grad_out [B,S,T] -> grad_est [B,S,T] and, unless NULL, grad_mix [B,1,T].
+ * 'uniform' (0) needs neither `mix` nor scratch; 'magsq' (1) reads `mix` and needs
+ * sdr_mixture_consistency_backward_scratch_bytes(B, S, T, 1) bytes of 16-byte aligned scratch (0 for 'uniform').
+ * Its reductions are fp64 per-chunk partials added in index order: bitwise reproducible, no synchronisation.    */
+size_t sdr_mixture_consistency_backward_scratch_bytes(int B, int S, int64_t T, int weights_type);
+int sdr_mixture_consistency_backward(const float* est, const float* mix, const float* grad_out, float* grad_est,
+                                     float* grad_mix_or_null, int B, int S, int64_t T, int weights_type,
+                                     void* scratch, sdr_stream stream);
+
 /* ---- per-stage entry points (stage-level parity tests; same kernels the
  *      forward launches).  "Deferred GlobLN": a producer stores its RAW output
  *      and accumulates per-sample (sum, sum of squares) in fp64 into `stats`
@@ -403,6 +412,22 @@ size_t sdr_stabilized_sisdr_scratch_bytes(int B, int n_est, int n_act);
 int sdr_stabilized_sisdr(const float* est, const float* target, float* best, int32_t* perm_index,
                          int B, int est_rows, int n_est, int n_act, int64_t T,
                          int zero_mean, int improvement, double eps, void* scratch, sdr_stream stream);
+
+/* PermInvariantSNRwithZeroRefs.forward (dnn/losses/snr.py:13-142; backward_loss=False, return_individual_results=True),
+ * the training loss of run_fuss_separation.py:257-259: est, target [B,S,T] (already cropped to one length) ->
+ * value[b] = max over itertools.permutations(range(S)) of num_active * sum_k 10 a_k log10(nom_k / den_k + eps),
+ * perm_index[b] = index of that permutation (torch.max's rule: the first NaN, else the first maximum).  Also writes
+ * into `coef` (sdr_snr_zero_refs_coef_bytes(B, S), 8-byte aligned) what sdr_snr_zero_refs_backward reads.  Scratch:
+ * sdr_snr_zero_refs_scratch_bytes(B, S, T), per-chunk fp64 Gram partials added in index order.  1 <= S <= 4.
+ * sdr_snr_zero_refs_backward: grad_value [B] = dL/d value -> grad_est [B,S,T_grad] (rows T_grad >= T apart, zero
+ * past T).  No call synchronises; a forward and a backward are bitwise reproducible.                                */
+size_t sdr_snr_zero_refs_scratch_bytes(int B, int S, int64_t T);
+size_t sdr_snr_zero_refs_coef_bytes(int B, int S);
+int sdr_snr_zero_refs(const float* est, const float* target, float* value, int32_t* perm_index, void* coef,
+                      int B, int S, int64_t T, int zero_mean, double inactivity_threshold, double eps,
+                      void* scratch, sdr_stream stream);
+int sdr_snr_zero_refs_backward(const float* est, const float* target, const void* coef, const float* grad_value,
+                               float* grad_est, int B, int S, int64_t T, int64_t T_grad, sdr_stream stream);
 
 /* ---- training of the improved model (variant 0) ---------------------------
  * sdr_forward_train runs sdr_forward's kernels (same plan, pyramid choice and GEMMs, no mixture consistency) and

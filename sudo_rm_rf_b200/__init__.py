@@ -5,9 +5,11 @@ Mirrors ``sudo_rm_rf.dnn.models.improved_sudormrf`` /
 ``sudo_rm_rf.dnn.models.causal_improved_sudormrf_v3`` /
 ``sudo_rm_rf.dnn.models.sudormrf`` (the original model; its class is also called ``SuDORMRF``, so it is
 exported here as ``OriginalSuDORMRF``) /
-``sudo_rm_rf.dnn.experiments.utils.mixture_consistency`` of etzinis/sudo_rm_rf.
+``sudo_rm_rf.dnn.experiments.utils.mixture_consistency`` of etzinis/sudo_rm_rf, and the FUSS training loss
+``PermInvariantSNRwithZeroRefs`` of ``sudo_rm_rf.dnn.losses.snr`` (module ``snr``).
 """
 from . import improved_sudormrf, groupcomm_sudormrf_v2, causal_improved_sudormrf_v3, sudormrf, mixture_consistency   # noqa: F401
+from . import snr                                                             # noqa: F401
 from .improved_sudormrf import SuDORMRF                                       # noqa: F401
 from .groupcomm_sudormrf_v2 import GroupCommSudoRmRf                          # noqa: F401
 from .causal_improved_sudormrf_v3 import CausalSuDORMRF                       # noqa: F401
@@ -15,5 +17,5 @@ from .sudormrf import SuDORMRF as OriginalSuDORMRF                            # 
 from ._engine import refresh_weights                                          # noqa: F401
 
 __all__ = ["SuDORMRF", "GroupCommSudoRmRf", "CausalSuDORMRF", "OriginalSuDORMRF", "improved_sudormrf",
-           "groupcomm_sudormrf_v2", "causal_improved_sudormrf_v3", "sudormrf", "mixture_consistency",
+           "groupcomm_sudormrf_v2", "causal_improved_sudormrf_v3", "sudormrf", "mixture_consistency", "snr",
            "refresh_weights"]

@@ -73,6 +73,9 @@ _SIGNATURES = {
                                           C.c_int, C.c_void_p]),
     "sdr_mixture_consistency": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                           C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
+    "sdr_mixture_consistency_backward_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int64, C.c_int]),
+    "sdr_mixture_consistency_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                   C.c_int, C.c_int, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
     "sdr_encoder": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                               C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p]),
     "sdr_encoder_mma_packed_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
@@ -134,6 +137,12 @@ _SIGNATURES = {
     "sdr_stabilized_sisdr_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
     "sdr_stabilized_sisdr": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int,
                                        C.c_int64, C.c_int, C.c_int, C.c_double, C.c_void_p, C.c_void_p]),
+    "sdr_snr_zero_refs_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int64]),
+    "sdr_snr_zero_refs_coef_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "sdr_snr_zero_refs": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                    C.c_int64, C.c_int, C.c_double, C.c_double, C.c_void_p, C.c_void_p]),
+    "sdr_snr_zero_refs_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                             C.c_int, C.c_int64, C.c_int64, C.c_void_p]),
     "sdr_train_saved_bytes": (C.c_size_t, [C.POINTER(SdrConfig), C.c_int, C.c_int64]),
     "sdr_backward_workspace_bytes": (C.c_size_t, [C.POINTER(SdrConfig), C.c_int, C.c_int64]),
     "sdr_forward_train": (C.c_int, [C.POINTER(SdrConfig), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64,

@@ -1172,6 +1172,18 @@ int sdr_mixture_consistency(const float* est, const float* mix, float* out, int 
                                       static_cast<cudaStream_t>(stream));
 }
 
+size_t sdr_mixture_consistency_backward_scratch_bytes(int B, int S, int64_t T, int weights_type) {
+    return mc_backward_scratch_bytes(B, S, T, weights_type);
+}
+
+int sdr_mixture_consistency_backward(const float* est, const float* mix, const float* grad_out, float* grad_est,
+                                     float* grad_mix_or_null, int B, int S, int64_t T, int weights_type, void* scratch,
+                                     sdr_stream stream) {
+    if (scratch && reinterpret_cast<uintptr_t>(scratch) % 16) return SDR_ERR_BAD_ARGUMENT;
+    return launch_mixture_consistency_backward(est, mix, grad_out, grad_est, grad_mix_or_null, B, S, T, weights_type,
+                                               scratch, static_cast<cudaStream_t>(stream));
+}
+
 int sdr_encoder(const float* wav, const float* weight, float* enc, double* stats,
                 int B, int A, int64_t T, int N, int K, int L, sdr_stream stream) {
     if (!wav || !weight || !enc || !stats) return SDR_ERR_BAD_ARGUMENT;
@@ -1410,6 +1422,25 @@ int sdr_stabilized_sisdr(const float* est, const float* target, float* best, int
     if (scratch && reinterpret_cast<uintptr_t>(scratch) % 8) return SDR_ERR_BAD_ARGUMENT;
     return launch_stabilized_sisdr(est, target, best, perm_index, B, est_rows, n_est, n_act, T, zero_mean, improvement, eps,
                                    scratch, static_cast<cudaStream_t>(stream));
+}
+
+size_t sdr_snr_zero_refs_scratch_bytes(int B, int S, int64_t T) { return snr_zero_refs_scratch_bytes(B, S, T); }
+size_t sdr_snr_zero_refs_coef_bytes(int B, int S) { return snr_zero_refs_coef_bytes(B, S); }
+
+int sdr_snr_zero_refs(const float* est, const float* target, float* value, int32_t* perm_index, void* coef, int B, int S,
+                      int64_t T, int zero_mean, double inactivity_threshold, double eps, void* scratch,
+                      sdr_stream stream) {
+    if ((scratch && reinterpret_cast<uintptr_t>(scratch) % 8) || (coef && reinterpret_cast<uintptr_t>(coef) % 8))
+        return SDR_ERR_BAD_ARGUMENT;
+    return launch_snr_zero_refs(est, target, value, perm_index, coef, B, S, T, zero_mean, inactivity_threshold, eps,
+                                scratch, static_cast<cudaStream_t>(stream));
+}
+
+int sdr_snr_zero_refs_backward(const float* est, const float* target, const void* coef, const float* grad_value,
+                               float* grad_est, int B, int S, int64_t T, int64_t T_grad, sdr_stream stream) {
+    if (coef && reinterpret_cast<uintptr_t>(coef) % 8) return SDR_ERR_BAD_ARGUMENT;
+    return launch_snr_zero_refs_backward(est, target, coef, grad_value, grad_est, B, S, T, T_grad,
+                                         static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"

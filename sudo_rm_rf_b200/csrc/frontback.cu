@@ -240,4 +240,134 @@ int launch_mixture_consistency(const float* est, const float* mix, float* out, i
     return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
 }
 
+// ---------------------------------------------------------------------------
+// backward of the projection.  With r = mix - sum_s est_s and g = dL/dout:
+//   uniform: d est_k = g_k - (1/S) sum_s g_s,                  d mix = (1/S) sum_s g_s
+//   magsq:   P_s = mean_t est_s^2, Q = sum_s P_s + 1e-9, w_s = P_s / Q, c_s = <g_s, r>,
+//            d est_k = g_k - sum_s w_s g_s + alpha_k est_k,    d mix = sum_s w_s g_s,
+//            alpha_k = (2 / T) (c_k / Q - sum_s c_s P_s / Q^2)
+// magsq: mc_bwd_partials_kernel writes (sum est_s^2, c_s) per (row, chunk) in fp64, mc_bwd_coef_kernel adds the
+// chunks in index order and forms (w_s, alpha_s).  No atomics, so a backward is bitwise reproducible.
+// ---------------------------------------------------------------------------
+static int mc_bwd_chunks(long long T) {
+    long long c = (T + 4095) / 4096;
+    return (int)(c < 1 ? 1 : (c > 64 ? 64 : c));
+}
+
+size_t mc_backward_scratch_bytes(int B, int S, long long T, int weights_type) {
+    if (B <= 0 || S <= 0 || T <= 0 || weights_type != 1) return 0;
+    return sizeof(double) * 2 * (size_t)B * S * (mc_bwd_chunks(T) + 1);
+}
+
+// grid = rows * chunks (rows = B * S); part[row][chunk] = (sum est^2, <g, r>) over the chunk
+__global__ void __launch_bounds__(256)
+mc_bwd_partials_kernel(const float* __restrict__ est, const float* __restrict__ mix, const float* __restrict__ g,
+                       double2* __restrict__ part, int S, long long T, int chunks) {
+    __shared__ double red[2][8];
+    const long long row = blockIdx.x / chunks;
+    const int chunk = (int)(blockIdx.x - row * chunks);
+    const long long b = row / S;
+    const long long per = (T + chunks - 1) / chunks;
+    const long long t0 = (long long)chunk * per;
+    const long long t1 = t0 + per < T ? t0 + per : T;
+    const float* eb = est + (size_t)b * S * T;
+    const float* er = est + (size_t)row * T;
+    const float* gr = g + (size_t)row * T;
+    double p = 0.0, c = 0.0;
+    for (long long t = t0 + threadIdx.x; t < t1; t += 256) {
+        float sum = 0.f;
+        for (int s = 0; s < S; ++s) sum += __ldg(eb + (size_t)s * T + t);
+        const double r = (double)(__ldg(mix + (size_t)b * T + t) - sum);      // the residual as the forward forms it
+        const double e = (double)__ldg(er + t);
+        p = fma(e, e, p);
+        c = fma((double)__ldg(gr + t), r, c);
+    }
+    p = warp_sum_f64(p);
+    c = warp_sum_f64(c);
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    if (lane == 0) { red[0][warp] = p; red[1][warp] = c; }
+    __syncthreads();
+    if (threadIdx.x == 0) {
+        double tp = 0.0, tc = 0.0;
+        for (int w = 0; w < 8; ++w) { tp += red[0][w]; tc += red[1][w]; }
+        part[blockIdx.x] = make_double2(tp, tc);
+    }
+}
+
+// one thread per item: coef[b * S + s] = (w_s, alpha_s)
+__global__ void __launch_bounds__(256)
+mc_bwd_coef_kernel(const double2* __restrict__ part, double2* __restrict__ coef, int B, int S, long long T, int chunks) {
+    for (long long b = blockIdx.x * 256LL + threadIdx.x; b < B; b += (long long)gridDim.x * 256) {
+        double q = 0.0, cp = 0.0;
+        for (int s = 0; s < S; ++s) {
+            double ps = 0.0, cs = 0.0;
+            const double2* pr = part + ((size_t)b * S + s) * chunks;
+            for (int k = 0; k < chunks; ++k) { ps += pr[k].x; cs += pr[k].y; }
+            ps /= (double)T;                                      // P_s = mean_t est_s^2
+            coef[(size_t)b * S + s] = make_double2(ps, cs);
+            q += ps;
+            cp += cs * ps;
+        }
+        q += 1e-9;
+        for (int s = 0; s < S; ++s) {
+            const double2 v = coef[(size_t)b * S + s];
+            coef[(size_t)b * S + s] = make_double2(v.x / q, 2.0 / (double)T * (v.y / q - cp / (q * q)));
+        }
+    }
+}
+
+// grid (T tiles, min(B, 65535)): gsum = sum_s w_s g_s; d est_k = g_k - gsum + alpha_k est_k; d mix = gsum.
+// magsq runs in fp64: a dominant source has w close to 1, and g_k - w_k g_k would cancel in fp32.
+__global__ void __launch_bounds__(256)
+mc_bwd_apply_kernel(const float* __restrict__ est, const float* __restrict__ g, const double2* __restrict__ coef,
+                    float* __restrict__ grad_est, float* __restrict__ grad_mix, int B, int S, long long T) {
+    const long long tau = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+    if (tau >= T) return;
+    for (long long b = blockIdx.y; b < B; b += gridDim.y) {
+        const float* gb = g + (size_t)b * S * T + tau;
+        if (coef) {
+            const double2* cb = coef + (size_t)b * S;
+            double gsum = 0.0;
+            for (int s = 0; s < S; ++s) gsum = fma(cb[s].x, (double)__ldg(gb + (size_t)s * T), gsum);
+            for (int s = 0; s < S; ++s) {
+                const size_t i = ((size_t)b * S + s) * T + tau;
+                grad_est[i] = (float)(fma(cb[s].y, (double)__ldg(est + i), (double)__ldg(g + i) - gsum));
+            }
+            if (grad_mix) grad_mix[(size_t)b * T + tau] = (float)gsum;
+        } else {
+            float gsum = 0.f;
+            for (int s = 0; s < S; ++s) gsum += __ldg(gb + (size_t)s * T);
+            gsum *= 1.0f / S;
+            for (int s = 0; s < S; ++s) {
+                const size_t i = ((size_t)b * S + s) * T + tau;
+                grad_est[i] = __ldg(g + i) - gsum;
+            }
+            if (grad_mix) grad_mix[(size_t)b * T + tau] = gsum;
+        }
+    }
+}
+
+int launch_mixture_consistency_backward(const float* est, const float* mix, const float* grad_out, float* grad_est,
+                                        float* grad_mix, int B, int S, long long T, int weights_type, void* scratch,
+                                        cudaStream_t st) {
+    if (B <= 0 || S <= 0 || T <= 0 || !est || !grad_out || !grad_est) return SDR_ERR_BAD_ARGUMENT;
+    if (weights_type != 0 && weights_type != 1) return SDR_ERR_BAD_ARGUMENT;
+    if ((long long)B * S > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
+    double2* coef = nullptr;
+    if (weights_type == 1) {
+        if (!mix || !scratch) return SDR_ERR_BAD_ARGUMENT;
+        const int chunks = mc_bwd_chunks(T);
+        const long long rows = (long long)B * S, grid = rows * chunks;
+        if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
+        double2* part = static_cast<double2*>(scratch);
+        coef = part + (size_t)grid;
+        mc_bwd_partials_kernel<<<(unsigned)grid, 256, 0, st>>>(est, mix, grad_out, part, S, T, chunks);
+        const long long cb = (B + 255) / 256;
+        mc_bwd_coef_kernel<<<(unsigned)(cb < 4096 ? cb : 4096), 256, 0, st>>>(part, coef, B, S, T, chunks);
+    }
+    dim3 grid((unsigned)((T + 255) / 256), (unsigned)(B < 65535 ? B : 65535));
+    mc_bwd_apply_kernel<<<grid, 256, 0, st>>>(est, grad_out, coef, grad_est, grad_mix, B, S, T);
+    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+}
+
 }  // namespace sdr

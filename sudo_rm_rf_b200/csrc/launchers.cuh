@@ -44,6 +44,10 @@ int launch_overlap_add(const float* frames, const float* mix, const float* bias,
                        int B, int SA, int K, int L, long long T, cudaStream_t st);
 int launch_mixture_consistency(const float* est, const float* mix, float* out, int B, int S,
                                long long T, int weights_type, void* scratch, cudaStream_t st);
+size_t mc_backward_scratch_bytes(int B, int S, long long T, int weights_type);
+int launch_mixture_consistency_backward(const float* est, const float* mix, const float* grad_out, float* grad_est,
+                                        float* grad_mix, int B, int S, long long T, int weights_type, void* scratch,
+                                        cudaStream_t st);
 
 // transform-average-concatenate of the GroupComm blocks (tac.cu)
 int launch_tac(const float* x, const float* const* params, float* o, double* stats,
@@ -92,6 +96,12 @@ size_t pit_sisdr_scratch_bytes(int B, int S);
 int launch_pit_sisdr(const float* est, const float* tgt, const float* mix, float* best, int* perm,
                      int B, int S, long long T, int zero_mean, int improvement, double eps,
                      void* scratch, cudaStream_t st);
+size_t snr_zero_refs_scratch_bytes(int B, int S, long long T);
+size_t snr_zero_refs_coef_bytes(int B, int S);
+int launch_snr_zero_refs(const float* est, const float* tgt, float* value, int* perm, void* coef, int B, int S,
+                         long long T, int zero_mean, double threshold, double eps, void* scratch, cudaStream_t st);
+int launch_snr_zero_refs_backward(const float* est, const float* tgt, const void* coef, const float* grad_value,
+                                  float* grad, int B, int S, long long T, long long Tg, cudaStream_t st);
 
 // tensor-core path (pointwise_mma.cu)
 bool pointwise_mma_eligible(int M, int K);

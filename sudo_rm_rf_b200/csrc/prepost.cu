@@ -357,7 +357,9 @@ template <int SE, int SA> struct StabLayout {
     static constexpr int ET = V, EE = ET + SE * SA, TT = EE + SE, N = TT + SA * SA;
 };
 
-template <int SE, int SA>
+// kOrdered: each CTA writes its chunk's sums to acc[blockIdx.x] (layout [b][chunk][N]) instead of adding them to
+// acc[b] atomically, and the consumer adds the chunks in index order, so the result is bitwise reproducible.
+template <int SE, int SA, bool kOrdered = false>
 __global__ void __launch_bounds__(256)
 stab_gram_kernel(const float* __restrict__ est, const float* __restrict__ tgt, double* __restrict__ acc,
                  long long T, int chunks, int rows) {
@@ -408,7 +410,8 @@ stab_gram_kernel(const float* __restrict__ est, const float* __restrict__ tgt, d
     for (int i = threadIdx.x; i < P::N; i += 256) {
         double v = 0.0;
         for (int w = 0; w < 8; ++w) v += red[w][i];
-        atomicAdd(acc + (size_t)b * P::N + i, v);
+        if (kOrdered) acc[(size_t)blockIdx.x * P::N + i] = v;
+        else atomicAdd(acc + (size_t)b * P::N + i, v);
     }
 }
 
@@ -542,6 +545,185 @@ int launch_stabilized_sisdr(const float* est, const float* tgt, float* best, int
     SDR_STAB(4, 1) SDR_STAB(4, 2) SDR_STAB(4, 3) SDR_STAB(4, 4)
 #undef SDR_STAB
     return SDR_ERR_UNSUPPORTED;
+}
+
+// ---------------------------------------------------------------------------
+// PermInvariantSNRwithZeroRefs (dnn/losses/snr.py:13-142), the training loss of run_fuss_separation.py:257-259.
+// The ordered StabLayout<S, S> Gram holds every term: with means removed under zero_mean,
+//     tt_k = ||t_k||^2,  mixture power mp = sum_jk <t_j, t_k> = ||sum_j t_j||^2,
+//     active_k = 10 log10(tt_k / (mp + eps)) >= threshold,  stab_k = 1e-3 (active_k ? tt_k : mp),
+//     nom_k = tt_k + eps,  den_ik = ||e_i - t_k||^2 + stab_k + eps = ee_i - 2 <e_i, t_k> + tt_k + stab_k + eps,
+//     score(p) = num_active * sum_k 10 a_k log10(nom_k / den_{p[k] k} + eps)                    (:86-109)
+// best over itertools.permutations(range(S)) by torch.max's rule.  For the backward, coef[b] holds per estimate row
+// i = p*[k]: dscore/d den * 2 = -20 a_k num_active / ln10 * nom_k / (den^2 (nom_k / den + eps)), the target k it
+// is matched to, and the row means of estimates and targets (zero under !zero_mean):  [coef S][k S][me S][mt S].
+// ---------------------------------------------------------------------------
+static int snr_chunks(long long T) {
+    long long c = (T + 4095) / 4096;
+    return (int)(c < 1 ? 1 : (c > 64 ? 64 : c));
+}
+
+size_t snr_zero_refs_scratch_bytes(int B, int S, long long T) {
+    if (B <= 0 || S < 1 || S > 4 || T <= 0) return 0;
+    return sizeof(double) * (size_t)B * snr_chunks(T) * (2 * S + 2 * S * S + S);
+}
+
+size_t snr_zero_refs_coef_bytes(int B, int S) {
+    if (B <= 0 || S < 1 || S > 4) return 0;
+    return sizeof(double) * (size_t)B * 4 * S;
+}
+
+template <int S>
+__global__ void __launch_bounds__(256)
+snr_zero_refs_finalize_kernel(const double* __restrict__ part, int chunks, float* __restrict__ value,
+                              int* __restrict__ perm, double* __restrict__ coef, int B, long long T, int zero_mean,
+                              double threshold, double eps) {
+    using P = StabLayout<S, S>;
+    const double n = (double)T;
+    for (long long b = blockIdx.x * 256LL + threadIdx.x; b < B; b += (long long)gridDim.x * 256) {
+        double a[P::N];
+#pragma unroll
+        for (int i = 0; i < P::N; ++i) a[i] = 0.0;
+        for (int c = 0; c < chunks; ++c) {
+            const double* pc = part + ((size_t)b * chunks + c) * P::N;
+#pragma unroll
+            for (int i = 0; i < P::N; ++i) a[i] += pc[i];
+        }
+        double me[S], mt[S];
+#pragma unroll
+        for (int i = 0; i < S; ++i) { me[i] = zero_mean ? a[i] / n : 0.0; mt[i] = zero_mean ? a[S + i] / n : 0.0; }
+        double tt[S], mp = 0.0;
+#pragma unroll
+        for (int j = 0; j < S; ++j)
+#pragma unroll
+            for (int k = 0; k < S; ++k) {
+                const double v = a[P::TT + j * S + k] - n * mt[j] * mt[k];
+                mp += v;
+                if (j == k) tt[j] = clamp_energy(v);
+            }
+        mp = clamp_energy(mp);
+        double act[S], nom[S], stab[S];
+        int num_active = 0;
+#pragma unroll
+        for (int k = 0; k < S; ++k) {
+            const bool on = 10.0 * log10(tt[k] / (mp + eps)) >= threshold;        // NaN: inactive, as Tensor.ge
+            act[k] = on ? 1.0 : 0.0;
+            num_active += on ? 1 : 0;
+            nom[k] = tt[k] + eps;
+            stab[k] = 1e-3 * (on ? tt[k] : mp);
+        }
+        double den[S][S], sc[S][S];
+#pragma unroll
+        for (int i = 0; i < S; ++i) {
+            const double ee = clamp_energy(a[P::EE + i] - n * me[i] * me[i]);
+#pragma unroll
+            for (int k = 0; k < S; ++k) {
+                double err = ee - 2.0 * (a[P::ET + i * S + k] - n * me[i] * mt[k]) + tt[k];
+                if (isinf(ee) && isfinite(tt[k])) err = ee;              // ||e - t||^2 with an inf in e: inf - inf above
+                err = clamp_energy(err);
+                den[i][k] = err + stab[k] + eps;
+                sc[i][k] = 10.0 * act[k] * log10(nom[k] / den[i][k] + eps);
+            }
+        }
+        double bestv = 0.0;
+        int besti = 0, idx = 0;
+        int p[S], bp[S];
+#pragma unroll
+        for (int i = 0; i < S; ++i) { p[i] = i; bp[i] = i; }
+        while (true) {
+            double m = 0.0;
+            for (int k = 0; k < S; ++k) m += sc[p[k]][k];
+            m *= (double)num_active;
+            if (takes_max(m, bestv, idx)) {
+                bestv = m; besti = idx;
+                for (int k = 0; k < S; ++k) bp[k] = p[k];
+            }
+            ++idx;
+            int k = S - 2;                                               // next lexicographic permutation
+            while (k >= 0 && p[k] > p[k + 1]) --k;
+            if (k < 0) break;
+            int l = S - 1;
+            while (p[l] < p[k]) --l;
+            int tmp = p[k]; p[k] = p[l]; p[l] = tmp;
+            for (int lo = k + 1, hi = S - 1; lo < hi; ++lo, --hi) { tmp = p[lo]; p[lo] = p[hi]; p[hi] = tmp; }
+        }
+        value[b] = (float)bestv;
+        perm[b] = besti;
+        double* cb = coef + (size_t)b * 4 * S;
+        for (int k = 0; k < S; ++k) {
+            double d = 0.0, nk = 0.0, ak = 0.0;
+#pragma unroll
+            for (int i = 0; i < S; ++i) if (bp[k] == i) d = den[i][k];
+#pragma unroll
+            for (int j = 0; j < S; ++j) if (j == k) { nk = nom[j]; ak = act[j]; }
+            const int i = bp[k];
+            cb[i] = -20.0 * ak * (double)num_active / 2.302585092994045684 * nk / (d * d * (nk / d + eps));
+            cb[S + i] = (double)k;
+        }
+#pragma unroll
+        for (int i = 0; i < S; ++i) { cb[2 * S + i] = me[i]; cb[3 * S + i] = mt[i]; }
+    }
+}
+
+// grad[b][i][t] = g[b] coef_i ((e_i - me_i) - (t_k - mt_k)) for t < T, 0 for T <= t < Tg (rows Tg apart); est and tgt
+// rows are T apart.  grid (time tiles, min(B S, 65535)).
+__global__ void __launch_bounds__(256)
+snr_zero_refs_backward_kernel(const float* __restrict__ est, const float* __restrict__ tgt,
+                              const double* __restrict__ coef, const float* __restrict__ grad_value,
+                              float* __restrict__ grad, int B, int S, long long T, long long Tg) {
+    const long long rows = (long long)B * S;
+    for (long long row = blockIdx.y; row < rows; row += gridDim.y) {
+        const long long b = row / S;
+        const int i = (int)(row - b * S);
+        const double* cb = coef + (size_t)b * 4 * S;
+        const int k = (int)cb[S + i];
+        const double c = cb[i] * (double)__ldg(grad_value + b);
+        const double mi = cb[2 * S + i], mk = cb[3 * S + k];
+        const float* er = est + (size_t)row * T;
+        const float* tr = tgt + ((size_t)b * S + k) * T;
+        float* gr = grad + (size_t)row * Tg;
+        for (long long t = (long long)blockIdx.x * 256 + threadIdx.x; t < Tg; t += (long long)gridDim.x * 256)
+            gr[t] = t < T ? (float)(c * (((double)__ldg(er + t) - mi) - ((double)__ldg(tr + t) - mk))) : 0.f;
+    }
+}
+
+template <int S>
+static int launch_snr_s(const float* est, const float* tgt, float* value, int* perm, double* coef, int B, long long T,
+                        int zero_mean, double threshold, double eps, double* part, cudaStream_t st) {
+    const int chunks = snr_chunks(T);
+    const long long grid = (long long)B * chunks;
+    if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
+    stab_gram_kernel<S, S, true><<<(unsigned)grid, 256, 0, st>>>(est, tgt, part, T, chunks, S);
+    const long long fb = (B + 255) / 256;
+    snr_zero_refs_finalize_kernel<S><<<(unsigned)(fb < 4096 ? fb : 4096), 256, 0, st>>>(
+        part, chunks, value, perm, coef, B, T, zero_mean, threshold, eps);
+    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+}
+
+int launch_snr_zero_refs(const float* est, const float* tgt, float* value, int* perm, void* coef, int B, int S,
+                         long long T, int zero_mean, double threshold, double eps, void* scratch, cudaStream_t st) {
+    if (!est || !tgt || !value || !perm || !coef || !scratch || B <= 0 || T <= 0) return SDR_ERR_BAD_ARGUMENT;
+    double* part = static_cast<double*>(scratch);
+    double* cf = static_cast<double*>(coef);
+    switch (S) {
+        case 1: return launch_snr_s<1>(est, tgt, value, perm, cf, B, T, zero_mean, threshold, eps, part, st);
+        case 2: return launch_snr_s<2>(est, tgt, value, perm, cf, B, T, zero_mean, threshold, eps, part, st);
+        case 3: return launch_snr_s<3>(est, tgt, value, perm, cf, B, T, zero_mean, threshold, eps, part, st);
+        case 4: return launch_snr_s<4>(est, tgt, value, perm, cf, B, T, zero_mean, threshold, eps, part, st);
+        default: return SDR_ERR_UNSUPPORTED;     // S! permutations are enumerated per item; 4 sources = 24
+    }
+}
+
+int launch_snr_zero_refs_backward(const float* est, const float* tgt, const void* coef, const float* grad_value,
+                                  float* grad, int B, int S, long long T, long long Tg, cudaStream_t st) {
+    if (!est || !tgt || !coef || !grad_value || !grad || B <= 0 || T <= 0 || Tg < T) return SDR_ERR_BAD_ARGUMENT;
+    if (S < 1 || S > 4) return SDR_ERR_UNSUPPORTED;
+    const long long rows = (long long)B * S;
+    long long gx = (Tg + 256 * 4 - 1) / (256 * 4);
+    if (gx > 4096) gx = 4096;
+    snr_zero_refs_backward_kernel<<<dim3((unsigned)gx, (unsigned)(rows < 65535 ? rows : 65535)), 256, 0, st>>>(
+        est, tgt, static_cast<const double*>(coef), grad_value, grad, B, S, T, Tg);
+    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
 }
 
 size_t pit_sisdr_scratch_bytes(int B, int S) {
