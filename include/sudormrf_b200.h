@@ -394,6 +394,19 @@ int sdr_separate_ragged(const sdr_config* cfg, const void* packed, const float* 
 int sdr_pairwise_neg_sdr(const float* est, const float* target, float* out, int B, int S, int64_t T, int sdr_type,
                          int zero_mean, int take_log, void* scratch, sdr_stream stream);
 
+/* The same [B, S, S] output for training (PairwiseNegSDR under autograd, the loss of run_improved_sudormrf.py:64-66
+ * through PITLossWrapper): also writes into `coef` (sdr_pairwise_neg_sdr_coef_bytes(B, S), 8-byte aligned) the fp64
+ * coefficients of d out / d est that sdr_pairwise_neg_sdr_backward reads.  Scratch:
+ * sdr_pairwise_neg_sdr_train_scratch_bytes(B, S, T), per-chunk fp64 Gram partials added in index order.  1 <= S <= 4.
+ * sdr_pairwise_neg_sdr_backward: grad_out [B,S,S] = dL/d out -> grad_est [B,S,T].  No call synchronises; a forward
+ * and a backward are bitwise reproducible.                                                                          */
+size_t sdr_pairwise_neg_sdr_train_scratch_bytes(int B, int S, int64_t T);
+size_t sdr_pairwise_neg_sdr_coef_bytes(int B, int S);
+int sdr_pairwise_neg_sdr_train(const float* est, const float* target, float* out, void* coef, int B, int S,
+                               int64_t T, int sdr_type, int zero_mean, int take_log, void* scratch, sdr_stream stream);
+int sdr_pairwise_neg_sdr_backward(const float* est, const float* target, const void* coef, const float* grad_out,
+                                  float* grad_est, int B, int S, int64_t T, sdr_stream stream);
+
 size_t sdr_pit_sisdr_scratch_bytes(int B, int S);
 int sdr_pit_sisdr(const float* est, const float* target, const float* mixture_or_null,
                   float* best, int32_t* perm_index, int B, int S, int64_t T,

@@ -131,6 +131,12 @@ _SIGNATURES = {
                                       C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
     "sdr_pairwise_neg_sdr": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int,
                                        C.c_int, C.c_void_p, C.c_void_p]),
+    "sdr_pairwise_neg_sdr_train_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int64]),
+    "sdr_pairwise_neg_sdr_coef_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "sdr_pairwise_neg_sdr_train": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                             C.c_int64, C.c_int, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "sdr_pairwise_neg_sdr_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                                C.c_int, C.c_int64, C.c_void_p]),
     "sdr_pit_sisdr_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "sdr_pit_sisdr": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                 C.c_int, C.c_int64, C.c_int, C.c_int, C.c_double, C.c_void_p, C.c_void_p]),

@@ -1404,6 +1404,24 @@ int sdr_pairwise_neg_sdr(const float* est, const float* target, float* out, int 
                                    static_cast<cudaStream_t>(stream));
 }
 
+size_t sdr_pairwise_neg_sdr_train_scratch_bytes(int B, int S, int64_t T) { return pairwise_train_scratch_bytes(B, S, T); }
+size_t sdr_pairwise_neg_sdr_coef_bytes(int B, int S) { return pairwise_coef_bytes(B, S); }
+
+int sdr_pairwise_neg_sdr_train(const float* est, const float* target, float* out, void* coef, int B, int S, int64_t T,
+                               int sdr_type, int zero_mean, int take_log, void* scratch, sdr_stream stream) {
+    if ((scratch && reinterpret_cast<uintptr_t>(scratch) % 8) || (coef && reinterpret_cast<uintptr_t>(coef) % 8))
+        return SDR_ERR_BAD_ARGUMENT;
+    return launch_pairwise_neg_sdr_train(est, target, out, coef, B, S, T, sdr_type, zero_mean, take_log, scratch,
+                                         static_cast<cudaStream_t>(stream));
+}
+
+int sdr_pairwise_neg_sdr_backward(const float* est, const float* target, const void* coef, const float* grad_out,
+                                  float* grad_est, int B, int S, int64_t T, sdr_stream stream) {
+    if (coef && reinterpret_cast<uintptr_t>(coef) % 8) return SDR_ERR_BAD_ARGUMENT;
+    return launch_pairwise_neg_sdr_backward(est, target, coef, grad_out, grad_est, B, S, T,
+                                            static_cast<cudaStream_t>(stream));
+}
+
 size_t sdr_pit_sisdr_scratch_bytes(int B, int S) { return pit_sisdr_scratch_bytes(B, S); }
 
 int sdr_pit_sisdr(const float* est, const float* target, const float* mixture_or_null, float* best, int32_t* perm_index,

@@ -88,6 +88,13 @@ int launch_normalize_rows(const float* wav, const float2* mean_std, float* out, 
                           const long long* lengths, cudaStream_t st);
 int launch_pairwise_neg_sdr(const float* est, const float* tgt, float* out, int B, int S, long long T, int sdr_type,
                             int zero_mean, int take_log, void* scratch, cudaStream_t st);
+size_t pairwise_train_scratch_bytes(int B, int S, long long T);
+size_t pairwise_coef_bytes(int B, int S);
+int launch_pairwise_neg_sdr_train(const float* est, const float* tgt, float* out, void* coef, int B, int S,
+                                  long long T, int sdr_type, int zero_mean, int take_log, void* scratch,
+                                  cudaStream_t st);
+int launch_pairwise_neg_sdr_backward(const float* est, const float* tgt, const void* coef, const float* grad_out,
+                                     float* grad, int B, int S, long long T, cudaStream_t st);
 size_t stabilized_sisdr_scratch_bytes(int B, int n_est, int n_act);
 int launch_stabilized_sisdr(const float* est, const float* tgt, float* best, int* perm, int B, int rows, int n_est,
                             int n_act, long long T, int zero_mean, int improvement, double eps, void* scratch,

@@ -283,6 +283,17 @@ static int launch_pit_s(const float* est, const float* tgt, const float* mix, fl
 //     snr:    |proj|^2 = tt,      |noise|^2 = ee - 2 d + tt
 //     sdr = |proj|^2 / (|noise|^2 + 1e-8);  take_log: 10 log10(sdr + 1e-8)
 // ---------------------------------------------------------------------------
+struct PairTerms { double c, proj, q; };        // c, |proj|^2 and |noise|^2 + 1e-8 of one (estimate, target) pair
+
+__device__ __forceinline__ PairTerms pairwise_terms(double d, double tt, double ee, int sdr_type) {
+    const double c = d / (tt + 1e-8);
+    const double proj = sdr_type == 0 ? tt : c * c * tt;                                // 0 snr, 1 sisdr, 2 sdsdr
+    double noise = sdr_type == 1 ? ee - 2.0 * c * d + c * c * tt : ee - 2.0 * d + tt;
+    if (sdr_type != 1 && isinf(ee) && isfinite(tt)) noise = ee;            // |e - t|^2 with an inf in e: inf - inf above
+    if (noise < 0.0) noise = 0.0;
+    return {c, proj, noise + 1e-8};
+}
+
 template <int S>
 __global__ void __launch_bounds__(256)
 pairwise_finalize_kernel(const double* __restrict__ acc, float* __restrict__ out, int B, long long T,
@@ -300,13 +311,8 @@ pairwise_finalize_kernel(const double* __restrict__ acc, float* __restrict__ out
 #pragma unroll
             for (int j = 0; j < S; ++j) {
                 const double tt = clamp_energy(a[P::TT + j] - n * mt[j] * mt[j]);
-                const double d = a[P::ET + i * S + j] - n * me[i] * mt[j];
-                const double c = d / (tt + 1e-8);
-                const double proj = sdr_type == 0 ? tt : c * c * tt;                       // 0 snr, 1 sisdr, 2 sdsdr
-                double noise = sdr_type == 1 ? ee - 2.0 * c * d + c * c * tt : ee - 2.0 * d + tt;
-                if (sdr_type != 1 && isinf(ee) && isfinite(tt)) noise = ee;    // |e - t|^2 with an inf in e: inf - inf above
-                if (noise < 0.0) noise = 0.0;
-                double v = proj / (noise + 1e-8);
+                const PairTerms p = pairwise_terms(a[P::ET + i * S + j] - n * me[i] * mt[j], tt, ee, sdr_type);
+                double v = p.proj / p.q;
                 if (take_log) v = 10.0 * log10(v + 1e-8);
                 out[((size_t)b * S + i) * S + j] = (float)(-v);
             }
@@ -723,6 +729,162 @@ int launch_snr_zero_refs_backward(const float* est, const float* tgt, const void
     if (gx > 4096) gx = 4096;
     snr_zero_refs_backward_kernel<<<dim3((unsigned)gx, (unsigned)(rows < 65535 ? rows : 65535)), 256, 0, st>>>(
         est, tgt, static_cast<const double*>(coef), grad_value, grad, B, S, T, Tg);
+    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+}
+
+// ---------------------------------------------------------------------------
+// PairwiseNegSDR under autograd, the training loss of run_improved_sudormrf.py:64-66 through PITLossWrapper.  The
+// forward runs the ordered StabLayout<S, S> Gram (the diagonal of its TT is the <t_j, t_j> above) and
+// pairwise_train_finalize_kernel, which writes out[b, i, j] by pairwise_finalize_kernel's arithmetic and, per entry,
+// the three coefficients of
+//     d out[b, i, j] / d e_i = alpha_ij (e'_i - k_ij t'_j) + beta_ij t'_j
+// where e' = e - mu_e and t' = t - mu_t (the row means under zero_mean, else 0; the mean removal's own derivative
+// subtracts the mean of this gradient, which is zero) and e'_i - k_ij t'_j is the noise vector: k = c for sisdr, 1 for
+// sdsdr and snr.  With d, tt, ee, c and E = tt + 1e-8 as above, P = |proj|^2, Q = |noise|^2 + 1e-8 and r = P / Q:
+//     dr/de = (dP/de - r dQ/de) / Q,  dQ/de = 2 noise + q t',  dP/de = p t'
+//     sisdr:  p = 2 c tt / E,  q = -2 c 1e-8 / E   (<noise, t'> = c 1e-8; c depends on e)
+//     sdsdr:  p = 2 c tt / E,  q = 0
+//     snr:    p = 0,           q = 0
+// out = -r, or -10 log10(r + 1e-8) with take_log, so alpha = s 2 r / Q and beta = -s (p - r q) / Q with s = 1, or
+// 10 / (ln 10 (r + 1e-8)).  Written on the noise vector, the two terms do not cancel each other: with an estimate
+// equal to its target, alpha is ~1e16 and the noise exactly 0.  coef[b] = [alpha, k, beta per (i, j)][mu_e S][mu_t S],
+// fp64.  pairwise_backward_kernel is one elementwise pass:
+//     grad_e_i[t] = sum_j g_ij (alpha_ij (e'_i[t] - k_ij t'_j[t]) + beta_ij t'_j[t]).
+// ---------------------------------------------------------------------------
+size_t pairwise_train_scratch_bytes(int B, int S, long long T) { return snr_zero_refs_scratch_bytes(B, S, T); }
+
+size_t pairwise_coef_bytes(int B, int S) {
+    if (B <= 0 || S < 1 || S > 4) return 0;
+    return sizeof(double) * (size_t)B * (3 * S * S + 2 * S);
+}
+
+template <int S>
+__global__ void __launch_bounds__(256)
+pairwise_train_finalize_kernel(const double* __restrict__ part, int chunks, float* __restrict__ out,
+                               double* __restrict__ coef, int B, long long T, int sdr_type, int zero_mean,
+                               int take_log) {
+    using P = StabLayout<S, S>;
+    const double n = (double)T;
+    for (long long b = blockIdx.x * 256LL + threadIdx.x; b < B; b += (long long)gridDim.x * 256) {
+        double a[P::N];
+#pragma unroll
+        for (int i = 0; i < P::N; ++i) a[i] = 0.0;
+        for (int c = 0; c < chunks; ++c) {
+            const double* pc = part + ((size_t)b * chunks + c) * P::N;
+#pragma unroll
+            for (int i = 0; i < P::N; ++i) a[i] += pc[i];
+        }
+        double me[S], mt[S];
+#pragma unroll
+        for (int i = 0; i < S; ++i) { me[i] = zero_mean ? a[i] / n : 0.0; mt[i] = zero_mean ? a[S + i] / n : 0.0; }
+        double* cb = coef + (size_t)b * (3 * S * S + 2 * S);
+#pragma unroll
+        for (int i = 0; i < S; ++i) {
+            const double ee = clamp_energy(a[P::EE + i] - n * me[i] * me[i]);
+#pragma unroll
+            for (int j = 0; j < S; ++j) {
+                const double tt = clamp_energy(a[P::TT + j * S + j] - n * mt[j] * mt[j]);
+                const PairTerms p = pairwise_terms(a[P::ET + i * S + j] - n * me[i] * mt[j], tt, ee, sdr_type);
+                const double r = p.proj / p.q;
+                const double E = tt + 1e-8;
+                const double dp = sdr_type == 0 ? 0.0 : 2.0 * p.c * tt / E;
+                const double dq = sdr_type == 1 ? -2.0 * p.c * 1e-8 / E : 0.0;
+                const double s = take_log ? 10.0 / (2.302585092994045684 * (r + 1e-8)) : 1.0;
+                out[((size_t)b * S + i) * S + j] = (float)(-(take_log ? 10.0 * log10(r + 1e-8) : r));
+                double* cij = cb + 3 * (i * S + j);
+                cij[0] = s * 2.0 * r / p.q;
+                cij[1] = sdr_type == 1 ? p.c : 1.0;
+                cij[2] = -s * (dp - r * dq) / p.q;
+            }
+        }
+#pragma unroll
+        for (int i = 0; i < S; ++i) { cb[3 * S * S + i] = me[i]; cb[3 * S * S + S + i] = mt[i]; }
+    }
+}
+
+// grid (time tiles, min(B S, 65535)); est, tgt and grad rows are T apart
+template <int S>
+__global__ void __launch_bounds__(256)
+pairwise_backward_kernel(const float* __restrict__ est, const float* __restrict__ tgt, const double* __restrict__ coef,
+                         const float* __restrict__ grad_out, float* __restrict__ grad, int B, long long T) {
+    const long long rows = (long long)B * S;
+    for (long long row = blockIdx.y; row < rows; row += gridDim.y) {
+        const long long b = row / S;
+        const int i = (int)(row - b * S);
+        const double* cb = coef + (size_t)b * (3 * S * S + 2 * S);
+        const float* go = grad_out + (size_t)row * S;
+        double al[S], k[S], be[S], mt[S];
+#pragma unroll
+        for (int j = 0; j < S; ++j) {
+            const double g = (double)__ldg(go + j);
+            const double* cij = cb + 3 * (i * S + j);
+            al[j] = g * cij[0];
+            k[j] = cij[1];
+            be[j] = g * cij[2];
+            mt[j] = cb[3 * S * S + S + j];
+        }
+        const double mi = cb[3 * S * S + i];
+        const float* er = est + (size_t)row * T;
+        const float* tb = tgt + (size_t)b * S * T;
+        float* gr = grad + (size_t)row * T;
+        for (long long t = (long long)blockIdx.x * 256 + threadIdx.x; t < T; t += (long long)gridDim.x * 256) {
+            const double e = (double)__ldg(er + t) - mi;
+            double v = 0.0;
+#pragma unroll
+            for (int j = 0; j < S; ++j) {
+                const double tj = (double)__ldg(tb + (size_t)j * T + t) - mt[j];
+                v = fma(al[j], fma(-k[j], tj, e), v);                   // the noise e' - k t', then its weight
+                v = fma(be[j], tj, v);
+            }
+            gr[t] = (float)v;
+        }
+    }
+}
+
+template <int S>
+static int launch_pairwise_train_s(const float* est, const float* tgt, float* out, double* coef, int B, long long T,
+                                   int sdr_type, int zero_mean, int take_log, double* part, cudaStream_t st) {
+    const int chunks = snr_chunks(T);
+    const long long grid = (long long)B * chunks;
+    if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
+    stab_gram_kernel<S, S, true><<<(unsigned)grid, 256, 0, st>>>(est, tgt, part, T, chunks, S);
+    const long long fb = (B + 255) / 256;
+    pairwise_train_finalize_kernel<S><<<(unsigned)(fb < 4096 ? fb : 4096), 256, 0, st>>>(
+        part, chunks, out, coef, B, T, sdr_type, zero_mean, take_log);
+    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+}
+
+int launch_pairwise_neg_sdr_train(const float* est, const float* tgt, float* out, void* coef, int B, int S,
+                                  long long T, int sdr_type, int zero_mean, int take_log, void* scratch,
+                                  cudaStream_t st) {
+    if (!est || !tgt || !out || !coef || !scratch || B <= 0 || T <= 0 || sdr_type < 0 || sdr_type > 2)
+        return SDR_ERR_BAD_ARGUMENT;
+    double* part = static_cast<double*>(scratch);
+    double* cf = static_cast<double*>(coef);
+    switch (S) {
+        case 1: return launch_pairwise_train_s<1>(est, tgt, out, cf, B, T, sdr_type, zero_mean, take_log, part, st);
+        case 2: return launch_pairwise_train_s<2>(est, tgt, out, cf, B, T, sdr_type, zero_mean, take_log, part, st);
+        case 3: return launch_pairwise_train_s<3>(est, tgt, out, cf, B, T, sdr_type, zero_mean, take_log, part, st);
+        case 4: return launch_pairwise_train_s<4>(est, tgt, out, cf, B, T, sdr_type, zero_mean, take_log, part, st);
+        default: return SDR_ERR_UNSUPPORTED;
+    }
+}
+
+int launch_pairwise_neg_sdr_backward(const float* est, const float* tgt, const void* coef, const float* grad_out,
+                                     float* grad, int B, int S, long long T, cudaStream_t st) {
+    if (!est || !tgt || !coef || !grad_out || !grad || B <= 0 || T <= 0) return SDR_ERR_BAD_ARGUMENT;
+    const long long rows = (long long)B * S;
+    long long gx = (T + 256 * 4 - 1) / (256 * 4);
+    if (gx > 4096) gx = 4096;
+    const dim3 grid((unsigned)gx, (unsigned)(rows < 65535 ? rows : 65535));
+    const double* cf = static_cast<const double*>(coef);
+    switch (S) {
+        case 1: pairwise_backward_kernel<1><<<grid, 256, 0, st>>>(est, tgt, cf, grad_out, grad, B, T); break;
+        case 2: pairwise_backward_kernel<2><<<grid, 256, 0, st>>>(est, tgt, cf, grad_out, grad, B, T); break;
+        case 3: pairwise_backward_kernel<3><<<grid, 256, 0, st>>>(est, tgt, cf, grad_out, grad, B, T); break;
+        case 4: pairwise_backward_kernel<4><<<grid, 256, 0, st>>>(est, tgt, cf, grad_out, grad, B, T); break;
+        default: return SDR_ERR_UNSUPPORTED;
+    }
     return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
 }
 

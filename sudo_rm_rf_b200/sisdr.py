@@ -1,19 +1,42 @@
-"""H100-native mirror of the evaluation metrics in ``sudo_rm_rf/dnn/losses/sisdr.py``.
+"""H100-native mirror of the losses and metrics in ``sudo_rm_rf/dnn/losses/sisdr.py``.
 
 ``PermInvariantSISDR`` keeps the reference's constructor arguments, ``forward``
 signature and return conventions (sisdr.py:66-194), but it is the *metric* the
 validation loops compute right after ``model(...)``
 (run_improved_sudormrf.py:82-85,201-205): inference only, no autograd.  The
 arithmetic (one fp64 Gram pass over the batch + a permutation search per item)
-runs in ``libsudormrf_b200.so`` (``sdr_pit_sisdr``).
+runs in ``libsudormrf_b200.so`` (``sdr_pit_sisdr``).  ``StabilizedPermInvSISDRMetric``
+is metric-only as well.
+
+``PITLossWrapper(PairwiseNegSDR("sisdr"), pit_from="pw_mtx")`` is the training loss of
+run_improved_sudormrf.py:64-66.  ``PairwiseNegSDR`` is differentiable with respect to
+``est_targets``: one fp64 Gram pass (``sdr_pairwise_neg_sdr_train``) in the forward, one
+elementwise kernel (``sdr_pairwise_neg_sdr_backward``) in the backward, neither of which
+synchronises with the host, so a training step that uses the loss can be captured in a CUDA graph.
 """
 import ctypes as C
 import itertools
 
 import torch
 import torch.nn as nn
+from torch.autograd.function import once_differentiable
 
 from . import _native as N
+
+_PERMS = {}
+
+
+def _perms(n_src, device):
+    """itertools.permutations(range(n_src)) as a long tensor on `device`, made once per (n_src, device): building it
+    on every call is a pageable host-to-device copy, which a CUDA graph cannot capture."""
+    key = (n_src, device)
+    if key not in _PERMS:
+        _PERMS[key] = torch.tensor(list(itertools.permutations(range(n_src))), dtype=torch.long, device=device)
+    return _PERMS[key]
+
+
+def _stream(dev):
+    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
 
 
 class PermInvariantSISDR(nn.Module):
@@ -158,10 +181,50 @@ class StabilizedPermInvSISDRMetric(nn.Module):
         return result
 
 
+class _PairwiseNegSDR(torch.autograd.Function):
+    """The [B, S, S] pairwise losses as a function of est_targets (fp32 contiguous copies est, tgt are passed along)."""
+
+    @staticmethod
+    def forward(ctx, est_targets, est, tgt, sdr_type, zero_mean, take_log):
+        lib = N.lib()
+        B, S, T = est.shape
+        dev = est.device
+        with torch.cuda.device(dev):
+            scratch = torch.empty(lib.sdr_pairwise_neg_sdr_train_scratch_bytes(B, S, T), dtype=torch.uint8, device=dev)
+            coef = torch.empty(lib.sdr_pairwise_neg_sdr_coef_bytes(B, S), dtype=torch.uint8, device=dev)
+            out = torch.empty((B, S, S), dtype=torch.float32, device=dev)
+            N.check(lib.sdr_pairwise_neg_sdr_train(
+                C.c_void_p(est.data_ptr()), C.c_void_p(tgt.data_ptr()), C.c_void_p(out.data_ptr()),
+                C.c_void_p(coef.data_ptr()), B, S, T, sdr_type, 1 if zero_mean else 0, 1 if take_log else 0,
+                C.c_void_p(scratch.data_ptr()), _stream(dev)), "sdr_pairwise_neg_sdr_train")
+        ctx.save_for_backward(est, tgt, coef)
+        ctx.dtype = est_targets.dtype
+        return out
+
+    @staticmethod
+    @once_differentiable
+    def backward(ctx, grad_out):
+        est, tgt, coef = ctx.saved_tensors
+        B, S, T = est.shape
+        dev = est.device
+        g = grad_out.to(torch.float32).contiguous()
+        with torch.cuda.device(dev):
+            grad = torch.empty((B, S, T), dtype=torch.float32, device=dev)
+            N.check(N.lib().sdr_pairwise_neg_sdr_backward(
+                C.c_void_p(est.data_ptr()), C.c_void_p(tgt.data_ptr()), C.c_void_p(coef.data_ptr()),
+                C.c_void_p(g.data_ptr()), C.c_void_p(grad.data_ptr()), B, S, T, _stream(dev)),
+                "sdr_pairwise_neg_sdr_backward")
+        return grad.to(ctx.dtype), None, None, None, None, None
+
+
 class PairwiseNegSDR(nn.Module):
     """Pairwise negative SNR / SI-SDR / SD-SDR on a batch (sisdr.py:372-457): same constructor and ``forward``
-    as the reference class; returns ``[batch, n_src, n_src]`` with ``[b, i, j] = -sdr(estimate i, target j)``.
-    Evaluation only (no autograd); the arithmetic is one fp64 Gram pass in ``libsudormrf_b200.so``."""
+    as the reference class; returns ``[batch, n_src, n_src]`` fp32 with ``[b, i, j] = -sdr(estimate i, target j)``.
+    The arithmetic is one fp64 Gram pass in ``libsudormrf_b200.so``.  With grad mode on and ``est_targets`` requiring
+    grad the result is differentiable with respect to ``est_targets`` (the gradient comes back in its dtype; fp16,
+    bf16 and fp64 inputs are computed on in fp32), its Gram sums are added in a fixed order, and a forward and a
+    backward are bitwise reproducible.  Gradients with respect to ``targets`` are not computed: ``targets`` that
+    require grad are refused.  1..4 sources."""
     _TYPES = {"snr": 0, "sisdr": 1, "sdsdr": 2}
 
     def __init__(self, sdr_type, zero_mean=True, take_log=True):
@@ -175,14 +238,19 @@ class PairwiseNegSDR(nn.Module):
         assert targets.size() == est_targets.size()
         if est_targets.dim() != 3:
             raise RuntimeError("expected est_targets and targets of shape [batch, n_src, time]")
+        if not 1 <= est_targets.shape[1] <= 4:
+            raise N.NativeError("sdr_pairwise_neg_sdr supports 1..4 sources")
+        if torch.is_grad_enabled() and targets.requires_grad:
+            raise RuntimeError("PairwiseNegSDR computes the gradient with respect to est_targets only: "
+                               "pass targets that do not require grad (e.g. `targets.detach()`)")
         if not (est_targets.is_cuda and targets.is_cuda):
             raise RuntimeError("sudo_rm_rf_b200.sisdr runs on CUDA tensors only (no CPU path)")
-        if torch.is_grad_enabled() and (est_targets.requires_grad or targets.requires_grad):
-            raise RuntimeError("sudo_rm_rf_b200.sisdr is the evaluation metric only (no autograd): "
-                               "wrap the call in torch.no_grad()")
         dev = est_targets.device
         est = est_targets.detach().to(torch.float32).contiguous()
         tgt = targets.detach().to(device=dev, dtype=torch.float32).contiguous()
+        if torch.is_grad_enabled() and est_targets.requires_grad:
+            return _PairwiseNegSDR.apply(est_targets, est, tgt, self._TYPES[self.sdr_type], self.zero_mean,
+                                         self.take_log)
         B, S, T = est.shape
         lib = N.lib()
         nbytes = lib.sdr_pit_sisdr_scratch_bytes(B, S)
@@ -203,8 +271,10 @@ class PITLossWrapper(nn.Module):
     """Permutation-invariant wrapper (sisdr.py:197-369): same constructor, ``forward`` signature and return
     conventions as the reference class.  The pairwise matrix comes from ``loss_func`` (``PairwiseNegSDR`` above for
     ``pit_from='pw_mtx'``); the search over the n_src! permutations works on that ``[batch, n_src, n_src]`` tensor
-    with a handful of tiny torch ops, exactly as the reference does (host logic, not a hot path).  The reference's copy
-    calls ``best_perm_from_perm_avg_loss`` / ``reorder_source`` without defining them (``pit_from='perm_avg'`` and
+    with a handful of tiny torch ops, exactly as the reference does (host logic, not a hot path), and gradients flow
+    through them to whatever ``loss_func`` differentiates.  The permutation table is made once per (n_src, device),
+    so a training step through ``PairwiseNegSDR`` and ``pit_from='pw_mtx'`` can be captured in a CUDA graph.  The
+    reference's copy calls ``best_perm_from_perm_avg_loss`` / ``reorder_source`` without defining them (``pit_from='perm_avg'`` and
     ``return_est=True`` raise there); the two helpers below follow the asteroid definitions the file was copied from."""
 
     def __init__(self, loss_func, pit_from="pw_mtx", perm_reduce=None):
@@ -250,7 +320,7 @@ class PITLossWrapper(nn.Module):
     @staticmethod
     def find_best_perm(pair_wise_losses, n_src, perm_reduce=None, **kwargs):
         pwl = pair_wise_losses.transpose(-1, -2)             # dim 1: sources, dim 2: estimates
-        perms = pwl.new_tensor(list(itertools.permutations(range(n_src))), dtype=torch.long)
+        perms = _perms(n_src, pwl.device)
         idx = torch.unsqueeze(perms, 2)
         if perm_reduce is None:
             one_hot = pwl.new_zeros((*perms.size(), n_src)).scatter_(2, idx, 1)
@@ -272,6 +342,6 @@ class PITLossWrapper(nn.Module):
 
     @staticmethod
     def reorder_source(source, n_src, min_loss_idx):
-        perms = source.new_tensor(list(itertools.permutations(range(n_src))), dtype=torch.long)
+        perms = _perms(n_src, source.device)
         min_loss_perm = torch.index_select(perms, dim=0, index=min_loss_idx)
         return torch.stack([torch.index_select(s, 0, b) for s, b in zip(source, min_loss_perm)])
