@@ -188,10 +188,6 @@ class NativeModuleMixin:
         return state
 
 
-def _stream_ptr(device) -> C.c_void_p:
-    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
-
-
 def _enter_stream(st: _DeviceState, device):
     """One workspace per (model, device): a call arriving on a different stream than the previous one waits
     for it (the scratch buffers are shared), and tells the caching allocator about the second stream."""
@@ -345,7 +341,7 @@ def packed_weights(model, cfg: N.SdrConfig, device) -> torch.Tensor:
     packed = torch.empty(nbytes, dtype=torch.uint8, device=device)
     ptrs = (C.c_void_p * n)(*[C.c_void_p(t.data_ptr()) for t in flat])
     N.check(lib.sdr_pack_weights(C.byref(cfg), ptrs, n, C.c_void_p(packed.data_ptr()), nbytes,
-                                 _stream_ptr(device)), "sdr_pack_weights")
+                                 N.stream(device)), "sdr_pack_weights")
     st.sig, st.storages = sig, (weight_storages(tensors) if sig is not None else None)
     _replace(st, "packed", packed)
     _hand_out(st, "packed")
@@ -491,7 +487,7 @@ def forward_host(model, host_wav: torch.Tensor, host_out: torch.Tensor = None,
                                          B, T, mc,
                                          C.c_void_p(st.staging.data_ptr()), st.staging.numel(),
                                          C.c_void_p(st.workspace.data_ptr()), st.workspace.numel(),
-                                         _stream_ptr(device)), "sdr_forward_host")
+                                         N.stream(device)), "sdr_forward_host")
 
         graphable = use_graph and host_wav.is_pinned() and host_out.is_pinned() \
             and not torch.cuda.is_current_stream_capturing()

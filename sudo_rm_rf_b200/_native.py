@@ -11,6 +11,8 @@ import os
 import subprocess
 import threading
 
+import torch
+
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get("SDR_B200_LIB") or os.path.join(_HERE, "libsudormrf_b200.so")   # env override: A/B-testing kernel builds
 CSRC = os.path.join(_HERE, "csrc")
@@ -208,6 +210,11 @@ def lib():
                 raise NativeError("libsudormrf_b200.so ABI version mismatch; rebuild")
             _lib = handle
     return _lib
+
+
+def stream(device) -> C.c_void_p:
+    """The current CUDA stream of `device`, as the ``cudaStream_t`` argument every entry takes."""
+    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
 
 
 def check(code: int, what: str = "") -> None:

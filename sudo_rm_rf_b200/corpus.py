@@ -111,7 +111,7 @@ def separate_corpus(model, wavs: Iterable[torch.Tensor], max_batch: int = 32,
                 C.c_void_p(lengths.data_ptr()), C.c_void_p(out.data_ptr()), B, Tp,
                 1 if mixture_consistency else 0, 1 if rescale else 0,
                 C.c_void_p(st.workspace.data_ptr()), st.workspace.numel(),
-                _engine._stream_ptr(device)), "sdr_separate_ragged")
+                N.stream(device)), "sdr_separate_ragged")
             for r, i in enumerate(idx):
                 results[i] = out[r, :, :wavs[i].shape[0]].clone()
     return results
@@ -265,7 +265,7 @@ class CorpusSeparator:
                         side.wait_stream(self._s_cmp)
                         graph = torch.cuda.CUDAGraph()
                         with torch.cuda.graph(graph, stream=side):
-                            enqueue(C.c_void_p(torch.cuda.current_stream(dev).cuda_stream))
+                            enqueue(N.stream(dev))
                         self._s_cmp.wait_stream(side)
                         self.graphs[key] = graph
                         graph.replay()

@@ -147,4 +147,19 @@ __device__ __forceinline__ float4 ldg4(const float* p) {
 
 inline int ceil_div(int a, int b) { return (a + b - 1) / b; }
 
+// CTAs per item of the fp64 reductions over time that end in per-(item, chunk) sums (the SDR Gram pass, the mixture
+// consistency backward): one per 4096 samples, 1..64.
+inline int gram_chunks(long long T) {
+    const long long c = (T + 4095) / 4096;
+    return (int)(c < 1 ? 1 : (c > 64 ? 64 : c));
+}
+
+// Grid of an elementwise pass of 256-thread CTAs over `rows` rows of T samples: x tiles of 1024 samples (1..4096) and
+// y rows (at most 65535); the kernel strides over the time and the rows beyond the grid.
+inline dim3 row_tiled_grid(long long rows, long long T) {
+    long long gx = (T + 256 * 4 - 1) / (256 * 4);
+    gx = gx < 1 ? 1 : (gx > 4096 ? 4096 : gx);
+    return dim3((unsigned)gx, (unsigned)(rows < 65535 ? rows : 65535));
+}
+
 }  // namespace sdr

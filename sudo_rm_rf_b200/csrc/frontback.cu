@@ -249,14 +249,9 @@ int launch_mixture_consistency(const float* est, const float* mix, float* out, i
 // magsq: mc_bwd_partials_kernel writes (sum est_s^2, c_s) per (row, chunk) in fp64, mc_bwd_coef_kernel adds the
 // chunks in index order and forms (w_s, alpha_s).  No atomics, so a backward is bitwise reproducible.
 // ---------------------------------------------------------------------------
-static int mc_bwd_chunks(long long T) {
-    long long c = (T + 4095) / 4096;
-    return (int)(c < 1 ? 1 : (c > 64 ? 64 : c));
-}
-
 size_t mc_backward_scratch_bytes(int B, int S, long long T, int weights_type) {
     if (B <= 0 || S <= 0 || T <= 0 || weights_type != 1) return 0;
-    return sizeof(double) * 2 * (size_t)B * S * (mc_bwd_chunks(T) + 1);
+    return sizeof(double) * 2 * (size_t)B * S * (gram_chunks(T) + 1);
 }
 
 // grid = rows * chunks (rows = B * S); part[row][chunk] = (sum est^2, <g, r>) over the chunk
@@ -356,7 +351,7 @@ int launch_mixture_consistency_backward(const float* est, const float* mix, cons
     double2* coef = nullptr;
     if (weights_type == 1) {
         if (!mix || !scratch) return SDR_ERR_BAD_ARGUMENT;
-        const int chunks = mc_bwd_chunks(T);
+        const int chunks = gram_chunks(T);
         const long long rows = (long long)B * S, grid = rows * chunks;
         if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
         double2* part = static_cast<double2*>(scratch);

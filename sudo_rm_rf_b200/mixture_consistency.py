@@ -17,8 +17,7 @@ def _project(est, mix, magsq):
         N.check(lib.sdr_mixture_consistency(
             C.c_void_p(est.data_ptr()), C.c_void_p(mix.data_ptr()), C.c_void_p(out.data_ptr()),
             B, S, T, 1 if magsq else 0,
-            C.c_void_p(scratch.data_ptr() if scratch is not None else 0),
-            C.c_void_p(torch.cuda.current_stream(est.device).cuda_stream)),
+            C.c_void_p(scratch.data_ptr() if scratch is not None else 0), N.stream(est.device)),
             "sdr_mixture_consistency")
     return out
 
@@ -54,7 +53,7 @@ class _Consistency(torch.autograd.Function):
                 C.c_void_p(est.data_ptr()), C.c_void_p(mix.data_ptr()), C.c_void_p(g.data_ptr()),
                 C.c_void_p(grad_est.data_ptr()), C.c_void_p(grad_mix.data_ptr() if want_mix else 0),
                 B, S, T, 1 if ctx.magsq else 0, C.c_void_p(scratch.data_ptr() if scratch is not None else 0),
-                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "sdr_mixture_consistency_backward")
+                N.stream(dev)), "sdr_mixture_consistency_backward")
         return (grad_est.to(ctx.dtypes[0]) if ctx.needs_input_grad[0] else None,
                 grad_mix.to(ctx.dtypes[1]) if want_mix else None, None)
 

@@ -35,8 +35,15 @@ def _perms(n_src, device):
     return _PERMS[key]
 
 
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+def _result(metric, best, perm, return_best_permutation):
+    """The reference metrics' return conventions: the best score per item (``return_individual_results``) or its batch
+    mean, negated with ``backward_loss``, and optionally the best permutations ``[B, n_sources]``."""
+    result = best if metric.return_individual_results else best.mean()
+    if metric.backward_loss:
+        result = -result
+    if return_best_permutation:
+        return result, metric.permutations_tensor.to(best.device)[perm.long()]
+    return result
 
 
 class PermInvariantSISDR(nn.Module):
@@ -97,14 +104,8 @@ class PermInvariantSISDR(nn.Module):
                 C.c_void_p(mix.data_ptr() if (mix is not None and self.improvement) else 0),
                 C.c_void_p(best.data_ptr()), C.c_void_p(perm.data_ptr()), B, S, T,
                 1 if self.perform_zero_mean else 0, 1 if self.improvement else 0, float(eps),
-                C.c_void_p(scratch.data_ptr()),
-                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "sdr_pit_sisdr")
-        result = best if self.return_individual_results else best.mean()
-        if self.backward_loss:
-            result = -result
-        if return_best_permutation:
-            return result, self.permutations_tensor.to(dev)[perm.long()]
-        return result
+                C.c_void_p(scratch.data_ptr()), N.stream(dev)), "sdr_pit_sisdr")
+        return _result(self, best, perm, return_best_permutation)
 
 
 class StabilizedPermInvSISDRMetric(nn.Module):
@@ -171,14 +172,8 @@ class StabilizedPermInvSISDRMetric(nn.Module):
                 C.c_void_p(est.data_ptr()), C.c_void_p(tgt.data_ptr()), C.c_void_p(best.data_ptr()),
                 C.c_void_p(perm.data_ptr()), B, rows, self.n_estimated_sources, self.n_actual_sources, T,
                 1 if self.perform_zero_mean else 0, 1 if self.improvement else 0, float(eps),
-                C.c_void_p(scratch.data_ptr()),
-                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "sdr_stabilized_sisdr")
-        result = best if self.return_individual_results else best.mean()
-        if self.backward_loss:
-            result = -result
-        if return_best_permutation:
-            return result, self.permutations_tensor.to(dev)[perm.long()]
-        return result
+                C.c_void_p(scratch.data_ptr()), N.stream(dev)), "sdr_stabilized_sisdr")
+        return _result(self, best, perm, return_best_permutation)
 
 
 class _PairwiseNegSDR(torch.autograd.Function):
@@ -196,7 +191,7 @@ class _PairwiseNegSDR(torch.autograd.Function):
             N.check(lib.sdr_pairwise_neg_sdr_train(
                 C.c_void_p(est.data_ptr()), C.c_void_p(tgt.data_ptr()), C.c_void_p(out.data_ptr()),
                 C.c_void_p(coef.data_ptr()), B, S, T, sdr_type, 1 if zero_mean else 0, 1 if take_log else 0,
-                C.c_void_p(scratch.data_ptr()), _stream(dev)), "sdr_pairwise_neg_sdr_train")
+                C.c_void_p(scratch.data_ptr()), N.stream(dev)), "sdr_pairwise_neg_sdr_train")
         ctx.save_for_backward(est, tgt, coef)
         ctx.dtype = est_targets.dtype
         return out
@@ -212,7 +207,7 @@ class _PairwiseNegSDR(torch.autograd.Function):
             grad = torch.empty((B, S, T), dtype=torch.float32, device=dev)
             N.check(N.lib().sdr_pairwise_neg_sdr_backward(
                 C.c_void_p(est.data_ptr()), C.c_void_p(tgt.data_ptr()), C.c_void_p(coef.data_ptr()),
-                C.c_void_p(g.data_ptr()), C.c_void_p(grad.data_ptr()), B, S, T, _stream(dev)),
+                C.c_void_p(g.data_ptr()), C.c_void_p(grad.data_ptr()), B, S, T, N.stream(dev)),
                 "sdr_pairwise_neg_sdr_backward")
         return grad.to(ctx.dtype), None, None, None, None, None
 
@@ -262,8 +257,7 @@ class PairwiseNegSDR(nn.Module):
             N.check(lib.sdr_pairwise_neg_sdr(
                 C.c_void_p(est.data_ptr()), C.c_void_p(tgt.data_ptr()), C.c_void_p(out.data_ptr()), B, S, T,
                 self._TYPES[self.sdr_type], 1 if self.zero_mean else 0, 1 if self.take_log else 0,
-                C.c_void_p(scratch.data_ptr()),
-                C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)), "sdr_pairwise_neg_sdr")
+                C.c_void_p(scratch.data_ptr()), N.stream(dev)), "sdr_pairwise_neg_sdr")
         return out
 
 

@@ -14,10 +14,7 @@ import torch.nn as nn
 from torch.autograd.function import once_differentiable
 
 from . import _native as N
-
-
-def _stream(dev):
-    return C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
+from .sisdr import _result
 
 
 def _forward(est, tgt, zero_mean, threshold, eps):
@@ -33,7 +30,7 @@ def _forward(est, tgt, zero_mean, threshold, eps):
         N.check(lib.sdr_snr_zero_refs(
             C.c_void_p(est.data_ptr()), C.c_void_p(tgt.data_ptr()), C.c_void_p(best.data_ptr()),
             C.c_void_p(perm.data_ptr()), C.c_void_p(coef.data_ptr()), B, S, T, 1 if zero_mean else 0,
-            float(threshold), float(eps), C.c_void_p(scratch.data_ptr()), _stream(dev)), "sdr_snr_zero_refs")
+            float(threshold), float(eps), C.c_void_p(scratch.data_ptr()), N.stream(dev)), "sdr_snr_zero_refs")
     return best, perm, coef
 
 
@@ -59,7 +56,7 @@ class _SNRZeroRefs(torch.autograd.Function):
             grad = torch.empty(ctx.shape, dtype=torch.float32, device=dev)
             N.check(N.lib().sdr_snr_zero_refs_backward(
                 C.c_void_p(est.data_ptr()), C.c_void_p(tgt.data_ptr()), C.c_void_p(coef.data_ptr()),
-                C.c_void_p(g.data_ptr()), C.c_void_p(grad.data_ptr()), B, S, T, ctx.shape[-1], _stream(dev)),
+                C.c_void_p(g.data_ptr()), C.c_void_p(grad.data_ptr()), B, S, T, ctx.shape[-1], N.stream(dev)),
                 "sdr_snr_zero_refs_backward")
         return grad.to(ctx.dtype), None, None, None, None, None
 
@@ -107,9 +104,4 @@ class PermInvariantSNRwithZeroRefs(nn.Module):
                                             self.inactivity_threshold, eps)
         else:
             best, perm, _ = _forward(est, tgt, self.perform_zero_mean, self.inactivity_threshold, eps)
-        result = best if self.return_individual_results else best.mean()
-        if self.backward_loss:
-            result = -result
-        if return_best_permutation:
-            return result, self.permutations_tensor.to(dev)[perm.long()]
-        return result
+        return _result(self, best, perm, return_best_permutation)

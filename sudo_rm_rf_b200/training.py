@@ -92,7 +92,7 @@ class _NativeTrain(torch.autograd.Function):
             N.check(lib.sdr_backward(C.byref(cfg), C.c_void_p(ctx.packed.data_ptr()), C.c_void_p(wav.data_ptr()),
                                      C.c_void_p(ctx.saved.data_ptr()), C.c_void_p(g.data_ptr()),
                                      C.c_void_p(flat.data_ptr()), B, T, C.c_void_p(ws.data_ptr()), ws.numel(),
-                                     _engine._stream_ptr(device)), "sdr_backward")
+                                     N.stream(device)), "sdr_backward")
         ctx.saved = None
         grads = []
         for p, part in zip(params, flat.split(numel)):
