@@ -442,6 +442,29 @@ int sdr_snr_zero_refs(const float* est, const float* target, float* value, int32
 int sdr_snr_zero_refs_backward(const float* est, const float* target, const void* coef, const float* grad_value,
                                float* grad_est, int B, int S, int64_t T, int64_t T_grad, sdr_stream stream);
 
+/* BSS-eval v3 source criteria (mir_eval.separation.bss_eval_sources, the sdr / sir / sar of asteroid's get_metrics):
+ * reference, estimate [B,S,T] -> sdr, sir, sar [B,S] fp64 in dB and perm [B,S] (perm[b][j] = the estimate scored
+ * against reference j).  Per item, with F-tap distortion filters (mir_eval: 512), in R^(T+F-1), P_j e the projection
+ * of e onto the F delays of reference j and P_all e onto the delays of every reference:
+ *     SDR = 10 log10(|P_j e|^2 / |e - P_j e|^2),  SIR = 10 log10(|P_j e|^2 / |P_all e - P_j e|^2),
+ *     SAR = 10 log10(|P_all e|^2 / |e - P_all e|^2)     (a zero denominator: +inf).
+ * compute_permutation != 0 scores every (estimate, reference) pair and takes the assignment with the largest mean SIR
+ * (the first in itertools.permutations order); else estimate j is scored against reference j.  An item with an
+ * all-zero reference or estimate row gets NaN in every output and perm -1.  perm_or_null may be NULL.  The outputs
+ * are bitwise reproducible; no call synchronises.  1 <= S <= 4, 1 <= F <= 512, T >= (S - 1) F + 1 (no more delayed
+ * references than dimensions: for S = 1 any T >= 1); scratch:
+ * sdr_bss_eval_scratch_bytes(B, S, T, F) (0: unsupported arguments), 8-byte aligned.
+ * sdr_bss_eval_mixture also scores mixture [B,1,T] as the estimate of every reference into mix_sdr, mix_sir,
+ * mix_sar [B,S] (NaN where the mixture or a reference is silent), from the same reference correlations and solves. */
+size_t sdr_bss_eval_scratch_bytes(int B, int S, int64_t T, int F);
+int sdr_bss_eval(const float* reference, const float* estimate, double* sdr, double* sir, double* sar,
+                 int32_t* perm_or_null, int B, int S, int64_t T, int F, int compute_permutation, void* scratch,
+                 sdr_stream stream);
+int sdr_bss_eval_mixture(const float* reference, const float* estimate, const float* mixture, double* sdr,
+                         double* sir, double* sar, int32_t* perm_or_null, double* mix_sdr, double* mix_sir,
+                         double* mix_sar, int B, int S, int64_t T, int F, int compute_permutation, void* scratch,
+                         sdr_stream stream);
+
 /* ---- training of the improved model (variant 0) ---------------------------
  * sdr_forward_train runs sdr_forward's kernels (same plan, pyramid choice and GEMMs, no mixture consistency) and
  * also copies into `saved` what the backward recomputes from: the statistics slots, the raw encoder output and every

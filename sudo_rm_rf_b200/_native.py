@@ -151,6 +151,12 @@ _SIGNATURES = {
                                     C.c_int64, C.c_int, C.c_double, C.c_double, C.c_void_p, C.c_void_p]),
     "sdr_snr_zero_refs_backward": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                              C.c_int, C.c_int64, C.c_int64, C.c_void_p]),
+    "sdr_bss_eval_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int64, C.c_int]),
+    "sdr_bss_eval": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                               C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "sdr_bss_eval_mixture": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64,
+                                       C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
     "sdr_train_saved_bytes": (C.c_size_t, [C.POINTER(SdrConfig), C.c_int, C.c_int64]),
     "sdr_backward_workspace_bytes": (C.c_size_t, [C.POINTER(SdrConfig), C.c_int, C.c_int64]),
     "sdr_forward_train": (C.c_int, [C.POINTER(SdrConfig), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64,

@@ -1461,5 +1461,24 @@ int sdr_snr_zero_refs_backward(const float* est, const float* target, const void
                                          static_cast<cudaStream_t>(stream));
 }
 
+size_t sdr_bss_eval_scratch_bytes(int B, int S, int64_t T, int F) { return bss_eval_scratch_bytes(B, S, T, F); }
+
+int sdr_bss_eval(const float* reference, const float* estimate, double* sdr, double* sir, double* sar,
+                 int32_t* perm_or_null, int B, int S, int64_t T, int F, int compute_permutation, void* scratch,
+                 sdr_stream stream) {
+    if (scratch && reinterpret_cast<uintptr_t>(scratch) % 8) return SDR_ERR_BAD_ARGUMENT;
+    return launch_bss_eval(reference, estimate, nullptr, sdr, sir, sar, perm_or_null, nullptr, nullptr, nullptr, B, S,
+                           T, F, compute_permutation, scratch, static_cast<cudaStream_t>(stream));
+}
+
+int sdr_bss_eval_mixture(const float* reference, const float* estimate, const float* mixture, double* sdr,
+                         double* sir, double* sar, int32_t* perm_or_null, double* mix_sdr, double* mix_sir,
+                         double* mix_sar, int B, int S, int64_t T, int F, int compute_permutation, void* scratch,
+                         sdr_stream stream) {
+    if (!mixture || (scratch && reinterpret_cast<uintptr_t>(scratch) % 8)) return SDR_ERR_BAD_ARGUMENT;
+    return launch_bss_eval(reference, estimate, mixture, sdr, sir, sar, perm_or_null, mix_sdr, mix_sir, mix_sar, B, S,
+                           T, F, compute_permutation, scratch, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"
 #pragma GCC visibility pop

@@ -110,6 +110,11 @@ int launch_snr_zero_refs(const float* est, const float* tgt, float* value, int* 
 int launch_snr_zero_refs_backward(const float* est, const float* tgt, const void* coef, const float* grad_value,
                                   float* grad, int B, int S, long long T, long long Tg, cudaStream_t st);
 
+size_t bss_eval_scratch_bytes(int B, int S, long long T, int F);
+int launch_bss_eval(const float* ref, const float* est, const float* mix, double* sdr, double* sir, double* sar,
+                    int* perm, double* msdr, double* msir, double* msar, int B, int S, long long T, int F,
+                    int compute_permutation, void* scratch, cudaStream_t st);
+
 // tensor-core path (pointwise_mma.cu)
 bool pointwise_mma_eligible(int M, int K);
 size_t pointwise_mma_packed_bytes(int M, int K);
