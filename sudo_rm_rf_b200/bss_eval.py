@@ -30,7 +30,9 @@ def bss_eval_sources(reference_sources, estimated_sources, compute_permutation=T
     Returns ``(sdr, sir, sar, perm)`` on the device: fp64 ``[..., S]`` in dB and int64 ``[..., S]`` where ``perm[j]``
     is the estimate scored against reference j.  With ``compute_permutation`` that is the assignment with the largest
     mean SIR (the first in ``itertools.permutations`` order), otherwise estimate j.  Where mir_eval raises on an
-    all-zero reference or estimate row, that item gets NaN in every output and ``perm = -1``.
+    all-zero reference or estimate row, and where such a row holds a NaN or an infinity, that item gets NaN in every
+    output and ``perm = -1``.  So does an item whose references are too close to dependent for the normal equations
+    (several band-limited references with deep stop bands), where the solve would give no projection.
 
     With ``mixture`` (``[T]``, ``[1, T]``, ``[B, T]`` or ``[B, 1, T]``) the call also returns the mixture scored as the
     estimate of every reference and the improvements, as a dict ``{"sdr", "sir", "sar"}`` of the mixture's scores and

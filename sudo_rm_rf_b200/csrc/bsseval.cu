@@ -34,6 +34,29 @@ __host__ __device__ inline int bss_corr_chunks(long long T) {
 }
 __host__ __device__ inline int bss_energy_chunks(long long T, int F) { return bss_corr_chunks(T + F - 1); }
 
+// A row can be scored when its energy is positive and finite: an all-zero row, or one holding a NaN or an infinity
+// (whose energy is NaN or inf), gives its item NaN and perm -1 rather than a NaN score and an arbitrary assignment.
+__device__ __forceinline__ bool bss_scorable(double energy) { return energy > 0.0 && energy < (double)INFINITY; }
+
+// An orthogonal projection p of e leaves a residual orthogonal to it: |p|^2 + |e - p|^2 = |e|^2.  The recursion on the
+// normal equations loses that when the delays are nearly, but not numerically, dependent (several band-limited
+// references with deep stop bands: G's condition number near 1 / eps, and the prediction-error matrices lose
+// definiteness).  Its scores are then those of no projection, so the item is reported NaN.  Where the recursion
+// holds, the defect stays below 1e-3 of |e|^2 (a few 1e-4 next to dropped delays, rounding elsewhere).
+constexpr double kBssProjectionDefect = 1e-2;
+__device__ __forceinline__ bool bss_is_projection(double p2, double r2, double e2) {
+    return fabs(p2 + r2 - e2) <= kBssProjectionDefect * e2;
+}
+
+// Estimate row e's energies (bss_energy_kernel's layout) come from projections: the joint one and every own one.
+template <int S>
+__device__ __forceinline__ bool bss_projections_hold(const double (&en)[3 * S + 3]) {
+    bool ok = bss_is_projection(en[3 * S], en[3 * S + 1], en[3 * S + 2]);
+#pragma unroll
+    for (int j = 0; j < S; ++j) ok = ok && bss_is_projection(en[j], en[S + j], en[3 * S + 2]);
+    return ok;
+}
+
 // Scratch carve-up, sized for S estimates plus the mixture whether or not it is given.  Doubles:
 //   part  [B][chunks][S][2S+1][F]   correlation partials (rows: S references, then the NE estimate rows)
 //   rj    [B][F][S][S]              the joint system's normalised blocks
@@ -356,7 +379,7 @@ bss_solve_kernel(const double* __restrict__ part, int chunks, double* __restrict
     __syncthreads();
     bool silent = false;
 #pragma unroll
-    for (int i = 0; i < S; ++i) silent = silent || !(sE[i] > 0.0);
+    for (int i = 0; i < S; ++i) silent = silent || !bss_scorable(sE[i]);
     if (sys == 0 && threadIdx.x < S) eref[(size_t)b * S + threadIdx.x] = sE[threadIdx.x];
     double* out = (sys == 0 ? cj : ct) + (size_t)b * (S + 1) * S * F;
     if (silent) {                                       // the item's outputs are NaN; its filters are set to zero
@@ -485,10 +508,11 @@ bss_final_kernel(const double* __restrict__ epart, const double* __restrict__ er
         }
         bool silent_ref = false;
 #pragma unroll
-        for (int i = 0; i < S; ++i) silent_ref = silent_ref || !(eref[(size_t)b * S + i] > 0.0);
+        for (int i = 0; i < S; ++i) silent_ref = silent_ref || !bss_scorable(eref[(size_t)b * S + i]);
         bool silent = silent_ref;
 #pragma unroll
-        for (int e = 0; e < S; ++e) silent = silent || !(en[e][3 * S + 2] > 0.0);
+        for (int e = 0; e < S; ++e)
+            silent = silent || !bss_scorable(en[e][3 * S + 2]) || !bss_projections_hold<S>(en[e]);
         double d[NE][S], i_[NE][S], a[NE][S];
 #pragma unroll
         for (int e = 0; e < NE; ++e)
@@ -522,7 +546,7 @@ bss_final_kernel(const double* __restrict__ epart, const double* __restrict__ er
             sar[o] = silent ? nan : aj;
             if (perm) perm[o] = silent ? -1 : p[j];
             if constexpr (NE > S) {
-                const bool ms = silent_ref || !(en[S][3 * S + 2] > 0.0);
+                const bool ms = silent_ref || !bss_scorable(en[S][3 * S + 2]) || !bss_projections_hold<S>(en[S]);
                 msdr[o] = ms ? nan : d[S][j];
                 msir[o] = ms ? nan : i_[S][j];
                 msar[o] = ms ? nan : a[S][j];

@@ -1,12 +1,14 @@
-"""BSS-eval without a GPU: the two fp64 oracle formulations agree, the C-ABI symbols bind, the scratch query refuses
+"""BSS-eval without a GPU: the fp64 oracle formulations agree (the span oracle with the others where the recursion
+drops nothing; on windowed tones the normal equations fail), the C-ABI symbols bind, the scratch query refuses
 unsupported arguments, and the Python entry refuses CPU tensors and inputs that require grad."""
 import numpy as np
 import pytest
 import torch
+from scipy.signal import lfilter
 
 import sudo_rm_rf_b200 as P
 from sudo_rm_rf_b200 import _native as N
-from bss_oracle import bss_eval, bss_eval_direct
+from bss_oracle import _criteria, bss_eval, bss_eval_direct, bss_eval_recursion, bss_eval_span, kept_delays
 
 SYMBOLS = ("sdr_bss_eval_scratch_bytes", "sdr_bss_eval", "sdr_bss_eval_mixture")
 
@@ -70,3 +72,61 @@ def test_refusals():
     with pytest.raises(RuntimeError, match="CUDA|no autograd"):
         P.bss_eval_sources(g, x)
     assert P.bss_eval_sources is P.bss_eval.bss_eval_sources
+
+
+@pytest.mark.parametrize("S,T,F,seed", [(1, 60, 8, 0), (2, 200, 16, 1), (3, 150, 24, 2), (4, 120, 12, 3),
+                                        (2, 90, 30, 4)])
+def test_span_oracle_equals_full_projection_when_nothing_is_dropped(S, T, F, seed):
+    """On the well-conditioned cases above the recursion keeps every delay, and QR onto them and the restated
+    recursion give the normal equations' and lstsq's values within 1e-9 dB."""
+    rng = np.random.default_rng(seed)
+    refs = rng.standard_normal((S, T))
+    refs[-1] = np.convolve(refs[-1], [1.0, 0.9, 0.5])[:T]
+    ests = rng.standard_normal((S, S)) @ refs + 0.05 * rng.standard_normal((S, T))
+    ests[0] = np.convolve(ests[0], [0.7, -0.2, 0.1])[:T]
+    assert kept_delays(refs, F).all()
+    for perm in (True, False):
+        a, b = bss_eval(refs, ests, perm, F), bss_eval_direct(refs, ests, perm, F)
+        c, d = bss_eval_span(refs, ests, perm, F), bss_eval_recursion(refs, ests, perm, F)
+        for x, y, z, w in zip(a[:3], b[:3], c[:3], d[:3]):
+            assert agree(x, z, 1e-9) and agree(y, z, 1e-9) and agree(w, z, 1e-9), (x, y, z, w)
+        assert np.array_equal(a[3], c[3]) and np.array_equal(a[3], d[3])
+
+
+@pytest.mark.parametrize("S,pole", [(1, 0.0), (2, 0.9), (4, 0.95), (2, 0.999)])
+def test_nothing_dropped_on_white_and_ar_references(S, pole):
+    rng = np.random.default_rng(20 + S)
+    refs = lfilter([1.0], [1.0, -pole], rng.standard_normal((S, 4000)), axis=1).astype(np.float32)
+    assert kept_delays(refs.astype(np.float64), 512).all()
+
+
+def windowed_tones(T=32000):
+    t = np.arange(T)
+    return (sum(np.sin(2 * np.pi * f / 16000 * t + i) for i, f in enumerate((100, 200, 300)))
+            * np.hanning(T)).astype(np.float32).astype(np.float64)
+
+
+def test_windowed_tones_defeat_the_normal_equations():
+    """A Hann-windowed sum of three tones (fp32) with an estimate at 20 dB SNR, T = 32000, F = 512.  Its 512 delays
+    span a handful of dimensions to 1e-15, so G's condition number is ~1e15: np.linalg.solve (mir_eval's method)
+    reports an SDR many dB off (1.1 dB with one LAPACK build; the figure depends on the build), QR onto every delay
+    20.06 dB, QR onto the kept delays 20.00 dB, the noise level.  The recursion keeps a prefix of 5 lags, then
+    nothing."""
+    rng = np.random.default_rng(0)
+    T, F = 32000, 512
+    ref = windowed_tones(T)[None]
+    noise = rng.standard_normal(T)
+    est = (ref[0] + noise * np.sqrt(np.sum(ref[0] ** 2) / np.sum(noise ** 2) / 100)).astype(np.float32)
+    est = est.astype(np.float64)[None]
+    kept = kept_delays(ref, F)[:, 0]
+    n = int(kept.sum())
+    assert 3 <= n <= 12 and kept[:n].all(), n
+    span = bss_eval_span(ref, est, False, F)[0][0]
+    solve = bss_eval(ref, est, False, F)[0][0]
+    cols = np.stack([np.r_[np.zeros(l), ref[0], np.zeros(F - 1 - l)] for l in range(F)], 1)
+    Q = np.linalg.qr(cols)[0]
+    e = np.r_[est[0], np.zeros(F - 1)]
+    full = _criteria(e, Q @ (Q.T @ e), Q @ (Q.T @ e))[0]
+    assert abs(span - 20.0) < 0.05, span
+    assert 0.0 <= full - span < 0.2, (full, span)
+    assert abs(solve - full) > 3.0, (solve, full)
