@@ -228,14 +228,72 @@ def _replace(st: _DeviceState, slot: str, buf) -> None:
     setattr(st, slot, buf)
 
 
-def _ensure_workspace(st: _DeviceState, nbytes: int, device) -> None:
-    if st.workspace is None or st.workspace.numel() < nbytes:
+def _ensure(st: _DeviceState, slot: str, nbytes: int, device) -> torch.Tensor:
+    """The buffer in ``slot`` ("workspace" or "staging"), replaced by one of ``nbytes`` if it is smaller."""
+    buf = getattr(st, slot)
+    if buf is None or buf.numel() < nbytes:
         if st.event is not None:
             st.event.synchronize()      # kernels of an earlier call (possibly on another stream) still use it
-        _replace(st, "workspace", None)
-        st.graphs.clear()               # captured graphs point into the old workspace
-        st.workspace = torch.empty(nbytes, dtype=torch.uint8, device=device)
-    _hand_out(st, "workspace")
+        _replace(st, slot, None)
+        st.graphs.clear()               # captured graphs point into the old buffer
+        buf = torch.empty(nbytes, dtype=torch.uint8, device=device)
+        setattr(st, slot, buf)
+    _hand_out(st, slot)
+    return buf
+
+
+def _call_shared(model, cfg: N.SdrConfig, device, ws_bytes: int, refusal: str, enqueue) -> torch.Tensor:
+    """Every call that runs on the model's cached state goes through here: packs (or reuses) the weights, sizes the
+    shared workspace, hands it over from the previous call's stream and runs ``enqueue(packed, workspace)``, which
+    enqueues on the current stream.  ``ws_bytes`` is the caller's size query; 0 raises ``refusal``.  Returns the
+    packed weights the call ran with."""
+    with torch.cuda.device(device):
+        packed = packed_weights(model, cfg, device)
+        if ws_bytes == 0:
+            raise N.NativeError(refusal)
+        st = _state(model, device)
+        ws = _ensure(st, "workspace", ws_bytes, device)
+        cur = _enter_stream(st, device)
+        enqueue(packed, ws)
+        _leave_stream(st, cur)
+    return packed
+
+
+def _graphed(graphs: dict, key, bound: int, device, enqueue) -> str:
+    """Runs ``enqueue`` (which enqueues on the current stream) eagerly on the first call with ``key``, which also warms
+    every kernel; captures it into a CUDA graph on a side stream on the second, and replays that graph from then on.
+    ``graphs`` is cleared when it holds ``bound`` keys.  Returns "eager", "captured" or "replayed"."""
+    entry = graphs.get(key)
+    if entry is None:
+        if len(graphs) >= bound:
+            graphs.clear()
+        graphs[key] = "warm"
+        enqueue()
+        return "eager"
+    if entry == "warm":
+        cur = torch.cuda.current_stream(device)
+        side = torch.cuda.Stream(device=device)
+        side.wait_stream(cur)
+        graph = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(graph, stream=side):
+            enqueue()
+        cur.wait_stream(side)
+        graphs[key] = graph
+        graph.replay()
+        return "captured"
+    entry.replay()
+    return "replayed"
+
+
+def _model_device(model, refusal: str, device=None) -> torch.device:
+    """``device``, or the device of the model's parameters, with a missing index resolved to the current device.
+    Raises ``refusal`` when it is not a CUDA device."""
+    device = torch.device(device) if device is not None else _fetch(model, _probe_names(model)[0]).device
+    if device.type != "cuda":
+        raise RuntimeError(refusal)
+    if device.index is None:
+        device = torch.device("cuda", torch.cuda.current_device())
+    return device
 
 
 def _walk(model, names):
@@ -349,7 +407,8 @@ def packed_weights(model, cfg: N.SdrConfig, device) -> torch.Tensor:
     return packed
 
 
-def _check_input(model, cfg, wav: torch.Tensor) -> torch.Tensor:
+def _check_mixture(cfg, wav: torch.Tensor) -> None:
+    """A [B, A, T] CUDA mixture with the model's channel count and no empty dimension."""
     if wav.dim() != 3:
         raise RuntimeError(
             f"Expected 3D input [batch, channels, time] to the encoder, got {list(wav.shape)}")
@@ -359,13 +418,17 @@ def _check_input(model, cfg, wav: torch.Tensor) -> torch.Tensor:
         raise RuntimeError(
             "sudo_rm_rf_b200 runs on CUDA (sm_90a) only and has no CPU path: move the model "
             "and the mixture to an H100 (`model.cuda()`, `mixture.cuda()`).")
+    if wav.shape[0] == 0 or wav.shape[-1] == 0:
+        raise RuntimeError("empty batch or zero-length mixture")
+
+
+def _check_input(model, cfg, wav: torch.Tensor) -> torch.Tensor:
+    _check_mixture(cfg, wav)
     if torch.is_grad_enabled() and model.training and \
             any(_fetch(model, n).requires_grad for n in _probe_names(model)):
         raise RuntimeError(
             "sudo_rm_rf_b200 implements the inference forward only (no autograd): call "
             "model.eval() and/or wrap the call in torch.no_grad().")
-    if wav.shape[0] == 0 or wav.shape[-1] == 0:
-        raise RuntimeError("empty batch or zero-length mixture")
     global _warned_detached
     if torch.is_grad_enabled() and not _warned_detached and \
             any(_fetch(model, n).requires_grad for n in _probe_names(model)):
@@ -386,22 +449,15 @@ def forward(model, wav: torch.Tensor, mixture_consistency: bool = False) -> torc
                            f"this model has in_audio_channels={cfg.in_audio_channels}")
     device = x.device
     B, _, T = x.shape
-    with torch.cuda.device(device):
-        packed = packed_weights(model, cfg, device)
-        st = _state(model, device)
-        ws_bytes = lib.sdr_workspace_bytes(C.byref(cfg), B, T)
-        if ws_bytes == 0:
-            raise N.NativeError("bad model configuration (sdr_workspace_bytes returned 0)")
-        _ensure_workspace(st, ws_bytes, device)
-        out = torch.empty((B, cfg.num_sources * cfg.in_audio_channels, T),
-                          dtype=torch.float32, device=device)
-        cur = _enter_stream(st, device)
+    out = torch.empty((B, cfg.num_sources * cfg.in_audio_channels, T), dtype=torch.float32, device=device)
+
+    def enqueue(packed, ws):
         N.check(lib.sdr_forward(C.byref(cfg), C.c_void_p(packed.data_ptr()),
                                 C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()),
                                 B, T, 1 if mixture_consistency else 0,
-                                C.c_void_p(st.workspace.data_ptr()), st.workspace.numel(),
-                                C.c_void_p(cur.cuda_stream)), "sdr_forward")
-        _leave_stream(st, cur)
+                                C.c_void_p(ws.data_ptr()), ws.numel(), N.stream(device)), "sdr_forward")
+    _call_shared(model, cfg, device, lib.sdr_workspace_bytes(C.byref(cfg), B, T),
+                 "bad model configuration (sdr_workspace_bytes returned 0)", enqueue)
     return out
 
 
@@ -420,21 +476,15 @@ def separate(model, wav: torch.Tensor, mixture_consistency: bool = False) -> tor
         raise RuntimeError("separate() follows the README recipe, which is written for mono mixtures")
     device = x.device
     B, _, T = x.shape
-    with torch.cuda.device(device):
-        packed = packed_weights(model, cfg, device)
-        st = _state(model, device)
-        ws_bytes = lib.sdr_separate_workspace_bytes(C.byref(cfg), B, T)
-        if ws_bytes == 0:
-            raise N.NativeError("bad model configuration (sdr_separate_workspace_bytes returned 0)")
-        _ensure_workspace(st, ws_bytes, device)
-        out = torch.empty((B, cfg.num_sources, T), dtype=torch.float32, device=device)
-        cur = _enter_stream(st, device)
+    out = torch.empty((B, cfg.num_sources, T), dtype=torch.float32, device=device)
+
+    def enqueue(packed, ws):
         N.check(lib.sdr_separate(C.byref(cfg), C.c_void_p(packed.data_ptr()),
                                  C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()),
                                  B, T, 1 if mixture_consistency else 0,
-                                 C.c_void_p(st.workspace.data_ptr()), st.workspace.numel(),
-                                 C.c_void_p(cur.cuda_stream)), "sdr_separate")
-        _leave_stream(st, cur)
+                                 C.c_void_p(ws.data_ptr()), ws.numel(), N.stream(device)), "sdr_separate")
+    _call_shared(model, cfg, device, lib.sdr_separate_workspace_bytes(C.byref(cfg), B, T),
+                 "bad model configuration (sdr_separate_workspace_bytes returned 0)", enqueue)
     return out
 
 
@@ -451,11 +501,7 @@ def forward_host(model, host_wav: torch.Tensor, host_out: torch.Tensor = None,
     if host_wav.dim() != 3 or host_wav.is_cuda or host_wav.dtype != torch.float32 \
             or not host_wav.is_contiguous():
         raise RuntimeError("forward_host expects a contiguous fp32 CPU tensor [B, A, T]")
-    device = torch.device(device) if device is not None else _fetch(model, _probe_names(model)[0]).device
-    if device.type != "cuda":
-        raise RuntimeError("the model must live on a CUDA device")
-    if device.index is None:
-        device = torch.device("cuda", torch.cuda.current_device())
+    device = _model_device(model, "the model must live on a CUDA device", device)
     B, A, T = host_wav.shape
     if A != cfg.in_audio_channels:
         raise RuntimeError(f"expected {cfg.in_audio_channels} audio channel(s), got {A}")
@@ -465,55 +511,28 @@ def forward_host(model, host_wav: torch.Tensor, host_out: torch.Tensor = None,
             or host_out.is_cuda or not host_out.is_contiguous():
         raise RuntimeError("host_out must be a contiguous fp32 CPU tensor [B, S*A, T]")
     mc = 1 if mixture_consistency else 0
-    with torch.cuda.device(device):
-        packed = packed_weights(model, cfg, device)
-        st = _state(model, device)
-        ws_bytes = lib.sdr_workspace_bytes(C.byref(cfg), B, T)
-        io_bytes = lib.sdr_host_staging_bytes(C.byref(cfg), B, T)
-        if ws_bytes == 0 or io_bytes == 0:
-            raise N.NativeError("bad model configuration")
-        _ensure_workspace(st, ws_bytes, device)
-        if st.staging is None or st.staging.numel() < io_bytes:
-            if st.event is not None:
-                st.event.synchronize()
-            st.graphs.clear()
-            _replace(st, "staging", torch.empty(io_bytes, dtype=torch.uint8, device=device))
-        _hand_out(st, "staging")
-        cur0 = _enter_stream(st, device)
+    io_bytes = lib.sdr_host_staging_bytes(C.byref(cfg), B, T)
+    if io_bytes == 0:
+        raise N.NativeError("bad model configuration")
+    st = _state(model, device)
 
-        def enqueue():
+    def enqueue(packed, ws):
+        staging = _ensure(st, "staging", io_bytes, device)
+
+        def call():
             N.check(lib.sdr_forward_host(C.byref(cfg), C.c_void_p(packed.data_ptr()),
                                          C.c_void_p(host_wav.data_ptr()), C.c_void_p(host_out.data_ptr()),
-                                         B, T, mc,
-                                         C.c_void_p(st.staging.data_ptr()), st.staging.numel(),
-                                         C.c_void_p(st.workspace.data_ptr()), st.workspace.numel(),
+                                         B, T, mc, C.c_void_p(staging.data_ptr()), staging.numel(),
+                                         C.c_void_p(ws.data_ptr()), ws.numel(),
                                          N.stream(device)), "sdr_forward_host")
 
-        graphable = use_graph and host_wav.is_pinned() and host_out.is_pinned() \
-            and not torch.cuda.is_current_stream_capturing()
-        if not graphable:
-            enqueue()
-            _leave_stream(st, cur0)
-            return host_out
-        key = (host_wav.data_ptr(), host_out.data_ptr(), B, T, mc, st.workspace.data_ptr(),
-               st.staging.data_ptr(), packed.data_ptr())
-        entry = st.graphs.get(key)
-        if entry is None:
-            if len(st.graphs) >= 8:
-                st.graphs.clear()
-            st.graphs[key] = "warm"          # first call with this key: eager (also warms every kernel)
-            enqueue()
-        elif entry == "warm":
-            cur = torch.cuda.current_stream(device)
-            side = torch.cuda.Stream(device=device)
-            side.wait_stream(cur)
-            graph = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(graph, stream=side):
-                enqueue()
-            cur.wait_stream(side)
-            st.graphs[key] = graph
-            graph.replay()
+        if use_graph and host_wav.is_pinned() and host_out.is_pinned() \
+                and not torch.cuda.is_current_stream_capturing():
+            key = (host_wav.data_ptr(), host_out.data_ptr(), B, T, mc, ws.data_ptr(), staging.data_ptr(),
+                   packed.data_ptr())
+            _graphed(st.graphs, key, 8, device, call)
         else:
-            entry.replay()
-        _leave_stream(st, cur0)
+            call()
+    _call_shared(model, cfg, device, lib.sdr_workspace_bytes(C.byref(cfg), B, T), "bad model configuration",
+                 enqueue)
     return host_out

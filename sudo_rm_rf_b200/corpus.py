@@ -84,34 +84,29 @@ def separate_corpus(model, wavs: Iterable[torch.Tensor], max_batch: int = 32,
     cfg = _engine.make_config(model)
     if cfg.in_audio_channels != 1:
         raise RuntimeError("separate_corpus follows the README recipe, which is written for mono mixtures")
-    device = _engine._fetch(model, _engine._probe_names(model)[0]).device
-    if device.type != "cuda":
-        raise RuntimeError("sudo_rm_rf_b200 runs on CUDA (sm_90a) only: move the model to an H100")
+    device = _engine._model_device(model, "sudo_rm_rf_b200 runs on CUDA (sm_90a) only: move the model to an H100")
     if torch.is_grad_enabled() and model.training:
         raise RuntimeError("sudo_rm_rf_b200 implements the inference forward only: call model.eval()")
     plan = plan_buckets([int(w.shape[0]) for w in wavs], model_padding_rule(cfg), max_batch)
     results: List[torch.Tensor] = [None] * len(wavs)
     S = cfg.num_sources
     with torch.cuda.device(device), torch.no_grad():
-        packed = _engine.packed_weights(model, cfg, device)
-        st = _engine._state(model, device)
         for Tp, idx in plan:
             B = len(idx)
             batch = torch.zeros((B, 1, Tp), dtype=torch.float32, device=device)
             for r, i in enumerate(idx):
                 batch[r, 0, :wavs[i].shape[0]] = wavs[i].detach().to(device=device, dtype=torch.float32)
             lengths = torch.tensor([int(wavs[i].shape[0]) for i in idx], dtype=torch.int64, device=device)
-            ws_bytes = lib.sdr_separate_workspace_bytes(C.byref(cfg), B, Tp)
-            if ws_bytes == 0:
-                raise N.NativeError("bad model configuration (sdr_separate_workspace_bytes returned 0)")
-            _engine._ensure_workspace(st, ws_bytes, device)
             out = torch.empty((B, S, Tp), dtype=torch.float32, device=device)
-            N.check(lib.sdr_separate_ragged(
-                C.byref(cfg), C.c_void_p(packed.data_ptr()), C.c_void_p(batch.data_ptr()),
-                C.c_void_p(lengths.data_ptr()), C.c_void_p(out.data_ptr()), B, Tp,
-                1 if mixture_consistency else 0, 1 if rescale else 0,
-                C.c_void_p(st.workspace.data_ptr()), st.workspace.numel(),
-                N.stream(device)), "sdr_separate_ragged")
+
+            def enqueue(packed, ws):
+                N.check(lib.sdr_separate_ragged(
+                    C.byref(cfg), C.c_void_p(packed.data_ptr()), C.c_void_p(batch.data_ptr()),
+                    C.c_void_p(lengths.data_ptr()), C.c_void_p(out.data_ptr()), B, Tp,
+                    1 if mixture_consistency else 0, 1 if rescale else 0,
+                    C.c_void_p(ws.data_ptr()), ws.numel(), N.stream(device)), "sdr_separate_ragged")
+            _engine._call_shared(model, cfg, device, lib.sdr_separate_workspace_bytes(C.byref(cfg), B, Tp),
+                                 "bad model configuration (sdr_separate_workspace_bytes returned 0)", enqueue)
             for r, i in enumerate(idx):
                 results[i] = out[r, :, :wavs[i].shape[0]].clone()
     return results
@@ -171,9 +166,8 @@ class CorpusSeparator:
         self.cfg = _engine.make_config(model)
         if self.cfg.in_audio_channels != 1:
             raise RuntimeError("CorpusSeparator follows the README recipe, which is written for mono mixtures")
-        self.device = _engine._fetch(model, _engine._probe_names(model)[0]).device
-        if self.device.type != "cuda":
-            raise RuntimeError("sudo_rm_rf_b200 runs on CUDA (sm_90a) only: move the model to an H100")
+        self.device = _engine._model_device(model,
+                                            "sudo_rm_rf_b200 runs on CUDA (sm_90a) only: move the model to an H100")
         self.quantum = model_padding_rule(self.cfg)      # T -> padded length (the model's own rule)
         self.graphs = {}           # (B, Tp, slot) -> "warm" | CUDAGraph
         self.launches = {"eager": 0, "captured": 0, "replayed": 0}
@@ -196,7 +190,6 @@ class CorpusSeparator:
         results: List[torch.Tensor] = [None] * len(wavs)
         with torch.cuda.device(dev), torch.no_grad():
             packed = _engine.packed_weights(self.model, cfg, dev)
-            st = _engine._state(self.model, dev)
             key_buf = (max_in, ws_bytes, packed.data_ptr())
             if getattr(self, "_buf_key", None) != key_buf:      # (re)allocate staging once per corpus shape: graphs hold addresses
                 self.graphs.clear()
@@ -242,37 +235,21 @@ class CorpusSeparator:
                     ev_in = torch.cuda.Event()
                     ev_in.record(self._s_in)
 
-                def enqueue(stream_ptr, B=B, Tp=Tp, slot=slot):
+                def enqueue():
                     N.check(lib.sdr_separate_ragged(
                         C.byref(cfg), C.c_void_p(packed.data_ptr()), C.c_void_p(self._d_in[slot].data_ptr()),
                         C.c_void_p(self._d_len[slot].data_ptr()), C.c_void_p(self._d_out[slot].data_ptr()), B, Tp,
-                        self.mc, self.rescale, C.c_void_p(self._ws.data_ptr()), self._ws.numel(), stream_ptr),
+                        self.mc, self.rescale, C.c_void_p(self._ws.data_ptr()), self._ws.numel(), N.stream(dev)),
                         "sdr_separate_ragged")
 
                 with torch.cuda.stream(self._s_cmp):
                     self._s_cmp.wait_event(ev_in)
-                    key = (B, Tp, slot)
-                    entry = self.graphs.get(key) if self.use_graphs else None
-                    if not self.use_graphs or entry is None:
-                        if self.use_graphs:
-                            if len(self.graphs) >= self.max_graphs:
-                                self.graphs.clear()
-                            self.graphs[key] = "warm"
-                        enqueue(C.c_void_p(self._s_cmp.cuda_stream))
-                        self.launches["eager"] += 1
-                    elif entry == "warm":
-                        side = torch.cuda.Stream(device=dev)
-                        side.wait_stream(self._s_cmp)
-                        graph = torch.cuda.CUDAGraph()
-                        with torch.cuda.graph(graph, stream=side):
-                            enqueue(N.stream(dev))
-                        self._s_cmp.wait_stream(side)
-                        self.graphs[key] = graph
-                        graph.replay()
-                        self.launches["captured"] += 1
+                    if self.use_graphs:
+                        how = _engine._graphed(self.graphs, (B, Tp, slot), self.max_graphs, dev, enqueue)
                     else:
-                        entry.replay()
-                        self.launches["replayed"] += 1
+                        enqueue()
+                        how = "eager"
+                    self.launches[how] += 1
                     ev_cmp = torch.cuda.Event()
                     ev_cmp.record(self._s_cmp)
                 free_in[slot] = ev_cmp

@@ -58,12 +58,8 @@ class CausalStream:
         ws_bytes = lib.sdr_stream_workspace_bytes(C.byref(cfg), B, Cs)
         if ws_bytes == 0:
             raise ValueError(f"sdr_stream_workspace_bytes refused batch_size={B}, chunk_samples={Cs}")
-        device = _engine._fetch(model, "encoder.weight").device
-        if device.type != "cuda":
-            raise RuntimeError("sudo_rm_rf_b200 streams on CUDA (sm_90a) only and has no CPU path: move the model "
-                               "to an H100 (`model.cuda()`)")
-        if device.index is None:
-            device = torch.device("cuda", torch.cuda.current_device())
+        device = _engine._model_device(model, "sudo_rm_rf_b200 streams on CUDA (sm_90a) only and has no CPU path: "
+                                              "move the model to an H100 (`model.cuda()`)")
         self.model = model
         self.device = device
         self.batch_size = B
@@ -76,23 +72,20 @@ class CausalStream:
         self._ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
         self.reset()
 
-    def _stream_ptr(self):
-        return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
-
     def reset(self, slots: Optional[Iterable[int]] = None) -> None:
         """Start slots over (all of them when ``slots`` is None): their next step is the start of a new stream."""
         lib = N.lib()
         with torch.cuda.device(self.device):
             if slots is None:
                 rc = lib.sdr_stream_reset(C.byref(self._cfg), C.c_void_p(self._state.data_ptr()), self.batch_size,
-                                          None, 0, self._stream_ptr())
+                                          None, 0, N.stream(self.device))
             else:
                 idx = [int(s) for s in slots]
                 if any(s < 0 or s >= self.batch_size for s in idx):
                     raise IndexError(f"slots {idx} out of range for batch_size={self.batch_size}")
                 arr = (C.c_int32 * max(1, len(idx)))(*idx)
                 rc = lib.sdr_stream_reset(C.byref(self._cfg), C.c_void_p(self._state.data_ptr()), self.batch_size,
-                                          arr, len(idx), self._stream_ptr())
+                                          arr, len(idx), N.stream(self.device))
             N.check(rc, "sdr_stream_reset")
 
     def step(self, chunk: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -116,7 +109,7 @@ class CausalStream:
             N.check(lib.sdr_stream_step(C.byref(cfg), C.c_void_p(packed.data_ptr()), C.c_void_p(self._state.data_ptr()),
                                         C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()), B, Cs,
                                         1 if self.mixture_consistency else 0, C.c_void_p(self._ws.data_ptr()),
-                                        self._ws.numel(), self._stream_ptr()), "sdr_stream_step")
+                                        self._ws.numel(), N.stream(self.device)), "sdr_stream_step")
         return out
 
     def flush(self) -> torch.Tensor:
@@ -128,6 +121,6 @@ class CausalStream:
                            dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
             N.check(lib.sdr_stream_flush(C.byref(cfg), C.c_void_p(self._state.data_ptr()), C.c_void_p(tail.data_ptr()),
-                                         self.batch_size, 1 if self.mixture_consistency else 0, self._stream_ptr()),
+                                         self.batch_size, 1 if self.mixture_consistency else 0, N.stream(self.device)),
                     "sdr_stream_flush")
         return tail

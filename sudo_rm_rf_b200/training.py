@@ -31,15 +31,7 @@ def _check(model, cfg, wav: torch.Tensor) -> torch.Tensor:
         raise RuntimeError("sudo_rm_rf_b200 training computes parameter gradients only: the gradient with respect "
                            "to the mixture is not built, so pass a mixture that does not require grad "
                            "(e.g. `mixture.detach()`).")
-    if wav.dim() != 3:
-        raise RuntimeError(f"Expected 3D input [batch, channels, time] to the encoder, got {list(wav.shape)}")
-    if wav.shape[1] != cfg.in_audio_channels:
-        raise RuntimeError(f"expected {cfg.in_audio_channels} audio channel(s), got {wav.shape[1]}")
-    if not wav.is_cuda:
-        raise RuntimeError("sudo_rm_rf_b200 runs on CUDA (sm_90a) only and has no CPU path: move the model and the "
-                           "mixture to an H100 (`model.cuda()`, `mixture.cuda()`).")
-    if wav.shape[0] == 0 or wav.shape[-1] == 0:
-        raise RuntimeError("empty batch or zero-length mixture")
+    _engine._check_mixture(cfg, wav)
     return wav.to(torch.float32).contiguous()
 
 
@@ -49,23 +41,21 @@ class _NativeTrain(torch.autograd.Function):
         lib = N.lib()
         device = wav.device
         B, _, T = wav.shape
-        with torch.cuda.device(device):
-            packed = _engine.packed_weights(model, cfg, device)
-            st = _engine._state(model, device)
-            ws_bytes = lib.sdr_workspace_bytes(C.byref(cfg), B, T)
-            saved_bytes = lib.sdr_train_saved_bytes(C.byref(cfg), B, T)
-            if ws_bytes == 0 or saved_bytes == 0:
-                raise N.NativeError("configuration not supported by the training path")
-            _engine._ensure_workspace(st, ws_bytes, device)
-            # per call, so that several forwards before one backward keep their own activations
-            saved = torch.empty(saved_bytes, dtype=torch.uint8, device=device)
-            out = torch.empty((B, cfg.num_sources, T), dtype=torch.float32, device=device)
-            cur = _engine._enter_stream(st, device)
+        unsupported = "configuration not supported by the training path"
+        saved_bytes = lib.sdr_train_saved_bytes(C.byref(cfg), B, T)
+        if saved_bytes == 0:
+            raise N.NativeError(unsupported)
+        # per call, so that several forwards before one backward keep their own activations
+        saved = torch.empty(saved_bytes, dtype=torch.uint8, device=device)
+        out = torch.empty((B, cfg.num_sources, T), dtype=torch.float32, device=device)
+
+        def enqueue(packed, ws):
             N.check(lib.sdr_forward_train(C.byref(cfg), C.c_void_p(packed.data_ptr()), C.c_void_p(wav.data_ptr()),
                                           C.c_void_p(out.data_ptr()), B, T, C.c_void_p(saved.data_ptr()),
-                                          saved.numel(), C.c_void_p(st.workspace.data_ptr()), st.workspace.numel(),
-                                          C.c_void_p(cur.cuda_stream)), "sdr_forward_train")
-            _engine._leave_stream(st, cur)
+                                          saved.numel(), C.c_void_p(ws.data_ptr()), ws.numel(),
+                                          N.stream(device)), "sdr_forward_train")
+        packed = _engine._call_shared(model, cfg, device, lib.sdr_workspace_bytes(C.byref(cfg), B, T), unsupported,
+                                      enqueue)
         ctx.cfg = cfg
         ctx.packed = packed          # the weights this forward ran with, whatever a later forward packs
         ctx.saved = saved
