@@ -244,15 +244,6 @@ static long long padded_len(const Layout& l, long long T) {
     return (T + q - 1) / q * q;
 }
 
-// decoder.weight [C=S*A*N][SA][K]  ->  [SA*K][C]
-__global__ void transpose_decoder_kernel(const float* __restrict__ w, float* __restrict__ wt,
-                                         int C, int SAK) {
-    const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
-    if (i >= (long long)C * SAK) return;
-    const int c = (int)(i % C), r = (int)(i / C);
-    wt[i] = w[(size_t)c * SAK + r];
-}
-
 // Byte offsets of 256-byte aligned segments, handed out in order; `total` bytes hold them all.
 struct Segments {
     size_t total = 0;
@@ -348,7 +339,7 @@ static int decoder_tail(const Layout& l, const Plan& p, const float* pk, const N
 // and the bottleneck (original model: l1) into x with ln folded into its operand load.
 static int front_end(const Layout& l, const Plan& p, const float* pk, const float* mixture, int B, long long T,
                      char* ws, cudaStream_t st) {
-    if (cudaMemsetAsync(p.stats(ws), 0, p.stats_doubles * sizeof(double), st) != cudaSuccess) return SDR_ERR_CUDA;
+    SDR_TRY(cuda_status(cudaMemsetAsync(p.stats(ws), 0, p.stats_doubles * sizeof(double), st)));
     float* e = p.buf(ws, p.o_e);
     SDR_TRY(encoder(l, pk, mixture, e, p.stats(ws), B, T, p.L, st));
     const NormIn ln{p.stats(ws), pk + l.ln_g, pk + l.ln_be, nullptr, (double)l.N * p.L, 0};
@@ -560,7 +551,7 @@ static Saved saved_layout(const Layout& l, const Plan& p, int B) {
 }
 
 static int copy_d2d(void* dst, const void* src, size_t bytes, cudaStream_t st) {
-    return cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st) == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return cuda_status(cudaMemcpyAsync(dst, src, bytes, cudaMemcpyDeviceToDevice, st));
 }
 
 // `save` (improved model only, else null): the training forward's copy of what saved_layout lists.
@@ -740,7 +731,7 @@ static int backward_impl(const Layout& l, const Plan& p, const BwdPlan& bp, cons
     for (int i = l.U - 1; i >= 0; --i) {
         const UBlockOff& u = l.ub[i];
         const float* xi = sv.x(saved, i);
-        if (cudaMemsetAsync(bst, 0, (size_t)(D + 2) * B * 2 * sizeof(double), st) != cudaSuccess) return SDR_ERR_CUDA;
+        SDR_TRY(cuda_status(cudaMemsetAsync(bst, 0, (size_t)(D + 2) * B * 2 * sizeof(double), st)));
         SDR_TRY(gemm(pk, u.proj, xi, kNoNorm, y, slot(0), B, L, st));
         const NormIn n0{slot(0), pk + u.proj_g, pk + u.proj_be, pk + u.proj_a, (double)Ci * L, 0};
         NormIn nl[kMaxDepthApi];
@@ -853,21 +844,18 @@ int sdr_pack_weights(const sdr_config* cfg, const float* const* params, int n_pa
     SDR_TRY(check_buffers({{packed, 16, packed_bytes, l.total * sizeof(float)}}));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     float* pk = static_cast<float*>(packed);
-    if (cudaMemsetAsync(pk, 0, l.total * sizeof(float), st) != cudaSuccess) return SDR_ERR_CUDA;
+    SDR_TRY(cuda_status(cudaMemsetAsync(pk, 0, l.total * sizeof(float), st)));
     for (size_t i = 0; i < l.off.size(); ++i) {
         if (!params[i]) return SDR_ERR_BAD_ARGUMENT;
-        if (cudaMemcpyAsync(pk + l.off[i], params[i], l.numel[i] * sizeof(float),
-                            cudaMemcpyDeviceToDevice, st) != cudaSuccess) return SDR_ERR_CUDA;
+        SDR_TRY(copy_d2d(pk + l.off[i], params[i], l.numel[i] * sizeof(float), st));
     }
     // the derived regions, then the images (some are packed from a derived region): all in stream order
     if (l.orig) {
         SDR_TRY(launch_toeplitz_mask(pk + l.m_w, pk + l.m_b, pk + l.mask.w, pk + l.mask.b, l.S, l.N, st));
         SDR_TRY(launch_grouped_decoder(pk + l.dec_w, pk + l.dec.w, l.S, l.N, l.K, st));
     } else {
-        const int C = l.dec.K, SAK = l.dec.M;
-        const long long n = (long long)C * SAK;
-        transpose_decoder_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(pk + l.dec_w, pk + l.dec.w, C, SAK);
-        if (cudaGetLastError() != cudaSuccess) return SDR_ERR_CUDA;
+        // decoder.weight [C][SA][K] -> [SA*K][C]
+        SDR_TRY(launch_transpose(pk + l.dec_w, pk + l.dec.w, l.dec.K, l.dec.M, st));
     }
     if (l.causal) {
         SDR_TRY(launch_take_taps(pk + l.enc_w, pk + l.enc_wc, (long long)l.N * l.A, 2 * l.K - 1, l.K, st));
@@ -1081,12 +1069,12 @@ int sdr_stream_reset(const sdr_config* cfg, void* state, int B, const int32_t* h
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     const size_t slot = stream_state(l).slot * sizeof(float);
     if (!host_slots_or_null)
-        return cudaMemsetAsync(state, 0, (size_t)B * slot, st) == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+        return cuda_status(cudaMemsetAsync(state, 0, (size_t)B * slot, st));
     for (int i = 0; i < n; ++i)
         if (host_slots_or_null[i] < 0 || host_slots_or_null[i] >= B) return SDR_ERR_BAD_ARGUMENT;
     for (int i = 0; i < n; ++i)
-        if (cudaMemsetAsync(static_cast<char*>(state) + (size_t)host_slots_or_null[i] * slot, 0, slot, st) != cudaSuccess)
-            return SDR_ERR_CUDA;
+        SDR_TRY(cuda_status(
+            cudaMemsetAsync(static_cast<char*>(state) + (size_t)host_slots_or_null[i] * slot, 0, slot, st)));
     return SDR_OK;
 }
 
@@ -1160,10 +1148,9 @@ int sdr_forward_host(const sdr_config* cfg, const void* packed, const float* hos
     const size_t out_bytes = (size_t)B * l.S * l.A * T * sizeof(float);
     float* d_in = static_cast<float*>(dev_io);
     float* d_out = reinterpret_cast<float*>(static_cast<char*>(dev_io) + io.est);
-    if (cudaMemcpyAsync(d_in, host_mixture, in_bytes, cudaMemcpyHostToDevice, st) != cudaSuccess) return SDR_ERR_CUDA;
+    SDR_TRY(cuda_status(cudaMemcpyAsync(d_in, host_mixture, in_bytes, cudaMemcpyHostToDevice, st)));
     SDR_TRY(sdr_forward(cfg, packed, d_in, d_out, B, T, apply_mixture_consistency, workspace, workspace_bytes, stream));
-    if (cudaMemcpyAsync(host_out, d_out, out_bytes, cudaMemcpyDeviceToHost, st) != cudaSuccess) return SDR_ERR_CUDA;
-    return SDR_OK;
+    return cuda_status(cudaMemcpyAsync(host_out, d_out, out_bytes, cudaMemcpyDeviceToHost, st));
 }
 
 int sdr_mixture_consistency(const float* est, const float* mix, float* out, int B, int S, int64_t T,

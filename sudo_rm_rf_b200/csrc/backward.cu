@@ -127,14 +127,13 @@ int launch_wgrad(const float* dY, const float* X, const NormIn& nin, float* dW, 
     const int ktiles = (K + kWgTile - 1) / kWgTile, mtiles = (M + kWgTile - 1) / kWgTile;
     const long long ctas = P * ktiles * mtiles;
     if (ctas > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-    wgrad_partial_kernel<<<(unsigned)ctas, kBwThreads, 0, st>>>(dY, X, nin, scratch, M, K, L, nchunk, ktiles, mtiles,
-                                                                 db ? 1 : 0);
-    if (cudaGetLastError() != cudaSuccess) return SDR_ERR_CUDA;
+    if (const int rc = launch(wgrad_partial_kernel, (unsigned)ctas, kBwThreads, 0, st, dY, X, nin, scratch, M, K, L,
+                              nchunk, ktiles, mtiles, db ? 1 : 0))
+        return rc;
     const long long MK = (long long)M * K, n = MK + (db ? M : 0);
     // the partial stride is M*K + M whether or not the bias is reduced
-    wgrad_reduce_kernel<<<(unsigned)((n + kBwThreads - 1) / kBwThreads), kBwThreads, 0, st>>>(
-        scratch, (int)P, MK, MK + M, n, dW, db);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(wgrad_reduce_kernel, (unsigned)((n + kBwThreads - 1) / kBwThreads), kBwThreads, 0, st, scratch,
+                  (int)P, MK, MK + M, n, dW, db);
 }
 
 // ---------------------------------------------------------------------------
@@ -247,11 +246,10 @@ int launch_norm_bwd(const float* x, const NormIn& nin, const float* dp, float* o
     if (nin.stats && (!nin.gamma || !nin.beta)) return SDR_ERR_BAD_ARGUMENT;
     const long long rows = (long long)samples * C;
     if (rows > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-    norm_bwd_reduce_kernel<<<(unsigned)rows, kBwThreads, 0, st>>>(x, nin, dp, scratch, C, L);
-    if (cudaGetLastError() != cudaSuccess) return SDR_ERR_CUDA;
-    norm_bwd_apply_kernel<<<(unsigned)rows, kBwThreads, 0, st>>>(x, nin, dp, scratch, out, accumulate, g_gamma, g_beta,
-                                                                  g_slope, samples, C, L);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    if (const int rc = launch(norm_bwd_reduce_kernel, (unsigned)rows, kBwThreads, 0, st, x, nin, dp, scratch, C, L))
+        return rc;
+    return launch(norm_bwd_apply_kernel, (unsigned)rows, kBwThreads, 0, st, x, nin, dp, scratch, out, accumulate,
+                  g_gamma, g_beta, g_slope, samples, C, L);
 }
 
 // ---------------------------------------------------------------------------
@@ -331,13 +329,11 @@ int launch_dw_bwd(const float* dz, const float* x, const NormIn& nin, const floa
     if (nin.prelu_pc) return SDR_ERR_UNSUPPORTED;
     const long long rows = (long long)samples * C;
     if (rows > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-    dw_bwd_kernel<<<(unsigned)rows, kBwThreads, 0, st>>>(dz, x, nin, w5, pool, pool ? P : 0, din,
-                                                          dz ? scratch : nullptr, C, Lin, stride);
-    if (cudaGetLastError() != cudaSuccess) return SDR_ERR_CUDA;
-    if (!dz) return SDR_OK;
-    dw_finish_kernel<<<(unsigned)((C * 6 + kBwThreads - 1) / kBwThreads), kBwThreads, 0, st>>>(scratch, gw, gb,
-                                                                                              samples, C);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    const int rc = launch(dw_bwd_kernel, (unsigned)rows, kBwThreads, 0, st, dz, x, nin, w5, pool, pool ? P : 0, din,
+                          dz ? scratch : nullptr, C, Lin, stride);
+    if (rc != SDR_OK || !dz) return rc;
+    return launch(dw_finish_kernel, (unsigned)((C * 6 + kBwThreads - 1) / kBwThreads), kBwThreads, 0, st, scratch, gw,
+                  gb, samples, C);
 }
 
 // ---------------------------------------------------------------------------
@@ -376,18 +372,16 @@ mask_bwd_kernel(const float* __restrict__ mlog, const float* __restrict__ e, flo
 int launch_mask_apply(const float* mlog, const float* e, float* masked, int B, int S, int N, int L, cudaStream_t st) {
     if (!mlog || !e || !masked || B <= 0 || S <= 0 || N <= 0 || L <= 0) return SDR_ERR_BAD_ARGUMENT;
     const long long total = (long long)B * S * N * L;
-    mask_apply_kernel<<<(unsigned)((total + kBwThreads - 1) / kBwThreads), kBwThreads, 0, st>>>(mlog, e, masked, S, N,
-                                                                                               L, total);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(mask_apply_kernel, (unsigned)((total + kBwThreads - 1) / kBwThreads), kBwThreads, 0, st, mlog, e,
+                  masked, S, N, L, total);
 }
 
 int launch_mask_bwd(const float* mlog, const float* e, float* dmasked, float* de, int B, int S, int N, int L,
                     cudaStream_t st) {
     if (!mlog || !e || !dmasked || !de || B <= 0 || S <= 0 || N <= 0 || L <= 0) return SDR_ERR_BAD_ARGUMENT;
     const long long total = (long long)B * N * L;
-    mask_bwd_kernel<<<(unsigned)((total + kBwThreads - 1) / kBwThreads), kBwThreads, 0, st>>>(mlog, e, dmasked, de, S,
-                                                                                             N, L, total);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(mask_bwd_kernel, (unsigned)((total + kBwThreads - 1) / kBwThreads), kBwThreads, 0, st, mlog, e,
+                  dmasked, de, S, N, L, total);
 }
 
 // ---------------------------------------------------------------------------
@@ -411,8 +405,7 @@ int launch_frame_gather(const float* wav, float* frames, int B, int SA, int K, i
     const long long total = (long long)B * SA * K * L;
     const long long grid = (total + kBwThreads - 1) / kBwThreads;
     if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-    frame_gather_kernel<<<(unsigned)grid, kBwThreads, 0, st>>>(wav, frames, SA, K, L, T, total);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(frame_gather_kernel, (unsigned)grid, kBwThreads, 0, st, wav, frames, SA, K, L, T, total);
 }
 
 // ---------------------------------------------------------------------------
@@ -429,8 +422,7 @@ transpose_kernel(const float* __restrict__ w, float* __restrict__ wt, int R, int
 int launch_transpose(const float* w, float* wt, int R, int C, cudaStream_t st) {
     if (!w || !wt || R <= 0 || C <= 0) return SDR_ERR_BAD_ARGUMENT;
     const long long n = (long long)R * C;
-    transpose_kernel<<<(unsigned)((n + kBwThreads - 1) / kBwThreads), kBwThreads, 0, st>>>(w, wt, R, C);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(transpose_kernel, (unsigned)((n + kBwThreads - 1) / kBwThreads), kBwThreads, 0, st, w, wt, R, C);
 }
 
 }  // namespace sdr

@@ -563,12 +563,6 @@ size_t bss_eval_scratch_bytes(int B, int S, long long T, int F) {
     return BssScratch(nullptr, B, S, T, F).bytes;
 }
 
-template <class K>
-static int bss_smem(K kern, size_t bytes) {
-    return cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)bytes) == cudaSuccess
-        ? SDR_OK : SDR_ERR_CUDA;
-}
-
 template <int S, int NE>
 static int bss_eval_launch(const float* ref, const float* est, const float* mix, double* sdr, double* sir,
                            double* sar, int* perm, double* msdr, double* msir, double* msar, int B, long long T, int F,
@@ -580,18 +574,17 @@ static int bss_eval_launch(const float* ref, const float* est, const float* mix,
     const size_t solve_smem = sizeof(double) * (size_t)F * (2 * S * S + NE * S);
     const size_t energy_smem = sizeof(double) * (size_t)S * (kBssEnergyTile + F - 1 + 2 * F);
     int e;
-    if ((e = bss_smem(bss_corr_kernel<S, NE>, corr_smem))) return e;
-    if ((e = bss_smem(bss_solve_kernel<S, NE>, solve_smem))) return e;
-    if ((e = bss_smem(bss_energy_kernel<S, NE>, energy_smem))) return e;
-    bss_corr_kernel<S, NE><<<(unsigned)((long long)B * cc), kBssCorrTile, corr_smem, st>>>(ref, est, mix, s.part, T,
-                                                                                          F, cc);
-    bss_solve_kernel<S, NE><<<(unsigned)((long long)B * (S + 1)), 256, solve_smem, st>>>(s.part, cc, s.rj, s.rt,
-                                                                                         s.eref, s.cj, s.ct, F);
-    bss_energy_kernel<S, NE><<<(unsigned)((long long)B * ec), kBssEnergyTile, energy_smem, st>>>(
-        ref, est, mix, s.cj, s.ct, s.epart, T, F, ec);
-    bss_final_kernel<S, NE><<<item_blocks(B), 256, 0, st>>>(s.epart, s.eref, ec, sdr, sir, sar, perm, msdr, msir, msar,
-                                                             B, compute_permutation);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    if ((e = launch(bss_corr_kernel<S, NE>, (unsigned)((long long)B * cc), kBssCorrTile, corr_smem, st, ref, est, mix,
+                    s.part, T, F, cc)))
+        return e;
+    if ((e = launch(bss_solve_kernel<S, NE>, (unsigned)((long long)B * (S + 1)), 256, solve_smem, st, s.part, cc, s.rj,
+                    s.rt, s.eref, s.cj, s.ct, F)))
+        return e;
+    if ((e = launch(bss_energy_kernel<S, NE>, (unsigned)((long long)B * ec), kBssEnergyTile, energy_smem, st, ref, est,
+                    mix, s.cj, s.ct, s.epart, T, F, ec)))
+        return e;
+    return launch(bss_final_kernel<S, NE>, item_blocks(B), 256, 0, st, s.epart, s.eref, ec, sdr, sir, sar, perm, msdr,
+                  msir, msar, B, compute_permutation);
 }
 
 int launch_bss_eval(const float* ref, const float* est, const float* mix, double* sdr, double* sir, double* sar,

@@ -188,18 +188,13 @@ int launch_causal_pyramid(const float* y, const float* slope_in, const float* co
     }
     const size_t smem = cur * sizeof(float);
     if (smem > 200 * 1024) return SDR_ERR_UNSUPPORTED;
-    if (smem > 48 * 1024) {
-        if (cudaFuncSetAttribute(causal_pyramid_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-            return SDR_ERR_CUDA;
-    }
     const long long grid = (long long)samples * C * a.tiles;
     if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
     // block size: measured at the default model's rows (L = 3200, D = 4, one window per row, 6 CTAs per SM by shared
     // memory): 128 / 160 / 192 / 224 / 256 threads = 206 / 192 / 187 / 193 / 196 us; short windows take fewer threads
     int threads = 192;
     while (threads > 128 && (a.W >> 2) < threads) threads -= 32;
-    causal_pyramid_kernel<<<(unsigned)grid, threads, smem, st>>>(a);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(causal_pyramid_kernel, (unsigned)grid, threads, smem, st, a);
 }
 
 // ---------------------------------------------------------------------------
@@ -224,13 +219,11 @@ __global__ void scale_by_scalar_kernel(const float* __restrict__ src, const floa
 
 int launch_take_taps(const float* src, float* dst, long long rows, int src_taps, int dst_taps, cudaStream_t st) {
     const long long n = rows * dst_taps;
-    take_taps_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(src, dst, rows, src_taps, dst_taps);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(take_taps_kernel, (unsigned)((n + 255) / 256), 256, 0, st, src, dst, rows, src_taps, dst_taps);
 }
 
 int launch_scale_by_scalar(const float* src, const float* gain, float* dst, long long n, cudaStream_t st) {
-    scale_by_scalar_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(src, gain, dst, n);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(scale_by_scalar_kernel, (unsigned)((n + 255) / 256), 256, 0, st, src, gain, dst, n);
 }
 
 }  // namespace sdr

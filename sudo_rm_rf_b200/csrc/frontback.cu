@@ -101,17 +101,12 @@ int launch_encoder(const float* wav, const float* weight, const float* bias, int
                    int B, int A, long long T, int N, int K, int L, int pad, cudaStream_t st) {
     if (B <= 0 || A <= 0 || T <= 0 || N <= 0 || K < 3 || L <= 0) return SDR_ERR_BAD_ARGUMENT;
     if (!encoder_ffma_fits(A, K)) return SDR_ERR_UNSUPPORTED;
-    const size_t smem = encoder_smem_bytes(A, K);
-    if (smem > 48 * 1024) {
-        cudaError_t e = cudaFuncSetAttribute(encoder_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
-        if (e != cudaSuccess) return SDR_ERR_CUDA;
-    }
     const int t_tiles = (L + kEncThreads - 1) / kEncThreads;
     const long long gx = (long long)t_tiles * B;
     if (gx > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
     dim3 grid((unsigned)gx, (unsigned)((N + kEncNB - 1) / kEncNB));
-    encoder_kernel<<<grid, kEncThreads, smem, st>>>(wav, weight, bias, enc, stats, A, T, N, K, L, t_tiles, pad, relu);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(encoder_kernel, grid, kEncThreads, encoder_smem_bytes(A, K), st, wav, weight, bias, enc, stats, A, T,
+                  N, K, L, t_tiles, pad, relu);
 }
 
 // ---------------------------------------------------------------------------
@@ -160,8 +155,7 @@ int launch_overlap_add(const float* frames, const float* mix, const float* bias,
     if (B <= 0 || SA <= 0 || K < 3 || L <= 0 || T <= 0) return SDR_ERR_BAD_ARGUMENT;
     if (SA > kMaxSrc) return SDR_ERR_UNSUPPORTED;
     dim3 grid((unsigned)((T + 255) / 256), (unsigned)(B < 65535 ? B : 65535));
-    overlap_add_kernel<<<grid, 256, 0, st>>>(frames, mix, bias, rescale, out, B, SA, K, L, T);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(overlap_add_kernel, grid, 256, 0, st, frames, mix, bias, rescale, out, B, SA, K, L, T);
 }
 
 // ---------------------------------------------------------------------------
@@ -228,16 +222,17 @@ int launch_mixture_consistency(const float* est, const float* mix, float* out, i
         if (!scratch) return SDR_ERR_BAD_ARGUMENT;
         power = static_cast<double*>(scratch);
         const int rows = B * S;
-        if (cudaMemsetAsync(power, 0, sizeof(double) * rows, st) != cudaSuccess) return SDR_ERR_CUDA;
+        if (const int rc = cuda_status(cudaMemsetAsync(power, 0, sizeof(double) * rows, st))) return rc;
         int gx = (int)((T + 256 * 8 - 1) / (256 * 8));
         if (gx < 1) gx = 1;
-        mc_power_kernel<<<dim3((unsigned)gx, (unsigned)(rows < 65535 ? rows : 65535)), 256, 0, st>>>(est, power, rows, T);
+        if (const int rc = launch(mc_power_kernel, dim3((unsigned)gx, (unsigned)(rows < 65535 ? rows : 65535)), 256, 0,
+                                  st, est, power, rows, T))
+            return rc;
     } else if (weights_type != 0) {
         return SDR_ERR_BAD_ARGUMENT;
     }
     dim3 grid((unsigned)((T + 255) / 256), (unsigned)(B < 65535 ? B : 65535));
-    mc_apply_kernel<<<grid, 256, 0, st>>>(est, mix, power, out, B, S, T);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(mc_apply_kernel, grid, 256, 0, st, est, mix, power, out, B, S, T);
 }
 
 // ---------------------------------------------------------------------------
@@ -356,13 +351,16 @@ int launch_mixture_consistency_backward(const float* est, const float* mix, cons
         if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
         double2* part = static_cast<double2*>(scratch);
         coef = part + (size_t)grid;
-        mc_bwd_partials_kernel<<<(unsigned)grid, 256, 0, st>>>(est, mix, grad_out, part, S, T, chunks);
+        if (const int rc = launch(mc_bwd_partials_kernel, (unsigned)grid, 256, 0, st, est, mix, grad_out, part, S, T,
+                                  chunks))
+            return rc;
         const long long cb = (B + 255) / 256;
-        mc_bwd_coef_kernel<<<(unsigned)(cb < 4096 ? cb : 4096), 256, 0, st>>>(part, coef, B, S, T, chunks);
+        if (const int rc = launch(mc_bwd_coef_kernel, (unsigned)(cb < 4096 ? cb : 4096), 256, 0, st, part, coef, B, S,
+                                  T, chunks))
+            return rc;
     }
     dim3 grid((unsigned)((T + 255) / 256), (unsigned)(B < 65535 ? B : 65535));
-    mc_bwd_apply_kernel<<<grid, 256, 0, st>>>(est, grad_out, coef, grad_est, grad_mix, B, S, T);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(mc_bwd_apply_kernel, grid, 256, 0, st, est, grad_out, coef, grad_est, grad_mix, B, S, T);
 }
 
 }  // namespace sdr

@@ -1,8 +1,9 @@
 // The host launchers and eligibility predicates that api.cu calls, by defining file.  api.cu and every file that
 // defines one of them include this header, so a definition that drifts from its declaration is a compile or link
-// error (the library is linked with undefined symbols refused) instead of a failure at load time.
+// error (the library is linked with undefined symbols refused) instead of a failure at load time.  Every launcher
+// enqueues its kernels through launch.cuh.
 #pragma once
-#include "common.cuh"
+#include "launch.cuh"
 
 namespace sdr {
 

@@ -421,27 +421,24 @@ int launch_depthwise(const float* x, const NormIn& nin, const float* w5, const f
         const long long grid = (long long)chunks * samples;
         if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
         const bool act = nin.prelu != nullptr;
-#define SDR_DW(S, A) dw5_wide_kernel<S, A><<<(unsigned)grid, kDw8Threads, 0, st>>>(x, nin, w5, bias, y, stats_out, C, Lin, Lout, chunks)
-        if (stride == 1) { if (act) SDR_DW(1, true); else SDR_DW(1, false); }
-        else             { if (act) SDR_DW(2, true); else SDR_DW(2, false); }
-#undef SDR_DW
+        const auto kern = stride == 1 ? (act ? dw5_wide_kernel<1, true> : dw5_wide_kernel<1, false>)
+                                      : (act ? dw5_wide_kernel<2, true> : dw5_wide_kernel<2, false>);
+        return launch(kern, (unsigned)grid, kDw8Threads, 0, st, x, nin, w5, bias, y, stats_out, C, Lin, Lout, chunks);
     } else if (vec) {
         const long long items = (long long)C * (Lout / 4);
         const int chunks = (int)((items + kDwThreads * kDwItems - 1) / (kDwThreads * kDwItems));
         const long long grid = (long long)chunks * samples;
         if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-        if (stride == 1)
-            dw5_vec_kernel<1><<<(unsigned)grid, kDwThreads, 0, st>>>(x, nin, w5, bias, y, stats_out, C, Lin, Lout, chunks);
-        else
-            dw5_vec_kernel<2><<<(unsigned)grid, kDwThreads, 0, st>>>(x, nin, w5, bias, y, stats_out, C, Lin, Lout, chunks);
+        return launch(stride == 1 ? dw5_vec_kernel<1> : dw5_vec_kernel<2>, (unsigned)grid, kDwThreads, 0, st, x, nin,
+                      w5, bias, y, stats_out, C, Lin, Lout, chunks);
     } else {
         const long long items = (long long)C * Lout;
         const int chunks = (int)((items + kDwThreads * 4 - 1) / (kDwThreads * 4));
         const long long grid = (long long)chunks * samples;
         if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-        dw5_scalar_kernel<<<(unsigned)grid, kDwThreads, 0, st>>>(x, nin, w5, bias, y, stats_out, C, Lin, Lout, stride, chunks);
+        return launch(dw5_scalar_kernel, (unsigned)grid, kDwThreads, 0, st, x, nin, w5, bias, y, stats_out, C, Lin,
+                      Lout, stride, chunks);
     }
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
 }
 
 int launch_merge(const float* const* z, const NormIn* nins, int depth, float* m, double* stats_out,
@@ -465,21 +462,20 @@ int launch_merge(const float* const* z, const NormIn* nins, int depth, float* m,
         const int chunks = (int)((items + per_cta - 1) / per_cta);
         const long long grid = (long long)chunks * samples;
         if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-        merge_wide_kernel<<<(unsigned)grid, kMg16Threads, 0, st>>>(a, m, stats_out, C, L, chunks);
+        return launch(merge_wide_kernel, (unsigned)grid, kMg16Threads, 0, st, a, m, stats_out, C, L, chunks);
     } else if (vec) {
         const long long items = (long long)C * (L / 4);
         const int chunks = (int)((items + kMgThreads * kMgItems - 1) / (kMgThreads * kMgItems));
         const long long grid = (long long)chunks * samples;
         if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-        merge_vec_kernel<<<(unsigned)grid, kMgThreads, 0, st>>>(a, m, stats_out, C, L, chunks);
+        return launch(merge_vec_kernel, (unsigned)grid, kMgThreads, 0, st, a, m, stats_out, C, L, chunks);
     } else {
         const long long items = (long long)C * L;
         const int chunks = (int)((items + kMgThreads * 4 - 1) / (kMgThreads * 4));
         const long long grid = (long long)chunks * samples;
         if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-        merge_scalar_kernel<<<(unsigned)grid, kMgThreads, 0, st>>>(a, m, stats_out, C, L, chunks);
+        return launch(merge_scalar_kernel, (unsigned)grid, kMgThreads, 0, st, a, m, stats_out, C, L, chunks);
     }
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
 }
 
 }  // namespace sdr

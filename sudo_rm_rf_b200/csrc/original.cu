@@ -76,9 +76,8 @@ int launch_residual_norm(const float* e, const NormIn& fe, float* x, const NormI
     const long long chunks = (items + per_cta - 1) / per_cta;
     const long long grid = chunks * samples;
     if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-    if (vec) residual_norm_kernel<true><<<(unsigned)grid, kRnThreads, 0, st>>>(e, fe, x, fx, stats_out, C, L, (int)chunks);
-    else     residual_norm_kernel<false><<<(unsigned)grid, kRnThreads, 0, st>>>(e, fe, x, fx, stats_out, C, L, (int)chunks);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(vec ? residual_norm_kernel<true> : residual_norm_kernel<false>, (unsigned)grid, kRnThreads, 0, st, e,
+                  fe, x, fx, stats_out, C, L, (int)chunks);
 }
 
 // ---------------------------------------------------------------------------
@@ -161,13 +160,12 @@ softmax_gate_kernel(const float* logits, const float* __restrict__ enc, float* o
 }
 
 template <bool VEC>
-static void launch_sg(dim3 grid, const float* logits, const float* enc, float* out, int B, int S, long long NL,
-                      cudaStream_t st) {
+static auto softmax_gate_for(int S) {
     switch (S) {
-        case 2: softmax_gate_kernel<VEC, 2><<<grid, 256, 0, st>>>(logits, enc, out, B, S, NL); break;
-        case 3: softmax_gate_kernel<VEC, 3><<<grid, 256, 0, st>>>(logits, enc, out, B, S, NL); break;
-        case 4: softmax_gate_kernel<VEC, 4><<<grid, 256, 0, st>>>(logits, enc, out, B, S, NL); break;
-        default: softmax_gate_kernel<VEC, 0><<<grid, 256, 0, st>>>(logits, enc, out, B, S, NL); break;
+        case 2: return softmax_gate_kernel<VEC, 2>;
+        case 3: return softmax_gate_kernel<VEC, 3>;
+        case 4: return softmax_gate_kernel<VEC, 4>;
+        default: return softmax_gate_kernel<VEC, 0>;
     }
 }
 
@@ -181,9 +179,8 @@ int launch_softmax_gate(const float* logits, const float* enc, float* out, int B
     const long long gx = (threads + 255) / 256;
     if (gx > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
     dim3 grid((unsigned)gx, (unsigned)(B < 65535 ? B : 65535));
-    if (vec) launch_sg<true>(grid, logits, enc, out, B, S, NL, st);
-    else     launch_sg<false>(grid, logits, enc, out, B, S, NL, st);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(vec ? softmax_gate_for<true>(S) : softmax_gate_for<false>(S), grid, 256, 0, st, logits, enc, out, B,
+                  S, NL);
 }
 
 // ---------------------------------------------------------------------------
@@ -208,8 +205,7 @@ __global__ void toeplitz_mask_kernel(const float* __restrict__ w, const float* _
 int launch_toeplitz_mask(const float* w, const float* bias, float* W, float* brow, int S, int N, cudaStream_t st) {
     if (!w || !bias || !W || !brow || S <= 0 || N <= 0) return SDR_ERR_BAD_ARGUMENT;
     const long long total = (long long)S * N * N;
-    toeplitz_mask_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(w, bias, W, brow, S, N);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(toeplitz_mask_kernel, (unsigned)((total + 255) / 256), 256, 0, st, w, bias, W, brow, S, N);
 }
 
 // decoder = nn.ConvTranspose1d(S*N, S, K, groups=S) (sudormrf.py:245-252): weight [S*N][1][K]; source s only sees its
@@ -228,8 +224,7 @@ __global__ void grouped_decoder_kernel(const float* __restrict__ w, float* __res
 int launch_grouped_decoder(const float* w, float* wt, int S, int N, int K, cudaStream_t st) {
     if (!w || !wt || S <= 0 || N <= 0 || K <= 0) return SDR_ERR_BAD_ARGUMENT;
     const long long total = (long long)S * N * S * K;
-    grouped_decoder_kernel<<<(unsigned)((total + 255) / 256), 256, 0, st>>>(w, wt, S, N, K);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(grouped_decoder_kernel, (unsigned)((total + 255) / 256), 256, 0, st, w, wt, S, N, K);
 }
 
 }  // namespace sdr

@@ -529,16 +529,8 @@ static int launch_tile(const PwArgs& a, int samples, int threads, cudaStream_t s
     if (gx > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
     const int rows = PRE ? 2 * a.K : a.K;
     const size_t smem = (size_t)rows * P * sizeof(float);
-    auto go = [&](auto kern) -> int {
-        if (smem > 40 * 1024 &&
-            cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) {
-            cudaGetLastError();
-            return SDR_ERR_CUDA;
-        }
-        kern<<<(unsigned)gx, threads, smem, st>>>(a, tiles, P);
-        return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
-    };
-    return a.M <= 16 ? go(pw_tile_kernel<PRE, 16>) : go(pw_tile_kernel<PRE, 32>);
+    return launch(a.M <= 16 ? pw_tile_kernel<PRE, 16> : pw_tile_kernel<PRE, 32>, (unsigned)gx, threads, smem, st, a,
+                  tiles, P);
 }
 
 // block size for rows of `quads` position quads: the multiple of 32 in [128, 256] that wastes the fewest threads
@@ -557,10 +549,8 @@ static int launch_bm(const PwArgs& a, int samples, bool vec, cudaStream_t st) {
     const long long gx = (long long)a.l_tiles * samples;
     const int gy = (a.M + BM - 1) / BM;
     if (gx > 0x7fffffffLL || gy > 65535) return SDR_ERR_UNSUPPORTED;
-    dim3 grid((unsigned)gx, (unsigned)gy);
-    if (vec) pw_gemm_kernel<BM, true><<<grid, kPwThreads, 0, st>>>(a);
-    else     pw_gemm_kernel<BM, false><<<grid, kPwThreads, 0, st>>>(a);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(vec ? pw_gemm_kernel<BM, true> : pw_gemm_kernel<BM, false>, dim3((unsigned)gx, (unsigned)gy),
+                  kPwThreads, 0, st, a);
 }
 
 int launch_pointwise_ffma(const float* x, const NormIn& nin, const float* W, const float* bias,
@@ -586,8 +576,7 @@ int launch_pointwise_ffma(const float* x, const NormIn& nin, const float* W, con
         const long long gx = (long long)chunks * samples;
         if (gx > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
         dim3 grid((unsigned)gx, (unsigned)((M + kSmMT - 1) / kSmMT));
-        pw_small_kernel<false><<<grid, threads, 0, st>>>(a, chunks);
-        return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+        return launch(pw_small_kernel<false>, grid, threads, 0, st, a, chunks);
     }
     if (M > 64) return launch_bm<128>(a, samples, vec, st);
     if (M > 32) return launch_bm<64>(a, samples, vec, st);
@@ -621,8 +610,7 @@ int launch_pointwise_small_preadd(const float* x, const float* pre_add, const No
     const long long gx = (long long)chunks * samples;
     if (gx > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
     dim3 grid((unsigned)gx, (unsigned)((M + kSmMT - 1) / kSmMT));
-    pw_small_kernel<true><<<grid, threads, 0, st>>>(a, chunks);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(pw_small_kernel<true>, grid, threads, 0, st, a, chunks);
 }
 
 }  // namespace sdr

@@ -30,8 +30,6 @@
 #include <cstdio>
 #include <cstdlib>
 #include <cstring>
-#include <mutex>
-#include <vector>
 #include <cuda.h>
 #include <cuda_bf16.h>
 #include "common.cuh"
@@ -606,9 +604,8 @@ int pack_pointwise_mma(const float* W, int M, int K, void* packed, cudaStream_t 
     if (!pointwise_mma_eligible(M, K)) return SDR_ERR_UNSUPPORTED;
     const int Mpad = mma_pad_m(M);
     const long long chunks = (long long)Mpad * K / 8;
-    pack_weight_mma_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, st>>>(
-        W, static_cast<uint8_t*>(packed), M, Mpad, K, K);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(pack_weight_mma_kernel, (unsigned)((chunks + 255) / 256), 256, 0, st, W,
+                  static_cast<uint8_t*>(packed), M, Mpad, K, K);
 }
 
 constexpr size_t kMmaSmemBytes = 1024 + (size_t)kRawStages * kRawStageBytes + (size_t)kStages * kBStageBytes +
@@ -625,7 +622,7 @@ static EncodeTiledFn encode_tiled_fn() {
     static EncodeTiledFn fn = [] {
         void* ptr = nullptr;
         cudaDriverEntryPointQueryResult qres = cudaDriverEntryPointSymbolNotFound;
-        if (cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres) != cudaSuccess ||
+        if (cuda_status(cudaGetDriverEntryPoint("cuTensorMapEncodeTiled", &ptr, cudaEnableDefault, &qres)) ||
             qres != cudaDriverEntryPointSuccess)
             ptr = nullptr;
         return reinterpret_cast<EncodeTiledFn>(ptr);
@@ -668,34 +665,13 @@ static int make_act_map(CUtensorMap* tm, const float* x, int samples, int C, int
 static_assert(kBlockK == 64 && kTileN == 2 * 64, "activation boxes are 64 channels: one k-block, half a channel tile");
 
 // Persistent launch: one CTA per SM (the shared-memory footprint allows no second), never more than there are tiles.
-// (All instantiations share one function-pointer type, so the per-kernel state is keyed by the pointer, not by Kern.)
-struct MmaLaunchInfo { const void* fn; int dev; int sms; };
-static std::mutex g_launch_mutex;
-static std::vector<MmaLaunchInfo> g_launch_info;
-
 template <typename Kern>
 static int launch_persistent(Kern kern, const MmaArgs& a, const CUtensorMap& wmap, const CUtensorMap& xmap,
                              const CUtensorMap& emap, const CUtensorMap& ymap, cudaStream_t st) {
-    int dev = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess) return SDR_ERR_CUDA;
-    int sms = 0;
-    {
-        std::lock_guard<std::mutex> lock(g_launch_mutex);
-        for (const MmaLaunchInfo& e : g_launch_info)
-            if (e.fn == reinterpret_cast<const void*>(kern) && e.dev == dev) { sms = e.sms; break; }
-        if (sms == 0) {                           // first launch of this kernel on this device
-            if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMmaSmemBytes) != cudaSuccess) {
-                cudaGetLastError();
-                return SDR_ERR_CUDA;
-            }
-            if (cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess || sms <= 0) return SDR_ERR_CUDA;
-            g_launch_info.push_back(MmaLaunchInfo{reinterpret_cast<const void*>(kern), dev, sms});
-        }
-    }
-    const int grid = a.num_tiles < sms ? a.num_tiles : sms;
-    kern<<<grid, kMmaThreads, kMmaSmemBytes, st>>>(a, wmap, xmap, emap, ymap);
-    if (cudaGetLastError() != cudaSuccess) return SDR_ERR_CUDA;
-    return SDR_OK;
+    const int sms = sm_count();
+    if (sms <= 0) return SDR_ERR_CUDA;
+    return launch(kern, a.num_tiles < sms ? a.num_tiles : sms, kMmaThreads, kMmaSmemBytes, st, a, wmap, xmap, emap,
+                  ymap);
 }
 
 int launch_pointwise_mma(const float* x, const NormIn& nin, const void* wpk, const float* bias,
@@ -758,9 +734,8 @@ int pack_encoder_mma(const float* W, int N, int A, int Kk, void* packed, cudaStr
     if (!encoder_mma_packed_bytes(N, A, Kk)) return SDR_ERR_UNSUPPORTED;
     const int Mpad = mma_pad_m(N), K = enc_kpad(A, Kk);
     const long long chunks = (long long)Mpad * K / 8;
-    pack_weight_mma_kernel<<<(unsigned)((chunks + 255) / 256), 256, 0, st>>>(
-        W, static_cast<uint8_t*>(packed), N, Mpad, A * Kk, K);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(pack_weight_mma_kernel, (unsigned)((chunks + 255) / 256), 256, 0, st, W,
+                  static_cast<uint8_t*>(packed), N, Mpad, A * Kk, K);
 }
 
 int launch_encoder_mma(const float* wav, const void* wpk, const float* bias, int relu, float* enc, double* stats,

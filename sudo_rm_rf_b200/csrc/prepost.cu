@@ -85,22 +85,20 @@ normalize_rows_kernel(const float* __restrict__ x, const float2* __restrict__ ms
 int launch_utterance_stats(const float* wav, double* sums, float2* mean_std, int rows, long long T,
                            const long long* lengths, cudaStream_t st) {
     if (!wav || !sums || !mean_std || rows <= 0 || T <= 0) return SDR_ERR_BAD_ARGUMENT;
-    if (cudaMemsetAsync(sums, 0, sizeof(double) * 2 * rows, st) != cudaSuccess) return SDR_ERR_CUDA;
+    if (const int rc = cuda_status(cudaMemsetAsync(sums, 0, sizeof(double) * 2 * rows, st))) return rc;
     int chunks = (int)((T + 8191) / 8192);
     if (chunks < 1) chunks = 1;
     if (chunks > 64) chunks = 64;
     const long long grid = (long long)rows * chunks;
     if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-    row_moments_kernel<<<(unsigned)grid, 256, 0, st>>>(wav, sums, T, chunks, lengths);
-    row_mean_std_kernel<<<(rows + 127) / 128, 128, 0, st>>>(sums, mean_std, rows, T, lengths);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    if (const int rc = launch(row_moments_kernel, (unsigned)grid, 256, 0, st, wav, sums, T, chunks, lengths)) return rc;
+    return launch(row_mean_std_kernel, (rows + 127) / 128, 128, 0, st, sums, mean_std, rows, T, lengths);
 }
 
 int launch_normalize_rows(const float* wav, const float2* mean_std, float* out, int rows, long long T,
                           const long long* lengths, cudaStream_t st) {
     if (!wav || !mean_std || !out || rows <= 0 || T <= 0) return SDR_ERR_BAD_ARGUMENT;
-    normalize_rows_kernel<<<row_tiled_grid(rows, T), 256, 0, st>>>(wav, mean_std, out, rows, T, lengths);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(normalize_rows_kernel, row_tiled_grid(rows, T), 256, 0, st, wav, mean_std, out, rows, T, lengths);
 }
 
 // ---------------------------------------------------------------------------
@@ -192,12 +190,12 @@ gram_kernel(const float* __restrict__ est, const float* __restrict__ tgt, const 
 template <class L, bool kOrdered>
 static int launch_gram(const float* est, const float* tgt, const float* extra, int rows, int B, long long T,
                        double* acc, cudaStream_t st) {
-    if (!kOrdered && cudaMemsetAsync(acc, 0, sizeof(double) * L::N * B, st) != cudaSuccess) return SDR_ERR_CUDA;
+    if (!kOrdered)
+        if (const int rc = cuda_status(cudaMemsetAsync(acc, 0, sizeof(double) * L::N * B, st))) return rc;
     const int chunks = gram_chunks(T);
     const long long grid = (long long)B * chunks;
     if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-    gram_kernel<L, kOrdered><<<(unsigned)grid, 256, 0, st>>>(est, tgt, extra, acc, T, chunks, rows);
-    return SDR_OK;
+    return launch(gram_kernel<L, kOrdered>, (unsigned)grid, 256, 0, st, est, tgt, extra, acc, T, chunks, rows);
 }
 
 // A mean-removed energy sum(x^2) - n * mean^2 can round to a few ulp below zero (a constant row under zero_mean);
@@ -313,8 +311,7 @@ int launch_pit_sisdr(const float* est, const float* tgt, const float* mix, float
     return with_sources(S, [&](auto s) {
         constexpr int n = decltype(s)::value;
         if (const int e = launch_gram<GramLayout<n, n, false, true>, false>(est, tgt, mix, n, B, T, acc, st)) return e;
-        pit_finalize_kernel<n><<<1, 256, 0, st>>>(acc, best, perm, B, T, zero_mean, improvement, eps);
-        return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+        return launch(pit_finalize_kernel<n>, 1, 256, 0, st, acc, best, perm, B, T, zero_mean, improvement, eps);
     });
 }
 
@@ -395,9 +392,8 @@ int launch_pairwise_neg_sdr(const float* est, const float* tgt, float* out, int 
         constexpr int n = decltype(s)::value;
         if (const int e = launch_gram<GramLayout<n, n, false, false>, false>(est, tgt, nullptr, n, B, T, acc, st))
             return e;
-        pairwise_finalize_kernel<n, false><<<item_blocks(B), 256, 0, st>>>(acc, 1, out, nullptr, B, T, sdr_type,
-                                                                          zero_mean, take_log);
-        return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+        return launch(pairwise_finalize_kernel<n, false>, item_blocks(B), 256, 0, st, acc, 1, out, nullptr, B, T,
+                      sdr_type, zero_mean, take_log);
     });
 }
 
@@ -418,9 +414,8 @@ int launch_pairwise_neg_sdr_train(const float* est, const float* tgt, float* out
         constexpr int n = decltype(s)::value;
         if (const int e = launch_gram<GramLayout<n, n, true, false>, true>(est, tgt, nullptr, n, B, T, part, st))
             return e;
-        pairwise_finalize_kernel<n, true><<<item_blocks(B), 256, 0, st>>>(
-            part, gram_chunks(T), out, static_cast<double*>(coef), B, T, sdr_type, zero_mean, take_log);
-        return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+        return launch(pairwise_finalize_kernel<n, true>, item_blocks(B), 256, 0, st, part, gram_chunks(T), out,
+                      static_cast<double*>(coef), B, T, sdr_type, zero_mean, take_log);
     });
 }
 
@@ -468,9 +463,8 @@ int launch_pairwise_neg_sdr_backward(const float* est, const float* tgt, const v
     if (!est || !tgt || !coef || !grad_out || !grad || B <= 0 || T <= 0) return SDR_ERR_BAD_ARGUMENT;
     return with_sources(S, [&](auto s) {
         constexpr int n = decltype(s)::value;
-        pairwise_backward_kernel<n><<<row_tiled_grid((long long)B * n, T), 256, 0, st>>>(
-            est, tgt, static_cast<const double*>(coef), grad_out, grad, B, T);
-        return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+        return launch(pairwise_backward_kernel<n>, row_tiled_grid((long long)B * n, T), 256, 0, st, est, tgt,
+                      static_cast<const double*>(coef), grad_out, grad, B, T);
     });
 }
 
@@ -549,8 +543,8 @@ int launch_stabilized_sisdr(const float* est, const float* tgt, float* best, int
                 if (const int e = launch_gram<GramLayout<E, A, true, false>, false>(est, tgt, nullptr, rows, B, T,
                                                                                    acc, st))
                     return e;
-                stab_finalize_kernel<E, A><<<1, 256, 0, st>>>(acc, best, perm, B, T, zero_mean, improvement, eps);
-                return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+                return launch(stab_finalize_kernel<E, A>, 1, 256, 0, st, acc, best, perm, B, T, zero_mean, improvement,
+                              eps);
             }
         });
     });
@@ -645,9 +639,8 @@ int launch_snr_zero_refs(const float* est, const float* tgt, float* value, int* 
         constexpr int n = decltype(s)::value;
         if (const int e = launch_gram<GramLayout<n, n, true, false>, true>(est, tgt, nullptr, n, B, T, part, st))
             return e;
-        snr_zero_refs_finalize_kernel<n><<<item_blocks(B), 256, 0, st>>>(
-            part, gram_chunks(T), value, perm, static_cast<double*>(coef), B, T, zero_mean, threshold, eps);
-        return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+        return launch(snr_zero_refs_finalize_kernel<n>, item_blocks(B), 256, 0, st, part, gram_chunks(T), value, perm,
+                      static_cast<double*>(coef), B, T, zero_mean, threshold, eps);
     });
 }
 
@@ -677,9 +670,8 @@ int launch_snr_zero_refs_backward(const float* est, const float* tgt, const void
                                   float* grad, int B, int S, long long T, long long Tg, cudaStream_t st) {
     if (!est || !tgt || !coef || !grad_value || !grad || B <= 0 || T <= 0 || Tg < T) return SDR_ERR_BAD_ARGUMENT;
     if (S < 1 || S > 4) return SDR_ERR_UNSUPPORTED;
-    snr_zero_refs_backward_kernel<<<row_tiled_grid((long long)B * S, Tg), 256, 0, st>>>(
-        est, tgt, static_cast<const double*>(coef), grad_value, grad, B, S, T, Tg);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(snr_zero_refs_backward_kernel, row_tiled_grid((long long)B * S, Tg), 256, 0, st, est, tgt,
+                  static_cast<const double*>(coef), grad_value, grad, B, S, T, Tg);
 }
 
 }  // namespace sdr

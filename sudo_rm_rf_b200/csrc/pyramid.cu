@@ -726,19 +726,16 @@ template <typename K>
 static int launch_pyramid_pass(K kern, const PyrArgs& a, int samples, cudaStream_t st) {
     const int threads = 32 * pyramid_windows(a.D, a.L);
     const size_t smem = (2 * (size_t)(a.L + 8)) * sizeof(float) + (size_t)samples * sizeof(float2);
-    int dev = 0, sms = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess ||
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return SDR_ERR_CUDA;
-    if (cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess) return SDR_ERR_CUDA;
+    const int sms = sm_count();
+    if (sms <= 0) return SDR_ERR_CUDA;
+    // the occupancy query finds no resident CTA when smem exceeds the kernel's limit, so the opt-in comes first
+    if (const int rc = allow_dynamic_smem(reinterpret_cast<const void*>(kern), smem)) return rc;
     int per_sm = 0;
-    if (cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem) != cudaSuccess || per_sm < 1) {
-        cudaGetLastError();
+    if (cuda_status(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, threads, smem)) || per_sm < 1)
         per_sm = 1;
-    }
     long long grid = (long long)sms * per_sm;
     if (grid > a.rows) grid = a.rows;
-    kern<<<(unsigned)grid, threads, smem, st>>>(a);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(kern, (unsigned)grid, threads, smem, st, a);
 }
 
 // y [samples][C][L] -> z[0] = z_0, z[d] = R_d, table (merge coefficients).  stats0: zeroed slot for the statistics of z_0.
@@ -751,23 +748,22 @@ int launch_pyramid(const float* y, const NormIn& nin, const float* const* w5, co
     int rc = pyramid_args(y, nin, w5, bias, gamma, beta, z, stats0, rowstats, table, D, samples, C, L, a, s);
     if (rc != SDR_OK) return rc;
     const int threads = 32 * pyramid_windows(D, L);
-    auto launch = [&](auto kern) -> int { return launch_pyramid_pass(kern, a, samples, st); };
+    auto pass = [&](auto kern) -> int { return launch_pyramid_pass(kern, a, samples, st); };
     if (nin.prelu && nin.prelu_pc) {
         if (threads <= 256)
-            rc = D == 4 ? launch(dw_pyramid_kernel<4, 256, kPyrMinB, true>)
-                        : (D == 5 ? launch(dw_pyramid_kernel<5, 256, kPyrMinB, true>) : launch(dw_pyramid_kernel<6, 256, kPyrMinB, true>));
+            rc = D == 4 ? pass(dw_pyramid_kernel<4, 256, kPyrMinB, true>)
+                        : (D == 5 ? pass(dw_pyramid_kernel<5, 256, kPyrMinB, true>) : pass(dw_pyramid_kernel<6, 256, kPyrMinB, true>));
         else
-            rc = D == 4 ? launch(dw_pyramid_kernel<4, 1024, 1, true>)
-                        : (D == 5 ? launch(dw_pyramid_kernel<5, 1024, 1, true>) : launch(dw_pyramid_kernel<6, 1024, 1, true>));
+            rc = D == 4 ? pass(dw_pyramid_kernel<4, 1024, 1, true>)
+                        : (D == 5 ? pass(dw_pyramid_kernel<5, 1024, 1, true>) : pass(dw_pyramid_kernel<6, 1024, 1, true>));
     } else if (threads <= 256)      // rows up to 7-8 windows (L <= 3712 / 3328): compiled for several resident CTAs per SM
-        rc = D == 4 ? launch(dw_pyramid_kernel<4, 256, kPyrMinB, false>)
-                    : (D == 5 ? launch(dw_pyramid_kernel<5, 256, kPyrMinB, false>) : launch(dw_pyramid_kernel<6, 256, kPyrMinB, false>));
+        rc = D == 4 ? pass(dw_pyramid_kernel<4, 256, kPyrMinB, false>)
+                    : (D == 5 ? pass(dw_pyramid_kernel<5, 256, kPyrMinB, false>) : pass(dw_pyramid_kernel<6, 256, kPyrMinB, false>));
     else
-        rc = D == 4 ? launch(dw_pyramid_kernel<4, 1024, 1, false>)
-                    : (D == 5 ? launch(dw_pyramid_kernel<5, 1024, 1, false>) : launch(dw_pyramid_kernel<6, 1024, 1, false>));
+        rc = D == 4 ? pass(dw_pyramid_kernel<4, 1024, 1, false>)
+                    : (D == 5 ? pass(dw_pyramid_kernel<5, 1024, 1, false>) : pass(dw_pyramid_kernel<6, 1024, 1, false>));
     if (rc != SDR_OK) return rc;
-    pyramid_solve_kernel<<<(unsigned)samples, kSolveThreads, 0, st>>>(s);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(pyramid_solve_kernel, (unsigned)samples, kSolveThreads, 0, st, s);
 }
 
 // One pass of the fused stage (M = kPyrStats or kPyrMerge), with the instantiation the row length and slope call for.
@@ -775,19 +771,19 @@ template <int M>
 static int launch_fused_pass(const PyrArgs& a, bool pc, int samples, cudaStream_t st) {
     constexpr int MB = M == kPyrMerge ? kPyrMergeMinB : kPyrStatsMinB;
     const int D = a.D, threads = 32 * pyramid_windows(a.D, a.L);
-    auto launch = [&](auto kern) -> int { return launch_pyramid_pass(kern, a, samples, st); };
+    auto pass = [&](auto kern) -> int { return launch_pyramid_pass(kern, a, samples, st); };
     if (pc) {
         if (threads <= 256)
-            return D == 4 ? launch(dw_pyramid_kernel<4, 256, MB, true, M>)
-                          : (D == 5 ? launch(dw_pyramid_kernel<5, 256, MB, true, M>) : launch(dw_pyramid_kernel<6, 256, MB, true, M>));
-        return D == 4 ? launch(dw_pyramid_kernel<4, 1024, 1, true, M>)
-                      : (D == 5 ? launch(dw_pyramid_kernel<5, 1024, 1, true, M>) : launch(dw_pyramid_kernel<6, 1024, 1, true, M>));
+            return D == 4 ? pass(dw_pyramid_kernel<4, 256, MB, true, M>)
+                          : (D == 5 ? pass(dw_pyramid_kernel<5, 256, MB, true, M>) : pass(dw_pyramid_kernel<6, 256, MB, true, M>));
+        return D == 4 ? pass(dw_pyramid_kernel<4, 1024, 1, true, M>)
+                      : (D == 5 ? pass(dw_pyramid_kernel<5, 1024, 1, true, M>) : pass(dw_pyramid_kernel<6, 1024, 1, true, M>));
     }
     if (threads <= 256)
-        return D == 4 ? launch(dw_pyramid_kernel<4, 256, MB, false, M>)
-                      : (D == 5 ? launch(dw_pyramid_kernel<5, 256, MB, false, M>) : launch(dw_pyramid_kernel<6, 256, MB, false, M>));
-    return D == 4 ? launch(dw_pyramid_kernel<4, 1024, 1, false, M>)
-                  : (D == 5 ? launch(dw_pyramid_kernel<5, 1024, 1, false, M>) : launch(dw_pyramid_kernel<6, 1024, 1, false, M>));
+        return D == 4 ? pass(dw_pyramid_kernel<4, 256, MB, false, M>)
+                      : (D == 5 ? pass(dw_pyramid_kernel<5, 256, MB, false, M>) : pass(dw_pyramid_kernel<6, 256, MB, false, M>));
+    return D == 4 ? pass(dw_pyramid_kernel<4, 1024, 1, false, M>)
+                  : (D == 5 ? pass(dw_pyramid_kernel<5, 1024, 1, false, M>) : pass(dw_pyramid_kernel<6, 1024, 1, false, M>));
 }
 
 // The whole depthwise stage without the levels in HBM: statistics pass over y, solve, merge pass over y.
@@ -805,8 +801,7 @@ int launch_pyramid_fused(const float* y, const NormIn& nin, const float* const* 
     if (reinterpret_cast<uintptr_t>(m) % 16 != 0) return SDR_ERR_UNSUPPORTED;
     const bool pc = nin.prelu && nin.prelu_pc;
     if ((rc = launch_fused_pass<kPyrStats>(a, pc, samples, st)) != SDR_OK) return rc;
-    pyramid_solve_kernel<<<(unsigned)samples, kSolveThreads, 0, st>>>(s);
-    if (cudaGetLastError() != cudaSuccess) return SDR_ERR_CUDA;
+    if ((rc = launch(pyramid_solve_kernel, (unsigned)samples, kSolveThreads, 0, st, s)) != SDR_OK) return rc;
     a.table = table; a.m = m; a.stats_m = stats_m;
     return launch_fused_pass<kPyrMerge>(a, pc, samples, st);
 }
@@ -825,8 +820,7 @@ int launch_merge_pyramid(const float* const* z, const float* table, int D, float
     const int chunks = (int)((items + per_cta - 1) / per_cta);
     const long long grid = (long long)chunks * samples;
     if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-    merge_pyramid_kernel<<<(unsigned)grid, kMpThreads, 0, st>>>(a, m, stats_out, chunks);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(merge_pyramid_kernel, (unsigned)grid, kMpThreads, 0, st, a, m, stats_out, chunks);
 }
 
 }  // namespace sdr

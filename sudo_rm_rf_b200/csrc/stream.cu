@@ -48,9 +48,8 @@ stream_frame_kernel(const float* __restrict__ chunk, const float* __restrict__ s
 int launch_stream_frame(const float* chunk, const float* state, long long slot_stride, float* framed, int B, int A,
                         int k, int Kr, int F, long long C, cudaStream_t st) {
     const long long n = (long long)Kr * B * F;
-    stream_frame_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(chunk, state, slot_stride, framed, A, k, Kr, F,
-                                                                       B * F, C);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(stream_frame_kernel, (unsigned)((n + 255) / 256), 256, 0, st, chunk, state, slot_stride, framed, A,
+                  k, Kr, F, B * F, C);
 }
 
 // ---------------------------------------------------------------------------
@@ -212,13 +211,8 @@ int launch_causal_stream(const float* y, const float* slope_in, const float* con
     while (R > 1 && (size_t)R * pos * sizeof(float) > kStSmemSmall) R >>= 1;
     const size_t smem = (size_t)R * pos * sizeof(float);
     if (smem > kStSmemMax) return SDR_ERR_UNSUPPORTED;
-    if (smem > kStSmemSmall &&
-        cudaFuncSetAttribute(causal_stream_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-        return SDR_ERR_CUDA;
     a.R = R;
-    dim3 grid((unsigned)ceil_div(C, R), (unsigned)B);
-    causal_stream_kernel<<<grid, kStThreads, smem, st>>>(a);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(causal_stream_kernel, dim3((unsigned)ceil_div(C, R), (unsigned)B), kStThreads, smem, st, a);
 }
 
 // ---------------------------------------------------------------------------
@@ -297,8 +291,8 @@ int launch_stream_ola(const float* frames, const float* chunk, float* state, lon
     const int hop = k / 2;
     if (SA > kStMaxSrc || 2 * hop + 2 > kOlaThreads || B > 65535 || C <= hop) return SDR_ERR_UNSUPPORTED;
     dim3 grid((unsigned)(1 + (C - hop - 1 + kOlaThreads - 1) / kOlaThreads), (unsigned)B);
-    stream_ola_kernel<<<grid, kOlaThreads, 0, st>>>(frames, chunk, state, slot_stride, carry_off, out, SA, A, k, F, B, C, mc);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(stream_ola_kernel, grid, kOlaThreads, 0, st, frames, chunk, state, slot_stride, carry_off, out, SA, A,
+                  k, F, B, C, mc);
 }
 
 // The pending tail: the model's output samples n*C - hop .. n*C - 1 are the carry (no later frame reaches them once
@@ -321,8 +315,8 @@ int launch_stream_flush(const float* state, long long slot_stride, long long car
                         int hop, int mc, cudaStream_t st) {
     if (SA > kStMaxSrc) return SDR_ERR_UNSUPPORTED;
     const long long n = (long long)B * hop;
-    stream_flush_kernel<<<(unsigned)((n + 255) / 256), 256, 0, st>>>(state, slot_stride, carry_off, tail, SA, hop, B, mc);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(stream_flush_kernel, (unsigned)((n + 255) / 256), 256, 0, st, state, slot_stride, carry_off, tail, SA,
+                  hop, B, mc);
 }
 
 }  // namespace sdr

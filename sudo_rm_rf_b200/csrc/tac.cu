@@ -352,16 +352,12 @@ static int launch_tac_mma16(const float* x, const TacParams& p, float* o, double
     const int tiles_per_b = (L + 15) / 16;
     const long long total = (long long)tiles_per_b * B;
     if (total > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-    int dev = 0, sms = 0;
-    if (cudaGetDevice(&dev) != cudaSuccess ||
-        cudaDeviceGetAttribute(&sms, cudaDevAttrMultiProcessorCount, dev) != cudaSuccess) return SDR_ERR_CUDA;
-    const size_t smem = sizeof(TacFrags);
-    if (cudaFuncSetAttribute(tac_mma16_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-        return SDR_ERR_CUDA;
+    const int sms = sm_count();
+    if (sms <= 0) return SDR_ERR_CUDA;
     long long grid = (total + kTacWarps - 1) / kTacWarps;
     if (grid > (long long)kTacMinB * sms) grid = (long long)kTacMinB * sms;                   // warps loop over tiles; the weight fragments are built once per CTA
-    tac_mma16_kernel<<<(unsigned)grid, 32 * kTacWarps, smem, st>>>(x, p, o, stats, G, L, tiles_per_b, (int)total);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(tac_mma16_kernel, (unsigned)grid, 32 * kTacWarps, sizeof(TacFrags), st, x, p, o, stats, G, L,
+                  tiles_per_b, (int)total);
 }
 
 template <int NPG>
@@ -373,14 +369,10 @@ static int launch_tac_n(const float* x, const TacParams& p, float* o, double* st
                           (size_t)NPG * G * 32;
     const size_t smem = floats * sizeof(float);
     if (smem > 220 * 1024) return SDR_ERR_UNSUPPORTED;
-    if (smem > 48 * 1024 &&
-        cudaFuncSetAttribute(tac_kernel<NPG>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem) != cudaSuccess)
-        return SDR_ERR_CUDA;
     const int t_tiles = (L + 31) / 32;
     const long long grid = (long long)t_tiles * B;
     if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-    tac_kernel<NPG><<<(unsigned)grid, 32 * G, smem, st>>>(x, p, o, stats, G, L, t_tiles);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(tac_kernel<NPG>, (unsigned)grid, 32 * G, smem, st, x, p, o, stats, G, L, t_tiles);
 }
 
 int launch_tac(const float* x, const float* const* params, float* o, double* stats,
@@ -426,8 +418,7 @@ int launch_tac_apply(const float* x, const float* o, const NormIn& nin, float* o
     const int chunks = (int)((items + 1023) / 1024);
     const long long grid = (long long)chunks * samples;
     if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-    tac_apply_kernel<<<(unsigned)grid, 256, 0, st>>>(x, o, nin, out, n, L, chunks);
-    return cudaGetLastError() == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    return launch(tac_apply_kernel, (unsigned)grid, 256, 0, st, x, o, nin, out, n, L, chunks);
 }
 
 }  // namespace sdr
