@@ -129,7 +129,7 @@ def _fetch(model, dotted: str) -> torch.Tensor:
 class _DeviceState:
     """Per (model, device) cache: packed weights + workspace."""
     __slots__ = ("sig", "storages", "packed", "workspace", "staging", "captured", "retired", "tensors", "pslots",
-                 "mslots", "graphs", "stream", "event")
+                 "mslots", "graphs", "stream", "event", "lock")
 
     def __init__(self):
         self.sig = None
@@ -145,6 +145,7 @@ class _DeviceState:
         self.graphs = {}         # forward_host: CUDA graphs keyed by (host buffers, shape, weights signature)
         self.stream = None       # stream of the last enqueue on this workspace
         self.event = None        # recorded after the last enqueue (cross-stream serialisation)
+        self.lock = threading.Lock()     # held over a call's host section: pack, size, hand-over, enqueue, event
 
 
 def _state(model, device) -> _DeviceState:
@@ -188,27 +189,48 @@ class NativeModuleMixin:
         return state
 
 
-def _enter_stream(st: _DeviceState, device):
-    """One workspace per (model, device): a call arriving on a different stream than the previous one waits
-    for it (the scratch buffers are shared), and tells the caching allocator about the second stream."""
+class _Order:
+    """The stream and event of the last enqueue on buffers that several streams take turns on."""
+    __slots__ = ("stream", "event")
+
+    def __init__(self):
+        self.stream = None
+        self.event = None
+
+
+def _enter_stream(order, device, buffers):
+    """A call arriving on a different stream than the previous one (recorded in ``order``: a ``_DeviceState`` or an
+    ``_Order``) waits for it.  Every buffer the call reads is recorded on its stream, whichever stream allocated it,
+    so that the caching allocator does not hand it out again while the call is in flight."""
     cur = torch.cuda.current_stream(device)
     if torch.cuda.is_current_stream_capturing():     # the capturing caller owns the ordering
         return cur
-    if st.stream is not None and st.stream != cur and st.event is not None:
-        cur.wait_event(st.event)
-        for buf in (st.workspace, st.staging, st.packed):
-            if buf is not None:
-                buf.record_stream(cur)
+    if order.stream is not None and order.stream != cur and order.event is not None:
+        cur.wait_event(order.event)
+    for buf in buffers:
+        if buf is not None:
+            buf.record_stream(cur)
     return cur
 
 
-def _leave_stream(st: _DeviceState, cur) -> None:
+def _leave_stream(order, cur) -> None:
     if torch.cuda.is_current_stream_capturing():
         return
-    if st.event is None:
-        st.event = torch.cuda.Event()
-    st.event.record(cur)
-    st.stream = cur
+    if order.event is None:
+        order.event = torch.cuda.Event()
+    order.event.record(cur)
+    order.stream = cur
+
+
+def packed_for(model, cfg: N.SdrConfig, device, stream) -> torch.Tensor:
+    """``packed_weights`` for a call that reads them on ``stream`` outside ``_call_shared`` (a stream step, a corpus
+    pass), recorded on that stream: a repack by another call then cannot hand the buffer out early."""
+    st = _state(model, device)
+    with st.lock:
+        packed = packed_weights(model, cfg, device)
+    if not torch.cuda.is_current_stream_capturing():
+        packed.record_stream(stream)
+    return packed
 
 
 def _hand_out(st: _DeviceState, slot: str) -> None:
@@ -232,9 +254,7 @@ def _ensure(st: _DeviceState, slot: str, nbytes: int, device) -> torch.Tensor:
     """The buffer in ``slot`` ("workspace" or "staging"), replaced by one of ``nbytes`` if it is smaller."""
     buf = getattr(st, slot)
     if buf is None or buf.numel() < nbytes:
-        if st.event is not None:
-            st.event.synchronize()      # kernels of an earlier call (possibly on another stream) still use it
-        _replace(st, slot, None)
+        _replace(st, slot, None)        # recorded on every stream that read it: the allocator waits for those
         st.graphs.clear()               # captured graphs point into the old buffer
         buf = torch.empty(nbytes, dtype=torch.uint8, device=device)
         setattr(st, slot, buf)
@@ -246,14 +266,15 @@ def _call_shared(model, cfg: N.SdrConfig, device, ws_bytes: int, refusal: str, e
     """Every call that runs on the model's cached state goes through here: packs (or reuses) the weights, sizes the
     shared workspace, hands it over from the previous call's stream and runs ``enqueue(packed, workspace)``, which
     enqueues on the current stream.  ``ws_bytes`` is the caller's size query; 0 raises ``refusal``.  Returns the
-    packed weights the call ran with."""
-    with torch.cuda.device(device):
+    packed weights the call ran with.  One call at a time per (model, device): host threads sharing a model queue
+    here, so each one's call waits on the stream for the previous one's."""
+    st = _state(model, device)
+    with torch.cuda.device(device), st.lock:         # host work only: nothing in here waits for the GPU
         packed = packed_weights(model, cfg, device)
         if ws_bytes == 0:
             raise N.NativeError(refusal)
-        st = _state(model, device)
         ws = _ensure(st, "workspace", ws_bytes, device)
-        cur = _enter_stream(st, device)
+        cur = _enter_stream(st, device, (st.workspace, st.staging, st.packed))
         enqueue(packed, ws)
         _leave_stream(st, cur)
     return packed

@@ -170,6 +170,7 @@ class CorpusSeparator:
                                             "sudo_rm_rf_b200 runs on CUDA (sm_90a) only: move the model to an H100")
         self.quantum = model_padding_rule(self.cfg)      # T -> padded length (the model's own rule)
         self.graphs = {}           # (B, Tp, slot) -> "warm" | CUDAGraph
+        self._s_in, self._s_cmp, self._s_out = (torch.cuda.Stream(device=self.device) for _ in range(3))
         self.launches = {"eager": 0, "captured": 0, "replayed": 0}
 
     def run(self, wavs: Iterable[torch.Tensor]) -> List[torch.Tensor]:
@@ -189,7 +190,7 @@ class CorpusSeparator:
             raise N.NativeError("bad model configuration (sdr_separate_workspace_bytes returned 0)")
         results: List[torch.Tensor] = [None] * len(wavs)
         with torch.cuda.device(dev), torch.no_grad():
-            packed = _engine.packed_weights(self.model, cfg, dev)
+            packed = _engine.packed_for(self.model, cfg, dev, self._s_cmp)
             key_buf = (max_in, ws_bytes, packed.data_ptr())
             if getattr(self, "_buf_key", None) != key_buf:      # (re)allocate staging once per corpus shape: graphs hold addresses
                 self.graphs.clear()
@@ -201,7 +202,6 @@ class CorpusSeparator:
                 self._d_in = [torch.empty(max_in, dtype=torch.float32, device=dev) for _ in range(2)]
                 self._d_len = [torch.empty(self.max_batch, dtype=torch.int64, device=dev) for _ in range(2)]
                 self._d_out = [torch.empty(max_in * S, dtype=torch.float32, device=dev) for _ in range(2)]
-                self._s_in, self._s_cmp, self._s_out = (torch.cuda.Stream(device=dev) for _ in range(3))
             cur = torch.cuda.current_stream(dev)
             for s in (self._s_in, self._s_cmp, self._s_out):
                 s.wait_stream(cur)

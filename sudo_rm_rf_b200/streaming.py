@@ -31,7 +31,8 @@ class CausalStream:
     Owns its state and step workspace, apart from the model's forward workspace, so ``model(x)`` and open streams
     can interleave.  Every step reads the model's weights through the same packed-weight cache as ``forward``, so
     changed weights are picked up on the next step.  Steps run on the current CUDA stream, never synchronise and can
-    be captured in a CUDA graph (``step(chunk, out=...)`` with fixed buffers)."""
+    be captured in a CUDA graph (``step(chunk, out=...)`` with fixed buffers).  A step, reset or flush on another
+    CUDA stream than the previous one waits for it on the device, so consecutive calls may switch streams."""
 
     def __init__(self, model, batch_size: int, chunk_samples: int, mixture_consistency: bool = False):
         lib = N.lib()
@@ -70,12 +71,14 @@ class CausalStream:
         self._cfg = cfg
         self._state = torch.empty(lib.sdr_stream_state_bytes(C.byref(cfg), B), dtype=torch.uint8, device=device)
         self._ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
+        self._order = _engine._Order()      # the stream of the last call on the state
         self.reset()
 
     def reset(self, slots: Optional[Iterable[int]] = None) -> None:
         """Start slots over (all of them when ``slots`` is None): their next step is the start of a new stream."""
         lib = N.lib()
         with torch.cuda.device(self.device):
+            cur = _engine._enter_stream(self._order, self.device, (self._state,))
             if slots is None:
                 rc = lib.sdr_stream_reset(C.byref(self._cfg), C.c_void_p(self._state.data_ptr()), self.batch_size,
                                           None, 0, N.stream(self.device))
@@ -87,6 +90,7 @@ class CausalStream:
                 rc = lib.sdr_stream_reset(C.byref(self._cfg), C.c_void_p(self._state.data_ptr()), self.batch_size,
                                           arr, len(idx), N.stream(self.device))
             N.check(rc, "sdr_stream_reset")
+            _engine._leave_stream(self._order, cur)
 
     def step(self, chunk: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """[B, A, C] chunk -> [B, S*A, C] estimates of the model's output samples ``c*C - hop .. (c+1)*C - hop - 1``."""
@@ -105,11 +109,14 @@ class CausalStream:
                 or not out.is_contiguous():
             raise RuntimeError(f"out must be a contiguous fp32 tensor [{B}, {SA}, {Cs}] on {self.device}")
         with torch.cuda.device(self.device):
-            packed = _engine.packed_weights(self.model, cfg, self.device)
+            cur = torch.cuda.current_stream(self.device)
+            packed = _engine.packed_for(self.model, cfg, self.device, cur)
+            _engine._enter_stream(self._order, self.device, (self._state, self._ws))
             N.check(lib.sdr_stream_step(C.byref(cfg), C.c_void_p(packed.data_ptr()), C.c_void_p(self._state.data_ptr()),
                                         C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()), B, Cs,
                                         1 if self.mixture_consistency else 0, C.c_void_p(self._ws.data_ptr()),
                                         self._ws.numel(), N.stream(self.device)), "sdr_stream_step")
+            _engine._leave_stream(self._order, cur)
         return out
 
     def flush(self) -> torch.Tensor:
@@ -120,7 +127,9 @@ class CausalStream:
         tail = torch.empty((self.batch_size, cfg.num_sources * cfg.in_audio_channels, self.latency),
                            dtype=torch.float32, device=self.device)
         with torch.cuda.device(self.device):
+            cur = _engine._enter_stream(self._order, self.device, (self._state,))
             N.check(lib.sdr_stream_flush(C.byref(cfg), C.c_void_p(self._state.data_ptr()), C.c_void_p(tail.data_ptr()),
                                          self.batch_size, 1 if self.mixture_consistency else 0, N.stream(self.device)),
                     "sdr_stream_flush")
+            _engine._leave_stream(self._order, cur)
         return tail
