@@ -25,7 +25,7 @@
  *     pyramid entries comes back as pre-load + sums); the padding of a ragged batch zero (sdr_separate_ragged).
  *   - Size: the byte count the matching size query returns suffices exactly.
  *   - Alignment: 256 bytes for workspaces, `saved` and the staging buffer; 16 bytes for the packed weights and the
- *     stream state; 8 bytes for the scratch of the three metrics.
+ *     stream state; 8 bytes for the scratch of the metrics.
  *   - The whole-model entries (sdr_pack_weights, sdr_forward, sdr_forward_host, sdr_separate, sdr_separate_ragged,
  *     sdr_stream_reset / _step / _flush, sdr_forward_train, sdr_backward) refuse a null, too small
  *     (SDR_ERR_WORKSPACE) or misaligned (SDR_ERR_BAD_ARGUMENT) buffer before anything is enqueued.
@@ -464,6 +464,23 @@ int sdr_bss_eval_mixture(const float* reference, const float* estimate, const fl
                          double* sir, double* sar, int32_t* perm_or_null, double* mix_sdr, double* mix_sir,
                          double* mix_sar, int B, int S, int64_t T, int F, int compute_permutation, void* scratch,
                          sdr_stream stream);
+
+/* STOI (pystoi 0.3.3's stoi(x, y, fs_sig, extended=False), the stoi of asteroid's get_metrics): reference and
+ * estimate [B,S,T], mixture_or_null [B,T] -> stoi [B,S] fp64 (estimate j scored against reference j) and, with the
+ * mixture, mix_stoi [B,S] (the mixture scored against every reference).  Rows are resampled from fs to 10 kHz as
+ * Octave's resample does (scipy resample_poly alignment), frames more than 40 dB below the reference's loudest are
+ * dropped from both signals, and the 30-frame segment correlations of the 15 third-octave band magnitudes are
+ * averaged; fewer than 30 spectral frames (including rows of at most 256 samples after resampling) give 1e-5.
+ * lengths_or_null (device [B]) scores item b over its first lengths[b] samples and reads nothing past them; a length
+ * outside [1, T] gives NaN in the item's outputs.  A NaN or infinity in reference j or estimate j gives stoi[b][j]
+ * NaN, in reference j or the mixture mix_stoi[b][j] NaN; nothing else changes.  Any integer fs >= 1000 whose reduced
+ * ratio 10000 / fs has max(p, q) <= 441 (44.1 and 22.05 kHz included).  fp64 after the inputs, no atomics: bitwise
+ * reproducible; no call synchronises or allocates.  Scratch: sdr_stoi_scratch_bytes(B, S, T, fs) (0: unsupported
+ * arguments), 8-byte aligned. */
+size_t sdr_stoi_scratch_bytes(int B, int S, int64_t T, int fs);
+int sdr_stoi(const float* reference, const float* estimate, const float* mixture_or_null,
+             const int64_t* lengths_or_null, double* stoi, double* mix_stoi_or_null, int B, int S, int64_t T, int fs,
+             void* scratch, sdr_stream stream);
 
 /* ---- training of the improved model (variant 0) ---------------------------
  * sdr_forward_train runs sdr_forward's kernels (same plan, pyramid choice and GEMMs, no mixture consistency) and

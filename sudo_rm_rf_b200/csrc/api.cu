@@ -1467,5 +1467,15 @@ int sdr_bss_eval_mixture(const float* reference, const float* estimate, const fl
                            T, F, compute_permutation, scratch, static_cast<cudaStream_t>(stream));
 }
 
+size_t sdr_stoi_scratch_bytes(int B, int S, int64_t T, int fs) { return stoi_scratch_bytes(B, S, T, fs); }
+
+int sdr_stoi(const float* reference, const float* estimate, const float* mixture_or_null,
+             const int64_t* lengths_or_null, double* stoi, double* mix_stoi_or_null, int B, int S, int64_t T, int fs,
+             void* scratch, sdr_stream stream) {
+    if (scratch && reinterpret_cast<uintptr_t>(scratch) % 8) return SDR_ERR_BAD_ARGUMENT;
+    return launch_stoi(reference, estimate, mixture_or_null, reinterpret_cast<const long long*>(lengths_or_null), stoi,
+                       mix_stoi_or_null, B, S, T, fs, scratch, static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"
 #pragma GCC visibility pop

@@ -116,6 +116,11 @@ int launch_bss_eval(const float* ref, const float* est, const float* mix, double
                     int* perm, double* msdr, double* msir, double* msar, int B, int S, long long T, int F,
                     int compute_permutation, void* scratch, cudaStream_t st);
 
+// STOI (stoi.cu)
+size_t stoi_scratch_bytes(int B, int S, long long T, int fs);
+int launch_stoi(const float* ref, const float* est, const float* mix, const long long* lengths, double* out,
+                double* mout, int B, int S, long long T, int fs, void* scratch, cudaStream_t st);
+
 // tensor-core path (pointwise_mma.cu)
 bool pointwise_mma_eligible(int M, int K);
 size_t pointwise_mma_packed_bytes(int M, int K);
