@@ -120,6 +120,11 @@ def stoi(x, y, fs_sig):
     if fs_sig != FS:
         x = resample_oct(x, FS, fs_sig)
         y = resample_oct(y, FS, fs_sig)
+    return stoi_at_fs(x, y)
+
+
+def stoi_at_fs(x, y):
+    """The rest of ``stoi`` once x and y are at FS."""
     kept = remove_silent_frames(x, y, DYN_RANGE, N_FRAME, int(N_FRAME / 2))
     if kept is None:
         return 1e-5
@@ -152,6 +157,38 @@ def resampled_length(n, fs_sig):
     g = math.gcd(FS, fs_sig)
     p, q = FS // g, fs_sig // g
     return n if p == q else -(-n * p // q)
+
+
+def at_fs(x, fs_sig):
+    """x as fp64 at FS, as ``stoi`` resamples it."""
+    x = np.asarray(x, np.float64)
+    return x if fs_sig == FS else resample_oct(x, FS, fs_sig)
+
+
+def frame_energies(x, fs_sig=FS):
+    """The energies in dB that ``remove_silent_frames`` gives the frames of clean signal x."""
+    x = at_fs(x, fs_sig)
+    w = hann()
+    frames = np.array([w * x[i:i + N_FRAME] for i in range(0, len(x) - N_FRAME, N_FRAME // 2)])
+    return 20 * np.log10(np.linalg.norm(frames, axis=1) + EPS) if len(frames) else np.zeros(0)
+
+
+def mask_margin(x, fs_sig=FS):
+    """(indices of the frames of clean signal x that ``remove_silent_frames`` keeps, and the smallest distance in dB of
+    any frame energy from the threshold max - DYN_RANGE).  A computation that rounds a frame energy differently keeps
+    the same frames as long as its error stays below the margin.  ([], inf) when x has no frame."""
+    e = frame_energies(x, fs_sig)
+    if len(e) == 0:
+        return np.zeros(0, np.int64), math.inf
+    d = np.max(e) - DYN_RANGE - e
+    return np.flatnonzero(d < 0), float(np.min(np.abs(d)))
+
+
+def score(x, ys, fs_sig):
+    """(``stoi(x, y, fs_sig)`` for every y of ys, kept frame indices, mask margin) with x resampled once."""
+    x10 = at_fs(x, fs_sig)
+    kept, margin = mask_margin(x10)
+    return [stoi_at_fs(x10, at_fs(y, fs_sig)) for y in ys], kept, margin
 
 
 def spectral_frames(x, fs_sig):

@@ -1,8 +1,8 @@
 """Past 2^31 elements: the kernels that test_gpu_scale.py does not reach there.
 
 The one-pass depthwise pyramid (fused and level-writing), the wide merge, the causal pyramid, both TAC kernels, both
-encoders, the metrics' Gram kernels, the loss and mixture-consistency backward kernels, the backward stage kernels and
-three whole models.  The method is test_gpu_scale.py's:
+encoders, the metrics' Gram kernels, the loss and mixture-consistency backward kernels, the backward stage kernels,
+three whole models and STOI.  The method is test_gpu_scale.py's:
 
 1. the rows under test start past element 2^31 (past 2^32 where the tensors fit in about 24 GiB), asserted in Python
    before anything is launched;
@@ -28,7 +28,8 @@ import torch.nn.functional as F
 from sudo_rm_rf_b200 import _engine
 from sudo_rm_rf_b200 import _native as N
 from oracle import sudormrf_oracle as O
-from guards import GUARD, GUARD_BITS, assert_guards_intact
+import stoi_oracle as SO
+from guards import GUARD, GUARD_BITS, POISON_NAN, assert_guards_intact, check_bands, guarded, poisoned
 from test_gpu_long import CLASSES, normalised_input
 from test_gpu_model_space import TOL, build, gc, imp
 from test_gpu_pyramid_fused import PYR_MAX_SAMPLES, arr, chain_ref, run_fused, stage_inputs
@@ -909,6 +910,83 @@ def test_model_past_2_31_elements(name, variant, kw, T):
 
 
 # =====================================================================================================================
+# STOI
+# =====================================================================================================================
+STOI_BIG = [
+    # (name, fs, S, seconds, B, mixture): the rows past 2^31 and where they start
+    ("input_rows", 44100, 2, 25, 975, True),     # the last reference and estimate rows start at 2,148,772,500 samples
+    ("sig_rows", 8000, 2, 60, 900, False),       # the last estimate row of sig starts at 2,159,400,000 doubles
+]
+STOI_PERIOD = 7                                  # distinct items, tiled: a row read from the wrong item shows
+
+
+def stoi_call(ref, est, mix, fs):
+    """sdr_stoi on a poisoned scratch of exactly the queried size, outputs NaN inside guard bands."""
+    lib = N.lib()
+    B, S, T = ref.shape
+    sc = poisoned(lib.sdr_stoi_scratch_bytes(B, S, T, fs), POISON_NAN)
+    nan = torch.full((B, S), float("nan"), dtype=torch.float64, device=DEV)
+    out, mout = guarded(nan), guarded(nan)
+    N.check(lib.sdr_stoi(p(ref), p(est), p(mix), None, p(out), p(mout) if mix is not None else None, B, S, T, fs,
+                         p(sc), stream()), "sdr_stoi")
+    check_bands(sc, "scratch")
+    assert_guards_intact(out, "stoi")
+    assert_guards_intact(mout, "mix_stoi")
+    return out, (mout if mix is not None else None)
+
+
+@gpu
+@pytest.mark.parametrize("name,fs,S,seconds,B,with_mix", STOI_BIG, ids=[c[0] for c in STOI_BIG])
+def test_stoi_past_2_31_elements(name, fs, S, seconds, B, with_mix):
+    """sdr_stoi with the last item's input rows past 2^31 samples (44.1 kHz) or its resampled estimate rows past 2^31
+    doubles of the scratch (8 kHz); both also pass the spectra kernel's 2^20-CTA grid.  The last item bitwise against
+    the same call on it alone, and against the fp64 restatement; the first item finite."""
+    T = seconds * fs
+    R = B * S
+    g_ = math.gcd(SO.FS, fs)
+    pr, qr = SO.FS // g_, fs // g_
+    Tn = -(-T * pr // qr)
+    M = -(-(Tn - 256) // 128) - 1
+    work = (3 if with_mix else 2) * R * ((M + 3) // 4)
+    print(f"\n{name}: last input row at {(R - 1) * T}, last estimate sig row at {(2 * R - 1) * Tn}, "
+          f"spectra work items {work}")
+    past(work, 1 << 20)
+    if name == "input_rows":
+        past((R - 1) * T)
+    else:
+        past((2 * R - 1) * Tn)
+    lib = N.lib()
+    need((2 * R + B) * T * 4 / GiB + lib.sdr_stoi_scratch_bytes(B, S, T, fs) / GiB + 1)
+    g = torch.Generator(device=DEV).manual_seed(231)
+    base = torch.randn(STOI_PERIOD, S, T, device=DEV, generator=g)
+    base.mul_(torch.rand(STOI_PERIOD, S, 1, device=DEV, generator=g) + 0.1)
+    base[:, :, T // 3:T // 2] *= 1e-3                   # a quiet stretch the mask drops
+    noise = torch.randn(STOI_PERIOD, S, T, device=DEV, generator=g) * torch.linspace(
+        0.1, 2.0, STOI_PERIOD, device=DEV).view(-1, 1, 1)
+    idx = torch.arange(B, device=DEV) % STOI_PERIOD
+    ref = base[idx]
+    est = noise[idx].add_(ref)
+    del noise
+    mix = (base.sum(1) + 0.3 * torch.randn(STOI_PERIOD, T, device=DEV, generator=g))[idx] if with_mix else None
+    del base
+    d, m = stoi_call(ref, est, mix, fs)
+    one = stoi_call(ref[-1:].contiguous(), est[-1:].contiguous(), None if mix is None else mix[-1:].contiguous(), fs)
+    torch.cuda.synchronize()
+    assert torch.isfinite(d[0]).all() and torch.isfinite(d[-1]).all(), (d[0], d[-1])
+    assert torch.equal(d[-1:], one[0]), (d[-1], one[0])
+    if with_mix:
+        assert torch.isfinite(m[0]).all() and torch.equal(m[-1:], one[1]), (m[-1], one[1])
+    xr, yr = ref[-1].cpu().double().numpy(), est[-1].cpu().double().numpy()
+    mr = None if mix is None else mix[-1].cpu().double().numpy()
+    for j in range(S):
+        w, _, margin = SO.score(xr[j], [yr[j]] + ([] if mr is None else [mr]), fs)
+        assert margin >= 1e-6, margin
+        err = max(abs(float(d[-1, j]) - w[0]), abs(float(m[-1, j]) - w[1]) if with_mix else 0.0)
+        print(f"{name}: source {j} |GPU - oracle| {err:.2e}")
+        assert err <= 1e-9, (j, d[-1], m if m is None else m[-1], w)
+
+
+# =====================================================================================================================
 # the list of kernels and the cases that run them past 2^31 (no GPU)
 # =====================================================================================================================
 COVERED = {
@@ -940,12 +1018,18 @@ COVERED = {
     "frame_gather_kernel": ["test_overlap_add_backward_past_2_31_elements"],
     "wgrad_partial_kernel": ["test_encoder_wgrad_past_2_31_elements", "test_pointwise_wgrad_past_2_31_elements"],
     "wgrad_reduce_kernel": ["test_encoder_wgrad_past_2_31_elements", "test_pointwise_wgrad_past_2_31_elements"],
+    "stoi_filter_kernel": ["test_stoi_past_2_31_elements"],
+    "stoi_resample_kernel": ["test_stoi_past_2_31_elements"],
+    "stoi_mask_kernel": ["test_stoi_past_2_31_elements"],
+    "stoi_spectra_kernel": ["test_stoi_past_2_31_elements"],
+    "stoi_segment_kernel": ["test_stoi_past_2_31_elements"],
 }
 
 
 def test_past_2_31_kernel_list_is_in_step():
     """Every kernel listed exists in csrc/ and names cases of this module that exist; every kernel of backward.cu is
-    listed except the training forward's mask and the weight transpose, which move no activation-sized gradient."""
+    listed except the training forward's mask and the weight transpose, which move no activation-sized gradient, and
+    every kernel of stoi.cu is listed."""
     csrc = os.path.join(REPO, "sudo_rm_rf_b200", "csrc")
     src = {f: open(os.path.join(csrc, f)).read() for f in os.listdir(csrc) if f.endswith((".cu", ".cuh"))}
     defined = {k for s in src.values() for k in re.findall(r"\b(\w+_kernel)\s*\(", s)}
@@ -954,3 +1038,5 @@ def test_past_2_31_kernel_list_is_in_step():
         assert cases and all(callable(globals().get(c)) for c in cases), (k, cases)
     backward = set(re.findall(r"^(\w+_kernel)\(", src["backward.cu"], re.M)) - {"mask_apply_kernel", "transpose_kernel"}
     assert backward and backward <= set(COVERED), sorted(backward - set(COVERED))
+    stoi = set(re.findall(r"__global__[^;{]*?\b(\w+_kernel)\s*\(", src["stoi.cu"]))
+    assert len(stoi) == 5 and stoi <= set(COVERED), sorted(stoi - set(COVERED))

@@ -9,6 +9,7 @@ import torch
 import sudo_rm_rf_b200 as P
 from sudo_rm_rf_b200 import _native as N
 import stoi_oracle as O
+import stoi_rates
 
 SYMBOLS = ("sdr_stoi_scratch_bytes", "sdr_stoi")
 
@@ -93,6 +94,29 @@ def test_symbols_bind_and_scratch_limits():
     assert lib.sdr_stoi(x, x, x, None, x, None, 1, 2, 100, 8000, x, None) == -2             # mixture, no mix_stoi
     assert lib.sdr_stoi(x, x, None, None, x, None, 1, 2, 100, 8000, 12, None) == -2           # misaligned scratch
     assert lib.sdr_stoi(x, x, None, None, x, None, 1, 2, 100, 35360, x, None) == -5           # past the cap
+
+
+def test_scratch_query_accepts_exactly_the_supported_rates():
+    """For every integer fs in [1, 4.5 MHz]: the scratch query is non-zero exactly where fs >= 1000 and 10000 / fs
+    reduces to p / q with max(p, q) <= 441 (3918 rates, from 1000 Hz to 4.41 MHz)."""
+    lib = N.lib()
+    want = set(stoi_rates.accepted(1, 4_500_000).tolist())
+    assert len(want) == 3918
+    got = {fs for fs in range(1, 4_500_001) if lib.sdr_stoi_scratch_bytes(1, 1, 1000, fs) > 0}
+    assert got == want, (sorted(got - want)[:10], sorted(want - got)[:10])
+
+
+def test_scratch_query_size_limits():
+    """B S up to 715,827,882 = (2^31 - 1) / 3 (the 3 B S tob rows), T up to 2^40."""
+    lib = N.lib()
+    top = (2 ** 31 - 1) // 3
+    for B, S in ((top, 1), (1, top), (top // 2, 2)):
+        assert lib.sdr_stoi_scratch_bytes(B, S, 1000, 8000) > 0, (B, S)
+    for B, S in ((top + 1, 1), (1, top + 1), (top // 2 + 1, 2)):
+        assert lib.sdr_stoi_scratch_bytes(B, S, 1000, 8000) == 0, (B, S)
+    for fs in (1000, 8000, 10000, 44100):
+        assert lib.sdr_stoi_scratch_bytes(1, 1, 2 ** 40, fs) > 0, fs
+        assert lib.sdr_stoi_scratch_bytes(1, 1, 2 ** 40 + 1, fs) == 0, fs
 
 
 def test_refusals():
