@@ -482,6 +482,35 @@ int sdr_stoi(const float* reference, const float* estimate, const float* mixture
              const int64_t* lengths_or_null, double* stoi, double* mix_stoi_or_null, int B, int S, int64_t T, int fs,
              void* scratch, sdr_stream stream);
 
+/* ---- windowed separation of long recordings (DESIGN.md section 7e) ---------
+ * A recording of T samples is cut into K = sdr_window_count(T, W, H) windows (1 when T <= W, else
+ * 1 + ceil((T - W) / H)); window k covers samples [k H, k H + W), zeros at T and beyond.  W/2 <= H < W and
+ * 2 <= W <= 2^24; sdr_window_count returns 0 for anything else.  Windows are processed in batches k0 .. k0+M-1 in
+ * increasing k0, without gaps:
+ *   sdr_window_gather copies them out of mixture [B][A][T] into batch [B][M][A][W];
+ *   the caller separates the batch ([B M, A, W] through sdr_forward or sdr_separate) into estimates
+ *   [B][M][S A][W];
+ *   sdr_window_merge aligns and overlap-adds them.  For each window k >= 1 of the batch it takes
+ *   C_k[i][j] = sum_a sum_t (p_ia - mean p_ia)(c_ja - mean c_ja) in fp64 over the overlap [k H, (k-1) H + W) below T
+ *   (p: window k-1's source i, c: window k's source j, rows s A + a), and rho_k, the first maximum of
+ *   sum_i C_k[i][rho(i)] over the permutations in itertools order (the identity when C_k is not finite).  With
+ *   pi_0 = id and pi_k(s) = rho_k(pi_{k-1}(s)), output source s of window k is its raw source pi_k(s).  It writes out
+ *   [B][S A][T] over [k0 H, (k0 + M) H), or up to T in the last batch: a sample in one window takes that window's
+ *   value, sample k H + j of overlap k takes (1 - r) prev + r cur in fp32 with r = (j + 1) / (W - H + 1).
+ *   perm_or_null [B][K][S] receives pi_k of the batch's windows.
+ * carry (sdr_window_carry_bytes(B, S, A, W), 256-byte aligned) holds pi and the raw estimate of the batch's last
+ * window for the next batch: ignored when k0 = 0, else it must hold what the merge of the previous batch left.
+ * Scratch: sdr_window_merge_scratch_bytes(B, S, M), 8-byte aligned.  1 <= S <= 4 (else 0 / SDR_ERR_UNSUPPORTED).
+ * A NaN or infinity in one recording changes no other recording's output.  No atomics, fixed-order reductions and
+ * no synchronisation: given the same estimates the output is bitwise independent of the batch sizes M. */
+int64_t sdr_window_count(int64_t T, int64_t W, int64_t H);
+size_t  sdr_window_carry_bytes(int B, int S, int A, int64_t W);
+size_t  sdr_window_merge_scratch_bytes(int B, int S, int M);
+int     sdr_window_gather(const float* mixture, float* batch, int B, int A, int64_t T, int64_t W, int64_t H,
+                          int64_t k0, int M, sdr_stream stream);
+int     sdr_window_merge(const float* estimates, void* carry, int32_t* perm_or_null, float* out, int B, int S, int A,
+                         int64_t T, int64_t W, int64_t H, int64_t k0, int M, void* scratch, sdr_stream stream);
+
 /* ---- training of the improved model (variant 0) ---------------------------
  * sdr_forward_train runs sdr_forward's kernels (same plan, pyramid choice and GEMMs, no mixture consistency) and
  * also copies into `saved` what the backward recomputes from: the statistics slots, the raw encoder output and every

@@ -160,6 +160,13 @@ _SIGNATURES = {
     "sdr_stoi_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int64, C.c_int]),
     "sdr_stoi": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                            C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
+    "sdr_window_count": (C.c_int64, [C.c_int64, C.c_int64, C.c_int64]),
+    "sdr_window_carry_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int64]),
+    "sdr_window_merge_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
+    "sdr_window_gather": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_int64,
+                                    C.c_int64, C.c_int, C.c_void_p]),
+    "sdr_window_merge": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                   C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
     "sdr_train_saved_bytes": (C.c_size_t, [C.POINTER(SdrConfig), C.c_int, C.c_int64]),
     "sdr_backward_workspace_bytes": (C.c_size_t, [C.POINTER(SdrConfig), C.c_int, C.c_int64]),
     "sdr_forward_train": (C.c_int, [C.POINTER(SdrConfig), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64,

@@ -12,6 +12,7 @@ import torch
 import torch.nn as nn
 
 from . import _engine
+from . import windowed
 from .improved_sudormrf import _not_standalone, _xavier_uniform_
 
 
@@ -126,6 +127,14 @@ class CausalSuDORMRF(_engine.NativeModuleMixin, nn.Module):
         if normalize:
             return _engine.separate(self, input_wav, mixture_consistency=mixture_consistency)
         return _engine.forward(self, input_wav, mixture_consistency=mixture_consistency)
+
+    def separate_long(self, input_wav, window, hop=None, normalize=True, mixture_consistency=False,
+                      max_windows=32):
+        """``separate`` for recordings of any length: overlapping windows of ``window`` samples every ``hop``,
+        separated in batches of ``max_windows`` per recording, aligned and cross-faded on the device (see
+        ``windowed.separate_long``)."""
+        return windowed.separate_long(self, input_wav, window, hop, normalize=normalize,
+                                      mixture_consistency=mixture_consistency, max_windows=max_windows)
 
     def forward_host(self, host_wav, host_out=None, mixture_consistency=False):
         """End-to-end call on pinned HOST tensors (H2D, forward, D2H on the current stream)."""

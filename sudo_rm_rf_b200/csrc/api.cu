@@ -1477,5 +1477,22 @@ int sdr_stoi(const float* reference, const float* estimate, const float* mixture
                        mix_stoi_or_null, B, S, T, fs, scratch, static_cast<cudaStream_t>(stream));
 }
 
+int64_t sdr_window_count(int64_t T, int64_t W, int64_t H) { return window_count(T, W, H); }
+
+size_t sdr_window_carry_bytes(int B, int S, int A, int64_t W) { return window_carry_bytes(B, S, A, W); }
+
+size_t sdr_window_merge_scratch_bytes(int B, int S, int M) { return window_merge_scratch_bytes(B, S, M); }
+
+int sdr_window_gather(const float* mixture, float* batch, int B, int A, int64_t T, int64_t W, int64_t H, int64_t k0,
+                      int M, sdr_stream stream) {
+    return launch_window_gather(mixture, batch, B, A, T, W, H, k0, M, static_cast<cudaStream_t>(stream));
+}
+
+int sdr_window_merge(const float* estimates, void* carry, int32_t* perm_or_null, float* out, int B, int S, int A,
+                     int64_t T, int64_t W, int64_t H, int64_t k0, int M, void* scratch, sdr_stream stream) {
+    return launch_window_merge(estimates, carry, perm_or_null, out, B, S, A, T, W, H, k0, M, scratch,
+                               static_cast<cudaStream_t>(stream));
+}
+
 }  // extern "C"
 #pragma GCC visibility pop

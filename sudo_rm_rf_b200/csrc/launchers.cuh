@@ -121,6 +121,15 @@ size_t stoi_scratch_bytes(int B, int S, long long T, int fs);
 int launch_stoi(const float* ref, const float* est, const float* mix, const long long* lengths, double* out,
                 double* mout, int B, int S, long long T, int fs, void* scratch, cudaStream_t st);
 
+// windowed separation (windowed.cu)
+long long window_count(long long T, long long W, long long H);
+size_t window_carry_bytes(int B, int S, int A, long long W);
+size_t window_merge_scratch_bytes(int B, int S, int M);
+int launch_window_gather(const float* x, float* batch, int B, int A, long long T, long long W, long long H,
+                         long long k0, int M, cudaStream_t st);
+int launch_window_merge(const float* est, void* carry, int* perm, float* out, int B, int S, int A, long long T,
+                        long long W, long long H, long long k0, int M, void* scratch, cudaStream_t st);
+
 // tensor-core path (pointwise_mma.cu)
 bool pointwise_mma_eligible(int M, int K);
 size_t pointwise_mma_packed_bytes(int M, int K);
