@@ -511,6 +511,43 @@ int     sdr_window_gather(const float* mixture, float* batch, int B, int A, int6
 int     sdr_window_merge(const float* estimates, void* carry, int32_t* perm_or_null, float* out, int B, int S, int A,
                          int64_t T, int64_t W, int64_t H, int64_t k0, int M, void* scratch, sdr_stream stream);
 
+/* ---- windowed stream (DESIGN.md section 7f) --------------------------------
+ * separate_long's windows, taken step by step for B independent slots.  With q = C / H (C a positive multiple of
+ * H) and n = j C the samples a slot has received since its reset, a step's output [B][S A][C] is samples
+ * [n - H, n + C - H) of the windowed separation of the slot's input up to n + C (zeros below 0), and the flush's
+ * [B][S A][H] is samples [n - H, n) of the separation up to n.  Per step:
+ *   sdr_window_stream_gather copies windows c-1 .. c+q-2 of each slot (c = n / H, the slot's window counter; the
+ *   window below 0 of a slot's first step is all zeros) out of its history and chunk [B][A][C] into batch
+ *   [B][q][A][W], and makes the chunk's last H samples the history;
+ *   the caller separates the batch ([B q, A, W] through sdr_forward or sdr_separate) into estimates [B][q][S A][W];
+ *   sdr_window_stream_merge aligns, scans and overlap-adds them as sdr_window_merge does, with each slot's own window
+ *   origin, into out [B][S A][C], keeps the carry and advances the counters by q.
+ * Flush: sdr_window_stream_gather with chunk_or_null = NULL and C = 0 writes the window that starts at n - H, the
+ * history followed by zeros, into batch [B][A][W]; the caller separates it (needed when W < 2 H) and, as `single`
+ * [B][S A][H], the history alone (the whole recording of a slot with n = H); sdr_window_stream_flush picks per slot
+ * on the device: zeros (n = 0), single (n = H), else the carry and, when W < 2 H, the flush window.  Neither the
+ * flush gather nor the flush changes the state.
+ * State: sdr_window_stream_state_bytes(B, S, A, W, H), 256-byte aligned: the carry of sdr_window_carry_bytes, the
+ * history [B][A][H] fp32 and the counters [B] int64, each starting on a 256-byte boundary.  sdr_window_stream_reset zeroes it (all
+ * slots, or the n listed in host memory) before a slot's first step.  Scratch: sdr_window_stream_merge_scratch_bytes
+ * (B, S, C, H) and sdr_window_stream_flush_scratch_bytes(B, S), 8-byte aligned.  1 <= S <= 4, W/2 <= H < W,
+ * W <= 2^24 (else 0 / SDR_ERR_UNSUPPORTED for S, SDR_ERR_BAD_ARGUMENT otherwise).  sdr_window_stream_launch_count is
+ * the number of kernels a step's gather and merge launch.  No atomics, fixed-order reductions and no
+ * synchronisation: a step can be captured in a CUDA graph, and given the same window estimates its output is
+ * bitwise sdr_window_merge's. */
+size_t sdr_window_stream_state_bytes(int B, int S, int A, int64_t W, int64_t H);
+int    sdr_window_stream_reset(void* state, int B, int S, int A, int64_t W, int64_t H,
+                               const int32_t* host_slots_or_null, int n, sdr_stream stream);
+int    sdr_window_stream_gather(void* state, const float* chunk_or_null, float* batch, int B, int S, int A, int64_t C,
+                                int64_t W, int64_t H, sdr_stream stream);
+size_t sdr_window_stream_merge_scratch_bytes(int B, int S, int64_t C, int64_t H);
+int    sdr_window_stream_merge(const float* estimates, void* state, float* out, int B, int S, int A, int64_t C,
+                               int64_t W, int64_t H, void* scratch, sdr_stream stream);
+size_t sdr_window_stream_flush_scratch_bytes(int B, int S);
+int    sdr_window_stream_flush(const float* single, const float* estimates_or_null, const void* state, float* out,
+                               int B, int S, int A, int64_t W, int64_t H, void* scratch, sdr_stream stream);
+int    sdr_window_stream_launch_count(int B, int S, int A, int64_t C, int64_t W, int64_t H);
+
 /* ---- training of the improved model (variant 0) ---------------------------
  * sdr_forward_train runs sdr_forward's kernels (same plan, pyramid choice and GEMMs, no mixture consistency) and
  * also copies into `saved` what the backward recomputes from: the statistics slots, the raw encoder output and every

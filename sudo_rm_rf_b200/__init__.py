@@ -19,7 +19,8 @@ from .groupcomm_sudormrf_v2 import GroupCommSudoRmRf                          # 
 from .causal_improved_sudormrf_v3 import CausalSuDORMRF                       # noqa: F401
 from .sudormrf import SuDORMRF as OriginalSuDORMRF                            # noqa: F401
 from ._engine import refresh_weights                                          # noqa: F401
+from .window_stream import WindowedStream                                     # noqa: F401
 
 __all__ = ["SuDORMRF", "GroupCommSudoRmRf", "CausalSuDORMRF", "OriginalSuDORMRF", "improved_sudormrf",
            "groupcomm_sudormrf_v2", "causal_improved_sudormrf_v3", "sudormrf", "mixture_consistency", "snr",
-           "bss_eval_sources", "stoi", "refresh_weights"]
+           "bss_eval_sources", "stoi", "refresh_weights", "WindowedStream"]

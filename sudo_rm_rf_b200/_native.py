@@ -167,6 +167,18 @@ _SIGNATURES = {
                                     C.c_int64, C.c_int, C.c_void_p]),
     "sdr_window_merge": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                    C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
+    "sdr_window_stream_state_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64]),
+    "sdr_window_stream_reset": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_void_p,
+                                          C.c_int, C.c_void_p]),
+    "sdr_window_stream_gather": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64,
+                                           C.c_int64, C.c_int64, C.c_void_p]),
+    "sdr_window_stream_merge_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int64, C.c_int64]),
+    "sdr_window_stream_merge": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64,
+                                          C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
+    "sdr_window_stream_flush_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "sdr_window_stream_flush": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                          C.c_int64, C.c_int64, C.c_void_p, C.c_void_p]),
+    "sdr_window_stream_launch_count": (C.c_int, [C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_int64]),
     "sdr_train_saved_bytes": (C.c_size_t, [C.POINTER(SdrConfig), C.c_int, C.c_int64]),
     "sdr_backward_workspace_bytes": (C.c_size_t, [C.POINTER(SdrConfig), C.c_int, C.c_int64]),
     "sdr_forward_train": (C.c_int, [C.POINTER(SdrConfig), C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int64,

@@ -1494,5 +1494,42 @@ int sdr_window_merge(const float* estimates, void* carry, int32_t* perm_or_null,
                                static_cast<cudaStream_t>(stream));
 }
 
+size_t sdr_window_stream_state_bytes(int B, int S, int A, int64_t W, int64_t H) {
+    return window_stream_state_bytes(B, S, A, W, H);
+}
+
+int sdr_window_stream_reset(void* state, int B, int S, int A, int64_t W, int64_t H, const int32_t* host_slots_or_null,
+                            int n, sdr_stream stream) {
+    return window_stream_reset(state, B, S, A, W, H, host_slots_or_null, n, static_cast<cudaStream_t>(stream));
+}
+
+int sdr_window_stream_gather(void* state, const float* chunk_or_null, float* batch, int B, int S, int A, int64_t C,
+                             int64_t W, int64_t H, sdr_stream stream) {
+    return launch_window_stream_gather(state, chunk_or_null, batch, B, S, A, C, W, H,
+                                       static_cast<cudaStream_t>(stream));
+}
+
+size_t sdr_window_stream_merge_scratch_bytes(int B, int S, int64_t C, int64_t H) {
+    return window_stream_merge_scratch_bytes(B, S, C, H);
+}
+
+int sdr_window_stream_merge(const float* estimates, void* state, float* out, int B, int S, int A, int64_t C,
+                            int64_t W, int64_t H, void* scratch, sdr_stream stream) {
+    return launch_window_stream_merge(estimates, state, out, B, S, A, C, W, H, scratch,
+                                      static_cast<cudaStream_t>(stream));
+}
+
+size_t sdr_window_stream_flush_scratch_bytes(int B, int S) { return window_stream_flush_scratch_bytes(B, S); }
+
+int sdr_window_stream_flush(const float* single, const float* estimates_or_null, const void* state, float* out, int B,
+                            int S, int A, int64_t W, int64_t H, void* scratch, sdr_stream stream) {
+    return launch_window_stream_flush(single, estimates_or_null, state, out, B, S, A, W, H, scratch,
+                                      static_cast<cudaStream_t>(stream));
+}
+
+int sdr_window_stream_launch_count(int B, int S, int A, int64_t C, int64_t W, int64_t H) {
+    return window_stream_launch_count(B, S, A, C, W, H);
+}
+
 }  // extern "C"
 #pragma GCC visibility pop

@@ -129,6 +129,18 @@ int launch_window_gather(const float* x, float* batch, int B, int A, long long T
                          long long k0, int M, cudaStream_t st);
 int launch_window_merge(const float* est, void* carry, int* perm, float* out, int B, int S, int A, long long T,
                         long long W, long long H, long long k0, int M, void* scratch, cudaStream_t st);
+size_t window_stream_state_bytes(int B, int S, int A, long long W, long long H);
+int window_stream_reset(void* state, int B, int S, int A, long long W, long long H, const int* slots, int n,
+                        cudaStream_t st);
+int launch_window_stream_gather(void* state, const float* chunk, float* batch, int B, int S, int A, long long C,
+                                long long W, long long H, cudaStream_t st);
+size_t window_stream_merge_scratch_bytes(int B, int S, long long C, long long H);
+int launch_window_stream_merge(const float* est, void* state, float* out, int B, int S, int A, long long C,
+                               long long W, long long H, void* scratch, cudaStream_t st);
+size_t window_stream_flush_scratch_bytes(int B, int S);
+int launch_window_stream_flush(const float* single, const float* est, const void* state, float* out, int B, int S,
+                               int A, long long W, long long H, void* scratch, cudaStream_t st);
+int window_stream_launch_count(int B, int S, int A, long long C, long long W, long long H);
 
 // tensor-core path (pointwise_mma.cu)
 bool pointwise_mma_eligible(int M, int K);

@@ -10,6 +10,13 @@
 //                           applied on read and overlaps cross-faded
 //   window_carry_kernel     window k0+M-1's raw estimate kept for the next batch
 // No atomics and fixed-order reductions: bitwise reproducible, and independent of how the windows are batched.
+//
+// A windowed stream (DESIGN.md section 7f) runs the same align / scan / overlap-add / carry kernels on each step's
+// q = C / H windows, with every slot's own window origin read from its counter on the device (WinOrigin), and its
+// output origin at the step's first output sample.  Its state per slot is the carry, the last H input samples and
+// the counter c (c H samples received since the slot's reset):
+//   window_stream_gather_kernel   windows c-1 .. c+q-2 out of [history | chunk] into [B][q][A][W] (zeros below 0)
+//   window_stream_history_kernel  the chunk's last H samples become the history
 #include "assign.cuh"
 #include "launch.cuh"
 #include "launchers.cuh"
@@ -43,6 +50,39 @@ struct WindowCarry {
         bytes = pi_bytes + (size_t)B * S * A * W * 4;
     }
 };
+
+// A stream's state: the carry, then the history [B][A][H] fp32, then the window counters [B] (int64), each region
+// starting on a 256-byte boundary.
+struct WindowStreamState {
+    WindowCarry carry;
+    float* hist;
+    long long* count;
+    size_t hist_off, count_off, bytes;
+    WindowStreamState(void* base, int B, int S, int A, long long W, long long H) : carry(base, B, S, A, W) {
+        char* c = static_cast<char*>(base);
+        hist_off = (carry.bytes + 255) / 256 * 256;         // every region 256-byte aligned (the counters are int64)
+        count_off = hist_off + ((size_t)B * A * H * 4 + 255) / 256 * 256;
+        bytes = count_off + (size_t)B * 8;
+        hist = reinterpret_cast<float*>(c ? c + hist_off : nullptr);
+        count = reinterpret_cast<long long*>(c ? c + count_off : nullptr);
+    }
+};
+
+// Where a batch lies in each recording: windows k0 .. k0+M-1 of a recording of T samples.  The offline merge gives
+// every recording the same k0 and T.  A stream reads each slot's counter c: k0 = c + dk and T = c H + dT.
+struct WinOrigin {
+    const long long* count;
+    long long k0, T;
+    __device__ __forceinline__ long long first(long long b) const { return count ? count[b] + k0 : k0; }
+    __device__ __forceinline__ long long length(long long b, long long H) const {
+        return count ? count[b] * H + T : T;
+    }
+};
+constexpr long long kWinUnbounded = 1LL << 62;   // a stream step's T: every window it merges overlaps in full
+
+__host__ __device__ __forceinline__ long long win_count(long long T, long long W, long long H) {
+    return T <= W ? 1 : 1 + (T - W + H - 1) / H;
+}
 
 // Merge scratch: rho [B][M][S], then pis [B][M+1][S] (pis[b][m] = pi of window k0+m-1), int32.
 struct WindowScratch {
@@ -95,12 +135,13 @@ __device__ __forceinline__ void block_sums(double (&v)[N], double* red) {
 template <int S>
 __global__ void __launch_bounds__(kWinThreads)
 window_align_kernel(const float* __restrict__ est, const float* __restrict__ carry_est, int* __restrict__ rho, int B,
-                    int M, int A, long long T, long long W, long long H, long long k0) {
+                    int M, int A, long long W, long long H, WinOrigin org) {
     __shared__ double red[kWinThreads / 32 * S * S];
     const long long bm = blockIdx.x;
-    const long long b = bm / M, m = bm % M, k = k0 + m;
+    const long long b = bm / M, m = bm % M, k = org.first(b) + m, T = org.length(b, H);
     int* out = rho + bm * S;
-    if (k == 0 || S == 1) {        // pi_0 is the identity; one source has nothing to search
+    // pi_0 is the identity; one source has nothing to search; a stream's window below 0 or past its last is never read
+    if (k <= 0 || k >= win_count(T, W, H) || S == 1) {
         if (threadIdx.x < S) out[threadIdx.x] = threadIdx.x;
         return;
     }
@@ -173,12 +214,15 @@ window_align_kernel(const float* __restrict__ est, const float* __restrict__ car
 }
 
 // One thread per recording: pi_{k0-1} (the identity before window 0) composed with rho_k0 .. rho_{k0+M-1}.
-__global__ void window_scan_kernel(const int* __restrict__ rho, int* __restrict__ pis, int* __restrict__ carry_pi,
-                                   int* __restrict__ perm, int B, int S, int M, long long K, long long k0) {
+// carry_out (null: left as it is) receives the last; it may be carry_in.
+__global__ void window_scan_kernel(const int* __restrict__ rho, int* __restrict__ pis, const int* carry_in,
+                                   int* carry_out, int* __restrict__ perm, int B, int S, int M, long long K,
+                                   WinOrigin org) {
     const long long b = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (b >= B) return;
+    const long long k0 = org.first(b);
     int pi[4];
-    for (int s = 0; s < S; ++s) pi[s] = k0 == 0 ? s : carry_pi[b * S + s];
+    for (int s = 0; s < S; ++s) pi[s] = k0 <= 0 ? s : carry_in[b * S + s];
     for (int s = 0; s < S; ++s) pis[b * (M + 1) * S + s] = pi[s];
     for (int m = 0; m < M; ++m) {
         const int* r = rho + (b * M + m) * S;
@@ -187,7 +231,8 @@ __global__ void window_scan_kernel(const int* __restrict__ rho, int* __restrict_
         if (perm)
             for (int s = 0; s < S; ++s) perm[(b * K + k0 + m) * S + s] = pi[s];
     }
-    for (int s = 0; s < S; ++s) carry_pi[b * S + s] = pi[s];
+    if (carry_out)
+        for (int s = 0; s < S; ++s) carry_out[b * S + s] = pi[s];
 }
 
 // The cross-fade of overlap sample j (0 <= j < W - H): the weights 1 - r and r sum to one, so it needs no division by
@@ -197,41 +242,83 @@ __device__ __forceinline__ float window_fade(float prev, float cur, long long j,
     return __fadd_rn(__fmul_rn(__fsub_rn(1.f, r), prev), __fmul_rn(r, cur));
 }
 
-// Row r = (b, s, a) of the output over [t0, t1): sample t takes window k = min(t / H, K - 1) (its latest window) and,
-// when t also lies in window k - 1, the cross-fade of the two; source s of window k is raw source pi_k(s).
+// Row r = (b, s, a) of the output over samples t = k0 H + u, 0 <= u < len: t takes window k = min(t / H, K - 1) (its
+// latest window) and, when t also lies in window k - 1, the cross-fade of the two; source s of window k is raw source
+// pi_k(s), and window k0 - 1 is the carry.  Sample t goes to out[r ld + o0 + u].  A stream's samples below 0 are 0,
+// and `single` (a stream's flush, null otherwise) holds the whole-recording estimate [B][S A][len] of a slot that is
+// one window long and starts at window 0.
 __global__ void __launch_bounds__(kWinThreads)
 window_ola_kernel(const float* __restrict__ est, const float* __restrict__ carry_est, const int* __restrict__ pis,
-                  float* __restrict__ out, long long rows, int S, int A, int M, long long T, long long W, long long H,
-                  long long K, long long k0, long long t0, long long t1) {
+                  const float* __restrict__ single, float* __restrict__ out, long long rows, int S, int A, int M,
+                  long long W, long long H, WinOrigin org, long long len, long long ld, long long o0) {
     const long long SA = (long long)S * A;
     for (long long r = blockIdx.y; r < rows; r += gridDim.y) {
         const long long a = r % A, s = (r / A) % S, b = r / SA;
+        const long long k0 = org.first(b), T = org.length(b, H), K = win_count(T, W, H);
         const int* pb = pis + b * (M + 1) * S;
-        for (long long t = t0 + blockIdx.x * (long long)blockDim.x + threadIdx.x; t < t1;
-             t += (long long)gridDim.x * blockDim.x) {
-            const long long k = min(t / H, K - 1), j = t - k * H, m = k - k0;
-            const float c = est[((b * M + m) * SA + (long long)pb[(m + 1) * S + s] * A + a) * W + j];
-            float v = c;
-            if (k > 0 && j < W - H) {
-                const long long row = (long long)pb[m * S + s] * A + a;
-                const float p = m == 0 ? carry_est[(b * SA + row) * W + H + j]
-                                       : est[((b * M + m - 1) * SA + row) * W + H + j];
-                v = window_fade(p, c, j, W - H);
+        const float* raw = est + b * M * SA * W;             // window k0 + m of recording b (m = -1: the carry)
+        const float* car = carry_est + b * SA * W;
+        for (long long u = blockIdx.x * (long long)blockDim.x + threadIdx.x; u < len;
+             u += (long long)gridDim.x * blockDim.x) {
+            const long long k = min(k0 + u / H, K - 1), j = k0 * H + u - k * H, m = k - k0;
+            float v = 0.f;
+            if (single && k0 == 0 && T <= W) {
+                v = single[r * len + u];
+            } else if (k >= 0) {
+                const long long crow = (long long)pb[(m + 1) * S + s] * A + a;
+                const float c = m < 0 ? car[crow * W + j] : raw[(m * SA + crow) * W + j];
+                v = c;
+                if (k > 0 && j < W - H) {
+                    const long long row = (long long)pb[m * S + s] * A + a;       // m >= 0 here
+                    const float p = m == 0 ? car[row * W + H + j] : raw[((m - 1) * SA + row) * W + H + j];
+                    v = window_fade(p, c, j, W - H);
+                }
             }
-            out[r * T + t] = v;
+            out[r * ld + o0 + u] = v;
         }
     }
 }
 
+// Also advances a stream's counters (null: none) by `advance` windows, after every kernel that reads them.
 __global__ void __launch_bounds__(kWinThreads)
 window_carry_kernel(const float* __restrict__ est, float* __restrict__ carry_est, long long rows, long long SA, int M,
-                    long long W) {
+                    long long W, long long* __restrict__ count, long long advance) {
     for (long long r = blockIdx.y; r < rows; r += gridDim.y) {       // r = b SA + row
         const float* src = est + ((r / SA * M + M - 1) * SA + r % SA) * W;
         for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < W;
              t += (long long)gridDim.x * blockDim.x)
             carry_est[r * W + t] = src[t];
+        if (count && r % SA == 0 && blockIdx.x == 0 && threadIdx.x == 0) count[r / SA] += advance;
     }
+}
+
+// Window m of slot b's step is window c - 1 + m, samples [m H, m H + W) of [history (H) | chunk (C)]; zeros below
+// window 0.  chunk = null (C = 0, q = 1): the flush's window, the history followed by zeros.
+__global__ void __launch_bounds__(kWinThreads)
+window_stream_gather_kernel(const float* __restrict__ hist, const float* __restrict__ chunk,
+                            const long long* __restrict__ count, float* __restrict__ batch, long long rows, int q,
+                            int A, long long C, long long W, long long H) {
+    for (long long r = blockIdx.y; r < rows; r += gridDim.y) {       // r = (b q + m) A + a
+        const long long a = r % A, bm = r / A, m = bm % q, b = bm / q;
+        const bool valid = count[b] - 1 + m >= 0;
+        const float* h = hist + (b * A + a) * H;
+        const float* x = chunk ? chunk + (b * A + a) * C : nullptr;
+        float* dst = batch + r * W;
+        for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < W;
+             t += (long long)gridDim.x * blockDim.x) {
+            const long long p = m * H + t;
+            dst[t] = !valid ? 0.f : p < H ? h[p] : x && p - H < C ? x[p - H] : 0.f;
+        }
+    }
+}
+
+__global__ void __launch_bounds__(kWinThreads)
+window_stream_history_kernel(const float* __restrict__ chunk, float* __restrict__ hist, long long rows, long long C,
+                             long long H) {
+    for (long long r = blockIdx.y; r < rows; r += gridDim.y)         // r = b A + a
+        for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < H;
+             t += (long long)gridDim.x * blockDim.x)
+            hist[r * H + t] = chunk[r * C + C - H + t];
 }
 
 long long window_count(long long T, long long W, long long H) {
@@ -259,6 +346,31 @@ int launch_window_gather(const float* x, float* batch, int B, int A, long long T
                   k0);
 }
 
+// Align, scan and overlap-add windows org.first(b) .. + M - 1 of every recording.  `single` non-null: a stream's flush,
+// which leaves the carry as it is.  Otherwise the carry receives the batch's last window and a stream's counters
+// (null for the offline merge) advance by `advance`.
+static int merge_stages(const float* est, const WindowCarry& c, const float* single, int* perm, float* out, int B,
+                        int S, int A, long long W, long long H, int M, WinOrigin org, long long K, long long len,
+                        long long ld, long long o0, void* scratch, long long* count, long long advance,
+                        cudaStream_t st) {
+    const WindowScratch s(scratch, B, S, M);
+    int e = with_sources(S, [&](auto sc) {
+        return launch(window_align_kernel<decltype(sc)::value>, (unsigned)((long long)B * M), kWinThreads, 0, st, est,
+                      c.est, s.rho, B, M, A, W, H, org);
+    });
+    if (e) return e;
+    if ((e = launch(window_scan_kernel, (unsigned)((B + 127) / 128), 128, 0, st, s.rho, s.pis, c.pi,
+                    single ? nullptr : c.pi, perm, B, S, M, K, org)))
+        return e;
+    const long long rows = (long long)B * S * A;
+    if ((e = launch(window_ola_kernel, row_tiled_grid(rows, len), kWinThreads, 0, st, est, c.est, s.pis, single, out,
+                    rows, S, A, M, W, H, org, len, ld, o0)))
+        return e;
+    if (single) return SDR_OK;
+    return launch(window_carry_kernel, row_tiled_grid(rows, W), kWinThreads, 0, st, est, c.est, rows,
+                  (long long)S * A, M, W, count, advance);
+}
+
 int launch_window_merge(const float* est, void* carry, int* perm, float* out, int B, int S, int A, long long T,
                         long long W, long long H, long long k0, int M, void* scratch, cudaStream_t st) {
     if (!est || !carry || !out || !scratch) return SDR_ERR_BAD_ARGUMENT;
@@ -268,22 +380,96 @@ int launch_window_merge(const float* est, void* carry, int* perm, float* out, in
     const WindowPlan g(T, W, H);
     if (!g.ok || B <= 0 || S <= 0 || A <= 0 || M <= 0 || k0 < 0 || k0 + M > g.K) return SDR_ERR_BAD_ARGUMENT;
     const WindowCarry c(carry, B, S, A, W);
-    const WindowScratch s(scratch, B, S, M);
-    int e = with_sources(S, [&](auto sc) {
-        return launch(window_align_kernel<decltype(sc)::value>, (unsigned)((long long)B * M), kWinThreads, 0, st, est,
-                      c.est, s.rho, B, M, A, T, W, H, k0);
-    });
-    if (e) return e;
-    if ((e = launch(window_scan_kernel, (unsigned)((B + 127) / 128), 128, 0, st, s.rho, s.pis, c.pi, perm, B, S, M,
-                    g.K, k0)))
-        return e;
     const long long t0 = k0 * H, t1 = k0 + M == g.K ? T : (k0 + M) * H;
-    const long long rows = (long long)B * S * A;
-    if ((e = launch(window_ola_kernel, row_tiled_grid(rows, t1 - t0), kWinThreads, 0, st, est, c.est, s.pis, out,
-                    rows, S, A, M, T, W, H, g.K, k0, t0, t1)))
-        return e;
-    return launch(window_carry_kernel, row_tiled_grid(rows, W), kWinThreads, 0, st, est, c.est, rows,
-                  (long long)S * A, M, W);
+    return merge_stages(est, c, nullptr, perm, out, B, S, A, W, H, M, WinOrigin{nullptr, k0, T}, g.K, t1 - t0, T, t0,
+                        scratch, nullptr, 0, st);
+}
+
+// ---- windowed stream (DESIGN.md section 7f) ----------------------------------------------------------------------
+
+static bool stream_shape_ok(int B, int S, int A, long long W, long long H) {
+    return B > 0 && S > 0 && S <= 4 && A > 0 && WindowPlan(W + 1, W, H).ok;
+}
+
+size_t window_stream_state_bytes(int B, int S, int A, long long W, long long H) {
+    if (!stream_shape_ok(B, S, A, W, H)) return 0;
+    return WindowStreamState(nullptr, B, S, A, W, H).bytes;
+}
+
+int window_stream_reset(void* state, int B, int S, int A, long long W, long long H, const int* slots, int n,
+                        cudaStream_t st) {
+    if (!state || (slots && n < 0)) return SDR_ERR_BAD_ARGUMENT;
+    if (!stream_shape_ok(B, S, A, W, H)) return S > 4 ? SDR_ERR_UNSUPPORTED : SDR_ERR_BAD_ARGUMENT;
+    if (reinterpret_cast<uintptr_t>(state) % 256) return SDR_ERR_BAD_ARGUMENT;
+    const WindowStreamState ss(state, B, S, A, W, H);
+    if (!slots) return cudaMemsetAsync(state, 0, ss.bytes, st) == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
+    for (int i = 0; i < n; ++i)
+        if (slots[i] < 0 || slots[i] >= B) return SDR_ERR_BAD_ARGUMENT;
+    const size_t SAW = (size_t)S * A * W, AH = (size_t)A * H;
+    for (int i = 0; i < n; ++i) {      // the counter alone decides what a step reads; the rest is zeroed for hygiene
+        const size_t b = slots[i];
+        if (cudaMemsetAsync(ss.carry.pi + b * S, 0, (size_t)S * 4, st) != cudaSuccess ||
+            cudaMemsetAsync(ss.carry.est + b * SAW, 0, SAW * 4, st) != cudaSuccess ||
+            cudaMemsetAsync(ss.hist + b * AH, 0, AH * 4, st) != cudaSuccess ||
+            cudaMemsetAsync(ss.count + b, 0, 8, st) != cudaSuccess)
+            return SDR_ERR_CUDA;
+    }
+    return SDR_OK;
+}
+
+// C = 0 with chunk null: the flush's window [B][A][W]; nothing in the state changes.
+int launch_window_stream_gather(void* state, const float* chunk, float* batch, int B, int S, int A, long long C,
+                                long long W, long long H, cudaStream_t st) {
+    if (!state || !batch || (!chunk && C != 0)) return SDR_ERR_BAD_ARGUMENT;
+    if (!stream_shape_ok(B, S, A, W, H)) return S > 4 ? SDR_ERR_UNSUPPORTED : SDR_ERR_BAD_ARGUMENT;
+    if (chunk && (C <= 0 || C % H)) return SDR_ERR_BAD_ARGUMENT;
+    if (reinterpret_cast<uintptr_t>(state) % 256) return SDR_ERR_BAD_ARGUMENT;
+    const WindowStreamState ss(state, B, S, A, W, H);
+    const int q = chunk ? (int)(C / H) : 1;
+    const long long rows = (long long)B * q * A;
+    int e = launch(window_stream_gather_kernel, row_tiled_grid(rows, W), kWinThreads, 0, st, ss.hist, chunk, ss.count,
+                   batch, rows, q, A, C, W, H);
+    if (e || !chunk) return e;
+    return launch(window_stream_history_kernel, row_tiled_grid((long long)B * A, H), kWinThreads, 0, st, chunk,
+                  ss.hist, (long long)B * A, C, H);
+}
+
+size_t window_stream_merge_scratch_bytes(int B, int S, long long C, long long H) {
+    if (B <= 0 || S <= 0 || S > 4 || H <= 0 || C <= 0 || C % H || C / H > (1 << 30)) return 0;
+    return WindowScratch(nullptr, B, S, (int)(C / H)).bytes;
+}
+
+int launch_window_stream_merge(const float* est, void* state, float* out, int B, int S, int A, long long C,
+                               long long W, long long H, void* scratch, cudaStream_t st) {
+    if (!est || !state || !out || !scratch) return SDR_ERR_BAD_ARGUMENT;
+    if (!stream_shape_ok(B, S, A, W, H)) return S > 4 ? SDR_ERR_UNSUPPORTED : SDR_ERR_BAD_ARGUMENT;
+    if (window_stream_merge_scratch_bytes(B, S, C, H) == 0) return SDR_ERR_BAD_ARGUMENT;
+    if (reinterpret_cast<uintptr_t>(state) % 256 || reinterpret_cast<uintptr_t>(scratch) % 8)
+        return SDR_ERR_BAD_ARGUMENT;
+    WindowStreamState ss(state, B, S, A, W, H);
+    const int q = (int)(C / H);
+    return merge_stages(est, ss.carry, nullptr, nullptr, out, B, S, A, W, H, q, WinOrigin{ss.count, -1, kWinUnbounded},
+                        kWinUnbounded, C, C, 0, scratch, ss.count, q, st);
+}
+
+size_t window_stream_flush_scratch_bytes(int B, int S) { return window_merge_scratch_bytes(B, S, 1); }
+
+int launch_window_stream_flush(const float* single, const float* est, const void* state, float* out, int B, int S,
+                               int A, long long W, long long H, void* scratch, cudaStream_t st) {
+    if (!single || !state || !out || !scratch || (!est && W < 2 * H)) return SDR_ERR_BAD_ARGUMENT;
+    if (!stream_shape_ok(B, S, A, W, H)) return S > 4 ? SDR_ERR_UNSUPPORTED : SDR_ERR_BAD_ARGUMENT;
+    if (reinterpret_cast<uintptr_t>(state) % 256 || reinterpret_cast<uintptr_t>(scratch) % 8)
+        return SDR_ERR_BAD_ARGUMENT;
+    // the state is only read: the carry's pi is not written when `single` is given
+    WindowStreamState ss(const_cast<void*>(state), B, S, A, W, H);
+    return merge_stages(est, ss.carry, single, nullptr, out, B, S, A, W, H, 1, WinOrigin{ss.count, -1, 0}, 0, H, H, 0,
+                        scratch, nullptr, 0, st);
+}
+
+int window_stream_launch_count(int B, int S, int A, long long C, long long W, long long H) {
+    if (!stream_shape_ok(B, S, A, W, H)) return S > 4 ? SDR_ERR_UNSUPPORTED : SDR_ERR_BAD_ARGUMENT;
+    if (window_stream_merge_scratch_bytes(B, S, C, H) == 0) return SDR_ERR_BAD_ARGUMENT;
+    return 6;          // gather, history; align, scan, overlap-add, carry (the forward between them not counted)
 }
 
 }  // namespace sdr

@@ -10,7 +10,7 @@ import torch
 import torch.nn as nn
 
 from . import _engine
-from . import windowed
+from . import window_stream, windowed
 from .improved_sudormrf import (GlobLN, ConvNormAct, NormAct, DilatedConvNorm, UConvBlock,
                                 _LayerNorm, _not_standalone, _xavier_uniform_)
 
@@ -110,6 +110,13 @@ class GroupCommSudoRmRf(_engine.NativeModuleMixin, nn.Module):
         ``windowed.separate_long``)."""
         return windowed.separate_long(self, input_wav, window, hop, normalize=normalize,
                                       mixture_consistency=mixture_consistency, max_windows=max_windows)
+
+    def stream_windows(self, batch_size, chunk_samples, window, hop=None, normalize=True,
+                       mixture_consistency=True):
+        """A ``window_stream.WindowedStream``: ``separate_long``'s windows taken step by step for ``batch_size``
+        slots of ``chunk_samples`` samples per step (a multiple of the hop), one hop late."""
+        return window_stream.WindowedStream(self, batch_size, chunk_samples, window, hop, normalize=normalize,
+                                            mixture_consistency=mixture_consistency)
 
     def forward_host(self, host_wav, host_out=None, mixture_consistency=False):
         return _engine.forward_host(self, host_wav, host_out, mixture_consistency)

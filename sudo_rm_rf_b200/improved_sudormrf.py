@@ -20,7 +20,7 @@ import torch
 import torch.nn as nn
 
 from . import _engine
-from . import windowed
+from . import window_stream, windowed
 from . import training
 
 
@@ -181,6 +181,13 @@ class SuDORMRF(_engine.NativeModuleMixin, nn.Module):
         ``windowed.separate_long``)."""
         return windowed.separate_long(self, input_wav, window, hop, normalize=normalize,
                                       mixture_consistency=mixture_consistency, max_windows=max_windows)
+
+    def stream_windows(self, batch_size, chunk_samples, window, hop=None, normalize=True,
+                       mixture_consistency=False):
+        """A ``window_stream.WindowedStream``: ``separate_long``'s windows taken step by step for ``batch_size``
+        slots of ``chunk_samples`` samples per step (a multiple of the hop), one hop late."""
+        return window_stream.WindowedStream(self, batch_size, chunk_samples, window, hop, normalize=normalize,
+                                            mixture_consistency=mixture_consistency)
 
     def forward_host(self, host_wav, host_out=None, mixture_consistency=False):
         """End-to-end call on pinned HOST tensors (H2D, forward, D2H on the current stream)."""
