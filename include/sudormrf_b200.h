@@ -482,6 +482,21 @@ int sdr_stoi(const float* reference, const float* estimate, const float* mixture
              const int64_t* lengths_or_null, double* stoi, double* mix_stoi_or_null, int B, int S, int64_t T, int fs,
              void* scratch, sdr_stream stream);
 
+/* ---- polyphase resampling (DESIGN.md section 7g) ---------------------------
+ * scipy.signal.resample_poly(x, up, down) with its defaults (window=('kaiser', 5.0), padtype='constant') on every row
+ * of x [rows][T] fp32 -> out [rows][ceil(T p / q)] fp32, up / down reduced to p / q by their gcd.  The filter is
+ * firwin(2L + 1, 1 / max(p, q), window=('kaiser', 5.0)) * p with L = 10 max(p, q), designed on the device into
+ * scratch; out[i] = sum_t h[i q + L - t p] x[t] over the taps inside [0, 2L], summed in fp64 in ascending t and
+ * rounded once, so every row is bitwise independent of the others and of rows.  A NaN or infinity in x[t] makes
+ * exactly the outputs whose support holds t non-finite.  p == q copies x.  up, down >= 1 and max(p, q) <= 4096 (else
+ * 0 / SDR_ERR_UNSUPPORTED; up or down < 1: SDR_ERR_BAD_ARGUMENT), rows >= 1, 1 <= T <= 2^40.  Scratch:
+ * sdr_resample_poly_scratch_bytes(up, down) = 8 (20 max(p, q) + 1), 8-byte aligned; a null, misaligned
+ * (SDR_ERR_BAD_ARGUMENT) or smaller (SDR_ERR_WORKSPACE) scratch is refused before anything is enqueued.  x and out
+ * must not overlap.  No call synchronises or allocates: a call can be captured in a CUDA graph. */
+size_t sdr_resample_poly_scratch_bytes(int up, int down);
+int    sdr_resample_poly(const float* x, float* out, int64_t rows, int64_t T, int up, int down, void* scratch,
+                         size_t scratch_bytes, sdr_stream stream);
+
 /* ---- windowed separation of long recordings (DESIGN.md section 7e) ---------
  * A recording of T samples is cut into K = sdr_window_count(T, W, H) windows (1 when T <= W, else
  * 1 + ceil((T - W) / H)); window k covers samples [k H, k H + W), zeros at T and beyond.  W/2 <= H < W and

@@ -8,12 +8,13 @@ exported here as ``OriginalSuDORMRF``) /
 ``sudo_rm_rf.dnn.experiments.utils.mixture_consistency`` of etzinis/sudo_rm_rf, and the FUSS training loss
 ``PermInvariantSNRwithZeroRefs`` of ``sudo_rm_rf.dnn.losses.snr`` (module ``snr``), and the BSS-eval
 source criteria of the evaluation scripts (``bss_eval_sources``, mir_eval's definition) and their STOI (``stoi``,
-pystoi's definition; module ``stoi_metric``).
+pystoi's definition; module ``stoi_metric``), and scipy's ``resample_poly`` (module ``resample``).
 """
 from . import improved_sudormrf, groupcomm_sudormrf_v2, causal_improved_sudormrf_v3, sudormrf, mixture_consistency   # noqa: F401
 from . import snr                                                             # noqa: F401
 from .bss_eval import bss_eval_sources                                         # noqa: F401
 from .stoi_metric import stoi                                                 # noqa: F401
+from .resample import resample_poly                                           # noqa: F401
 from .improved_sudormrf import SuDORMRF                                       # noqa: F401
 from .groupcomm_sudormrf_v2 import GroupCommSudoRmRf                          # noqa: F401
 from .causal_improved_sudormrf_v3 import CausalSuDORMRF                       # noqa: F401
@@ -23,4 +24,4 @@ from .window_stream import WindowedStream                                     # 
 
 __all__ = ["SuDORMRF", "GroupCommSudoRmRf", "CausalSuDORMRF", "OriginalSuDORMRF", "improved_sudormrf",
            "groupcomm_sudormrf_v2", "causal_improved_sudormrf_v3", "sudormrf", "mixture_consistency", "snr",
-           "bss_eval_sources", "stoi", "refresh_weights", "WindowedStream"]
+           "bss_eval_sources", "stoi", "resample_poly", "refresh_weights", "WindowedStream"]

@@ -160,6 +160,9 @@ _SIGNATURES = {
     "sdr_stoi_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int64, C.c_int]),
     "sdr_stoi": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                            C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
+    "sdr_resample_poly_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "sdr_resample_poly": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_void_p,
+                                    C.c_size_t, C.c_void_p]),
     "sdr_window_count": (C.c_int64, [C.c_int64, C.c_int64, C.c_int64]),
     "sdr_window_carry_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int64]),
     "sdr_window_merge_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),

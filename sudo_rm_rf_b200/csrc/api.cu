@@ -1477,6 +1477,13 @@ int sdr_stoi(const float* reference, const float* estimate, const float* mixture
                        mix_stoi_or_null, B, S, T, fs, scratch, static_cast<cudaStream_t>(stream));
 }
 
+size_t sdr_resample_poly_scratch_bytes(int up, int down) { return resample_poly_scratch_bytes(up, down); }
+
+int sdr_resample_poly(const float* x, float* out, int64_t rows, int64_t T, int up, int down, void* scratch,
+                      size_t scratch_bytes, sdr_stream stream) {
+    return launch_resample_poly(x, out, rows, T, up, down, scratch, scratch_bytes, static_cast<cudaStream_t>(stream));
+}
+
 int64_t sdr_window_count(int64_t T, int64_t W, int64_t H) { return window_count(T, W, H); }
 
 size_t sdr_window_carry_bytes(int B, int S, int A, int64_t W) { return window_carry_bytes(B, S, A, W); }

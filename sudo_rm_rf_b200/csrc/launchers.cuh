@@ -121,6 +121,11 @@ size_t stoi_scratch_bytes(int B, int S, long long T, int fs);
 int launch_stoi(const float* ref, const float* est, const float* mix, const long long* lengths, double* out,
                 double* mout, int B, int S, long long T, int fs, void* scratch, cudaStream_t st);
 
+// polyphase resampling (resample.cu)
+size_t resample_poly_scratch_bytes(int up, int down);
+int launch_resample_poly(const float* x, float* out, long long rows, long long T, int up, int down, void* scratch,
+                         size_t scratch_bytes, cudaStream_t st);
+
 // windowed separation (windowed.cu)
 long long window_count(long long T, long long W, long long H);
 size_t window_carry_bytes(int B, int S, int A, long long W);

@@ -17,6 +17,7 @@
 #include <cmath>
 #include <numeric>
 #include "launchers.cuh"
+#include "resample.cuh"
 
 namespace sdr {
 
@@ -78,21 +79,8 @@ struct StoiScratch {
     }
 };
 
-__device__ __forceinline__ long long stoi_resampled(long long len, int p, int q) { return (len * p + q - 1) / q; }
-
 // np.hanning(258)[1:-1][k] = 0.5 + 0.5 cos(pi (2k - 255) / 257)
 __device__ __forceinline__ double stoi_hann(int k) { return 0.5 + 0.5 * cospi((2.0 * k - 255.0) / 257.0); }
-
-// The modified Bessel function I0 by its power series sum ((x/2)^k / k!)^2, to full precision for x <= 6.
-__device__ double stoi_i0(double x) {
-    const double q = 0.25 * x * x;
-    double term = 1.0, sum = 1.0;
-    for (int k = 1; k < 64 && term > 1e-18 * sum; ++k) {
-        term *= q / ((double)k * k);
-        sum += term;
-    }
-    return sum;
-}
 
 // One CTA of 256 threads.  h[t + L] = kaiser(2L+1, 0.1102 (60 - 8.7))[t + L] * 2 p cutoff sinc(2 cutoff t),
 // cutoff = 1 / (2 max(p, q)), then h / sum(h) * p: pystoi's window normalised to sum 1, times resample_poly's gain p.
@@ -105,16 +93,11 @@ __global__ void __launch_bounds__(256) stoi_filter_kernel(double* __restrict__ h
         return;
     }
     const int taps = 2 * L + 1;
-    const double cutoff = 1.0 / (2.0 * (double)(p > q ? p : q));
     const double beta = 0.1102 * (60.0 - 8.7);
-    const double i0b = stoi_i0(beta);
+    const double i0b = resample_i0(beta);
     double part = 0.0;
     for (int i = threadIdx.x; i < taps; i += 256) {
-        const int t = i - L;
-        const double a = 2.0 * cutoff * t;
-        const double sinc = t == 0 ? 1.0 : sinpi(a) / (CUDART_PI * a);
-        const double r = (double)(i - L) / (double)L;
-        const double v = stoi_i0(beta * sqrt(1.0 - r * r)) / i0b * (2.0 * p * cutoff * sinc);
+        const double v = kaiser_sinc_tap(i, L, p > q ? p : q, beta, i0b, 2.0 * p);
         h[i] = v;
         part += v;
     }
@@ -145,15 +128,13 @@ stoi_resample_kernel(const float* __restrict__ ref, const float* __restrict__ es
         else { b = row - 2 * R; x = mix + b * T; }
         const long long len = lengths ? lengths[b] : T;
         if (len < 1 || len > T) continue;
-        const long long n = stoi_resampled(len, p, q);
+        const long long n = resampled_length(len, p, q);
         double* out = sig + row * Tn;
         for (long long i = blockIdx.x * 256LL + threadIdx.x; i < n; i += gridDim.x * 256LL) {
-            const long long c = i * q + L;                      // tap index c - t p, in [0, 2L]
-            const long long lo = c - 2LL * L;
-            const long long t0 = lo <= 0 ? 0 : (lo + p - 1) / p;
-            const long long t1 = c / p < len - 1 ? c / p : len - 1;
+            const long long c = i * q + L;
+            const ResampleSupport s = resample_support(c / p, (int)(c % p), p, L, len);
             double acc = 0.0;
-            for (long long t = t0; t <= t1; ++t) acc = fma(__ldg(h + (c - t * p)), (double)__ldg(x + t), acc);
+            for (long long t = s.t0; t <= s.t1; ++t) acc = fma(__ldg(h + (c - t * p)), (double)__ldg(x + t), acc);
             out[i] = acc;
         }
     }
@@ -192,7 +173,7 @@ stoi_mask_kernel(const float* __restrict__ ref, const float* __restrict__ est, c
     for (int k = threadIdx.x; k < kStoiFrame; k += 512) win[k] = stoi_hann(k);
     if (threadIdx.x == 0) base = 0;
     __syncthreads();
-    const long long n = stoi_resampled(len, p, q);
+    const long long n = resampled_length(len, p, q);
     const long long F0 = n > kStoiFrame ? (n - kStoiFrame + kStoiHop - 1) / kStoiHop : 0;
     const double* x = sig + r * Tn;
     double* e = energy + r * F0max;

@@ -20,7 +20,7 @@ import torch
 import torch.nn as nn
 
 from . import _engine
-from . import window_stream, windowed
+from . import resample, window_stream, windowed
 from . import training
 
 
@@ -162,25 +162,33 @@ class SuDORMRF(_engine.NativeModuleMixin, nn.Module):
             return training.forward(self, input_wav)
         return _engine.forward(self, input_wav, mixture_consistency=False)
 
-    def separate(self, input_wav, mixture_consistency=False, normalize=False):
+    def separate(self, input_wav, mixture_consistency=False, normalize=False, sample_rate=None, model_rate=None):
         """forward() with the uniform mixture-consistency projection
         (mixture_consistency.py:14-36) fused into the decoder epilogue.
 
         ``normalize=True`` runs the whole README recipe (reference README.md:100-114) on the
         device: ``input_wav`` is the raw mixture ``[B, T]`` or ``[B, 1, T]``; it is normalised per
         utterance (mean, unbiased std), separated, and the estimates are rescaled with the
-        mixture's std and mean (then, optionally, projected onto the normalised mixture)."""
-        if normalize:
-            return _engine.separate(self, input_wav, mixture_consistency=mixture_consistency)
-        return _engine.forward(self, input_wav, mixture_consistency=mixture_consistency)
+        mixture's std and mean (then, optionally, projected onto the normalised mixture).
+
+        ``sample_rate`` and ``model_rate`` (both or neither): the mixture's rate and the rate the model was trained
+        at.  When they differ the mixture is resampled to ``model_rate`` (``resample.resample_poly``), separated there,
+        and every source is resampled back and cropped to the input's length, so the sources sum to the band-limited
+        mixture rather than to the mixture itself (``resample.at_model_rate``)."""
+        run = _engine.separate if normalize else _engine.forward
+        return resample.at_model_rate(lambda wav: run(self, wav, mixture_consistency=mixture_consistency),
+                                      input_wav, sample_rate, model_rate)
 
     def separate_long(self, input_wav, window, hop=None, normalize=True, mixture_consistency=False,
-                      max_windows=32):
+                      max_windows=32, sample_rate=None, model_rate=None):
         """``separate`` for recordings of any length: overlapping windows of ``window`` samples every ``hop``,
         separated in batches of ``max_windows`` per recording, aligned and cross-faded on the device (see
-        ``windowed.separate_long``)."""
-        return windowed.separate_long(self, input_wav, window, hop, normalize=normalize,
-                                      mixture_consistency=mixture_consistency, max_windows=max_windows)
+        ``windowed.separate_long``).  ``window`` and ``hop`` count samples at ``model_rate``; ``sample_rate`` and
+        ``model_rate`` as for ``separate``."""
+        return resample.at_model_rate(
+            lambda wav: windowed.separate_long(self, wav, window, hop, normalize=normalize,
+                                               mixture_consistency=mixture_consistency, max_windows=max_windows),
+            input_wav, sample_rate, model_rate)
 
     def stream_windows(self, batch_size, chunk_samples, window, hop=None, normalize=True,
                        mixture_consistency=False):
