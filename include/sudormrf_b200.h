@@ -171,6 +171,9 @@ int     sdr_stream_reset(const sdr_config* cfg, void* state, int B, const int32_
                          sdr_stream stream);
 /* chunk [B, A, C] -> out [B, S*A, C]: the model's output samples c*C - hop .. (c+1)*C - hop - 1 of the c-th step;
  * apply_mixture_consistency: the uniform projection against the mixture delayed by hop (mono models only)      */
+/* sdr_stream_reset of the slots b < B whose mask[b] (device memory, uint8) is nonzero: the same bytes, with the slots
+ * chosen on the device, so that a captured graph can reset them */
+int     sdr_stream_reset_masked(const sdr_config* cfg, void* state, int B, const uint8_t* mask, sdr_stream stream);
 int     sdr_stream_step(const sdr_config* cfg, const void* packed, void* state, const float* chunk, float* out,
                         int B, int64_t C, int apply_mixture_consistency, void* ws, size_t ws_bytes, sdr_stream stream);
 /* tail [B, S*A, hop]: the pending overlap-add sums; the state is left as it is */
@@ -497,6 +500,37 @@ size_t sdr_resample_poly_scratch_bytes(int up, int down);
 int    sdr_resample_poly(const float* x, float* out, int64_t rows, int64_t T, int up, int down, void* scratch,
                          size_t scratch_bytes, sdr_stream stream);
 
+/* ---- streaming resampler (DESIGN.md section 7h) ----------------------------
+ * resample_poly chunk by chunk for B independent slots of `rows` rows.  With up / down reduced to p / q (p != q,
+ * max(p, q) <= 4096) and L = 10 max(p, q), per slot let s be `lead` zeros followed by everything the slot received
+ * since its reset and r = resample_poly(s) as sdr_resample_poly computes it.  Step j since the reset takes chunk
+ * [B][rows][C] (C a positive multiple of q) and writes out [B][rows][C p / q] = samples [j C p / q - delay,
+ * (j + 1) C p / q - delay) of r, zeros below index 0.  The flush takes tail_or_null [B][rows][tail_len] (any
+ * tail_len >= 0) and writes out [B][rows][ceil((lead + tail_len) p / q) + delay] = the rest of r with s extended by
+ * the tail, up to ceil(len(s) p / q); it leaves the state as it was.  Every value is bitwise sdr_resample_poly's on
+ * the concatenation: the same filter, each output summed in fp64 by fma in ascending input index over the same
+ * support and rounded once.  delay >= floor((L - lead p) / q) (the smallest delay at which every output of a step has
+ * its whole support received), 0 <= lead <= 2^40, 1 <= B <= 65535, rows >= 1.  zero_slots_or_null (device, uint8
+ * [B]): the chunk or tail of a slot whose byte is nonzero is read as zeros.
+ * State: sdr_resample_stream_state_bytes(...), 256-byte aligned: the filter [2L + 1] fp64, the step counters [B]
+ * int64 and two histories [2][B][rows][Hs] fp32, Hs = lead + floor((delay q + L) / p) + 1, each region on a 256-byte
+ * boundary (0 bytes for arguments the entries refuse).  sdr_resample_stream_reset with host_slots_or_null = NULL
+ * designs the filter and zeroes every slot; with n slots listed in host memory it zeroes those slots' counters and
+ * histories.  A step is two launches (the outputs and the next history, then the counters), the flush one.  Every
+ * entry refuses a null (SDR_ERR_BAD_ARGUMENT), small (SDR_ERR_WORKSPACE) or misaligned (SDR_ERR_BAD_ARGUMENT) state
+ * and arguments out of range (SDR_ERR_BAD_ARGUMENT; p == q or max(p, q) > 4096: SDR_ERR_UNSUPPORTED) before anything
+ * is enqueued.  No atomics and no synchronisation: a step with fixed buffers can be captured in a CUDA graph. */
+size_t sdr_resample_stream_state_bytes(int B, int rows, int64_t C, int up, int down, int64_t delay, int64_t lead);
+int    sdr_resample_stream_reset(void* state, size_t state_bytes, int B, int rows, int64_t C, int up, int down,
+                                 int64_t delay, int64_t lead, const int32_t* host_slots_or_null, int n,
+                                 sdr_stream stream);
+int    sdr_resample_stream_step(void* state, size_t state_bytes, const float* chunk, const uint8_t* zero_slots_or_null,
+                                float* out, int B, int rows, int64_t C, int up, int down, int64_t delay, int64_t lead,
+                                sdr_stream stream);
+int    sdr_resample_stream_flush(const void* state, size_t state_bytes, const float* tail_or_null, int64_t tail_len,
+                                 const uint8_t* zero_slots_or_null, float* out, int B, int rows, int64_t C, int up,
+                                 int down, int64_t delay, int64_t lead, sdr_stream stream);
+
 /* ---- windowed separation of long recordings (DESIGN.md section 7e) ---------
  * A recording of T samples is cut into K = sdr_window_count(T, W, H) windows (1 when T <= W, else
  * 1 + ceil((T - W) / H)); window k covers samples [k H, k H + W), zeros at T and beyond.  W/2 <= H < W and
@@ -553,6 +587,9 @@ int     sdr_window_merge(const float* estimates, void* carry, int32_t* perm_or_n
 size_t sdr_window_stream_state_bytes(int B, int S, int A, int64_t W, int64_t H);
 int    sdr_window_stream_reset(void* state, int B, int S, int A, int64_t W, int64_t H,
                                const int32_t* host_slots_or_null, int n, sdr_stream stream);
+/* sdr_window_stream_reset of the slots b < B whose mask[b] (device memory, uint8) is nonzero, chosen on the device */
+int    sdr_window_stream_reset_masked(void* state, int B, int S, int A, int64_t W, int64_t H, const uint8_t* mask,
+                                      sdr_stream stream);
 int    sdr_window_stream_gather(void* state, const float* chunk_or_null, float* batch, int B, int S, int A, int64_t C,
                                 int64_t W, int64_t H, sdr_stream stream);
 size_t sdr_window_stream_merge_scratch_bytes(int B, int S, int64_t C, int64_t H);

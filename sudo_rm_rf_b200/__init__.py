@@ -21,7 +21,9 @@ from .causal_improved_sudormrf_v3 import CausalSuDORMRF                       # 
 from .sudormrf import SuDORMRF as OriginalSuDORMRF                            # noqa: F401
 from ._engine import refresh_weights                                          # noqa: F401
 from .window_stream import WindowedStream                                     # noqa: F401
+from .resample_stream import ResampleStream, ResampledStream                   # noqa: F401
 
 __all__ = ["SuDORMRF", "GroupCommSudoRmRf", "CausalSuDORMRF", "OriginalSuDORMRF", "improved_sudormrf",
            "groupcomm_sudormrf_v2", "causal_improved_sudormrf_v3", "sudormrf", "mixture_consistency", "snr",
-           "bss_eval_sources", "stoi", "resample_poly", "refresh_weights", "WindowedStream"]
+           "bss_eval_sources", "stoi", "resample_poly", "refresh_weights", "WindowedStream",
+           "ResampleStream", "ResampledStream"]

@@ -67,6 +67,7 @@ _SIGNATURES = {
     "sdr_stream_workspace_bytes": (C.c_size_t, [C.POINTER(SdrConfig), C.c_int, C.c_int64]),
     "sdr_stream_launch_count": (C.c_int, [C.POINTER(SdrConfig), C.c_int, C.c_int64]),
     "sdr_stream_reset": (C.c_int, [C.POINTER(SdrConfig), C.c_void_p, C.c_int, C.c_void_p, C.c_int, C.c_void_p]),
+    "sdr_stream_reset_masked": (C.c_int, [C.POINTER(SdrConfig), C.c_void_p, C.c_int, C.c_void_p, C.c_void_p]),
     "sdr_stream_step": (C.c_int, [C.POINTER(SdrConfig), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
                                   C.c_int64, C.c_int, C.c_void_p, C.c_size_t, C.c_void_p]),
     "sdr_stream_flush": (C.c_int, [C.POINTER(SdrConfig), C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_void_p]),
@@ -163,6 +164,15 @@ _SIGNATURES = {
     "sdr_resample_poly_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int]),
     "sdr_resample_poly": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_void_p,
                                     C.c_size_t, C.c_void_p]),
+    "sdr_resample_stream_state_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int64,
+                                                     C.c_int64]),
+    "sdr_resample_stream_reset": (C.c_int, [C.c_void_p, C.c_size_t, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int,
+                                            C.c_int64, C.c_int64, C.c_void_p, C.c_int, C.c_void_p]),
+    "sdr_resample_stream_step": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
+                                           C.c_int64, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_void_p]),
+    "sdr_resample_stream_flush": (C.c_int, [C.c_void_p, C.c_size_t, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p,
+                                            C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_int64, C.c_int64,
+                                            C.c_void_p]),
     "sdr_window_count": (C.c_int64, [C.c_int64, C.c_int64, C.c_int64]),
     "sdr_window_carry_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int64]),
     "sdr_window_merge_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int]),
@@ -173,6 +183,8 @@ _SIGNATURES = {
     "sdr_window_stream_state_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64]),
     "sdr_window_stream_reset": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_void_p,
                                           C.c_int, C.c_void_p]),
+    "sdr_window_stream_reset_masked": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64,
+                                                 C.c_void_p, C.c_void_p]),
     "sdr_window_stream_gather": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64,
                                            C.c_int64, C.c_int64, C.c_void_p]),
     "sdr_window_stream_merge_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int64, C.c_int64]),

@@ -1078,6 +1078,15 @@ int sdr_stream_reset(const sdr_config* cfg, void* state, int B, const int32_t* h
     return SDR_OK;
 }
 
+int sdr_stream_reset_masked(const sdr_config* cfg, void* state, int B, const uint8_t* mask, sdr_stream stream) {
+    const Layout l = make_layout(cfg);
+    SDR_TRY(check_stream_config(l));
+    if (B <= 0) return SDR_ERR_BAD_ARGUMENT;
+    SDR_TRY(check_buffers({{state, 16}, {mask}}));
+    return launch_zero_masked_slots(state, B, stream_state(l).slot * sizeof(float), mask,
+                                    static_cast<cudaStream_t>(stream));
+}
+
 int sdr_stream_step(const sdr_config* cfg, const void* packed, void* state, const float* chunk, float* out, int B,
                     int64_t C, int apply_mixture_consistency, void* ws, size_t ws_bytes, sdr_stream stream) {
     const Layout l = make_layout(cfg);
@@ -1484,6 +1493,30 @@ int sdr_resample_poly(const float* x, float* out, int64_t rows, int64_t T, int u
     return launch_resample_poly(x, out, rows, T, up, down, scratch, scratch_bytes, static_cast<cudaStream_t>(stream));
 }
 
+size_t sdr_resample_stream_state_bytes(int B, int rows, int64_t C, int up, int down, int64_t delay, int64_t lead) {
+    return resample_stream_state_bytes(B, rows, C, up, down, delay, lead);
+}
+
+int sdr_resample_stream_reset(void* state, size_t state_bytes, int B, int rows, int64_t C, int up, int down,
+                              int64_t delay, int64_t lead, const int32_t* host_slots_or_null, int n, sdr_stream stream) {
+    return resample_stream_reset(state, state_bytes, B, rows, C, up, down, delay, lead, host_slots_or_null, n,
+                                 static_cast<cudaStream_t>(stream));
+}
+
+int sdr_resample_stream_step(void* state, size_t state_bytes, const float* chunk, const uint8_t* zero_slots_or_null,
+                             float* out, int B, int rows, int64_t C, int up, int down, int64_t delay, int64_t lead,
+                             sdr_stream stream) {
+    return launch_resample_stream_step(state, state_bytes, chunk, zero_slots_or_null, out, B, rows, C, up, down, delay,
+                                       lead, static_cast<cudaStream_t>(stream));
+}
+
+int sdr_resample_stream_flush(const void* state, size_t state_bytes, const float* tail_or_null, int64_t tail_len,
+                              const uint8_t* zero_slots_or_null, float* out, int B, int rows, int64_t C, int up,
+                              int down, int64_t delay, int64_t lead, sdr_stream stream) {
+    return launch_resample_stream_flush(state, state_bytes, tail_or_null, tail_len, zero_slots_or_null, out, B, rows,
+                                        C, up, down, delay, lead, static_cast<cudaStream_t>(stream));
+}
+
 int64_t sdr_window_count(int64_t T, int64_t W, int64_t H) { return window_count(T, W, H); }
 
 size_t sdr_window_carry_bytes(int B, int S, int A, int64_t W) { return window_carry_bytes(B, S, A, W); }
@@ -1508,6 +1541,11 @@ size_t sdr_window_stream_state_bytes(int B, int S, int A, int64_t W, int64_t H) 
 int sdr_window_stream_reset(void* state, int B, int S, int A, int64_t W, int64_t H, const int32_t* host_slots_or_null,
                             int n, sdr_stream stream) {
     return window_stream_reset(state, B, S, A, W, H, host_slots_or_null, n, static_cast<cudaStream_t>(stream));
+}
+
+int sdr_window_stream_reset_masked(void* state, int B, int S, int A, int64_t W, int64_t H, const uint8_t* mask,
+                                   sdr_stream stream) {
+    return window_stream_reset_masked(state, B, S, A, W, H, mask, static_cast<cudaStream_t>(stream));
 }
 
 int sdr_window_stream_gather(void* state, const float* chunk_or_null, float* batch, int B, int S, int A, int64_t C,

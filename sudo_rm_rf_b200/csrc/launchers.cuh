@@ -72,6 +72,7 @@ int launch_causal_stream(const float* y, const float* slope_in, const float* con
                          int F, cudaStream_t st);
 int launch_stream_ola(const float* frames, const float* chunk, float* state, long long slot_stride, long long carry_off,
                       float* out, int B, int SA, int A, int k, int F, long long C, int mc, cudaStream_t st);
+int launch_zero_masked_slots(void* base, int B, size_t slot_bytes, const unsigned char* mask, cudaStream_t st);
 int launch_stream_flush(const float* state, long long slot_stride, long long carry_off, float* tail, int B, int SA,
                         int hop, int mc, cudaStream_t st);
 
@@ -125,6 +126,16 @@ int launch_stoi(const float* ref, const float* est, const float* mix, const long
 size_t resample_poly_scratch_bytes(int up, int down);
 int launch_resample_poly(const float* x, float* out, long long rows, long long T, int up, int down, void* scratch,
                          size_t scratch_bytes, cudaStream_t st);
+size_t resample_stream_state_bytes(int B, int rows, long long C, int up, int down, long long delay, long long lead);
+long long resample_stream_flush_length(int p, int q, long long delay, long long lead, long long tail_len);
+int resample_stream_reset(void* state, size_t state_bytes, int B, int rows, long long C, int up, int down, long long delay,
+                          long long lead, const int* slots, int n, cudaStream_t st);
+int launch_resample_stream_step(void* state, size_t state_bytes, const float* chunk, const unsigned char* zero,
+                                float* out, int B, int rows, long long C, int up, int down, long long delay,
+                                long long lead, cudaStream_t st);
+int launch_resample_stream_flush(const void* state, size_t state_bytes, const float* tail, long long tail_len,
+                                 const unsigned char* zero, float* out, int B, int rows, long long C, int up,
+                                 int down, long long delay, long long lead, cudaStream_t st);
 
 // windowed separation (windowed.cu)
 long long window_count(long long T, long long W, long long H);
@@ -137,6 +148,8 @@ int launch_window_merge(const float* est, void* carry, int* perm, float* out, in
 size_t window_stream_state_bytes(int B, int S, int A, long long W, long long H);
 int window_stream_reset(void* state, int B, int S, int A, long long W, long long H, const int* slots, int n,
                         cudaStream_t st);
+int window_stream_reset_masked(void* state, int B, int S, int A, long long W, long long H, const unsigned char* mask,
+                               cudaStream_t st);
 int launch_window_stream_gather(void* state, const float* chunk, float* batch, int B, int S, int A, long long C,
                                 long long W, long long H, cudaStream_t st);
 size_t window_stream_merge_scratch_bytes(int B, int S, long long C, long long H);

@@ -319,4 +319,21 @@ int launch_stream_flush(const float* state, long long slot_stride, long long car
                   hop, B, mc);
 }
 
+// Zeroes the slot_bytes (a multiple of 4) of every slot b < B of `base` whose mask[b] is set: a reset whose slots are
+// chosen on the device, so that a captured graph can run it.
+__global__ void zero_masked_slots_kernel(unsigned* __restrict__ base, long long words, long long total,
+                                         const unsigned char* __restrict__ mask) {
+    for (long long e = (long long)blockIdx.x * 256 + threadIdx.x; e < total; e += (long long)gridDim.x * 256)
+        if (mask[e / words]) base[e] = 0u;
+}
+
+int launch_zero_masked_slots(void* base, int B, size_t slot_bytes, const unsigned char* mask, cudaStream_t st) {
+    if (!base || !mask || B <= 0 || slot_bytes % 4 || reinterpret_cast<uintptr_t>(base) % 4) return SDR_ERR_BAD_ARGUMENT;
+    const long long words = (long long)(slot_bytes / 4), total = words * B;
+    if (total == 0) return SDR_OK;
+    const long long grid = std::min((total + 255) / 256, (long long)std::max(sm_count(), 1) * 8);
+    return launch(zero_masked_slots_kernel, (unsigned)grid, 256, 0, st, static_cast<unsigned*>(base), words, total,
+                  mask);
+}
+
 }  // namespace sdr

@@ -417,6 +417,21 @@ int window_stream_reset(void* state, int B, int S, int A, long long W, long long
     return SDR_OK;
 }
 
+// window_stream_reset of the slots whose mask[b] is set, the mask read on the device.
+int window_stream_reset_masked(void* state, int B, int S, int A, long long W, long long H, const unsigned char* mask,
+                               cudaStream_t st) {
+    if (!state || !mask) return SDR_ERR_BAD_ARGUMENT;
+    if (!stream_shape_ok(B, S, A, W, H)) return S > 4 ? SDR_ERR_UNSUPPORTED : SDR_ERR_BAD_ARGUMENT;
+    if (reinterpret_cast<uintptr_t>(state) % 256) return SDR_ERR_BAD_ARGUMENT;
+    const WindowStreamState ss(state, B, S, A, W, H);
+    int e;
+    if ((e = launch_zero_masked_slots(ss.carry.pi, B, (size_t)S * 4, mask, st)) ||
+        (e = launch_zero_masked_slots(ss.carry.est, B, (size_t)S * A * W * 4, mask, st)) ||
+        (e = launch_zero_masked_slots(ss.hist, B, (size_t)A * H * 4, mask, st)))
+        return e;
+    return launch_zero_masked_slots(ss.count, B, 8, mask, st);
+}
+
 // C = 0 with chunk null: the flush's window [B][A][W]; nothing in the state changes.
 int launch_window_stream_gather(void* state, const float* chunk, float* batch, int B, int S, int A, long long C,
                                 long long W, long long H, cudaStream_t st) {

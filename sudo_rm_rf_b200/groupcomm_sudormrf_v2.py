@@ -10,7 +10,7 @@ import torch
 import torch.nn as nn
 
 from . import _engine
-from . import resample, window_stream, windowed
+from . import resample, resample_stream, windowed
 from .improved_sudormrf import (GlobLN, ConvNormAct, NormAct, DilatedConvNorm, UConvBlock,
                                 _LayerNorm, _not_standalone, _xavier_uniform_)
 
@@ -120,11 +120,15 @@ class GroupCommSudoRmRf(_engine.NativeModuleMixin, nn.Module):
             input_wav, sample_rate, model_rate)
 
     def stream_windows(self, batch_size, chunk_samples, window, hop=None, normalize=True,
-                       mixture_consistency=True):
+                       mixture_consistency=True, sample_rate=None, model_rate=None):
         """A ``window_stream.WindowedStream``: ``separate_long``'s windows taken step by step for ``batch_size``
-        slots of ``chunk_samples`` samples per step (a multiple of the hop), one hop late."""
-        return window_stream.WindowedStream(self, batch_size, chunk_samples, window, hop, normalize=normalize,
-                                            mixture_consistency=mixture_consistency)
+        slots of ``chunk_samples`` samples per step (a multiple of the hop), one hop late.
+
+        ``sample_rate`` and ``model_rate`` (both or neither, as for ``separate``): with different rates, a
+        ``resample_stream.ResampledStream`` whose output is ``separate_long``'s with those rates, ``latency``
+        samples late; ``chunk_samples`` then counts input-rate samples and ``window`` / ``hop`` model-rate ones."""
+        return resample_stream.windowed_stream(self, batch_size, chunk_samples, window, hop, normalize,
+                                               mixture_consistency, sample_rate, model_rate)
 
     def forward_host(self, host_wav, host_out=None, mixture_consistency=False):
         return _engine.forward_host(self, host_wav, host_out, mixture_consistency)
