@@ -306,15 +306,20 @@ def _graphed(graphs: dict, key, bound: int, device, enqueue) -> str:
     return "replayed"
 
 
-def _model_device(model, refusal: str, device=None) -> torch.device:
-    """``device``, or the device of the model's parameters, with a missing index resolved to the current device.
-    Raises ``refusal`` when it is not a CUDA device."""
-    device = torch.device(device) if device is not None else _fetch(model, _probe_names(model)[0]).device
-    if device.type != "cuda":
+def _cuda_device(device, refusal: str) -> torch.device:
+    """``device`` with a missing index resolved to the current device.  Raises ``refusal`` when it is not a CUDA
+    device, or when there is none."""
+    device = torch.device(device)
+    if device.type != "cuda" or not torch.cuda.is_available():
         raise RuntimeError(refusal)
     if device.index is None:
         device = torch.device("cuda", torch.cuda.current_device())
     return device
+
+
+def _model_device(model, refusal: str, device=None) -> torch.device:
+    """``_cuda_device`` of ``device``, or of the device of the model's parameters."""
+    return _cuda_device(device if device is not None else _fetch(model, _probe_names(model)[0]).device, refusal)
 
 
 def _walk(model, names):
@@ -418,8 +423,8 @@ def packed_weights(model, cfg: N.SdrConfig, device) -> torch.Tensor:
     # the master (and a replica on the master's device, which shares this state) may have graphs / in-flight
     # kernels on the old buffer: always pack into a fresh one, the allocator recycles it stream-safely
     packed = torch.empty(nbytes, dtype=torch.uint8, device=device)
-    ptrs = (C.c_void_p * n)(*[C.c_void_p(t.data_ptr()) for t in flat])
-    N.check(lib.sdr_pack_weights(C.byref(cfg), ptrs, n, C.c_void_p(packed.data_ptr()), nbytes,
+    ptrs = (C.c_void_p * n)(*[N.ptr(t) for t in flat])
+    N.check(lib.sdr_pack_weights(C.byref(cfg), ptrs, n, N.ptr(packed), nbytes,
                                  N.stream(device)), "sdr_pack_weights")
     st.sig, st.storages = sig, (weight_storages(tensors) if sig is not None else None)
     _replace(st, "packed", packed)
@@ -473,10 +478,9 @@ def forward(model, wav: torch.Tensor, mixture_consistency: bool = False) -> torc
     out = torch.empty((B, cfg.num_sources * cfg.in_audio_channels, T), dtype=torch.float32, device=device)
 
     def enqueue(packed, ws):
-        N.check(lib.sdr_forward(C.byref(cfg), C.c_void_p(packed.data_ptr()),
-                                C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()),
-                                B, T, 1 if mixture_consistency else 0,
-                                C.c_void_p(ws.data_ptr()), ws.numel(), N.stream(device)), "sdr_forward")
+        N.check(lib.sdr_forward(C.byref(cfg), N.ptr(packed), N.ptr(x), N.ptr(out), B, T,
+                                1 if mixture_consistency else 0, N.ptr(ws), ws.numel(), N.stream(device)),
+                "sdr_forward")
     _call_shared(model, cfg, device, lib.sdr_workspace_bytes(C.byref(cfg), B, T),
                  "bad model configuration (sdr_workspace_bytes returned 0)", enqueue)
     return out
@@ -500,10 +504,9 @@ def separate(model, wav: torch.Tensor, mixture_consistency: bool = False) -> tor
     out = torch.empty((B, cfg.num_sources, T), dtype=torch.float32, device=device)
 
     def enqueue(packed, ws):
-        N.check(lib.sdr_separate(C.byref(cfg), C.c_void_p(packed.data_ptr()),
-                                 C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()),
-                                 B, T, 1 if mixture_consistency else 0,
-                                 C.c_void_p(ws.data_ptr()), ws.numel(), N.stream(device)), "sdr_separate")
+        N.check(lib.sdr_separate(C.byref(cfg), N.ptr(packed), N.ptr(x), N.ptr(out), B, T,
+                                 1 if mixture_consistency else 0, N.ptr(ws), ws.numel(), N.stream(device)),
+                "sdr_separate")
     _call_shared(model, cfg, device, lib.sdr_separate_workspace_bytes(C.byref(cfg), B, T),
                  "bad model configuration (sdr_separate_workspace_bytes returned 0)", enqueue)
     return out
@@ -541,11 +544,9 @@ def forward_host(model, host_wav: torch.Tensor, host_out: torch.Tensor = None,
         staging = _ensure(st, "staging", io_bytes, device)
 
         def call():
-            N.check(lib.sdr_forward_host(C.byref(cfg), C.c_void_p(packed.data_ptr()),
-                                         C.c_void_p(host_wav.data_ptr()), C.c_void_p(host_out.data_ptr()),
-                                         B, T, mc, C.c_void_p(staging.data_ptr()), staging.numel(),
-                                         C.c_void_p(ws.data_ptr()), ws.numel(),
-                                         N.stream(device)), "sdr_forward_host")
+            N.check(lib.sdr_forward_host(C.byref(cfg), N.ptr(packed), N.ptr(host_wav), N.ptr(host_out), B, T, mc,
+                                         N.ptr(staging), staging.numel(), N.ptr(ws), ws.numel(), N.stream(device)),
+                    "sdr_forward_host")
 
         if use_graph and host_wav.is_pinned() and host_out.is_pinned() \
                 and not torch.cuda.is_current_stream_capturing():

@@ -256,8 +256,15 @@ def lib():
 
 
 def stream(device) -> C.c_void_p:
-    """The current CUDA stream of `device`, as the ``cudaStream_t`` argument every entry takes."""
+    """The current CUDA stream of `device`, as the ``cudaStream_t`` argument every entry takes.  Every handle the
+    package passes to the library is spelled this way, inside the function that makes the call, so that
+    ``tests/test_gpu_concurrency.py`` finds every entry that enqueues work."""
     return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
+
+
+def ptr(t) -> C.c_void_p:
+    """The address of tensor ``t`` as a pointer argument; NULL for None."""
+    return C.c_void_p(t.data_ptr() if t is not None else None)
 
 
 def check(code: int, what: str = "") -> None:

@@ -14,8 +14,6 @@ the permutation search) runs in ``libsudormrf_b200.so`` (``sdr_bss_eval``) witho
 call can be captured in a CUDA graph.  Zero-padding an item to a longer length changes none of its values, so a
 ragged corpus can be scored in zero-padded batches.
 """
-import ctypes as C
-
 import torch
 
 from . import _native as N
@@ -74,15 +72,15 @@ def bss_eval_sources(reference_sources, estimated_sources, compute_permutation=T
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         out = torch.empty((3 if mix is None else 6, B, S), dtype=torch.float64, device=dev)
         perm = torch.empty((B, S), dtype=torch.int32, device=dev)
-        ptr = lambda t: C.c_void_p(t.data_ptr())   # noqa: E731
         if mix is None:
-            N.check(lib.sdr_bss_eval(ptr(ref), ptr(est), ptr(out[0]), ptr(out[1]), ptr(out[2]), ptr(perm), B, S, T, F,
-                                     1 if compute_permutation else 0, ptr(scratch), N.stream(dev)), "sdr_bss_eval")
+            N.check(lib.sdr_bss_eval(N.ptr(ref), N.ptr(est), N.ptr(out[0]), N.ptr(out[1]), N.ptr(out[2]), N.ptr(perm),
+                                     B, S, T, F, 1 if compute_permutation else 0, N.ptr(scratch), N.stream(dev)),
+                    "sdr_bss_eval")
         else:
             N.check(lib.sdr_bss_eval_mixture(
-                ptr(ref), ptr(est), ptr(mix), ptr(out[0]), ptr(out[1]), ptr(out[2]), ptr(perm), ptr(out[3]),
-                ptr(out[4]), ptr(out[5]), B, S, T, F, 1 if compute_permutation else 0, ptr(scratch), N.stream(dev)),
-                "sdr_bss_eval_mixture")
+                N.ptr(ref), N.ptr(est), N.ptr(mix), N.ptr(out[0]), N.ptr(out[1]), N.ptr(out[2]), N.ptr(perm),
+                N.ptr(out[3]), N.ptr(out[4]), N.ptr(out[5]), B, S, T, F, 1 if compute_permutation else 0,
+                N.ptr(scratch), N.stream(dev)), "sdr_bss_eval_mixture")
     if single:
         out, perm = out[:, 0], perm[0]
     sdr, sir, sar = out[0], out[1], out[2]

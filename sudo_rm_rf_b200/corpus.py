@@ -101,10 +101,9 @@ def separate_corpus(model, wavs: Iterable[torch.Tensor], max_batch: int = 32,
 
             def enqueue(packed, ws):
                 N.check(lib.sdr_separate_ragged(
-                    C.byref(cfg), C.c_void_p(packed.data_ptr()), C.c_void_p(batch.data_ptr()),
-                    C.c_void_p(lengths.data_ptr()), C.c_void_p(out.data_ptr()), B, Tp,
+                    C.byref(cfg), N.ptr(packed), N.ptr(batch), N.ptr(lengths), N.ptr(out), B, Tp,
                     1 if mixture_consistency else 0, 1 if rescale else 0,
-                    C.c_void_p(ws.data_ptr()), ws.numel(), N.stream(device)), "sdr_separate_ragged")
+                    N.ptr(ws), ws.numel(), N.stream(device)), "sdr_separate_ragged")
             _engine._call_shared(model, cfg, device, lib.sdr_separate_workspace_bytes(C.byref(cfg), B, Tp),
                                  "bad model configuration (sdr_separate_workspace_bytes returned 0)", enqueue)
             for r, i in enumerate(idx):
@@ -237,9 +236,9 @@ class CorpusSeparator:
 
                 def enqueue():
                     N.check(lib.sdr_separate_ragged(
-                        C.byref(cfg), C.c_void_p(packed.data_ptr()), C.c_void_p(self._d_in[slot].data_ptr()),
-                        C.c_void_p(self._d_len[slot].data_ptr()), C.c_void_p(self._d_out[slot].data_ptr()), B, Tp,
-                        self.mc, self.rescale, C.c_void_p(self._ws.data_ptr()), self._ws.numel(), N.stream(dev)),
+                        C.byref(cfg), N.ptr(packed), N.ptr(self._d_in[slot]), N.ptr(self._d_len[slot]),
+                        N.ptr(self._d_out[slot]), B, Tp, self.mc, self.rescale, N.ptr(self._ws), self._ws.numel(),
+                        N.stream(dev)),
                         "sdr_separate_ragged")
 
                 with torch.cuda.stream(self._s_cmp):

@@ -6,13 +6,12 @@ and ``forward(input_wav)`` as the reference's ``GroupCommSudoRmRf``
 (groupcomm_sudormrf_v2.py:231-339); the arithmetic runs in the sm_90a
 kernels behind ``include/sudormrf_b200.h``.
 """
-import torch
 import torch.nn as nn
 
 from . import _engine
-from . import resample, resample_stream, windowed
+from ._surface import NativeSeparator, _not_standalone
 from .improved_sudormrf import (GlobLN, ConvNormAct, NormAct, DilatedConvNorm, UConvBlock,
-                                _LayerNorm, _not_standalone, _xavier_uniform_)
+                                _LayerNorm, _xavier_uniform_)
 
 __all__ = ["GroupCommSudoRmRf", "TAC", "GC_UConvBlock", "GlobLN", "ConvNormAct", "NormAct",
            "DilatedConvNorm", "UConvBlock"]
@@ -44,7 +43,7 @@ class GC_UConvBlock(nn.Module):
     forward = _not_standalone
 
 
-class GroupCommSudoRmRf(_engine.NativeModuleMixin, nn.Module):
+class GroupCommSudoRmRf(NativeSeparator, nn.Module):
     """Group-communication SuDoRM-RF (reference :231-339) on the H100 native path."""
 
     def __init__(self, in_audio_channels=1, out_channels=256, in_channels=512, num_blocks=16,
@@ -92,55 +91,16 @@ class GroupCommSudoRmRf(_engine.NativeModuleMixin, nn.Module):
         """[B, in_audio_channels, T] -> [B, num_sources*in_audio_channels, T]."""
         return _engine.forward(self, input_wav, mixture_consistency=False)
 
+    # The reference applies the uniform mixture consistency to this model family (README.md:113-114): on by default.
     def separate(self, input_wav, mixture_consistency=True, normalize=False, sample_rate=None, model_rate=None):
-        """forward() followed by the uniform mixture consistency the reference applies
-        to this model family (README.md:113-114), fused into the decoder epilogue.
-
-        ``normalize=True``: the whole README recipe on the device (README.md:100-114): raw
-        mixture ``[B, T]`` / ``[B, 1, T]`` -> per-utterance normalisation -> model -> rescale
-        with the mixture's std and mean -> mixture consistency against the normalised mixture.
-
-        ``sample_rate`` and ``model_rate`` (both or neither): the mixture's rate and the rate the model was trained
-        at.  When they differ the mixture is resampled to ``model_rate`` (``resample.resample_poly``), separated there,
-        and every source is resampled back and cropped to the input's length, so the sources sum to the band-limited
-        mixture rather than to the mixture itself (``resample.at_model_rate``)."""
-        run = _engine.separate if normalize else _engine.forward
-        return resample.at_model_rate(lambda wav: run(self, wav, mixture_consistency=mixture_consistency),
-                                      input_wav, sample_rate, model_rate)
+        return super().separate(input_wav, mixture_consistency, normalize, sample_rate, model_rate)
 
     def separate_long(self, input_wav, window, hop=None, normalize=True, mixture_consistency=True,
                       max_windows=32, sample_rate=None, model_rate=None):
-        """``separate`` for recordings of any length: overlapping windows of ``window`` samples every ``hop``,
-        separated in batches of ``max_windows`` per recording, aligned and cross-faded on the device (see
-        ``windowed.separate_long``).  ``window`` and ``hop`` count samples at ``model_rate``; ``sample_rate`` and
-        ``model_rate`` as for ``separate``."""
-        return resample.at_model_rate(
-            lambda wav: windowed.separate_long(self, wav, window, hop, normalize=normalize,
-                                               mixture_consistency=mixture_consistency, max_windows=max_windows),
-            input_wav, sample_rate, model_rate)
+        return super().separate_long(input_wav, window, hop, normalize, mixture_consistency, max_windows,
+                                     sample_rate, model_rate)
 
     def stream_windows(self, batch_size, chunk_samples, window, hop=None, normalize=True,
                        mixture_consistency=True, sample_rate=None, model_rate=None):
-        """A ``window_stream.WindowedStream``: ``separate_long``'s windows taken step by step for ``batch_size``
-        slots of ``chunk_samples`` samples per step (a multiple of the hop), one hop late.
-
-        ``sample_rate`` and ``model_rate`` (both or neither, as for ``separate``): with different rates, a
-        ``resample_stream.ResampledStream`` whose output is ``separate_long``'s with those rates, ``latency``
-        samples late; ``chunk_samples`` then counts input-rate samples and ``window`` / ``hop`` model-rate ones."""
-        return resample_stream.windowed_stream(self, batch_size, chunk_samples, window, hop, normalize,
-                                               mixture_consistency, sample_rate, model_rate)
-
-    def forward_host(self, host_wav, host_out=None, mixture_consistency=False):
-        return _engine.forward_host(self, host_wav, host_out, mixture_consistency)
-
-    def pad_to_appropriate_length(self, x):
-        T = x.shape[-1]
-        q = self.n_least_samples_req
-        Tp = q if T < q else ((T + q - 1) // q) * q
-        out = torch.zeros(list(x.shape[:-1]) + [Tp], dtype=torch.float32, device=x.device)
-        out[..., :T] = x
-        return out
-
-    @staticmethod
-    def remove_trailing_zeros(padded_x, initial_x):
-        return padded_x[..., :initial_x.shape[-1]]
+        return super().stream_windows(batch_size, chunk_samples, window, hop, normalize, mixture_consistency,
+                                      sample_rate, model_rate)

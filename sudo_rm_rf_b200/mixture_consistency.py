@@ -1,6 +1,4 @@
 """H100-native mirror of ``sudo_rm_rf/dnn/experiments/utils/mixture_consistency.py``."""
-import ctypes as C
-
 import torch
 from torch.autograd.function import once_differentiable
 
@@ -14,11 +12,8 @@ def _project(est, mix, magsq):
     out = torch.empty_like(est)
     with torch.cuda.device(est.device):
         scratch = torch.empty(B * S, dtype=torch.float64, device=est.device) if magsq else None
-        N.check(lib.sdr_mixture_consistency(
-            C.c_void_p(est.data_ptr()), C.c_void_p(mix.data_ptr()), C.c_void_p(out.data_ptr()),
-            B, S, T, 1 if magsq else 0,
-            C.c_void_p(scratch.data_ptr() if scratch is not None else 0), N.stream(est.device)),
-            "sdr_mixture_consistency")
+        N.check(lib.sdr_mixture_consistency(N.ptr(est), N.ptr(mix), N.ptr(out), B, S, T, 1 if magsq else 0,
+                                            N.ptr(scratch), N.stream(est.device)), "sdr_mixture_consistency")
     return out
 
 
@@ -50,10 +45,8 @@ class _Consistency(torch.autograd.Function):
             grad_est = torch.empty_like(est)
             grad_mix = torch.empty_like(mix) if want_mix else None
             N.check(lib.sdr_mixture_consistency_backward(
-                C.c_void_p(est.data_ptr()), C.c_void_p(mix.data_ptr()), C.c_void_p(g.data_ptr()),
-                C.c_void_p(grad_est.data_ptr()), C.c_void_p(grad_mix.data_ptr() if want_mix else 0),
-                B, S, T, 1 if ctx.magsq else 0, C.c_void_p(scratch.data_ptr() if scratch is not None else 0),
-                N.stream(dev)), "sdr_mixture_consistency_backward")
+                N.ptr(est), N.ptr(mix), N.ptr(g), N.ptr(grad_est), N.ptr(grad_mix), B, S, T, 1 if ctx.magsq else 0,
+                N.ptr(scratch), N.stream(dev)), "sdr_mixture_consistency_backward")
         return (grad_est.to(ctx.dtypes[0]) if ctx.needs_input_grad[0] else None,
                 grad_mix.to(ctx.dtypes[1]) if want_mix else None, None)
 

@@ -6,7 +6,6 @@ The filter is designed on the device and every output is summed in fp64 in a fix
 ``libsudormrf_b200.so``), so a call never copies from the host, can be captured in a CUDA graph and repeats bit for
 bit, whatever the batch.
 """
-import ctypes as C
 import math
 
 import torch
@@ -58,9 +57,8 @@ def resample_poly(x, up, down):
         out = torch.empty(lead + (-(-T * p // q),), dtype=torch.float32, device=dev)
         # The scratch and the output are allocated here on the current stream and released to it: the caching
         # allocator orders their reuse, and no state outlives the call.
-        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        N.check(lib.sdr_resample_poly(C.c_void_p(src.data_ptr()), C.c_void_p(out.data_ptr()), rows, T, up, down,
-                                      C.c_void_p(scratch.data_ptr()), nbytes, stream), "sdr_resample_poly")
+        N.check(lib.sdr_resample_poly(N.ptr(src), N.ptr(out), rows, T, up, down, N.ptr(scratch), nbytes,
+                                      N.stream(dev)), "sdr_resample_poly")
     return out
 
 

@@ -11,7 +11,6 @@ and so produces ``separate`` / ``separate_long`` with ``sample_rate`` and ``mode
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Iterable, Optional
 
 import torch
@@ -19,8 +18,8 @@ import torch
 from . import _engine
 from . import _native as N
 from .resample import _ratio, check_rates
-from .streaming import MAX_SLOTS, CausalStream
-from .window_stream import WindowedStream, _handle
+from .streaming import MAX_SLOTS, CausalStream, SlotStream, _granule
+from .window_stream import WindowedStream
 from .windowed import window_hop
 
 
@@ -37,7 +36,7 @@ def min_delay(up, down, lead=0):
     return (10 * max(p, q) - lead * p) // q
 
 
-class ResampleStream:
+class ResampleStream(SlotStream):
     """``resample_poly`` taken chunk by chunk for ``batch_size`` independent slots of ``rows`` rows each.
 
     Per slot, let s be ``lead`` zeros followed by everything the slot received since its reset, and r
@@ -74,20 +73,16 @@ class ResampleStream:
         if state_bytes == 0:
             raise N.NativeError(f"sdr_resample_stream_state_bytes refused batch_size={batch_size}, rows={rows}, "
                                 f"chunk_samples={chunk_samples}, delay={delay}, lead={lead} (64-bit sizes)")
-        device = torch.device(device) if device is not None else torch.device("cuda")
-        if device.type != "cuda" or not torch.cuda.is_available():
-            raise RuntimeError("sudo_rm_rf_b200 resamples on CUDA (sm_90a) only and has no CPU path")
-        if device.index is None:
-            device = torch.device("cuda", torch.cuda.current_device())
-        self.device = device
-        self.batch_size, self.rows, self.chunk_samples = batch_size, rows, chunk_samples
+        super().__init__(_engine._cuda_device(device if device is not None else "cuda",
+                                              "sudo_rm_rf_b200 resamples on CUDA (sm_90a) only and has no CPU path"),
+                         batch_size)
+        self.rows, self.chunk_samples = rows, chunk_samples
         self.up, self.down, self.p, self.q = up, down, p, q
         self.delay, self.lead = delay, lead
         self.latency = delay
         self.out_samples = chunk_samples // q * p
         self._args = args
-        self._state = torch.empty(state_bytes, dtype=torch.uint8, device=device)
-        self._order = _engine._Order()      # the stream of the last call on the state
+        self._state = torch.empty(state_bytes, dtype=torch.uint8, device=self.device)
         self.reset()
 
     def flush_samples(self, tail_samples: int = 0) -> int:
@@ -107,31 +102,12 @@ class ResampleStream:
             raise RuntimeError("a resampling stream has no autograd: wrap the call in torch.no_grad()")
         return x.detach().to(torch.float32).contiguous()
 
-    def _out(self, out, n):
-        shape = (self.batch_size, self.rows, n)
-        if out is None:
-            return torch.empty(shape, dtype=torch.float32, device=self.device)
-        if tuple(out.shape) != shape or out.dtype != torch.float32 or out.device != self.device \
-                or not out.is_contiguous():
-            raise RuntimeError(f"out must be a contiguous fp32 tensor {list(shape)} on {self.device}")
-        return out
-
     def reset(self, slots: Optional[Iterable[int]] = None) -> None:
         """Start slots over (all of them when ``slots`` is None): their next step is the start of a new stream."""
-        lib = N.lib()
-        B = self.batch_size
-        if slots is None:
-            arr, n = None, 0
-        else:
-            idx = [int(s) for s in slots]
-            if any(s < 0 or s >= B for s in idx):
-                raise IndexError(f"slots {idx} out of range for batch_size={B}")
-            arr, n = (C.c_int32 * max(1, len(idx)))(*idx), len(idx)
-        with torch.cuda.device(self.device):
-            cur = _engine._enter_stream(self._order, self.device, (self._state,))
-            N.check(lib.sdr_resample_stream_reset(C.c_void_p(self._state.data_ptr()), self._state.numel(), *self._args,
-                                                  arr, n, _handle(cur)), "sdr_resample_stream_reset")
-            _engine._leave_stream(self._order, cur)
+        arr, n = self._slot_array(slots)
+        with self._ordered(self._state):
+            N.check(N.lib().sdr_resample_stream_reset(N.ptr(self._state), self._state.numel(), *self._args, arr, n,
+                                                      N.stream(self.device)), "sdr_resample_stream_reset")
 
     def step(self, chunk: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """[B, rows, C] chunk -> [B, rows, C p / q]: samples ``j C p/q - delay ..`` of each slot's resampled input."""
@@ -139,17 +115,12 @@ class ResampleStream:
 
     def _step(self, chunk, out, zero):
         """``step``; the chunks of the slots whose ``zero`` byte (device uint8 [B], or None) is set read as zeros."""
-        lib = N.lib()
         x = self._check(chunk, "chunk", self.chunk_samples)
-        out = self._out(out, self.out_samples)
-        with torch.cuda.device(self.device):
-            cur = _engine._enter_stream(self._order, self.device, (self._state,))
-            N.check(lib.sdr_resample_stream_step(C.c_void_p(self._state.data_ptr()), self._state.numel(),
-                                                 C.c_void_p(x.data_ptr()),
-                                                 C.c_void_p(zero.data_ptr() if zero is not None else None),
-                                                 C.c_void_p(out.data_ptr()), *self._args, _handle(cur)),
+        out = self._out(out, (self.batch_size, self.rows, self.out_samples))
+        with self._ordered(self._state):
+            N.check(N.lib().sdr_resample_stream_step(N.ptr(self._state), self._state.numel(), N.ptr(x), N.ptr(zero),
+                                                     N.ptr(out), *self._args, N.stream(self.device)),
                     "sdr_resample_stream_step")
-            _engine._leave_stream(self._order, cur)
         return out
 
     def flush(self, tail: Optional[torch.Tensor] = None) -> torch.Tensor:
@@ -158,22 +129,17 @@ class ResampleStream:
         return self._flush(tail, None)
 
     def _flush(self, tail, zero):
-        lib = N.lib()
         x = self._check(tail, "tail") if tail is not None else None
         t = x.shape[-1] if x is not None else 0
-        out = self._out(None, self.flush_samples(t))
-        with torch.cuda.device(self.device):
-            cur = _engine._enter_stream(self._order, self.device, (self._state,))
-            N.check(lib.sdr_resample_stream_flush(C.c_void_p(self._state.data_ptr()), self._state.numel(),
-                                                  C.c_void_p(x.data_ptr() if t else None), t,
-                                                  C.c_void_p(zero.data_ptr() if zero is not None else None),
-                                                  C.c_void_p(out.data_ptr()), *self._args, _handle(cur)),
+        out = self._out(None, (self.batch_size, self.rows, self.flush_samples(t)))
+        with self._ordered(self._state):
+            N.check(N.lib().sdr_resample_stream_flush(N.ptr(self._state), self._state.numel(), N.ptr(x if t else None),
+                                                      t, N.ptr(zero), N.ptr(out), *self._args, N.stream(self.device)),
                     "sdr_resample_stream_flush")
-            _engine._leave_stream(self._order, cur)
         return out
 
 
-class ResampledStream:
+class ResampledStream(SlotStream):
     """A model stream (``inner``: a ``CausalStream`` or a ``WindowedStream`` at ``model_rate``) fed and read at
     ``sample_rate``.  ``chunk_samples`` C counts input-rate samples; with ``model_rate / sample_rate = p / q``, the
     inner stream takes Cm = C p / q samples per step.  For a slot that has received n = j C samples,
@@ -187,8 +153,7 @@ class ResampledStream:
     origin: the inner stream resets that slot after it, and its estimate counts as zeros.  Which slots are in that
     step is a device-side mask, so a step captured in a CUDA graph stays right across later resets."""
 
-    def __init__(self, make_inner, chunk_samples: int, sample_rate: int, model_rate: int, unit: int, unit_name: str,
-                 inner_latency: int):
+    def __init__(self, make_inner, chunk_samples: int, sample_rate: int, model_rate: int, unit: int, unit_name: str):
         p, q = _ratio(model_rate, sample_rate, ("model_rate", "sample_rate"))
         L = 10 * max(p, q)
         Cs = chunk_samples
@@ -204,84 +169,58 @@ class ResampledStream:
             raise ValueError(f"chunk_samples={Cs} gives {Cm} samples at the model's rate per step, which is not a "
                              f"multiple of the inner stream's {unit_name} ({unit} samples)")
         inner = make_inner(Cm)
-        assert inner.latency == inner_latency
-        B, dev = inner.batch_size, inner.device
+        super().__init__(inner.device, inner.batch_size)
+        B, dev = self.batch_size, self.device
         cfg = inner._cfg
         A, SA = cfg.in_audio_channels, cfg.num_sources * cfg.in_audio_channels
         lat = inner.latency
         m = -(-(Cm + lat) // p)
         self.inner = inner
-        self.device = dev
-        self.batch_size = B
         self.chunk_samples = Cs
         self.sample_rate, self.model_rate = sample_rate, model_rate
-        self._in = ResampleStream(B, A, Cs, model_rate, sample_rate, delay=Cm, device=dev)
-        self._out = ResampleStream(B, SA, Cm, sample_rate, model_rate, lead=m * p - (Cm + lat), device=dev)
+        self._to_model = ResampleStream(B, A, Cs, model_rate, sample_rate, delay=Cm, device=dev)
+        self._to_input = ResampleStream(B, SA, Cm, sample_rate, model_rate, lead=m * p - (Cm + lat), device=dev)
         self.latency = Cs + (lat * q + L) // p
-        assert self.latency == self._out.delay + m * q
+        assert self.latency == self._to_input.delay + m * q
         self._mid = torch.empty((B, A, Cm), dtype=torch.float32, device=dev)
         self._est = torch.empty((B, SA, Cm), dtype=torch.float32, device=dev)
-        self._fresh = torch.ones(B, dtype=torch.uint8, device=dev)
-        self._order = _engine._Order()
+        self._fresh = torch.empty(B, dtype=torch.uint8, device=dev)
+        self.reset()
 
     def reset(self, slots: Optional[Iterable[int]] = None) -> None:
         """Start slots over (all of them when ``slots`` is None): their next step is the start of a new stream."""
-        idx = None if slots is None else [int(s) for s in slots]
-        if idx is not None and any(s < 0 or s >= self.batch_size for s in idx):
-            raise IndexError(f"slots {idx} out of range for batch_size={self.batch_size}")
-        with torch.cuda.device(self.device):
-            cur = _engine._enter_stream(self._order, self.device, (self._fresh,))
-            self._in.reset(idx)
-            self._out.reset(idx)
+        arr, n = self._slot_array(slots)
+        idx = None if arr is None else arr[:n]
+        with self._ordered(self._fresh):
+            self._to_model.reset(idx)
+            self._to_input.reset(idx)
             if idx is None:
                 self._fresh.fill_(1)
             elif idx:
                 self._fresh.index_fill_(0, torch.tensor(idx, dtype=torch.long).to(self.device, non_blocking=True), 1)
-            _engine._leave_stream(self._order, cur)
 
     def step(self, chunk: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """[B, A, C] chunk at ``sample_rate`` -> [B, S*A, C]: the slots' separated samples ``n - D .. n + C - D - 1``
         at ``sample_rate``."""
-        inner = self.inner
-        if isinstance(inner, CausalStream):
-            reset = self._reset_causal
-        else:
-            reset = self._reset_windowed
-        with torch.cuda.device(self.device):
-            cur = _engine._enter_stream(self._order, self.device, (self._mid, self._est, self._fresh))
-            mid = self._in.step(chunk, out=self._mid)
-            est = inner.step(mid, out=self._est)
-            reset(cur)
-            out = self._out._step(est, out, self._fresh)
+        with self._ordered(self._mid, self._est, self._fresh):
+            mid = self._to_model.step(chunk, out=self._mid)
+            est = self.inner.step(mid, out=self._est)
+            self.inner._reset_masked(self._fresh)
+            out = self._to_input._step(est, out, self._fresh)
             self._fresh.zero_()
-            _engine._leave_stream(self._order, cur)
         return out
-
-    def _reset_causal(self, cur):
-        inner = self.inner
-        N.check(N.lib().sdr_stream_reset_masked(C.byref(inner._cfg), C.c_void_p(inner._state.data_ptr()),
-                                                inner.batch_size, C.c_void_p(self._fresh.data_ptr()), _handle(cur)),
-                "sdr_stream_reset_masked")
-
-    def _reset_windowed(self, cur):
-        inner = self.inner
-        N.check(N.lib().sdr_window_stream_reset_masked(C.c_void_p(inner._state.data_ptr()), *inner._shape(),
-                                                       C.c_void_p(self._fresh.data_ptr()), _handle(cur)),
-                "sdr_window_stream_reset_masked")
 
     def flush(self) -> torch.Tensor:
         """[B, S*A, latency]: each slot's last ``latency`` samples of the separation of everything it received (zeros
         for a slot without a step since its reset).  Every state is left as it was."""
         inner = self.inner
-        with torch.cuda.device(self.device):
-            cur = _engine._enter_stream(self._order, self.device, (self._fresh,))
-            mid = self._in.flush()                      # model-rate samples [(j-1) Cm, j Cm): one inner chunk
+        with self._ordered(self._fresh):
+            mid = self._to_model.flush()                # model-rate samples [(j-1) Cm, j Cm): one inner chunk
             saved = inner._state.clone()
             est = inner.step(mid)
             tail = torch.cat([est, inner.flush()], dim=-1)
             inner._state.copy_(saved)
-            out = self._out._flush(tail, self._fresh)
-            _engine._leave_stream(self._order, cur)
+            out = self._to_input._flush(tail, self._fresh)
         return out
 
 
@@ -290,14 +229,8 @@ def causal_stream(model, batch_size, chunk_samples, mixture_consistency, sample_
     check_rates(sample_rate, model_rate)
     if sample_rate == model_rate:
         return CausalStream(model, batch_size, chunk_samples, mixture_consistency=mixture_consistency)
-    cfg = _engine.make_config(model)
-    if cfg.variant != 2:
-        raise RuntimeError("only CausalSuDORMRF can be streamed: the other models normalise over the whole clip")
-    granule = N.lib().sdr_stream_granule(C.byref(cfg))
-    if granule < 0:
-        N.check(int(granule), "sdr_stream_granule")
     return ResampledStream(lambda Cm: CausalStream(model, batch_size, Cm, mixture_consistency=mixture_consistency),
-                           chunk_samples, sample_rate, model_rate, int(granule), "granule", cfg.enc_kernel_size // 2)
+                           chunk_samples, sample_rate, model_rate, _granule(_engine.make_config(model)), "granule")
 
 
 def windowed_stream(model, batch_size, chunk_samples, window, hop, normalize, mixture_consistency, sample_rate,
@@ -311,4 +244,4 @@ def windowed_stream(model, batch_size, chunk_samples, window, hop, normalize, mi
     W, H = window_hop(window, hop)
     return ResampledStream(lambda Cm: WindowedStream(model, batch_size, Cm, W, H, normalize=normalize,
                                                      mixture_consistency=mixture_consistency),
-                           chunk_samples, sample_rate, model_rate, H, "hop", H)
+                           chunk_samples, sample_rate, model_rate, H, "hop")

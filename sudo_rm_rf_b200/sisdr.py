@@ -14,7 +14,6 @@ run_improved_sudormrf.py:64-66.  ``PairwiseNegSDR`` is differentiable with respe
 elementwise kernel (``sdr_pairwise_neg_sdr_backward``) in the backward, neither of which
 synchronises with the host, so a training step that uses the loss can be captured in a CUDA graph.
 """
-import ctypes as C
 import itertools
 
 import torch
@@ -100,11 +99,9 @@ class PermInvariantSISDR(nn.Module):
             best = torch.empty(B, dtype=torch.float32, device=dev)
             perm = torch.empty(B, dtype=torch.int32, device=dev)
             N.check(lib.sdr_pit_sisdr(
-                C.c_void_p(est.data_ptr()), C.c_void_p(tgt.data_ptr()),
-                C.c_void_p(mix.data_ptr() if (mix is not None and self.improvement) else 0),
-                C.c_void_p(best.data_ptr()), C.c_void_p(perm.data_ptr()), B, S, T,
+                N.ptr(est), N.ptr(tgt), N.ptr(mix if self.improvement else None), N.ptr(best), N.ptr(perm), B, S, T,
                 1 if self.perform_zero_mean else 0, 1 if self.improvement else 0, float(eps),
-                C.c_void_p(scratch.data_ptr()), N.stream(dev)), "sdr_pit_sisdr")
+                N.ptr(scratch), N.stream(dev)), "sdr_pit_sisdr")
         return _result(self, best, perm, return_best_permutation)
 
 
@@ -169,10 +166,10 @@ class StabilizedPermInvSISDRMetric(nn.Module):
             best = torch.empty(B, dtype=torch.float32, device=dev)
             perm = torch.empty(B, dtype=torch.int32, device=dev)
             N.check(lib.sdr_stabilized_sisdr(
-                C.c_void_p(est.data_ptr()), C.c_void_p(tgt.data_ptr()), C.c_void_p(best.data_ptr()),
-                C.c_void_p(perm.data_ptr()), B, rows, self.n_estimated_sources, self.n_actual_sources, T,
+                N.ptr(est), N.ptr(tgt), N.ptr(best), N.ptr(perm), B, rows, self.n_estimated_sources,
+                self.n_actual_sources, T,
                 1 if self.perform_zero_mean else 0, 1 if self.improvement else 0, float(eps),
-                C.c_void_p(scratch.data_ptr()), N.stream(dev)), "sdr_stabilized_sisdr")
+                N.ptr(scratch), N.stream(dev)), "sdr_stabilized_sisdr")
         return _result(self, best, perm, return_best_permutation)
 
 
@@ -189,9 +186,9 @@ class _PairwiseNegSDR(torch.autograd.Function):
             coef = torch.empty(lib.sdr_pairwise_neg_sdr_coef_bytes(B, S), dtype=torch.uint8, device=dev)
             out = torch.empty((B, S, S), dtype=torch.float32, device=dev)
             N.check(lib.sdr_pairwise_neg_sdr_train(
-                C.c_void_p(est.data_ptr()), C.c_void_p(tgt.data_ptr()), C.c_void_p(out.data_ptr()),
-                C.c_void_p(coef.data_ptr()), B, S, T, sdr_type, 1 if zero_mean else 0, 1 if take_log else 0,
-                C.c_void_p(scratch.data_ptr()), N.stream(dev)), "sdr_pairwise_neg_sdr_train")
+                N.ptr(est), N.ptr(tgt), N.ptr(out), N.ptr(coef), B, S, T, sdr_type, 1 if zero_mean else 0,
+                1 if take_log else 0,
+                N.ptr(scratch), N.stream(dev)), "sdr_pairwise_neg_sdr_train")
         ctx.save_for_backward(est, tgt, coef)
         ctx.dtype = est_targets.dtype
         return out
@@ -206,8 +203,7 @@ class _PairwiseNegSDR(torch.autograd.Function):
         with torch.cuda.device(dev):
             grad = torch.empty((B, S, T), dtype=torch.float32, device=dev)
             N.check(N.lib().sdr_pairwise_neg_sdr_backward(
-                C.c_void_p(est.data_ptr()), C.c_void_p(tgt.data_ptr()), C.c_void_p(coef.data_ptr()),
-                C.c_void_p(g.data_ptr()), C.c_void_p(grad.data_ptr()), B, S, T, N.stream(dev)),
+                N.ptr(est), N.ptr(tgt), N.ptr(coef), N.ptr(g), N.ptr(grad), B, S, T, N.stream(dev)),
                 "sdr_pairwise_neg_sdr_backward")
         return grad.to(ctx.dtype), None, None, None, None, None
 
@@ -255,9 +251,9 @@ class PairwiseNegSDR(nn.Module):
             scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
             out = torch.empty((B, S, S), dtype=torch.float32, device=dev)
             N.check(lib.sdr_pairwise_neg_sdr(
-                C.c_void_p(est.data_ptr()), C.c_void_p(tgt.data_ptr()), C.c_void_p(out.data_ptr()), B, S, T,
+                N.ptr(est), N.ptr(tgt), N.ptr(out), B, S, T,
                 self._TYPES[self.sdr_type], 1 if self.zero_mean else 0, 1 if self.take_log else 0,
-                C.c_void_p(scratch.data_ptr()), N.stream(dev)), "sdr_pairwise_neg_sdr")
+                N.ptr(scratch), N.stream(dev)), "sdr_pairwise_neg_sdr")
         return out
 
 

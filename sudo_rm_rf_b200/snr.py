@@ -6,7 +6,6 @@ it is differentiable with respect to ``pr_batch``: one fp64 Gram pass and a per-
 (``sdr_snr_zero_refs``) in the forward, one elementwise kernel (``sdr_snr_zero_refs_backward``) in the backward.
 Neither synchronises with the host, so a training step that uses the loss can be captured in a CUDA graph.
 """
-import ctypes as C
 import itertools
 
 import torch
@@ -28,9 +27,8 @@ def _forward(est, tgt, zero_mean, threshold, eps):
         best = torch.empty(B, dtype=torch.float32, device=dev)
         perm = torch.empty(B, dtype=torch.int32, device=dev)
         N.check(lib.sdr_snr_zero_refs(
-            C.c_void_p(est.data_ptr()), C.c_void_p(tgt.data_ptr()), C.c_void_p(best.data_ptr()),
-            C.c_void_p(perm.data_ptr()), C.c_void_p(coef.data_ptr()), B, S, T, 1 if zero_mean else 0,
-            float(threshold), float(eps), C.c_void_p(scratch.data_ptr()), N.stream(dev)), "sdr_snr_zero_refs")
+            N.ptr(est), N.ptr(tgt), N.ptr(best), N.ptr(perm), N.ptr(coef), B, S, T, 1 if zero_mean else 0,
+            float(threshold), float(eps), N.ptr(scratch), N.stream(dev)), "sdr_snr_zero_refs")
     return best, perm, coef
 
 
@@ -55,8 +53,7 @@ class _SNRZeroRefs(torch.autograd.Function):
         with torch.cuda.device(dev):
             grad = torch.empty(ctx.shape, dtype=torch.float32, device=dev)
             N.check(N.lib().sdr_snr_zero_refs_backward(
-                C.c_void_p(est.data_ptr()), C.c_void_p(tgt.data_ptr()), C.c_void_p(coef.data_ptr()),
-                C.c_void_p(g.data_ptr()), C.c_void_p(grad.data_ptr()), B, S, T, ctx.shape[-1], N.stream(dev)),
+                N.ptr(est), N.ptr(tgt), N.ptr(coef), N.ptr(g), N.ptr(grad), B, S, T, ctx.shape[-1], N.stream(dev)),
                 "sdr_snr_zero_refs_backward")
         return grad.to(ctx.dtype), None, None, None, None, None
 

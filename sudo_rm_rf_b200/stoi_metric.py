@@ -9,8 +9,6 @@ magnitudes of x and of y (scaled to x and clipped 15 dB above it) are averaged.
 The whole computation runs in fp64 from the fp32 inputs in ``libsudormrf_b200.so`` (``sdr_stoi``) without
 synchronising with the host, so a call can be captured in a CUDA graph, and repeats bit for bit.
 """
-import ctypes as C
-
 import torch
 
 from . import _native as N
@@ -74,11 +72,10 @@ def stoi(x, y, fs_sig, extended=False, mixture=None, lengths=None):
     with torch.cuda.device(dev):
         scratch = torch.empty(nbytes, dtype=torch.uint8, device=dev)
         out = torch.empty((1 if mix is None else 2, B, S), dtype=torch.float64, device=dev)
-        ptr = lambda t: C.c_void_p(t.data_ptr() if t is not None else None)   # noqa: E731
         # Every buffer of the call is allocated here on the current stream and released to it: the caching allocator
         # orders their reuse, and no state outlives the call (tests/test_gpu_stoi.py runs it across streams and threads).
-        stream = C.c_void_p(torch.cuda.current_stream(dev).cuda_stream)
-        N.check(lib.sdr_stoi(ptr(ref), ptr(est), ptr(mix), ptr(lens), ptr(out[0]),
-                             ptr(out[1]) if mix is not None else None, B, S, T, fs, ptr(scratch), stream), "sdr_stoi")
+        N.check(lib.sdr_stoi(N.ptr(ref), N.ptr(est), N.ptr(mix), N.ptr(lens), N.ptr(out[0]),
+                             N.ptr(out[1] if mix is not None else None), B, S, T, fs, N.ptr(scratch), N.stream(dev)),
+                "sdr_stoi")
     out = out.reshape((out.shape[0],) + tuple(lead))
     return out[0] if mix is None else (out[0], out[1])

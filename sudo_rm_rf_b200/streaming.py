@@ -13,6 +13,7 @@ cannot be streamed.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes as C
 from typing import Iterable, Optional
 
@@ -25,7 +26,54 @@ MAX_SLOTS = 65535            # slots per step (one grid row per slot, include/su
 MAX_CHUNK_FRAMES = 4096      # encoder frames per slot and step, i.e. chunk_samples <= 4096 * hop
 
 
-class CausalStream:
+class SlotStream:
+    """What every stream of ``batch_size`` independent slots shares: its device, and the CUDA stream of the last call
+    on its buffers, which a call on another stream waits for on the device."""
+
+    def __init__(self, device: torch.device, batch_size: int):
+        self.device = device
+        self.batch_size = batch_size
+        self._order = _engine._Order()      # the stream of the last call on the state
+
+    def _slot_array(self, slots: Optional[Iterable[int]]):
+        """``(int32 array, n)`` of the slots ``reset(slots)`` names; ``(None, 0)`` for all of them."""
+        if slots is None:
+            return None, 0
+        idx = [int(s) for s in slots]
+        if any(s < 0 or s >= self.batch_size for s in idx):
+            raise IndexError(f"slots {idx} out of range for batch_size={self.batch_size}")
+        return (C.c_int32 * max(1, len(idx)))(*idx), len(idx)
+
+    def _out(self, out: Optional[torch.Tensor], shape: tuple) -> torch.Tensor:
+        """``out``, checked to be a contiguous fp32 tensor of ``shape`` on the stream's device, or a new one."""
+        if out is None:
+            return torch.empty(shape, dtype=torch.float32, device=self.device)
+        if tuple(out.shape) != shape or out.dtype != torch.float32 or out.device != self.device \
+                or not out.is_contiguous():
+            raise RuntimeError(f"out must be a contiguous fp32 tensor {list(shape)} on {self.device}")
+        return out
+
+    @contextlib.contextmanager
+    def _ordered(self, *buffers):
+        """The body runs on the stream's device after the previous call, and ``buffers`` are recorded on the current
+        stream.  Only a body that returns counts as the last call: a refused one leaves the order as it was."""
+        with torch.cuda.device(self.device):
+            cur = _engine._enter_stream(self._order, self.device, buffers)
+            yield
+            _engine._leave_stream(self._order, cur)
+
+
+def _granule(cfg: N.SdrConfig) -> int:
+    """The chunk granule of a ``CausalSuDORMRF`` configuration; the other models are refused."""
+    if cfg.variant != 2:
+        raise RuntimeError("only CausalSuDORMRF can be streamed: the other models normalise over the whole clip")
+    granule = N.lib().sdr_stream_granule(C.byref(cfg))
+    if granule < 0:
+        N.check(int(granule), "sdr_stream_granule")
+    return int(granule)
+
+
+class CausalStream(SlotStream):
     """``batch_size`` independent streams (slots) of ``chunk_samples`` samples per step.
 
     Owns its state and step workspace, apart from the model's forward workspace, so ``model(x)`` and open streams
@@ -37,11 +85,7 @@ class CausalStream:
     def __init__(self, model, batch_size: int, chunk_samples: int, mixture_consistency: bool = False):
         lib = N.lib()
         cfg = _engine.make_config(model)
-        if cfg.variant != 2:
-            raise RuntimeError("only CausalSuDORMRF can be streamed: the other models normalise over the whole clip")
-        granule = lib.sdr_stream_granule(C.byref(cfg))
-        if granule < 0:
-            N.check(int(granule), "sdr_stream_granule")
+        granule = _granule(cfg)
         # the arguments are checked before the device, so that each refusal names the limit it hit
         B, Cs = int(batch_size), int(chunk_samples)
         if B <= 0 or B > MAX_SLOTS:
@@ -59,42 +103,34 @@ class CausalStream:
         ws_bytes = lib.sdr_stream_workspace_bytes(C.byref(cfg), B, Cs)
         if ws_bytes == 0:
             raise ValueError(f"sdr_stream_workspace_bytes refused batch_size={B}, chunk_samples={Cs}")
-        device = _engine._model_device(model, "sudo_rm_rf_b200 streams on CUDA (sm_90a) only and has no CPU path: "
-                                              "move the model to an H100 (`model.cuda()`)")
+        super().__init__(_engine._model_device(model, "sudo_rm_rf_b200 streams on CUDA (sm_90a) only and has no CPU "
+                                                      "path: move the model to an H100 (`model.cuda()`)"), B)
         self.model = model
-        self.device = device
-        self.batch_size = B
         self.chunk_samples = Cs
-        self.granule = int(granule)
+        self.granule = granule
         self.latency = cfg.enc_kernel_size // 2
         self.mixture_consistency = bool(mixture_consistency)
         self._cfg = cfg
-        self._state = torch.empty(lib.sdr_stream_state_bytes(C.byref(cfg), B), dtype=torch.uint8, device=device)
-        self._ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
-        self._order = _engine._Order()      # the stream of the last call on the state
+        self._state = torch.empty(lib.sdr_stream_state_bytes(C.byref(cfg), B), dtype=torch.uint8, device=self.device)
+        self._ws = torch.empty(ws_bytes, dtype=torch.uint8, device=self.device)
         self.reset()
 
     def reset(self, slots: Optional[Iterable[int]] = None) -> None:
         """Start slots over (all of them when ``slots`` is None): their next step is the start of a new stream."""
-        lib = N.lib()
-        with torch.cuda.device(self.device):
-            cur = _engine._enter_stream(self._order, self.device, (self._state,))
-            if slots is None:
-                rc = lib.sdr_stream_reset(C.byref(self._cfg), C.c_void_p(self._state.data_ptr()), self.batch_size,
-                                          None, 0, N.stream(self.device))
-            else:
-                idx = [int(s) for s in slots]
-                if any(s < 0 or s >= self.batch_size for s in idx):
-                    raise IndexError(f"slots {idx} out of range for batch_size={self.batch_size}")
-                arr = (C.c_int32 * max(1, len(idx)))(*idx)
-                rc = lib.sdr_stream_reset(C.byref(self._cfg), C.c_void_p(self._state.data_ptr()), self.batch_size,
-                                          arr, len(idx), N.stream(self.device))
-            N.check(rc, "sdr_stream_reset")
-            _engine._leave_stream(self._order, cur)
+        arr, n = self._slot_array(slots)
+        with self._ordered(self._state):
+            N.check(N.lib().sdr_stream_reset(C.byref(self._cfg), N.ptr(self._state), self.batch_size, arr, n,
+                                             N.stream(self.device)), "sdr_stream_reset")
+
+    def _reset_masked(self, mask: torch.Tensor) -> None:
+        """Starts over the slots whose byte in ``mask`` (device uint8 [B]) is set, on the current stream, inside the
+        caller's ``_ordered`` section right after a step: the mask is read on the device, so a captured graph resets
+        whichever slots it names at replay."""
+        N.check(N.lib().sdr_stream_reset_masked(C.byref(self._cfg), N.ptr(self._state), self.batch_size, N.ptr(mask),
+                                                N.stream(self.device)), "sdr_stream_reset_masked")
 
     def step(self, chunk: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """[B, A, C] chunk -> [B, S*A, C] estimates of the model's output samples ``c*C - hop .. (c+1)*C - hop - 1``."""
-        lib = N.lib()
         cfg = self._cfg
         x = _engine._check_input(self.model, cfg, chunk)
         B, Cs = self.batch_size, self.chunk_samples
@@ -102,34 +138,22 @@ class CausalStream:
             raise RuntimeError(f"expected a chunk of shape [{B}, {cfg.in_audio_channels}, {Cs}], got {list(chunk.shape)}")
         if x.device != self.device:
             raise RuntimeError(f"chunk is on {x.device}, the stream on {self.device}")
-        SA = cfg.num_sources * cfg.in_audio_channels
-        if out is None:
-            out = torch.empty((B, SA, Cs), dtype=torch.float32, device=self.device)
-        elif tuple(out.shape) != (B, SA, Cs) or out.dtype != torch.float32 or out.device != self.device \
-                or not out.is_contiguous():
-            raise RuntimeError(f"out must be a contiguous fp32 tensor [{B}, {SA}, {Cs}] on {self.device}")
-        with torch.cuda.device(self.device):
-            cur = torch.cuda.current_stream(self.device)
-            packed = _engine.packed_for(self.model, cfg, self.device, cur)
-            _engine._enter_stream(self._order, self.device, (self._state, self._ws))
-            N.check(lib.sdr_stream_step(C.byref(cfg), C.c_void_p(packed.data_ptr()), C.c_void_p(self._state.data_ptr()),
-                                        C.c_void_p(x.data_ptr()), C.c_void_p(out.data_ptr()), B, Cs,
-                                        1 if self.mixture_consistency else 0, C.c_void_p(self._ws.data_ptr()),
-                                        self._ws.numel(), N.stream(self.device)), "sdr_stream_step")
-            _engine._leave_stream(self._order, cur)
+        out = self._out(out, (B, cfg.num_sources * cfg.in_audio_channels, Cs))
+        with self._ordered(self._state, self._ws):
+            packed = _engine.packed_for(self.model, cfg, self.device, torch.cuda.current_stream(self.device))
+            N.check(N.lib().sdr_stream_step(C.byref(cfg), N.ptr(packed), N.ptr(self._state), N.ptr(x), N.ptr(out), B,
+                                            Cs, 1 if self.mixture_consistency else 0, N.ptr(self._ws),
+                                            self._ws.numel(), N.stream(self.device)), "sdr_stream_step")
         return out
 
     def flush(self) -> torch.Tensor:
         """[B, S*A, hop]: the last ``hop`` output samples, which only the end of the stream completes.  The state is
         left as it is; ``reset()`` starts the slots over."""
-        lib = N.lib()
         cfg = self._cfg
         tail = torch.empty((self.batch_size, cfg.num_sources * cfg.in_audio_channels, self.latency),
                            dtype=torch.float32, device=self.device)
-        with torch.cuda.device(self.device):
-            cur = _engine._enter_stream(self._order, self.device, (self._state,))
-            N.check(lib.sdr_stream_flush(C.byref(cfg), C.c_void_p(self._state.data_ptr()), C.c_void_p(tail.data_ptr()),
-                                         self.batch_size, 1 if self.mixture_consistency else 0, N.stream(self.device)),
+        with self._ordered(self._state):
+            N.check(N.lib().sdr_stream_flush(C.byref(cfg), N.ptr(self._state), N.ptr(tail), self.batch_size,
+                                             1 if self.mixture_consistency else 0, N.stream(self.device)),
                     "sdr_stream_flush")
-            _engine._leave_stream(self._order, cur)
         return tail

@@ -16,8 +16,7 @@ import torch
 import torch.nn as nn
 
 from . import _engine
-from . import resample, resample_stream, windowed
-from .improved_sudormrf import _not_standalone
+from ._surface import NativeSeparator, _not_standalone
 
 
 class ConvNormAct(nn.Module):
@@ -96,7 +95,7 @@ class UBlock(nn.Module):
     forward = _not_standalone
 
 
-class SuDORMRF(_engine.NativeModuleMixin, nn.Module):
+class SuDORMRF(NativeSeparator, nn.Module):
     """The original SuDoRM-RF separator (reference :185-297) on the H100 native path."""
 
     _b200_variant = 3
@@ -141,45 +140,6 @@ class SuDORMRF(_engine.NativeModuleMixin, nn.Module):
         """[B, 1, T] mixture -> [B, num_sources, T] estimates (fp32, same device)."""
         return _engine.forward(self, input_wav, mixture_consistency=False)
 
-    def separate(self, input_wav, mixture_consistency=False, normalize=False, sample_rate=None, model_rate=None):
-        """forward() with the uniform mixture-consistency projection fused into the decoder epilogue;
-        ``normalize=True`` runs the README recipe (README.md:100-114) on the device, see
-        ``improved_sudormrf.SuDORMRF.separate``.
-
-        ``sample_rate`` and ``model_rate`` (both or neither): the mixture's rate and the rate the model was trained
-        at.  When they differ the mixture is resampled to ``model_rate`` (``resample.resample_poly``), separated there,
-        and every source is resampled back and cropped to the input's length, so the sources sum to the band-limited
-        mixture rather than to the mixture itself (``resample.at_model_rate``)."""
-        run = _engine.separate if normalize else _engine.forward
-        return resample.at_model_rate(lambda wav: run(self, wav, mixture_consistency=mixture_consistency),
-                                      input_wav, sample_rate, model_rate)
-
-    def separate_long(self, input_wav, window, hop=None, normalize=True, mixture_consistency=False,
-                      max_windows=32, sample_rate=None, model_rate=None):
-        """``separate`` for recordings of any length: overlapping windows of ``window`` samples every ``hop``,
-        separated in batches of ``max_windows`` per recording, aligned and cross-faded on the device (see
-        ``windowed.separate_long``).  ``window`` and ``hop`` count samples at ``model_rate``; ``sample_rate`` and
-        ``model_rate`` as for ``separate``."""
-        return resample.at_model_rate(
-            lambda wav: windowed.separate_long(self, wav, window, hop, normalize=normalize,
-                                               mixture_consistency=mixture_consistency, max_windows=max_windows),
-            input_wav, sample_rate, model_rate)
-
-    def stream_windows(self, batch_size, chunk_samples, window, hop=None, normalize=True,
-                       mixture_consistency=False, sample_rate=None, model_rate=None):
-        """A ``window_stream.WindowedStream``: ``separate_long``'s windows taken step by step for ``batch_size``
-        slots of ``chunk_samples`` samples per step (a multiple of the hop), one hop late.
-
-        ``sample_rate`` and ``model_rate`` (both or neither, as for ``separate``): with different rates, a
-        ``resample_stream.ResampledStream`` whose output is ``separate_long``'s with those rates, ``latency``
-        samples late; ``chunk_samples`` then counts input-rate samples and ``window`` / ``hop`` model-rate ones."""
-        return resample_stream.windowed_stream(self, batch_size, chunk_samples, window, hop, normalize,
-                                               mixture_consistency, sample_rate, model_rate)
-
-    def forward_host(self, host_wav, host_out=None, mixture_consistency=False):
-        """End-to-end call on pinned HOST tensors (H2D, forward, D2H on the current stream)."""
-        return _engine.forward_host(self, host_wav, host_out, mixture_consistency)
-
     def pad_to_appropriate_length(self, x):
         """Reference :283-293 (device-side; the native encoder pads implicitly)."""
         rem = int(x.shape[-1]) % self.lcm
@@ -188,7 +148,3 @@ class SuDORMRF(_engine.NativeModuleMixin, nn.Module):
             out[..., :x.shape[-1]] = x
             return out
         return x
-
-    @staticmethod
-    def remove_trailing_zeros(padded_x, initial_x):
-        return padded_x[..., :initial_x.shape[-1]]

@@ -50,10 +50,8 @@ class _NativeTrain(torch.autograd.Function):
         out = torch.empty((B, cfg.num_sources, T), dtype=torch.float32, device=device)
 
         def enqueue(packed, ws):
-            N.check(lib.sdr_forward_train(C.byref(cfg), C.c_void_p(packed.data_ptr()), C.c_void_p(wav.data_ptr()),
-                                          C.c_void_p(out.data_ptr()), B, T, C.c_void_p(saved.data_ptr()),
-                                          saved.numel(), C.c_void_p(ws.data_ptr()), ws.numel(),
-                                          N.stream(device)), "sdr_forward_train")
+            N.check(lib.sdr_forward_train(C.byref(cfg), N.ptr(packed), N.ptr(wav), N.ptr(out), B, T, N.ptr(saved),
+                                          saved.numel(), N.ptr(ws), ws.numel(), N.stream(device)), "sdr_forward_train")
         packed = _engine._call_shared(model, cfg, device, lib.sdr_workspace_bytes(C.byref(cfg), B, T), unsupported,
                                       enqueue)
         ctx.cfg = cfg
@@ -79,10 +77,8 @@ class _NativeTrain(torch.autograd.Function):
             ws = torch.empty(ws_bytes, dtype=torch.uint8, device=device)
             numel = [p.numel() for p in params]
             flat = torch.empty(sum(numel), dtype=torch.float32, device=device)
-            N.check(lib.sdr_backward(C.byref(cfg), C.c_void_p(ctx.packed.data_ptr()), C.c_void_p(wav.data_ptr()),
-                                     C.c_void_p(ctx.saved.data_ptr()), C.c_void_p(g.data_ptr()),
-                                     C.c_void_p(flat.data_ptr()), B, T, C.c_void_p(ws.data_ptr()), ws.numel(),
-                                     N.stream(device)), "sdr_backward")
+            N.check(lib.sdr_backward(C.byref(cfg), N.ptr(ctx.packed), N.ptr(wav), N.ptr(ctx.saved), N.ptr(g),
+                                     N.ptr(flat), B, T, N.ptr(ws), ws.numel(), N.stream(device)), "sdr_backward")
         ctx.saved = None
         grads = []
         for p, part in zip(params, flat.split(numel)):

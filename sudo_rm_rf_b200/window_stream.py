@@ -14,23 +14,17 @@ the model's shared workspace, so its cost and memory stay the same however long 
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Iterable, Optional
 
 import torch
 
 from . import _engine
 from . import _native as N
-from .streaming import MAX_SLOTS
+from .streaming import MAX_SLOTS, SlotStream
 from .windowed import window_hop
 
 
-def _handle(stream) -> C.c_void_p:
-    """The ``cudaStream_t`` of the stream a call entered on (``_engine._enter_stream``)."""
-    return C.c_void_p(stream.cuda_stream)
-
-
-class WindowedStream:
+class WindowedStream(SlotStream):
     """``batch_size`` independent streams (slots) of ``chunk_samples`` samples per step, separated in windows of
     ``window`` samples every ``hop``.
 
@@ -63,11 +57,10 @@ class WindowedStream:
         if state_bytes == 0 or scratch_bytes == 0:
             raise N.NativeError(f"windowed streams support 1 to 4 sources and windows of at most 2^24 samples "
                                 f"(num_sources={S}, window={W})")
-        device = _engine._model_device(model, "sudo_rm_rf_b200 streams on CUDA (sm_90a) only and has no CPU path: "
-                                              "move the model to an H100 (`model.cuda()`)")
+        super().__init__(_engine._model_device(model, "sudo_rm_rf_b200 streams on CUDA (sm_90a) only and has no CPU "
+                                                      "path: move the model to an H100 (`model.cuda()`)"), B)
+        device = self.device
         self.model = model
-        self.device = device
-        self.batch_size = B
         self.chunk_samples = Cs
         self.window, self.hop = W, H
         self.latency = H
@@ -78,7 +71,6 @@ class WindowedStream:
         self._state = torch.empty(state_bytes, dtype=torch.uint8, device=device)
         self._batch = torch.empty((B * self._q, A, W), dtype=torch.float32, device=device)
         self._scratch = torch.empty(scratch_bytes, dtype=torch.uint8, device=device)
-        self._order = _engine._Order()      # the stream of the last call on the state
         self.reset()
 
     def _shape(self):
@@ -91,20 +83,15 @@ class WindowedStream:
 
     def reset(self, slots: Optional[Iterable[int]] = None) -> None:
         """Start slots over (all of them when ``slots`` is None): their next step is the start of a new stream."""
-        lib = N.lib()
-        B = self.batch_size
-        if slots is None:
-            arr, n = None, 0
-        else:
-            idx = [int(s) for s in slots]
-            if any(s < 0 or s >= B for s in idx):
-                raise IndexError(f"slots {idx} out of range for batch_size={B}")
-            arr, n = (C.c_int32 * max(1, len(idx)))(*idx), len(idx)
-        with torch.cuda.device(self.device):
-            cur = _engine._enter_stream(self._order, self.device, (self._state,))
-            N.check(lib.sdr_window_stream_reset(C.c_void_p(self._state.data_ptr()), *self._shape(), arr, n,
-                                                _handle(cur)), "sdr_window_stream_reset")
-            _engine._leave_stream(self._order, cur)
+        arr, n = self._slot_array(slots)
+        with self._ordered(self._state):
+            N.check(N.lib().sdr_window_stream_reset(N.ptr(self._state), *self._shape(), arr, n, N.stream(self.device)),
+                    "sdr_window_stream_reset")
+
+    def _reset_masked(self, mask: torch.Tensor) -> None:
+        """``CausalStream._reset_masked`` for the window counters and carries."""
+        N.check(N.lib().sdr_window_stream_reset_masked(N.ptr(self._state), *self._shape(), N.ptr(mask),
+                                                       N.stream(self.device)), "sdr_window_stream_reset_masked")
 
     def step(self, chunk: torch.Tensor, out: Optional[torch.Tensor] = None) -> torch.Tensor:
         """[B, A, C] chunk -> [B, S*A, C]: the slots' separated samples ``n - hop .. n + C - hop - 1``."""
@@ -119,24 +106,14 @@ class WindowedStream:
             raise RuntimeError(f"expected a chunk of shape [{B}, {A}, {Cs}], got {list(chunk.shape)}")
         if x.device != self.device:
             raise RuntimeError(f"chunk is on {x.device}, the stream on {self.device}")
-        SA = S * A
-        if out is None:
-            out = torch.empty((B, SA, Cs), dtype=torch.float32, device=self.device)
-        elif tuple(out.shape) != (B, SA, Cs) or out.dtype != torch.float32 or out.device != self.device \
-                or not out.is_contiguous():
-            raise RuntimeError(f"out must be a contiguous fp32 tensor [{B}, {SA}, {Cs}] on {self.device}")
-        with torch.cuda.device(self.device):
-            cur = _engine._enter_stream(self._order, self.device, (self._state, self._batch, self._scratch))
-            N.check(lib.sdr_window_stream_gather(C.c_void_p(self._state.data_ptr()), C.c_void_p(x.data_ptr()),
-                                                 C.c_void_p(self._batch.data_ptr()), B, S, A, Cs, W, H,
-                                                 _handle(cur)), "sdr_window_stream_gather")
+        out = self._out(out, (B, S * A, Cs))
+        with self._ordered(self._state, self._batch, self._scratch):
+            N.check(lib.sdr_window_stream_gather(N.ptr(self._state), N.ptr(x), N.ptr(self._batch), B, S, A, Cs, W, H,
+                                                 N.stream(self.device)), "sdr_window_stream_gather")
             # the model's shared workspace and packed weights, as for any forward of B q windows
             est = self._run(self._batch)
-            N.check(lib.sdr_window_stream_merge(C.c_void_p(est.data_ptr()), C.c_void_p(self._state.data_ptr()),
-                                                C.c_void_p(out.data_ptr()), B, S, A, Cs, W, H,
-                                                C.c_void_p(self._scratch.data_ptr()), _handle(cur)),
-                    "sdr_window_stream_merge")
-            _engine._leave_stream(self._order, cur)
+            N.check(lib.sdr_window_stream_merge(N.ptr(est), N.ptr(self._state), N.ptr(out), B, S, A, Cs, W, H,
+                                                N.ptr(self._scratch), N.stream(self.device)), "sdr_window_stream_merge")
         return out
 
     def flush(self) -> torch.Tensor:
@@ -144,21 +121,16 @@ class WindowedStream:
         for a slot without a step since its reset).  The state is left as it is; ``reset()`` starts slots over."""
         lib = N.lib()
         B, S, A, W, H = self._shape()
-        with torch.cuda.device(self.device):
-            cur = _engine._enter_stream(self._order, self.device, (self._state,))
+        with self._ordered(self._state):
             win = torch.empty((B, A, W), dtype=torch.float32, device=self.device)
-            N.check(lib.sdr_window_stream_gather(C.c_void_p(self._state.data_ptr()), None, C.c_void_p(win.data_ptr()),
-                                                 B, S, A, 0, W, H, _handle(cur)), "sdr_window_stream_gather")
+            N.check(lib.sdr_window_stream_gather(N.ptr(self._state), None, N.ptr(win), B, S, A, 0, W, H,
+                                                 N.stream(self.device)), "sdr_window_stream_gather")
             # a slot that has received H samples is one window long: separate_long separates them unpadded
             single = self._run(win[..., :H].contiguous())
             est = self._run(win) if W < 2 * H else None
             scratch = torch.empty(lib.sdr_window_stream_flush_scratch_bytes(B, S), dtype=torch.uint8,
                                   device=self.device)
             tail = torch.empty((B, S * A, H), dtype=torch.float32, device=self.device)
-            N.check(lib.sdr_window_stream_flush(C.c_void_p(single.data_ptr()),
-                                                C.c_void_p(est.data_ptr() if est is not None else None),
-                                                C.c_void_p(self._state.data_ptr()), C.c_void_p(tail.data_ptr()),
-                                                B, S, A, W, H, C.c_void_p(scratch.data_ptr()), _handle(cur)),
-                    "sdr_window_stream_flush")
-            _engine._leave_stream(self._order, cur)
+            N.check(lib.sdr_window_stream_flush(N.ptr(single), N.ptr(est), N.ptr(self._state), N.ptr(tail), B, S, A, W,
+                                                H, N.ptr(scratch), N.stream(self.device)), "sdr_window_stream_flush")
         return tail

@@ -8,8 +8,6 @@ batches of at most ``max_windows`` per recording through ``separate`` (``sdr_sep
 centred correlation over their overlap) and cross-fades the overlaps.  Its memory is set by the window batch, not by
 the length.  Everything after the input checks runs on the current stream without a host synchronisation.
 """
-import ctypes as C
-
 import torch
 
 from . import _engine
@@ -36,24 +34,19 @@ def window_plan(T, W, H):
 
 # The stage calls below run on buffers the caller allocated on the current stream for this one call (see
 # separate_long): the caching allocator orders their reuse, and no state outlives the call.
-def _current(device):
-    return C.c_void_p(torch.cuda.current_stream(device).cuda_stream)
-
-
 def gather(x, batch, W, H, k0, M):
     """Windows k0 .. k0+M-1 of x [B, A, T] into batch [B, M, A, W] (its first B M A W floats), zeros past T."""
     B, A, T = x.shape
-    N.check(N.lib().sdr_window_gather(C.c_void_p(x.data_ptr()), C.c_void_p(batch.data_ptr()), B, A, T, W, H, k0, M,
-                                      _current(x.device)), "sdr_window_gather")
+    N.check(N.lib().sdr_window_gather(N.ptr(x), N.ptr(batch), B, A, T, W, H, k0, M, N.stream(x.device)),
+            "sdr_window_gather")
 
 
 def merge(est, carry, perm, out, S, A, W, H, k0, M, scratch):
     """Aligns and overlap-adds the estimates [B, M, S A, W] of windows k0 .. k0+M-1 into out [B, S A, T]; ``carry``
     holds what the previous batch's merge left, ``perm`` ([B, K, S] int32 or None) receives each window's order."""
     B, T = out.shape[0], out.shape[-1]
-    ptr = lambda t: C.c_void_p(t.data_ptr() if t is not None else None)   # noqa: E731
-    N.check(N.lib().sdr_window_merge(ptr(est), ptr(carry), ptr(perm), ptr(out), B, S, A, T, W, H, k0, M,
-                                     ptr(scratch), _current(out.device)), "sdr_window_merge")
+    N.check(N.lib().sdr_window_merge(N.ptr(est), N.ptr(carry), N.ptr(perm), N.ptr(out), B, S, A, T, W, H, k0, M,
+                                     N.ptr(scratch), N.stream(out.device)), "sdr_window_merge")
 
 
 def separate_long(model, wav, window, hop=None, normalize=True, mixture_consistency=False, max_windows=32,

@@ -420,7 +420,8 @@ def test_corpus_graphs_evicted_while_replays_are_queued():
 # 3. One CausalStream across streams
 # ---------------------------------------------------------------------------------------------------------------------
 def alternated(s, chunks, streams, hold_on):
-    """Steps, a reset of slot 1 and the flush, alternating over ``streams``; those in ``hold_on`` sleep first."""
+    """Steps, a reset of slot 1 and the flush, the i-th on ``streams[i % len(streams)]``; those in ``hold_on`` sleep
+    first."""
     ops = [("step", 0), ("step", 1), ("reset", None), ("step", 2), ("step", 3), ("flush", None)]
     outs = []
     for i, (op, k) in enumerate(ops):
@@ -461,6 +462,34 @@ def test_causal_stream_alternating_streams():
     for k in range(5):
         for row, r in ((0, ref[k][0:1]), (1, ref1[k]), (2, ref[k][2:3])):
             fp64(got[k][row:row + 1], r)
+
+
+@gpu
+@pytest.mark.parametrize("inner", ["causal", "windowed"])
+def test_resampled_stream_alternating_streams(inner):
+    """A ``ResampledStream`` at 44.1 kHz around the model at 8 kHz: its two resamplers, the inner stream (a
+    ``CausalStream`` or a ``WindowedStream``) and the inner stream's masked reset.  The steps alternate between two
+    side streams, the first of them held; ``reset([1])`` runs on the other stream than the step before it and the flush
+    on a third.  Bitwise the same calls on one stream."""
+    cfg, sd, m = build("causal")
+    Cs = 4 * 441                    # 320 samples at 8 kHz: four granules of the causal stream, one hop of the windows
+    x = mixture(3, 1, 4 * Cs, seed=31)
+    chunks = [x[..., k * Cs:(k + 1) * Cs].to(DEV) for k in range(4)]
+
+    def make():
+        if inner == "causal":
+            return m.stream(3, Cs, sample_rate=44100, model_rate=8000)
+        return m.stream_windows(3, Cs, 480, 320, sample_rate=44100, model_rate=8000)
+    with torch.no_grad():
+        want = alternated(make(), chunks, [torch.cuda.current_stream()], [])
+        torch.cuda.synchronize()
+        a, b, c = torch.cuda.Stream(), torch.cuda.Stream(), torch.cuda.Stream()
+        s = make()
+        assert isinstance(s, P.ResampledStream)
+        got = alternated(s, chunks, [a, b, a, b, a, c], [a])
+        torch.cuda.synchronize()
+    for k, (g, w) in enumerate(zip(got, want)):
+        assert torch.equal(g, w), f"output {k}: max |d| = {(g - w).abs().max().item():.3e}"
 
 
 # ---------------------------------------------------------------------------------------------------------------------
@@ -762,6 +791,23 @@ COVERED = {
                                     "test_causal_stream_alternating_streams", "test_first_launches_from_racing_threads"],
     "streaming.CausalStream.reset": ["test_causal_stream_alternating_streams"],
     "streaming.CausalStream.flush": ["test_causal_stream_alternating_streams"],
+    "streaming.CausalStream._reset_masked": ["test_resampled_stream_alternating_streams"],
+    "window_stream.WindowedStream.step": ["test_steps_alternating_between_cuda_streams (test_gpu_window_stream.py)",
+                                         "test_resampled_stream_alternating_streams"],
+    "window_stream.WindowedStream.reset": ["test_steps_alternating_between_cuda_streams (test_gpu_window_stream.py)"],
+    "window_stream.WindowedStream.flush": ["test_steps_alternating_between_cuda_streams (test_gpu_window_stream.py)",
+                                          "test_resampled_stream_alternating_streams"],
+    "window_stream.WindowedStream._reset_masked": ["test_resampled_stream_alternating_streams"],
+    "resample_stream.ResampleStream._step": [
+        "test_alternating_cuda_streams_and_host_threads (test_gpu_resample_stream.py)",
+        "test_resampled_stream_alternating_streams"],
+    "resample_stream.ResampleStream._flush": [
+        "test_alternating_cuda_streams_and_host_threads (test_gpu_resample_stream.py)",
+        "test_resampled_stream_alternating_streams"],
+    "resample_stream.ResampleStream.reset": ["test_resampled_stream_alternating_streams"],
+    "resample_stream.ResampledStream.step": ["test_resampled_stream_alternating_streams"],
+    "resample_stream.ResampledStream.reset": ["test_resampled_stream_alternating_streams"],
+    "resample_stream.ResampledStream.flush": ["test_resampled_stream_alternating_streams"],
     "training._NativeTrain.forward": ["test_training_on_a_side_stream_survives_a_repack",
                                       "test_buffers_released_during_a_call"],
     "training._NativeTrain.backward": ["test_training_on_a_side_stream_survives_a_repack",
@@ -773,14 +819,15 @@ COVERED = {
 # and outputs): the caching allocator orders their reuse by itself, and no state outlives the call.
 PER_CALL = {"sisdr.StabilizedPermInvSISDRMetric.forward", "sisdr._PairwiseNegSDR.forward",
             "sisdr._PairwiseNegSDR.backward", "sisdr.PairwiseNegSDR.forward", "snr._forward",
-            "snr._SNRZeroRefs.backward", "mixture_consistency._project", "mixture_consistency._Consistency.backward"}
+            "snr._SNRZeroRefs.backward", "mixture_consistency._project", "mixture_consistency._Consistency.backward",
+            "windowed.gather", "windowed.merge", "resample.resample_poly", "stoi_metric.stoi"}
 # The shared machinery every entry above goes through.
-MACHINERY = {"_engine._call_shared", "_engine.packed_weights"}
+MACHINERY = {"_engine._call_shared", "_engine.packed_weights", "streaming.SlotStream._ordered"}
 
 
 def enqueuing_functions():
-    """``module.Class.method`` of every function in the package that hands a stream to the library or runs a call on
-    the model's shared state."""
+    """``module.Class.method`` of every function in the package that hands a stream to the library (``N.stream``), runs
+    a call on the model's shared state (``_call_shared``) or orders a stream's calls (``_ordered``)."""
     found = set()
     for path in glob.glob(os.path.join(REPO, "sudo_rm_rf_b200", "*.py")):
         mod = os.path.basename(path)[:-3]
@@ -791,13 +838,13 @@ def enqueuing_functions():
                     walk(ch, prefix + ch.name + ".")
                 elif isinstance(ch, ast.FunctionDef):
                     src = ast.unparse(ch)
-                    if "N.stream(" in src or "_call_shared(" in src:
+                    if "N.stream(" in src or "_call_shared(" in src or "_ordered(" in src:
                         found.add(mod + "." + prefix + ch.name)
         walk(ast.parse(open(path).read()), "")
     return found
 
 
-def test_every_enqueuing_entry_is_covered():
+def test_every_enqueuing_or_ordered_entry_is_covered():
     found = enqueuing_functions()
     assert len(found) >= 20
     listed = set(COVERED) | PER_CALL | MACHINERY

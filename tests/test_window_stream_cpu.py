@@ -246,9 +246,26 @@ def test_other_refusals():
 
 
 def test_defaults_follow_separate():
+    """The public signatures of the methods the four classes share, defaults included: GroupComm applies mixture
+    consistency by default everywhere but in ``forward_host``."""
     import inspect
+    want = {
+        "separate": "(self, input_wav, mixture_consistency={mc}, normalize=False, sample_rate=None, model_rate=None)",
+        "separate_long": "(self, input_wav, window, hop=None, normalize=True, mixture_consistency={mc}, "
+                         "max_windows=32, sample_rate=None, model_rate=None)",
+        "stream_windows": "(self, batch_size, chunk_samples, window, hop=None, normalize=True, "
+                          "mixture_consistency={mc}, sample_rate=None, model_rate=None)",
+        "forward_host": "(self, host_wav, host_out=None, mixture_consistency=False)",
+        "pad_to_appropriate_length": "(self, x)",
+        "remove_trailing_zeros": "(padded_x, initial_x)",
+    }
     for cls in (P.SuDORMRF, P.GroupCommSudoRmRf, P.CausalSuDORMRF, P.OriginalSuDORMRF):
+        for name, sig in want.items():
+            got = str(inspect.signature(getattr(cls, name)))
+            assert got == sig.format(mc=cls is P.GroupCommSudoRmRf), (cls, name, got)
         sep = inspect.signature(cls.separate).parameters["mixture_consistency"].default
         sw = inspect.signature(cls.stream_windows).parameters
         assert sw["mixture_consistency"].default == sep and sw["normalize"].default is True, cls
+    assert str(inspect.signature(P.CausalSuDORMRF.stream)) == \
+        "(self, batch_size, chunk_samples, mixture_consistency=False, sample_rate=None, model_rate=None)"
     assert P.WindowedStream is P.window_stream.WindowedStream
