@@ -1070,12 +1070,7 @@ int sdr_stream_reset(const sdr_config* cfg, void* state, int B, const int32_t* h
     const size_t slot = stream_state(l).slot * sizeof(float);
     if (!host_slots_or_null)
         return cuda_status(cudaMemsetAsync(state, 0, (size_t)B * slot, st));
-    for (int i = 0; i < n; ++i)
-        if (host_slots_or_null[i] < 0 || host_slots_or_null[i] >= B) return SDR_ERR_BAD_ARGUMENT;
-    for (int i = 0; i < n; ++i)
-        SDR_TRY(cuda_status(
-            cudaMemsetAsync(static_cast<char*>(state) + (size_t)host_slots_or_null[i] * slot, 0, slot, st)));
-    return SDR_OK;
+    return reset_slots({{state, slot}}, B, host_slots_or_null, n, nullptr, st);
 }
 
 int sdr_stream_reset_masked(const sdr_config* cfg, void* state, int B, const uint8_t* mask, sdr_stream stream) {
@@ -1083,8 +1078,8 @@ int sdr_stream_reset_masked(const sdr_config* cfg, void* state, int B, const uin
     SDR_TRY(check_stream_config(l));
     if (B <= 0) return SDR_ERR_BAD_ARGUMENT;
     SDR_TRY(check_buffers({{state, 16}, {mask}}));
-    return launch_zero_masked_slots(state, B, stream_state(l).slot * sizeof(float), mask,
-                                    static_cast<cudaStream_t>(stream));
+    return reset_slots({{state, stream_state(l).slot * sizeof(float)}}, B, nullptr, 0, mask,
+                       static_cast<cudaStream_t>(stream));
 }
 
 int sdr_stream_step(const sdr_config* cfg, const void* packed, void* state, const float* chunk, float* out, int B,

@@ -3,6 +3,7 @@
 // error (the library is linked with undefined symbols refused) instead of a failure at load time.  Every launcher
 // enqueues its kernels through launch.cuh.
 #pragma once
+#include <initializer_list>
 #include "launch.cuh"
 
 namespace sdr {
@@ -72,7 +73,10 @@ int launch_causal_stream(const float* y, const float* slope_in, const float* con
                          int F, cudaStream_t st);
 int launch_stream_ola(const float* frames, const float* chunk, float* state, long long slot_stride, long long carry_off,
                       float* out, int B, int SA, int A, int k, int F, long long C, int mc, cudaStream_t st);
-int launch_zero_masked_slots(void* base, int B, size_t slot_bytes, const unsigned char* mask, cudaStream_t st);
+// slot b of a region is [base + b * slot_bytes, base + (b + 1) * slot_bytes)
+struct SlotRegion { void* base; size_t slot_bytes; };
+int reset_slots(std::initializer_list<SlotRegion> regions, int B, const int* slots, int n, const unsigned char* mask,
+                cudaStream_t st);
 int launch_stream_flush(const float* state, long long slot_stride, long long carry_off, float* tail, int B, int SA,
                         int hop, int mc, cudaStream_t st);
 

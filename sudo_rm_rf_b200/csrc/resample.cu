@@ -293,37 +293,33 @@ size_t resample_stream_state_bytes(int B, int rows, long long C, int up, int dow
     return g.err == SDR_OK ? g.bytes : 0;
 }
 
+// The refusals of every streaming entry in order: the plan's, a null state or !args_ok, a small state, a misaligned one.
+static int stream_refusal(const ResampleStreamPlan& g, const void* state, bool args_ok, size_t state_bytes) {
+    if (g.err) return g.err;
+    if (!state || !args_ok) return SDR_ERR_BAD_ARGUMENT;
+    if (state_bytes < g.bytes) return SDR_ERR_WORKSPACE;
+    return reinterpret_cast<uintptr_t>(state) % 256 ? SDR_ERR_BAD_ARGUMENT : SDR_OK;
+}
+
 int resample_stream_reset(void* state, size_t state_bytes, int B, int rows, long long C, int up, int down, long long delay,
                           long long lead, const int* slots, int n, cudaStream_t st) {
     const ResampleStreamPlan g(B, rows, C, up, down, delay, lead);
-    if (g.err) return g.err;
-    if (!state || (slots && n < 0)) return SDR_ERR_BAD_ARGUMENT;
-    if (state_bytes < g.bytes) return SDR_ERR_WORKSPACE;
-    if (reinterpret_cast<uintptr_t>(state) % 256) return SDR_ERR_BAD_ARGUMENT;
-    if (slots)
-        for (int i = 0; i < n; ++i)
-            if (slots[i] < 0 || slots[i] >= B) return SDR_ERR_BAD_ARGUMENT;
+    if (const int e = stream_refusal(g, state, !(slots && n < 0), state_bytes)) return e;
     char* base = static_cast<char*>(state);
     long long* count = reinterpret_cast<long long*>(base + g.count_off);
     float* hist = reinterpret_cast<float*>(base + g.hist_off);
-    const long long R = (long long)B * rows, slot = (long long)rows * g.Hs;
-    int e;
     if (!slots) {                                 // the whole state: the filter, the counters and both histories
         double* h = reinterpret_cast<double*>(base);
+        int e;
         if ((e = launch(resample_taps_kernel, (unsigned)((2 * g.L + 1 + 255) / 256), 256, 0, st, h, g.L,
                         std::max(g.p, g.q))))
             return e;
         if ((e = launch(resample_normalise_kernel, 1, 1024, 0, st, h, g.L, g.p))) return e;
         return cuda_status(cudaMemsetAsync(count, 0, g.bytes - g.count_off, st));
     }
-    for (int i = 0; i < n; ++i) {
-        const long long b = slots[i];
-        if ((e = cuda_status(cudaMemsetAsync(count + b, 0, sizeof(long long), st))) ||
-            (e = cuda_status(cudaMemsetAsync(hist + b * slot, 0, slot * sizeof(float), st))) ||
-            (e = cuda_status(cudaMemsetAsync(hist + R * g.Hs + b * slot, 0, slot * sizeof(float), st))))
-            return e;
-    }
-    return SDR_OK;
+    const size_t slot = (size_t)rows * g.Hs * sizeof(float);        // one slot's rows of one history buffer
+    return reset_slots({{count, sizeof(long long)}, {hist, slot}, {hist + (long long)B * rows * g.Hs, slot}}, B, slots,
+                       n, nullptr, st);
 }
 
 // A step (tail_len < 0: x is the chunk of C samples) or a flush (x is the tail of tail_len samples, maybe null when
@@ -367,10 +363,7 @@ int launch_resample_stream_step(void* state, size_t state_bytes, const float* ch
                                 float* out, int B, int rows, long long C, int up, int down, long long delay,
                                 long long lead, cudaStream_t st) {
     const ResampleStreamPlan g(B, rows, C, up, down, delay, lead);
-    if (g.err) return g.err;
-    if (!state || !chunk || !out) return SDR_ERR_BAD_ARGUMENT;
-    if (state_bytes < g.bytes) return SDR_ERR_WORKSPACE;
-    if (reinterpret_cast<uintptr_t>(state) % 256) return SDR_ERR_BAD_ARGUMENT;
+    if (const int e = stream_refusal(g, state, chunk && out, state_bytes)) return e;
     return resample_stream_run(g, state, chunk, -1, zero, out, B, rows, C, delay, lead, st);
 }
 
@@ -378,11 +371,8 @@ int launch_resample_stream_flush(const void* state, size_t state_bytes, const fl
                                  const unsigned char* zero, float* out, int B, int rows, long long C, int up,
                                  int down, long long delay, long long lead, cudaStream_t st) {
     const ResampleStreamPlan g(B, rows, C, up, down, delay, lead);
-    if (g.err) return g.err;
-    if (!state || !out || tail_len < 0 || tail_len > kResampleMaxT || (!tail && tail_len > 0))
-        return SDR_ERR_BAD_ARGUMENT;
-    if (state_bytes < g.bytes) return SDR_ERR_WORKSPACE;
-    if (reinterpret_cast<uintptr_t>(state) % 256) return SDR_ERR_BAD_ARGUMENT;
+    const bool args_ok = out && tail_len >= 0 && tail_len <= kResampleMaxT && (tail || tail_len == 0);
+    if (const int e = stream_refusal(g, state, args_ok, state_bytes)) return e;
     // the state is only read: no history is written and the counters do not move
     return resample_stream_run(g, const_cast<void*>(state), tail, tail_len, zero, out, B, rows, C, delay, lead, st);
 }

@@ -327,13 +327,32 @@ __global__ void zero_masked_slots_kernel(unsigned* __restrict__ base, long long 
         if (mask[e / words]) base[e] = 0u;
 }
 
-int launch_zero_masked_slots(void* base, int B, size_t slot_bytes, const unsigned char* mask, cudaStream_t st) {
+static int launch_zero_masked_slots(void* base, int B, size_t slot_bytes, const unsigned char* mask, cudaStream_t st) {
     if (!base || !mask || B <= 0 || slot_bytes % 4 || reinterpret_cast<uintptr_t>(base) % 4) return SDR_ERR_BAD_ARGUMENT;
     const long long words = (long long)(slot_bytes / 4), total = words * B;
     if (total == 0) return SDR_OK;
     const long long grid = std::min((total + 255) / 256, (long long)std::max(sm_count(), 1) * 8);
     return launch(zero_masked_slots_kernel, (unsigned)grid, 256, 0, st, static_cast<unsigned*>(base), words, total,
                   mask);
+}
+
+// Zeroes slot b of every region for the n slots listed on the host (all checked before the first memset) or the slots
+// whose mask[b] is set (one launch per region); exactly one of `slots` and `mask` is given.
+int reset_slots(std::initializer_list<SlotRegion> regions, int B, const int* slots, int n, const unsigned char* mask,
+                cudaStream_t st) {
+    if (mask) {
+        for (const SlotRegion& r : regions)
+            if (const int e = launch_zero_masked_slots(r.base, B, r.slot_bytes, mask, st)) return e;
+        return SDR_OK;
+    }
+    for (int i = 0; i < n; ++i)
+        if (slots[i] < 0 || slots[i] >= B) return SDR_ERR_BAD_ARGUMENT;
+    for (int i = 0; i < n; ++i)
+        for (const SlotRegion& r : regions)
+            if (const int e = cuda_status(cudaMemsetAsync(static_cast<char*>(r.base) + (size_t)slots[i] * r.slot_bytes,
+                                                          0, r.slot_bytes, st)))
+                return e;
+    return SDR_OK;
 }
 
 }  // namespace sdr

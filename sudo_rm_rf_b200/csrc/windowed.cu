@@ -387,58 +387,49 @@ int launch_window_merge(const float* est, void* carry, int* perm, float* out, in
 
 // ---- windowed stream (DESIGN.md section 7f) ----------------------------------------------------------------------
 
-static bool stream_shape_ok(int B, int S, int A, long long W, long long H) {
-    return B > 0 && S > 0 && S <= 4 && A > 0 && WindowPlan(W + 1, W, H).ok;
+// SDR_OK, or the refusal of a bad shape (more than 4 sources: unsupported) or of a state off a 256-byte boundary.
+static int stream_refusal(const void* state, int B, int S, int A, long long W, long long H) {
+    if (!(B > 0 && S > 0 && S <= 4 && A > 0 && WindowPlan(W + 1, W, H).ok))
+        return S > 4 ? SDR_ERR_UNSUPPORTED : SDR_ERR_BAD_ARGUMENT;
+    return reinterpret_cast<uintptr_t>(state) % 256 ? SDR_ERR_BAD_ARGUMENT : SDR_OK;
 }
 
 size_t window_stream_state_bytes(int B, int S, int A, long long W, long long H) {
-    if (!stream_shape_ok(B, S, A, W, H)) return 0;
+    if (stream_refusal(nullptr, B, S, A, W, H)) return 0;
     return WindowStreamState(nullptr, B, S, A, W, H).bytes;
+}
+
+// Zeroes the whole state (neither slots nor mask given) or each chosen slot's pi, carried estimate, history and
+// counter.  The counter alone decides what a step reads; the rest is zeroed for hygiene.
+static int reset_stream(void* state, int B, int S, int A, long long W, long long H, const int* slots, int n,
+                        const unsigned char* mask, cudaStream_t st) {
+    if (const int e = stream_refusal(state, B, S, A, W, H)) return e;
+    const WindowStreamState ss(state, B, S, A, W, H);
+    if (!slots && !mask) return cuda_status(cudaMemsetAsync(state, 0, ss.bytes, st));
+    return reset_slots({{ss.carry.pi, (size_t)S * 4}, {ss.carry.est, (size_t)S * A * W * 4},
+                        {ss.hist, (size_t)A * H * 4}, {ss.count, 8}},
+                       B, slots, n, mask, st);
 }
 
 int window_stream_reset(void* state, int B, int S, int A, long long W, long long H, const int* slots, int n,
                         cudaStream_t st) {
     if (!state || (slots && n < 0)) return SDR_ERR_BAD_ARGUMENT;
-    if (!stream_shape_ok(B, S, A, W, H)) return S > 4 ? SDR_ERR_UNSUPPORTED : SDR_ERR_BAD_ARGUMENT;
-    if (reinterpret_cast<uintptr_t>(state) % 256) return SDR_ERR_BAD_ARGUMENT;
-    const WindowStreamState ss(state, B, S, A, W, H);
-    if (!slots) return cudaMemsetAsync(state, 0, ss.bytes, st) == cudaSuccess ? SDR_OK : SDR_ERR_CUDA;
-    for (int i = 0; i < n; ++i)
-        if (slots[i] < 0 || slots[i] >= B) return SDR_ERR_BAD_ARGUMENT;
-    const size_t SAW = (size_t)S * A * W, AH = (size_t)A * H;
-    for (int i = 0; i < n; ++i) {      // the counter alone decides what a step reads; the rest is zeroed for hygiene
-        const size_t b = slots[i];
-        if (cudaMemsetAsync(ss.carry.pi + b * S, 0, (size_t)S * 4, st) != cudaSuccess ||
-            cudaMemsetAsync(ss.carry.est + b * SAW, 0, SAW * 4, st) != cudaSuccess ||
-            cudaMemsetAsync(ss.hist + b * AH, 0, AH * 4, st) != cudaSuccess ||
-            cudaMemsetAsync(ss.count + b, 0, 8, st) != cudaSuccess)
-            return SDR_ERR_CUDA;
-    }
-    return SDR_OK;
+    return reset_stream(state, B, S, A, W, H, slots, n, nullptr, st);
 }
 
 // window_stream_reset of the slots whose mask[b] is set, the mask read on the device.
 int window_stream_reset_masked(void* state, int B, int S, int A, long long W, long long H, const unsigned char* mask,
                                cudaStream_t st) {
     if (!state || !mask) return SDR_ERR_BAD_ARGUMENT;
-    if (!stream_shape_ok(B, S, A, W, H)) return S > 4 ? SDR_ERR_UNSUPPORTED : SDR_ERR_BAD_ARGUMENT;
-    if (reinterpret_cast<uintptr_t>(state) % 256) return SDR_ERR_BAD_ARGUMENT;
-    const WindowStreamState ss(state, B, S, A, W, H);
-    int e;
-    if ((e = launch_zero_masked_slots(ss.carry.pi, B, (size_t)S * 4, mask, st)) ||
-        (e = launch_zero_masked_slots(ss.carry.est, B, (size_t)S * A * W * 4, mask, st)) ||
-        (e = launch_zero_masked_slots(ss.hist, B, (size_t)A * H * 4, mask, st)))
-        return e;
-    return launch_zero_masked_slots(ss.count, B, 8, mask, st);
+    return reset_stream(state, B, S, A, W, H, nullptr, 0, mask, st);
 }
 
 // C = 0 with chunk null: the flush's window [B][A][W]; nothing in the state changes.
 int launch_window_stream_gather(void* state, const float* chunk, float* batch, int B, int S, int A, long long C,
                                 long long W, long long H, cudaStream_t st) {
     if (!state || !batch || (!chunk && C != 0)) return SDR_ERR_BAD_ARGUMENT;
-    if (!stream_shape_ok(B, S, A, W, H)) return S > 4 ? SDR_ERR_UNSUPPORTED : SDR_ERR_BAD_ARGUMENT;
+    if (const int e = stream_refusal(state, B, S, A, W, H)) return e;
     if (chunk && (C <= 0 || C % H)) return SDR_ERR_BAD_ARGUMENT;
-    if (reinterpret_cast<uintptr_t>(state) % 256) return SDR_ERR_BAD_ARGUMENT;
     const WindowStreamState ss(state, B, S, A, W, H);
     const int q = chunk ? (int)(C / H) : 1;
     const long long rows = (long long)B * q * A;
@@ -457,9 +448,8 @@ size_t window_stream_merge_scratch_bytes(int B, int S, long long C, long long H)
 int launch_window_stream_merge(const float* est, void* state, float* out, int B, int S, int A, long long C,
                                long long W, long long H, void* scratch, cudaStream_t st) {
     if (!est || !state || !out || !scratch) return SDR_ERR_BAD_ARGUMENT;
-    if (!stream_shape_ok(B, S, A, W, H)) return S > 4 ? SDR_ERR_UNSUPPORTED : SDR_ERR_BAD_ARGUMENT;
-    if (window_stream_merge_scratch_bytes(B, S, C, H) == 0) return SDR_ERR_BAD_ARGUMENT;
-    if (reinterpret_cast<uintptr_t>(state) % 256 || reinterpret_cast<uintptr_t>(scratch) % 8)
+    if (const int e = stream_refusal(state, B, S, A, W, H)) return e;
+    if (window_stream_merge_scratch_bytes(B, S, C, H) == 0 || reinterpret_cast<uintptr_t>(scratch) % 8)
         return SDR_ERR_BAD_ARGUMENT;
     WindowStreamState ss(state, B, S, A, W, H);
     const int q = (int)(C / H);
@@ -472,9 +462,8 @@ size_t window_stream_flush_scratch_bytes(int B, int S) { return window_merge_scr
 int launch_window_stream_flush(const float* single, const float* est, const void* state, float* out, int B, int S,
                                int A, long long W, long long H, void* scratch, cudaStream_t st) {
     if (!single || !state || !out || !scratch || (!est && W < 2 * H)) return SDR_ERR_BAD_ARGUMENT;
-    if (!stream_shape_ok(B, S, A, W, H)) return S > 4 ? SDR_ERR_UNSUPPORTED : SDR_ERR_BAD_ARGUMENT;
-    if (reinterpret_cast<uintptr_t>(state) % 256 || reinterpret_cast<uintptr_t>(scratch) % 8)
-        return SDR_ERR_BAD_ARGUMENT;
+    if (const int e = stream_refusal(state, B, S, A, W, H)) return e;
+    if (reinterpret_cast<uintptr_t>(scratch) % 8) return SDR_ERR_BAD_ARGUMENT;
     // the state is only read: the carry's pi is not written when `single` is given
     WindowStreamState ss(const_cast<void*>(state), B, S, A, W, H);
     return merge_stages(est, ss.carry, single, nullptr, out, B, S, A, W, H, 1, WinOrigin{ss.count, -1, 0}, 0, H, H, 0,
@@ -482,7 +471,7 @@ int launch_window_stream_flush(const float* single, const float* est, const void
 }
 
 int window_stream_launch_count(int B, int S, int A, long long C, long long W, long long H) {
-    if (!stream_shape_ok(B, S, A, W, H)) return S > 4 ? SDR_ERR_UNSUPPORTED : SDR_ERR_BAD_ARGUMENT;
+    if (const int e = stream_refusal(nullptr, B, S, A, W, H)) return e;
     if (window_stream_merge_scratch_bytes(B, S, C, H) == 0) return SDR_ERR_BAD_ARGUMENT;
     return 6;          // gather, history; align, scan, overlap-add, carry (the forward between them not counted)
 }

@@ -315,31 +315,40 @@ def test_mixture_consistency_matches_separate():
         st.stream(2, 160, mixture_consistency=True)
 
 
-def test_launch_count_matches_profiler():
+def test_launch_count_matches_captured_graph():
+    """The kernels two consecutive steps enqueue, counted as the kernel nodes of a CUDA graph captured from them
+    (memsets are nodes of another type), against sdr_stream_launch_count.  torch.profiler's device records are not
+    used: in a process that has profiled many times they can miss a kernel or a whole step."""
     cfg, sd, m = build(MID)
     G = granule(cfg)
     s = m.stream(3, 2 * G)
     x = mixture(3, 1, 2 * G, seed=10).to(DEV)
-    with torch.no_grad():
-        s.step(x)
-        torch.cuda.synchronize()
-        with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CPU,
-                                                torch.profiler.ProfilerActivity.CUDA]) as prof:
-            for _ in range(4):
-                s.step(x)
-            torch.cuda.synchronize()
-    ev = sorted((e.time_range.start, e.name) for e in prof.events()
-                if e.device_type == torch.autograd.DeviceType.CUDA
-                and not e.name.startswith(("Memset", "Memcpy", "memset", "memcpy")))
+    out = torch.empty(3, 2, 2 * G, device=DEV)
     want = N.lib().sdr_stream_launch_count(C.byref(_engine.make_config(m)), 3, 2 * G)
     assert want == 3 * MID["num_blocks"] + 6
-    # a step ends with its overlap-add kernel: count the kernels of the steps that lie wholly inside the window
-    # (the profiler may miss records at the edges of a short window)
-    ends = [i for i, (_, n) in enumerate(ev) if "stream_ola_kernel" in n]
-    assert len(ends) >= 3, collections.Counter(n for _, n in ev)
-    per_step = [ends[j + 1] - ends[j] for j in range(len(ends) - 1)]
-    print("kernels per profiled step:", per_step)
-    assert all(p == want for p in per_step), (want, per_step, collections.Counter(n for _, n in ev[ends[0] + 1:ends[1] + 1]))
+    with torch.no_grad():
+        side = torch.cuda.Stream()
+        side.wait_stream(torch.cuda.current_stream())
+        with torch.cuda.stream(side):           # warm-up outside capture: weights packed, shared memory opted in
+            s.step(x, out=out)
+        torch.cuda.current_stream().wait_stream(side)
+        graph = torch.cuda.CUDAGraph(keep_graph=True)
+        with torch.cuda.graph(graph):
+            s.step(x, out=out)
+            s.step(x, out=out)
+    cu = C.CDLL("libcuda.so.1")
+    g = C.c_void_p(graph.raw_cuda_graph())
+    n = C.c_size_t(0)
+    assert cu.cuGraphGetNodes(g, None, C.byref(n)) == 0
+    nodes = (C.c_void_p * n.value)()
+    assert cu.cuGraphGetNodes(g, nodes, C.byref(n)) == 0
+    types = []
+    for node in nodes:
+        t = C.c_int(-1)
+        assert cu.cuGraphNodeGetType(C.c_void_p(node), C.byref(t)) == 0
+        types.append(t.value)
+    print("graph nodes of two steps by type:", collections.Counter(types))
+    assert types.count(0) == 2 * want, (want, collections.Counter(types))      # 0: CU_GRAPH_NODE_TYPE_KERNEL
 
 
 def test_argument_errors():
