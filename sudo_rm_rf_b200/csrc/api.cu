@@ -1157,24 +1157,6 @@ int sdr_forward_host(const sdr_config* cfg, const void* packed, const float* hos
     return cuda_status(cudaMemcpyAsync(host_out, d_out, out_bytes, cudaMemcpyDeviceToHost, st));
 }
 
-int sdr_mixture_consistency(const float* est, const float* mix, float* out, int B, int S, int64_t T,
-                            int weights_type, void* scratch, sdr_stream stream) {
-    return launch_mixture_consistency(est, mix, out, B, S, T, weights_type, scratch,
-                                      static_cast<cudaStream_t>(stream));
-}
-
-size_t sdr_mixture_consistency_backward_scratch_bytes(int B, int S, int64_t T, int weights_type) {
-    return mc_backward_scratch_bytes(B, S, T, weights_type);
-}
-
-int sdr_mixture_consistency_backward(const float* est, const float* mix, const float* grad_out, float* grad_est,
-                                     float* grad_mix_or_null, int B, int S, int64_t T, int weights_type, void* scratch,
-                                     sdr_stream stream) {
-    if (scratch && reinterpret_cast<uintptr_t>(scratch) % 16) return SDR_ERR_BAD_ARGUMENT;
-    return launch_mixture_consistency_backward(est, mix, grad_out, grad_est, grad_mix_or_null, B, S, T, weights_type,
-                                               scratch, static_cast<cudaStream_t>(stream));
-}
-
 int sdr_encoder(const float* wav, const float* weight, float* enc, double* stats,
                 int B, int A, int64_t T, int N, int K, int L, sdr_stream stream) {
     if (!wav || !weight || !enc || !stats) return SDR_ERR_BAD_ARGUMENT;
@@ -1240,46 +1222,6 @@ int sdr_depthwise(const float* x, const sdr_norm_in* fin, const float* w5, const
     if (stride == 2 && (Lin % 2)) return SDR_ERR_BAD_ARGUMENT;
     return launch_depthwise(x, make_norm(fin), w5, bias, y, stats_out, samples, C, Lin, stride,
                             static_cast<cudaStream_t>(stream));
-}
-
-static size_t pyr_table_offset(int samples, int C, int D) {
-    return (pyramid_rowstats_bytes(samples, C, D) + 255) & ~(size_t)255;
-}
-
-size_t sdr_pyramid_scratch_bytes(int samples, int C, int D, int L) {
-    if (samples <= 0 || !pyramid_eligible(D, samples, C, L)) return 0;
-    return pyr_table_offset(samples, C, D) + pyramid_table_bytes(samples, C, D);
-}
-
-int sdr_depthwise_pyramid(const float* y, const sdr_norm_in* fin, const float* const* w5, const float* const* bias,
-                          const float* const* gamma, const float* const* beta, float* const* z, double* stats0,
-                          void* scratch, int D, int samples, int C, int L, sdr_stream stream) {
-    if (!y || !w5 || !bias || !gamma || !beta || !z || !stats0 || !scratch) return SDR_ERR_BAD_ARGUMENT;
-    if (!pyramid_eligible(D, samples, C, L)) return SDR_ERR_UNSUPPORTED;
-    char* sc = static_cast<char*>(scratch);
-    return launch_pyramid(y, make_norm(fin), w5, bias, gamma, beta, z, stats0, reinterpret_cast<double*>(sc),
-                          reinterpret_cast<float*>(sc + pyr_table_offset(samples, C, D)), D, samples, C, L,
-                          static_cast<cudaStream_t>(stream));
-}
-
-int sdr_merge_pyramid(const float* const* z, const void* scratch, int D, float* m, double* stats_out,
-                      int samples, int C, int L, sdr_stream stream) {
-    if (!z || !scratch || !m || !stats_out) return SDR_ERR_BAD_ARGUMENT;
-    if (!pyramid_eligible(D, samples, C, L)) return SDR_ERR_UNSUPPORTED;
-    const char* sc = static_cast<const char*>(scratch);
-    return launch_merge_pyramid(z, reinterpret_cast<const float*>(sc + pyr_table_offset(samples, C, D)), D, m, stats_out,
-                                samples, C, L, static_cast<cudaStream_t>(stream));
-}
-
-int sdr_depthwise_pyramid_fused(const float* y, const sdr_norm_in* fin, const float* const* w5, const float* const* bias,
-                                const float* const* gamma, const float* const* beta, float* m, double* stats0,
-                                double* stats_m, void* scratch, int D, int samples, int C, int L, sdr_stream stream) {
-    if (!y || !w5 || !bias || !gamma || !beta || !m || !stats0 || !stats_m || !scratch) return SDR_ERR_BAD_ARGUMENT;
-    if (!pyramid_eligible(D, samples, C, L)) return SDR_ERR_UNSUPPORTED;
-    char* sc = static_cast<char*>(scratch);
-    return launch_pyramid_fused(y, make_norm(fin), w5, bias, gamma, beta, m, stats0, stats_m, reinterpret_cast<double*>(sc),
-                                reinterpret_cast<float*>(sc + pyr_table_offset(samples, C, D)), D, samples, C, L,
-                                static_cast<cudaStream_t>(stream));
 }
 
 int sdr_causal_pyramid(const float* y, const float* slope_in, const float* const* w21, const float* const* bias,
@@ -1386,189 +1328,6 @@ int sdr_separate_ragged(const sdr_config* cfg, const void* packed, const float* 
     if (T <= 0 || padded_len(l, T) != T) return SDR_ERR_BAD_ARGUMENT;   // the bucket width is a padded length
     return separate_impl(cfg, packed, wav, lengths, out, B, T, apply_mixture_consistency, rescale,
                          workspace, workspace_bytes, stream);
-}
-
-int sdr_pairwise_neg_sdr(const float* est, const float* target, float* out, int B, int S, int64_t T, int sdr_type,
-                         int zero_mean, int take_log, void* scratch, sdr_stream stream) {
-    if (scratch && reinterpret_cast<uintptr_t>(scratch) % 8) return SDR_ERR_BAD_ARGUMENT;
-    return launch_pairwise_neg_sdr(est, target, out, B, S, T, sdr_type, zero_mean, take_log, scratch,
-                                   static_cast<cudaStream_t>(stream));
-}
-
-size_t sdr_pairwise_neg_sdr_train_scratch_bytes(int B, int S, int64_t T) { return pairwise_train_scratch_bytes(B, S, T); }
-size_t sdr_pairwise_neg_sdr_coef_bytes(int B, int S) { return pairwise_coef_bytes(B, S); }
-
-int sdr_pairwise_neg_sdr_train(const float* est, const float* target, float* out, void* coef, int B, int S, int64_t T,
-                               int sdr_type, int zero_mean, int take_log, void* scratch, sdr_stream stream) {
-    if ((scratch && reinterpret_cast<uintptr_t>(scratch) % 8) || (coef && reinterpret_cast<uintptr_t>(coef) % 8))
-        return SDR_ERR_BAD_ARGUMENT;
-    return launch_pairwise_neg_sdr_train(est, target, out, coef, B, S, T, sdr_type, zero_mean, take_log, scratch,
-                                         static_cast<cudaStream_t>(stream));
-}
-
-int sdr_pairwise_neg_sdr_backward(const float* est, const float* target, const void* coef, const float* grad_out,
-                                  float* grad_est, int B, int S, int64_t T, sdr_stream stream) {
-    if (coef && reinterpret_cast<uintptr_t>(coef) % 8) return SDR_ERR_BAD_ARGUMENT;
-    return launch_pairwise_neg_sdr_backward(est, target, coef, grad_out, grad_est, B, S, T,
-                                            static_cast<cudaStream_t>(stream));
-}
-
-size_t sdr_pit_sisdr_scratch_bytes(int B, int S) { return pit_sisdr_scratch_bytes(B, S); }
-
-int sdr_pit_sisdr(const float* est, const float* target, const float* mixture_or_null, float* best, int32_t* perm_index,
-                  int B, int S, int64_t T, int zero_mean, int improvement, double eps,
-                  void* scratch, sdr_stream stream) {
-    if (scratch && reinterpret_cast<uintptr_t>(scratch) % 8) return SDR_ERR_BAD_ARGUMENT;
-    return launch_pit_sisdr(est, target, mixture_or_null, best, perm_index, B, S, T, zero_mean, improvement, eps,
-                            scratch, static_cast<cudaStream_t>(stream));
-}
-
-size_t sdr_stabilized_sisdr_scratch_bytes(int B, int n_est, int n_act) { return stabilized_sisdr_scratch_bytes(B, n_est, n_act); }
-
-int sdr_stabilized_sisdr(const float* est, const float* target, float* best, int32_t* perm_index, int B, int est_rows,
-                         int n_est, int n_act, int64_t T, int zero_mean, int improvement, double eps,
-                         void* scratch, sdr_stream stream) {
-    if (scratch && reinterpret_cast<uintptr_t>(scratch) % 8) return SDR_ERR_BAD_ARGUMENT;
-    return launch_stabilized_sisdr(est, target, best, perm_index, B, est_rows, n_est, n_act, T, zero_mean, improvement, eps,
-                                   scratch, static_cast<cudaStream_t>(stream));
-}
-
-size_t sdr_snr_zero_refs_scratch_bytes(int B, int S, int64_t T) { return snr_zero_refs_scratch_bytes(B, S, T); }
-size_t sdr_snr_zero_refs_coef_bytes(int B, int S) { return snr_zero_refs_coef_bytes(B, S); }
-
-int sdr_snr_zero_refs(const float* est, const float* target, float* value, int32_t* perm_index, void* coef, int B, int S,
-                      int64_t T, int zero_mean, double inactivity_threshold, double eps, void* scratch,
-                      sdr_stream stream) {
-    if ((scratch && reinterpret_cast<uintptr_t>(scratch) % 8) || (coef && reinterpret_cast<uintptr_t>(coef) % 8))
-        return SDR_ERR_BAD_ARGUMENT;
-    return launch_snr_zero_refs(est, target, value, perm_index, coef, B, S, T, zero_mean, inactivity_threshold, eps,
-                                scratch, static_cast<cudaStream_t>(stream));
-}
-
-int sdr_snr_zero_refs_backward(const float* est, const float* target, const void* coef, const float* grad_value,
-                               float* grad_est, int B, int S, int64_t T, int64_t T_grad, sdr_stream stream) {
-    if (coef && reinterpret_cast<uintptr_t>(coef) % 8) return SDR_ERR_BAD_ARGUMENT;
-    return launch_snr_zero_refs_backward(est, target, coef, grad_value, grad_est, B, S, T, T_grad,
-                                         static_cast<cudaStream_t>(stream));
-}
-
-size_t sdr_bss_eval_scratch_bytes(int B, int S, int64_t T, int F) { return bss_eval_scratch_bytes(B, S, T, F); }
-
-int sdr_bss_eval(const float* reference, const float* estimate, double* sdr, double* sir, double* sar,
-                 int32_t* perm_or_null, int B, int S, int64_t T, int F, int compute_permutation, void* scratch,
-                 sdr_stream stream) {
-    if (scratch && reinterpret_cast<uintptr_t>(scratch) % 8) return SDR_ERR_BAD_ARGUMENT;
-    return launch_bss_eval(reference, estimate, nullptr, sdr, sir, sar, perm_or_null, nullptr, nullptr, nullptr, B, S,
-                           T, F, compute_permutation, scratch, static_cast<cudaStream_t>(stream));
-}
-
-int sdr_bss_eval_mixture(const float* reference, const float* estimate, const float* mixture, double* sdr,
-                         double* sir, double* sar, int32_t* perm_or_null, double* mix_sdr, double* mix_sir,
-                         double* mix_sar, int B, int S, int64_t T, int F, int compute_permutation, void* scratch,
-                         sdr_stream stream) {
-    if (!mixture || (scratch && reinterpret_cast<uintptr_t>(scratch) % 8)) return SDR_ERR_BAD_ARGUMENT;
-    return launch_bss_eval(reference, estimate, mixture, sdr, sir, sar, perm_or_null, mix_sdr, mix_sir, mix_sar, B, S,
-                           T, F, compute_permutation, scratch, static_cast<cudaStream_t>(stream));
-}
-
-size_t sdr_stoi_scratch_bytes(int B, int S, int64_t T, int fs) { return stoi_scratch_bytes(B, S, T, fs); }
-
-int sdr_stoi(const float* reference, const float* estimate, const float* mixture_or_null,
-             const int64_t* lengths_or_null, double* stoi, double* mix_stoi_or_null, int B, int S, int64_t T, int fs,
-             void* scratch, sdr_stream stream) {
-    if (scratch && reinterpret_cast<uintptr_t>(scratch) % 8) return SDR_ERR_BAD_ARGUMENT;
-    return launch_stoi(reference, estimate, mixture_or_null, reinterpret_cast<const long long*>(lengths_or_null), stoi,
-                       mix_stoi_or_null, B, S, T, fs, scratch, static_cast<cudaStream_t>(stream));
-}
-
-size_t sdr_resample_poly_scratch_bytes(int up, int down) { return resample_poly_scratch_bytes(up, down); }
-
-int sdr_resample_poly(const float* x, float* out, int64_t rows, int64_t T, int up, int down, void* scratch,
-                      size_t scratch_bytes, sdr_stream stream) {
-    return launch_resample_poly(x, out, rows, T, up, down, scratch, scratch_bytes, static_cast<cudaStream_t>(stream));
-}
-
-size_t sdr_resample_stream_state_bytes(int B, int rows, int64_t C, int up, int down, int64_t delay, int64_t lead) {
-    return resample_stream_state_bytes(B, rows, C, up, down, delay, lead);
-}
-
-int sdr_resample_stream_reset(void* state, size_t state_bytes, int B, int rows, int64_t C, int up, int down,
-                              int64_t delay, int64_t lead, const int32_t* host_slots_or_null, int n, sdr_stream stream) {
-    return resample_stream_reset(state, state_bytes, B, rows, C, up, down, delay, lead, host_slots_or_null, n,
-                                 static_cast<cudaStream_t>(stream));
-}
-
-int sdr_resample_stream_step(void* state, size_t state_bytes, const float* chunk, const uint8_t* zero_slots_or_null,
-                             float* out, int B, int rows, int64_t C, int up, int down, int64_t delay, int64_t lead,
-                             sdr_stream stream) {
-    return launch_resample_stream_step(state, state_bytes, chunk, zero_slots_or_null, out, B, rows, C, up, down, delay,
-                                       lead, static_cast<cudaStream_t>(stream));
-}
-
-int sdr_resample_stream_flush(const void* state, size_t state_bytes, const float* tail_or_null, int64_t tail_len,
-                              const uint8_t* zero_slots_or_null, float* out, int B, int rows, int64_t C, int up,
-                              int down, int64_t delay, int64_t lead, sdr_stream stream) {
-    return launch_resample_stream_flush(state, state_bytes, tail_or_null, tail_len, zero_slots_or_null, out, B, rows,
-                                        C, up, down, delay, lead, static_cast<cudaStream_t>(stream));
-}
-
-int64_t sdr_window_count(int64_t T, int64_t W, int64_t H) { return window_count(T, W, H); }
-
-size_t sdr_window_carry_bytes(int B, int S, int A, int64_t W) { return window_carry_bytes(B, S, A, W); }
-
-size_t sdr_window_merge_scratch_bytes(int B, int S, int M) { return window_merge_scratch_bytes(B, S, M); }
-
-int sdr_window_gather(const float* mixture, float* batch, int B, int A, int64_t T, int64_t W, int64_t H, int64_t k0,
-                      int M, sdr_stream stream) {
-    return launch_window_gather(mixture, batch, B, A, T, W, H, k0, M, static_cast<cudaStream_t>(stream));
-}
-
-int sdr_window_merge(const float* estimates, void* carry, int32_t* perm_or_null, float* out, int B, int S, int A,
-                     int64_t T, int64_t W, int64_t H, int64_t k0, int M, void* scratch, sdr_stream stream) {
-    return launch_window_merge(estimates, carry, perm_or_null, out, B, S, A, T, W, H, k0, M, scratch,
-                               static_cast<cudaStream_t>(stream));
-}
-
-size_t sdr_window_stream_state_bytes(int B, int S, int A, int64_t W, int64_t H) {
-    return window_stream_state_bytes(B, S, A, W, H);
-}
-
-int sdr_window_stream_reset(void* state, int B, int S, int A, int64_t W, int64_t H, const int32_t* host_slots_or_null,
-                            int n, sdr_stream stream) {
-    return window_stream_reset(state, B, S, A, W, H, host_slots_or_null, n, static_cast<cudaStream_t>(stream));
-}
-
-int sdr_window_stream_reset_masked(void* state, int B, int S, int A, int64_t W, int64_t H, const uint8_t* mask,
-                                   sdr_stream stream) {
-    return window_stream_reset_masked(state, B, S, A, W, H, mask, static_cast<cudaStream_t>(stream));
-}
-
-int sdr_window_stream_gather(void* state, const float* chunk_or_null, float* batch, int B, int S, int A, int64_t C,
-                             int64_t W, int64_t H, sdr_stream stream) {
-    return launch_window_stream_gather(state, chunk_or_null, batch, B, S, A, C, W, H,
-                                       static_cast<cudaStream_t>(stream));
-}
-
-size_t sdr_window_stream_merge_scratch_bytes(int B, int S, int64_t C, int64_t H) {
-    return window_stream_merge_scratch_bytes(B, S, C, H);
-}
-
-int sdr_window_stream_merge(const float* estimates, void* state, float* out, int B, int S, int A, int64_t C,
-                            int64_t W, int64_t H, void* scratch, sdr_stream stream) {
-    return launch_window_stream_merge(estimates, state, out, B, S, A, C, W, H, scratch,
-                                      static_cast<cudaStream_t>(stream));
-}
-
-size_t sdr_window_stream_flush_scratch_bytes(int B, int S) { return window_stream_flush_scratch_bytes(B, S); }
-
-int sdr_window_stream_flush(const float* single, const float* estimates_or_null, const void* state, float* out, int B,
-                            int S, int A, int64_t W, int64_t H, void* scratch, sdr_stream stream) {
-    return launch_window_stream_flush(single, estimates_or_null, state, out, B, S, A, W, H, scratch,
-                                      static_cast<cudaStream_t>(stream));
-}
-
-int sdr_window_stream_launch_count(int B, int S, int A, int64_t C, int64_t W, int64_t H) {
-    return window_stream_launch_count(B, S, A, C, W, H);
 }
 
 }  // extern "C"

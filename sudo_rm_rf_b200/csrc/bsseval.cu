@@ -555,14 +555,6 @@ bss_final_kernel(const double* __restrict__ epart, const double* __restrict__ er
     }
 }
 
-size_t bss_eval_scratch_bytes(int B, int S, long long T, int F) {
-    if (B <= 0 || S < 1 || S > 4 || T <= 0 || F < 1 || F > kBssMaxF) return 0;
-    // S F delayed references in R^(T+F-1): more than the dimensions (T < (S-1) F + 1) makes the joint system singular
-    // by construction, where the recursion's rounding no longer separates dependent pivots from independent ones
-    if ((long long)S * F > T + F - 1) return 0;
-    return BssScratch(nullptr, B, S, T, F).bytes;
-}
-
 template <int S, int NE>
 static int bss_eval_launch(const float* ref, const float* est, const float* mix, double* sdr, double* sir,
                            double* sar, int* perm, double* msdr, double* msir, double* msar, int B, long long T, int F,
@@ -587,12 +579,14 @@ static int bss_eval_launch(const float* ref, const float* est, const float* mix,
                   msir, msar, B, compute_permutation);
 }
 
-int launch_bss_eval(const float* ref, const float* est, const float* mix, double* sdr, double* sir, double* sar,
+// sdr_bss_eval (mix null) and sdr_bss_eval_mixture
+static int bss_eval(const float* ref, const float* est, const float* mix, double* sdr, double* sir, double* sar,
                     int* perm, double* msdr, double* msir, double* msar, int B, int S, long long T, int F,
                     int compute_permutation, void* scratch, cudaStream_t st) {
-    if (!ref || !est || !sdr || !sir || !sar || !scratch) return SDR_ERR_BAD_ARGUMENT;
+    if (!ref || !est || !sdr || !sir || !sar || !scratch || reinterpret_cast<uintptr_t>(scratch) % 8)
+        return SDR_ERR_BAD_ARGUMENT;
     if (mix && (!msdr || !msir || !msar)) return SDR_ERR_BAD_ARGUMENT;
-    if (!bss_eval_scratch_bytes(B, S, T, F)) return B <= 0 || T <= 0 ? SDR_ERR_BAD_ARGUMENT : SDR_ERR_UNSUPPORTED;
+    if (!sdr_bss_eval_scratch_bytes(B, S, T, F)) return B <= 0 || T <= 0 ? SDR_ERR_BAD_ARGUMENT : SDR_ERR_UNSUPPORTED;
     return with_sources(S, [&](auto s) {
         constexpr int n = decltype(s)::value;
         return mix ? bss_eval_launch<n, n + 1>(ref, est, mix, sdr, sir, sar, perm, msdr, msir, msar, B, T, F,
@@ -603,3 +597,35 @@ int launch_bss_eval(const float* ref, const float* est, const float* mix, double
 }
 
 }  // namespace sdr
+
+using namespace sdr;
+
+#pragma GCC visibility push(default)
+extern "C" {
+
+size_t sdr_bss_eval_scratch_bytes(int B, int S, int64_t T, int F) {
+    if (B <= 0 || S < 1 || S > 4 || T <= 0 || F < 1 || F > kBssMaxF) return 0;
+    // S F delayed references in R^(T+F-1): more than the dimensions (T < (S-1) F + 1) makes the joint system singular
+    // by construction, where the recursion's rounding no longer separates dependent pivots from independent ones
+    if ((long long)S * F > T + F - 1) return 0;
+    return BssScratch(nullptr, B, S, T, F).bytes;
+}
+
+int sdr_bss_eval(const float* reference, const float* estimate, double* sdr, double* sir, double* sar,
+                 int32_t* perm_or_null, int B, int S, int64_t T, int F, int compute_permutation, void* scratch,
+                 sdr_stream stream) {
+    return bss_eval(reference, estimate, nullptr, sdr, sir, sar, perm_or_null, nullptr, nullptr, nullptr, B, S, T, F,
+                    compute_permutation, scratch, static_cast<cudaStream_t>(stream));
+}
+
+int sdr_bss_eval_mixture(const float* reference, const float* estimate, const float* mixture, double* sdr,
+                         double* sir, double* sar, int32_t* perm_or_null, double* mix_sdr, double* mix_sir,
+                         double* mix_sar, int B, int S, int64_t T, int F, int compute_permutation, void* scratch,
+                         sdr_stream stream) {
+    if (!mixture) return SDR_ERR_BAD_ARGUMENT;
+    return bss_eval(reference, estimate, mixture, sdr, sir, sar, perm_or_null, mix_sdr, mix_sir, mix_sar, B, S, T, F,
+                    compute_permutation, scratch, static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"
+#pragma GCC visibility pop

@@ -213,28 +213,6 @@ mc_apply_kernel(const float* __restrict__ est, const float* __restrict__ mix,
     }
 }
 
-int launch_mixture_consistency(const float* est, const float* mix, float* out, int B, int S,
-                               long long T, int weights_type, void* scratch, cudaStream_t st) {
-    if (B <= 0 || S <= 0 || T <= 0 || !est || !mix || !out) return SDR_ERR_BAD_ARGUMENT;
-    if ((long long)B * S > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;   // rows are indexed in int
-    double* power = nullptr;
-    if (weights_type == 1) {
-        if (!scratch) return SDR_ERR_BAD_ARGUMENT;
-        power = static_cast<double*>(scratch);
-        const int rows = B * S;
-        if (const int rc = cuda_status(cudaMemsetAsync(power, 0, sizeof(double) * rows, st))) return rc;
-        int gx = (int)((T + 256 * 8 - 1) / (256 * 8));
-        if (gx < 1) gx = 1;
-        if (const int rc = launch(mc_power_kernel, dim3((unsigned)gx, (unsigned)(rows < 65535 ? rows : 65535)), 256, 0,
-                                  st, est, power, rows, T))
-            return rc;
-    } else if (weights_type != 0) {
-        return SDR_ERR_BAD_ARGUMENT;
-    }
-    dim3 grid((unsigned)((T + 255) / 256), (unsigned)(B < 65535 ? B : 65535));
-    return launch(mc_apply_kernel, grid, 256, 0, st, est, mix, power, out, B, S, T);
-}
-
 // ---------------------------------------------------------------------------
 // backward of the projection.  With r = mix - sum_s est_s and g = dL/dout:
 //   uniform: d est_k = g_k - (1/S) sum_s g_s,                  d mix = (1/S) sum_s g_s
@@ -244,10 +222,6 @@ int launch_mixture_consistency(const float* est, const float* mix, float* out, i
 // magsq: mc_bwd_partials_kernel writes (sum est_s^2, c_s) per (row, chunk) in fp64, mc_bwd_coef_kernel adds the
 // chunks in index order and forms (w_s, alpha_s).  No atomics, so a backward is bitwise reproducible.
 // ---------------------------------------------------------------------------
-size_t mc_backward_scratch_bytes(int B, int S, long long T, int weights_type) {
-    if (B <= 0 || S <= 0 || T <= 0 || weights_type != 1) return 0;
-    return sizeof(double) * 2 * (size_t)B * S * (gram_chunks(T) + 1);
-}
 
 // grid = rows * chunks (rows = B * S); part[row][chunk] = (sum est^2, <g, r>) over the chunk
 __global__ void __launch_bounds__(256)
@@ -337,10 +311,47 @@ mc_bwd_apply_kernel(const float* __restrict__ est, const float* __restrict__ g, 
     }
 }
 
-int launch_mixture_consistency_backward(const float* est, const float* mix, const float* grad_out, float* grad_est,
-                                        float* grad_mix, int B, int S, long long T, int weights_type, void* scratch,
-                                        cudaStream_t st) {
-    if (B <= 0 || S <= 0 || T <= 0 || !est || !grad_out || !grad_est) return SDR_ERR_BAD_ARGUMENT;
+}  // namespace sdr
+
+using namespace sdr;
+
+#pragma GCC visibility push(default)
+extern "C" {
+
+int sdr_mixture_consistency(const float* est, const float* mix, float* out, int B, int S, int64_t T,
+                            int weights_type, void* scratch, sdr_stream stream) {
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (B <= 0 || S <= 0 || T <= 0 || !est || !mix || !out) return SDR_ERR_BAD_ARGUMENT;
+    if ((long long)B * S > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;   // rows are indexed in int
+    double* power = nullptr;
+    if (weights_type == 1) {
+        if (!scratch) return SDR_ERR_BAD_ARGUMENT;
+        power = static_cast<double*>(scratch);
+        const int rows = B * S;
+        if (const int rc = cuda_status(cudaMemsetAsync(power, 0, sizeof(double) * rows, st))) return rc;
+        int gx = (int)((T + 256 * 8 - 1) / (256 * 8));
+        if (gx < 1) gx = 1;
+        if (const int rc = launch(mc_power_kernel, dim3((unsigned)gx, (unsigned)(rows < 65535 ? rows : 65535)), 256, 0,
+                                  st, est, power, rows, T))
+            return rc;
+    } else if (weights_type != 0) {
+        return SDR_ERR_BAD_ARGUMENT;
+    }
+    dim3 grid((unsigned)((T + 255) / 256), (unsigned)(B < 65535 ? B : 65535));
+    return launch(mc_apply_kernel, grid, 256, 0, st, est, mix, power, out, B, S, T);
+}
+
+size_t sdr_mixture_consistency_backward_scratch_bytes(int B, int S, int64_t T, int weights_type) {
+    if (B <= 0 || S <= 0 || T <= 0 || weights_type != 1) return 0;
+    return sizeof(double) * 2 * (size_t)B * S * (gram_chunks(T) + 1);
+}
+
+int sdr_mixture_consistency_backward(const float* est, const float* mix, const float* grad_out, float* grad_est,
+                                     float* grad_mix, int B, int S, int64_t T, int weights_type, void* scratch,
+                                     sdr_stream stream) {
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (B <= 0 || S <= 0 || T <= 0 || !est || !grad_out || !grad_est || reinterpret_cast<uintptr_t>(scratch) % 16)
+        return SDR_ERR_BAD_ARGUMENT;
     if (weights_type != 0 && weights_type != 1) return SDR_ERR_BAD_ARGUMENT;
     if ((long long)B * S > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
     double2* coef = nullptr;
@@ -363,4 +374,5 @@ int launch_mixture_consistency_backward(const float* est, const float* mix, cons
     return launch(mc_bwd_apply_kernel, grid, 256, 0, st, est, grad_out, coef, grad_est, grad_mix, B, S, T);
 }
 
-}  // namespace sdr
+}  // extern "C"
+#pragma GCC visibility pop

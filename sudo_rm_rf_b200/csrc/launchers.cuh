@@ -1,7 +1,10 @@
-// The host launchers and eligibility predicates that api.cu calls, by defining file.  api.cu and every file that
-// defines one of them include this header, so a definition that drifts from its declaration is a compile or link
-// error (the library is linked with undefined symbols refused) instead of a failure at load time.  Every launcher
+// The host launchers and eligibility predicates that api.cu's model code calls, by defining file.  api.cu and every
+// file that defines one of them include this header, so a definition that drifts from its declaration is a compile or
+// link error (the library is linked with undefined symbols refused) instead of a failure at load time.  Every launcher
 // enqueues its kernels through launch.cuh.
+// A C-ABI entry whose work no model code shares (mixture consistency, the metrics, resampling, windowed separation and
+// the pyramid stage entries) is defined in the file that implements it instead, inside that file's one extern "C"
+// block: there the public header's declaration makes a drifting definition a compile error the same way.
 #pragma once
 #include <initializer_list>
 #include "launch.cuh"
@@ -19,14 +22,9 @@ int launch_merge(const float* const* z, const NormIn* nins, int depth, float* m,
 bool pyramid_eligible(int D, int samples, int C, int L);
 size_t pyramid_rowstats_bytes(int samples, int C, int D);
 size_t pyramid_table_bytes(int samples, int C, int D);
-int launch_pyramid(const float* y, const NormIn& nin, const float* const* w5, const float* const* bias,
-                   const float* const* gamma, const float* const* beta, float* const* z, double* stats0,
-                   double* rowstats, float* table, int D, int samples, int C, int L, cudaStream_t st);
 int launch_pyramid_fused(const float* y, const NormIn& nin, const float* const* w5, const float* const* bias,
                          const float* const* gamma, const float* const* beta, float* m, double* stats0, double* stats_m,
                          double* rowstats, float* table, int D, int samples, int C, int L, cudaStream_t st);
-int launch_merge_pyramid(const float* const* z, const float* table, int D, float* m, double* stats_out,
-                         int samples, int C, int L, cudaStream_t st);
 
 // 1x1 convolutions, FFMA path (pointwise.cu)
 int launch_pointwise_ffma(const float* x, const NormIn& nin, const float* W, const float* bias,
@@ -38,18 +36,12 @@ int launch_pointwise_small_preadd(const float* x, const float* pre_add, const No
                                   const float* W, const float* bias, float* y, double* stats_out,
                                   int samples, int M, int K, int L, cudaStream_t st);
 
-// encoder, overlap-add and mixture consistency (frontback.cu)
+// encoder and overlap-add (frontback.cu)
 bool encoder_ffma_fits(int A, int K);
 int launch_encoder(const float* wav, const float* weight, const float* bias, int relu, float* enc, double* stats,
                    int B, int A, long long T, int N, int K, int L, int pad, cudaStream_t st);
 int launch_overlap_add(const float* frames, const float* mix, const float* bias, const float2* rescale, float* out,
                        int B, int SA, int K, int L, long long T, cudaStream_t st);
-int launch_mixture_consistency(const float* est, const float* mix, float* out, int B, int S,
-                               long long T, int weights_type, void* scratch, cudaStream_t st);
-size_t mc_backward_scratch_bytes(int B, int S, long long T, int weights_type);
-int launch_mixture_consistency_backward(const float* est, const float* mix, const float* grad_out, float* grad_est,
-                                        float* grad_mix, int B, int S, long long T, int weights_type, void* scratch,
-                                        cudaStream_t st);
 
 // transform-average-concatenate of the GroupComm blocks (tac.cu)
 int launch_tac(const float* x, const float* const* params, float* o, double* stats,
@@ -92,80 +84,8 @@ int launch_utterance_stats(const float* wav, double* sums, float2* mean_std, int
                            const long long* lengths, cudaStream_t st);
 int launch_normalize_rows(const float* wav, const float2* mean_std, float* out, int rows, long long T,
                           const long long* lengths, cudaStream_t st);
-int launch_pairwise_neg_sdr(const float* est, const float* tgt, float* out, int B, int S, long long T, int sdr_type,
-                            int zero_mean, int take_log, void* scratch, cudaStream_t st);
-size_t pairwise_train_scratch_bytes(int B, int S, long long T);
-size_t pairwise_coef_bytes(int B, int S);
-int launch_pairwise_neg_sdr_train(const float* est, const float* tgt, float* out, void* coef, int B, int S,
-                                  long long T, int sdr_type, int zero_mean, int take_log, void* scratch,
-                                  cudaStream_t st);
-int launch_pairwise_neg_sdr_backward(const float* est, const float* tgt, const void* coef, const float* grad_out,
-                                     float* grad, int B, int S, long long T, cudaStream_t st);
-size_t stabilized_sisdr_scratch_bytes(int B, int n_est, int n_act);
-int launch_stabilized_sisdr(const float* est, const float* tgt, float* best, int* perm, int B, int rows, int n_est,
-                            int n_act, long long T, int zero_mean, int improvement, double eps, void* scratch,
-                            cudaStream_t st);
-size_t pit_sisdr_scratch_bytes(int B, int S);
-int launch_pit_sisdr(const float* est, const float* tgt, const float* mix, float* best, int* perm,
-                     int B, int S, long long T, int zero_mean, int improvement, double eps,
-                     void* scratch, cudaStream_t st);
-size_t snr_zero_refs_scratch_bytes(int B, int S, long long T);
-size_t snr_zero_refs_coef_bytes(int B, int S);
-int launch_snr_zero_refs(const float* est, const float* tgt, float* value, int* perm, void* coef, int B, int S,
-                         long long T, int zero_mean, double threshold, double eps, void* scratch, cudaStream_t st);
-int launch_snr_zero_refs_backward(const float* est, const float* tgt, const void* coef, const float* grad_value,
-                                  float* grad, int B, int S, long long T, long long Tg, cudaStream_t st);
-
-size_t bss_eval_scratch_bytes(int B, int S, long long T, int F);
-int launch_bss_eval(const float* ref, const float* est, const float* mix, double* sdr, double* sir, double* sar,
-                    int* perm, double* msdr, double* msir, double* msar, int B, int S, long long T, int F,
-                    int compute_permutation, void* scratch, cudaStream_t st);
-
-// STOI (stoi.cu)
-size_t stoi_scratch_bytes(int B, int S, long long T, int fs);
-int launch_stoi(const float* ref, const float* est, const float* mix, const long long* lengths, double* out,
-                double* mout, int B, int S, long long T, int fs, void* scratch, cudaStream_t st);
-
-// polyphase resampling (resample.cu)
-size_t resample_poly_scratch_bytes(int up, int down);
-int launch_resample_poly(const float* x, float* out, long long rows, long long T, int up, int down, void* scratch,
-                         size_t scratch_bytes, cudaStream_t st);
-size_t resample_stream_state_bytes(int B, int rows, long long C, int up, int down, long long delay, long long lead);
-long long resample_stream_flush_length(int p, int q, long long delay, long long lead, long long tail_len);
-int resample_stream_reset(void* state, size_t state_bytes, int B, int rows, long long C, int up, int down, long long delay,
-                          long long lead, const int* slots, int n, cudaStream_t st);
-int launch_resample_stream_step(void* state, size_t state_bytes, const float* chunk, const unsigned char* zero,
-                                float* out, int B, int rows, long long C, int up, int down, long long delay,
-                                long long lead, cudaStream_t st);
-int launch_resample_stream_flush(const void* state, size_t state_bytes, const float* tail, long long tail_len,
-                                 const unsigned char* zero, float* out, int B, int rows, long long C, int up,
-                                 int down, long long delay, long long lead, cudaStream_t st);
-
-// windowed separation (windowed.cu)
-long long window_count(long long T, long long W, long long H);
-size_t window_carry_bytes(int B, int S, int A, long long W);
-size_t window_merge_scratch_bytes(int B, int S, int M);
-int launch_window_gather(const float* x, float* batch, int B, int A, long long T, long long W, long long H,
-                         long long k0, int M, cudaStream_t st);
-int launch_window_merge(const float* est, void* carry, int* perm, float* out, int B, int S, int A, long long T,
-                        long long W, long long H, long long k0, int M, void* scratch, cudaStream_t st);
-size_t window_stream_state_bytes(int B, int S, int A, long long W, long long H);
-int window_stream_reset(void* state, int B, int S, int A, long long W, long long H, const int* slots, int n,
-                        cudaStream_t st);
-int window_stream_reset_masked(void* state, int B, int S, int A, long long W, long long H, const unsigned char* mask,
-                               cudaStream_t st);
-int launch_window_stream_gather(void* state, const float* chunk, float* batch, int B, int S, int A, long long C,
-                                long long W, long long H, cudaStream_t st);
-size_t window_stream_merge_scratch_bytes(int B, int S, long long C, long long H);
-int launch_window_stream_merge(const float* est, void* state, float* out, int B, int S, int A, long long C,
-                               long long W, long long H, void* scratch, cudaStream_t st);
-size_t window_stream_flush_scratch_bytes(int B, int S);
-int launch_window_stream_flush(const float* single, const float* est, const void* state, float* out, int B, int S,
-                               int A, long long W, long long H, void* scratch, cudaStream_t st);
-int window_stream_launch_count(int B, int S, int A, long long C, long long W, long long H);
 
 // tensor-core path (pointwise_mma.cu)
-bool pointwise_mma_eligible(int M, int K);
 size_t pointwise_mma_packed_bytes(int M, int K);
 int pack_pointwise_mma(const float* W, int M, int K, void* packed, cudaStream_t st);
 int launch_pointwise_mma(const float* x, const NormIn& nin, const void* wpk, const float* bias,

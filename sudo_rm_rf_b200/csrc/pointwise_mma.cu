@@ -591,7 +591,7 @@ static inline int mma_pad_m(int M) { return (M + kTileN - 1) / kTileN * kTileN; 
 
 // Output-channel counts that are not a multiple of 128 are zero-padded (decoder: 2*21 = 42 rows);
 // the reduction dimension must fill whole 64-channel k-blocks.
-bool pointwise_mma_eligible(int M, int K) {
+static bool pointwise_mma_eligible(int M, int K) {
     return M >= 32 && K >= kBlockK && (K % kBlockK) == 0;
 }
 

@@ -296,25 +296,6 @@ pit_finalize_kernel(const double* __restrict__ acc, float* __restrict__ best, in
     if (improvement) subtract_batch_baseline(best, B, base_sum, (double)B * S);
 }
 
-size_t pit_sisdr_scratch_bytes(int B, int S) {
-    if (B <= 0 || S < 1 || S > 4) return 0;
-    const int V = 2 * S + 1;
-    return sizeof(double) * (size_t)B * (V + S * S + 3 * S + 1);
-}
-
-int launch_pit_sisdr(const float* est, const float* tgt, const float* mix, float* best, int* perm,
-                     int B, int S, long long T, int zero_mean, int improvement, double eps,
-                     void* scratch, cudaStream_t st) {
-    if (!est || !tgt || !best || !perm || !scratch || B <= 0 || T <= 0) return SDR_ERR_BAD_ARGUMENT;
-    if (improvement && !mix) return SDR_ERR_BAD_ARGUMENT;
-    double* acc = static_cast<double*>(scratch);
-    return with_sources(S, [&](auto s) {
-        constexpr int n = decltype(s)::value;
-        if (const int e = launch_gram<GramLayout<n, n, false, true>, false>(est, tgt, mix, n, B, T, acc, st)) return e;
-        return launch(pit_finalize_kernel<n>, 1, 256, 0, st, acc, best, perm, B, T, zero_mean, improvement, eps);
-    });
-}
-
 // ---------------------------------------------------------------------------
 // pairwise negative SNR / SI-SDR / SD-SDR (sisdr.py:372-457, PairwiseNegSDR): out[b, i, j] = -sdr(estimate i, target j).
 // With d = <e_i, t_j>, tt = <t_j, t_j>, ee = <e_i, e_i> (means removed when zero_mean) and c = d / (tt + 1e-8):
@@ -384,41 +365,6 @@ pairwise_finalize_kernel(const double* __restrict__ acc, int chunks, float* __re
     }
 }
 
-int launch_pairwise_neg_sdr(const float* est, const float* tgt, float* out, int B, int S, long long T, int sdr_type,
-                            int zero_mean, int take_log, void* scratch, cudaStream_t st) {
-    if (!est || !tgt || !out || !scratch || B <= 0 || T <= 0 || sdr_type < 0 || sdr_type > 2) return SDR_ERR_BAD_ARGUMENT;
-    double* acc = static_cast<double*>(scratch);
-    return with_sources(S, [&](auto s) {
-        constexpr int n = decltype(s)::value;
-        if (const int e = launch_gram<GramLayout<n, n, false, false>, false>(est, tgt, nullptr, n, B, T, acc, st))
-            return e;
-        return launch(pairwise_finalize_kernel<n, false>, item_blocks(B), 256, 0, st, acc, 1, out, nullptr, B, T,
-                      sdr_type, zero_mean, take_log);
-    });
-}
-
-size_t pairwise_train_scratch_bytes(int B, int S, long long T) { return snr_zero_refs_scratch_bytes(B, S, T); }
-
-size_t pairwise_coef_bytes(int B, int S) {
-    if (B <= 0 || S < 1 || S > 4) return 0;
-    return sizeof(double) * (size_t)B * (3 * S * S + 2 * S);
-}
-
-int launch_pairwise_neg_sdr_train(const float* est, const float* tgt, float* out, void* coef, int B, int S,
-                                  long long T, int sdr_type, int zero_mean, int take_log, void* scratch,
-                                  cudaStream_t st) {
-    if (!est || !tgt || !out || !coef || !scratch || B <= 0 || T <= 0 || sdr_type < 0 || sdr_type > 2)
-        return SDR_ERR_BAD_ARGUMENT;
-    double* part = static_cast<double*>(scratch);
-    return with_sources(S, [&](auto s) {
-        constexpr int n = decltype(s)::value;
-        if (const int e = launch_gram<GramLayout<n, n, true, false>, true>(est, tgt, nullptr, n, B, T, part, st))
-            return e;
-        return launch(pairwise_finalize_kernel<n, true>, item_blocks(B), 256, 0, st, part, gram_chunks(T), out,
-                      static_cast<double*>(coef), B, T, sdr_type, zero_mean, take_log);
-    });
-}
-
 // grid row_tiled_grid(B S, T); est, tgt and grad rows are T apart
 template <int S>
 __global__ void __launch_bounds__(256)
@@ -456,16 +402,6 @@ pairwise_backward_kernel(const float* __restrict__ est, const float* __restrict_
             gr[t] = (float)v;
         }
     }
-}
-
-int launch_pairwise_neg_sdr_backward(const float* est, const float* tgt, const void* coef, const float* grad_out,
-                                     float* grad, int B, int S, long long T, cudaStream_t st) {
-    if (!est || !tgt || !coef || !grad_out || !grad || B <= 0 || T <= 0) return SDR_ERR_BAD_ARGUMENT;
-    return with_sources(S, [&](auto s) {
-        constexpr int n = decltype(s)::value;
-        return launch(pairwise_backward_kernel<n>, row_tiled_grid((long long)B * n, T), 256, 0, st, est, tgt,
-                      static_cast<const double*>(coef), grad_out, grad, B, T);
-    });
 }
 
 // ---------------------------------------------------------------------------
@@ -522,34 +458,6 @@ stab_finalize_kernel(const double* __restrict__ acc, float* __restrict__ best, i
     if (improvement) subtract_batch_baseline(best, B, base_sum, (double)B * SA);
 }
 
-size_t stabilized_sisdr_scratch_bytes(int B, int n_est, int n_act) {
-    if (B <= 0 || n_est < 1 || n_est > 4 || n_act < 1 || n_act > n_est) return 0;
-    return sizeof(double) * (size_t)B * (n_est + n_act + n_est * n_act + n_est + n_act * n_act);
-}
-
-int launch_stabilized_sisdr(const float* est, const float* tgt, float* best, int* perm, int B, int rows, int n_est,
-                            int n_act, long long T, int zero_mean, int improvement, double eps, void* scratch,
-                            cudaStream_t st) {
-    if (!est || !tgt || !best || !perm || !scratch || B <= 0 || T <= 0 || rows < 1) return SDR_ERR_BAD_ARGUMENT;
-    if (rows != n_est && n_est != 1) return SDR_ERR_BAD_ARGUMENT;          // summing the rows is the single_source mode
-    if (!stabilized_sisdr_scratch_bytes(B, n_est, n_act)) return SDR_ERR_UNSUPPORTED;
-    double* acc = static_cast<double*>(scratch);
-    return with_sources(n_est, [&](auto se) {
-        return with_sources(n_act, [&](auto sa) -> int {
-            constexpr int E = decltype(se)::value, A = decltype(sa)::value;
-            if constexpr (A > E) {
-                return SDR_ERR_UNSUPPORTED;
-            } else {
-                if (const int e = launch_gram<GramLayout<E, A, true, false>, false>(est, tgt, nullptr, rows, B, T,
-                                                                                   acc, st))
-                    return e;
-                return launch(stab_finalize_kernel<E, A>, 1, 256, 0, st, acc, best, perm, B, T, zero_mean, improvement,
-                              eps);
-            }
-        });
-    });
-}
-
 // ---------------------------------------------------------------------------
 // PermInvariantSNRwithZeroRefs (dnn/losses/snr.py:13-142), the training loss of run_fuss_separation.py:257-259.
 // The ordered full Gram holds every term: with means removed under zero_mean,
@@ -561,16 +469,6 @@ int launch_stabilized_sisdr(const float* est, const float* tgt, float* best, int
 // i = p*[k]: dscore/d den * 2 = -20 a_k num_active / ln10 * nom_k / (den^2 (nom_k / den + eps)), the target k it
 // is matched to, and the row means of estimates and targets (zero under !zero_mean):  [coef S][k S][me S][mt S].
 // ---------------------------------------------------------------------------
-size_t snr_zero_refs_scratch_bytes(int B, int S, long long T) {
-    if (B <= 0 || S < 1 || S > 4 || T <= 0) return 0;
-    return sizeof(double) * (size_t)B * gram_chunks(T) * (2 * S + 2 * S * S + S);
-}
-
-size_t snr_zero_refs_coef_bytes(int B, int S) {
-    if (B <= 0 || S < 1 || S > 4) return 0;
-    return sizeof(double) * (size_t)B * 4 * S;
-}
-
 template <int S>
 __global__ void __launch_bounds__(256)
 snr_zero_refs_finalize_kernel(const double* __restrict__ part, int chunks, float* __restrict__ value,
@@ -631,19 +529,6 @@ snr_zero_refs_finalize_kernel(const double* __restrict__ part, int chunks, float
     }
 }
 
-int launch_snr_zero_refs(const float* est, const float* tgt, float* value, int* perm, void* coef, int B, int S,
-                         long long T, int zero_mean, double threshold, double eps, void* scratch, cudaStream_t st) {
-    if (!est || !tgt || !value || !perm || !coef || !scratch || B <= 0 || T <= 0) return SDR_ERR_BAD_ARGUMENT;
-    double* part = static_cast<double*>(scratch);
-    return with_sources(S, [&](auto s) {
-        constexpr int n = decltype(s)::value;
-        if (const int e = launch_gram<GramLayout<n, n, true, false>, true>(est, tgt, nullptr, n, B, T, part, st))
-            return e;
-        return launch(snr_zero_refs_finalize_kernel<n>, item_blocks(B), 256, 0, st, part, gram_chunks(T), value, perm,
-                      static_cast<double*>(coef), B, T, zero_mean, threshold, eps);
-    });
-}
-
 // grad[b][i][t] = g[b] coef_i ((e_i - me_i) - (t_k - mt_k)) for t < T, 0 for T <= t < Tg (rows Tg apart); est and tgt
 // rows are T apart.  grid row_tiled_grid(B S, Tg).
 __global__ void __launch_bounds__(256)
@@ -666,12 +551,153 @@ snr_zero_refs_backward_kernel(const float* __restrict__ est, const float* __rest
     }
 }
 
-int launch_snr_zero_refs_backward(const float* est, const float* tgt, const void* coef, const float* grad_value,
-                                  float* grad, int B, int S, long long T, long long Tg, cudaStream_t st) {
-    if (!est || !tgt || !coef || !grad_value || !grad || B <= 0 || T <= 0 || Tg < T) return SDR_ERR_BAD_ARGUMENT;
-    if (S < 1 || S > 4) return SDR_ERR_UNSUPPORTED;
-    return launch(snr_zero_refs_backward_kernel, row_tiled_grid((long long)B * S, Tg), 256, 0, st, est, tgt,
-                  static_cast<const double*>(coef), grad_value, grad, B, S, T, Tg);
+}  // namespace sdr
+
+using namespace sdr;
+
+#pragma GCC visibility push(default)
+extern "C" {
+
+size_t sdr_pit_sisdr_scratch_bytes(int B, int S) {
+    if (B <= 0 || S < 1 || S > 4) return 0;
+    const int V = 2 * S + 1;
+    return sizeof(double) * (size_t)B * (V + S * S + 3 * S + 1);
 }
 
-}  // namespace sdr
+int sdr_pit_sisdr(const float* est, const float* tgt, const float* mix, float* best, int32_t* perm, int B, int S,
+                  int64_t T, int zero_mean, int improvement, double eps, void* scratch, sdr_stream stream) {
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (!est || !tgt || !best || !perm || !scratch || reinterpret_cast<uintptr_t>(scratch) % 8 || B <= 0 || T <= 0)
+        return SDR_ERR_BAD_ARGUMENT;
+    if (improvement && !mix) return SDR_ERR_BAD_ARGUMENT;
+    double* acc = static_cast<double*>(scratch);
+    return with_sources(S, [&](auto s) {
+        constexpr int n = decltype(s)::value;
+        if (const int e = launch_gram<GramLayout<n, n, false, true>, false>(est, tgt, mix, n, B, T, acc, st)) return e;
+        return launch(pit_finalize_kernel<n>, 1, 256, 0, st, acc, best, perm, B, T, zero_mean, improvement, eps);
+    });
+}
+
+int sdr_pairwise_neg_sdr(const float* est, const float* tgt, float* out, int B, int S, int64_t T, int sdr_type,
+                         int zero_mean, int take_log, void* scratch, sdr_stream stream) {
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (!est || !tgt || !out || !scratch || reinterpret_cast<uintptr_t>(scratch) % 8 || B <= 0 || T <= 0 ||
+        sdr_type < 0 || sdr_type > 2)
+        return SDR_ERR_BAD_ARGUMENT;
+    double* acc = static_cast<double*>(scratch);
+    return with_sources(S, [&](auto s) {
+        constexpr int n = decltype(s)::value;
+        if (const int e = launch_gram<GramLayout<n, n, false, false>, false>(est, tgt, nullptr, n, B, T, acc, st))
+            return e;
+        return launch(pairwise_finalize_kernel<n, false>, item_blocks(B), 256, 0, st, acc, 1, out, nullptr, B, T,
+                      sdr_type, zero_mean, take_log);
+    });
+}
+
+size_t sdr_pairwise_neg_sdr_train_scratch_bytes(int B, int S, int64_t T) {
+    return sdr_snr_zero_refs_scratch_bytes(B, S, T);
+}
+
+size_t sdr_pairwise_neg_sdr_coef_bytes(int B, int S) {
+    if (B <= 0 || S < 1 || S > 4) return 0;
+    return sizeof(double) * (size_t)B * (3 * S * S + 2 * S);
+}
+
+int sdr_pairwise_neg_sdr_train(const float* est, const float* tgt, float* out, void* coef, int B, int S, int64_t T,
+                               int sdr_type, int zero_mean, int take_log, void* scratch, sdr_stream stream) {
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (!est || !tgt || !out || !coef || !scratch || reinterpret_cast<uintptr_t>(scratch) % 8 ||
+        reinterpret_cast<uintptr_t>(coef) % 8 || B <= 0 || T <= 0 || sdr_type < 0 || sdr_type > 2)
+        return SDR_ERR_BAD_ARGUMENT;
+    double* part = static_cast<double*>(scratch);
+    return with_sources(S, [&](auto s) {
+        constexpr int n = decltype(s)::value;
+        if (const int e = launch_gram<GramLayout<n, n, true, false>, true>(est, tgt, nullptr, n, B, T, part, st))
+            return e;
+        return launch(pairwise_finalize_kernel<n, true>, item_blocks(B), 256, 0, st, part, gram_chunks(T), out,
+                      static_cast<double*>(coef), B, T, sdr_type, zero_mean, take_log);
+    });
+}
+
+int sdr_pairwise_neg_sdr_backward(const float* est, const float* tgt, const void* coef, const float* grad_out,
+                                  float* grad, int B, int S, int64_t T, sdr_stream stream) {
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (!est || !tgt || !coef || reinterpret_cast<uintptr_t>(coef) % 8 || !grad_out || !grad || B <= 0 || T <= 0)
+        return SDR_ERR_BAD_ARGUMENT;
+    return with_sources(S, [&](auto s) {
+        constexpr int n = decltype(s)::value;
+        return launch(pairwise_backward_kernel<n>, row_tiled_grid((long long)B * n, T), 256, 0, st, est, tgt,
+                      static_cast<const double*>(coef), grad_out, grad, B, T);
+    });
+}
+
+size_t sdr_stabilized_sisdr_scratch_bytes(int B, int n_est, int n_act) {
+    if (B <= 0 || n_est < 1 || n_est > 4 || n_act < 1 || n_act > n_est) return 0;
+    return sizeof(double) * (size_t)B * (n_est + n_act + n_est * n_act + n_est + n_act * n_act);
+}
+
+int sdr_stabilized_sisdr(const float* est, const float* tgt, float* best, int32_t* perm, int B, int rows, int n_est,
+                         int n_act, int64_t T, int zero_mean, int improvement, double eps, void* scratch,
+                         sdr_stream stream) {
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (!est || !tgt || !best || !perm || !scratch || reinterpret_cast<uintptr_t>(scratch) % 8 || B <= 0 || T <= 0 ||
+        rows < 1)
+        return SDR_ERR_BAD_ARGUMENT;
+    if (rows != n_est && n_est != 1) return SDR_ERR_BAD_ARGUMENT;          // summing the rows is the single_source mode
+    if (!sdr_stabilized_sisdr_scratch_bytes(B, n_est, n_act)) return SDR_ERR_UNSUPPORTED;
+    double* acc = static_cast<double*>(scratch);
+    return with_sources(n_est, [&](auto se) {
+        return with_sources(n_act, [&](auto sa) -> int {
+            constexpr int E = decltype(se)::value, A = decltype(sa)::value;
+            if constexpr (A > E) {
+                return SDR_ERR_UNSUPPORTED;
+            } else {
+                if (const int e = launch_gram<GramLayout<E, A, true, false>, false>(est, tgt, nullptr, rows, B, T,
+                                                                                   acc, st))
+                    return e;
+                return launch(stab_finalize_kernel<E, A>, 1, 256, 0, st, acc, best, perm, B, T, zero_mean, improvement,
+                              eps);
+            }
+        });
+    });
+}
+
+size_t sdr_snr_zero_refs_scratch_bytes(int B, int S, int64_t T) {
+    if (B <= 0 || S < 1 || S > 4 || T <= 0) return 0;
+    return sizeof(double) * (size_t)B * gram_chunks(T) * (2 * S + 2 * S * S + S);
+}
+
+size_t sdr_snr_zero_refs_coef_bytes(int B, int S) {
+    if (B <= 0 || S < 1 || S > 4) return 0;
+    return sizeof(double) * (size_t)B * 4 * S;
+}
+
+int sdr_snr_zero_refs(const float* est, const float* tgt, float* value, int32_t* perm, void* coef, int B, int S,
+                      int64_t T, int zero_mean, double threshold, double eps, void* scratch, sdr_stream stream) {
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (!est || !tgt || !value || !perm || !coef || !scratch || reinterpret_cast<uintptr_t>(scratch) % 8 ||
+        reinterpret_cast<uintptr_t>(coef) % 8 || B <= 0 || T <= 0)
+        return SDR_ERR_BAD_ARGUMENT;
+    double* part = static_cast<double*>(scratch);
+    return with_sources(S, [&](auto s) {
+        constexpr int n = decltype(s)::value;
+        if (const int e = launch_gram<GramLayout<n, n, true, false>, true>(est, tgt, nullptr, n, B, T, part, st))
+            return e;
+        return launch(snr_zero_refs_finalize_kernel<n>, item_blocks(B), 256, 0, st, part, gram_chunks(T), value, perm,
+                      static_cast<double*>(coef), B, T, zero_mean, threshold, eps);
+    });
+}
+
+int sdr_snr_zero_refs_backward(const float* est, const float* tgt, const void* coef, const float* grad_value,
+                               float* grad, int B, int S, int64_t T, int64_t Tg, sdr_stream stream) {
+    if (!est || !tgt || !coef || reinterpret_cast<uintptr_t>(coef) % 8 || !grad_value || !grad || B <= 0 || T <= 0 ||
+        Tg < T)
+        return SDR_ERR_BAD_ARGUMENT;
+    if (S < 1 || S > 4) return SDR_ERR_UNSUPPORTED;
+    return launch(snr_zero_refs_backward_kernel, row_tiled_grid((long long)B * S, Tg), 256, 0,
+                  static_cast<cudaStream_t>(stream), est, tgt, static_cast<const double*>(coef), grad_value, grad, B,
+                  S, T, Tg);
+}
+
+}  // extern "C"
+#pragma GCC visibility pop

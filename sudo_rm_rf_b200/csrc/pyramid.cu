@@ -738,34 +738,6 @@ static int launch_pyramid_pass(K kern, const PyrArgs& a, int samples, cudaStream
     return launch(kern, (unsigned)grid, threads, smem, st, a);
 }
 
-// y [samples][C][L] -> z[0] = z_0, z[d] = R_d, table (merge coefficients).  stats0: zeroed slot for the statistics of z_0.
-int launch_pyramid(const float* y, const NormIn& nin, const float* const* w5, const float* const* bias,
-                   const float* const* gamma, const float* const* beta, float* const* z, double* stats0,
-                   double* rowstats, float* table, int D, int samples, int C, int L, cudaStream_t st) {
-    if (!z) return SDR_ERR_BAD_ARGUMENT;
-    PyrArgs a;
-    SolveArgs s;
-    int rc = pyramid_args(y, nin, w5, bias, gamma, beta, z, stats0, rowstats, table, D, samples, C, L, a, s);
-    if (rc != SDR_OK) return rc;
-    const int threads = 32 * pyramid_windows(D, L);
-    auto pass = [&](auto kern) -> int { return launch_pyramid_pass(kern, a, samples, st); };
-    if (nin.prelu && nin.prelu_pc) {
-        if (threads <= 256)
-            rc = D == 4 ? pass(dw_pyramid_kernel<4, 256, kPyrMinB, true>)
-                        : (D == 5 ? pass(dw_pyramid_kernel<5, 256, kPyrMinB, true>) : pass(dw_pyramid_kernel<6, 256, kPyrMinB, true>));
-        else
-            rc = D == 4 ? pass(dw_pyramid_kernel<4, 1024, 1, true>)
-                        : (D == 5 ? pass(dw_pyramid_kernel<5, 1024, 1, true>) : pass(dw_pyramid_kernel<6, 1024, 1, true>));
-    } else if (threads <= 256)      // rows up to 7-8 windows (L <= 3712 / 3328): compiled for several resident CTAs per SM
-        rc = D == 4 ? pass(dw_pyramid_kernel<4, 256, kPyrMinB, false>)
-                    : (D == 5 ? pass(dw_pyramid_kernel<5, 256, kPyrMinB, false>) : pass(dw_pyramid_kernel<6, 256, kPyrMinB, false>));
-    else
-        rc = D == 4 ? pass(dw_pyramid_kernel<4, 1024, 1, false>)
-                    : (D == 5 ? pass(dw_pyramid_kernel<5, 1024, 1, false>) : pass(dw_pyramid_kernel<6, 1024, 1, false>));
-    if (rc != SDR_OK) return rc;
-    return launch(pyramid_solve_kernel, (unsigned)samples, kSolveThreads, 0, st, s);
-}
-
 // One pass of the fused stage (M = kPyrStats or kPyrMerge), with the instantiation the row length and slope call for.
 template <int M>
 static int launch_fused_pass(const PyrArgs& a, bool pc, int samples, cudaStream_t st) {
@@ -806,12 +778,64 @@ int launch_pyramid_fused(const float* y, const NormIn& nin, const float* const* 
     return launch_fused_pass<kPyrMerge>(a, pc, samples, st);
 }
 
-int launch_merge_pyramid(const float* const* z, const float* table, int D, float* m, double* stats_out,
-                         int samples, int C, int L, cudaStream_t st) {
+// The stage entries' scratch: the row statistics, then the merge table at a 256-byte boundary.
+static size_t pyr_table_offset(int samples, int C, int D) {
+    return (pyramid_rowstats_bytes(samples, C, D) + 255) & ~(size_t)255;
+}
+
+}  // namespace sdr
+
+using namespace sdr;
+
+#pragma GCC visibility push(default)
+extern "C" {
+
+size_t sdr_pyramid_scratch_bytes(int samples, int C, int D, int L) {
+    if (samples <= 0 || !pyramid_eligible(D, samples, C, L)) return 0;
+    return pyr_table_offset(samples, C, D) + pyramid_table_bytes(samples, C, D);
+}
+
+// y [samples][C][L] -> z[0] = z_0, z[d] = R_d, table (merge coefficients).  stats0: zeroed slot for the statistics of z_0.
+int sdr_depthwise_pyramid(const float* y, const sdr_norm_in* fin, const float* const* w5, const float* const* bias,
+                          const float* const* gamma, const float* const* beta, float* const* z, double* stats0,
+                          void* scratch, int D, int samples, int C, int L, sdr_stream stream) {
+    if (!y || !w5 || !bias || !gamma || !beta || !z || !stats0 || !scratch) return SDR_ERR_BAD_ARGUMENT;
+    if (!pyramid_eligible(D, samples, C, L)) return SDR_ERR_UNSUPPORTED;
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const NormIn nin = make_norm(fin);
+    char* sc = static_cast<char*>(scratch);
+    PyrArgs a;
+    SolveArgs s;
+    int rc = pyramid_args(y, nin, w5, bias, gamma, beta, z, stats0, reinterpret_cast<double*>(sc),
+                          reinterpret_cast<float*>(sc + pyr_table_offset(samples, C, D)), D, samples, C, L, a, s);
+    if (rc != SDR_OK) return rc;
+    const int threads = 32 * pyramid_windows(D, L);
+    auto pass = [&](auto kern) -> int { return launch_pyramid_pass(kern, a, samples, st); };
+    if (nin.prelu && nin.prelu_pc) {
+        if (threads <= 256)
+            rc = D == 4 ? pass(dw_pyramid_kernel<4, 256, kPyrMinB, true>)
+                        : (D == 5 ? pass(dw_pyramid_kernel<5, 256, kPyrMinB, true>) : pass(dw_pyramid_kernel<6, 256, kPyrMinB, true>));
+        else
+            rc = D == 4 ? pass(dw_pyramid_kernel<4, 1024, 1, true>)
+                        : (D == 5 ? pass(dw_pyramid_kernel<5, 1024, 1, true>) : pass(dw_pyramid_kernel<6, 1024, 1, true>));
+    } else if (threads <= 256)      // rows up to 7-8 windows (L <= 3712 / 3328): compiled for several resident CTAs per SM
+        rc = D == 4 ? pass(dw_pyramid_kernel<4, 256, kPyrMinB, false>)
+                    : (D == 5 ? pass(dw_pyramid_kernel<5, 256, kPyrMinB, false>) : pass(dw_pyramid_kernel<6, 256, kPyrMinB, false>));
+    else
+        rc = D == 4 ? pass(dw_pyramid_kernel<4, 1024, 1, false>)
+                    : (D == 5 ? pass(dw_pyramid_kernel<5, 1024, 1, false>) : pass(dw_pyramid_kernel<6, 1024, 1, false>));
+    if (rc != SDR_OK) return rc;
+    return launch(pyramid_solve_kernel, (unsigned)samples, kSolveThreads, 0, st, s);
+}
+
+int sdr_merge_pyramid(const float* const* z, const void* scratch, int D, float* m, double* stats_out,
+                      int samples, int C, int L, sdr_stream stream) {
+    if (!z || !scratch || !m || !stats_out) return SDR_ERR_BAD_ARGUMENT;
     if (!pyramid_eligible(D, samples, C, L)) return SDR_ERR_UNSUPPORTED;
     MergePyrArgs a;
     memset(&a, 0, sizeof(a));
-    a.table = table; a.D = D; a.C = C; a.L = L;
+    a.table = reinterpret_cast<const float*>(static_cast<const char*>(scratch) + pyr_table_offset(samples, C, D));
+    a.D = D; a.C = C; a.L = L;
     uintptr_t al = reinterpret_cast<uintptr_t>(m);
     for (int d = 0; d < D; ++d) { a.z[d] = z[d]; al |= reinterpret_cast<uintptr_t>(z[d]); }
     if (al % 16 != 0) return SDR_ERR_UNSUPPORTED;
@@ -820,7 +844,20 @@ int launch_merge_pyramid(const float* const* z, const float* table, int D, float
     const int chunks = (int)((items + per_cta - 1) / per_cta);
     const long long grid = (long long)chunks * samples;
     if (grid > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-    return launch(merge_pyramid_kernel, (unsigned)grid, kMpThreads, 0, st, a, m, stats_out, chunks);
+    return launch(merge_pyramid_kernel, (unsigned)grid, kMpThreads, 0, static_cast<cudaStream_t>(stream), a, m,
+                  stats_out, chunks);
 }
 
-}  // namespace sdr
+int sdr_depthwise_pyramid_fused(const float* y, const sdr_norm_in* fin, const float* const* w5, const float* const* bias,
+                                const float* const* gamma, const float* const* beta, float* m, double* stats0,
+                                double* stats_m, void* scratch, int D, int samples, int C, int L, sdr_stream stream) {
+    if (!y || !w5 || !bias || !gamma || !beta || !m || !stats0 || !stats_m || !scratch) return SDR_ERR_BAD_ARGUMENT;
+    if (!pyramid_eligible(D, samples, C, L)) return SDR_ERR_UNSUPPORTED;
+    char* sc = static_cast<char*>(scratch);
+    return launch_pyramid_fused(y, make_norm(fin), w5, bias, gamma, beta, m, stats0, stats_m, reinterpret_cast<double*>(sc),
+                                reinterpret_cast<float*>(sc + pyr_table_offset(samples, C, D)), D, samples, C, L,
+                                static_cast<cudaStream_t>(stream));
+}
+
+}  // extern "C"
+#pragma GCC visibility pop

@@ -136,40 +136,6 @@ resample_poly_kernel(const float* __restrict__ x, float* __restrict__ out, const
     }
 }
 
-size_t resample_poly_scratch_bytes(int up, int down) {
-    const ResamplePlan g(up, down);
-    return g.ok ? g.scratch_bytes() : 0;
-}
-
-int launch_resample_poly(const float* x, float* out, long long rows, long long T, int up, int down, void* scratch,
-                         size_t scratch_bytes, cudaStream_t st) {
-    if (!x || !out || !scratch || reinterpret_cast<uintptr_t>(scratch) % 8) return SDR_ERR_BAD_ARGUMENT;
-    if (rows < 1 || T < 1 || T > kResampleMaxT || rows > (1LL << 62) / (T * 4096)) return SDR_ERR_BAD_ARGUMENT;
-    const ResamplePlan g(up, down);
-    if (!g.ok) return up < 1 || down < 1 ? SDR_ERR_BAD_ARGUMENT : SDR_ERR_UNSUPPORTED;
-    if (scratch_bytes < g.scratch_bytes()) return SDR_ERR_WORKSPACE;
-    if (g.p == g.q)
-        return cuda_status(cudaMemcpyAsync(out, x, (size_t)(rows * T) * sizeof(float), cudaMemcpyDeviceToDevice, st));
-    double* h = static_cast<double*>(scratch);
-    const int taps = 2 * g.L + 1;
-    int e;
-    if ((e = launch(resample_taps_kernel, (unsigned)((taps + 255) / 256), 256, 0, st, h, g.L, std::max(g.p, g.q))))
-        return e;
-    if ((e = launch(resample_normalise_kernel, 1, 1024, 0, st, h, g.L, g.p))) return e;
-    const long long n = resampled_length(T, g.p, g.q);
-    const bool smem_filter = taps <= kResampleSmemTaps;
-    const size_t smem = (kResampleChunk + (smem_filter ? taps : 0)) * sizeof(double);
-    auto kern = smem_filter ? resample_poly_kernel<true> : resample_poly_kernel<false>;
-    if ((e = allow_dynamic_smem(reinterpret_cast<const void*>(kern), smem))) return e;
-    int per_sm = 0;
-    if ((e = cuda_status(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kResampleThreads, smem))))
-        return e;
-    const long long work = rows * ((n + kResampleThreads - 1) / kResampleThreads);
-    const long long grid = std::min(work, (long long)std::max(per_sm, 1) * std::max(sm_count(), 1));
-    return launch(kern, (unsigned)grid, kResampleThreads, smem, st, x, out, h, rows, T, n, g.p, g.q, g.L);
-}
-
-
 // ---- streaming resampler (DESIGN.md section 7h) ------------------------------------------------------------------
 // Per slot, s = `lead` zeros then everything received since the reset, and r = resample_poly(s).  Step j (the slot's
 // counter) writes r[j P - delay + i], i < P = C p / q (zeros below 0), summed exactly as resample_poly_kernel sums
@@ -288,11 +254,6 @@ __global__ void resample_stream_advance_kernel(long long* __restrict__ count, in
     if (b < B) count[b] += 1;
 }
 
-size_t resample_stream_state_bytes(int B, int rows, long long C, int up, int down, long long delay, long long lead) {
-    const ResampleStreamPlan g(B, rows, C, up, down, delay, lead);
-    return g.err == SDR_OK ? g.bytes : 0;
-}
-
 // The refusals of every streaming entry in order: the plan's, a null state or !args_ok, a small state, a misaligned one.
 static int stream_refusal(const ResampleStreamPlan& g, const void* state, bool args_ok, size_t state_bytes) {
     if (g.err) return g.err;
@@ -301,25 +262,8 @@ static int stream_refusal(const ResampleStreamPlan& g, const void* state, bool a
     return reinterpret_cast<uintptr_t>(state) % 256 ? SDR_ERR_BAD_ARGUMENT : SDR_OK;
 }
 
-int resample_stream_reset(void* state, size_t state_bytes, int B, int rows, long long C, int up, int down, long long delay,
-                          long long lead, const int* slots, int n, cudaStream_t st) {
-    const ResampleStreamPlan g(B, rows, C, up, down, delay, lead);
-    if (const int e = stream_refusal(g, state, !(slots && n < 0), state_bytes)) return e;
-    char* base = static_cast<char*>(state);
-    long long* count = reinterpret_cast<long long*>(base + g.count_off);
-    float* hist = reinterpret_cast<float*>(base + g.hist_off);
-    if (!slots) {                                 // the whole state: the filter, the counters and both histories
-        double* h = reinterpret_cast<double*>(base);
-        int e;
-        if ((e = launch(resample_taps_kernel, (unsigned)((2 * g.L + 1 + 255) / 256), 256, 0, st, h, g.L,
-                        std::max(g.p, g.q))))
-            return e;
-        if ((e = launch(resample_normalise_kernel, 1, 1024, 0, st, h, g.L, g.p))) return e;
-        return cuda_status(cudaMemsetAsync(count, 0, g.bytes - g.count_off, st));
-    }
-    const size_t slot = (size_t)rows * g.Hs * sizeof(float);        // one slot's rows of one history buffer
-    return reset_slots({{count, sizeof(long long)}, {hist, slot}, {hist + (long long)B * rows * g.Hs, slot}}, B, slots,
-                       n, nullptr, st);
+static long long resample_stream_flush_length(int p, int q, long long delay, long long lead, long long tail_len) {
+    return resampled_length(lead + tail_len, p, q) + delay;
 }
 
 // A step (tail_len < 0: x is the chunk of C samples) or a flush (x is the tail of tail_len samples, maybe null when
@@ -355,26 +299,93 @@ static int resample_stream_run(const ResampleStreamPlan& g, void* state, const f
     return launch(resample_stream_advance_kernel, (unsigned)((B + 255) / 256), 256, 0, st, count, B);
 }
 
-long long resample_stream_flush_length(int p, int q, long long delay, long long lead, long long tail_len) {
-    return resampled_length(lead + tail_len, p, q) + delay;
+}  // namespace sdr
+
+using namespace sdr;
+
+#pragma GCC visibility push(default)
+extern "C" {
+
+size_t sdr_resample_poly_scratch_bytes(int up, int down) {
+    const ResamplePlan g(up, down);
+    return g.ok ? g.scratch_bytes() : 0;
 }
 
-int launch_resample_stream_step(void* state, size_t state_bytes, const float* chunk, const unsigned char* zero,
-                                float* out, int B, int rows, long long C, int up, int down, long long delay,
-                                long long lead, cudaStream_t st) {
+int sdr_resample_poly(const float* x, float* out, int64_t rows, int64_t T, int up, int down, void* scratch,
+                      size_t scratch_bytes, sdr_stream stream) {
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (!x || !out || !scratch || reinterpret_cast<uintptr_t>(scratch) % 8) return SDR_ERR_BAD_ARGUMENT;
+    if (rows < 1 || T < 1 || T > kResampleMaxT || rows > (1LL << 62) / (T * 4096)) return SDR_ERR_BAD_ARGUMENT;
+    const ResamplePlan g(up, down);
+    if (!g.ok) return up < 1 || down < 1 ? SDR_ERR_BAD_ARGUMENT : SDR_ERR_UNSUPPORTED;
+    if (scratch_bytes < g.scratch_bytes()) return SDR_ERR_WORKSPACE;
+    if (g.p == g.q)
+        return cuda_status(cudaMemcpyAsync(out, x, (size_t)(rows * T) * sizeof(float), cudaMemcpyDeviceToDevice, st));
+    double* h = static_cast<double*>(scratch);
+    const int taps = 2 * g.L + 1;
+    int e;
+    if ((e = launch(resample_taps_kernel, (unsigned)((taps + 255) / 256), 256, 0, st, h, g.L, std::max(g.p, g.q))))
+        return e;
+    if ((e = launch(resample_normalise_kernel, 1, 1024, 0, st, h, g.L, g.p))) return e;
+    const long long n = resampled_length(T, g.p, g.q);
+    const bool smem_filter = taps <= kResampleSmemTaps;
+    const size_t smem = (kResampleChunk + (smem_filter ? taps : 0)) * sizeof(double);
+    auto kern = smem_filter ? resample_poly_kernel<true> : resample_poly_kernel<false>;
+    if ((e = allow_dynamic_smem(reinterpret_cast<const void*>(kern), smem))) return e;
+    int per_sm = 0;
+    if ((e = cuda_status(cudaOccupancyMaxActiveBlocksPerMultiprocessor(&per_sm, kern, kResampleThreads, smem))))
+        return e;
+    const long long work = rows * ((n + kResampleThreads - 1) / kResampleThreads);
+    const long long grid = std::min(work, (long long)std::max(per_sm, 1) * std::max(sm_count(), 1));
+    return launch(kern, (unsigned)grid, kResampleThreads, smem, st, x, out, h, rows, T, n, g.p, g.q, g.L);
+}
+
+size_t sdr_resample_stream_state_bytes(int B, int rows, int64_t C, int up, int down, int64_t delay, int64_t lead) {
+    const ResampleStreamPlan g(B, rows, C, up, down, delay, lead);
+    return g.err == SDR_OK ? g.bytes : 0;
+}
+
+int sdr_resample_stream_reset(void* state, size_t state_bytes, int B, int rows, int64_t C, int up, int down,
+                              int64_t delay, int64_t lead, const int32_t* slots, int n, sdr_stream stream) {
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    const ResampleStreamPlan g(B, rows, C, up, down, delay, lead);
+    if (const int e = stream_refusal(g, state, !(slots && n < 0), state_bytes)) return e;
+    char* base = static_cast<char*>(state);
+    long long* count = reinterpret_cast<long long*>(base + g.count_off);
+    float* hist = reinterpret_cast<float*>(base + g.hist_off);
+    if (!slots) {                                 // the whole state: the filter, the counters and both histories
+        double* h = reinterpret_cast<double*>(base);
+        int e;
+        if ((e = launch(resample_taps_kernel, (unsigned)((2 * g.L + 1 + 255) / 256), 256, 0, st, h, g.L,
+                        std::max(g.p, g.q))))
+            return e;
+        if ((e = launch(resample_normalise_kernel, 1, 1024, 0, st, h, g.L, g.p))) return e;
+        return cuda_status(cudaMemsetAsync(count, 0, g.bytes - g.count_off, st));
+    }
+    const size_t slot = (size_t)rows * g.Hs * sizeof(float);        // one slot's rows of one history buffer
+    return reset_slots({{count, sizeof(long long)}, {hist, slot}, {hist + (long long)B * rows * g.Hs, slot}}, B, slots,
+                       n, nullptr, st);
+}
+
+int sdr_resample_stream_step(void* state, size_t state_bytes, const float* chunk, const uint8_t* zero, float* out,
+                             int B, int rows, int64_t C, int up, int down, int64_t delay, int64_t lead,
+                             sdr_stream stream) {
     const ResampleStreamPlan g(B, rows, C, up, down, delay, lead);
     if (const int e = stream_refusal(g, state, chunk && out, state_bytes)) return e;
-    return resample_stream_run(g, state, chunk, -1, zero, out, B, rows, C, delay, lead, st);
+    return resample_stream_run(g, state, chunk, -1, zero, out, B, rows, C, delay, lead,
+                               static_cast<cudaStream_t>(stream));
 }
 
-int launch_resample_stream_flush(const void* state, size_t state_bytes, const float* tail, long long tail_len,
-                                 const unsigned char* zero, float* out, int B, int rows, long long C, int up,
-                                 int down, long long delay, long long lead, cudaStream_t st) {
+int sdr_resample_stream_flush(const void* state, size_t state_bytes, const float* tail, int64_t tail_len,
+                              const uint8_t* zero, float* out, int B, int rows, int64_t C, int up, int down,
+                              int64_t delay, int64_t lead, sdr_stream stream) {
     const ResampleStreamPlan g(B, rows, C, up, down, delay, lead);
     const bool args_ok = out && tail_len >= 0 && tail_len <= kResampleMaxT && (tail || tail_len == 0);
     if (const int e = stream_refusal(g, state, args_ok, state_bytes)) return e;
     // the state is only read: no history is written and the counters do not move
-    return resample_stream_run(g, const_cast<void*>(state), tail, tail_len, zero, out, B, rows, C, delay, lead, st);
+    return resample_stream_run(g, const_cast<void*>(state), tail, tail_len, zero, out, B, rows, C, delay, lead,
+                               static_cast<cudaStream_t>(stream));
 }
 
-}  // namespace sdr
+}  // extern "C"
+#pragma GCC visibility pop

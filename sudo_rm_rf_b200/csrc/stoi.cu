@@ -356,14 +356,24 @@ stoi_segment_kernel(const double* __restrict__ tob, const int* __restrict__ coun
     }
 }
 
-size_t stoi_scratch_bytes(int B, int S, long long T, int fs) {
+}  // namespace sdr
+
+using namespace sdr;
+
+#pragma GCC visibility push(default)
+extern "C" {
+
+size_t sdr_stoi_scratch_bytes(int B, int S, int64_t T, int fs) {
     const StoiPlan g(B, S, T, fs);
     return g.ok ? StoiScratch(nullptr, g, B, S).bytes : 0;
 }
 
-int launch_stoi(const float* ref, const float* est, const float* mix, const long long* lengths, double* out,
-                double* mout, int B, int S, long long T, int fs, void* scratch, cudaStream_t st) {
-    if (!ref || !est || !out || !scratch || (mix && !mout)) return SDR_ERR_BAD_ARGUMENT;
+int sdr_stoi(const float* ref, const float* est, const float* mix, const int64_t* lengths_or_null, double* out,
+             double* mout, int B, int S, int64_t T, int fs, void* scratch, sdr_stream stream) {
+    const long long* lengths = reinterpret_cast<const long long*>(lengths_or_null);
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (!ref || !est || !out || !scratch || reinterpret_cast<uintptr_t>(scratch) % 8 || (mix && !mout))
+        return SDR_ERR_BAD_ARGUMENT;
     const StoiPlan g(B, S, T, fs);
     if (!g.ok) return B <= 0 || S <= 0 || T <= 0 ? SDR_ERR_BAD_ARGUMENT : SDR_ERR_UNSUPPORTED;
     const StoiScratch s(scratch, g, B, S);
@@ -389,4 +399,5 @@ int launch_stoi(const float* ref, const float* est, const float* mix, const long
     return launch(stoi_segment_kernel, (unsigned)R, 256, 0, st, s.tob, s.count, s.flags, out, mout, R, g.M, clip1);
 }
 
-}  // namespace sdr
+}  // extern "C"
+#pragma GCC visibility pop

@@ -321,31 +321,6 @@ window_stream_history_kernel(const float* __restrict__ chunk, float* __restrict_
             hist[r * H + t] = chunk[r * C + C - H + t];
 }
 
-long long window_count(long long T, long long W, long long H) {
-    const WindowPlan g(T, W, H);
-    return g.ok ? g.K : 0;
-}
-
-size_t window_carry_bytes(int B, int S, int A, long long W) {
-    if (B <= 0 || S <= 0 || S > 4 || A <= 0 || W < 2 || W > kWinMaxW) return 0;
-    return WindowCarry(nullptr, B, S, A, W).bytes;
-}
-
-size_t window_merge_scratch_bytes(int B, int S, int M) {
-    if (B <= 0 || S <= 0 || S > 4 || M <= 0) return 0;
-    return WindowScratch(nullptr, B, S, M).bytes;
-}
-
-int launch_window_gather(const float* x, float* batch, int B, int A, long long T, long long W, long long H,
-                         long long k0, int M, cudaStream_t st) {
-    if (!x || !batch) return SDR_ERR_BAD_ARGUMENT;
-    const WindowPlan g(T, W, H);
-    if (!g.ok || B <= 0 || A <= 0 || M <= 0 || k0 < 0 || k0 + M > g.K) return SDR_ERR_BAD_ARGUMENT;
-    const long long rows = (long long)B * M * A;
-    return launch(window_gather_kernel, row_tiled_grid(rows, W), kWinThreads, 0, st, x, batch, rows, M, A, T, W, H,
-                  k0);
-}
-
 // Align, scan and overlap-add windows org.first(b) .. + M - 1 of every recording.  `single` non-null: a stream's flush,
 // which leaves the carry as it is.  Otherwise the carry receives the batch's last window and a stream's counters
 // (null for the offline merge) advance by `advance`.
@@ -371,20 +346,6 @@ static int merge_stages(const float* est, const WindowCarry& c, const float* sin
                   (long long)S * A, M, W, count, advance);
 }
 
-int launch_window_merge(const float* est, void* carry, int* perm, float* out, int B, int S, int A, long long T,
-                        long long W, long long H, long long k0, int M, void* scratch, cudaStream_t st) {
-    if (!est || !carry || !out || !scratch) return SDR_ERR_BAD_ARGUMENT;
-    if (reinterpret_cast<uintptr_t>(carry) % 256 || reinterpret_cast<uintptr_t>(scratch) % 8)
-        return SDR_ERR_BAD_ARGUMENT;
-    if (S > 4) return SDR_ERR_UNSUPPORTED;
-    const WindowPlan g(T, W, H);
-    if (!g.ok || B <= 0 || S <= 0 || A <= 0 || M <= 0 || k0 < 0 || k0 + M > g.K) return SDR_ERR_BAD_ARGUMENT;
-    const WindowCarry c(carry, B, S, A, W);
-    const long long t0 = k0 * H, t1 = k0 + M == g.K ? T : (k0 + M) * H;
-    return merge_stages(est, c, nullptr, perm, out, B, S, A, W, H, M, WinOrigin{nullptr, k0, T}, g.K, t1 - t0, T, t0,
-                        scratch, nullptr, 0, st);
-}
-
 // ---- windowed stream (DESIGN.md section 7f) ----------------------------------------------------------------------
 
 // SDR_OK, or the refusal of a bad shape (more than 4 sources: unsupported) or of a state off a 256-byte boundary.
@@ -392,11 +353,6 @@ static int stream_refusal(const void* state, int B, int S, int A, long long W, l
     if (!(B > 0 && S > 0 && S <= 4 && A > 0 && WindowPlan(W + 1, W, H).ok))
         return S > 4 ? SDR_ERR_UNSUPPORTED : SDR_ERR_BAD_ARGUMENT;
     return reinterpret_cast<uintptr_t>(state) % 256 ? SDR_ERR_BAD_ARGUMENT : SDR_OK;
-}
-
-size_t window_stream_state_bytes(int B, int S, int A, long long W, long long H) {
-    if (stream_refusal(nullptr, B, S, A, W, H)) return 0;
-    return WindowStreamState(nullptr, B, S, A, W, H).bytes;
 }
 
 // Zeroes the whole state (neither slots nor mask given) or each chosen slot's pi, carried estimate, history and
@@ -411,22 +367,74 @@ static int reset_stream(void* state, int B, int S, int A, long long W, long long
                        B, slots, n, mask, st);
 }
 
-int window_stream_reset(void* state, int B, int S, int A, long long W, long long H, const int* slots, int n,
-                        cudaStream_t st) {
-    if (!state || (slots && n < 0)) return SDR_ERR_BAD_ARGUMENT;
-    return reset_stream(state, B, S, A, W, H, slots, n, nullptr, st);
+}  // namespace sdr
+
+using namespace sdr;
+
+#pragma GCC visibility push(default)
+extern "C" {
+
+int64_t sdr_window_count(int64_t T, int64_t W, int64_t H) {
+    const WindowPlan g(T, W, H);
+    return g.ok ? g.K : 0;
 }
 
-// window_stream_reset of the slots whose mask[b] is set, the mask read on the device.
-int window_stream_reset_masked(void* state, int B, int S, int A, long long W, long long H, const unsigned char* mask,
-                               cudaStream_t st) {
+size_t sdr_window_carry_bytes(int B, int S, int A, int64_t W) {
+    if (B <= 0 || S <= 0 || S > 4 || A <= 0 || W < 2 || W > kWinMaxW) return 0;
+    return WindowCarry(nullptr, B, S, A, W).bytes;
+}
+
+size_t sdr_window_merge_scratch_bytes(int B, int S, int M) {
+    if (B <= 0 || S <= 0 || S > 4 || M <= 0) return 0;
+    return WindowScratch(nullptr, B, S, M).bytes;
+}
+
+int sdr_window_gather(const float* x, float* batch, int B, int A, int64_t T, int64_t W, int64_t H, int64_t k0, int M,
+                      sdr_stream stream) {
+    if (!x || !batch) return SDR_ERR_BAD_ARGUMENT;
+    const WindowPlan g(T, W, H);
+    if (!g.ok || B <= 0 || A <= 0 || M <= 0 || k0 < 0 || k0 + M > g.K) return SDR_ERR_BAD_ARGUMENT;
+    const long long rows = (long long)B * M * A;
+    return launch(window_gather_kernel, row_tiled_grid(rows, W), kWinThreads, 0, static_cast<cudaStream_t>(stream), x,
+                  batch, rows, M, A, T, W, H, k0);
+}
+
+int sdr_window_merge(const float* est, void* carry, int32_t* perm, float* out, int B, int S, int A, int64_t T,
+                     int64_t W, int64_t H, int64_t k0, int M, void* scratch, sdr_stream stream) {
+    if (!est || !carry || !out || !scratch) return SDR_ERR_BAD_ARGUMENT;
+    if (reinterpret_cast<uintptr_t>(carry) % 256 || reinterpret_cast<uintptr_t>(scratch) % 8)
+        return SDR_ERR_BAD_ARGUMENT;
+    if (S > 4) return SDR_ERR_UNSUPPORTED;
+    const WindowPlan g(T, W, H);
+    if (!g.ok || B <= 0 || S <= 0 || A <= 0 || M <= 0 || k0 < 0 || k0 + M > g.K) return SDR_ERR_BAD_ARGUMENT;
+    const WindowCarry c(carry, B, S, A, W);
+    const long long t0 = k0 * H, t1 = k0 + M == g.K ? T : (k0 + M) * H;
+    return merge_stages(est, c, nullptr, perm, out, B, S, A, W, H, M, WinOrigin{nullptr, k0, T}, g.K, t1 - t0, T, t0,
+                        scratch, nullptr, 0, static_cast<cudaStream_t>(stream));
+}
+
+size_t sdr_window_stream_state_bytes(int B, int S, int A, int64_t W, int64_t H) {
+    if (stream_refusal(nullptr, B, S, A, W, H)) return 0;
+    return WindowStreamState(nullptr, B, S, A, W, H).bytes;
+}
+
+int sdr_window_stream_reset(void* state, int B, int S, int A, int64_t W, int64_t H, const int32_t* slots, int n,
+                            sdr_stream stream) {
+    if (!state || (slots && n < 0)) return SDR_ERR_BAD_ARGUMENT;
+    return reset_stream(state, B, S, A, W, H, slots, n, nullptr, static_cast<cudaStream_t>(stream));
+}
+
+// sdr_window_stream_reset of the slots whose mask[b] is set, the mask read on the device.
+int sdr_window_stream_reset_masked(void* state, int B, int S, int A, int64_t W, int64_t H, const uint8_t* mask,
+                                   sdr_stream stream) {
     if (!state || !mask) return SDR_ERR_BAD_ARGUMENT;
-    return reset_stream(state, B, S, A, W, H, nullptr, 0, mask, st);
+    return reset_stream(state, B, S, A, W, H, nullptr, 0, mask, static_cast<cudaStream_t>(stream));
 }
 
 // C = 0 with chunk null: the flush's window [B][A][W]; nothing in the state changes.
-int launch_window_stream_gather(void* state, const float* chunk, float* batch, int B, int S, int A, long long C,
-                                long long W, long long H, cudaStream_t st) {
+int sdr_window_stream_gather(void* state, const float* chunk, float* batch, int B, int S, int A, int64_t C, int64_t W,
+                             int64_t H, sdr_stream stream) {
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
     if (!state || !batch || (!chunk && C != 0)) return SDR_ERR_BAD_ARGUMENT;
     if (const int e = stream_refusal(state, B, S, A, W, H)) return e;
     if (chunk && (C <= 0 || C % H)) return SDR_ERR_BAD_ARGUMENT;
@@ -440,40 +448,41 @@ int launch_window_stream_gather(void* state, const float* chunk, float* batch, i
                   ss.hist, (long long)B * A, C, H);
 }
 
-size_t window_stream_merge_scratch_bytes(int B, int S, long long C, long long H) {
+size_t sdr_window_stream_merge_scratch_bytes(int B, int S, int64_t C, int64_t H) {
     if (B <= 0 || S <= 0 || S > 4 || H <= 0 || C <= 0 || C % H || C / H > (1 << 30)) return 0;
     return WindowScratch(nullptr, B, S, (int)(C / H)).bytes;
 }
 
-int launch_window_stream_merge(const float* est, void* state, float* out, int B, int S, int A, long long C,
-                               long long W, long long H, void* scratch, cudaStream_t st) {
+int sdr_window_stream_merge(const float* est, void* state, float* out, int B, int S, int A, int64_t C, int64_t W,
+                            int64_t H, void* scratch, sdr_stream stream) {
     if (!est || !state || !out || !scratch) return SDR_ERR_BAD_ARGUMENT;
     if (const int e = stream_refusal(state, B, S, A, W, H)) return e;
-    if (window_stream_merge_scratch_bytes(B, S, C, H) == 0 || reinterpret_cast<uintptr_t>(scratch) % 8)
+    if (sdr_window_stream_merge_scratch_bytes(B, S, C, H) == 0 || reinterpret_cast<uintptr_t>(scratch) % 8)
         return SDR_ERR_BAD_ARGUMENT;
     WindowStreamState ss(state, B, S, A, W, H);
     const int q = (int)(C / H);
     return merge_stages(est, ss.carry, nullptr, nullptr, out, B, S, A, W, H, q, WinOrigin{ss.count, -1, kWinUnbounded},
-                        kWinUnbounded, C, C, 0, scratch, ss.count, q, st);
+                        kWinUnbounded, C, C, 0, scratch, ss.count, q, static_cast<cudaStream_t>(stream));
 }
 
-size_t window_stream_flush_scratch_bytes(int B, int S) { return window_merge_scratch_bytes(B, S, 1); }
+size_t sdr_window_stream_flush_scratch_bytes(int B, int S) { return sdr_window_merge_scratch_bytes(B, S, 1); }
 
-int launch_window_stream_flush(const float* single, const float* est, const void* state, float* out, int B, int S,
-                               int A, long long W, long long H, void* scratch, cudaStream_t st) {
+int sdr_window_stream_flush(const float* single, const float* est, const void* state, float* out, int B, int S, int A,
+                            int64_t W, int64_t H, void* scratch, sdr_stream stream) {
     if (!single || !state || !out || !scratch || (!est && W < 2 * H)) return SDR_ERR_BAD_ARGUMENT;
     if (const int e = stream_refusal(state, B, S, A, W, H)) return e;
     if (reinterpret_cast<uintptr_t>(scratch) % 8) return SDR_ERR_BAD_ARGUMENT;
     // the state is only read: the carry's pi is not written when `single` is given
     WindowStreamState ss(const_cast<void*>(state), B, S, A, W, H);
     return merge_stages(est, ss.carry, single, nullptr, out, B, S, A, W, H, 1, WinOrigin{ss.count, -1, 0}, 0, H, H, 0,
-                        scratch, nullptr, 0, st);
+                        scratch, nullptr, 0, static_cast<cudaStream_t>(stream));
 }
 
-int window_stream_launch_count(int B, int S, int A, long long C, long long W, long long H) {
+int sdr_window_stream_launch_count(int B, int S, int A, int64_t C, int64_t W, int64_t H) {
     if (const int e = stream_refusal(nullptr, B, S, A, W, H)) return e;
-    if (window_stream_merge_scratch_bytes(B, S, C, H) == 0) return SDR_ERR_BAD_ARGUMENT;
+    if (sdr_window_stream_merge_scratch_bytes(B, S, C, H) == 0) return SDR_ERR_BAD_ARGUMENT;
     return 6;          // gather, history; align, scan, overlap-add, carry (the forward between them not counted)
 }
 
-}  // namespace sdr
+}  // extern "C"
+#pragma GCC visibility pop

@@ -46,7 +46,7 @@ def pyr_windows(D, L):
 
 
 def pyr_threads(D, L):
-    """Block size launch_pyramid picks: the <= 256-thread instantiation up to 8 windows, else the 1024-thread one."""
+    """sdr_depthwise_pyramid's block size: the <= 256-thread instantiation up to 8 windows, else 1024 threads."""
     return 256 if 32 * pyr_windows(D, L) <= 256 else 1024
 
 

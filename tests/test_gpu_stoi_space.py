@@ -27,7 +27,7 @@ MIN_MARGIN = 1e-6           # dB
 HOP = O.N_FRAME // 2
 WORST = {}                  # case group -> (largest |GPU - oracle|, where)
 
-# launch_stoi's grid limits (stoi.cu): resampling chunks of 256 samples in grid.x and rows in grid.y, at most 65535
+# sdr_stoi's grid limits (stoi.cu): resampling chunks of 256 samples in grid.x and rows in grid.y, at most 65535
 # each; spectra work items (a warp group of 4 spectral frames of one tob row) in at most 2^20 CTAs
 GRID_X = GRID_Y = 65535
 SPECTRA_CTAS = 1 << 20
@@ -46,7 +46,7 @@ def device_memory(request):
 
 
 def plan(B, S, T, fs, mix):
-    """launch_stoi's geometry: (Tn, M, resampling chunks, resampling rows, spectra work items)."""
+    """sdr_stoi's geometry: (Tn, M, resampling chunks, resampling rows, spectra work items)."""
     p, q = stoi_rates.ratio(fs)
     Tn = -(-T * p // q)
     F0 = -(-(Tn - O.N_FRAME) // HOP) if Tn > O.N_FRAME else 0
