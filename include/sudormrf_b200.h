@@ -560,6 +560,31 @@ int     sdr_window_gather(const float* mixture, float* batch, int B, int A, int6
 int     sdr_window_merge(const float* estimates, void* carry, int32_t* perm_or_null, float* out, int B, int S, int A,
                          int64_t T, int64_t W, int64_t H, int64_t k0, int M, void* scratch, sdr_stream stream);
 
+/* ---- a corpus of recordings of different lengths in shared window batches (DESIGN.md section 7i) ----
+ * R recordings, each longer than W, laid out back to back: recording r's mixture [A][T_r] starts at element A off_r of
+ * the flat mixture and its output [S A][T_r] at element S A off_r of the flat output.  desc (device memory, int64,
+ * 8-byte aligned) is [R][3]: (off_r, T_r, g_r), g_r = the sum of K_s = sdr_window_count(T_s, W, H) over s < r, the
+ * first global window of recording r.  Global window g = g_r + k is window k of recording r.  Batches are the global
+ * windows g0 .. g0+M-1, in increasing g0 without gaps, g0 + M at most the corpus's window count:
+ *   sdr_window_gather_ragged copies them into batch [M][A][W], zeros past each T_r;
+ *   the caller separates the batch into estimates [M][S A][W];
+ *   sdr_window_merge_ragged aligns and overlap-adds each window exactly as sdr_window_merge does for its recording
+ *   alone with B = 1 (pi restarts at the identity at every recording's window 0): window k < K_r - 1 writes samples
+ *   [k H, (k + 1) H) of its recording, the last one [k H, T_r).  perm_or_null [G][S] (G the corpus's window count)
+ *   receives pi of global window g in row g.
+ * carry (sdr_window_ragged_carry_bytes(S, A, W) = sdr_window_carry_bytes(1, S, A, W), 256-byte aligned) holds the
+ * batch's last window for the next batch, read only when that batch's first window is not its recording's window 0.
+ * Scratch: sdr_window_ragged_scratch_bytes(S, M), 8-byte aligned.  1 <= S <= 4 (else 0 / SDR_ERR_UNSUPPORTED).
+ * Given the same estimates, the output is bitwise independent of M and bitwise sdr_window_merge's on each recording
+ * alone. */
+size_t  sdr_window_ragged_carry_bytes(int S, int A, int64_t W);
+size_t  sdr_window_ragged_scratch_bytes(int S, int M);
+int     sdr_window_gather_ragged(const float* mixture, const int64_t* desc, int R, int A, int64_t W, int64_t H,
+                                 int64_t g0, int M, float* batch, sdr_stream stream);
+int     sdr_window_merge_ragged(const float* estimates, const int64_t* desc, int R, void* carry, int32_t* perm_or_null,
+                                float* out, int S, int A, int64_t W, int64_t H, int64_t g0, int M, void* scratch,
+                                sdr_stream stream);
+
 /* ---- windowed stream (DESIGN.md section 7f) --------------------------------
  * separate_long's windows, taken step by step for B independent slots.  With q = C / H (C a positive multiple of
  * H) and n = j C the samples a slot has received since its reset, a step's output [B][S A][C] is samples

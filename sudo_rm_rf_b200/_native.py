@@ -180,6 +180,12 @@ _SIGNATURES = {
                                     C.c_int64, C.c_int, C.c_void_p]),
     "sdr_window_merge": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                    C.c_int64, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
+    "sdr_window_ragged_carry_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int64]),
+    "sdr_window_ragged_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int]),
+    "sdr_window_gather_ragged": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_int64,
+                                           C.c_int, C.c_void_p, C.c_void_p]),
+    "sdr_window_merge_ragged": (C.c_int, [C.c_void_p, C.c_void_p, C.c_int, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int,
+                                          C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),
     "sdr_window_stream_state_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64]),
     "sdr_window_stream_reset": (C.c_int, [C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_void_p,
                                           C.c_int, C.c_void_p]),

@@ -44,6 +44,16 @@ class NativeSeparator(_engine.NativeModuleMixin):
                                                mixture_consistency=mixture_consistency, max_windows=max_windows),
             input_wav, sample_rate, model_rate)
 
+    def separate_long_corpus(self, wavs, window, hop=None, normalize=True, mixture_consistency=False,
+                             max_windows=32, return_permutations=False):
+        """``separate_long`` for a corpus of recordings of different lengths (a sequence of CUDA tensors [A, T_r] or
+        [T_r] on one device): their windows share batches of ``max_windows``, and recording r's [S A, T_r] result is
+        ``separate_long`` on it alone (see ``windowed.separate_long_corpus``).  Returns a list, and with
+        ``return_permutations`` also the list of each recording's [K_r, S] window orders (None for one window)."""
+        return windowed.separate_long_corpus(self, wavs, window, hop, normalize=normalize,
+                                             mixture_consistency=mixture_consistency, max_windows=max_windows,
+                                             return_permutations=return_permutations)
+
     def stream_windows(self, batch_size, chunk_samples, window, hop=None, normalize=True,
                        mixture_consistency=False, sample_rate=None, model_rate=None):
         """A ``window_stream.WindowedStream``: ``separate_long``'s windows taken step by step for ``batch_size``

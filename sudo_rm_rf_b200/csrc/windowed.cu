@@ -17,6 +17,11 @@
 // the counter c (c H samples received since the slot's reset):
 //   window_stream_gather_kernel   windows c-1 .. c+q-2 out of [history | chunk] into [B][q][A][W] (zeros below 0)
 //   window_stream_history_kernel  the chunk's last H samples become the history
+//
+// A corpus of recordings of different lengths (DESIGN.md section 7i) shares window batches: slot m of a batch holds
+// global window g0 + m, window k of the recording whose descriptor it finds (RaggedOrigin).  The align and scan
+// kernels take that origin in place of WinOrigin; window_gather_ragged_kernel and window_ola_ragged_kernel gather and
+// overlap-add per slot, the latter through the same window_value as window_ola_kernel.
 #include "assign.cuh"
 #include "launch.cuh"
 #include "launchers.cuh"
@@ -68,8 +73,14 @@ struct WindowStreamState {
     }
 };
 
+__host__ __device__ __forceinline__ long long win_count(long long T, long long W, long long H) {
+    return T <= W ? 1 : 1 + (T - W + H - 1) / H;
+}
+
 // Where a batch lies in each recording: windows k0 .. k0+M-1 of a recording of T samples.  The offline merge gives
 // every recording the same k0 and T.  A stream reads each slot's counter c: k0 = c + dk and T = c H + dT.
+// at(b, m, k, T): window m of recording b's batch is its window k, of a recording of T samples; false when the slot
+// holds no window (never, here).  perm_row: the row of perm [B][K][S] that window takes.
 struct WinOrigin {
     const long long* count;
     long long k0, T;
@@ -77,12 +88,49 @@ struct WinOrigin {
     __device__ __forceinline__ long long length(long long b, long long H) const {
         return count ? count[b] * H + T : T;
     }
+    __device__ __forceinline__ bool at(long long b, long long m, long long H, long long& k, long long& t) const {
+        k = first(b) + m;
+        t = length(b, H);
+        return true;
+    }
+    __device__ __forceinline__ long long perm_row(long long b, long long m, long long K) const {
+        return b * K + first(b) + m;
+    }
 };
 constexpr long long kWinUnbounded = 1LL << 62;   // a stream step's T: every window it merges overlaps in full
 
-__host__ __device__ __forceinline__ long long win_count(long long T, long long W, long long H) {
-    return T <= W ? 1 : 1 + (T - W + H - 1) / H;
-}
+// A corpus of recordings of different lengths (DESIGN.md section 7i): recording r's first sample per channel in the
+// flat buffers (its mixture [A][T] at A off, its output [S A][T] at S A off), its length T and its first global window
+// g, ascending in r.  The layout of the C-ABI's int64 descriptor [R][3].
+struct WinRec {
+    long long off, T, g;
+};
+
+// A ragged batch (B = 1): slot m holds global window g0 + m, window k = g0 + m - g of the last recording whose first
+// window g is at or below it.  A slot past the corpus's last window holds none.
+struct RaggedOrigin {
+    const WinRec* desc;
+    int R;
+    long long g0, W, H;
+    __device__ __forceinline__ bool slot(long long m, WinRec& d, long long& k) const {
+        const long long g = g0 + m;
+        int lo = 0, hi = R - 1;
+        while (lo < hi) {
+            const int mid = (lo + hi + 1) >> 1;
+            if (desc[mid].g <= g) lo = mid; else hi = mid - 1;
+        }
+        d = desc[lo];
+        k = g - d.g;
+        return k >= 0 && k < win_count(d.T, W, H);
+    }
+    __device__ __forceinline__ bool at(long long, long long m, long long, long long& k, long long& t) const {
+        WinRec d;
+        const bool ok = slot(m, d, k);
+        t = d.T;
+        return ok;
+    }
+    __device__ __forceinline__ long long perm_row(long long, long long m, long long) const { return g0 + m; }
+};
 
 // Merge scratch: rho [B][M][S], then pis [B][M+1][S] (pis[b][m] = pi of window k0+m-1), int32.
 struct WindowScratch {
@@ -130,18 +178,21 @@ __device__ __forceinline__ void block_sums(double (&v)[N], double* red) {
     __syncthreads();
 }
 
-// One CTA per (recording b, window k0 + m).  p = window k-1's rows at H .. H + O - 1, c = window k's rows at 0 .. O-1;
-// per channel a, the means over the overlap, then the centred cross products, summed over a in order.
-template <int S>
+// One CTA per (recording b, window k0 + m), or per slot m of a ragged batch.  p = window k-1's rows at H .. H + O - 1,
+// c = window k's rows at 0 .. O-1; per channel a, the means over the overlap, then the centred cross products, summed
+// over a in order.
+template <int S, class Org>
 __global__ void __launch_bounds__(kWinThreads)
 window_align_kernel(const float* __restrict__ est, const float* __restrict__ carry_est, int* __restrict__ rho, int B,
-                    int M, int A, long long W, long long H, WinOrigin org) {
+                    int M, int A, long long W, long long H, Org org) {
     __shared__ double red[kWinThreads / 32 * S * S];
     const long long bm = blockIdx.x;
-    const long long b = bm / M, m = bm % M, k = org.first(b) + m, T = org.length(b, H);
+    const long long b = bm / M, m = bm % M;
+    long long k, T;
+    const bool valid = org.at(b, m, H, k, T);
     int* out = rho + bm * S;
     // pi_0 is the identity; one source has nothing to search; a stream's window below 0 or past its last is never read
-    if (k <= 0 || k >= win_count(T, W, H) || S == 1) {
+    if (!valid || k <= 0 || k >= win_count(T, W, H) || S == 1) {
         if (threadIdx.x < S) out[threadIdx.x] = threadIdx.x;
         return;
     }
@@ -213,23 +264,29 @@ window_align_kernel(const float* __restrict__ est, const float* __restrict__ car
     for (int i = 0; i < S; ++i) out[i] = p[i];
 }
 
-// One thread per recording: pi_{k0-1} (the identity before window 0) composed with rho_k0 .. rho_{k0+M-1}.
-// carry_out (null: left as it is) receives the last; it may be carry_in.
+// One thread per recording (one for a ragged batch): pi_{k0-1} (the identity before window 0) composed with
+// rho_k0 .. rho_{k0+M-1}; the composition restarts from the identity at every recording's window 0.  carry_out
+// (null: left as it is) receives the last; it may be carry_in.
+template <class Org>
 __global__ void window_scan_kernel(const int* __restrict__ rho, int* __restrict__ pis, const int* carry_in,
-                                   int* carry_out, int* __restrict__ perm, int B, int S, int M, long long K,
-                                   WinOrigin org) {
+                                   int* carry_out, int* __restrict__ perm, int B, int S, int M, long long K, long long H,
+                                   Org org) {
     const long long b = blockIdx.x * (long long)blockDim.x + threadIdx.x;
     if (b >= B) return;
-    const long long k0 = org.first(b);
+    long long k, T;
+    bool valid = org.at(b, 0, H, k, T);
     int pi[4];
-    for (int s = 0; s < S; ++s) pi[s] = k0 <= 0 ? s : carry_in[b * S + s];
+    for (int s = 0; s < S; ++s) pi[s] = !valid || k <= 0 ? s : carry_in[b * S + s];
     for (int s = 0; s < S; ++s) pis[b * (M + 1) * S + s] = pi[s];
     for (int m = 0; m < M; ++m) {
+        valid = org.at(b, m, H, k, T);
+        if (!valid || k <= 0)
+            for (int s = 0; s < S; ++s) pi[s] = s;
         const int* r = rho + (b * M + m) * S;
         for (int s = 0; s < S; ++s) pi[s] = r[pi[s]];
         for (int s = 0; s < S; ++s) pis[(b * (M + 1) + m + 1) * S + s] = pi[s];
-        if (perm)
-            for (int s = 0; s < S; ++s) perm[(b * K + k0 + m) * S + s] = pi[s];
+        if (perm && valid)
+            for (int s = 0; s < S; ++s) perm[org.perm_row(b, m, K) * S + s] = pi[s];
     }
     if (carry_out)
         for (int s = 0; s < S; ++s) carry_out[b * S + s] = pi[s];
@@ -240,6 +297,17 @@ __global__ void window_scan_kernel(const int* __restrict__ rho, int* __restrict_
 __device__ __forceinline__ float window_fade(float prev, float cur, long long j, long long overlap) {
     const float r = __fdiv_rn((float)(j + 1), (float)(overlap + 1));
     return __fadd_rn(__fmul_rn(__fsub_rn(1.f, r), prev), __fmul_rn(r, cur));
+}
+
+// Sample j of window k's output source s, channel a: raw source pi_k(s) of `cur` and, inside overlap k (k > 0 and
+// j < W - H), its cross-fade with raw source pi_{k-1}(s) of `prev` at H + j.  cur, prev: estimates [S A][W].
+__device__ __forceinline__ float window_value(const float* cur, const float* prev, const int* pi_cur,
+                                              const int* pi_prev, long long s, long long a, long long A, long long j,
+                                              bool overlap, long long W, long long H) {
+    const float c = cur[((long long)pi_cur[s] * A + a) * W + j];
+    if (!overlap) return c;
+    const float p = prev[((long long)pi_prev[s] * A + a) * W + H + j];
+    return window_fade(p, c, j, W - H);
 }
 
 // Row r = (b, s, a) of the output over samples t = k0 H + u, 0 <= u < len: t takes window k = min(t / H, K - 1) (its
@@ -265,14 +333,9 @@ window_ola_kernel(const float* __restrict__ est, const float* __restrict__ carry
             if (single && k0 == 0 && T <= W) {
                 v = single[r * len + u];
             } else if (k >= 0) {
-                const long long crow = (long long)pb[(m + 1) * S + s] * A + a;
-                const float c = m < 0 ? car[crow * W + j] : raw[(m * SA + crow) * W + j];
-                v = c;
-                if (k > 0 && j < W - H) {
-                    const long long row = (long long)pb[m * S + s] * A + a;       // m >= 0 here
-                    const float p = m == 0 ? car[row * W + H + j] : raw[((m - 1) * SA + row) * W + H + j];
-                    v = window_fade(p, c, j, W - H);
-                }
+                // an overlap lies in window k0 or later: m >= 0 wherever `prev` is read
+                v = window_value(m < 0 ? car : raw + m * SA * W, m <= 0 ? car : raw + (m - 1) * SA * W,
+                                 pb + (m + 1) * S, pb + max(m, 0LL) * S, s, a, A, j, k > 0 && j < W - H, W, H);
             }
             out[r * ld + o0 + u] = v;
         }
@@ -330,12 +393,12 @@ static int merge_stages(const float* est, const WindowCarry& c, const float* sin
                         cudaStream_t st) {
     const WindowScratch s(scratch, B, S, M);
     int e = with_sources(S, [&](auto sc) {
-        return launch(window_align_kernel<decltype(sc)::value>, (unsigned)((long long)B * M), kWinThreads, 0, st, est,
-                      c.est, s.rho, B, M, A, W, H, org);
+        return launch(window_align_kernel<decltype(sc)::value, WinOrigin>, (unsigned)((long long)B * M), kWinThreads,
+                      0, st, est, c.est, s.rho, B, M, A, W, H, org);
     });
     if (e) return e;
-    if ((e = launch(window_scan_kernel, (unsigned)((B + 127) / 128), 128, 0, st, s.rho, s.pis, c.pi,
-                    single ? nullptr : c.pi, perm, B, S, M, K, org)))
+    if ((e = launch(window_scan_kernel<WinOrigin>, (unsigned)((B + 127) / 128), 128, 0, st, s.rho, s.pis, c.pi,
+                    single ? nullptr : c.pi, perm, B, S, M, K, H, org)))
         return e;
     const long long rows = (long long)B * S * A;
     if ((e = launch(window_ola_kernel, row_tiled_grid(rows, len), kWinThreads, 0, st, est, c.est, s.pis, single, out,
@@ -344,6 +407,49 @@ static int merge_stages(const float* est, const WindowCarry& c, const float* sin
     if (single) return SDR_OK;
     return launch(window_carry_kernel, row_tiled_grid(rows, W), kWinThreads, 0, st, est, c.est, rows,
                   (long long)S * A, M, W, count, advance);
+}
+
+// ---- a corpus of recordings in shared window batches (DESIGN.md section 7i) -------------------------------------
+
+// Row (m, a) of the batch [M][A][W]: window k of slot m's recording, zeros past its T and for a slot past the corpus.
+__global__ void __launch_bounds__(kWinThreads)
+window_gather_ragged_kernel(const float* __restrict__ x, float* __restrict__ batch, long long rows, int A, long long W,
+                            RaggedOrigin org) {
+    for (long long r = blockIdx.y; r < rows; r += gridDim.y) {       // r = m A + a
+        const long long a = r % A, m = r / A;
+        WinRec d;
+        long long k;
+        const bool valid = org.slot(m, d, k);
+        const long long start = k * org.H;
+        const float* src = x + (A * d.off + a * d.T);
+        float* dst = batch + r * W;
+        for (long long t = blockIdx.x * (long long)blockDim.x + threadIdx.x; t < W;
+             t += (long long)gridDim.x * blockDim.x)
+            dst[t] = valid && start + t < d.T ? src[start + t] : 0.f;
+    }
+}
+
+// Row (m, s, a) of a ragged batch: the samples slot m's window k finalises, [k H, (k + 1) H), or up to T in its
+// recording's last window, each as window_ola_kernel computes it; slot m - 1 (the carry for m = 0) is window k - 1
+// wherever k > 0.  Sample t of row s A + a of recording r goes to out[S A off + (s A + a) T + t].
+__global__ void __launch_bounds__(kWinThreads)
+window_ola_ragged_kernel(const float* __restrict__ est, const float* __restrict__ carry_est,
+                         const int* __restrict__ pis, float* __restrict__ out, long long rows, int S, int A,
+                         RaggedOrigin org) {
+    const long long SA = (long long)S * A, W = org.W, H = org.H;
+    for (long long r = blockIdx.y; r < rows; r += gridDim.y) {       // r = (m S + s) A + a
+        const long long a = r % A, s = (r / A) % S, m = r / SA;
+        WinRec d;
+        long long k;
+        if (!org.slot(m, d, k)) continue;
+        const long long len = k == win_count(d.T, W, H) - 1 ? d.T - k * H : H;
+        const float* cur = est + m * SA * W;
+        const float* prev = m == 0 ? carry_est : cur - SA * W;
+        float* dst = out + (SA * d.off + (s * A + a) * d.T + k * H);
+        for (long long u = blockIdx.x * (long long)blockDim.x + threadIdx.x; u < len;
+             u += (long long)gridDim.x * blockDim.x)
+            dst[u] = window_value(cur, prev, pis + (m + 1) * S, pis + m * S, s, a, A, u, k > 0 && u < W - H, W, H);
+    }
 }
 
 // ---- windowed stream (DESIGN.md section 7f) ----------------------------------------------------------------------
@@ -411,6 +517,49 @@ int sdr_window_merge(const float* est, void* carry, int32_t* perm, float* out, i
     const long long t0 = k0 * H, t1 = k0 + M == g.K ? T : (k0 + M) * H;
     return merge_stages(est, c, nullptr, perm, out, B, S, A, W, H, M, WinOrigin{nullptr, k0, T}, g.K, t1 - t0, T, t0,
                         scratch, nullptr, 0, static_cast<cudaStream_t>(stream));
+}
+
+size_t sdr_window_ragged_carry_bytes(int S, int A, int64_t W) { return sdr_window_carry_bytes(1, S, A, W); }
+
+size_t sdr_window_ragged_scratch_bytes(int S, int M) { return sdr_window_merge_scratch_bytes(1, S, M); }
+
+int sdr_window_gather_ragged(const float* x, const int64_t* desc, int R, int A, int64_t W, int64_t H, int64_t g0,
+                             int M, float* batch, sdr_stream stream) {
+    if (!x || !desc || !batch || reinterpret_cast<uintptr_t>(desc) % 8) return SDR_ERR_BAD_ARGUMENT;
+    if (!WindowPlan(W + 1, W, H).ok || R <= 0 || A <= 0 || M <= 0 || g0 < 0) return SDR_ERR_BAD_ARGUMENT;
+    const RaggedOrigin org{reinterpret_cast<const WinRec*>(desc), R, g0, W, H};
+    const long long rows = (long long)M * A;
+    return launch(window_gather_ragged_kernel, row_tiled_grid(rows, W), kWinThreads, 0,
+                  static_cast<cudaStream_t>(stream), x, batch, rows, A, W, org);
+}
+
+int sdr_window_merge_ragged(const float* est, const int64_t* desc, int R, void* carry, int32_t* perm, float* out,
+                            int S, int A, int64_t W, int64_t H, int64_t g0, int M, void* scratch, sdr_stream stream) {
+    const cudaStream_t st = static_cast<cudaStream_t>(stream);
+    if (!est || !desc || !carry || !out || !scratch) return SDR_ERR_BAD_ARGUMENT;
+    if (reinterpret_cast<uintptr_t>(carry) % 256 || reinterpret_cast<uintptr_t>(scratch) % 8 ||
+        reinterpret_cast<uintptr_t>(desc) % 8)
+        return SDR_ERR_BAD_ARGUMENT;
+    if (S > 4) return SDR_ERR_UNSUPPORTED;
+    if (!WindowPlan(W + 1, W, H).ok || R <= 0 || S <= 0 || A <= 0 || M <= 0 || g0 < 0) return SDR_ERR_BAD_ARGUMENT;
+    const RaggedOrigin org{reinterpret_cast<const WinRec*>(desc), R, g0, W, H};
+    const WindowCarry c(carry, 1, S, A, W);
+    const WindowScratch s(scratch, 1, S, M);
+    // the stages of merge_stages with B = 1, each slot's window and recording looked up in the descriptors
+    int e = with_sources(S, [&](auto sc) {
+        return launch(window_align_kernel<decltype(sc)::value, RaggedOrigin>, (unsigned)M, kWinThreads, 0, st, est,
+                      c.est, s.rho, 1, M, A, W, H, org);
+    });
+    if (e) return e;
+    if ((e = launch(window_scan_kernel<RaggedOrigin>, 1u, 128, 0, st, s.rho, s.pis, c.pi, c.pi, perm, 1, S, M, 0LL, H,
+                    org)))
+        return e;
+    const long long rows = (long long)M * S * A;
+    if ((e = launch(window_ola_ragged_kernel, row_tiled_grid(rows, W), kWinThreads, 0, st, est, c.est, s.pis, out,
+                    rows, S, A, org)))
+        return e;
+    return launch(window_carry_kernel, row_tiled_grid((long long)S * A, W), kWinThreads, 0, st, est, c.est,
+                  (long long)S * A, (long long)S * A, M, W, nullptr, 0LL);
 }
 
 size_t sdr_window_stream_state_bytes(int B, int S, int A, int64_t W, int64_t H) {

@@ -100,6 +100,11 @@ class GroupCommSudoRmRf(NativeSeparator, nn.Module):
         return super().separate_long(input_wav, window, hop, normalize, mixture_consistency, max_windows,
                                      sample_rate, model_rate)
 
+    def separate_long_corpus(self, wavs, window, hop=None, normalize=True, mixture_consistency=True, max_windows=32,
+                             return_permutations=False):
+        return super().separate_long_corpus(wavs, window, hop, normalize, mixture_consistency, max_windows,
+                                            return_permutations)
+
     def stream_windows(self, batch_size, chunk_samples, window, hop=None, normalize=True,
                        mixture_consistency=True, sample_rate=None, model_rate=None):
         return super().stream_windows(batch_size, chunk_samples, window, hop, normalize, mixture_consistency,
