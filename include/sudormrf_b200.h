@@ -90,6 +90,15 @@ const char* sdr_error_string(int code);
  * never reads (:264).                                                         */
 int     sdr_num_params(const sdr_config* cfg);
 int64_t sdr_param_numel(const sdr_config* cfg, int index);
+/* The state_dict key of parameter i, e.g. "sm.3.spp_dw.2.norm.gamma": the
+ * library names every entry it packs, with the same exception (the original
+ * model's ln_mask_in.{weight,bias} has no index).  Returns the key's length
+ * without the terminating NUL, and writes the key with its NUL when buf_bytes
+ * exceeds that length.  buf = NULL with buf_bytes = 0 is a size query.
+ * SDR_ERR_BAD_CONFIG for a bad config; SDR_ERR_BAD_ARGUMENT for an index
+ * outside [0, sdr_num_params) or a NULL buf with buf_bytes > 0;
+ * SDR_ERR_WORKSPACE, writing nothing, for a non-NULL buf that is too small.    */
+int64_t sdr_param_name(const sdr_config* cfg, int index, char* buf, size_t buf_bytes);
 
 /* Padded length rule of pad_to_appropriate_length (improved_sudormrf.py:303-310;
  * variant 3: sudormrf.py:206-209,283-293, multiples of lcm(hop, 2^depth)).     */

@@ -54,67 +54,30 @@ def make_config(model) -> N.SdrConfig:
         num_sources=int(model.num_sources), group_size=group)
 
 
+_names = {}     # cfg.key() -> state_dict_names(cfg)
+
+
 def state_dict_names(cfg: N.SdrConfig) -> List[str]:
-    """Parameter names in the reference's ``state_dict()`` order
-    (improved_sudormrf.py:247-281,170-196; groupcomm_sudormrf_v2.py:347-354,401-403)."""
-    if cfg.variant == 2:       # causal_improved_sudormrf_v3.py:146-189, block :71-96
-        names = ["encoder.weight", "bottleneck.weight", "bottleneck.bias"]
-        for i in range(cfg.num_blocks):
-            p = f"sm.{i}."
-            names += [p + "skipinit_gain", p + "proj_1x1.conv.weight", p + "proj_1x1.conv.bias", p + "proj_1x1.act.weight"]
-            for d in range(cfg.upsampling_depth):
-                names += [p + f"spp_dw.{d}.conv.weight", p + f"spp_dw.{d}.conv.bias", p + f"spp_dw.{d}.act.weight"]
-            names += [p + "res_conv.weight", p + "res_conv.bias"]
-        names += ["mask_net.0.weight", "mask_net.1.weight", "mask_net.1.bias", "decoder.weight", "mask_nl_class.weight"]
-        return names
-    if cfg.variant == 3:       # the original model, sudormrf.py:211-252 (block :134-162); ln_mask_in (:253) is never read
-        names = ["encoder.0.weight", "encoder.0.bias", "ln.weight", "ln.bias", "l1.weight", "l1.bias"]
-        for i in range(cfg.num_blocks):
-            p = f"sm.{i}."
-            names += [p + "proj_1x1.conv.weight", p + "proj_1x1.conv.bias", p + "proj_1x1.norm.weight",
-                      p + "proj_1x1.norm.bias", p + "proj_1x1.act.weight"]
-            for d in range(cfg.upsampling_depth):
-                names += [p + f"spp_dw.{d}.conv.weight", p + f"spp_dw.{d}.conv.bias",
-                          p + f"spp_dw.{d}.norm.weight", p + f"spp_dw.{d}.norm.bias"]
-            names += [p + "conv_1x1_exp.conv.weight", p + "conv_1x1_exp.conv.bias", p + "conv_1x1_exp.norm.weight",
-                      p + "conv_1x1_exp.norm.bias", p + "final_norm.norm.weight", p + "final_norm.norm.bias",
-                      p + "final_norm.act.weight", p + "module_act.norm.weight", p + "module_act.norm.bias",
-                      p + "module_act.act.weight"]
-        if cfg.out_channels != cfg.enc_num_basis:
-            names += ["reshape_before_masks.weight", "reshape_before_masks.bias"]
-        names += ["m.weight", "m.bias", "decoder.weight", "decoder.bias"]
-        return names
-    names = ["encoder.weight", "ln.gamma", "ln.beta", "bottleneck.weight", "bottleneck.bias"]
-
-    def ublock(p):
-        out = [p + "proj_1x1.conv.weight", p + "proj_1x1.conv.bias", p + "proj_1x1.norm.gamma",
-               p + "proj_1x1.norm.beta", p + "proj_1x1.act.weight"]
-        for d in range(cfg.upsampling_depth):
-            out += [p + f"spp_dw.{d}.conv.weight", p + f"spp_dw.{d}.conv.bias",
-                    p + f"spp_dw.{d}.norm.gamma", p + f"spp_dw.{d}.norm.beta"]
-        out += [p + "final_norm.norm.gamma", p + "final_norm.norm.beta",
-                p + "final_norm.act.weight", p + "res_conv.weight", p + "res_conv.bias"]
-        return out
-
-    for i in range(cfg.num_blocks):
-        if cfg.variant == 0:
-            names += ublock(f"sm.{i}.")
-        else:
-            t = f"sm.{i}.TAC."
-            names += [t + "TAC_input.0.weight", t + "TAC_input.0.bias", t + "TAC_input.1.weight",
-                      t + "TAC_mean.0.weight", t + "TAC_mean.0.bias", t + "TAC_mean.1.weight",
-                      t + "TAC_output.0.weight", t + "TAC_output.0.bias", t + "TAC_output.1.weight",
-                      t + "TAC_norm.gamma", t + "TAC_norm.beta"]
-            names += ublock(f"sm.{i}.UBlock.")
-    names += ["mask_net.0.weight", "mask_net.1.weight", "mask_net.1.bias", "decoder.weight"]
-    return names
+    """The state_dict keys the library packs, in its order (``sdr_param_name``): every entry of the reference's
+    ``state_dict()`` but the original model's unused ``ln_mask_in``."""
+    names = _names.get(cfg.key())
+    if names is None:
+        lib, buf, names = N.lib(), C.create_string_buffer(256), []
+        n = lib.sdr_num_params(C.byref(cfg))
+        if n < 0:
+            N.check(n, "sdr_num_params")
+        for i in range(n):
+            r = lib.sdr_param_name(C.byref(cfg), i, buf, len(buf))
+            if r < 0:
+                N.check(r, "sdr_param_name")
+            names.append(buf.value.decode())
+        names = _names[cfg.key()] = tuple(names)
+    return list(names)
 
 
 def _probe_names(model):
-    """First and last parameter of the model (device / requires_grad probes)."""
-    if getattr(model, "_b200_variant", None) == 3:
-        return ("encoder.0.weight", "decoder.weight")
-    return ("encoder.weight", "decoder.weight")
+    """The first parameter and the decoder's weight, which every variant has (device / requires_grad probes)."""
+    return (state_dict_names(make_config(model))[0], "decoder.weight")
 
 
 def _fetch(model, dotted: str) -> torch.Tensor:

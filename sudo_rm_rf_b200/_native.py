@@ -48,6 +48,7 @@ _SIGNATURES = {
     "sdr_error_string": (C.c_char_p, [C.c_int]),
     "sdr_num_params": (C.c_int, [C.POINTER(SdrConfig)]),
     "sdr_param_numel": (C.c_int64, [C.POINTER(SdrConfig), C.c_int]),
+    "sdr_param_name": (C.c_int64, [C.POINTER(SdrConfig), C.c_int, C.c_char_p, C.c_size_t]),
     "sdr_padded_length": (C.c_int64, [C.POINTER(SdrConfig), C.c_int64]),
     "sdr_packed_weight_bytes": (C.c_size_t, [C.POINTER(SdrConfig)]),
     "sdr_pack_weights": (C.c_int, [C.POINTER(SdrConfig), C.POINTER(C.c_void_p), C.c_int,

@@ -4,6 +4,7 @@
 // caller's stream.
 #include <algorithm>
 #include <vector>
+#include <cstdio>
 #include <cstring>
 #include <initializer_list>
 #include "common.cuh"
@@ -55,6 +56,10 @@ struct CausalBlockOff {
     Conv1x1 res_g;                // derived: gain * res_conv.{weight,bias}, the one the forward runs
 };
 
+// A state_dict entry: its offset in the packed buffer, its element count and its key, printf(blk, i) + printf(name, d)
+// + leaf, from string literals, the block i and the level d: nothing is formatted until sdr_param_name asks.
+struct Entry { size_t off, numel; const char *blk, *name, *leaf; int i, d; };
+
 struct Layout {
     bool ok = false;
     int A, N, Co, Ci, U, D, K, S, G, hop;
@@ -76,7 +81,7 @@ struct Layout {
     std::vector<UBlockOff> ub;
     std::vector<TacOff> tac;
     std::vector<Conv1x1> images;  // every 1x1 convolution with a tensor-core image, in reservation order
-    std::vector<size_t> off, numel;   // per state_dict entry
+    std::vector<Entry> entries;   // per state_dict entry, in state_dict order
     size_t total = 0;             // floats
 };
 
@@ -117,14 +122,17 @@ static Layout make_layout(const sdr_config* c) {
     if (l.orig && (l.N % 2)) return l;   // (N+1) x 1 mask conv with padding N - N/2 returns N rows only for an even N (sudormrf.py:239-242,289)
 
     size_t cur = 0, grad = 0;
+    const char* blk = ""; int bi = 0;     // key prefix of the entries being added ("sm.%d." ...) and its block index
     auto derived = [&](size_t n) { const size_t o = cur; cur += (n + 3) & ~(size_t)3; return Param{o}; };   // made by sdr_pack_weights
-    auto add = [&](size_t n) {                                                                               // state_dict entry
-        l.off.push_back(cur); l.numel.push_back(n);
+    auto add = [&](size_t n, const char* name, const char* leaf = "", int d = 0) {                          // state_dict entry
+        l.entries.push_back({cur, n, blk, name, leaf, bi, d});
         const Param p{derived(n).off, grad};
         grad += n;
         return p;
     };
-    auto conv = [&](int M, int K) { Conv1x1 c; c.M = M; c.K = K; c.w = add((size_t)M * K); c.b = add(M); return c; };
+    auto conv = [&](int M, int K, const char* name) {
+        Conv1x1 c; c.M = M; c.K = K; c.w = add((size_t)M * K, name, "weight"); c.b = add(M, name, "bias"); return c;
+    };
     auto begin_images = [&] { cur = (cur + 63) & ~(size_t)63; };   // 256 B alignment for the bulk-TMA images
     auto image = [&](Conv1x1& c) {
         const size_t b = pointwise_mma_packed_bytes(c.M, c.K);
@@ -133,73 +141,84 @@ static Layout make_layout(const sdr_config* c) {
         cur += b / sizeof(float);
         l.images.push_back(c);
     };
-    auto proj_and_levels = [&](NormBlockOff& u, size_t slopes) {   // proj_1x1 and spp_dw: cib channels
-        u.proj = conv(l.cib, l.cob);
-        u.proj_g = add(l.cib); u.proj_be = add(l.cib); u.proj_a = add(slopes);
+    // proj_1x1 and spp_dw: cib channels; norms' affine parameters `g`, `be` (GlobLN: gamma, beta; GroupNorm: weight, bias)
+    auto proj_and_levels = [&](NormBlockOff& u, size_t slopes, const char* g, const char* be) {
+        u.proj = conv(l.cib, l.cob, "proj_1x1.conv.");
+        u.proj_g = add(l.cib, "proj_1x1.norm.", g); u.proj_be = add(l.cib, "proj_1x1.norm.", be);
+        u.proj_a = add(slopes, "proj_1x1.act.weight");
         for (int d = 0; d < l.D; ++d) {
-            u.dw_w[d] = add((size_t)l.cib * 5); u.dw_b[d] = add(l.cib);
-            u.dw_g[d] = add(l.cib); u.dw_be[d] = add(l.cib);
+            u.dw_w[d] = add((size_t)l.cib * 5, "spp_dw.%d.conv.", "weight", d); u.dw_b[d] = add(l.cib, "spp_dw.%d.conv.", "bias", d);
+            u.dw_g[d] = add(l.cib, "spp_dw.%d.norm.", g, d); u.dw_be[d] = add(l.cib, "spp_dw.%d.norm.", be, d);
         }
     };
     const int SA = l.S * l.A;
     if (l.orig) {
         // state_dict order of the original SuDORMRF (sudormrf.py:211-252; block :134-162) without ln_mask_in (:253, unused)
-        l.enc_w = add((size_t)l.N * l.K); l.enc_b = add(l.N);
-        l.ln_g = add(l.N); l.ln_be = add(l.N);
-        l.bn = conv(l.Co, l.N);                                                    // l1
+        l.enc_w = add((size_t)l.N * l.K, "encoder.0.weight"); l.enc_b = add(l.N, "encoder.0.bias");
+        l.ln_g = add(l.N, "ln.weight"); l.ln_be = add(l.N, "ln.bias");
+        l.bn = conv(l.Co, l.N, "l1.");
         for (int i = 0; i < l.U; ++i) {
-            OrigBlockOff u;
-            proj_and_levels(u, l.Ci);
-            u.exp = conv(l.Co, l.Ci); u.exp_g = add(l.Co); u.exp_be = add(l.Co);
-            u.fn_g = add(l.Ci); u.fn_be = add(l.Ci); u.fn_a = add(l.Ci);
-            u.ma_g = add(l.Co); u.ma_be = add(l.Co); u.ma_a = add(l.Co);
+            OrigBlockOff u; blk = "sm.%d."; bi = i;
+            proj_and_levels(u, l.Ci, "weight", "bias");
+            u.exp = conv(l.Co, l.Ci, "conv_1x1_exp.conv.");
+            u.exp_g = add(l.Co, "conv_1x1_exp.norm.weight"); u.exp_be = add(l.Co, "conv_1x1_exp.norm.bias");
+            u.fn_g = add(l.Ci, "final_norm.norm.weight"); u.fn_be = add(l.Ci, "final_norm.norm.bias"); u.fn_a = add(l.Ci, "final_norm.act.weight");
+            u.ma_g = add(l.Co, "module_act.norm.weight"); u.ma_be = add(l.Co, "module_act.norm.bias"); u.ma_a = add(l.Co, "module_act.act.weight");
             l.ob.push_back(u);
         }
-        if (l.Co != l.N) l.rs = conv(l.N, l.Co);                                   // :233-236
-        l.m_w = add((size_t)l.S * (l.N + 1)); l.m_b = add(l.S);
-        l.dec_w = add((size_t)l.S * l.N * l.K); l.dec_b = add(l.S);
+        blk = "";
+        if (l.Co != l.N) l.rs = conv(l.N, l.Co, "reshape_before_masks.");        // :233-236
+        l.m_w = add((size_t)l.S * (l.N + 1), "m.weight"); l.m_b = add(l.S, "m.bias");
+        l.dec_w = add((size_t)l.S * l.N * l.K, "decoder.weight"); l.dec_b = add(l.S, "decoder.bias");
         l.mask.M = l.S * l.N; l.mask.K = l.N;
         l.mask.w = derived((size_t)l.mask.M * l.mask.K);
         l.mask.b = derived(l.mask.M);
     } else if (l.causal) {
         // state_dict order of CausalSuDORMRF (causal_improved_sudormrf_v3.py:146-189; block :71-96)
-        l.enc_w = add((size_t)l.N * l.A * (2 * l.K - 1));
-        l.bn = conv(l.Co, l.N);
+        l.enc_w = add((size_t)l.N * l.A * (2 * l.K - 1), "encoder.weight");
+        l.bn = conv(l.Co, l.N, "bottleneck.");
         for (int i = 0; i < l.U; ++i) {
-            CausalBlockOff u;
-            u.gain = add(1);
-            u.proj = conv(l.Ci, l.Co); u.proj_a = add(1);
-            for (int d = 0; d < l.D; ++d) { u.dw_w[d] = add((size_t)l.Ci * 21); u.dw_b[d] = add(l.Ci); u.dw_a[d] = add(1); }
-            u.res = conv(l.Co, l.Ci);
+            CausalBlockOff u; blk = "sm.%d."; bi = i;
+            u.gain = add(1, "skipinit_gain");
+            u.proj = conv(l.Ci, l.Co, "proj_1x1.conv."); u.proj_a = add(1, "proj_1x1.act.weight");
+            for (int d = 0; d < l.D; ++d) {
+                u.dw_w[d] = add((size_t)l.Ci * 21, "spp_dw.%d.conv.", "weight", d); u.dw_b[d] = add(l.Ci, "spp_dw.%d.conv.", "bias", d);
+                u.dw_a[d] = add(1, "spp_dw.%d.act.weight", "", d);
+            }
+            u.res = conv(l.Co, l.Ci, "res_conv.");
             l.cb.push_back(u);
         }
-        l.mask_a = add(1);
-        l.mask = conv(SA * l.N, l.Co);
-        l.dec_w = add((size_t)l.N * SA * SA * l.K);
-        l.mask_nl = add(1);
+        blk = "";
+        l.mask_a = add(1, "mask_net.0.weight");
+        l.mask = conv(SA * l.N, l.Co, "mask_net.1.");
+        l.dec_w = add((size_t)l.N * SA * SA * l.K, "decoder.weight");
+        l.mask_nl = add(1, "mask_nl_class.weight");
     } else {
-        l.enc_w = add((size_t)l.N * l.A * l.K);
-        l.ln_g = add(l.N); l.ln_be = add(l.N);
-        l.bn = conv(l.Co, l.N);
+        // state_dict order of SuDORMRF (improved_sudormrf.py:247-281,170-196) and GroupCommSudoRmRf (groupcomm_sudormrf_v2.py:347-354,401-403)
+        l.enc_w = add((size_t)l.N * l.A * l.K, "encoder.weight");
+        l.ln_g = add(l.N, "ln.gamma"); l.ln_be = add(l.N, "ln.beta");
+        l.bn = conv(l.Co, l.N, "bottleneck.");
         for (int i = 0; i < l.U; ++i) {
+            bi = i;
             if (l.gc) {
-                TacOff t;
+                TacOff t; blk = "sm.%d.TAC.";
                 const size_t n = l.cob, H = 3 * (size_t)l.cob;
-                t.p[0] = add(H * n); t.p[1] = add(H); t.p[2] = add(1);
-                t.p[3] = add(H * H); t.p[4] = add(H); t.p[5] = add(1);
-                t.p[6] = add(n * 2 * H); t.p[7] = add(n); t.p[8] = add(1);
-                t.g = add(n); t.be = add(n);
+                t.p[0] = add(H * n, "TAC_input.0.weight"); t.p[1] = add(H, "TAC_input.0.bias"); t.p[2] = add(1, "TAC_input.1.weight");
+                t.p[3] = add(H * H, "TAC_mean.0.weight"); t.p[4] = add(H, "TAC_mean.0.bias"); t.p[5] = add(1, "TAC_mean.1.weight");
+                t.p[6] = add(n * 2 * H, "TAC_output.0.weight"); t.p[7] = add(n, "TAC_output.0.bias"); t.p[8] = add(1, "TAC_output.1.weight");
+                t.g = add(n, "TAC_norm.gamma"); t.be = add(n, "TAC_norm.beta");
                 l.tac.push_back(t);
             }
-            UBlockOff u;
-            proj_and_levels(u, 1);
-            u.fn_g = add(l.cib); u.fn_be = add(l.cib); u.fn_a = add(1);
-            u.res = conv(l.cob, l.cib);
+            UBlockOff u; blk = l.gc ? "sm.%d.UBlock." : "sm.%d.";
+            proj_and_levels(u, 1, "gamma", "beta");
+            u.fn_g = add(l.cib, "final_norm.norm.gamma"); u.fn_be = add(l.cib, "final_norm.norm.beta"); u.fn_a = add(1, "final_norm.act.weight");
+            u.res = conv(l.cob, l.cib, "res_conv.");
             l.ub.push_back(u);
         }
-        l.mask_a = add(1);
-        l.mask = conv(SA * l.N, l.Co);
-        l.dec_w = add((size_t)l.N * SA * SA * l.K);
+        blk = "";
+        l.mask_a = add(1, "mask_net.0.weight");
+        l.mask = conv(SA * l.N, l.Co, "mask_net.1.");
+        l.dec_w = add((size_t)l.N * SA * SA * l.K, "decoder.weight");
     }
     l.dec.M = SA * l.K; l.dec.K = SA * l.N;
     l.dec.w = derived((size_t)l.dec.M * l.dec.K);
@@ -814,14 +833,28 @@ const char* sdr_error_string(int code) {
 
 int sdr_num_params(const sdr_config* cfg) {
     const Layout l = make_layout(cfg);
-    return l.ok ? (int)l.off.size() : SDR_ERR_BAD_CONFIG;
+    return l.ok ? (int)l.entries.size() : SDR_ERR_BAD_CONFIG;
 }
 
 int64_t sdr_param_numel(const sdr_config* cfg, int index) {
     const Layout l = make_layout(cfg);
     if (!l.ok) return SDR_ERR_BAD_CONFIG;
-    if (index < 0 || index >= (int)l.numel.size()) return SDR_ERR_BAD_ARGUMENT;
-    return (int64_t)l.numel[index];
+    if (index < 0 || index >= (int)l.entries.size()) return SDR_ERR_BAD_ARGUMENT;
+    return (int64_t)l.entries[index].numel;
+}
+
+int64_t sdr_param_name(const sdr_config* cfg, int index, char* buf, size_t buf_bytes) {
+    const Layout l = make_layout(cfg);
+    if (!l.ok) return SDR_ERR_BAD_CONFIG;
+    if (index < 0 || index >= (int)l.entries.size() || (!buf && buf_bytes)) return SDR_ERR_BAD_ARGUMENT;
+    const Entry& e = l.entries[index];
+    char name[96];              // the longest key, "sm.<int>.UBlock.spp_dw.<d>.norm.gamma", takes 41 bytes
+    int n = snprintf(name, sizeof(name), e.blk, e.i);
+    n += snprintf(name + n, sizeof(name) - n, e.name, e.d);
+    n += snprintf(name + n, sizeof(name) - n, "%s", e.leaf);
+    if (buf && buf_bytes <= (size_t)n) return SDR_ERR_WORKSPACE;
+    if (buf) memcpy(buf, name, (size_t)n + 1);
+    return n;
 }
 
 int64_t sdr_padded_length(const sdr_config* cfg, int64_t T) {
@@ -840,14 +873,14 @@ int sdr_pack_weights(const sdr_config* cfg, const float* const* params, int n_pa
                      void* packed, size_t packed_bytes, sdr_stream stream) {
     const Layout l = make_layout(cfg);
     if (!l.ok) return SDR_ERR_BAD_CONFIG;
-    if (!params || n_params != (int)l.off.size()) return SDR_ERR_BAD_ARGUMENT;
+    if (!params || n_params != (int)l.entries.size()) return SDR_ERR_BAD_ARGUMENT;
     SDR_TRY(check_buffers({{packed, 16, packed_bytes, l.total * sizeof(float)}}));
     cudaStream_t st = static_cast<cudaStream_t>(stream);
     float* pk = static_cast<float*>(packed);
     SDR_TRY(cuda_status(cudaMemsetAsync(pk, 0, l.total * sizeof(float), st)));
-    for (size_t i = 0; i < l.off.size(); ++i) {
+    for (size_t i = 0; i < l.entries.size(); ++i) {
         if (!params[i]) return SDR_ERR_BAD_ARGUMENT;
-        SDR_TRY(copy_d2d(pk + l.off[i], params[i], l.numel[i] * sizeof(float), st));
+        SDR_TRY(copy_d2d(pk + l.entries[i].off, params[i], l.entries[i].numel * sizeof(float), st));
     }
     // the derived regions, then the images (some are packed from a derived region): all in stream order
     if (l.orig) {

@@ -13,6 +13,17 @@ from sudo_rm_rf_b200 import _engine, _native
 from oracle import sudormrf_oracle as O
 
 REPO = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+CLASSES = {"improved": P.SuDORMRF, "groupcomm": P.GroupCommSudoRmRf, "causal": P.CausalSuDORMRF,
+           "original": P.OriginalSuDORMRF}
+
+
+def _param_name(lib, cfg, i):
+    """sdr_param_name of entry i: a size query, then the name into a buffer one byte longer."""
+    n = lib.sdr_param_name(C.byref(cfg), i, None, 0)
+    assert n > 0, n
+    buf = C.create_string_buffer(n + 1)
+    assert lib.sdr_param_name(C.byref(cfg), i, buf, n + 1) == n
+    return buf.value.decode()
 
 
 def test_header_symbols_are_exported():
@@ -49,9 +60,7 @@ def test_header_symbols_are_exported():
                       enc_kernel_size=11, enc_num_basis=32, num_sources=3)),      # out_channels == enc_num_basis: no reshape layer
 ])
 def test_layout_matches_state_dict(variant, kw):
-    cls = {"improved": P.SuDORMRF, "groupcomm": P.GroupCommSudoRmRf, "causal": P.CausalSuDORMRF,
-           "original": P.OriginalSuDORMRF}[variant]
-    m = cls(**kw)
+    m = CLASSES[variant](**kw)
     cfg_o = O.Config(variant=variant, **kw)
     sd = m.state_dict()
     shapes = O.param_shapes(cfg_o)
@@ -66,13 +75,76 @@ def test_layout_matches_state_dict(variant, kw):
     lib = _native.lib()
     assert lib.sdr_num_params(C.byref(cfg)) == len(sd)
     total = 0
-    for i, v in enumerate(sd.values()):
+    for i, (k, v) in enumerate(sd.items()):
+        assert _param_name(lib, cfg, i) == k
         assert lib.sdr_param_numel(C.byref(cfg), i) == v.numel()
         total += v.numel()
     assert lib.sdr_packed_weight_bytes(C.byref(cfg)) >= 4 * total
     for T in (1, 100, 160, 320, 321, 32000, 32079):
         assert lib.sdr_padded_length(C.byref(cfg), T) == O.padded_length(cfg_o, T)
     assert lib.sdr_workspace_bytes(C.byref(cfg), 2, 32000) > 0
+
+
+def _name_grid():
+    small = dict(out_channels=16, in_channels=32, enc_kernel_size=11, enc_num_basis=16, num_sources=2)
+    for U in (0, 1, 3):
+        for D in range(1, 9):          # 8: the deepest level the layout takes (test_param_name_refusals: 9 is refused)
+            kw = dict(small, num_blocks=U, upsampling_depth=D)
+            at = f"U{U}-D{D}"
+            yield pytest.param("improved", kw, id=f"improved-{at}")
+            yield pytest.param("causal", kw, id=f"causal-{at}")
+            for G in (2, 4):
+                yield pytest.param("groupcomm", dict(kw, group_size=G), id=f"groupcomm-{at}-G{G}")
+            for Co in (16, 8):         # out_channels == enc_num_basis: no reshape_before_masks
+                yield pytest.param("original", dict(kw, out_channels=Co), id=f"original-{at}-Co{Co}")
+    stereo = dict(small, num_blocks=2, upsampling_depth=3, in_audio_channels=2)
+    yield pytest.param("groupcomm", dict(stereo, group_size=4), id="groupcomm-stereo")
+    yield pytest.param("causal", stereo, id="causal-stereo")
+
+
+@pytest.mark.parametrize("variant,kw", list(_name_grid()))
+def test_param_names_are_the_state_dict_keys(variant, kw):
+    """The library names every entry it packs with the module's state_dict key, in the module's order."""
+    m = CLASSES[variant](**kw)
+    keys = list(m.state_dict().keys())
+    if variant == "original":          # not packed: see test_layout_matches_state_dict
+        assert keys[-2:] == ["ln_mask_in.weight", "ln_mask_in.bias"]
+        keys = keys[:-2]
+    cfg = _engine.make_config(m)
+    lib = _native.lib()
+    assert lib.sdr_num_params(C.byref(cfg)) == len(keys)
+    assert [_param_name(lib, cfg, i) for i in range(len(keys))] == keys
+
+
+def test_param_name_refusals():
+    """Each refusal of sdr_param_name returns its code and writes nothing; a fitting buffer gets the name and its NUL."""
+    lib = _native.lib()
+    cfg = _engine.make_config(P.GroupCommSudoRmRf(1, 16, 32, 2, 3, 11, 16, 2, 4))
+    deep = _engine.make_config(P.SuDORMRF(16, 32, 1, 9, 11, 16, 2))      # one level deeper than the layout takes
+    n = lib.sdr_num_params(C.byref(cfg))
+    name = b"decoder.weight"
+    L = len(name)
+    assert lib.sdr_num_params(C.byref(deep)) == -1 and _param_name(lib, cfg, n - 1) == name.decode()
+    size = 64
+    for what, c, i, has_buf, nbytes, want in [
+        ("bad config", deep, 0, True, size, -1),
+        ("bad config, size query", deep, 0, False, 0, -1),
+        ("bad config before a bad index", deep, -1, True, size, -1),
+        ("index -1", cfg, -1, True, size, -2),
+        ("index n", cfg, n, True, size, -2),
+        ("index n, size query", cfg, n, False, 0, -2),
+        ("NULL buffer with a size", cfg, n - 1, False, size, -2),
+        ("NULL buffer of one byte", cfg, 0, False, 1, -2),
+        ("buffer as long as the name", cfg, n - 1, True, L, -3),
+        ("buffer of zero bytes", cfg, n - 1, True, 0, -3),
+        ("size query", cfg, n - 1, False, 0, L),
+        ("buffer one byte longer than the name", cfg, n - 1, True, L + 1, L),
+    ]:
+        buf = C.create_string_buffer(b"\xa5" * size, size)
+        got = lib.sdr_param_name(C.byref(c), i, buf if has_buf else None, nbytes)
+        assert got == want, what
+        written = name + b"\0" if has_buf and want >= 0 else b""
+        assert buf.raw == written + b"\xa5" * (size - len(written)), what
 
 
 def test_published_parameter_counts():
