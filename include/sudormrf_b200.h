@@ -499,6 +499,32 @@ int sdr_bss_eval_framewise(const float* reference, const float* estimate, const 
                            int64_t T, int64_t W, int64_t H, int F, int compute_permutation, void* scratch,
                            sdr_stream stream);
 
+/* BSS-eval of source images (mir_eval.separation.bss_eval_images), the multichannel criteria: reference, estimate
+ * [B,S,C,T] (S images of C channel rows, each row contiguous in time) -> sdr, isr, sir, sar [B,S] fp64 in dB and perm
+ * [B,S].  Per item, in R^(T+F-1) per channel, P_j e_i projects each channel of e_i onto the F delays of all C channels
+ * of s_j and P_all e_i onto all S C F delayed reference channels; energies sum over channels:
+ *     SDR = 10 log10(|s_j|^2 / |e_i - s_j|^2),             ISR = 10 log10(|s_j|^2 / |P_j e_i - s_j|^2),
+ *     SIR = 10 log10(|P_j e_i|^2 / |P_all e_i - P_j e_i|^2),  SAR = 10 log10(|P_all e_i|^2 / |e_i - P_all e_i|^2)
+ * (a zero denominator: +inf).  compute_permutation and perm as sdr_bss_eval (the largest mean SIR).  For C = 1, SIR
+ * and SAR are sdr_bss_eval's.  An all-zero channel of a non-silent image is dropped from its systems (the projection
+ * onto the other channels); an item with an all-zero reference or estimate image, or one holding a NaN or an
+ * infinity, gets NaN in every output and perm -1.  1 <= S C <= 4, 1 <= F <= 512, T >= (S C - 1) F + 1; scratch:
+ * sdr_bss_eval_images_scratch_bytes(B, S, C, T, F) (0: unsupported arguments), 8-byte aligned.  perm_or_null may be
+ * NULL.  Bitwise reproducible; no call synchronises.
+ * sdr_bss_eval_images_framewise scores [B,S,C,T] in windows as sdr_bss_eval_framewise does (the same window count,
+ * fallback, lengths_or_null and NaN columns; at most 128 windows per scratch) -> sdr, isr, sir, sar, perm
+ * [B,nwin,S], each column exactly sdr_bss_eval_images of its window.  W >= (S C - 1) F + 1 (T when the fallback
+ * applies). */
+size_t sdr_bss_eval_images_scratch_bytes(int B, int S, int C, int64_t T, int F);
+int sdr_bss_eval_images(const float* reference, const float* estimate, double* sdr, double* isr, double* sir,
+                        double* sar, int32_t* perm_or_null, int B, int S, int C, int64_t T, int F,
+                        int compute_permutation, void* scratch, sdr_stream stream);
+size_t sdr_bss_eval_images_framewise_scratch_bytes(int B, int S, int C, int64_t T, int64_t W, int64_t H, int F);
+int sdr_bss_eval_images_framewise(const float* reference, const float* estimate, const int64_t* lengths_or_null,
+                                  double* sdr, double* isr, double* sir, double* sar, int32_t* perm_or_null, int B,
+                                  int S, int C, int64_t T, int64_t W, int64_t H, int F, int compute_permutation,
+                                  void* scratch, sdr_stream stream);
+
 /* STOI (pystoi 0.3.3's stoi(x, y, fs_sig, extended=False), the stoi of asteroid's get_metrics): reference and
  * estimate [B,S,T], mixture_or_null [B,T] -> stoi [B,S] fp64 (estimate j scored against reference j) and, with the
  * mixture, mix_stoi [B,S] (the mixture scored against every reference).  Rows are resampled from fs to 10 kHz as

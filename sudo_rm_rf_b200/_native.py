@@ -164,6 +164,16 @@ _SIGNATURES = {
     "sdr_bss_eval_framewise": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                          C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                                          C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_void_p, C.c_void_p]),
+    "sdr_bss_eval_images_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int]),
+    "sdr_bss_eval_images": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                      C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int, C.c_int, C.c_void_p,
+                                      C.c_void_p]),
+    "sdr_bss_eval_images_framewise_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64,
+                                                                 C.c_int64, C.c_int]),
+    "sdr_bss_eval_images_framewise": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                                C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
+                                                C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_void_p,
+                                                C.c_void_p]),
     "sdr_stoi_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int64, C.c_int]),
     "sdr_stoi": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                            C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),

@@ -17,6 +17,15 @@
 //   bss_final_kernel   the criteria, the permutation search (best_assignment on the mean SIR) and the outputs.
 // The correlation and energy kernels read their items through a BssItems view: a whole [S, T] item of a contiguous
 // batch (sdr_bss_eval) or one window of a recording, read in place (sdr_bss_eval_framewise).
+//
+// Source images (mir_eval.separation.bss_eval_images, sdr_bss_eval_images): source j is an image s_j of C channel rows
+// and so is estimate i, R = S C rows each.  P_j projects each channel of e_i onto the F delays of all C rows of s_j,
+// P_all onto all R F delayed rows, and energies sum over channels:
+//     SDR = 10 log10(|s_j|^2 / |e_i - s_j|^2),         ISR = 10 log10(|s_j|^2 / |P_j e_i - s_j|^2),
+//     SIR = 10 log10(|P_j e_i|^2 / |P_all e_i - P_j e_i|^2),  SAR = 10 log10(|P_all e_i|^2 / |e_i - P_all e_i|^2)
+// The same four kernels with the reference rows grouped by source (template parameter C): the joint system has R
+// blocks and source j's own system its C rows.  The sources are the instance C = 1 without the images' two extra
+// energies, and compute what they computed before images existed.
 #include "assign.cuh"
 #include "launchers.cuh"
 
@@ -53,43 +62,48 @@ __device__ __forceinline__ bool bss_is_projection(double p2, double r2, double e
     return fabs(p2 + r2 - e2) <= kBssProjectionDefect * e2;
 }
 
-// Estimate row e's energies (bss_energy_kernel's layout) come from projections: the joint one and every own one.
-template <int S>
-__device__ __forceinline__ bool bss_projections_hold(const double (&en)[3 * S + 3]) {
+// Energies per estimate row (bss_energy_kernel's layout): 3 S + 3, and 2 S more for source images
+__host__ __device__ constexpr int bss_energy_count(int S, bool images) { return 3 * S + 3 + (images ? 2 * S : 0); }
+
+// Estimate row e's energies come from projections: the joint one and every own one.
+template <int S, int NV>
+__device__ __forceinline__ bool bss_projections_hold(const double (&en)[NV]) {
     bool ok = bss_is_projection(en[3 * S], en[3 * S + 1], en[3 * S + 2]);
 #pragma unroll
     for (int j = 0; j < S; ++j) ok = ok && bss_is_projection(en[j], en[S + j], en[3 * S + 2]);
     return ok;
 }
 
-// Scratch carve-up, sized for S estimates plus the mixture whether or not it is given.  Doubles:
-//   part  [B][chunks][S][2S+1][F]   correlation partials (rows: S references, then the NE estimate rows)
-//   rj    [B][F][S][S]              the joint system's normalised blocks
-//   rt    [B][S][F]                 each reference's normalised autocorrelation
-//   eref  [B][S]                    reference energies
-//   cj    [B][S+1][S][F]            joint filters per estimate row
-//   ct    [B][S+1][S][F]            own-reference filters per estimate row
-//   epart [B][echunks][S+1][3S+3]   energy partials
+// Scratch carve-up for R = S C reference rows, sized for R estimate rows plus the mixture's whether or not it is
+// given, and NV energies per estimate row.  Doubles:
+//   part  [B][chunks][R][2R+1][F]   correlation partials (rows: R references, then the NE estimate rows)
+//   rj    [B][F][R][R]              the joint system's normalised blocks
+//   rt    [B][S][F][C][C]           each source's own normalised blocks
+//   eref  [B][R]                    reference row energies
+//   cj    [B][R+1][R][F]            joint filters per estimate row
+//   ct    [B][R+1][R][F]            own-source filters per estimate row
+//   epart [B][echunks][R+1][NV]     energy partials
 struct BssScratch {
     double *part, *rj, *rt, *eref, *cj, *ct, *epart;
     size_t bytes;
-    BssScratch(void* base, int B, int S, long long T, int F) {
-        const size_t b = (size_t)B, s = (size_t)S, f = (size_t)F, ne = s + 1;
+    BssScratch(void* base, int B, int S, int C, long long T, int F, int NV) {
+        const size_t b = (size_t)B, s = (size_t)S, c = (size_t)C, r = s * c, f = (size_t)F, ne = r + 1;
         size_t off = 0;
         double* p = static_cast<double*>(base);
-        auto take = [&](size_t n) { double* r = p ? p + off : nullptr; off += n; return r; };
-        part = take(b * bss_corr_chunks(T) * s * (s + ne) * f);
-        rj = take(b * f * s * s);
-        rt = take(b * s * f);
-        eref = take(b * s);
-        cj = take(b * ne * s * f);
-        ct = take(b * ne * s * f);
-        epart = take(b * bss_energy_chunks(T, F) * ne * (3 * s + 3));
+        auto take = [&](size_t n) { double* q = p ? p + off : nullptr; off += n; return q; };
+        part = take(b * bss_corr_chunks(T) * r * (r + ne) * f);
+        rj = take(b * f * r * r);
+        rt = take(b * s * f * c * c);
+        eref = take(b * r);
+        cj = take(b * ne * r * f);
+        ct = take(b * ne * r * f);
+        epart = take(b * bss_energy_chunks(T, F) * ne * (size_t)NV);
         bytes = off * sizeof(double);
     }
 };
 
-// Row r of item b: references 0..S-1, estimates S..2S-1, the mixture 2S.
+// Row r of item b, S reference rows per item: references 0..S-1, estimates S..2S-1, the mixture 2S.  Source images
+// pass S = R: reference row j C + c is channel c of image j.
 __device__ __forceinline__ const float* bss_row(const float* ref, const float* est, const float* mix, int S,
                                                 long long b, int r, long long T) {
     if (r < S) return ref + ((size_t)b * S + r) * T;
@@ -124,7 +138,8 @@ struct BssItems {
     }
 };
 
-// grid = items * chunks, kBssCorrTile threads; smem [NB][kBssCorrTile + F - 1] doubles.  An item is cut into its own
+// grid = items * chunks, kBssCorrTile threads; smem [NB][kBssCorrTile + F - 1] doubles.  S counts reference rows (R
+// for source images).  An item is cut into its own
 // bss_corr_chunks(length) chunks, so its partials are those of the item scored alone; the launch's chunks past them
 // are written as zeros, which leave the reader's chunk-order sums unchanged.
 template <int S, int NE>
@@ -236,9 +251,11 @@ __device__ void bss_levinson(const BssCorr<S, NB>& cr, const int (&ch)[M], const
     constexpr int MM = M * M, NV = MM + NE * M;
     __shared__ double red[8][NV];
     __shared__ double sKf[MM], sKb[MM], sg[NE * M], srhs[NE * M];
+    // A zero-energy channel of a non-silent source image is dropped, not normalised: its rows and columns of the
+    // system are zero, so every pivot of it is dropped, and its filters are zero (mir_eval's lstsq fallback).
     double inv[M];
 #pragma unroll
-    for (int r = 0; r < M; ++r) inv[r] = 1.0 / sqrt(sE[ch[r]]);
+    for (int r = 0; r < M; ++r) inv[r] = sE[ch[r]] > 0.0 ? 1.0 / sqrt(sE[ch[r]]) : 0.0;
     for (int idx = threadIdx.x; idx < F * MM; idx += blockDim.x) {
         const int k = idx / MM, r = (idx / M) % M, q = idx % M;
         Rg[idx] = cr(ch[r], ch[q], k) * inv[r] * inv[q];
@@ -402,59 +419,73 @@ __device__ void bss_levinson(const BssCorr<S, NB>& cr, const int (&ch)[M], const
     }
 }
 
-// grid = B (S + 1): system 0 of an item is the joint one, system 1 + j reference j's own.  256 threads.
-template <int S, int NE>
+// Source j's energy, its C rows' summed in channel order (the row's own for C = 1)
+template <int C>
+__device__ __forceinline__ double bss_image_energy(const double* rows, int j) {
+    double e = rows[j * C];
+#pragma unroll
+    for (int c = 1; c < C; ++c) e += rows[j * C + c];
+    return e;
+}
+
+// grid = B (S + 1): system 0 of an item is the joint one over all R = S C reference rows, system 1 + j source j's own
+// over its C rows.  256 threads.
+template <int S, int NE, int C = 1>
 __global__ void __launch_bounds__(256)
 bss_solve_kernel(const double* __restrict__ part, int chunks, double* __restrict__ rj, double* __restrict__ rt,
                  double* __restrict__ eref, double* __restrict__ cj, double* __restrict__ ct, int F) {
-    constexpr int NB = S + NE;
+    constexpr int R = S * C, NB = R + NE;
     extern __shared__ double smem[];
-    __shared__ double sE[S];
+    __shared__ double sE[R];
     const long long b = blockIdx.x / (S + 1);
     const int sys = (int)(blockIdx.x - b * (S + 1));
-    const BssCorr<S, NB> cr{part + (size_t)b * chunks * S * NB * F, chunks, F};
-    if (threadIdx.x < S) sE[threadIdx.x] = cr(threadIdx.x, threadIdx.x, 0);
+    const BssCorr<R, NB> cr{part + (size_t)b * chunks * R * NB * F, chunks, F};
+    if (threadIdx.x < R) sE[threadIdx.x] = cr(threadIdx.x, threadIdx.x, 0);
     __syncthreads();
     bool silent = false;
 #pragma unroll
-    for (int i = 0; i < S; ++i) silent = silent || !bss_scorable(sE[i]);
-    if (sys == 0 && threadIdx.x < S) eref[(size_t)b * S + threadIdx.x] = sE[threadIdx.x];
-    double* out = (sys == 0 ? cj : ct) + (size_t)b * (S + 1) * S * F;
+    for (int i = 0; i < S; ++i) silent = silent || !bss_scorable(bss_image_energy<C>(sE, i));
+    if (sys == 0 && threadIdx.x < R) eref[(size_t)b * R + threadIdx.x] = sE[threadIdx.x];
+    double* out = (sys == 0 ? cj : ct) + (size_t)b * (R + 1) * R * F;
     if (silent) {                                       // the item's outputs are NaN; its filters are set to zero
-        for (int idx = threadIdx.x; idx < NE * S * F; idx += blockDim.x) {
-            const int e = idx / (S * F), r = (idx / F) % S;
-            if (sys == 0 || r == sys - 1) out[idx] = 0.0;
+        for (int idx = threadIdx.x; idx < NE * R * F; idx += blockDim.x) {
+            const int r = (idx / F) % R;
+            if (sys == 0 || r / C == sys - 1) out[idx] = 0.0;
         }
         return;
     }
     if (sys == 0) {
-        int ch[S];
+        int ch[R];
 #pragma unroll
-        for (int i = 0; i < S; ++i) ch[i] = i;
-        bss_levinson<S, NE>(cr, ch, sE, rj + (size_t)b * F * S * S, out, F, smem);
+        for (int i = 0; i < R; ++i) ch[i] = i;
+        bss_levinson<R, NE>(cr, ch, sE, rj + (size_t)b * F * R * R, out, F, smem);
     } else {
-        const int ch[1] = {sys - 1};
-        bss_levinson<1, NE>(cr, ch, sE, rt + ((size_t)b * S + sys - 1) * F, out, F, smem);
+        int ch[C];
+#pragma unroll
+        for (int c = 0; c < C; ++c) ch[c] = (sys - 1) * C + c;
+        bss_levinson<C, NE>(cr, ch, sE, rt + ((size_t)b * S + sys - 1) * F * C * C, out, F, smem);
     }
 }
 
-// grid = items * echunks, kBssEnergyTile threads; smem: references [S][kBssEnergyTile + F - 1], filters [2][S][F].
-// Over t < T + F - 1 (T the item's length), estimate row e's projections pa = sum_i cj_e,i * s_i and
-// pt_j = ct_e,j * s_j and the energies
+// grid = items * echunks, kBssEnergyTile threads; smem: reference rows [R][kBssEnergyTile + F - 1], filters
+// [2][R][F], R = S C.  Over t < T + F - 1 (T the item's length), estimate row e's projections pa = sum_r cj_e,r * s_r
+// and pt_j = sum_c ct_e,jC+c * s_jC+c and the energies
 //     [0, S)  |pt_j|^2,   [S, 2S)  |e - pt_j|^2,   [2S, 3S)  |pa - pt_j|^2,   3S |pa|^2,   3S+1 |e - pa|^2,   3S+2 |e|^2
+// and for source images (IMG), with s_j the row of reference j in e's channel (e mod C):
+//     [3S+3, 4S+3)  |pt_j - s_j|^2,   [4S+3, 5S+3)  |e - s_j|^2
 // Chunked as bss_corr_kernel: the item's own bss_energy_chunks, zero partials past them.
-template <int S, int NE>
+template <int S, int NE, int C = 1, bool IMG = false>
 __global__ void __launch_bounds__(kBssEnergyTile)
 bss_energy_kernel(const float* __restrict__ ref, const float* __restrict__ est, const float* __restrict__ mix,
                   const double* __restrict__ cj, const double* __restrict__ ct, double* __restrict__ epart,
                   BssItems items, int F, int chunks) {
-    constexpr int NV = 3 * S + 3;
+    constexpr int R = S * C, NV = bss_energy_count(S, IMG);
     extern __shared__ double sm[];
     __shared__ double red[kBssEnergyTile / 32][NV];
     const int W = kBssEnergyTile + F - 1;
-    double* sref = sm;                                  // [S][W]: s_i[tt - F + 1 + q]
-    double* sj = sref + (size_t)S * W;                  // [S][F]
-    double* st = sj + (size_t)S * F;                    // [S][F]
+    double* sref = sm;                                  // [R][W]: s_r[tt - F + 1 + q]
+    double* sj = sref + (size_t)R * W;                  // [R][F]
+    double* st = sj + (size_t)R * F;                    // [R][F]
     const long long it = blockIdx.x / chunks;
     const int chunk = (int)(blockIdx.x - it * chunks);
     long long b, T;
@@ -466,36 +497,40 @@ bss_energy_kernel(const float* __restrict__ ref, const float* __restrict__ est, 
     const long long t1 = t0 + per < L ? t0 + per : L;
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     for (int e = 0; e < NE; ++e) {
-        const float* er = bss_row(ref, est, mix, S, b, S + e, items.T) + off;
+        const float* er = bss_row(ref, est, mix, R, b, R + e, items.T) + off;
         __syncthreads();
-        for (int idx = threadIdx.x; idx < S * F; idx += kBssEnergyTile) {
-            sj[idx] = cj[((size_t)it * (S + 1) + e) * S * F + idx];
-            st[idx] = ct[((size_t)it * (S + 1) + e) * S * F + idx];
+        for (int idx = threadIdx.x; idx < R * F; idx += kBssEnergyTile) {
+            sj[idx] = cj[((size_t)it * (R + 1) + e) * R * F + idx];
+            st[idx] = ct[((size_t)it * (R + 1) + e) * R * F + idx];
         }
         double acc[NV];
 #pragma unroll
         for (int i = 0; i < NV; ++i) acc[i] = 0.0;
         for (long long tt = t0; tt < t1; tt += kBssEnergyTile) {
             __syncthreads();
-            for (int idx = threadIdx.x; idx < S * W; idx += kBssEnergyTile) {
+            for (int idx = threadIdx.x; idx < R * W; idx += kBssEnergyTile) {
                 const int i = idx / W, q = idx - i * W;
                 const long long t = tt - (F - 1) + q;
-                sref[idx] = t >= 0 && t < T ? (double)__ldg(ref + ((size_t)b * S + i) * items.T + off + t) : 0.0;
+                sref[idx] = t >= 0 && t < T ? (double)__ldg(ref + ((size_t)b * R + i) * items.T + off + t) : 0.0;
             }
             __syncthreads();
             const long long t = tt + threadIdx.x;
             if (t < t1) {
                 double pa = 0.0, pt[S];
 #pragma unroll
-                for (int i = 0; i < S; ++i) {
-                    const double* s = sref + (size_t)i * W + threadIdx.x + F - 1;
+                for (int j = 0; j < S; ++j) {
                     double p = 0.0;
-                    for (int l = 0; l < F; ++l) {
-                        const double v = s[-l];
-                        pa = fma(sj[i * F + l], v, pa);
-                        p = fma(st[i * F + l], v, p);
+#pragma unroll
+                    for (int c = 0; c < C; ++c) {
+                        const int i = j * C + c;
+                        const double* s = sref + (size_t)i * W + threadIdx.x + F - 1;
+                        for (int l = 0; l < F; ++l) {
+                            const double v = s[-l];
+                            pa = fma(sj[i * F + l], v, pa);
+                            p = fma(st[i * F + l], v, p);
+                        }
                     }
-                    pt[i] = p;
+                    pt[j] = p;
                 }
                 const double ev = t < T ? (double)__ldg(er + t) : 0.0;
 #pragma unroll
@@ -507,6 +542,15 @@ bss_energy_kernel(const float* __restrict__ ref, const float* __restrict__ est, 
                 acc[3 * S] = fma(pa, pa, acc[3 * S]);
                 acc[3 * S + 1] = fma(ev - pa, ev - pa, acc[3 * S + 1]);
                 acc[3 * S + 2] = fma(ev, ev, acc[3 * S + 2]);
+                if constexpr (IMG) {
+                    const int c = e % C;
+#pragma unroll
+                    for (int j = 0; j < S; ++j) {
+                        const double sv = sref[(size_t)(j * C + c) * W + threadIdx.x + F - 1];   // s_jC+c[t]
+                        acc[3 * S + 3 + j] = fma(pt[j] - sv, pt[j] - sv, acc[3 * S + 3 + j]);
+                        acc[4 * S + 3 + j] = fma(ev - sv, ev - sv, acc[4 * S + 3 + j]);
+                    }
+                }
             }
         }
 #pragma unroll
@@ -518,7 +562,7 @@ bss_energy_kernel(const float* __restrict__ ref, const float* __restrict__ est, 
         if (threadIdx.x < NV) {
             double s = 0.0;
             for (int w = 0; w < kBssEnergyTile / 32; ++w) s += red[w][threadIdx.x];
-            epart[(((size_t)it * chunks + chunk) * (S + 1) + e) * NV + threadIdx.x] = s;
+            epart[(((size_t)it * chunks + chunk) * (R + 1) + e) * NV + threadIdx.x] = s;
         }
     }
 }
@@ -529,13 +573,16 @@ __device__ __forceinline__ double bss_db(double num, double den) {
 }
 
 // one thread per item.  sdr/sir/sar/perm [B][S] for the estimates (perm[j]: the estimate given reference j); with the
-// mixture (NE == S + 1), msdr/msir/msar [B][S]: the mixture scored as the estimate of every reference.
-template <int S, int NE>
+// mixture (NE == S + 1), msdr/msir/msar [B][S]: the mixture scored as the estimate of every reference.  Source images
+// (IMG) sum each estimate image's rows' energies over its C channels, in channel order, and also write isr [B][S].
+template <int S, int NE, int C = 1, bool IMG = false>
 __global__ void __launch_bounds__(256)
 bss_final_kernel(const double* __restrict__ epart, const double* __restrict__ eref, int chunks, double* __restrict__ sdr,
-                 double* __restrict__ sir, double* __restrict__ sar, int* __restrict__ perm, double* __restrict__ msdr,
-                 double* __restrict__ msir, double* __restrict__ msar, int B, int compute_permutation) {
-    constexpr int NV = 3 * S + 3;
+                 double* __restrict__ isr, double* __restrict__ sir, double* __restrict__ sar, int* __restrict__ perm,
+                 double* __restrict__ msdr, double* __restrict__ msir, double* __restrict__ msar, int B,
+                 int compute_permutation) {
+    constexpr int R = S * C, NV = bss_energy_count(S, IMG);
+    constexpr int NI = IMG ? S : NE;                    // scored estimates: images, or rows (with the mixture's)
     for (long long b = blockIdx.x * 256LL + threadIdx.x; b < B; b += (long long)gridDim.x * 256) {
         double en[NE][NV];
 #pragma unroll
@@ -543,28 +590,62 @@ bss_final_kernel(const double* __restrict__ epart, const double* __restrict__ er
 #pragma unroll
             for (int i = 0; i < NV; ++i) en[e][i] = 0.0;
         for (int c = 0; c < chunks; ++c) {
-            const double* pc = epart + ((size_t)b * chunks + c) * (S + 1) * NV;
+            const double* pc = epart + ((size_t)b * chunks + c) * (R + 1) * NV;
 #pragma unroll
             for (int e = 0; e < NE; ++e)
 #pragma unroll
                 for (int i = 0; i < NV; ++i) en[e][i] += pc[e * NV + i];
         }
+        const double* er = eref + (size_t)b * R;
         bool silent_ref = false;
 #pragma unroll
-        for (int i = 0; i < S; ++i) silent_ref = silent_ref || !bss_scorable(eref[(size_t)b * S + i]);
+        for (int i = 0; i < S; ++i) silent_ref = silent_ref || !bss_scorable(bss_image_energy<C>(er, i));
         bool silent = silent_ref;
 #pragma unroll
-        for (int e = 0; e < S; ++e)
-            silent = silent || !bss_scorable(en[e][3 * S + 2]) || !bss_projections_hold<S>(en[e]);
-        double d[NE][S], i_[NE][S], a[NE][S];
+        for (int e = 0; e < S; ++e) {
+            double e2 = en[e * C][3 * S + 2];
+            bool held = bss_projections_hold<S>(en[e * C]);
 #pragma unroll
-        for (int e = 0; e < NE; ++e)
-#pragma unroll
-            for (int j = 0; j < S; ++j) {
-                d[e][j] = bss_db(en[e][j], en[e][S + j]);
-                i_[e][j] = bss_db(en[e][j], en[e][2 * S + j]);
-                a[e][j] = bss_db(en[e][3 * S], en[e][3 * S + 1]);
+            for (int c = 1; c < C; ++c) {
+                e2 += en[e * C + c][3 * S + 2];
+                held = held && bss_projections_hold<S>(en[e * C + c]);
             }
+            silent = silent || !bss_scorable(e2) || !held;
+        }
+        double d[NI][S], i_[NI][S], a[NI][S], g[IMG ? S : 1][S];
+        if constexpr (!IMG) {
+#pragma unroll
+            for (int e = 0; e < NE; ++e)
+#pragma unroll
+                for (int j = 0; j < S; ++j) {
+                    d[e][j] = bss_db(en[e][j], en[e][S + j]);
+                    i_[e][j] = bss_db(en[e][j], en[e][2 * S + j]);
+                    a[e][j] = bss_db(en[e][3 * S], en[e][3 * S + 1]);
+                }
+        } else {
+#pragma unroll
+            for (int e = 0; e < S; ++e)
+#pragma unroll
+                for (int j = 0; j < S; ++j) {
+                    // |P_j e|^2, |P_all e - P_j e|^2, |P_all e|^2, |e - P_all e|^2, |P_j e - s_j|^2, |e - s_j|^2
+                    double pj = 0.0, in = 0.0, pa = 0.0, ar = 0.0, sp = 0.0, dd = 0.0;
+#pragma unroll
+                    for (int c = 0; c < C; ++c) {
+                        const double* v = en[e * C + c];
+                        pj += v[j];
+                        in += v[2 * S + j];
+                        pa += v[3 * S];
+                        ar += v[3 * S + 1];
+                        sp += v[3 * S + 3 + j];
+                        dd += v[4 * S + 3 + j];
+                    }
+                    const double sj = bss_image_energy<C>(er, j);
+                    d[e][j] = bss_db(sj, dd);
+                    g[e][j] = bss_db(sj, sp);
+                    i_[e][j] = bss_db(pj, in);
+                    a[e][j] = bss_db(pa, ar);
+                }
+        }
         int p[S];
 #pragma unroll
         for (int j = 0; j < S; ++j) p[j] = j;
@@ -579,16 +660,20 @@ bss_final_kernel(const double* __restrict__ epart, const double* __restrict__ er
         const double nan = __longlong_as_double(0x7ff8000000000000LL);
 #pragma unroll
         for (int j = 0; j < S; ++j) {
-            double dj = 0.0, ij = 0.0, aj = 0.0;
+            double dj = 0.0, ij = 0.0, aj = 0.0, gj = 0.0;
 #pragma unroll
             for (int e = 0; e < S; ++e)
-                if (p[j] == e) { dj = d[e][j]; ij = i_[e][j]; aj = a[e][j]; }
+                if (p[j] == e) {
+                    dj = d[e][j]; ij = i_[e][j]; aj = a[e][j];
+                    if constexpr (IMG) gj = g[e][j];
+                }
             const size_t o = (size_t)b * S + j;
             sdr[o] = silent ? nan : dj;
             sir[o] = silent ? nan : ij;
             sar[o] = silent ? nan : aj;
+            if constexpr (IMG) isr[o] = silent ? nan : gj;
             if (perm) perm[o] = silent ? -1 : p[j];
-            if constexpr (NE > S) {
+            if constexpr (NI > S) {
                 const bool ms = silent_ref || !bss_scorable(en[S][3 * S + 2]) || !bss_projections_hold<S>(en[S]);
                 msdr[o] = ms ? nan : d[S][j];
                 msir[o] = ms ? nan : i_[S][j];
@@ -600,36 +685,38 @@ bss_final_kernel(const double* __restrict__ epart, const double* __restrict__ er
 
 // Scores n items of the view in launches of at most cap items, all through one scratch sized for cap items of at most
 // L samples: the launches follow each other on the stream with no host synchronisation between them, so a call can
-// be captured in a CUDA graph.  Item i's outputs are [i][S].
-template <int S, int NE>
-static int bss_eval_launch(const float* ref, const float* est, const float* mix, double* sdr, double* sir,
-                           double* sar, int* perm, double* msdr, double* msir, double* msar, BssItems items,
-                           long long n, long long cap, long long L, int F, int compute_permutation, void* scratch,
-                           cudaStream_t st) {
+// be captured in a CUDA graph.  Item i's outputs are [i][S].  Source images are <S, S C, C, true>.
+template <int S, int NE, int C = 1, bool IMG = false>
+static int bss_eval_launch(const float* ref, const float* est, const float* mix, double* sdr, double* isr,
+                           double* sir, double* sar, int* perm, double* msdr, double* msir, double* msar,
+                           BssItems items, long long n, long long cap, long long L, int F, int compute_permutation,
+                           void* scratch, cudaStream_t st) {
+    constexpr int R = S * C;
     const int m = (int)(n < cap ? n : cap);
-    const BssScratch s(scratch, m, S, L, F);
+    const BssScratch s(scratch, m, S, C, L, F, bss_energy_count(S, IMG));
     const int cc = bss_corr_chunks(L), ec = bss_energy_chunks(L, F);
     if ((long long)m * cc > 0x7fffffffLL || (long long)m * (S + 1) > 0x7fffffffLL) return SDR_ERR_UNSUPPORTED;
-    const size_t corr_smem = sizeof(double) * (S + NE) * (kBssCorrTile + F - 1);
-    const size_t solve_smem = sizeof(double) * (size_t)F * (2 * S * S + NE * S);
-    const size_t energy_smem = sizeof(double) * (size_t)S * (kBssEnergyTile + F - 1 + 2 * F);
+    const size_t corr_smem = sizeof(double) * (R + NE) * (kBssCorrTile + F - 1);
+    const size_t solve_smem = sizeof(double) * (size_t)F * (2 * R * R + NE * R);
+    const size_t energy_smem = sizeof(double) * (size_t)R * (kBssEnergyTile + F - 1 + 2 * F);
     for (long long first = 0; first < n; first += m) {
         const int k = (int)(n - first < m ? n - first : m);
         const size_t o = (size_t)first * S;
         items.first = first;
         int e;
-        if ((e = launch(bss_corr_kernel<S, NE>, (unsigned)((long long)k * cc), kBssCorrTile, corr_smem, st, ref, est,
+        if ((e = launch(bss_corr_kernel<R, NE>, (unsigned)((long long)k * cc), kBssCorrTile, corr_smem, st, ref, est,
                         mix, s.part, items, F, cc)))
             return e;
-        if ((e = launch(bss_solve_kernel<S, NE>, (unsigned)((long long)k * (S + 1)), 256, solve_smem, st, s.part, cc,
-                        s.rj, s.rt, s.eref, s.cj, s.ct, F)))
+        if ((e = launch(bss_solve_kernel<S, NE, C>, (unsigned)((long long)k * (S + 1)), 256, solve_smem, st, s.part,
+                        cc, s.rj, s.rt, s.eref, s.cj, s.ct, F)))
             return e;
-        if ((e = launch(bss_energy_kernel<S, NE>, (unsigned)((long long)k * ec), kBssEnergyTile, energy_smem, st, ref,
-                        est, mix, s.cj, s.ct, s.epart, items, F, ec)))
+        if ((e = launch(bss_energy_kernel<S, NE, C, IMG>, (unsigned)((long long)k * ec), kBssEnergyTile, energy_smem,
+                        st, ref, est, mix, s.cj, s.ct, s.epart, items, F, ec)))
             return e;
-        if ((e = launch(bss_final_kernel<S, NE>, item_blocks(k), 256, 0, st, s.epart, s.eref, ec, sdr + o, sir + o,
-                        sar + o, perm ? perm + o : nullptr, msdr ? msdr + o : nullptr, msir ? msir + o : nullptr,
-                        msar ? msar + o : nullptr, k, compute_permutation)))
+        if ((e = launch(bss_final_kernel<S, NE, C, IMG>, item_blocks(k), 256, 0, st, s.epart, s.eref, ec, sdr + o,
+                        isr ? isr + o : nullptr, sir + o, sar + o, perm ? perm + o : nullptr,
+                        msdr ? msdr + o : nullptr, msir ? msir + o : nullptr, msar ? msar + o : nullptr, k,
+                        compute_permutation)))
             return e;
     }
     return SDR_OK;
@@ -648,11 +735,31 @@ static int bss_dispatch(const float* ref, const float* est, const float* mix, do
                         long long cap, long long L, int F, int compute_permutation, void* scratch, cudaStream_t st) {
     return with_sources(S, [&](auto s) {
         constexpr int c = decltype(s)::value;
-        return mix ? bss_eval_launch<c, c + 1>(ref, est, mix, sdr, sir, sar, perm, msdr, msir, msar, items, n, cap, L,
-                                               F, compute_permutation, scratch, st)
-                   : bss_eval_launch<c, c>(ref, est, nullptr, sdr, sir, sar, perm, nullptr, nullptr, nullptr, items, n,
-                                           cap, L, F, compute_permutation, scratch, st);
+        return mix ? bss_eval_launch<c, c + 1>(ref, est, mix, sdr, nullptr, sir, sar, perm, msdr, msir, msar, items, n,
+                                               cap, L, F, compute_permutation, scratch, st)
+                   : bss_eval_launch<c, c>(ref, est, nullptr, sdr, nullptr, sir, sar, perm, nullptr, nullptr, nullptr,
+                                           items, n, cap, L, F, compute_permutation, scratch, st);
     });
+}
+
+// The source-image kernels are instantiated for S C <= 4: the joint system's shared memory, (2 R^2 + E R) F doubles
+// at R = E = S C, is 192 KiB at R = 4 and F = 512.
+static int bss_images_dispatch(const float* ref, const float* est, double* sdr, double* isr, double* sir, double* sar,
+                               int* perm, int S, int C, const BssItems& items, long long n, long long cap, long long L,
+                               int F, int compute_permutation, void* scratch, cudaStream_t st) {
+    auto run = [&](auto s, auto c) {
+        constexpr int S_ = decltype(s)::value, C_ = decltype(c)::value;
+        return bss_eval_launch<S_, S_ * C_, C_, true>(ref, est, nullptr, sdr, isr, sir, sar, perm, nullptr, nullptr,
+                                                      nullptr, items, n, cap, L, F, compute_permutation, scratch, st);
+    };
+    using I1 = std::integral_constant<int, 1>;
+    using I2 = std::integral_constant<int, 2>;
+    if (C == 1) return with_sources(S, [&](auto s) { return run(s, I1()); });
+    if (S == 1 && C == 2) return run(I1(), I2());
+    if (S == 1 && C == 3) return run(I1(), std::integral_constant<int, 3>());
+    if (S == 1 && C == 4) return run(I1(), std::integral_constant<int, 4>());
+    if (S == 2 && C == 2) return run(I2(), I2());
+    return SDR_ERR_UNSUPPORTED;
 }
 
 // sdr_bss_eval (mix null) and sdr_bss_eval_mixture: item b is the whole of recording b, all in one launch sequence
@@ -677,6 +784,29 @@ static long long bss_framewise_span(long long T, long long W, long long H) {
     return W > T || H - 1 > T - W ? T : W + H - 1;
 }
 
+// The scratch of B whole items of S sources of C rows (0: unsupported).  S F delayed references in R^(T+F-1), R = S C:
+// more than the dimensions (T < (R - 1) F + 1) makes the joint system singular by construction, where the recursion's
+// rounding no longer separates dependent pivots from independent ones.
+static size_t bss_scratch_bytes(int B, int S, int C, long long T, int F, bool images) {
+    if (B <= 0 || S < 1 || S > 4 || C < 1 || S * C > 4 || T <= 0 || F < 1 || F > kBssMaxF) return 0;
+    if ((long long)S * C * F > T + F - 1) return 0;
+    return BssScratch(nullptr, B, S, C, T, F, bss_energy_count(S, images)).bytes;
+}
+
+// The scratch of a framewise call: at most kBssFramewiseItems items of the longest length one can have (0: unsupported)
+static size_t bss_framewise_scratch_bytes(int B, int S, int C, long long T, long long W, long long H, int F,
+                                          bool images) {
+    if (B <= 0 || S < 1 || S > 4 || C < 1 || S * C > 4 || T <= 0 || W <= 0 || H <= 0 || F < 1 || F > kBssMaxF)
+        return 0;
+    const long long len = T - W < H ? T : W;               // the length of every item, or of the fallback's
+    if ((long long)S * C * F > len + F - 1) return 0;
+    const long long nwin = bss_window_count(T, W, H);
+    if (nwin > INT64_MAX / S / B) return 0;
+    const long long n = (long long)B * nwin;
+    return BssScratch(nullptr, (int)(n < kBssFramewiseItems ? n : kBssFramewiseItems), S, C,
+                      bss_framewise_span(T, W, H), F, bss_energy_count(S, images)).bytes;
+}
+
 }  // namespace sdr
 
 using namespace sdr;
@@ -684,13 +814,7 @@ using namespace sdr;
 #pragma GCC visibility push(default)
 extern "C" {
 
-size_t sdr_bss_eval_scratch_bytes(int B, int S, int64_t T, int F) {
-    if (B <= 0 || S < 1 || S > 4 || T <= 0 || F < 1 || F > kBssMaxF) return 0;
-    // S F delayed references in R^(T+F-1): more than the dimensions (T < (S-1) F + 1) makes the joint system singular
-    // by construction, where the recursion's rounding no longer separates dependent pivots from independent ones
-    if ((long long)S * F > T + F - 1) return 0;
-    return BssScratch(nullptr, B, S, T, F).bytes;
-}
+size_t sdr_bss_eval_scratch_bytes(int B, int S, int64_t T, int F) { return bss_scratch_bytes(B, S, 1, T, F, false); }
 
 int sdr_bss_eval(const float* reference, const float* estimate, double* sdr, double* sir, double* sar,
                  int32_t* perm_or_null, int B, int S, int64_t T, int F, int compute_permutation, void* scratch,
@@ -709,14 +833,7 @@ int sdr_bss_eval_mixture(const float* reference, const float* estimate, const fl
 }
 
 size_t sdr_bss_eval_framewise_scratch_bytes(int B, int S, int64_t T, int64_t W, int64_t H, int F) {
-    if (B <= 0 || S < 1 || S > 4 || T <= 0 || W <= 0 || H <= 0 || F < 1 || F > kBssMaxF) return 0;
-    const long long len = T - W < H ? T : W;               // the length of every item, or of the fallback's
-    if ((long long)S * F > len + F - 1) return 0;
-    const long long nwin = bss_window_count(T, W, H);
-    if (nwin > INT64_MAX / S / B) return 0;
-    const long long n = (long long)B * nwin;
-    return BssScratch(nullptr, (int)(n < kBssFramewiseItems ? n : kBssFramewiseItems), S, bss_framewise_span(T, W, H),
-                      F).bytes;
+    return bss_framewise_scratch_bytes(B, S, 1, T, W, H, F, false);
 }
 
 int sdr_bss_eval_framewise(const float* reference, const float* estimate, const float* mixture_or_null,
@@ -737,6 +854,43 @@ int sdr_bss_eval_framewise(const float* reference, const float* estimate, const 
                         mix ? mix_sir : nullptr, mix ? mix_sar : nullptr, S, items, (long long)B * nwin,
                         kBssFramewiseItems, bss_framewise_span(T, W, H), F, compute_permutation, scratch,
                         static_cast<cudaStream_t>(stream));
+}
+
+size_t sdr_bss_eval_images_scratch_bytes(int B, int S, int C, int64_t T, int F) {
+    return bss_scratch_bytes(B, S, C, T, F, true);
+}
+
+int sdr_bss_eval_images(const float* reference, const float* estimate, double* sdr, double* isr, double* sir,
+                        double* sar, int32_t* perm_or_null, int B, int S, int C, int64_t T, int F,
+                        int compute_permutation, void* scratch, sdr_stream stream) {
+    if (!isr || !bss_buffers_ok(reference, estimate, nullptr, sdr, sir, sar, nullptr, nullptr, nullptr, scratch))
+        return SDR_ERR_BAD_ARGUMENT;
+    if (!sdr_bss_eval_images_scratch_bytes(B, S, C, T, F))
+        return B <= 0 || T <= 0 ? SDR_ERR_BAD_ARGUMENT : SDR_ERR_UNSUPPORTED;
+    const BssItems whole{T, T, T, 1, 0, 0, nullptr};
+    return bss_images_dispatch(reference, estimate, sdr, isr, sir, sar, perm_or_null, S, C, whole, B, B, T, F,
+                               compute_permutation, scratch, static_cast<cudaStream_t>(stream));
+}
+
+size_t sdr_bss_eval_images_framewise_scratch_bytes(int B, int S, int C, int64_t T, int64_t W, int64_t H, int F) {
+    return bss_framewise_scratch_bytes(B, S, C, T, W, H, F, true);
+}
+
+int sdr_bss_eval_images_framewise(const float* reference, const float* estimate, const int64_t* lengths_or_null,
+                                  double* sdr, double* isr, double* sir, double* sar, int32_t* perm_or_null, int B,
+                                  int S, int C, int64_t T, int64_t W, int64_t H, int F, int compute_permutation,
+                                  void* scratch, sdr_stream stream) {
+    if (!isr || !bss_buffers_ok(reference, estimate, nullptr, sdr, sir, sar, nullptr, nullptr, nullptr, scratch) ||
+        reinterpret_cast<uintptr_t>(lengths_or_null) % 8)
+        return SDR_ERR_BAD_ARGUMENT;
+    if (!sdr_bss_eval_images_framewise_scratch_bytes(B, S, C, T, W, H, F))
+        return B <= 0 || T <= 0 || W <= 0 || H <= 0 ? SDR_ERR_BAD_ARGUMENT : SDR_ERR_UNSUPPORTED;
+    const long long nwin = bss_window_count(T, W, H);
+    const BssItems items{T, W, H, nwin, 0, (long long)(S * C - 1) * F + 1,
+                         reinterpret_cast<const long long*>(lengths_or_null)};
+    return bss_images_dispatch(reference, estimate, sdr, isr, sir, sar, perm_or_null, S, C, items,
+                               (long long)B * nwin, kBssFramewiseItems, bss_framewise_span(T, W, H), F,
+                               compute_permutation, scratch, static_cast<cudaStream_t>(stream));
 }
 
 }  // extern "C"
