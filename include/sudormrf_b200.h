@@ -524,6 +524,23 @@ int sdr_bss_eval_images_framewise(const float* reference, const float* estimate,
                                   double* sdr, double* isr, double* sir, double* sar, int32_t* perm_or_null, int B,
                                   int S, int C, int64_t T, int64_t W, int64_t H, int F, int compute_permutation,
                                   void* scratch, sdr_stream stream);
+/* BSS-eval v4 (museval.evaluate(..., mode='v4'), the SiSEC 2018 / MUSDB18 criteria): reference, estimate [B,S,C,T]
+ * as sdr_bss_eval_images -> sdr, isr, sir, sar, perm [B,nwin,S], nwin = (T - W) / H + 1.  The distortion filters are
+ * solved once per recording from the correlations of its whole length (those sdr_bss_eval_images computes on it);
+ * window k, [k H, k H + W), then filters its own reference slice (zero outside the window) with them, and its
+ * criteria are sdr_bss_eval_images' formulas on the window's slices and energies.  No whole-recording fallback.  A
+ * window with an all-zero reference or estimate image is NaN with perm -1; a NaN or an infinity anywhere in a
+ * recording, or whole-track filters that are no projection, make every window of that recording NaN with perm -1.
+ * lengths_or_null [B] (read on the device): recording b is its first lengths[b] samples, with its own filters and
+ * (n - W) / H + 1 windows; columns past them, and every column of a recording with n < W, n < (S C - 1) F + 1 or n
+ * outside [1, T], are NaN with perm -1.  1 <= S C <= 4, 1 <= F <= 512, T >= W and T >= (S C - 1) F + 1; scratch:
+ * sdr_bss_eval_v4_scratch_bytes (0: unsupported arguments), 8-byte aligned, bounded in T once T passes 512 chunks of
+ * 8192 samples per recording.  Bitwise reproducible, a recording's columns the same in any batch; no call
+ * synchronises. */
+size_t sdr_bss_eval_v4_scratch_bytes(int B, int S, int C, int64_t T, int64_t W, int64_t H, int F);
+int sdr_bss_eval_v4(const float* reference, const float* estimate, const int64_t* lengths_or_null, double* sdr,
+                    double* isr, double* sir, double* sar, int32_t* perm_or_null, int B, int S, int C, int64_t T,
+                    int64_t W, int64_t H, int F, int compute_permutation, void* scratch, sdr_stream stream);
 
 /* STOI (pystoi 0.3.3's stoi(x, y, fs_sig, extended=False), the stoi of asteroid's get_metrics): reference and
  * estimate [B,S,T], mixture_or_null [B,T] -> stoi [B,S] fp64 (estimate j scored against reference j) and, with the

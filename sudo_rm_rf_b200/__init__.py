@@ -9,13 +9,13 @@ exported here as ``OriginalSuDORMRF``) /
 ``PermInvariantSNRwithZeroRefs`` of ``sudo_rm_rf.dnn.losses.snr`` (module ``snr``), and the BSS-eval
 source criteria of the evaluation scripts (``bss_eval_sources``, mir_eval's definition, and its framewise form
 ``bss_eval_sources_framewise``; for multichannel separations the image criteria ``bss_eval_images`` and
-``bss_eval_images_framewise``) and their STOI (``stoi``,
+``bss_eval_images_framewise``, and museval's BSS-eval v4 ``bss_eval_v4``) and their STOI (``stoi``,
 pystoi's definition; module ``stoi_metric``), and scipy's ``resample_poly`` (module ``resample``).
 """
 from . import improved_sudormrf, groupcomm_sudormrf_v2, causal_improved_sudormrf_v3, sudormrf, mixture_consistency   # noqa: F401
 from . import snr                                                             # noqa: F401
 from .bss_eval import bss_eval_sources, bss_eval_sources_framewise            # noqa: F401
-from .bss_eval import bss_eval_images, bss_eval_images_framewise              # noqa: F401
+from .bss_eval import bss_eval_images, bss_eval_images_framewise, bss_eval_v4 # noqa: F401
 from .stoi_metric import stoi                                                 # noqa: F401
 from .resample import resample_poly                                           # noqa: F401
 from .improved_sudormrf import SuDORMRF                                       # noqa: F401
@@ -28,5 +28,6 @@ from .resample_stream import ResampleStream, ResampledStream                   #
 
 __all__ = ["SuDORMRF", "GroupCommSudoRmRf", "CausalSuDORMRF", "OriginalSuDORMRF", "improved_sudormrf",
            "groupcomm_sudormrf_v2", "causal_improved_sudormrf_v3", "sudormrf", "mixture_consistency", "snr",
-           "bss_eval_sources", "bss_eval_sources_framewise", "bss_eval_images", "bss_eval_images_framewise", "stoi",
+           "bss_eval_sources", "bss_eval_sources_framewise", "bss_eval_images", "bss_eval_images_framewise",
+           "bss_eval_v4", "stoi",
            "resample_poly", "refresh_weights", "WindowedStream", "ResampleStream", "ResampledStream"]

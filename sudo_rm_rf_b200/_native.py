@@ -174,6 +174,11 @@ _SIGNATURES = {
                                                 C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int, C.c_int,
                                                 C.c_int64, C.c_int64, C.c_int64, C.c_int, C.c_int, C.c_void_p,
                                                 C.c_void_p]),
+    "sdr_bss_eval_v4_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_int64,
+                                                   C.c_int]),
+    "sdr_bss_eval_v4": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_int, C.c_int, C.c_int, C.c_int64, C.c_int64, C.c_int64, C.c_int,
+                                  C.c_int, C.c_void_p, C.c_void_p]),
     "sdr_stoi_scratch_bytes": (C.c_size_t, [C.c_int, C.c_int, C.c_int64, C.c_int]),
     "sdr_stoi": (C.c_int, [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int, C.c_int,
                            C.c_int64, C.c_int, C.c_void_p, C.c_void_p]),

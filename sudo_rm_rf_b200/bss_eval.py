@@ -20,6 +20,9 @@ a fixed hop (``sdr_bss_eval_framewise``), each window read in place from the rec
 ``bss_eval_images`` and ``bss_eval_images_framewise`` are mir_eval's source-image criteria for multichannel
 separations (SDR, ISR, SIR and SAR; ``sdr_bss_eval_images``), the same kernels with each source's C channel rows
 projected together.
+
+``bss_eval_v4`` is museval's BSS-eval v4 (``sdr_bss_eval_v4``), the SiSEC 2018 / MUSDB18 criteria: the image criteria
+per window, with distortion filters solved once from the whole recording.
 """
 import torch
 
@@ -66,7 +69,7 @@ def _fp32(ref, est, mixture):
 
 
 def bss_eval_sources(reference_sources, estimated_sources, compute_permutation=True, filter_length=512,
-                     mixture=None, *, _windows=None, _images=False):
+                     mixture=None, *, _windows=None, _images=False, _v4=False):
     """mir_eval's ``bss_eval_sources`` on CUDA tensors.
 
     ``reference_sources`` and ``estimated_sources`` are ``[S, T]`` (mir_eval's shape) or ``[B, S, T]``, 1 <= S <= 4,
@@ -87,14 +90,15 @@ def bss_eval_sources(reference_sources, estimated_sources, compute_permutation=T
 
     ``_windows`` = ``(window, hop, lengths)`` is ``bss_eval_sources_framewise``'s call (see ``_framewise``): the
     outputs gain a last dimension of windows.  ``_images`` is ``bss_eval_images``' call (see ``_images_call``):
-    inputs ``[..., S, T, C]`` and outputs ``(sdr, isr, sir, sar, perm)``.  Every BSS-eval entry allocates and enqueues
-    here, on the caller's stream, so the stream and thread tests of this entry cover them all."""
+    inputs ``[..., S, T, C]`` and outputs ``(sdr, isr, sir, sar, perm)``; with ``_v4`` as well, ``bss_eval_v4``'s.
+    Every BSS-eval entry allocates and enqueues here, on the caller's stream, so the stream and thread tests of this
+    entry cover them all."""
     if _images:
         ref, est, single = _images_checked(reference_sources, estimated_sources)
         B, S, T, C = ref.shape
         F = int(filter_length)
         dev = ref.device
-        nbytes, shape, enqueue = _images_call(B, S, C, T, F, _windows, dev)
+        nbytes, shape, enqueue = (_v4_call if _v4 else _images_call)(B, S, C, T, F, _windows, dev)
         ref, est, mix = _rows(ref, dev), _rows(est, dev), None
     else:
         ref, est, single = _checked(reference_sources, estimated_sources, mixture)
@@ -311,6 +315,64 @@ def _images_call(B, S, C, T, F, windows, dev):
         return lib.sdr_bss_eval_images_framewise(N.ptr(ref), N.ptr(est), N.ptr(lens), *o, N.ptr(perm), B, S, C, T,
                                                  W, H, F, cp, N.ptr(scratch), stream), what
     return nbytes, shape, enqueue
+
+
+def bss_eval_v4(reference_sources, estimated_sources, window=44100, hop=44100, compute_permutation=False,
+                filter_length=512, lengths=None):
+    """museval's BSS-eval v4 (``museval.evaluate(..., mode='v4')``, the SiSEC 2018 / MUSDB18 metric) on CUDA tensors.
+
+    ``reference_sources`` and ``estimated_sources`` are in ``bss_eval_images``' layout: ``[S, T, C]``, ``[S, T]``
+    (C = 1) or ``[B, S, T, C]``.  The distortion filters are solved once per recording, from the correlations of its
+    whole length: they are those ``bss_eval_images`` computes on the whole recording.  Window k, ``[k hop, k hop +
+    window)``, then filters its own reference slice (zero outside the window) with them, and with ``s_j`` the reference
+    slice, ``P_j e_i`` and ``P_all e_i`` the slice filtered by the own and joint filters and ``e_i`` the estimate
+    slice, energies summed over channels::
+
+        SDR = 10 log10(|s_j|^2 / |e_i - s_j|^2)           ISR = 10 log10(|s_j|^2 / |P_j e_i - s_j|^2)
+        SIR = 10 log10(|P_j e_i|^2 / |P_all e_i - P_j e_i|^2)
+        SAR = 10 log10(|P_all e_i|^2 / |e_i - P_all e_i|^2)
+
+    (a zero denominator is +inf).  The defaults are museval's: one-second windows and hops at 44.1 kHz, no permutation
+    search.  Returns ``(sdr, isr, sir, sar, perm)``, each ``[..., S, nwin]`` with ``nwin = (T - window) // hop + 1``,
+    fp64 in dB and int64; with ``compute_permutation`` each window takes the assignment with the largest mean SIR in
+    that window.  There is no whole-recording fallback: T < window is refused.
+
+    A window in which a reference or estimate image is all zeros is NaN with ``perm = -1``.  A NaN or an infinity
+    anywhere in a recording poisons its whole-track correlations, so every window of that recording is NaN with
+    ``perm = -1`` (unlike ``bss_eval_images_framewise``, where only the windows holding it are); so is every window of
+    a recording whose whole-track filters are no projection (see ``bss_eval_sources``).  Other recordings keep their
+    values.  ``lengths`` (``[B]`` integers) gives each recording its own length, filters and window count; columns
+    past that count are NaN with ``perm = -1``, and so is every column of a recording shorter than ``window`` or than
+    ``(S * C - 1) * filter_length + 1``.  As a CUDA tensor they cost no host synchronisation and the call can be
+    captured in a CUDA graph; host lengths are refused during capture.  A recording's columns are the same, bit for
+    bit, in any batch.
+
+    Limits: 1 <= S * C <= 4 (four mono stems, or stereo vocals and accompaniment; not four stereo stems),
+    1 <= filter_length <= 512, T >= window and T >= (S * C - 1) * filter_length + 1.  The scratch stops growing with
+    T past a few million samples per recording.  Metric only: no autograd."""
+    W, H = int(window), int(hop)
+    if W < 1 or H < 1:
+        raise RuntimeError("window and hop must be positive")
+    return bss_eval_sources(reference_sources, estimated_sources, compute_permutation, filter_length,
+                            _windows=(W, H, lengths), _images=True, _v4=True)
+
+
+def _v4_call(B, S, C, T, F, windows, dev):
+    """sdr_bss_eval_v4's scratch size, outputs [B, nwin, S] and call, refused before anything is allocated."""
+    lib = N.lib()
+    W, H, lengths = windows
+    nbytes = lib.sdr_bss_eval_v4_scratch_bytes(B, S, C, T, W, H, F)
+    if nbytes == 0:
+        raise N.NativeError("sdr_bss_eval_v4 supports 1 <= sources * channels <= 4, filter lengths 1..512 and "
+                            "recordings of at least one window and (sources * channels - 1) * filter_length + 1 "
+                            f"samples; got {S} sources x {C} channels, {T} samples, window {W}, filter_length {F}")
+    lens = _lengths(lengths, B, dev)
+
+    def enqueue(ref, est, mix, out, perm, cp, scratch, stream):
+        o = [N.ptr(out[i]) for i in range(4)]
+        return lib.sdr_bss_eval_v4(N.ptr(ref), N.ptr(est), N.ptr(lens), *o, N.ptr(perm), B, S, C, T, W, H, F, cp,
+                                   N.ptr(scratch), stream), "sdr_bss_eval_v4"
+    return nbytes, (B, (T - W) // H + 1, S), enqueue
 
 
 def _rows(x, dev):

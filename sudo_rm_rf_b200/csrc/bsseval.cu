@@ -26,6 +26,12 @@
 // The same four kernels with the reference rows grouped by source (template parameter C): the joint system has R
 // blocks and source j's own system its C rows.  The sources are the instance C = 1 without the images' two extra
 // energies, and compute what they computed before images existed.
+//
+// BSS-eval v4 (museval's, sdr_bss_eval_v4): the image criteria with the filters solved once per recording, from the
+// correlations of its whole length (bss_corr_kernel in fixed track chunks, bss_fold_kernel adding them in chunk order),
+// tested by bss_track_check_kernel, and applied to each window's reference slice by bss_energy_kernel.
+#include <type_traits>
+
 #include "assign.cuh"
 #include "launchers.cuh"
 
@@ -62,8 +68,10 @@ __device__ __forceinline__ bool bss_is_projection(double p2, double r2, double e
     return fabs(p2 + r2 - e2) <= kBssProjectionDefect * e2;
 }
 
-// Energies per estimate row (bss_energy_kernel's layout): 3 S + 3, and 2 S more for source images
-__host__ __device__ constexpr int bss_energy_count(int S, bool images) { return 3 * S + 3 + (images ? 2 * S : 0); }
+// Energies per estimate row (bss_energy_kernel's layout): 3 S + 3, 2 S more for source images, and S more for v4
+__host__ __device__ constexpr int bss_energy_count(int S, bool images, bool v4 = false) {
+    return 3 * S + 3 + (images ? 2 * S : 0) + (v4 ? S : 0);
+}
 
 // Estimate row e's energies come from projections: the joint one and every own one.
 template <int S, int NV>
@@ -136,27 +144,72 @@ struct BssItems {
         if (k < (n - W) / H + 1) len = W;
         return k * H;
     }
+    // BSS-eval v4's windows (museval): (n - W) / H + 1 of them when n >= W and none otherwise, with no whole-recording
+    // fallback; a recording shorter than min_len has none either.
+    __device__ __forceinline__ long long window(long long i, long long& b, long long& len) const {
+        const long long g = first + i;
+        b = g / nwin;
+        const long long k = g - b * nwin;
+        const long long n = lengths ? lengths[b] : T;
+        len = 0;
+        if (n < W || n < min_len || n > T) return 0;
+        if (k < (n - W) / H + 1) len = W;
+        return k * H;
+    }
 };
 
-// grid = items * chunks, kBssCorrTile threads; smem [NB][kBssCorrTile + F - 1] doubles.  S counts reference rows (R
-// for source images).  An item is cut into its own
-// bss_corr_chunks(length) chunks, so its partials are those of the item scored alone; the launch's chunks past them
-// are written as zeros, which leave the reader's chunk-order sums unchanged.
-template <int S, int NE>
-__global__ void __launch_bounds__(kBssCorrTile)
-bss_corr_kernel(const float* __restrict__ ref, const float* __restrict__ est, const float* __restrict__ mix,
-                double* __restrict__ part, BssItems items, int F, int chunks) {
-    constexpr int NB = S + NE;
-    extern __shared__ double sm[];
-    const long long it = blockIdx.x / chunks;
-    const int chunk = (int)(blockIdx.x - it * chunks);
-    long long b, T;
-    const long long off = items.span(it, b, T);
+// The correlation kernel's chunk policy is the type of its last argument.  An int (the item entries): `chunks` per
+// item in the launch, the item cut into its own bss_corr_chunks(length) chunks, so its partials are those of the item
+// scored alone; the launch's chunks past them are written as zeros, which leave the reader's chunk-order sums unchanged.
+__device__ __forceinline__ int bss_chunk_count(int chunks) { return chunks; }
+__device__ __forceinline__ void bss_chunk_range(int, long long T, int chunk, long long& t0, long long& t1) {
     const int own = bss_corr_chunks(T);
     const long long per = (T + own - 1) / own;
-    const long long t0 = chunk < own ? (long long)chunk * per : T;
-    const long long t1 = t0 + per < T ? t0 + per : T;
+    t0 = chunk < own ? (long long)chunk * per : T;
+    t1 = t0 + per < T ? t0 + per : T;
+}
+
+// BSS-eval v4's whole-recording correlations: chunks of kBssTrackChunk samples at fixed positions in the recording, a
+// launch taking chunks [c0, c0 + n) of every recording.  Each chunk's partials also hold the estimate rows' energies
+// |e|^2 over the chunk, after its correlations.  bss_fold_kernel adds them in chunk order, so a recording's sums depend
+// on its own length only: not on the batch, nor on how many chunks a launch takes.
+constexpr long long kBssTrackChunk = 8192;
+struct BssTrackChunks {
+    int n;
+    long long c0;
+};
+__device__ __forceinline__ int bss_chunk_count(const BssTrackChunks& c) { return c.n; }
+__device__ __forceinline__ void bss_chunk_range(const BssTrackChunks& c, long long T, int chunk, long long& t0,
+                                                long long& t1) {
+    const long long s = (c.c0 + chunk) * kBssTrackChunk;
+    t0 = s < T ? s : T;
+    t1 = t0 + kBssTrackChunk < T ? t0 + kBssTrackChunk : T;
+}
+// Doubles per chunk partial: the correlations of S reference rows with NB rows, and for v4 the NE estimate energies
+__host__ __device__ constexpr size_t bss_partial_size(int S, int NE, int F, bool track) {
+    return (size_t)S * (S + NE) * F + (track ? NE : 0);
+}
+
+// grid = items * chunks, kBssCorrTile threads; smem [NB][kBssCorrTile + F - 1] doubles.  S counts reference rows (R
+// for source images).
+template <int S, int NE, class Chunks>
+__global__ void __launch_bounds__(kBssCorrTile)
+bss_corr_kernel(const float* __restrict__ ref, const float* __restrict__ est, const float* __restrict__ mix,
+                double* __restrict__ part, BssItems items, int F, Chunks chunks) {
+    constexpr int NB = S + NE;
+    constexpr bool kTrack = std::is_same<Chunks, BssTrackChunks>::value;
+    extern __shared__ double sm[];
+    const int nc = bss_chunk_count(chunks);
+    const long long it = blockIdx.x / nc;
+    const int chunk = (int)(blockIdx.x - it * nc);
+    long long b, T;
+    const long long off = items.span(it, b, T);
+    long long t0, t1;
+    bss_chunk_range(chunks, T, chunk, t0, t1);
     const int W = kBssCorrTile + F - 1;
+    double ee[kTrack ? NE : 1];
+#pragma unroll
+    for (int e = 0; e < (kTrack ? NE : 1); ++e) ee[e] = 0.0;
     const int k = threadIdx.x;
     double acc[S][NB];
 #pragma unroll
@@ -186,14 +239,58 @@ bss_corr_kernel(const float* __restrict__ ref, const float* __restrict__ est, co
                     for (int r = 0; r < NB; ++r) acc[i][r] = fma(a[i], v[r], acc[i][r]);
             }
         }
+        if constexpr (kTrack) {                       // sample q of the tile: one per thread
+            if (k < n) {
+#pragma unroll
+                for (int e = 0; e < NE; ++e) {
+                    const double v = sm[(S + e) * W + k];
+                    ee[e] = fma(v, v, ee[e]);
+                }
+            }
+        }
     }
+    double* const pc = kTrack ? part + ((size_t)it * nc + chunk) * bss_partial_size(S, NE, F, true)
+                              : part + ((size_t)it * nc + chunk) * S * NB * F;
     if (k < F) {
-        double* pc = part + ((size_t)it * chunks + chunk) * S * NB * F;
 #pragma unroll
         for (int i = 0; i < S; ++i)
 #pragma unroll
             for (int r = 0; r < NB; ++r) pc[((size_t)i * NB + r) * F + k] = acc[i][r];
     }
+    if constexpr (kTrack) {                           // the energies, reduced in a fixed order
+        __shared__ double red[kBssCorrTile / 32][NE];
+        const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+#pragma unroll
+        for (int e = 0; e < NE; ++e) {
+            const double s = warp_sum_f64(ee[e]);
+            if (lane == 0) red[warp][e] = s;
+        }
+        __syncthreads();
+        if (threadIdx.x < NE) {
+            double s = 0.0;
+            for (int w = 0; w < kBssCorrTile / 32; ++w) s += red[w][threadIdx.x];
+            pc[(size_t)S * NB * F + threadIdx.x] = s;
+        }
+    }
+}
+
+// v4: adds a launch's chunk partials (n per recording, the chunks from c0 on) to each recording's running totals,
+// correlations tot [B][csize] and estimate energies etot [B][NE], in chunk order, starting from zero at c0 = 0.  Chunks past a recording's length are skipped, so
+// its totals are the same whatever the batch.  One thread per (recording, double of the partial).
+__global__ void __launch_bounds__(256)
+bss_fold_kernel(const double* __restrict__ part, double* __restrict__ tot, double* __restrict__ etot, BssItems items,
+                int B, long long csize, int NE, BssTrackChunks chunks) {
+    const long long size = csize + NE;
+    const long long idx = blockIdx.x * 256LL + threadIdx.x;
+    if (idx >= B * size) return;
+    const long long b = idx / size, i = idx - b * size;
+    long long rb, len;
+    items.span(b, rb, len);
+    double* dst = i < csize ? tot + b * csize + i : etot + b * NE + (i - csize);
+    double s = chunks.c0 == 0 ? 0.0 : *dst;
+    for (int c = 0; c < chunks.n; ++c)
+        if ((chunks.c0 + c) * kBssTrackChunk < len) s += part[((size_t)b * chunks.n + c) * size + i];
+    *dst = s;
 }
 
 // One item's lagged correlations X_ar[k], its chunk partials added in chunk order.
@@ -473,13 +570,17 @@ bss_solve_kernel(const double* __restrict__ part, int chunks, double* __restrict
 //     [0, S)  |pt_j|^2,   [S, 2S)  |e - pt_j|^2,   [2S, 3S)  |pa - pt_j|^2,   3S |pa|^2,   3S+1 |e - pa|^2,   3S+2 |e|^2
 // and for source images (IMG), with s_j the row of reference j in e's channel (e mod C):
 //     [3S+3, 4S+3)  |pt_j - s_j|^2,   [4S+3, 5S+3)  |e - s_j|^2
+// and for BSS-eval v4 (V4, with IMG), whose items are museval's windows (BssItems::window) filtered by their
+// recording's whole-track filters (cj, ct indexed by recording), the window's own reference energies
+//     [5S+3, 6S+3)  |s_j|^2
 // Chunked as bss_corr_kernel: the item's own bss_energy_chunks, zero partials past them.
-template <int S, int NE, int C = 1, bool IMG = false>
+template <int S, int NE, int C = 1, bool IMG = false, bool V4 = false>
 __global__ void __launch_bounds__(kBssEnergyTile)
 bss_energy_kernel(const float* __restrict__ ref, const float* __restrict__ est, const float* __restrict__ mix,
                   const double* __restrict__ cj, const double* __restrict__ ct, double* __restrict__ epart,
                   BssItems items, int F, int chunks) {
-    constexpr int R = S * C, NV = bss_energy_count(S, IMG);
+    constexpr int R = S * C, NV = bss_energy_count(S, IMG, V4);
+    static_assert(!V4 || IMG, "v4 scores source images");
     extern __shared__ double sm[];
     __shared__ double red[kBssEnergyTile / 32][NV];
     const int W = kBssEnergyTile + F - 1;
@@ -489,7 +590,8 @@ bss_energy_kernel(const float* __restrict__ ref, const float* __restrict__ est, 
     const long long it = blockIdx.x / chunks;
     const int chunk = (int)(blockIdx.x - it * chunks);
     long long b, T;
-    const long long off = items.span(it, b, T);
+    const long long off = V4 ? items.window(it, b, T) : items.span(it, b, T);
+    const long long fi = V4 ? b : it;                   // whose filters
     const int own = bss_energy_chunks(T, F);
     const long long L = T + F - 1;
     const long long per = (L + own - 1) / own;
@@ -500,8 +602,8 @@ bss_energy_kernel(const float* __restrict__ ref, const float* __restrict__ est, 
         const float* er = bss_row(ref, est, mix, R, b, R + e, items.T) + off;
         __syncthreads();
         for (int idx = threadIdx.x; idx < R * F; idx += kBssEnergyTile) {
-            sj[idx] = cj[((size_t)it * (R + 1) + e) * R * F + idx];
-            st[idx] = ct[((size_t)it * (R + 1) + e) * R * F + idx];
+            sj[idx] = cj[((size_t)fi * (R + 1) + e) * R * F + idx];
+            st[idx] = ct[((size_t)fi * (R + 1) + e) * R * F + idx];
         }
         double acc[NV];
 #pragma unroll
@@ -549,6 +651,7 @@ bss_energy_kernel(const float* __restrict__ ref, const float* __restrict__ est, 
                         const double sv = sref[(size_t)(j * C + c) * W + threadIdx.x + F - 1];   // s_jC+c[t]
                         acc[3 * S + 3 + j] = fma(pt[j] - sv, pt[j] - sv, acc[3 * S + 3 + j]);
                         acc[4 * S + 3 + j] = fma(ev - sv, ev - sv, acc[4 * S + 3 + j]);
+                        if constexpr (V4) acc[5 * S + 3 + j] = fma(sv, sv, acc[5 * S + 3 + j]);
                     }
                 }
             }
@@ -575,13 +678,16 @@ __device__ __forceinline__ double bss_db(double num, double den) {
 // one thread per item.  sdr/sir/sar/perm [B][S] for the estimates (perm[j]: the estimate given reference j); with the
 // mixture (NE == S + 1), msdr/msir/msar [B][S]: the mixture scored as the estimate of every reference.  Source images
 // (IMG) sum each estimate image's rows' energies over its C channels, in channel order, and also write isr [B][S].
-template <int S, int NE, int C = 1, bool IMG = false>
+// BSS-eval v4 (V4, with IMG; eref unused) takes |s_j|^2 from the window's own energies and tests no projection per
+// window, where whole-track filters give none: bss_track_check_kernel has tested the recording and set the filters of
+// a recording that failed, or held a silent or non-finite row, to NaN, which makes its windows' energies NaN.
+template <int S, int NE, int C = 1, bool IMG = false, bool V4 = false>
 __global__ void __launch_bounds__(256)
 bss_final_kernel(const double* __restrict__ epart, const double* __restrict__ eref, int chunks, double* __restrict__ sdr,
                  double* __restrict__ isr, double* __restrict__ sir, double* __restrict__ sar, int* __restrict__ perm,
                  double* __restrict__ msdr, double* __restrict__ msir, double* __restrict__ msar, int B,
                  int compute_permutation) {
-    constexpr int R = S * C, NV = bss_energy_count(S, IMG);
+    constexpr int R = S * C, NV = bss_energy_count(S, IMG, V4);
     constexpr int NI = IMG ? S : NE;                    // scored estimates: images, or rows (with the mixture's)
     for (long long b = blockIdx.x * 256LL + threadIdx.x; b < B; b += (long long)gridDim.x * 256) {
         double en[NE][NV];
@@ -596,19 +702,37 @@ bss_final_kernel(const double* __restrict__ epart, const double* __restrict__ er
 #pragma unroll
                 for (int i = 0; i < NV; ++i) en[e][i] += pc[e * NV + i];
         }
-        const double* er = eref + (size_t)b * R;
+        double wref[S];                                 // v4: the window's reference image energies
+        if constexpr (V4) {
+#pragma unroll
+            for (int j = 0; j < S; ++j) {
+                wref[j] = en[0][5 * S + 3 + j];
+#pragma unroll
+                for (int c = 1; c < C; ++c) wref[j] += en[c][5 * S + 3 + j];
+            }
+        }
+        const double* er = V4 ? nullptr : eref + (size_t)b * R;
         bool silent_ref = false;
 #pragma unroll
-        for (int i = 0; i < S; ++i) silent_ref = silent_ref || !bss_scorable(bss_image_energy<C>(er, i));
+        for (int i = 0; i < S; ++i)
+            silent_ref = silent_ref || !bss_scorable(V4 ? wref[i] : bss_image_energy<C>(er, i));
         bool silent = silent_ref;
 #pragma unroll
         for (int e = 0; e < S; ++e) {
             double e2 = en[e * C][3 * S + 2];
-            bool held = bss_projections_hold<S>(en[e * C]);
+            bool held = V4 || bss_projections_hold<S>(en[e * C]);
 #pragma unroll
             for (int c = 1; c < C; ++c) {
                 e2 += en[e * C + c][3 * S + 2];
-                held = held && bss_projections_hold<S>(en[e * C + c]);
+                held = held && (V4 || bss_projections_hold<S>(en[e * C + c]));
+            }
+            if constexpr (V4) {                         // NaN filters: a recording that cannot be scored
+#pragma unroll
+                for (int c = 0; c < C; ++c) {
+                    held = held && en[e * C + c][3 * S] < (double)INFINITY;
+#pragma unroll
+                    for (int j = 0; j < S; ++j) held = held && en[e * C + c][j] < (double)INFINITY;
+                }
             }
             silent = silent || !bss_scorable(e2) || !held;
         }
@@ -639,7 +763,7 @@ bss_final_kernel(const double* __restrict__ epart, const double* __restrict__ er
                         sp += v[3 * S + 3 + j];
                         dd += v[4 * S + 3 + j];
                     }
-                    const double sj = bss_image_energy<C>(er, j);
+                    const double sj = V4 ? wref[j] : bss_image_energy<C>(er, j);
                     d[e][j] = bss_db(sj, dd);
                     g[e][j] = bss_db(sj, sp);
                     i_[e][j] = bss_db(pj, in);
@@ -683,6 +807,76 @@ bss_final_kernel(const double* __restrict__ epart, const double* __restrict__ er
     }
 }
 
+// BSS-eval v4: tests each recording's whole-track filters.  grid = B (S + 1), the solve's systems; 256 threads; smem
+// [M][M][F] + [M][F] doubles for the system's M rows.  Estimate row e's filters c solve G c = D_e, so for a projection
+// c^T G c = c^T D_e = |P e|^2 over the whole track, and 2 |c^T G c - c^T D_e| is the defect |p|^2 + |e - p|^2 - |e|^2
+// that bss_final_kernel bounds per item for the other entries, here formed from the recording's correlations.  A
+// system that fails it for any estimate row, and every system of a recording with a silent or non-finite reference or
+// estimate image, has its filters set to NaN, which makes each of the recording's windows NaN.
+template <int S, int C>
+__global__ void __launch_bounds__(256)
+bss_track_check_kernel(const double* __restrict__ tot, const double* __restrict__ etot,
+                       const double* __restrict__ eref, double* __restrict__ cj, double* __restrict__ ct, int F) {
+    constexpr int R = S * C, NE = R, NB = R + NE;
+    extern __shared__ double smem[];
+    __shared__ double red[8][2];
+    __shared__ int held;
+    const long long b = blockIdx.x / (S + 1);
+    const int sys = (int)(blockIdx.x - b * (S + 1));
+    const int M = sys == 0 ? R : C, r0 = sys == 0 ? 0 : (sys - 1) * C;
+    const BssCorr<R, NB> cr{tot + (size_t)b * R * NB * F, 1, F};
+    const double* ee = etot + (size_t)b * NE;         // |e|^2 of each estimate row over the track
+    double* sg = smem;                                  // sg[(r M + q) F + k] = X_{r0+r, r0+q}[k]
+    double* sc = sg + (size_t)M * M * F;                // the filters of one estimate row
+    bool ok = true;
+#pragma unroll
+    for (int i = 0; i < S; ++i)
+        ok = ok && bss_scorable(bss_image_energy<C>(eref + (size_t)b * R, i)) && bss_scorable(bss_image_energy<C>(ee, i));
+    for (int idx = threadIdx.x; idx < M * M * F; idx += blockDim.x) {
+        const int r = idx / (M * F), q = (idx / F) % M, k = idx % F;
+        sg[idx] = cr(r0 + r, r0 + q, k);
+    }
+    double* fil = (sys == 0 ? cj : ct) + (size_t)b * (R + 1) * R * F;
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int e = 0; e < NE && ok; ++e) {                // ok is the same in every thread
+        __syncthreads();
+        for (int idx = threadIdx.x; idx < M * F; idx += blockDim.x)
+            sc[idx] = fil[((size_t)e * R + r0 + idx / F) * F + idx % F];
+        __syncthreads();
+        double cgc = 0.0, cd = 0.0;
+        for (int idx = threadIdx.x; idx < M * F; idx += blockDim.x) {
+            const int r = idx / F, l = idx % F;
+            double g = 0.0;                             // (G c)[(r, l)]
+            for (int q = 0; q < M; ++q) {
+                const double* xrq = sg + ((size_t)r * M + q) * F;
+                const double* xqr = sg + ((size_t)q * M + r) * F;
+                const double* cq = sc + (size_t)q * F;
+                for (int m = 0; m <= l; ++m) g = fma(xrq[l - m], cq[m], g);
+                for (int m = l + 1; m < F; ++m) g = fma(xqr[m - l], cq[m], g);
+            }
+            cgc = fma(sc[idx], g, cgc);
+            cd = fma(sc[idx], cr(r0 + r, R + e, l), cd);
+        }
+        cgc = warp_sum_f64(cgc);
+        cd = warp_sum_f64(cd);
+        if (lane == 0) { red[warp][0] = cgc; red[warp][1] = cd; }
+        __syncthreads();
+        if (threadIdx.x == 0) {
+            double a = 0.0, d = 0.0;
+            for (int w = 0; w < (int)(blockDim.x >> 5); ++w) { a += red[w][0]; d += red[w][1]; }
+            held = 2.0 * fabs(a - d) <= kBssProjectionDefect * ee[e];
+        }
+        __syncthreads();
+        ok = held != 0;
+    }
+    if (ok) return;
+    const double nan = __longlong_as_double(0x7ff8000000000000LL);
+    for (int idx = threadIdx.x; idx < NE * R * F; idx += blockDim.x) {
+        const int r = (idx / F) % R;
+        if (sys == 0 || r / C == sys - 1) fil[idx] = nan;
+    }
+}
+
 // Scores n items of the view in launches of at most cap items, all through one scratch sized for cap items of at most
 // L samples: the launches follow each other on the stream with no host synchronisation between them, so a call can
 // be captured in a CUDA graph.  Item i's outputs are [i][S].  Source images are <S, S C, C, true>.
@@ -704,7 +898,7 @@ static int bss_eval_launch(const float* ref, const float* est, const float* mix,
         const size_t o = (size_t)first * S;
         items.first = first;
         int e;
-        if ((e = launch(bss_corr_kernel<R, NE>, (unsigned)((long long)k * cc), kBssCorrTile, corr_smem, st, ref, est,
+        if ((e = launch(bss_corr_kernel<R, NE, int>, (unsigned)((long long)k * cc), kBssCorrTile, corr_smem, st, ref, est,
                         mix, s.part, items, F, cc)))
             return e;
         if ((e = launch(bss_solve_kernel<S, NE, C>, (unsigned)((long long)k * (S + 1)), 256, solve_smem, st, s.part,
@@ -744,14 +938,8 @@ static int bss_dispatch(const float* ref, const float* est, const float* mix, do
 
 // The source-image kernels are instantiated for S C <= 4: the joint system's shared memory, (2 R^2 + E R) F doubles
 // at R = E = S C, is 192 KiB at R = 4 and F = 512.
-static int bss_images_dispatch(const float* ref, const float* est, double* sdr, double* isr, double* sir, double* sar,
-                               int* perm, int S, int C, const BssItems& items, long long n, long long cap, long long L,
-                               int F, int compute_permutation, void* scratch, cudaStream_t st) {
-    auto run = [&](auto s, auto c) {
-        constexpr int S_ = decltype(s)::value, C_ = decltype(c)::value;
-        return bss_eval_launch<S_, S_ * C_, C_, true>(ref, est, nullptr, sdr, isr, sir, sar, perm, nullptr, nullptr,
-                                                      nullptr, items, n, cap, L, F, compute_permutation, scratch, st);
-    };
+// Calls run(std::integral_constant<int, S>(), std::integral_constant<int, C>()) for the instantiated (S, C).
+template <class Fn> static int with_images(int S, int C, const Fn& run) {
     using I1 = std::integral_constant<int, 1>;
     using I2 = std::integral_constant<int, 2>;
     if (C == 1) return with_sources(S, [&](auto s) { return run(s, I1()); });
@@ -760,6 +948,16 @@ static int bss_images_dispatch(const float* ref, const float* est, double* sdr, 
     if (S == 1 && C == 4) return run(I1(), std::integral_constant<int, 4>());
     if (S == 2 && C == 2) return run(I2(), I2());
     return SDR_ERR_UNSUPPORTED;
+}
+
+static int bss_images_dispatch(const float* ref, const float* est, double* sdr, double* isr, double* sir, double* sar,
+                               int* perm, int S, int C, const BssItems& items, long long n, long long cap, long long L,
+                               int F, int compute_permutation, void* scratch, cudaStream_t st) {
+    return with_images(S, C, [&](auto s, auto c) {
+        constexpr int S_ = decltype(s)::value, C_ = decltype(c)::value;
+        return bss_eval_launch<S_, S_ * C_, C_, true>(ref, est, nullptr, sdr, isr, sir, sar, perm, nullptr, nullptr,
+                                                      nullptr, items, n, cap, L, F, compute_permutation, scratch, st);
+    });
 }
 
 // sdr_bss_eval (mix null) and sdr_bss_eval_mixture: item b is the whole of recording b, all in one launch sequence
@@ -805,6 +1003,117 @@ static size_t bss_framewise_scratch_bytes(int B, int S, int C, long long T, long
     const long long n = (long long)B * nwin;
     return BssScratch(nullptr, (int)(n < kBssFramewiseItems ? n : kBssFramewiseItems), S, C,
                       bss_framewise_span(T, W, H), F, bss_energy_count(S, images)).bytes;
+}
+
+// BSS-eval v4's correlation launches take at most this many CTAs' chunks (kBssTrackChunk samples each) across the
+// batch, at least one chunk per recording: about four waves of the correlation kernel on an H100, so one recording
+// fills the GPU while the launch partials stay bounded (69 MB at R = 4, F = 512).
+constexpr long long kBssTrackBlocks = 512;
+
+static long long bss_track_chunks(long long T) { return (T + kBssTrackChunk - 1) / kBssTrackChunk; }
+
+// Chunks per recording in one v4 correlation launch
+static int bss_track_launch_chunks(int B, long long T) {
+    const long long g = kBssTrackBlocks / B < 1 ? 1 : kBssTrackBlocks / B, total = bss_track_chunks(T);
+    return (int)(g < total ? g : total);
+}
+
+// museval's window count: floor((T - W + H) / H) for T >= W
+static long long bss_v4_window_count(long long T, long long W, long long H) { return (T - W) / H + 1; }
+
+// BSS-eval v4's scratch for B recordings of R = S C rows and n windows.  Doubles:
+//   part  [B][G][R 2R F + R]   one correlation launch's chunk partials (G chunks per recording)
+//   tot   [B][R][2R][F]        each recording's correlations over its whole length
+//   etot  [B][R]               its estimate rows' energies
+//   rj, rt, eref, cj, ct       the solve's, per recording (as BssScratch with the mixture's row)
+//   epart [m][echunks][R+1][NV]  the energy partials of a launch of m <= kBssFramewiseItems windows of W samples
+struct BssV4Scratch {
+    double *part, *tot, *etot, *rj, *rt, *eref, *cj, *ct, *epart;
+    int G;
+    size_t bytes;
+    BssV4Scratch(void* base, int B, int S, int C, long long T, long long W, long long n, int F) {
+        const size_t b = (size_t)B, s = (size_t)S, c = (size_t)C, r = s * c, f = (size_t)F, ne = r + 1;
+        const size_t m = (size_t)(n < kBssFramewiseItems ? n : kBssFramewiseItems);
+        G = bss_track_launch_chunks(B, T);
+        size_t off = 0;
+        double* p = static_cast<double*>(base);
+        auto take = [&](size_t k) { double* q = p ? p + off : nullptr; off += k; return q; };
+        part = take(b * G * bss_partial_size((int)r, (int)r, F, true));
+        tot = take(b * r * 2 * r * f);
+        etot = take(b * r);
+        rj = take(b * f * r * r);
+        rt = take(b * s * f * c * c);
+        eref = take(b * r);
+        cj = take(b * ne * r * f);
+        ct = take(b * ne * r * f);
+        epart = take(m * bss_energy_chunks(W, F) * ne * (size_t)bss_energy_count(S, true, true));
+        bytes = off * sizeof(double);
+    }
+};
+
+static size_t bss_v4_scratch_bytes(int B, int S, int C, long long T, long long W, long long H, int F) {
+    if (B <= 0 || S < 1 || S > 4 || C < 1 || S * C > 4 || T <= 0 || W <= 0 || H <= 0 || F < 1 || F > kBssMaxF)
+        return 0;
+    if (T < W || (long long)S * C * F > T + F - 1) return 0;     // no window, or no recording that can be solved
+    const long long nwin = bss_v4_window_count(T, W, H);
+    if (nwin > INT64_MAX / S / B) return 0;
+    return BssV4Scratch(nullptr, B, S, C, T, W, (long long)B * nwin, F).bytes;
+}
+
+// Correlations over each whole recording in launches of G chunks per recording, each folded into the running totals;
+// one solve and one filter check per recording; then the windows, in launches of at most kBssFramewiseItems through
+// one scratch.  Nothing synchronises with the host.
+template <int S, int C>
+static int bss_v4_launch(const float* ref, const float* est, const long long* lengths, double* sdr, double* isr,
+                         double* sir, double* sar, int* perm, int B, long long T, long long W, long long H, int F,
+                         int compute_permutation, void* scratch, cudaStream_t st) {
+    constexpr int R = S * C, NE = R;
+    const long long nwin = bss_v4_window_count(T, W, H), n = (long long)B * nwin;
+    const BssV4Scratch s(scratch, B, S, C, T, W, n, F);
+    const long long min_len = (long long)(R - 1) * F + 1;
+    const size_t psize = bss_partial_size(R, NE, F, true);
+    const long long fold_blocks = ((long long)B * psize + 255) / 256;
+    const int ec = bss_energy_chunks(W, F);
+    const int m = (int)(n < kBssFramewiseItems ? n : kBssFramewiseItems);
+    if ((long long)B * s.G > 0x7fffffffLL || (long long)B * (S + 1) > 0x7fffffffLL || fold_blocks > 0x7fffffffLL ||
+        (long long)m * ec > 0x7fffffffLL)
+        return SDR_ERR_UNSUPPORTED;
+    const size_t corr_smem = sizeof(double) * (R + NE) * (kBssCorrTile + F - 1);
+    const size_t solve_smem = sizeof(double) * (size_t)F * (2 * R * R + NE * R);
+    const size_t check_smem = sizeof(double) * (size_t)F * (R * R + R);
+    const size_t energy_smem = sizeof(double) * (size_t)R * (kBssEnergyTile + F - 1 + 2 * F);
+    const BssItems whole{T, T, T, 1, 0, min_len, lengths};
+    const long long total = bss_track_chunks(T);
+    int e;
+    for (long long c0 = 0; c0 < total; c0 += s.G) {
+        const BssTrackChunks ch{(int)(total - c0 < s.G ? total - c0 : s.G), c0};
+        if ((e = launch(bss_corr_kernel<R, NE, BssTrackChunks>, (unsigned)((long long)B * ch.n), kBssCorrTile,
+                        corr_smem, st, ref, est, nullptr, s.part, whole, F, ch)))
+            return e;
+        if ((e = launch(bss_fold_kernel, (unsigned)fold_blocks, 256, 0, st, s.part, s.tot, s.etot, whole, B,
+                        (long long)R * 2 * R * F, NE, ch)))
+            return e;
+    }
+    if ((e = launch(bss_solve_kernel<S, NE, C>, (unsigned)(B * (S + 1)), 256, solve_smem, st, s.tot, 1, s.rj, s.rt,
+                    s.eref, s.cj, s.ct, F)))
+        return e;
+    if ((e = launch(bss_track_check_kernel<S, C>, (unsigned)(B * (S + 1)), 256, check_smem, st, s.tot, s.etot,
+                    s.eref, s.cj, s.ct, F)))
+        return e;
+    BssItems win{T, W, H, nwin, 0, min_len, lengths};
+    for (long long first = 0; first < n; first += m) {
+        const int k = (int)(n - first < m ? n - first : m);
+        const size_t o = (size_t)first * S;
+        win.first = first;
+        if ((e = launch(bss_energy_kernel<S, NE, C, true, true>, (unsigned)((long long)k * ec), kBssEnergyTile,
+                        energy_smem, st, ref, est, nullptr, s.cj, s.ct, s.epart, win, F, ec)))
+            return e;
+        if ((e = launch(bss_final_kernel<S, NE, C, true, true>, item_blocks(k), 256, 0, st, s.epart, nullptr, ec,
+                        sdr + o, isr + o, sir + o, sar + o, perm ? perm + o : nullptr, nullptr, nullptr, nullptr, k,
+                        compute_permutation)))
+            return e;
+    }
+    return SDR_OK;
 }
 
 }  // namespace sdr
@@ -891,6 +1200,25 @@ int sdr_bss_eval_images_framewise(const float* reference, const float* estimate,
     return bss_images_dispatch(reference, estimate, sdr, isr, sir, sar, perm_or_null, S, C, items,
                                (long long)B * nwin, kBssFramewiseItems, bss_framewise_span(T, W, H), F,
                                compute_permutation, scratch, static_cast<cudaStream_t>(stream));
+}
+
+size_t sdr_bss_eval_v4_scratch_bytes(int B, int S, int C, int64_t T, int64_t W, int64_t H, int F) {
+    return bss_v4_scratch_bytes(B, S, C, T, W, H, F);
+}
+
+int sdr_bss_eval_v4(const float* reference, const float* estimate, const int64_t* lengths_or_null, double* sdr,
+                    double* isr, double* sir, double* sar, int32_t* perm_or_null, int B, int S, int C, int64_t T,
+                    int64_t W, int64_t H, int F, int compute_permutation, void* scratch, sdr_stream stream) {
+    if (!isr || !bss_buffers_ok(reference, estimate, nullptr, sdr, sir, sar, nullptr, nullptr, nullptr, scratch) ||
+        reinterpret_cast<uintptr_t>(lengths_or_null) % 8)
+        return SDR_ERR_BAD_ARGUMENT;
+    if (!sdr_bss_eval_v4_scratch_bytes(B, S, C, T, W, H, F))
+        return B <= 0 || T <= 0 || W <= 0 || H <= 0 ? SDR_ERR_BAD_ARGUMENT : SDR_ERR_UNSUPPORTED;
+    return with_images(S, C, [&](auto s, auto c) {
+        return bss_v4_launch<decltype(s)::value, decltype(c)::value>(
+            reference, estimate, reinterpret_cast<const long long*>(lengths_or_null), sdr, isr, sir, sar,
+            perm_or_null, B, T, W, H, F, compute_permutation, scratch, static_cast<cudaStream_t>(stream));
+    });
 }
 
 }  // extern "C"
